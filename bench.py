@@ -8,7 +8,8 @@ scaling (8 ranks = config 4's 8192 chunks).  MB = 10^6 uncompressed bytes (pco_c
   value     resident: inputs already in HBM, device buffers in and out, through the C-ABI (*_ex, flags DEVICE).
   e2e       same calls with pinned HOST buffers (H2D of the inputs and D2H of the results inside the timed region), streamed in chunk groups by
             2 + 2 host threads; e2e.single_call = one call pair over the whole array; e2e.reference_abi = the reference's 3-function ABI as is.
-  roofline  fused_narrow_kernel (the decompress kernel on this data): (U + C) bytes / its CUDA-event duration vs MEASURED_PEAKS.json hbm_gbs;
+  roofline  fused_narrow_kernel (the decompress kernel on this data): (U + C) bytes / its CUDA-event duration vs MEASURED_PEAKS.json hbm_gbs
+            (when present) or the H100 SXM data sheet's 3.35 TB/s;
             roofline.call / roofline.compress = the same bytes over the whole decompress / compress call.
   cpu_baseline / --impl reference: oracle/ (C++ restatement of pco 1.0.3; the Rust reference cannot be built here)
             on the host cores - one worker process per host thread - on a bounded sample of the same chunks.
@@ -48,7 +49,10 @@ def parse_args():
     ap.add_argument("--no-index-free", action="store_true", help="skip the pco_b200_decompress_chunks timing (not part of `value`)")
     ap.add_argument("--results-csv", default=None, help="also merge this run into a CSV with the reference bench tool's schema and codec naming (pcodec_b200/benchfmt.py)")
     ap.add_argument("--no-gather-pages", action="store_true", help="N > 1: exchange only the per-chunk sizes; the default also gathers the compressed pages on the device (every rank ends up with the whole file)")
-    ap.add_argument("--gather-ctas", type=int, default=0, help="CTAs of the page-gather copy kernel (it runs beside the next step's kernels on a high-priority stream); 0 = 16 per rank of the job, at most 64 (profiles/r02_zz3_gather_sweep.txt)")
+    ap.add_argument("--gather-ctas", type=int, default=0, help="CTAs of the page-gather copy kernel (it runs beside the next step's kernels on a high-priority stream); 0 = 16 per rank of the job, at most 64")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step returned (rank 0) as DIR/<name>.npy: fixed, seeded samples of the "
+                         "decompressed numbers (float64) and of the compressed file and side index bytes (float32), and their sizes; 48 MB in all")
     return ap.parse_args()
 
 
@@ -244,6 +248,35 @@ def parse_profile(L):
             k, v = item.split("=")
             out[k] = out.get(k, 0.0) + float(v)
     return out
+
+
+DUMP_SAMPLE_NUMS = 1 << 21   # 16 MB of float64
+DUMP_SAMPLE_BYTES = 1 << 22  # 16 MB of float32 for each byte array
+
+
+def _seeded_sample(t, k, seed):
+    """Elements of 1-d tensor t at k positions drawn with a fixed seed (all of t when it is no longer), read back to the host."""
+    import torch
+
+    if t.numel() <= k:
+        return t.cpu().numpy()
+    pos = np.sort(np.random.default_rng(seed).choice(t.numel(), size=k, replace=False))
+    return t[torch.from_numpy(pos).to(t.device)].cpu().numpy()
+
+
+def dump_outputs(out_dir, d_out, d_file, d_index):
+    """What the caller of the timed path received in its last step: the decompressed numbers, the compressed file and the side
+    index, each as a seeded sample whose positions depend only on the array's length (stored in sizes.npy).  The values are exact
+    in the float types: the numbers of this workload stay below 2^53, bytes below 256."""
+    os.makedirs(out_dir, exist_ok=True)
+    nums = _seeded_sample(d_out.view(-1), DUMP_SAMPLE_NUMS, seed=1)
+    assert int(nums.max(initial=0)) < (1 << 53), "decompressed numbers are not exact in float64"
+    arrays = {"decompressed_sample": nums.astype(np.float64),
+              "compressed_sample": _seeded_sample(d_file, DUMP_SAMPLE_BYTES, seed=2).astype(np.float32),
+              "index_sample": _seeded_sample(d_index, DUMP_SAMPLE_BYTES, seed=3).astype(np.float32),
+              "sizes": np.array([d_out.numel(), d_file.numel(), d_index.numel()], dtype=np.float64)}  # numbers, file bytes, index bytes
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 def run_gpu_arm(args, rank, world):
@@ -473,6 +506,8 @@ def run_gpu_arm(args, rank, world):
         gather_info["ctas"] = gather_ctas
         gather_info["what"] = "sizes all-gather + scan + copy kernel on a high-priority side stream (overlaps decompress of the same step and compress of the next)"
     value = world * U / 1e6 / (ms_per_step / 1e3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, d_out, d_comp[:n_written.value], d_index[:ilen.value])
 
     # ---- the index-free path (not part of `value`): the same chunks decoded from their byte offsets alone
     # (pco_b200_decompress_chunks: one tANS walk per chunk builds the per-batch index on the device, all chunks in parallel)
@@ -719,7 +754,7 @@ def run_gpu_arm(args, rank, world):
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (measured copy bandwidth)"
     else:
-        peak, peak_src = 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "H100 SXM data sheet HBM3 bandwidth, 3.35 TB/s (not measured)"
     # the decompress path is two kernels: symwalk_kernel (tANS symbol walk) + decode_kernel (offsets, un-delta, join)
     dk_ms = float(np.mean([p.get("fused_narrow_kernel", 0.0) + p.get("decode_kernel", 0.0) + p.get("symwalk_kernel", 0.0) for p in prof_d]))
     dec_spans = {}
@@ -731,13 +766,6 @@ def run_gpu_arm(args, rank, world):
     achieved = alg_bytes / 1e9 / (dk_ms / 1e3) if dk_ms > 0 else None
     call_ms = float(np.mean(t_d))
     achieved_call = alg_bytes / 1e9 / (call_ms / 1e3)
-    # DRAM traffic of the same two kernels from the committed `ncu --set full` capture (dram__bytes_read.sum +
-    # dram__bytes_write.sum per launch, same workload); never measured under this run
-    traffic, traffic_src = None, None
-    tpath = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-    if os.path.exists(tpath) and n_chunks == N_CHUNKS:
-        tj = json.load(open(tpath))
-        traffic, traffic_src = int(sum(tj["dram_bytes_per_launch"].values())), tj["source"]
     comp_spans = {}
     for p in prof_c:
         for k, v in p.items():
@@ -762,7 +790,7 @@ def run_gpu_arm(args, rank, world):
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u64", "data": "synthetic",
         "config": {"workload": f"C2: {n_chunks} chunks x 2^18 u64 per GPU, classic mode, consecutive delta order 1, level 8 (cumsum of geometric(0.001)); "
                                "step = compress + decompress of every chunk, buffers resident in HBM",
-                   "chunks_per_gpu": n_chunks, "chunk_n": CHUNK_N, "l2": "inputs (2 GiB per GPU) exceed the 126 MB L2",
+                   "chunks_per_gpu": n_chunks, "chunk_n": CHUNK_N, "l2": "inputs (2 GiB per GPU) exceed the 50 MB L2",
                    "multi_gpu": (("independent chunk shards per rank (chunk c on rank c mod N); every step the compressed PAGES ARE GATHERED on the device: NCCL all-gather of the per-chunk "
                                   "sizes (device tensor), scan kernel, then each rank stores its chunks into every rank's file buffer over NVLink (P2P stores into cudaIpc-mapped peer memory) - "
                                   "all ranks end up with the whole standalone file; the gather of step k overlaps decompress(k) and compress(k+1)") if gather_on else
@@ -772,7 +800,7 @@ def run_gpu_arm(args, rank, world):
         "gather_ms": float(np.mean(t_g)), "gather": gather_info, "compressed_bytes_per_gpu": Cbytes, "index_bytes_per_gpu": Ibytes, "ratio": U / Cbytes,
         "kernel_ms": {**dec_spans, **comp_spans},
         "roofline": {"bound": "hbm", "kernel": "fused_narrow_kernel (tANS walk + offsets + un-delta + join of every chunk in one launch)", "achieved": achieved, "peak": peak,
-                     "unit": "GB/s", "frac": (achieved / peak) if achieved else None, "traffic": traffic, "traffic_source": traffic_src, "algorithmic_bytes": alg_bytes,
+                     "unit": "GB/s", "frac": (achieved / peak) if achieved else None, "algorithmic_bytes": alg_bytes,
                      "kernel_ms": dk_ms, "peak_source": peak_src,
                      "call": {"ms": call_ms, "achieved": achieved_call, "frac": achieved_call / peak, "what": "the whole pco_b200_decompress_ex call (device buffers), same bytes"},
                      "compress": {"ms": float(np.mean(t_c)), "achieved": alg_bytes / 1e9 / (float(np.mean(t_c)) / 1e3), "frac": alg_bytes / 1e9 / (float(np.mean(t_c)) / 1e3) / peak,
@@ -780,7 +808,7 @@ def run_gpu_arm(args, rank, world):
         "parity": parity,
         "index_free_decompress": ({**chunks_free, "roofline": {**chunks_free["roofline"], "peak": peak, "frac": chunks_free["roofline"]["achieved"] / peak}} if chunks_free else None),
         "cpu_baseline": cpu, "e2e": ({**e2e, "reference_abi": abi3} if e2e else e2e), "clocks": sampler.summary(),
-        # per step (profiles/r02_zz_launches.csv): compress = init_chunks, split_count, publish (flags readback), plan_solve, fallback, bin_lut,
+        # per step: compress = init_chunks, split_count, publish (flags readback), plan_solve, fallback, bin_lut,
         # ans_encode, layout, chunk_offsets, pack, header_footer, emit_index; decompress = fused_narrow_kernel + publish (statuses readback)
         "gpu_launches": 14 + (3 if gather_on else 0),  # + chunk_sizes_kernel, gather_offsets_kernel, push_pages_kernel of the page gather
     }

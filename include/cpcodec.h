@@ -4,7 +4,7 @@
  * (implemented in the reference by pco_c/src/lib.rs:127-195 on top of
  * pco::standalone::simple_compress_into / simple_decompress).  Same names, same
  * argument meaning, same error enum, same "caller allocates everything" contract;
- * the work is done by sm_100a CUDA kernels instead of the Rust CPU path.
+ * the work is done by sm_90a CUDA kernels instead of the Rust CPU path.
  *
  * Library name: libcpcodec.so (pco_c/Cargo.toml:6-8 names the reference's `cpcodec`).
  */

@@ -73,7 +73,7 @@ enum { PCO_B200_SRC_ON_DEVICE = 1u, PCO_B200_DST_ON_DEVICE = 2u, PCO_B200_INDEX_
 
 /* Message of the last error raised on the calling thread (pco::errors::PcoError::message). */
 const char *pco_b200_last_error_message(void);
-/* 1 if a usable sm_100 device is present. */
+/* 1 if a usable sm_90 (H100) device is present. */
 int pco_b200_device_available(void);
 
 /* pco::standalone::simple_decompress_into (pco/src/standalone/simple.rs:100-143): never errors on a

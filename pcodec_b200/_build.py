@@ -1,4 +1,4 @@
-"""Builds pcodec_b200/libcpcodec.so (CUDA kernels + C-ABI) in-tree with nvcc for sm_100a."""
+"""Builds pcodec_b200/libcpcodec.so (CUDA kernels + C-ABI) in-tree with nvcc for sm_90a (H100)."""
 import os
 import shutil
 import subprocess
@@ -9,7 +9,7 @@ INCLUDE = os.path.join(HERE, "..", "include")
 LIB = os.path.join(HERE, "libcpcodec.so")
 SOURCES = ["host_api.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared", "--fmad=false", "-cudart", "static",
 ]
 

@@ -1,4 +1,4 @@
-// Shared device-side definitions for the pco hot-path kernels (sm_100a).
+// Shared device-side definitions for the pco hot-path kernels (sm_90a).
 //
 // Format facts cited here are from the reference: docs/format.md and
 // pco/src/metadata/*.rs (paths relative to /root/reference).  Nothing in this

@@ -27,10 +27,8 @@ namespace pcob200 {
 #ifndef PCOB_FZ_WALKERS
 #define PCOB_FZ_WALKERS 2
 #endif
-// measured on C2 (1024 chunks x 2^18 u64, profiles/r02_c_fused_variants.txt), kernel / decompress call in ms:
-//   1 walker, 2 buffers, rows of 64: 1.010 / 1.068    2 walkers, 3 buffers, rows of 64: 0.676 / 0.753    rows of 128: 0.658 / 0.727
-//   3 walkers (5 decoders): 0.706 / 0.823             2 walkers, 2 buffers: 0.734 / 0.812              rows of 256 (3 CTAs/SM): 0.708 / 0.786
-//   round-1 pair symwalk_kernel + decode_narrow_kernel: 0.751 / 0.823
+// walkers, ring buffers and staged symbols per row are build-time knobs (-D); the defaults were chosen by timing C2 (1024 chunks x 2^18
+// u64) over 1..3 walkers, 2..3 buffers and rows of 64..256 symbols.
 #ifndef PCOB_FZ_ROW_SYMS
 #define PCOB_FZ_ROW_SYMS 128
 #endif

@@ -1,4 +1,4 @@
-// Decode-side kernels for the pco hot path on sm_100a:
+// Decode-side kernels for the pco hot path on sm_90a:
 //   walk_kernel    — K6: serial tANS walk that produces the per-batch side index (cold path)
 //   decode_kernel  — K7+K8+K9 fused: tANS symbols -> offsets unpack -> un-delta -> join -> store
 //
@@ -425,8 +425,7 @@ __device__ inline uint32_t walk_chunk_serial(const BitSrc& src, const ChunkHdr& 
   return ST_OK;
 }
 
-// One warp builds the tables, its first lane walks.  Measured for 1024 chunks (profiles/r02_k_walk_variants.txt): 128 threads x 8 CTAs/SM
-// (64 registers) 10.6 ms, 64 x 8 (128 registers) 13.6 ms, 64 x 16 15.3 ms, 32 x 8 8.5 ms
+// One warp builds the tables, its first lane walks.  A 32-thread CTA walked 1024 chunks faster than 64- or 128-thread ones.
 #ifndef PCOB_WALK_THREADS
 #define PCOB_WALK_THREADS 32
 #endif
@@ -780,32 +779,19 @@ __device__ __forceinline__ void undelta_chain_cold(L (&x)[8], DecodeSmem& sm, ui
   for (int e = 0; e < 8; e++) x[e] = tmp[e];
 }
 
-// 8 consecutive numbers of a lane -> global memory.  32-byte stores (STG.E.ENL2.256, sm_100) when the destination allows:
-// with 16-byte stores every instruction of the warp fills half of 32 sectors, and the L1 was the busiest unit of the decode
-// kernels (81 % of peak in decode_narrow_kernel; 0.78 -> 0.58 ms with whole-sector stores).
+// 8 consecutive numbers of a lane -> global memory.  16 bytes is the widest store sm_90 has (32-byte stores arrived with
+// sm_100), so 4- and 8-byte types take two or four of them; callers pass a 16-byte-aligned dst for those types.
 template <typename L>
 __device__ __forceinline__ void store8(L* __restrict__ dst, const L (&r)[8]) {
   if (sizeof(L) == 8) {
-    if ((reinterpret_cast<uintptr_t>(dst) & 31) == 0) {
 #pragma unroll
-      for (int q = 0; q < 2; q++)
-        asm volatile("st.global.v4.u64 [%0], {%1, %2, %3, %4};" ::"l"(dst + 4 * q), "l"(uint64_t(r[4 * q])), "l"(uint64_t(r[4 * q + 1])),
-                     "l"(uint64_t(r[4 * q + 2])), "l"(uint64_t(r[4 * q + 3])) : "memory");
-    } else {
-#pragma unroll
-      for (int q = 0; q < 4; q++)
-        asm volatile("st.global.v2.u64 [%0], {%1, %2};" ::"l"(dst + 2 * q), "l"(uint64_t(r[2 * q])), "l"(uint64_t(r[2 * q + 1])) : "memory");
-    }
+    for (int q = 0; q < 4; q++)
+      asm volatile("st.global.v2.u64 [%0], {%1, %2};" ::"l"(dst + 2 * q), "l"(uint64_t(r[2 * q])), "l"(uint64_t(r[2 * q + 1])) : "memory");
   } else if (sizeof(L) == 4) {
-    if ((reinterpret_cast<uintptr_t>(dst) & 31) == 0) {
-      asm volatile("st.global.v8.u32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(dst), "r"(uint32_t(r[0])), "r"(uint32_t(r[1])), "r"(uint32_t(r[2])),
-                   "r"(uint32_t(r[3])), "r"(uint32_t(r[4])), "r"(uint32_t(r[5])), "r"(uint32_t(r[6])), "r"(uint32_t(r[7])) : "memory");
-    } else {
 #pragma unroll
-      for (int q = 0; q < 2; q++)
-        asm volatile("st.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(dst + 4 * q), "r"(uint32_t(r[4 * q])), "r"(uint32_t(r[4 * q + 1])),
-                     "r"(uint32_t(r[4 * q + 2])), "r"(uint32_t(r[4 * q + 3])) : "memory");
-    }
+    for (int q = 0; q < 2; q++)
+      asm volatile("st.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(dst + 4 * q), "r"(uint32_t(r[4 * q])), "r"(uint32_t(r[4 * q + 1])),
+                   "r"(uint32_t(r[4 * q + 2])), "r"(uint32_t(r[4 * q + 3])) : "memory");
   } else if (sizeof(L) == 2) {  // 8 numbers = 16 bytes: one store when aligned
     if ((reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
       asm volatile("st.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "r"(uint32_t(r[0]) | (uint32_t(r[1]) << 16)), "r"(uint32_t(r[2]) | (uint32_t(r[3]) << 16)),
@@ -868,9 +854,8 @@ constexpr int SW_WARPS = SW_THREADS / 32;
 // Row staging: every lane keeps a private row with the bytes its next SW_ROW_SYMS symbols can read (<= 10 bits each,
 // + 16 bytes of start alignment + the window's over-read), refilled with 16-byte cp.async from its exact position.
 // Only tANS bits are staged (the offsets sections between them are not), so a CTA needs 32 KB and 7 fit on an SM.
-// Measured on C2 (1024 chunks): one 13 KiB stage per warp holding the whole span of its 32 batches, 3 CTAs per SM:
-// 0.305 ms; rows of 128 symbols, 5 CTAs: 0.305 ms; rows of 64 symbols, 7 CTAs: 0.266 ms.  More node replicas at the
-// price of CTAs per SM (16 / 32 copies, 5 / 4 CTAs) were slower: 0.300 / 0.312 ms.
+// On C2 (1024 chunks), rows of 64 symbols (7 CTAs per SM) were faster than rows of 128 or one stage per warp holding the span of
+// its 32 batches (5 / 3 CTAs per SM), and more node replicas at the price of CTAs per SM were slower.
 constexpr int SW_ROW_SYMS = PCOB_SW_ROWS;
 constexpr int SW_ROW_BLOCKS = ((SW_ROW_SYMS * SMALL_MAX_SIZE_LOG / 8 + 15) / 16 + 2) | 1;  // odd: rows start in different banks
 constexpr int SW_STAGE_BYTES = 32 * SW_ROW_BLOCKS * 16;

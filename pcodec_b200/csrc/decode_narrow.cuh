@@ -22,8 +22,8 @@ namespace pcob200 {
 #ifndef PCOB_NW_THREADS
 #define PCOB_NW_THREADS 256
 #endif
-// warps of a chunk's CTA.  More warps per chunk would mean shorter CTAs and a smaller tail wave (1024 chunks on 592 slots = 1.73
-// waves), but the carry chain hands over once per batch (~290 cycles per link): 16 warps: 0.60 ms, 32 warps: 1.04 ms, 8 warps: 0.48 ms.
+// warps of a chunk's CTA.  More warps per chunk would mean shorter CTAs and a smaller tail wave (1024 chunks on 132 SMs x 4 = 528 slots = 1.94
+// waves), but the carry chain hands over once per batch (~290 cycles per link), and 8 warps were faster than 16 or 32.
 constexpr int NW_THREADS = PCOB_NW_THREADS;
 constexpr int NW_WARPS = NW_THREADS / 32;
 constexpr int NW_RING = 2 * NW_WARPS < 32 ? 32 : 2 * NW_WARPS;  // carry-chain slots: more than the batches in flight
@@ -107,10 +107,10 @@ __device__ __forceinline__ void narrow_chunk(NarrowSmem& sm, const FileParams& f
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(win_sa + bufi * uint32_t(NW_WIN_WORDS * 4) + uint32_t(lane) * 16u), "l"(gp));
     asm volatile("cp.async.commit_group;");
   };
-  // (one cp.async.bulk of the 512 bytes per batch, signalled on an mbarrier, instead of 32 LDGSTS: correct, but 0.500 ms against 0.487 ms)
+  // (one cp.async.bulk of the 512 bytes per batch, signalled on an mbarrier, instead of 32 LDGSTS: correct, but slightly slower)
 
-  // a batch's section start is requested two batches ahead, its symbols and its window one batch ahead (symbols two ahead:
-  // 0.484 -> 0.490 ms; a __nanosleep back-off in the chain poll: no change once the hand-over was one record)
+  // a batch's section start is requested two batches ahead, its symbols and its window one batch ahead (symbols two ahead were
+  // slower; a __nanosleep back-off in the chain poll changed nothing once the hand-over was one record)
   constexpr int SY_STEP = NW_WARPS * (BATCH_N / 8);  // uint2 per round of NW_WARPS batches
   uint32_t off_cur = 0, off_nxt = 0;
   uint2 sy_nxt = make_uint2(0u, 0u);
@@ -226,10 +226,7 @@ __device__ __forceinline__ void narrow_chunk(NarrowSmem& sm, const FileParams& f
     }
     const uint32_t out_cnt = min(uint32_t(BATCH_N), n_out - b * BATCH_N);  // numbers this batch emits
     if (out_cnt == uint32_t(BATCH_N) && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
-      // 32-byte stores when aligned: a lane's 16-byte stores would each fill half a sector, and the L1 was the busiest
-      // unit with them (81 % of peak; 0.78 ms -> 0.58 ms).  Staging the batch in shared memory for 512-byte-contiguous
-      // stores instead: 0.61 ms.
-      store8<L>(dst, res);
+      store8<L>(dst, res);  // 16-byte vector stores when aligned
     } else {
 #pragma unroll
       for (int e = 0; e < 8; e++)

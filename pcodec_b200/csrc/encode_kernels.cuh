@@ -1,4 +1,4 @@
-// Encode-side kernels for the pco hot path on sm_100a (one launch handles many independent chunks):
+// Encode-side kernels for the pco hot path on sm_90a (one launch handles many independent chunks):
 //   split_delta_kernel  — K1+K2: mode split and consecutive delta encode, page moments, per-chunk min/max
 //   sort_keys_kernel    — range-reduced copy of the stored latents (input of the planner's segmented sort)
 //   plan_kernel         — bin training: equal-count histogram, bin-merge DP, tANS weight quantisation, tables
@@ -495,7 +495,7 @@ __global__ void __launch_bounds__(RS_THREADS, 1) radix_sort_segments_kernel(L* _
 //                       quantisation, tANS tables.  All chunks are resident at once, so the serial parts overlap.
 // ---------------------------------------------------------------------------
 constexpr int PLAN_THREADS = 512;
-constexpr int SOLVE_THREADS = 32;   // 128 (a barrier per DP step) measured slower with every chunk resident: 0.26 ms against 0.225 on C2
+constexpr int SOLVE_THREADS = 32;   // 128 (a barrier per DP step) measured slower with every chunk resident on C2
 constexpr uint32_t PLAN_MAX_COUNT_BITS = 15;  // counting histogram (no sort) when the key range fits 2^15 shared-memory counters
 
 // Order statistics handed from the probe kernel to the solver (per chunk and var, in HBM scratch)
@@ -1408,7 +1408,7 @@ constexpr int BINL_THREADS = 256;
 #ifndef PCOB_BINL_BATCHES
 #define PCOB_BINL_BATCHES 512
 #endif
-constexpr int BINL_BATCHES = PCOB_BINL_BATCHES;  // batches per CTA: every CTA rebuilds the chunk's lookup table first (128: 0.34 ms, 256: 0.28, 512: 0.26, 1024: 0.29)
+constexpr int BINL_BATCHES = PCOB_BINL_BATCHES;  // batches per CTA: every CTA rebuilds the chunk's lookup table first (512 beat 128, 256 and 1024 on C2)
 
 template <typename L>
 __global__ void __launch_bounds__(BINL_THREADS) bin_lut_kernel(EncParams ep, uint32_t batches_per_chunk, uint32_t parts_per_chunk,
@@ -1540,7 +1540,7 @@ struct AnsSmem {
 // The descriptor holds the step as two additions (the FSE formulation of the same arithmetic) in one 32-bit word:
 //   bits 0-19  A = (min_renorm_bits + 1) << 16 - cutoff :  bits = (state + A) >> 16       (= min_renorm_bits + (state >= cutoff))
 //   bits 20-31 B = cum - weight + 1024                   :  next  = next_states[B - 1024 + (state >> bits)]
-// (an 8-byte descriptor saves one more instruction per step but doubles the wavefronts of the lookups: 0.435 -> 0.467 ms)
+// (an 8-byte descriptor saves one more instruction per step but doubles the wavefronts of the lookups, and was slower)
 __device__ __forceinline__ uint32_t ans_step(uint32_t d, uint32_t& state, uint32_t& o, const uint16_t* next_states) {
   const uint32_t bits = ((state + d) >> 16) & 0xfu;  // state < 2^11 and B sits above bit 19: no carry into B
   o = (state & ~(0xffffffffu << bits)) | (bits << 12);  // bits <= ENC_MAX_SIZE_LOG = 10: value in bits 0-9, width in bits 12-15
@@ -1756,10 +1756,10 @@ __global__ void __launch_bounds__(ANS_THREADS, 4) ans_encode_kernel(EncParams ep
     uint32_t my_out = state;
     __syncthreads();
     // The speculation rests on tANS trajectories merging (a symbol of weight w maps all states onto w values).  Tables that merge slowly
-    // need other means, chosen by what they cost (times for 128 chunks per launch, r02_t / r02_u):
+    // need other means, chosen by what they cost:
     //   fix-up        a wrong segment re-runs from its true input next to the old trajectory until the two meet.  Cheap when they meet
-    //                 soon (C5 float64 order 0: a third of the guesses wrong, ~10 iterations, 1 ms in all); a correction that runs off its
-    //                 segment moves the problem one segment on per iteration (~0.13 ms each, 8.5 ms for a whole page).
+    //                 soon (C5 float64 order 0: a third of the guesses wrong, ~10 iterations); a correction that runs off its
+    //                 segment moves the problem one segment on per iteration (as slow as a whole page in order).
     //   transfer fn   after a step with a symbol of weight w the state is one of w values (next_states[cum + slot], slot =
     //                 (state >> bits) - w) whatever it was before.  Each (segment, chain) takes the lightest symbol among its first
     //                 ANS_TF_LOOK steps as the pivot, replays the rest of the segment quietly once per slot (<= ANS_TF_MAX of them, ~0.12 ms
@@ -1853,7 +1853,7 @@ __global__ void __launch_bounds__(ANS_THREADS, 4) ans_encode_kernel(EncParams ep
         if (changed) sm.out_state[s][j] = uint16_t(my_out);
         const uint32_t n_changed = uint32_t(__syncthreads_count(changed ? 1 : 0));
         converged = n_changed == 0;
-        if (iter == 0 && n_changed > n_round) break;  // more than a quarter of the 4 n_round pairs (an eighth sent C5 float64 order 0 in-order: 3 ms instead of 1)
+        if (iter == 0 && n_changed > n_round) break;  // more than a quarter of the 4 n_round pairs (an eighth sent C5 float64 order 0 in-order, three times slower)
       }
       if (!converged) {
         if (!pivots_enumerable()) {

@@ -91,7 +91,7 @@ __global__ void __launch_bounds__(1024) gather_offsets_kernel(const uint64_t* __
 // `n` bytes from src to dst by one CTA, any alignment on either side.  dst is written in aligned 16-byte stores (the unit NVLink moves
 // well); each is assembled from two ALIGNED 16-byte loads of the source (the second one is the next thread's first: an L1 hit) with a
 // word select and a funnel shift.  A thread keeps GATHER_UNROLL units in flight - the loop is bound by the latency of its loads, the
-// stores are posted - which is what lets a few CTAs fill the links (one unit per thread and iteration: 7 GB/s per CTA, four: ~13 GB/s, measured).
+// stores are posted - which is what lets a few CTAs fill the links (four units per thread and iteration nearly doubled a CTA's rate over one).
 #ifndef PCOB_GATHER_UNROLL
 #define PCOB_GATHER_UNROLL 8
 #endif

@@ -1,4 +1,4 @@
-// libcpcodec.so — C-ABI entry points (include/cpcodec.h, include/pco_b200.h) over the sm_100a kernels.
+// libcpcodec.so — C-ABI entry points (include/cpcodec.h, include/pco_b200.h) over the sm_90a kernels.
 // There is no CPU implementation of the hot path in this library: without a CUDA device every
 // compute entry point fails with PCO_B200_CUDA.
 #include <algorithm>
@@ -80,7 +80,7 @@ static PcoB200Error ensure_device(Context& c) {
       c.device = dev;
       e = cudaGetDeviceProperties(&prop, dev);
       if (e != cudaSuccess) c.device_err = cudaGetErrorString(e);
-      else if (prop.major < 10) c.device_err = std::string("device ") + prop.name + " is not sm_100";
+      else if (prop.major != 9 || prop.minor != 0) c.device_err = std::string("device ") + prop.name + " is not sm_90 (the kernels are built for sm_90a only)";
       else {
         c.sm_count = prop.multiProcessorCount;
         // binomials mod 2^64 by Pascal additions
@@ -221,7 +221,7 @@ static PcoB200Error launch_decode(Context& c, const FileParams& fp, const uint8_
 }
 
 // Index-free decompress, the parallel part (the reference's decompressor walks chunk after chunk, standalone/decompressor.rs:150-215;
-// so did this library's serial walk_kernel<<<1>>>, at one GPU thread's ~0.2 GB/s).  Chunk lengths are not in the file, but the chunks
+// so does this library's serial walk_kernel<<<1>>>, at one GPU thread's speed).  Chunk lengths are not in the file, but the chunks
 // of a file nearly always start with the same 4 bytes - the type byte and count - 1 (docs/format.md:186-192).  So, from the first
 // unread chunk at `*next_byte`:
 //   1. find_chunk_starts_kernel lists every position behind it that carries the same 4 bytes (the real chunk starts of that size

@@ -121,17 +121,16 @@ inline CallTrace& call_trace() {
 
 // ---- large host <-> device copies: sliced, one slice in flight -----------------------------------------------------------------------
 // Copies of one direction issued on different streams do not share the link slice by slice: a copy engine stays with the stream it is
-// serving for as long as that stream has a copy queued (measured on this B200 with PCOB200_TRACE, profiles/r02_p_trace_tail.txt: with a
-// 268 MB upload running - whole, in 4 MB slices submitted in one go, or throttled to two slices in the queue - another host thread's
-// 48 MB upload waited until the last byte of the big one, 5 ms; the same in the other direction).  Two host threads that stream chunk
+// serving for as long as that stream has a copy queued (seen with PCOB200_TRACE: with a large upload running - whole, in 4 MB slices
+// submitted in one go, or throttled to two slices in the queue - another host thread's upload waited until the last byte of the big
+// one; the same in the other direction).  Two host threads that stream chunk
 // groups through compress and decompress then wait for each other's big copy in turn and the two PCIe directions never overlap.  So a
 // big copy goes out in 32 MB slices and the host submits a slice only when the previous one has finished: the stream's queue runs empty
-// every 0.6 ms, the engine turns to whoever else is waiting, and the copies of two threads alternate.  Cost: the submit latency of
-// ~10 us per slice when the thread has the link for itself (8 / 16 / 32 MB slices: streamed e2e 72.7 / 67.0 / 66.4 ms, one whole-array
-// call 101.6 / 98.2 / 96.6 ms; without slicing 96-97 ms for both).
-// Big copies of one direction take turns (r02_w: bench.py e2e trace): two host threads that each stream chunk groups through compress
+// after every slice, the engine turns to whoever else is waiting, and the copies of two threads alternate.  Cost: the submit latency
+// of one slice at a time when the thread has the link for itself (32 MB slices did better than 8 or 16 MB in the streamed e2e leg).
+// Big copies of one direction take turns (bench.py e2e trace): two host threads that each stream chunk groups through compress
 // start their uploads together, share the link slice by slice, finish together - and then both run their kernels and their small
-// downloads while the upload direction idles (2.5 ms of every 8.4 ms epoch), in lockstep for the rest of the array.  A process-wide turn
+// downloads while the upload direction idles, in lockstep for the rest of the array.  A process-wide turn
 // per direction makes the second thread's big upload wait for the first one's: the threads fall out of step, one uploads while the
 // other computes, and the link stays busy.  Small copies (a group's compressed bytes, at most two slices) do not take a turn: they slip
 // in between two slices of whoever holds it.  PCOB200_COPY_FIFO=0 restores plain slice-by-slice sharing.
@@ -176,8 +175,8 @@ inline cudaError_t copy_sliced(void* dst, const void* src, size_t bytes, cudaMem
 // ---- small device -> host readbacks that do not queue on a copy engine --------------------------------------------------------------
 // A call reads a few words back between its kernels (the one-pass front end's flags, the file size, the decode statuses) and waits for
 // them.  As a cudaMemcpyAsync such a readback is an entry in the device-to-host copy queue - behind whatever 32 MB slice another host
-// thread's download has in flight there, up to 0.6 ms each time (r02_y phase trace of the streamed e2e leg: 1.1-1.75 ms from the last
-// upload slice to the flags of a 64-chunk group, for 0.1 ms of kernels).  publish_kernel stores the words into a page-locked, device-
+// thread's download has in flight there, many times longer than the group's own kernels in the streamed e2e leg.  publish_kernel
+// stores the words into a page-locked, device-
 // mapped bounce buffer of the calling thread instead: an ordinary kernel on the call's stream, nothing in any copy queue; the stream
 // synchronisation that follows makes the stores visible to the host.  Readbacks beyond the bounce buffer, and PCOB200_READBACK_KERNEL=0,
 // take the copy.

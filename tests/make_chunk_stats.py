@@ -1,8 +1,8 @@
 """Planner parameters of the BASELINE configs (SURVEY.md 8d: "always record ans_size_log, n_bins, mean ans/offset bits per latent,
 compressed size"), read with pcodec_b200.inspect from chunk 0 (seed 0, 2^18 numbers) of every config.
 
-The bytes come from the CPU oracle, so this runs without a GPU; profiles/r01_m_config_sweep.md (column "chunk 0 bytes == oracle")
-shows that the GPU path writes these same bytes for C1, C3 and every C5 row, tests/test_gpu_encode.py the same for C2.
+The bytes come from the CPU oracle, so this runs without a GPU; tests/test_gpu_baseline_fullsize.py checks that the GPU path writes
+these same bytes for C1, C2, C3 and every C5 row.
 Usage: python tests/make_chunk_stats.py [out.md]      (tests/ may use the oracle; the product never does)
 """
 import os
@@ -43,10 +43,10 @@ for dtype in (np.uint8, np.uint16, np.int32, np.int64, np.float32, np.float64):
     for order in range(8):
         add(f"C5 {np.dtype(dtype).name} order {order}", nums, mode=o.MODE_CLASSIC, delta=o.DELTA_CONSECUTIVE if order else o.DELTA_NOOP, delta_order=order, enable_8_bit=True)
 
-out = sys.argv[1] if len(sys.argv) > 1 else "profiles/chunk_stats.md"
+out = sys.argv[1] if len(sys.argv) > 1 else "chunk_stats.md"
 with open(out, "w") as f:
     f.write("Planner parameters of the BASELINE configs: chunk 0 (seed 0, 2^18 numbers, level 8) of each config, read by `pcodec_b200.inspect` from\n"
-            "the oracle's bytes (`tests/make_chunk_stats.py`; the GPU path writes the same bytes - `r01_m_config_sweep.md`, `tests/test_gpu_encode.py`).\n"
+            "the oracle's bytes (`tests/make_chunk_stats.py`; the GPU path writes the same bytes - `tests/test_gpu_baseline_fullsize.py`).\n"
             "avg bits are per stored latent, from the bin weights as `pco inspect` computes them (pco_cli/src/inspect/mod.rs:96-121): tANS part\n"
             "= sum w (size_log - log2 w) / 2^size_log, offset part = sum w offset_bits / 2^size_log.  ratio = number bytes / (chunk meta + page).\n\n")
     f.write("| config | mode | delta | primary n_bins | ans_size_log | avg tANS bits | avg offset bits | secondary n_bins | ans_size_log | avg tANS bits | avg offset bits | meta bytes | page bytes | ratio |\n")

@@ -2,9 +2,7 @@
 (pcodec_b200/csrc/compress_host.cuh, mode_search.hpp).  The search itself is covered on CPU (tests/test_mode_search_host.py); this file
 checks the wiring: with an explicit delta, Auto-mode bytes equal the oracle's Auto-mode bytes.
 
-NOT YET RUN ON A GPU: the wiring was written after round 1's GPU budget was spent, so the library keeps it opt-in and these cases
-only run when PCOB200_RUN_UNVALIDATED=1 is set (first thing to do with the next GPU budget); without it they are skipped.
-The library reads the switch once per process, hence the child process.
+The library keeps this search opt-in and reads the switch once per process, hence the child process.
 """
 import os
 import subprocess

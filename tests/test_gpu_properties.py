@@ -1,8 +1,6 @@
 """Property test of the GPU path against the oracle (hypothesis): for any in-scope number type, data shape, mode, consecutive delta
 order, level and paging, the GPU writes the oracle's bytes and decodes them back bit for bit; anything the path refuses is refused as
-Unsupported, never mis-encoded.  Same generators as tests/test_oracle_properties.py.
-
-First run on a B200 in round 2 (profiles/r02_a_unvalidated_tests.txt: passed), un-gated since."""
+Unsupported, never mis-encoded.  Same generators as tests/test_oracle_properties.py."""
 import numpy as np
 import pytest
 from hypothesis import HealthCheck, given, settings
@@ -25,12 +23,13 @@ def gpu_configs(draw, dtype):
 
 
 def _dump_failure(nums, kw, got, want):
-    """A falsifying example is data: keep it (numbers, config, both files) where the GPU call's scratch directory travels back from."""
+    """A falsifying example is data: keep it (numbers, config, both files) in $PCOB200_PROP_DUMP, or the temporary directory."""
     import hashlib
     import json
     import os
+    import tempfile
 
-    root = os.environ.get("PCOB200_PROP_DUMP") or os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out")
+    root = os.environ.get("PCOB200_PROP_DUMP") or os.path.join(tempfile.gettempdir(), "pcodec_prop_failures")
     try:
         os.makedirs(root, exist_ok=True)
         tag = hashlib.sha1(nums.tobytes() + repr(sorted((k, str(v)) for k, v in kw.items())).encode()).hexdigest()[:12]
