@@ -213,6 +213,46 @@ PcoB200Error pco_b200_chunk_meta_size(const void *src, size_t src_len, unsigned 
 PcoB200Error pco_b200_page_decompress(const void *chunk_meta, size_t meta_len, const void *page, size_t page_len, size_t page_n,
                                       unsigned char dtype, void *dst, size_t dst_len, PcoB200Progress *progress, size_t *bytes_read);
 
+/* ---- batched wrapped format (no reference counterpart; SURVEY.md 8b): many pages of a wrapped container in one call, every
+ * buffer optionally resident in HBM, work on the caller's stream (the call returns once it is done).  Wrapped format 4.x, the
+ * version pco_b200_file_decompressor_read_header accepts.
+ * One wrapped page: where its chunk's meta and its own bytes are.  Pages of one chunk share a meta by pointing at the same
+ * meta_offset (pco/src/wrapped/chunk_compressor.rs:129-140). */
+typedef struct PcoB200PageRef {
+  uint64_t meta_offset;  /* byte offset of the page's chunk meta in `metas` */
+  uint64_t meta_len;     /* byte length of that meta (a chunk meta is byte-padded) */
+  uint64_t page_offset;  /* byte offset of the page in `pages` */
+  uint64_t page_len;     /* bytes available for the page (may exceed what it uses) */
+  uint64_t page_n;       /* numbers in the page, 1..2^24 */
+} PcoB200PageRef;
+
+/* ChunkDecompressor::page_decompressor + PageDecompressor::read (pco/src/wrapped/page_decompressor.rs:193-252) for n_pages pages:
+ * page i decodes into dst right after page i - 1, in refs order, and *n_written = the sum of page_n.  Each page's numbers equal what
+ * pco_b200_page_decompress gives for it.  Refs may come in any order and may repeat a page; metas and pages may be one buffer.
+ * PCO_B200_SRC_ON_DEVICE covers metas and pages, PCO_B200_DST_ON_DEVICE covers dst; refs are host memory.
+ * Refused before any device work: null refs (n_pages > 0), a meta or page range outside its buffer, page_n outside 1..2^24 and
+ * dst_len < the sum of page_n (PCO_B200_INVALID_ARGUMENT), an unknown dtype (PCO_B200_INVALID_TYPE); n_pages == 0 is OK.
+ * A page that fails on the device fails the call with the kind of the lowest-index failing page, and the message names it
+ * ("page 17: ..."); a meta_len other than the length its meta parses to is PCO_B200_INVALID_ARGUMENT, a page cut short
+ * PCO_B200_INSUFFICIENT_DATA.  Pages the fast kernels decline (Dict, Lookback, Conv1, tables above 2^10 states or 256 bins,
+ * f16 FloatMult) are decoded by the single-thread catch-all decoder. */
+PcoB200Error pco_b200_decompress_pages(const void *metas, size_t metas_len, const void *pages, size_t pages_len,
+                                       unsigned char dtype, const PcoB200PageRef *refs, size_t n_pages,
+                                       void *dst, size_t dst_len, size_t *n_written, uint32_t flags, void *cuda_stream);
+
+/* FileCompressor::chunk_compressor + ChunkCompressor::write_meta / write_page (pco/src/wrapped/chunk_compressor.rs) for a whole
+ * array: split into the chunks pco_b200_simple_compress would write (config's PagingSpec), each written as a wrapped chunk of ONE
+ * page - byte-identical to the reference's ChunkCompressor with Exact([n_i]) paging, as its standalone compressor uses it
+ * (FileCompressor::chunk_compressor_dyn).  Metas go back to back into `metas`, pages into `pages`, one PcoB200PageRef per chunk
+ * into `refs`.  Accepts and refuses configs as pco_b200_compress_ex does.  PCO_B200_SRC_ON_DEVICE covers nums,
+ * PCO_B200_DST_ON_DEVICE covers metas and pages; refs are host memory.  A capacity that is too small is PCO_B200_IO, with
+ * *metas_len, *pages_len and *n_chunks still reporting what is needed. */
+PcoB200Error pco_b200_compress_wrapped(const void *nums, size_t n, unsigned char dtype, const PcoB200ChunkConfig *config,
+                                       void *metas, size_t metas_cap, size_t *metas_len,
+                                       void *pages, size_t pages_cap, size_t *pages_len,
+                                       PcoB200PageRef *refs, size_t refs_cap, size_t *n_chunks,
+                                       uint32_t flags, void *cuda_stream);
+
 #if defined(__cplusplus)
 }
 #endif

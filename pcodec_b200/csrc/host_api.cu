@@ -10,6 +10,7 @@
 #include "gather_kernels.cuh"
 #include "decode_cold.cuh"
 #include "host_common.hpp"
+#include "wrapped_kernels.cuh"
 
 namespace pcob200 {
 
@@ -24,6 +25,7 @@ struct Context {
   bool device_ok = false;
   std::string device_err;
   DevBuf src, out, index, statuses, misc, dec_syms, dec_offs, dec_narrow, gather, cold, spec;
+  DevBuf wrap_metas, wrap_frames, wrap_tab, wrap_res, wrap_file, wrap_index, wrap_out;  // pco_b200_decompress_pages / pco_b200_compress_wrapped
   CompressScratch enc;
   Binoms* d_binoms = nullptr;
   int sm_count = 0;
@@ -42,7 +44,8 @@ static Context& ctx() {
 }
 
 static void release_buffers(Context& c) {
-  for (DevBuf* b : {&c.src, &c.out, &c.index, &c.statuses, &c.misc, &c.dec_syms, &c.dec_offs, &c.dec_narrow, &c.gather, &c.cold, &c.spec}) b->release();
+  for (DevBuf* b : {&c.src, &c.out, &c.index, &c.statuses, &c.misc, &c.dec_syms, &c.dec_offs, &c.dec_narrow, &c.gather, &c.cold, &c.spec, &c.wrap_metas, &c.wrap_frames,
+                  &c.wrap_tab, &c.wrap_res, &c.wrap_file, &c.wrap_index, &c.wrap_out}) b->release();
   c.enc.release();
   c.gather_err = nullptr;
   c.d_cls = nullptr;
@@ -1039,6 +1042,330 @@ PcoB200Error pco_b200_decompress_chunks(const void* compressed, size_t compresse
   }
   if (n_written) *n_written = size_t(n_total);
   return PCO_B200_OK;
+}
+
+// ---------------------------------------------------------------------------
+// Batched wrapped pages (wrapped_kernels.cuh).  Decode: every page is framed as a standalone chunk in scratch, all of them are walked
+// at once and the ordinary decode kernels take the pages they serve; the pages they decline go through cold_decode_kernel, one launch
+// per page.  Encode: the CHUNKS_ONLY pipeline, then every chunk's meta and page are split into the caller's two buffers.
+// ---------------------------------------------------------------------------
+static PcoB200Error page_fail(PcoB200Error kind, size_t page, const std::string& what) {
+  return fail(kind, "page " + std::to_string(page) + ": " + what);
+}
+static PcoB200Error page_status_fail(uint32_t st, size_t page) {
+  const PcoB200Error e = status_to_error(st, "the page");
+  return page_fail(e, page, last_error_ref());
+}
+
+static PcoB200Error decompress_pages_impl(const void* metas, size_t metas_len, const void* pages, size_t pages_len, uint32_t dtype,
+                                          const PcoB200PageRef* refs, size_t n_pages, void* dst, size_t dst_len, size_t* n_written, uint32_t flags,
+                                          cudaStream_t stream) {
+  // ---- argument checks: host only, before any device work
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (n_written) *n_written = 0;
+  if (n_pages == 0) return PCO_B200_OK;
+  if (!refs) return fail(PCO_B200_INVALID_ARGUMENT, "refs are required");
+  if (n_pages > 0x7ffffffeull) return fail(PCO_B200_INVALID_ARGUMENT, "too many pages");
+  if ((!metas && metas_len) || (!pages && pages_len) || !dst) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  // page table, and the index skeleton: one IndexChunk per page plus a spare one (a failing page walked on its own)
+  const uint64_t chunks_offset = sizeof(IndexHeader);
+  uint64_t entries = (chunks_offset + (uint64_t(n_pages) + 1) * sizeof(IndexChunk) + 15) & ~uint64_t(15);
+  std::vector<WrappedPage> tab(n_pages);
+  std::vector<IndexChunk> recs(n_pages + 1);
+  uint64_t frames_len = 0, n_total = 0;
+  for (size_t i = 0; i < n_pages; i++) {
+    const PcoB200PageRef& r = refs[i];
+    if (r.meta_len > metas_len || r.meta_offset > metas_len - r.meta_len) return page_fail(PCO_B200_INVALID_ARGUMENT, i, "chunk meta lies outside metas");
+    if (r.page_len > pages_len || r.page_offset > pages_len - r.page_len) return page_fail(PCO_B200_INVALID_ARGUMENT, i, "page lies outside pages");
+    if (r.page_n == 0 || r.page_n > (uint64_t(1) << 24)) return page_fail(PCO_B200_INVALID_ARGUMENT, i, "page n must be 1..2^24");
+    WrappedPage& w = tab[i];
+    w.meta_off = r.meta_offset; w.meta_len = r.meta_len; w.page_off = r.page_offset; w.page_len = r.page_len;
+    w.frame_off = frames_len; w.page_n = uint32_t(r.page_n); w.pad = 0;
+    recs[i].chunk_offset = frames_len;
+    recs[i].n = uint32_t(r.page_n);
+    recs[i].n_vars = 0;
+    recs[i].entries_offset = entries;
+    recs[i].out_offset = n_total;
+    entries += (uint64_t(MAX_VARS) * n_batches_of(uint32_t(r.page_n)) * sizeof(BatchEntry) + 15) & ~uint64_t(15);
+    frames_len += (4 + r.meta_len + r.page_len + 15) & ~uint64_t(15);  // 16-byte aligned chunk starts for the kernels' block reads
+    n_total += r.page_n;
+  }
+  if (n_total > dst_len) return fail(PCO_B200_INVALID_ARGUMENT, "dst holds " + std::to_string(dst_len) + " numbers, the pages " + std::to_string(n_total));
+
+  Context& c = ctx();
+  if (PcoB200Error e = ensure_device(c)) return e;
+  const bool src_dev = flags & PCO_B200_SRC_ON_DEVICE, dst_dev = flags & PCO_B200_DST_ON_DEVICE;
+  const size_t elem = nt_bits(dtype) / 8;
+  const uint32_t n = uint32_t(n_pages);
+  const uint8_t* d_metas = static_cast<const uint8_t*>(metas);
+  const uint8_t* d_pages = static_cast<const uint8_t*>(pages);
+  if (!src_dev) {
+    PCOB_CUDA_TRY(c.wrap_metas.reserve(metas_len + 16));
+    PCOB_CUDA_TRY(c.src.reserve(pages_len + 16));
+    if (metas_len) PCOB_CUDA_TRY(copy_sliced(c.wrap_metas.p, metas, metas_len, cudaMemcpyHostToDevice, stream));
+    if (pages_len) PCOB_CUDA_TRY(copy_sliced(c.src.p, pages, pages_len, cudaMemcpyHostToDevice, stream));
+    d_metas = c.wrap_metas.as<uint8_t>();
+    d_pages = c.src.as<uint8_t>();
+  }
+  PCOB_CUDA_TRY(c.wrap_tab.reserve(n_pages * sizeof(WrappedPage)));
+  PCOB_CUDA_TRY(cudaMemcpyAsync(c.wrap_tab.p, tab.data(), n_pages * sizeof(WrappedPage), cudaMemcpyHostToDevice, stream));
+  PCOB_CUDA_TRY(c.index.reserve(entries + 64));
+  uint8_t* d_index = c.index.as<uint8_t>();
+  PCOB_CUDA_TRY(cudaMemcpyAsync(d_index + chunks_offset, recs.data(), n_pages * sizeof(IndexChunk), cudaMemcpyHostToDevice, stream));
+  PCOB_CUDA_TRY(c.wrap_frames.reserve(frames_len + 64));
+  uint8_t* d_frames = c.wrap_frames.as<uint8_t>();
+  // results: frame_pages_kernel's route per page | walk status per page | walk end per page | the spare walk's status
+  const size_t res_words = 2 * size_t(n) + 2 * size_t(n) + 2;
+  PCOB_CUDA_TRY(c.wrap_res.reserve(res_words * 4 + 64));
+  uint32_t* d_pstat = c.wrap_res.as<uint32_t>();
+  uint32_t* d_wst = d_pstat + n;
+  uint64_t* d_ends = reinterpret_cast<uint64_t*>(d_pstat + 2 * size_t(n));  // 8-byte aligned: 2n words behind the buffer's start
+  uint32_t* d_spare_st = reinterpret_cast<uint32_t*>(d_ends + n);
+  PCOB_CUDA_TRY(cudaMemsetAsync(d_wst, 0xff, size_t(n) * 4, stream));
+  PCOB_CUDA_TRY(c.misc.reserve(sizeof(WalkResult)));
+  profiler().begin("frame_pages_kernel", stream);
+  frame_pages_kernel<<<n, WRAP_THREADS, 0, stream>>>(d_metas, metas_len, d_pages, dtype, c.wrap_tab.as<WrappedPage>(), d_frames, d_pstat);
+  profiler().end(stream);
+  PCOB_CUDA_TRY(cudaGetLastError());
+  const FileParams fp{d_frames, frames_len, dtype, 0, 4};  // wrapped format 4.x; a page carries no uniform type
+  profiler().begin("walk_kernel", stream);
+  walk_kernel<SMALL_MAX_SIZE_LOG><<<n, WALK_THREADS, sizeof(WalkSmem<SMALL_MAX_SIZE_LOG>), stream>>>(
+      fp, d_index, chunks_offset, n, 0, entries, 0, 0, ~uint64_t(0), d_wst, c.misc.as<WalkResult>(), 0, d_ends);
+  profiler().end(stream);
+  PCOB_CUDA_TRY(cudaGetLastError());
+  std::vector<uint32_t> res(4 * size_t(n));
+  PCOB_CUDA_TRY(readback_small_sync(res.data(), d_pstat, res.size() * 4, stream));
+  const uint32_t* pstat = res.data();
+  const uint32_t* wst = pstat + n;
+  const uint64_t* ends = reinterpret_cast<const uint64_t*>(pstat + 2 * size_t(n));
+
+  // ---- routes: fast kernels, catch-all decoder, or the first failing page (nothing behind it needs decoding)
+  std::vector<uint32_t> fast, cold;
+  size_t fail_page = n_pages;
+  uint32_t fail_st = ST_OK;                   // the failure's device status, unless
+  PcoB200Error decode_kind = PCO_B200_OK;     // the decode kernels reported it (kind and message)
+  std::string decode_msg;
+  for (uint32_t i = 0; i < n; i++) {
+    const uint64_t frame_end = tab[i].frame_off + 4 + tab[i].meta_len + tab[i].page_len;
+    uint32_t st = pstat[i];
+    bool rewalk = false;
+    if (st == ST_OK) {
+      st = wst[i];
+      if (st == ST_UNSUPPORTED) st = WP_COLD;
+      else if (st == ST_OK && ends[i] > frame_end) st = ST_INSUFFICIENT_DATA;  // the walk ran past the page into the next frame
+      else rewalk = st != ST_OK;
+    }
+    if (st == ST_OK) { fast.push_back(i); continue; }
+    if (st == WP_COLD) { cold.push_back(i); continue; }
+    fail_page = i;
+    fail_st = st;
+    if (rewalk) {
+      // a walk that leaves its page reads the next frame, not the zeros pco_b200_page_decompress would see there: walk the page once
+      // more over its own frame alone for the kind that call reports
+      IndexChunk one = recs[i];
+      one.chunk_offset = 0;
+      PCOB_CUDA_TRY(cudaMemcpyAsync(d_index + chunks_offset + uint64_t(n) * sizeof(IndexChunk), &one, sizeof(one), cudaMemcpyHostToDevice, stream));
+      PCOB_CUDA_TRY(cudaMemsetAsync(d_spare_st, 0xff, 4, stream));
+      const FileParams fp1{d_frames + tab[i].frame_off, frame_end - tab[i].frame_off, dtype, 0, 4};
+      walk_kernel<SMALL_MAX_SIZE_LOG><<<1, WALK_THREADS, sizeof(WalkSmem<SMALL_MAX_SIZE_LOG>), stream>>>(
+          fp1, d_index, chunks_offset + uint64_t(n) * sizeof(IndexChunk), 1, 0, entries, 0, 0, ~uint64_t(0), d_spare_st, c.misc.as<WalkResult>(), 0);
+      PCOB_CUDA_TRY(cudaGetLastError());
+      uint32_t st1 = ST_OK;
+      PCOB_CUDA_TRY(readback_small_sync(&st1, d_spare_st, 4, stream));
+      if (st1 != ST_OK) fail_st = st1;
+    }
+    break;
+  }
+
+  void* d_out = dst;
+  if (!dst_dev) {
+    PCOB_CUDA_TRY(c.out.reserve(n_total * elem + 64));
+    d_out = c.out.p;
+  }
+  const uint64_t out_len = dst_dev ? uint64_t(dst_len) : n_total;
+  // ---- fast pages: the ordinary decode over their walked index records
+  if (!fast.empty()) {
+    if (fast.size() != n_pages) {  // some pages take another route: keep the records of the fast ones, in page order
+      std::vector<IndexChunk> walked(n_pages), sel;
+      PCOB_CUDA_TRY(cudaMemcpyAsync(walked.data(), d_index + chunks_offset, n_pages * sizeof(IndexChunk), cudaMemcpyDeviceToHost, stream));
+      PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
+      sel.reserve(fast.size());
+      for (uint32_t i : fast) sel.push_back(walked[i]);
+      PCOB_CUDA_TRY(cudaMemcpyAsync(d_index + chunks_offset, sel.data(), sel.size() * sizeof(IndexChunk), cudaMemcpyHostToDevice, stream));
+    }
+    if (PcoB200Error e = launch_decode(c, fp, d_index, entries, chunks_offset, uint32_t(fast.size()), d_out, out_len, stream)) {
+      if (e == PCO_B200_CUDA) return e;
+      // launch_decode names the first failing chunk of its launch ("... in chunk k"): the k-th fast page
+      const std::string msg = last_error_ref();
+      const size_t at = msg.rfind("chunk ");
+      const size_t k = at == std::string::npos ? 0 : size_t(std::strtoull(msg.c_str() + at + 6, nullptr, 10));
+      const size_t page = fast[std::min(k, fast.size() - 1)];
+      if (page < fail_page) {
+        fail_page = page;
+        decode_kind = e;
+        decode_msg = msg;
+      }
+    }
+  }
+  while (!cold.empty() && cold.back() > fail_page) cold.pop_back();  // pages behind a failing one need no decoding
+  // ---- pages only the catch-all decoder takes: one single-thread launch per page, straight into the page's slot of the output.
+  // One launch per page rather than one over a file of all of them: a page may be followed by bytes it does not use, and the catch-all
+  // decoder would read those as the next chunk.
+  if (!cold.empty()) {
+    const size_t nc = cold.size();
+    PCOB_CUDA_TRY(c.wrap_res.reserve(nc * sizeof(ColdResult) + 64));
+    ColdResult* d_cres = c.wrap_res.as<ColdResult>();
+    std::vector<ColdResult> cres(nc);
+    std::vector<size_t> todo(nc);
+    for (size_t k = 0; k < nc; k++) todo[k] = k;
+    for (uint32_t window_cap : {16u, COLD_MAX_WINDOW_LOG}) {  // lookback windows beyond 2^16 numbers get the large scratch on a second pass
+      if (todo.empty()) break;
+      PCOB_CUDA_TRY(c.cold.reserve(cold_scratch_bytes(window_cap)));
+      profiler().begin("cold_decode_kernel", stream);
+      for (size_t k : todo) {
+        const WrappedPage& w = tab[cold[k]];
+        const FileParams fpk{d_frames + w.frame_off, 4 + w.meta_len + w.page_len, dtype, 0, 4};
+        dispatch_latent(dtype, [&](auto tag) {
+          using L = decltype(tag);
+          cold_decode_kernel<L><<<1, 32, 0, stream>>>(fpk, 0, static_cast<L*>(d_out) + recs[cold[k]].out_offset, w.page_n, c.cold.as<uint8_t>(), window_cap, d_cres + k);
+          return 0;
+        });
+      }
+      profiler().end(stream);
+      PCOB_CUDA_TRY(cudaGetLastError());
+      PCOB_CUDA_TRY(readback_small_sync(cres.data(), d_cres, nc * sizeof(ColdResult), stream));
+      std::vector<size_t> again;
+      for (size_t k : todo)
+        if (cres[k].n_chunks == 0 && cres[k].status == ST_UNSUPPORTED) again.push_back(k);
+      todo.swap(again);
+    }
+    // the page is decoded once its chunk is (what the decoder reads behind it is not the page's)
+    for (size_t k = 0; k < nc; k++)
+      if (cres[k].n_chunks == 0) {
+        if (cold[k] < fail_page) { fail_page = cold[k]; fail_st = cres[k].status; decode_kind = PCO_B200_OK; }
+        break;
+      }
+  }
+  if (fail_page < n_pages) return decode_kind != PCO_B200_OK ? page_fail(decode_kind, fail_page, decode_msg) : page_status_fail(fail_st, fail_page);
+  if (!dst_dev) {
+    PCOB_CUDA_TRY(copy_sliced(dst, d_out, n_total * elem, cudaMemcpyDeviceToHost, stream));
+  }
+  PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
+  if (n_written) *n_written = size_t(n_total);
+  return PCO_B200_OK;
+}
+
+PcoB200Error pco_b200_decompress_pages(const void* metas, size_t metas_len, const void* pages, size_t pages_len, unsigned char dtype,
+                                       const PcoB200PageRef* refs, size_t n_pages, void* dst, size_t dst_len, size_t* n_written, uint32_t flags,
+                                       void* cuda_stream) {
+  const PcoB200Error e = decompress_pages_impl(metas, metas_len, pages, pages_len, dtype, refs, n_pages, dst, dst_len, n_written, flags,
+                                               static_cast<cudaStream_t>(cuda_stream));
+  profiler().resolve();
+  return e;
+}
+
+static PcoB200Error compress_wrapped_impl(const void* nums, size_t n, uint32_t dtype, const PcoB200ChunkConfig* config, void* metas, size_t metas_cap,
+                                          size_t* metas_len, void* pages, size_t pages_cap, size_t* pages_len, PcoB200PageRef* refs, size_t refs_cap,
+                                          size_t* n_chunks_out, uint32_t flags, cudaStream_t stream) {
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if ((!metas && metas_cap) || (!pages && pages_cap) || (!refs && refs_cap)) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (metas_len) *metas_len = 0;
+  if (pages_len) *pages_len = 0;
+  if (n_chunks_out) *n_chunks_out = 0;
+  PcoB200ChunkConfig cfg;
+  if (config) cfg = *config;
+  else {
+    std::memset(&cfg, 0, sizeof(cfg));  // pco::ChunkConfig::default()
+    cfg.compression_level = 8;
+  }
+  Context& c = ctx();
+  if (PcoB200Error e = ensure_device(c)) return e;
+  // the chunks simple_compress would write; a paging spec that does not fit is reported by the pipeline, with its other checks
+  std::vector<uint64_t> chunk_ns;
+  if (n_per_page(cfg, n, &chunk_ns) != PCO_B200_OK) chunk_ns.clear();
+  const uint32_t lbits = nt_bits(dtype);
+  size_t cap = 64;
+  for (uint64_t p : chunk_ns) cap += standalone_chunk_size_guarantee(lbits, size_t(p));
+  const size_t icap = pco_b200_index_size_bound(n, chunk_ns.size()) + 64 * chunk_ns.size();
+  PCOB_CUDA_TRY(c.wrap_file.reserve(cap + 32));
+  PCOB_CUDA_TRY(c.wrap_index.reserve(icap));
+  uint8_t* d_file = c.wrap_file.as<uint8_t>();
+  uint8_t* d_idx = c.wrap_index.as<uint8_t>();
+  CompressResult cr;
+  // an empty array is compressed (the config still checked) with host buffers: no chunk, nothing on the device to split
+  const bool empty = n == 0;
+  IndexHeader empty_ih;
+  uint8_t empty_dst[8];
+  const uint32_t cflags = (flags & PCO_B200_SRC_ON_DEVICE) | PCO_B200_CHUNKS_ONLY | (empty ? 0u : (PCO_B200_DST_ON_DEVICE | PCO_B200_INDEX_ON_DEVICE));
+  PcoB200Error e = dispatch_latent(dtype, [&](auto tag) {
+    using L = decltype(tag);
+    return compress_typed<L>(c.enc, nums, n, dtype, cfg, false, empty ? static_cast<void*>(empty_dst) : d_file, empty ? sizeof(empty_dst) : cap,
+                             empty ? static_cast<void*>(&empty_ih) : d_idx, empty ? sizeof(empty_ih) : icap, cflags, stream, &cr);
+  });
+  if (e != PCO_B200_OK || empty) return e;
+  const uint32_t nc = uint32_t(chunk_ns.size());
+  // scratch: sizes | refs | totals | error word
+  PCOB_CUDA_TRY(c.wrap_res.reserve(size_t(nc) * (8 + sizeof(PcoB200PageRef)) + 64));
+  uint64_t* d_sizes = c.wrap_res.as<uint64_t>();
+  PcoB200PageRef* d_refs = reinterpret_cast<PcoB200PageRef*>(d_sizes + nc);
+  uint64_t* d_tot = reinterpret_cast<uint64_t*>(d_refs + nc);
+  uint32_t* d_err = reinterpret_cast<uint32_t*>(d_tot + 2);
+  PCOB_CUDA_TRY(cudaMemsetAsync(d_err, 0, 4, stream));
+  profiler().begin("chunk_refs_kernel", stream);
+  chunk_sizes_kernel<<<std::min<uint32_t>((nc + 255) / 256, 1024), 256, 0, stream>>>(d_idx, cr.index_bytes, d_sizes, nc, d_err);
+  // compress_typed writes the IndexChunk records right behind the header
+  chunk_refs_kernel<<<1, 1024, 0, stream>>>(d_file, reinterpret_cast<const IndexChunk*>(d_idx + sizeof(IndexHeader)), d_sizes, nc, dtype, d_refs, d_tot, d_err);
+  profiler().end(stream);
+  PCOB_CUDA_TRY(cudaGetLastError());
+  const bool dst_dev = flags & PCO_B200_DST_ON_DEVICE;
+  const IndexChunk* d_chunks = reinterpret_cast<const IndexChunk*>(d_idx + sizeof(IndexHeader));
+  if (dst_dev) {
+    // device buffers: the split goes out right behind the scan and checks the totals against the capacities itself, so that one
+    // readback serves the whole call
+    profiler().begin("split_chunks_kernel", stream);
+    split_chunks_kernel<<<nc, WRAP_THREADS, 0, stream>>>(d_file, d_chunks, d_refs, d_tot, d_err, metas_cap, pages_cap, nc <= refs_cap ? 1u : 0u,
+                                                         static_cast<uint8_t*>(metas), static_cast<uint8_t*>(pages));
+    profiler().end(stream);
+    PCOB_CUDA_TRY(cudaGetLastError());
+  }
+  std::vector<PcoB200PageRef> h_refs(nc);
+  struct { uint64_t tot[2]; uint32_t err, pad; } tail;
+  static_assert(sizeof(PcoB200PageRef) == 40, "ref layout");
+  std::vector<uint32_t> back((size_t(nc) * sizeof(PcoB200PageRef) + 20) / 4);
+  PCOB_CUDA_TRY(readback_small_sync(back.data(), d_refs, back.size() * 4, stream));
+  std::memcpy(h_refs.data(), back.data(), size_t(nc) * sizeof(PcoB200PageRef));
+  std::memcpy(&tail, reinterpret_cast<const uint8_t*>(back.data()) + size_t(nc) * sizeof(PcoB200PageRef), 20);
+  if (tail.err != 0) return fail(PCO_B200_CUDA, "compressor returned chunks that do not split into meta and page");
+  if (metas_len) *metas_len = size_t(tail.tot[0]);
+  if (pages_len) *pages_len = size_t(tail.tot[1]);
+  if (n_chunks_out) *n_chunks_out = nc;
+  if (tail.tot[0] > metas_cap || tail.tot[1] > pages_cap || nc > refs_cap)
+    return fail(PCO_B200_IO, "failed to write whole buffer (need " + std::to_string(tail.tot[0]) + " meta bytes, " + std::to_string(tail.tot[1]) +
+                                 " page bytes and " + std::to_string(nc) + " refs)");
+  if (!dst_dev) {  // host buffers: split into scratch, then two copies down
+    const uint64_t pages_at = (tail.tot[0] + 15) & ~uint64_t(15);
+    PCOB_CUDA_TRY(c.wrap_out.reserve(pages_at + tail.tot[1] + 32));
+    uint8_t* d_metas = c.wrap_out.as<uint8_t>();
+    uint8_t* d_pages = d_metas + pages_at;
+    profiler().begin("split_chunks_kernel", stream);
+    split_chunks_kernel<<<nc, WRAP_THREADS, 0, stream>>>(d_file, d_chunks, d_refs, d_tot, d_err, ~uint64_t(0), ~uint64_t(0), 1u, d_metas, d_pages);
+    profiler().end(stream);
+    PCOB_CUDA_TRY(cudaGetLastError());
+    if (tail.tot[0]) PCOB_CUDA_TRY(copy_sliced(metas, d_metas, tail.tot[0], cudaMemcpyDeviceToHost, stream));
+    if (tail.tot[1]) PCOB_CUDA_TRY(copy_sliced(pages, d_pages, tail.tot[1], cudaMemcpyDeviceToHost, stream));
+    PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
+  }
+  std::memcpy(refs, h_refs.data(), size_t(nc) * sizeof(PcoB200PageRef));
+  return PCO_B200_OK;
+}
+
+PcoB200Error pco_b200_compress_wrapped(const void* nums, size_t n, unsigned char dtype, const PcoB200ChunkConfig* config, void* metas, size_t metas_cap,
+                                       size_t* metas_len, void* pages, size_t pages_cap, size_t* pages_len, PcoB200PageRef* refs, size_t refs_cap,
+                                       size_t* n_chunks, uint32_t flags, void* cuda_stream) {
+  const PcoB200Error e = compress_wrapped_impl(nums, n, dtype, config, metas, metas_cap, metas_len, pages, pages_cap, pages_len, refs, refs_cap, n_chunks,
+                                               flags, static_cast<cudaStream_t>(cuda_stream));
+  profiler().resolve();
+  return e;
 }
 
 PcoB200Error pco_b200_build_index(const void* compressed, size_t compressed_len, unsigned char dtype, void* index, size_t index_cap,

@@ -1,7 +1,12 @@
 """Mirror of pcodec.wrapped (pco_python/src/wrapped/{compressor,decompressor}.rs) over the C-ABI of libcpcodec.so.
 
-One page per chunk this round: `FileCompressor.chunk_compressor` raises PcoError("Unsupported") when the config's
-PagingSpec would cut the chunk into several pages (DESIGN.md section 8)."""
+A chunk's PagingSpec may cut it into several pages that share the chunk's bins.  Classic mode takes any number of pages; the
+two-var modes (IntMult / FloatMult / FloatQuant) take one page per chunk, and `FileCompressor.chunk_compressor` raises
+PcoError("Unsupported") when their PagingSpec would give several (DESIGN.md section 8).
+
+Batched forms for containers that keep chunk metas and pages themselves: `compress_chunks` writes a whole array as wrapped
+chunks of one page each, `decompress_pages` decodes any number of pages in one call.  Both take host buffers (bytes / numpy)
+or torch CUDA tensors; with CUDA tensors the work runs on torch.cuda.current_stream() and the outputs are CUDA tensors."""
 import ctypes as C
 
 import numpy as np
@@ -110,3 +115,120 @@ class FileDecompressor:
         n = C.c_size_t()
         _lib.check(_lib_wrapped().pco_b200_chunk_meta_size(sb.ctypes.data_as(C.c_void_p), C.c_size_t(sb.size), C.c_ubyte(_lib.dtype_byte(np.dtype(dtype))), C.byref(n)))
         return ChunkDecompressor(sb[: n.value].tobytes(), dtype), n.value
+
+
+# PcoB200PageRef (include/pco_b200.h): one page of a wrapped container
+PAGE_REF = np.dtype([("meta_offset", "<u8"), ("meta_len", "<u8"), ("page_offset", "<u8"), ("page_len", "<u8"), ("page_n", "<u8")])
+
+
+def _lib_batch():
+    L = _lib_wrapped()
+    if not getattr(L, "_batch_ready", False):
+        L.pco_b200_decompress_pages.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_ubyte, C.c_void_p, C.c_size_t, C.c_void_p,
+                                                C.c_size_t, C.POINTER(C.c_size_t), C.c_uint32, C.c_void_p]
+        L.pco_b200_compress_wrapped.argtypes = [C.c_void_p, C.c_size_t, C.c_ubyte, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t),
+                                                C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t),
+                                                C.c_uint32, C.c_void_p]
+        L._batch_ready = True
+    return L
+
+
+def _is_cuda(x):
+    return getattr(x, "is_cuda", False)
+
+
+def _torch_dtypes():
+    import torch
+
+    return {np.dtype(np.uint8): torch.uint8, np.dtype(np.int8): torch.int8, np.dtype(np.uint16): torch.uint16, np.dtype(np.int16): torch.int16,
+            np.dtype(np.float16): torch.float16, np.dtype(np.uint32): torch.uint32, np.dtype(np.int32): torch.int32, np.dtype(np.float32): torch.float32,
+            np.dtype(np.uint64): torch.uint64, np.dtype(np.int64): torch.int64, np.dtype(np.float64): torch.float64}
+
+
+def _host_u8(x):
+    if isinstance(x, np.ndarray):
+        return np.ascontiguousarray(x).reshape(-1).view(np.uint8)
+    return np.frombuffer(bytes(x), dtype=np.uint8)
+
+
+def _stream_of(t):
+    import torch
+
+    return C.c_void_p(torch.cuda.current_stream(t.device).cuda_stream)
+
+
+def compress_chunks(nums, config=None):
+    """Compresses `nums` into wrapped chunks of one page each - the chunks pco_b200_simple_compress would write for `config`'s
+    PagingSpec - in one call (pco_b200_compress_wrapped).  Returns (metas, pages, refs): the chunk metas back to back, the pages
+    back to back, and one PAGE_REF record per chunk.  Host input gives bytes; a torch CUDA tensor gives uint8 CUDA tensors."""
+    cfg = (config or ChunkConfig())._to_c()
+    L = _lib_batch()
+    ps = (config or ChunkConfig()).paging_spec
+    if _is_cuda(nums):
+        import torch
+
+        t = nums.contiguous()
+        dt = next(k for k, v in _torch_dtypes().items() if v == t.dtype)
+        n, src, flags, stream = t.numel(), C.c_void_p(t.data_ptr()), _lib.SRC_ON_DEVICE | _lib.DST_ON_DEVICE, _stream_of(t)
+
+        def alloc(nbytes):
+            return torch.empty(max(nbytes, 1), dtype=torch.uint8, device=t.device)
+
+        def ptr(buf):
+            return C.c_void_p(buf.data_ptr())
+    else:
+        arr = np.ascontiguousarray(nums)
+        dt, n, src, flags, stream = arr.dtype, arr.size, arr.ctypes.data_as(C.c_void_p), 0, None
+
+        def alloc(nbytes):
+            return np.empty(max(nbytes, 1), dtype=np.uint8)
+
+        def ptr(buf):
+            return buf.ctypes.data_as(C.c_void_p)
+    dtb = _lib.dtype_byte(dt)
+    n_chunks = len(ps.sizes) if ps.sizes is not None else -(-n // (ps.n or (1 << 18)))
+    caps = [n_chunks * 4096 + 64, L.pco_standalone_guarantee_file_size(n, dtb), n_chunks + 1]
+    ml, pl, nc = C.c_size_t(), C.c_size_t(), C.c_size_t()
+    for attempt in range(2):  # a first guess of the capacities, then what the call reported it needs
+        metas, pages, refs = alloc(caps[0]), alloc(caps[1]), np.zeros(max(caps[2], 1), dtype=PAGE_REF)
+        rc = L.pco_b200_compress_wrapped(src, C.c_size_t(n), C.c_ubyte(dtb), C.byref(cfg), ptr(metas), C.c_size_t(caps[0]), C.byref(ml), ptr(pages),
+                                         C.c_size_t(caps[1]), C.byref(pl), refs.ctypes.data_as(C.c_void_p), C.c_size_t(caps[2]), C.byref(nc),
+                                         C.c_uint32(flags), stream)
+        if rc == 4 and attempt == 0:  # PCO_B200_IO
+            caps = [max(caps[0], ml.value), max(caps[1], pl.value), max(caps[2], nc.value)]
+            continue
+        _lib.check(rc)
+        break
+    refs = refs[: nc.value].copy()
+    if _is_cuda(nums):
+        return metas[: ml.value], pages[: pl.value], refs
+    return metas[: ml.value].tobytes(), pages[: pl.value].tobytes(), refs
+
+
+def decompress_pages(metas, pages, refs, dtype):
+    """Decodes every page `refs` (PAGE_REF records, or anything with their five fields in that order) names into one array,
+    page after page in refs order (pco_b200_decompress_pages).  `metas` and `pages` are bytes / numpy, or torch CUDA tensors
+    (then the result is a CUDA tensor, computed on the current stream)."""
+    dt = np.dtype(dtype)
+    r = np.ascontiguousarray(np.asarray(refs).astype(PAGE_REF, copy=False))
+    total = int(r["page_n"].sum()) if r.size else 0
+    L = _lib_batch()
+    nw = C.c_size_t()
+    if _is_cuda(metas) or _is_cuda(pages):
+        import torch
+
+        if not (_is_cuda(metas) and _is_cuda(pages)):
+            raise TypeError("metas and pages must both be CUDA tensors or both be host buffers")
+        m, p = metas.contiguous(), pages.contiguous()
+        dst = torch.empty(max(total, 1), dtype=_torch_dtypes()[dt], device=p.device)
+        _lib.check(L.pco_b200_decompress_pages(C.c_void_p(m.data_ptr()), C.c_size_t(m.numel() * m.element_size()), C.c_void_p(p.data_ptr()),
+                                               C.c_size_t(p.numel() * p.element_size()), C.c_ubyte(_lib.dtype_byte(dt)), r.ctypes.data_as(C.c_void_p),
+                                               C.c_size_t(r.size), C.c_void_p(dst.data_ptr()), C.c_size_t(total), C.byref(nw),
+                                               C.c_uint32(_lib.SRC_ON_DEVICE | _lib.DST_ON_DEVICE), _stream_of(p)))
+        return dst[:total]
+    mb, pb = _host_u8(metas), _host_u8(pages)
+    dst = np.empty(max(total, 1), dtype=dt)
+    _lib.check(L.pco_b200_decompress_pages(mb.ctypes.data_as(C.c_void_p), C.c_size_t(mb.size), pb.ctypes.data_as(C.c_void_p), C.c_size_t(pb.size),
+                                           C.c_ubyte(_lib.dtype_byte(dt)), r.ctypes.data_as(C.c_void_p), C.c_size_t(r.size),
+                                           dst.ctypes.data_as(C.c_void_p), C.c_size_t(total), C.byref(nw), C.c_uint32(0), None))
+    return dst[:total]
