@@ -253,6 +253,51 @@ PcoB200Error pco_b200_compress_wrapped(const void *nums, size_t n, unsigned char
                                        PcoB200PageRef *refs, size_t refs_cap, size_t *n_chunks,
                                        uint32_t flags, void *cuda_stream);
 
+/* ---- batches of standalone files (no reference counterpart): many arrays of one number type in one call - a columnar writer's
+ * column chunks, a checkpoint's tensors - each its own standalone file with its own side index, every buffer optionally resident in
+ * HBM, work on the caller's stream (the call returns once it is done).  PCO_B200_SRC_ON_DEVICE covers `nums` / `src`,
+ * PCO_B200_DST_ON_DEVICE covers `dst`, PCO_B200_INDEX_ON_DEVICE covers `index`; `file_ns` and `files` are host memory.
+ * One file of a batch: where it is, and where its side index is. */
+typedef struct PcoB200FileRef {
+  uint64_t offset;        /* byte offset of the standalone file in its buffer */
+  uint64_t len;           /* its length in bytes */
+  uint64_t index_offset;  /* byte offset of its side index in the index buffer; a multiple of 16 */
+  uint64_t index_len;     /* 0 = no side index for this file */
+} PcoB200FileRef;
+
+/* pco_b200_compress_ex for n_files arrays at once: file i is the next file_ns[i] numbers of `nums`.  The files go into dst back to
+ * back from byte 0, each byte-identical to what pco_b200_compress_ex writes for its numbers alone with the same config and
+ * uniform_type_header; with a non-NULL `index`, each file's side index (as pco_b200_compress_ex writes it) goes into `index` at a
+ * 16-byte aligned offset (the offsets count from `index`, which itself may start at any byte).  files[i] reports both places; the
+ * output can be passed to pco_b200_decompress_files as it is.
+ * file_ns[i] == 0 gives an empty file (header + terminator); n_files == 0 is OK.  The call accepts exactly the files
+ * pco_b200_compress_ex accepts one at a time and refuses the others with the same kind; the message names the lowest refused file
+ * ("file 17: ...").  Files whose sizes imply different unoptimized_bins_log under ModeSpec / DeltaSpec Auto are fine (one pipeline
+ * pass per value).  PCO_B200_CHUNKS_ONLY is PCO_B200_INVALID_ARGUMENT.  A dst_cap or index_cap that is too small is PCO_B200_IO,
+ * with `files` still reporting the sizes needed. */
+PcoB200Error pco_b200_compress_files(const void *nums, const uint64_t *file_ns, size_t n_files, unsigned char dtype,
+                                     const PcoB200ChunkConfig *config, int uniform_type_header,
+                                     void *dst, size_t dst_cap, void *index, size_t index_cap,
+                                     PcoB200FileRef *files, uint32_t flags, void *cuda_stream);
+
+/* pco_b200_decompress_ex for n_files standalone files of one number type: file i's numbers land in dst right after file i - 1's, in
+ * `files` order; file_ns[i] = its count and *n_written = the total.  Each file's numbers equal what pco_b200_decompress_ex gives for
+ * it, with or without its index.  Files may come in any order and may repeat.  Files with a side index are decoded without a walk
+ * (their indexes are merged on the device into one chunk list); files without one are walked together, round by round; files the
+ * fast kernels decline (Dict, Lookback, Conv1, tables above 2^10 states or 256 bins, f16 FloatMult) go through the catch-all decoder.
+ * Refused before any device work: a file or index range outside its buffer, an index_offset that is not a multiple of 16, and
+ * files == NULL with n_files > 0 (PCO_B200_INVALID_ARGUMENT); an unknown dtype (PCO_B200_INVALID_TYPE).  A file that fails gives the
+ * kind pco_b200_decompress_ex gives for it, for the lowest failing file, and the message names it ("file 17: ...").  A dst_len below
+ * the total is PCO_B200_IO, naming the first file that does not fit.  Every record of a side index is checked against its own file
+ * before anything is decoded: a file whose records point outside its bytes, its index or its count is decoded on its own, exactly as
+ * pco_b200_decompress_ex decodes it, and cannot touch another file's output.  Two refusals go beyond pco_b200_decompress_ex, both as
+ * an index that does not belong to its file (PCO_B200_INVALID_ARGUMENT): batch entries at an offset that is not a multiple of 4, and a
+ * file of a format older than 4.x that only the catch-all decoder takes and that holds more numbers than its index counts. */
+PcoB200Error pco_b200_decompress_files(const void *src, size_t src_len, const void *index, size_t index_len,
+                                       unsigned char dtype, const PcoB200FileRef *files, size_t n_files,
+                                       void *dst, size_t dst_len, uint64_t *file_ns, size_t *n_written,
+                                       uint32_t flags, void *cuda_stream);
+
 #if defined(__cplusplus)
 }
 #endif

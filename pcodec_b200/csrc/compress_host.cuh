@@ -544,27 +544,33 @@ static PcoB200Error plan_front(CompressScratch& S, cudaStream_t stream, EncParam
     return PCO_B200_OK;
 }
 
-template <typename L>
-static PcoB200Error compress_typed(CompressScratch& S, const void* nums, size_t n, uint32_t dtype, const PcoB200ChunkConfig& cfg, bool uniform_type,
-                                   void* dst, size_t dst_cap, void* index_dst, size_t index_cap, uint32_t flags, cudaStream_t stream,
-                                   CompressResult* res) {
-  const bool src_dev = flags & PCO_B200_SRC_ON_DEVICE, dst_dev = flags & PCO_B200_DST_ON_DEVICE;
-  const uint32_t lbits = sizeof(L) * 8;
-  constexpr int LW = sizeof(L) == 1 ? 0 : sizeof(L) == 2 ? 1 : sizeof(L) == 4 ? 2 : 3;
+// What a ChunkConfig resolves to for an array of n numbers before any device work: the chunk sizes, the explicit mode and delta order, and
+// whether Auto searches run.  pco_b200_compress_files checks every file with it before the pipeline runs.
+struct ConfigCheck {
+  std::vector<uint64_t> pages;
+  ModeSel explicit_mode;
+  bool auto_mode = false, auto_delta = false;
+  uint32_t explicit_order = 0;
+};
+
+// config validation (pco/src/chunk_config.rs:269-314)
+inline PcoB200Error check_config(const PcoB200ChunkConfig& cfg, uint32_t dtype, size_t n, ConfigCheck* out) {
+  const uint32_t lbits = nt_bits(dtype);
   const bool is_float = nt_is_float(dtype);
-  // ---- config validation (pco/src/chunk_config.rs:269-314)
+  std::vector<uint64_t>& pages = out->pages;
+  ModeSel& explicit_mode = out->explicit_mode;
+  bool& auto_mode = out->auto_mode;
+  bool& auto_delta = out->auto_delta;
+  uint32_t& explicit_order = out->explicit_order;
   if (cfg.compression_level > 12) return fail(PCO_B200_INVALID_ARGUMENT, "compression level may not exceed 12");
   if (cfg.delta_spec == PCO_B200_DELTA_TRY_CONSECUTIVE && cfg.delta_order > 7)
     return fail(PCO_B200_INVALID_ARGUMENT, "consecutive delta order may not exceed 7");
   if (lbits == 8 && !cfg.enable_8_bit)
     return fail(PCO_B200_INVALID_ARGUMENT, "compressing 8-bit types with Pco is often a mistake; enable them on the ChunkConfig if you know what you're doing");
-  std::vector<uint64_t> pages;
   if (PcoB200Error e = n_per_page(cfg, n, &pages)) return e;
   for (uint64_t p : pages)
     if (p > (uint64_t(1) << 24)) return fail(PCO_B200_INVALID_ARGUMENT, "count may not exceed 16777216 per chunk");
-  // ---- the explicit mode, if any (Auto is resolved per chunk below)
-  ModeSel explicit_mode;
-  bool auto_mode = false;
+  // ---- the explicit mode, if any (Auto is resolved per chunk by compress_typed)
   switch (cfg.mode_spec) {
     case PCO_B200_MODE_CLASSIC: break;
     case PCO_B200_MODE_TRY_INT_MULT:
@@ -594,17 +600,32 @@ static PcoB200Error compress_typed(CompressScratch& S, const void* nums, size_t 
     case PCO_B200_MODE_AUTO: auto_mode = true; break;
     default: return fail(PCO_B200_UNSUPPORTED, "ModeSpec::TryDict is outside the GPU hot path");
   }
-  bool auto_delta = false;
-  uint32_t explicit_order = 0;
   switch (cfg.delta_spec) {
     case PCO_B200_DELTA_NOOP: break;
     case PCO_B200_DELTA_TRY_CONSECUTIVE: explicit_order = cfg.delta_order; break;
-    case PCO_B200_DELTA_AUTO: auto_delta = true; break;  // resolved per chunk below by the sampled search
+    case PCO_B200_DELTA_AUTO: auto_delta = true; break;  // resolved per chunk by compress_typed's sampled search
     case PCO_B200_DELTA_TRY_CONV1:
       if (cfg.delta_order == 0) break;
       return fail(PCO_B200_UNSUPPORTED, "DeltaSpec::TryConv1 is outside the GPU hot path");
     default: return fail(PCO_B200_UNSUPPORTED, "DeltaSpec::TryLookback is outside the GPU hot path");
   }
+  return PCO_B200_OK;
+}
+
+template <typename L>
+static PcoB200Error compress_typed(CompressScratch& S, const void* nums, size_t n, uint32_t dtype, const PcoB200ChunkConfig& cfg, bool uniform_type,
+                                   void* dst, size_t dst_cap, void* index_dst, size_t index_cap, uint32_t flags, cudaStream_t stream,
+                                   CompressResult* res) {
+  const bool src_dev = flags & PCO_B200_SRC_ON_DEVICE, dst_dev = flags & PCO_B200_DST_ON_DEVICE;
+  const uint32_t lbits = sizeof(L) * 8;
+  constexpr int LW = sizeof(L) == 1 ? 0 : sizeof(L) == 2 ? 1 : sizeof(L) == 4 ? 2 : 3;
+  const bool is_float = nt_is_float(dtype);
+  ConfigCheck checked;
+  if (PcoB200Error e = check_config(cfg, dtype, n, &checked)) return e;
+  const std::vector<uint64_t>& pages = checked.pages;
+  const ModeSel explicit_mode = checked.explicit_mode;
+  const bool auto_mode = checked.auto_mode, auto_delta = checked.auto_delta;
+  const uint32_t explicit_order = checked.explicit_order;
   const bool chunks_only = flags & PCO_B200_CHUNKS_ONLY;
   std::vector<uint8_t> header = make_standalone_header(n, uint8_t(uniform_type ? dtype : 0));
   if (chunks_only) header.clear();
@@ -933,6 +954,8 @@ static PcoB200Error compress_typed(CompressScratch& S, const void* nums, size_t 
     if (off > index_cap) return fail(PCO_B200_IO, "index buffer too small (need " + std::to_string(off) + " bytes)");
     index_total = off;
     PCOB_CUDA_TRY(S.idx_out.reserve(off + 64));  // assembled on the device run by run, one copy out
+    // the 16-byte padding behind a chunk's entries is written by no kernel: zero, so that the index is a function of the numbers
+    PCOB_CUDA_TRY(cudaMemsetAsync(S.idx_out.p, 0, off, stream));
   }
   uint64_t file_off = header.size();  // bytes of the file in front of the next run's first chunk
   uint8_t* d_out = static_cast<uint8_t*>(dst);

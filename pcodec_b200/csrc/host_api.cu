@@ -9,6 +9,7 @@
 #include "decode_fused.cuh"
 #include "gather_kernels.cuh"
 #include "decode_cold.cuh"
+#include "files_kernels.cuh"
 #include "host_common.hpp"
 #include "wrapped_kernels.cuh"
 
@@ -26,6 +27,7 @@ struct Context {
   std::string device_err;
   DevBuf src, out, index, statuses, misc, dec_syms, dec_offs, dec_narrow, gather, cold, spec;
   DevBuf wrap_metas, wrap_frames, wrap_tab, wrap_res, wrap_file, wrap_index, wrap_out;  // pco_b200_decompress_pages / pco_b200_compress_wrapped
+  DevBuf files_tab, files_res, files_out, files_idx, files_arena, files_cold;            // pco_b200_compress_files / pco_b200_decompress_files
   CompressScratch enc;
   Binoms* d_binoms = nullptr;
   int sm_count = 0;
@@ -45,7 +47,8 @@ static Context& ctx() {
 
 static void release_buffers(Context& c) {
   for (DevBuf* b : {&c.src, &c.out, &c.index, &c.statuses, &c.misc, &c.dec_syms, &c.dec_offs, &c.dec_narrow, &c.gather, &c.cold, &c.spec, &c.wrap_metas, &c.wrap_frames,
-                  &c.wrap_tab, &c.wrap_res, &c.wrap_file, &c.wrap_index, &c.wrap_out}) b->release();
+                  &c.wrap_tab, &c.wrap_res, &c.wrap_file, &c.wrap_index, &c.wrap_out, &c.files_tab, &c.files_res, &c.files_out, &c.files_idx,
+                  &c.files_arena, &c.files_cold}) b->release();
   c.enc.release();
   c.gather_err = nullptr;
   c.d_cls = nullptr;
@@ -1364,6 +1367,834 @@ PcoB200Error pco_b200_compress_wrapped(const void* nums, size_t n, unsigned char
                                        size_t* n_chunks, uint32_t flags, void* cuda_stream) {
   const PcoB200Error e = compress_wrapped_impl(nums, n, dtype, config, metas, metas_cap, metas_len, pages, pages_cap, pages_len, refs, refs_cap, n_chunks,
                                                flags, static_cast<cudaStream_t>(cuda_stream));
+  profiler().resolve();
+  return e;
+}
+
+// ---------------------------------------------------------------------------
+// Batches of standalone files (files_kernels.cuh).  Compress: the files' chunks run through the CHUNKS_ONLY pipeline as the chunks of
+// one call (Exact paging over every file's pages), then frame_files_kernel writes each file and its side index.  Under Auto the
+// pipeline takes one unoptimized_bins_log per call, so files are grouped by theirs and each group is one pass.
+// ---------------------------------------------------------------------------
+static PcoB200Error file_fail(PcoB200Error kind, size_t file, const std::string& what) {
+  return fail(kind, "file " + std::to_string(file) + ": " + what);
+}
+
+// Lowest file among [0, n_files) that pco_b200_compress_ex refuses on the device (the Auto searches' refusals), one file at a time.
+static PcoB200Error compress_files_find_refusal(Context& c, const void* nums, const uint64_t* file_ns, size_t n_files, uint32_t dtype,
+                                                const PcoB200ChunkConfig& cfg, bool uniform, uint32_t flags, cudaStream_t stream, size_t* refused) {
+  const size_t elem = nt_bits(dtype) / 8;
+  uint64_t at = 0;
+  for (size_t i = 0; i < n_files; i++) {
+    const size_t n = size_t(file_ns[i]);
+    std::vector<uint64_t> pages;
+    n_per_page(cfg, n, &pages);
+    size_t cap = 64, icap = pco_b200_index_size_bound(n, pages.size()) + 64 * pages.size();
+    for (uint64_t p : pages) cap += standalone_chunk_size_guarantee(nt_bits(dtype), size_t(p));
+    PCOB_CUDA_TRY(c.wrap_file.reserve(cap + 32));
+    PCOB_CUDA_TRY(c.wrap_index.reserve(icap));
+    CompressResult cr;
+    const PcoB200Error e = dispatch_latent(dtype, [&](auto tag) {
+      using L = decltype(tag);
+      return compress_typed<L>(c.enc, static_cast<const uint8_t*>(nums) + at * elem, n, dtype, cfg, uniform, c.wrap_file.p, cap, c.wrap_index.p, icap,
+                               (flags & PCO_B200_SRC_ON_DEVICE) | PCO_B200_CHUNKS_ONLY | PCO_B200_DST_ON_DEVICE | PCO_B200_INDEX_ON_DEVICE, stream, &cr);
+    });
+    if (e == PCO_B200_CUDA) return e;
+    if (e != PCO_B200_OK) { *refused = i; return e; }
+    at += n;
+  }
+  *refused = n_files;
+  return PCO_B200_OK;
+}
+
+static PcoB200Error compress_files_impl(const void* nums, const uint64_t* file_ns, size_t n_files, uint32_t dtype, const PcoB200ChunkConfig* config, bool uniform,
+                                        void* dst, size_t dst_cap, void* index, size_t index_cap, PcoB200FileRef* files, uint32_t flags, cudaStream_t stream) {
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (flags & PCO_B200_CHUNKS_ONLY) return fail(PCO_B200_INVALID_ARGUMENT, "PCO_B200_CHUNKS_ONLY does not apply to whole files");
+  if (n_files == 0) return PCO_B200_OK;
+  if (!file_ns || !files) return fail(PCO_B200_INVALID_ARGUMENT, "file_ns and files are required");
+  if ((!dst && dst_cap) || (!index && index_cap)) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  PcoB200ChunkConfig cfg;
+  if (config) cfg = *config;
+  else {
+    std::memset(&cfg, 0, sizeof(cfg));  // pco::ChunkConfig::default()
+    cfg.compression_level = 8;
+  }
+  // ---- every file's config check, on the host and in file order
+  const uint32_t lbits = nt_bits(dtype);
+  size_t first_bad = n_files;
+  PcoB200Error bad_kind = PCO_B200_OK;
+  std::string bad_msg;
+  bool auto_any = false;
+  std::vector<std::vector<uint64_t>> pages(n_files);
+  std::vector<uint32_t> bins(n_files, 0);
+  for (size_t i = 0; i < n_files; i++) {
+    ConfigCheck ck;
+    PcoB200Error e = check_config(cfg, dtype, size_t(file_ns[i]), &ck);
+    if (e == PCO_B200_OK && !ck.pages.empty()) {
+      bins[i] = choose_unoptimized_bins_log(cfg.compression_level, size_t(ck.pages[0]));
+      bool uniform_bins = true;
+      for (uint64_t p : ck.pages) uniform_bins = uniform_bins && choose_unoptimized_bins_log(cfg.compression_level, size_t(p)) == bins[i];
+      if (!uniform_bins && (ck.auto_mode || ck.auto_delta))  // compress_typed's refusal for one array
+        e = fail(PCO_B200_UNSUPPORTED, "ModeSpec::Auto / DeltaSpec::Auto over chunks whose sizes imply different unoptimized_bins_log in one call");
+    }
+    if (e != PCO_B200_OK) {
+      first_bad = i;
+      bad_kind = e;
+      bad_msg = last_error_ref();
+      break;
+    }
+    auto_any = ck.auto_mode || ck.auto_delta;
+    pages[i] = std::move(ck.pages);
+  }
+  // explicit specs: the pipeline refuses nothing the checks passed, so a refusal is final here; under Auto a file in front of it may
+  // still be refused by the device searches
+  if (first_bad == 0 || (first_bad < n_files && !auto_any)) return file_fail(bad_kind, first_bad, bad_msg);
+
+  Context& c = ctx();
+  if (PcoB200Error e = ensure_device(c)) return e;
+  const bool src_dev = flags & PCO_B200_SRC_ON_DEVICE, dst_dev = flags & PCO_B200_DST_ON_DEVICE, idx_dev = flags & PCO_B200_INDEX_ON_DEVICE;
+  const size_t elem = lbits / 8;
+  std::vector<uint64_t> num_at(first_bad + 1, 0);
+  for (size_t i = 0; i < first_bad; i++) num_at[i + 1] = num_at[i] + file_ns[i];
+  // ---- groups: one pipeline pass per unoptimized_bins_log.  Auto needs it; explicit specs gain from it: the pipeline splits a pass into
+  // runs wherever consecutive chunks change the value, and every run waits for the host, so files of mixed sizes in file order would
+  // make hundreds of runs.
+  std::map<uint32_t, std::vector<uint32_t>> groups;
+  for (size_t i = 0; i < first_bad; i++)
+    if (file_ns[i] > 0) groups[bins[i]].push_back(uint32_t(i));
+  struct Group { uint64_t out_at, out_cap, idx_at, idx_cap, total, index_bytes; std::vector<IndexChunk> recs; };
+  std::vector<Group> gs;
+  std::vector<uint32_t> file_group(first_bad, 0), file_c0(first_bad, 0);
+  uint64_t out_scratch = 0, idx_scratch = 0;
+  for (auto& kv : groups) {
+    Group g{};
+    uint64_t cap = 64, nc = 0, n = 0;
+    for (uint32_t f : kv.second) {
+      file_group[f] = uint32_t(gs.size());
+      file_c0[f] = uint32_t(nc);
+      for (uint64_t p : pages[f]) cap += standalone_chunk_size_guarantee(lbits, size_t(p));
+      nc += pages[f].size();
+      n += file_ns[f];
+    }
+    g.out_at = out_scratch;
+    g.out_cap = cap;
+    g.idx_at = idx_scratch;
+    g.idx_cap = pco_b200_index_size_bound(size_t(n), size_t(nc)) + 64 * nc;
+    out_scratch += (cap + 15) & ~uint64_t(15);
+    idx_scratch += (g.idx_cap + 15) & ~uint64_t(15);
+    gs.push_back(std::move(g));
+  }
+  PCOB_CUDA_TRY(c.wrap_file.reserve(out_scratch + 64));
+  PCOB_CUDA_TRY(c.wrap_index.reserve(idx_scratch + 64));
+  uint8_t* d_chunks = c.wrap_file.as<uint8_t>();
+  uint8_t* d_pidx = c.wrap_index.as<uint8_t>();
+  size_t gi = 0;
+  for (auto& kv : groups) {
+    Group& g = gs[gi++];
+    const std::vector<uint32_t>& fl = kv.second;
+    std::vector<uint64_t> exact;
+    for (uint32_t f : fl) exact.insert(exact.end(), pages[f].begin(), pages[f].end());
+    PcoB200ChunkConfig cg = cfg;
+    cg.paging_spec = PCO_B200_PAGING_EXACT;
+    cg.exact_page_ns = exact.data();
+    cg.n_exact_pages = exact.size();
+    // the group's numbers back to back: the array itself when the files of the group are consecutive, else gathered
+    const uint8_t* g_nums = static_cast<const uint8_t*>(nums) + num_at[fl.front()] * elem;
+    uint64_t g_n = 0;
+    for (uint32_t f : fl) g_n += file_ns[f];
+    std::vector<uint8_t> h_gather;
+    if (num_at[fl.back() + 1] - num_at[fl.front()] != g_n) {
+      if (src_dev) {
+        PCOB_CUDA_TRY(c.wrap_out.reserve(g_n * elem + 64));
+        uint64_t at = 0;
+        for (uint32_t f : fl) {
+          PCOB_CUDA_TRY(cudaMemcpyAsync(c.wrap_out.as<uint8_t>() + at * elem, static_cast<const uint8_t*>(nums) + num_at[f] * elem, file_ns[f] * elem,
+                                        cudaMemcpyDeviceToDevice, stream));
+          at += file_ns[f];
+        }
+        g_nums = c.wrap_out.as<uint8_t>();
+      } else {
+        h_gather.resize(g_n * elem);
+        uint64_t at = 0;
+        for (uint32_t f : fl) {
+          std::memcpy(h_gather.data() + at * elem, static_cast<const uint8_t*>(nums) + num_at[f] * elem, file_ns[f] * elem);
+          at += file_ns[f];
+        }
+        g_nums = h_gather.data();
+      }
+    }
+    CompressResult cr;
+    const PcoB200Error e = dispatch_latent(dtype, [&](auto tag) {
+      using L = decltype(tag);
+      return compress_typed<L>(c.enc, g_nums, size_t(g_n), dtype, cg, uniform, d_chunks + g.out_at, g.out_cap, d_pidx + g.idx_at, g.idx_cap,
+                               (src_dev ? PCO_B200_SRC_ON_DEVICE : 0u) | PCO_B200_CHUNKS_ONLY | PCO_B200_DST_ON_DEVICE | PCO_B200_INDEX_ON_DEVICE, stream, &cr);
+    });
+    if (e == PCO_B200_CUDA) return e;
+    if (e != PCO_B200_OK) {  // an Auto search refused a chunk: find the lowest file compress_ex refuses
+      size_t refused = first_bad;
+      const PcoB200Error e2 = compress_files_find_refusal(c, nums, file_ns, first_bad, dtype, cfg, uniform, flags, stream, &refused);
+      if (refused < first_bad) return file_fail(e2, refused, last_error_ref());
+      if (e2 != PCO_B200_OK) return e2;
+      if (first_bad < n_files) return file_fail(bad_kind, first_bad, bad_msg);
+      return fail(PCO_B200_CUDA, "a batch was refused that no file of it is refused alone");
+    }
+    g.total = cr.total_bytes;
+    g.index_bytes = cr.index_bytes;
+    g.recs.resize(exact.size());
+    PCOB_CUDA_TRY(cudaMemcpyAsync(g.recs.data(), d_pidx + g.idx_at + sizeof(IndexHeader), exact.size() * sizeof(IndexChunk), cudaMemcpyDeviceToHost, stream));
+    PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
+  }
+  if (first_bad < n_files) return file_fail(bad_kind, first_bad, bad_msg);
+
+  // ---- the files' layout in dst and index
+  std::vector<FileFrame> tab(n_files);
+  uint64_t dst_total = 0, idx_total = 0;
+  for (size_t i = 0; i < n_files; i++) {
+    FileFrame& f = tab[i];
+    std::memset(&f, 0, sizeof(f));
+    const std::vector<uint8_t> hdr = make_standalone_header(file_ns[i], uint8_t(uniform ? dtype : 0));
+    f.hdr_len = uint32_t(hdr.size());
+    std::memcpy(f.hdr, hdr.data(), hdr.size());
+    f.n = file_ns[i];
+    f.n_chunks = uint32_t(pages[i].size());
+    if (f.n_chunks) {
+      const Group& g = gs[file_group[i]];
+      const uint32_t c0 = file_c0[i], c1 = c0 + f.n_chunks;
+      const uint64_t end = c1 < g.recs.size() ? g.recs[c1].chunk_offset : g.total;
+      const uint64_t eend = c1 < g.recs.size() ? g.recs[c1].entries_offset : g.index_bytes;
+      f.chunks_src = g.out_at + g.recs[c0].chunk_offset;
+      f.chunks_len = end - g.recs[c0].chunk_offset;
+      f.recs_src = g.idx_at + sizeof(IndexHeader) + uint64_t(c0) * sizeof(IndexChunk);
+      f.entries_src = g.idx_at + g.recs[c0].entries_offset;
+      f.entries_len = eend - g.recs[c0].entries_offset;
+    }
+    f.dst_off = dst_total;
+    f.index_off = idx_total;
+    const uint64_t flen = f.hdr_len + f.chunks_len + 1;
+    const uint64_t ilen = sizeof(IndexHeader) + uint64_t(f.n_chunks) * sizeof(IndexChunk) + f.entries_len;
+    files[i].offset = dst_total;
+    files[i].len = flen;
+    files[i].index_offset = index ? idx_total : 0;
+    files[i].index_len = index ? ilen : 0;
+    dst_total += flen;
+    if (index) idx_total += (ilen + 15) & ~uint64_t(15);
+  }
+  if (dst_total > dst_cap || (index && idx_total > index_cap))
+    return fail(PCO_B200_IO, "failed to write whole buffer (need " + std::to_string(dst_total) + " file bytes and " + std::to_string(idx_total) + " index bytes)");
+
+  // ---- framing: the files straight into a device dst (byte-granular stores, any alignment) or into scratch for a host one; the
+  // indexes always into scratch, whose base is aligned for the kernel's 8-byte record stores, then one copy into the caller's buffer,
+  // which may start at any byte (as compress_ex's index may)
+  PCOB_CUDA_TRY(c.files_tab.reserve(n_files * sizeof(FileFrame)));
+  PCOB_CUDA_TRY(cudaMemcpyAsync(c.files_tab.p, tab.data(), n_files * sizeof(FileFrame), cudaMemcpyHostToDevice, stream));
+  uint8_t* d_dst = static_cast<uint8_t*>(dst);
+  uint8_t* d_index = nullptr;
+  if (!dst_dev) {
+    PCOB_CUDA_TRY(c.files_out.reserve(dst_total + 64));
+    d_dst = c.files_out.as<uint8_t>();
+  }
+  if (index) {
+    PCOB_CUDA_TRY(c.files_idx.reserve(idx_total + 64));
+    d_index = c.files_idx.as<uint8_t>();
+  }
+  profiler().begin("frame_files_kernel", stream);
+  frame_files_kernel<<<uint32_t(n_files), FILES_THREADS, 0, stream>>>(d_chunks, d_pidx, c.files_tab.as<FileFrame>(), d_dst, d_index);
+  profiler().end(stream);
+  PCOB_CUDA_TRY(cudaGetLastError());
+  if (!dst_dev) PCOB_CUDA_TRY(copy_sliced(dst, d_dst, dst_total, cudaMemcpyDeviceToHost, stream));
+  if (index) PCOB_CUDA_TRY(copy_sliced(index, d_index, idx_total, idx_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, stream));
+  PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
+  return PCO_B200_OK;
+}
+
+PcoB200Error pco_b200_compress_files(const void* nums, const uint64_t* file_ns, size_t n_files, unsigned char dtype, const PcoB200ChunkConfig* config,
+                                     int uniform_type_header, void* dst, size_t dst_cap, void* index, size_t index_cap, PcoB200FileRef* files, uint32_t flags,
+                                     void* cuda_stream) {
+  const PcoB200Error e = compress_files_impl(nums, file_ns, n_files, dtype, config, uniform_type_header != 0, dst, dst_cap, index, index_cap, files, flags,
+                                             static_cast<cudaStream_t>(cuda_stream));
+  profiler().resolve();
+  return e;
+}
+
+// Decompress.  Every file's count is known before anything is decoded - from its side index, or from walking it - so the numbers land
+// in place and the whole batch is ONE chunk list for the ordinary decode kernels (one launch_decode per header flavour and format
+// version, which FileParams carries per launch):
+//   1. the files' heads (and index headers) come back in one readback and are parsed on the host;
+//   2. index-free files are walked together: each round peeks every unfinished file's next 4 bytes, finds every file's candidate
+//      chunk starts in one find_file_starts_kernel launch, walks all candidates in one walk_kernel launch and follows each file's
+//      chain on the host (speculative_walk_rounds, for many files).  The walked records stay in an arena beside the staged indexes;
+//   3. a file whose next byte is then its terminator is done; any other (a chunk of odd size, corruption, truncation, an older
+//      format, a cold chunk) finishes on the serial walker, one file at a time, with the single-file semantics;
+//   4. check_index_kernel tests every indexed file's records against its own file (a file that fails decodes on its own, through
+//      decompress_core) and marks cold files; then
+//      merge_index_kernel writes the indexed files' records, rebased, into the list beside the walked ones; launch_decode runs over
+//      it.  A failing chunk names its file: a chunk the fast kernels decline makes that file cold and the list is decoded again
+//      without it; any other failure drops the files from it on and the rest is decoded again, so that the lowest failure is found;
+//   5. cold files go through cold_decode_kernel, one launch per file.
+struct BatchFile {
+  StandaloneHeader hdr;
+  bool indexed = false, walk = false, done = false, cold = false, staged = false;
+  bool alone = false;            // indexed, with a record outside its own file: decoded by itself, as decompress_ex decodes it
+  uint64_t count = 0;            // numbers: from the index, or walked so far
+  uint64_t begin = 0, end = 0;   // the file's bytes in src
+  uint64_t pos = 0;              // walk cursor (byte in src)
+  uint64_t idx_recs = 0;         // indexed: byte offset of its IndexChunk[0] in the arena
+  uint64_t idx_base = 0;         // indexed: byte offset of its index in the arena
+  uint64_t n_idx_chunks = 0;
+  std::vector<IndexChunk> recs;  // walked: chunk_offset in src, entries_offset in the arena, out_offset from the file's first number
+  uint64_t out_base = 0;
+  uint64_t staged_at = 0;        // cold without index: element offset of its numbers in files_cold
+};
+
+static PcoB200Error decompress_files_impl(const void* src, size_t src_len, const void* index, size_t index_len, uint32_t dtype, const PcoB200FileRef* files,
+                                          size_t n_files, void* dst, size_t dst_len, uint64_t* file_ns, size_t* n_written, uint32_t flags,
+                                          cudaStream_t stream) {
+  // ---- argument checks: host only, before any device work
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (n_written) *n_written = 0;
+  if (n_files == 0) return PCO_B200_OK;
+  if (!files) return fail(PCO_B200_INVALID_ARGUMENT, "files are required");
+  if (n_files > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "too many files");
+  if ((!src && src_len) || (!index && index_len) || (!dst && dst_len)) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  bool any_index = false;
+  for (size_t i = 0; i < n_files; i++) {
+    const PcoB200FileRef& r = files[i];
+    if (r.len > src_len || r.offset > src_len - r.len) return file_fail(PCO_B200_INVALID_ARGUMENT, i, "file lies outside src");
+    if (r.index_len) {
+      if (r.index_offset % 16) return file_fail(PCO_B200_INVALID_ARGUMENT, i, "index offset is not a multiple of 16");
+      if (r.index_len > index_len || r.index_offset > index_len - r.index_len) return file_fail(PCO_B200_INVALID_ARGUMENT, i, "side index lies outside index");
+      any_index = any_index || r.index_len >= sizeof(IndexHeader);
+    }
+  }
+  Context& c = ctx();
+  if (PcoB200Error e = ensure_device(c)) return e;
+  static const bool cold_ok = [] { const char* v = std::getenv("PCOB200_COLD_DECODE"); return !(v && v[0] == '0'); }();
+  const bool spec_ok = [] { const char* v = std::getenv("PCOB200_SPECULATIVE_WALK"); return !(v && v[0] == '0'); }();
+  const bool src_dev = flags & PCO_B200_SRC_ON_DEVICE, dst_dev = flags & PCO_B200_DST_ON_DEVICE, idx_dev = flags & PCO_B200_INDEX_ON_DEVICE;
+  const size_t elem = nt_bits(dtype) / 8;
+  const uint32_t n = uint32_t(n_files);
+  // the lowest failing file so far: files from it on need no work
+  size_t limit = n_files;
+  PcoB200Error fkind = PCO_B200_OK;
+  std::string fmsg;
+  auto fail_at = [&](size_t i, PcoB200Error k, const std::string& m) {
+    if (i < limit) { limit = i; fkind = k; fmsg = m; }
+  };
+
+  // ---- the bytes in HBM: src, and the arena = [the caller's index | walked records and entries | the merged chunk list]
+  const uint8_t* d_src = static_cast<const uint8_t*>(src);
+  if (!src_dev) {
+    PCOB_CUDA_TRY(c.src.reserve(src_len + 16));
+    if (src_len) PCOB_CUDA_TRY(copy_sliced(c.src.p, src, src_len, cudaMemcpyHostToDevice, stream));
+    d_src = c.src.as<uint8_t>();
+  }
+  uint64_t arena_end = any_index ? (uint64_t(index_len) + 15) & ~uint64_t(15) : 0;
+  PCOB_CUDA_TRY(c.files_arena.reserve(arena_end + 64));
+  if (any_index) PCOB_CUDA_TRY(copy_sliced(c.files_arena.p, index, index_len, idx_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, stream));
+  auto arena = [&]() { return c.files_arena.as<uint8_t>(); };
+  // bytes at many positions of a device buffer, in one readback
+  auto peek = [&](const uint8_t* d_base, const std::vector<uint64_t>& offs, const std::vector<uint64_t>& lens, uint32_t width, std::vector<uint8_t>* out) -> PcoB200Error {
+    const size_t m = offs.size();
+    out->assign(m * width, 0);
+    if (m == 0) return PCO_B200_OK;
+    PCOB_CUDA_TRY(c.files_tab.reserve(m * 16 + 64));
+    PCOB_CUDA_TRY(c.files_res.reserve(m * width + 64));
+    uint64_t* d_offs = c.files_tab.as<uint64_t>();
+    PCOB_CUDA_TRY(cudaMemcpyAsync(d_offs, offs.data(), m * 8, cudaMemcpyHostToDevice, stream));
+    PCOB_CUDA_TRY(cudaMemcpyAsync(d_offs + m, lens.data(), m * 8, cudaMemcpyHostToDevice, stream));
+    peek_bytes_kernel<<<uint32_t((m + 7) / 8), 256, 0, stream>>>(d_base, d_offs, d_offs + m, uint32_t(m), width, c.files_res.as<uint8_t>());
+    PCOB_CUDA_TRY(cudaGetLastError());
+    PCOB_CUDA_TRY(readback_small_sync(out->data(), c.files_res.p, (m * width + 3) & ~size_t(3), stream));
+    return PCO_B200_OK;
+  };
+  auto peek_src = [&](const std::vector<uint64_t>& offs, const std::vector<uint64_t>& lens, uint32_t width, std::vector<uint8_t>* out) -> PcoB200Error {
+    if (src_dev) return peek(d_src, offs, lens, width, out);
+    out->assign(offs.size() * width, 0);
+    for (size_t k = 0; k < offs.size(); k++) std::memcpy(out->data() + k * width, static_cast<const uint8_t*>(src) + offs[k], std::min<uint64_t>(lens[k], width));
+    return PCO_B200_OK;
+  };
+
+  // ---- 1. heads and index headers
+  std::vector<BatchFile> bf(n_files);
+  {
+    std::vector<uint64_t> offs(n), lens(n), ioffs, ilens;
+    std::vector<uint32_t> with_index;
+    for (uint32_t i = 0; i < n; i++) {
+      offs[i] = files[i].offset;
+      lens[i] = std::min<uint64_t>(files[i].len, 32);
+      if (files[i].index_len >= sizeof(IndexHeader)) {
+        with_index.push_back(i);
+        ioffs.push_back(files[i].index_offset);
+        ilens.push_back(sizeof(IndexHeader));
+      }
+    }
+    std::vector<uint8_t> heads, iheads;
+    if (PcoB200Error e = peek_src(offs, lens, 32, &heads)) return e;
+    if (idx_dev) {
+      if (PcoB200Error e = peek(arena(), ioffs, ilens, sizeof(IndexHeader), &iheads)) return e;
+    } else {
+      iheads.assign(ioffs.size() * sizeof(IndexHeader), 0);
+      for (size_t k = 0; k < ioffs.size(); k++) std::memcpy(iheads.data() + k * sizeof(IndexHeader), static_cast<const uint8_t*>(index) + ioffs[k], sizeof(IndexHeader));
+    }
+    size_t wi = 0;
+    for (uint32_t i = 0; i < n; i++) {
+      BatchFile& f = bf[i];
+      const PcoB200FileRef& r = files[i];
+      f.begin = r.offset;
+      f.end = r.offset + r.len;
+      if (PcoB200Error e = parse_standalone_header(heads.data() + size_t(i) * 32, size_t(lens[i]), size_t(r.len), &f.hdr)) {
+        fail_at(i, e, last_error_ref());
+        break;
+      }
+      if (wi < with_index.size() && with_index[wi] == i) {
+        IndexHeader ih;
+        std::memcpy(&ih, iheads.data() + wi * sizeof(IndexHeader), sizeof(ih));
+        wi++;
+        // as decompress_ex checks it; the chunk table must also be 8-byte aligned for the kernels' loads
+        if (ih.magic != INDEX_MAGIC || ih.version != 1 || ih.file_len != r.len || ih.chunks_offset > r.index_len || ih.chunks_offset % 8 != 0 ||
+            ih.n_chunks > (r.index_len - ih.chunks_offset) / sizeof(IndexChunk)) {
+          fail_at(i, PCO_B200_INVALID_ARGUMENT, "side index does not belong to this file");
+          break;
+        }
+        f.indexed = true;
+        f.count = ih.n_total;
+        f.n_idx_chunks = ih.n_chunks;
+        f.idx_base = r.index_offset;
+        f.idx_recs = r.index_offset + ih.chunks_offset;
+      } else {
+        f.walk = true;
+        f.pos = r.offset + f.hdr.first_chunk_byte;
+      }
+    }
+  }
+
+  // ---- 2. index-free files: speculative rounds over all of them at once
+  constexpr uint32_t CAND_CAP = 1u << 22;                  // candidates listed per round, all files together
+  constexpr uint32_t FILE_CAND_CAP = 1u << 16;             // a file with more is not worth speculating on (as for one file)
+  constexpr uint64_t INDEX_BUDGET = uint64_t(768) << 20;   // bytes of walked records and entries per round
+  std::vector<uint8_t> tail(n_files, 0);                   // 1: this file finishes on the serial walker
+  for (uint32_t i = 0; i < n; i++)
+    if (bf[i].walk && (!spec_ok || (bf[i].hdr.uniform_type != 0 && bf[i].hdr.uniform_type != dtype))) tail[i] = 1;  // the latter: no chunk can pass
+  for (int round = 0; round < 4096; round++) {
+    std::vector<uint32_t> act;
+    std::vector<uint64_t> offs, lens;
+    for (uint32_t i = 0; i < n && i < limit; i++)
+      if (bf[i].walk && !bf[i].done && !tail[i]) {
+        if (bf[i].pos + 4 > bf[i].end) { tail[i] = 1; continue; }
+        act.push_back(i);
+        offs.push_back(bf[i].pos);
+        lens.push_back(4);
+      }
+    if (act.empty()) break;
+    std::vector<uint8_t> h4;
+    if (PcoB200Error e = peek_src(offs, lens, 4, &h4)) return e;
+    std::vector<FileScan> scans;
+    std::vector<uint32_t> scan_file;
+    uint64_t blocks = 0;
+    const uint64_t per_block = uint64_t(FIND_THREADS) * FIND_PER_THREAD;
+    for (size_t k = 0; k < act.size(); k++) {
+      const uint32_t i = act[k];
+      const uint8_t* b = h4.data() + k * 4;
+      if (b[0] != dtype) { tail[i] = 1; continue; }  // the terminator, or a type byte the serial walker reports
+      FileScan s;
+      s.begin = bf[i].pos;
+      s.end = bf[i].end - 3;
+      s.pattern = uint32_t(b[0]) | (uint32_t(b[1]) << 8) | (uint32_t(b[2]) << 16) | (uint32_t(b[3]) << 24);
+      s.block0 = uint32_t(blocks);
+      blocks += (s.end - s.begin + per_block - 1) / per_block;
+      scans.push_back(s);
+      scan_file.push_back(i);
+    }
+    if (scans.empty()) break;
+    if (blocks > 0x7fffffffull) { for (uint32_t i : scan_file) tail[i] = 1; break; }
+    // scratch: count | candidate positions | their files | statuses | chunk ends
+    PCOB_CUDA_TRY(c.spec.reserve(64 + size_t(CAND_CAP) * (8 + 4)));
+    PCOB_CUDA_TRY(c.files_tab.reserve(scans.size() * sizeof(FileScan) + 64));
+    uint32_t* d_count = c.spec.as<uint32_t>();
+    uint64_t* d_cand = reinterpret_cast<uint64_t*>(c.spec.as<uint8_t>() + 64);
+    uint32_t* d_cfile = reinterpret_cast<uint32_t*>(d_cand + CAND_CAP);
+    PCOB_CUDA_TRY(cudaMemcpyAsync(c.files_tab.p, scans.data(), scans.size() * sizeof(FileScan), cudaMemcpyHostToDevice, stream));
+    PCOB_CUDA_TRY(cudaMemsetAsync(d_count, 0, 4, stream));
+    profiler().begin("find_file_starts_kernel", stream);
+    find_file_starts_kernel<<<uint32_t(blocks), FIND_THREADS, 0, stream>>>(d_src, c.files_tab.as<FileScan>(), uint32_t(scans.size()), d_cand, d_cfile, CAND_CAP, d_count);
+    profiler().end(stream);
+    PCOB_CUDA_TRY(cudaGetLastError());
+    uint32_t count = 0;
+    PCOB_CUDA_TRY(readback_small_sync(&count, d_count, 4, stream));
+    if (count > CAND_CAP) { for (uint32_t i : scan_file) tail[i] = 1; break; }
+    std::vector<uint64_t> cpos(count);
+    std::vector<uint32_t> cfile(count);
+    PCOB_CUDA_TRY(cudaMemcpyAsync(cpos.data(), d_cand, size_t(count) * 8, cudaMemcpyDeviceToHost, stream));
+    PCOB_CUDA_TRY(cudaMemcpyAsync(cfile.data(), d_cfile, size_t(count) * 4, cudaMemcpyDeviceToHost, stream));
+    PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
+    std::vector<std::vector<uint64_t>> cand(scans.size());
+    for (uint32_t k = 0; k < count; k++) cand[cfile[k]].push_back(cpos[k]);
+    // the round's walk: every file's candidates (as many as its budget share allows), one CTA each.  FileParams carries one uniform type
+    // and format version per launch, so the records are laid out flavour by flavour and each flavour present is one launch.
+    auto flavour = [&](uint32_t i) { return (bf[i].hdr.uniform_type << 8) | bf[i].hdr.format_major; };
+    std::vector<uint32_t> scan_order(scans.size());
+    for (size_t s = 0; s < scans.size(); s++) scan_order[s] = uint32_t(s);
+    std::stable_sort(scan_order.begin(), scan_order.end(), [&](uint32_t a, uint32_t b) { return flavour(scan_file[a]) < flavour(scan_file[b]); });
+    std::vector<IndexChunk> recs;
+    std::vector<uint32_t> walked;           // scan index of each file walked this round
+    std::vector<size_t> first_rec;          // its first record
+    uint64_t budget = INDEX_BUDGET;
+    const uint64_t chunks_at = (arena_end + 15) & ~uint64_t(15);
+    std::vector<uint64_t> strides;
+    for (uint32_t s : scan_order) {
+      const uint32_t i = scan_file[s];
+      std::vector<uint64_t>& cs = cand[s];
+      std::sort(cs.begin(), cs.end());
+      if (cs.empty() || cs.size() > FILE_CAND_CAP || cs[0] != bf[i].pos) { tail[i] = 1; continue; }
+      const uint32_t n0 = ((scans[s].pattern >> 8) & 0xffffffu) + 1;
+      const uint64_t stride = (uint64_t(MAX_VARS) * n_batches_of(n0) * sizeof(BatchEntry) + 15) & ~uint64_t(15);
+      uint64_t m = std::min<uint64_t>(cs.size(), std::max<uint64_t>(1, INDEX_BUDGET / (stride + sizeof(IndexChunk))));
+      if (!walked.empty() && m * (stride + sizeof(IndexChunk)) > budget) continue;  // waits for the next round
+      budget -= std::min(budget, m * (stride + sizeof(IndexChunk)));
+      cs.resize(m);
+      walked.push_back(uint32_t(s));
+      first_rec.push_back(recs.size());
+      strides.push_back(stride);
+      for (uint64_t k = 0; k < m; k++) {
+        IndexChunk ic;
+        ic.chunk_offset = cs[k];
+        ic.n = n0;
+        ic.n_vars = 0;
+        ic.entries_offset = 0;  // below
+        ic.out_offset = 0;
+        recs.push_back(ic);
+      }
+    }
+    if (recs.empty()) break;
+    const uint32_t mt = uint32_t(recs.size());
+    uint64_t e_at = (chunks_at + uint64_t(mt) * sizeof(IndexChunk) + 15) & ~uint64_t(15);
+    for (size_t w = 0; w < walked.size(); w++) {
+      const size_t r1 = w + 1 < walked.size() ? first_rec[w + 1] : recs.size();
+      for (size_t r = first_rec[w]; r < r1; r++) { recs[r].entries_offset = e_at; e_at += strides[w]; }
+    }
+    PCOB_CUDA_TRY(c.files_arena.grow_preserve(e_at + 64, arena_end, stream));
+    PCOB_CUDA_TRY(c.spec.reserve(64 + size_t(CAND_CAP) * (8 + 4) + size_t(mt) * (4 + 8) + 64));
+    uint32_t* d_stat = reinterpret_cast<uint32_t*>(c.spec.as<uint8_t>() + 64 + size_t(CAND_CAP) * 12);
+    uint64_t* d_ends = reinterpret_cast<uint64_t*>(c.spec.as<uint8_t>() + 64 + size_t(CAND_CAP) * 12 + ((size_t(mt) * 4 + 15) & ~size_t(15)));
+    PCOB_CUDA_TRY(cudaMemcpyAsync(arena() + chunks_at, recs.data(), size_t(mt) * sizeof(IndexChunk), cudaMemcpyHostToDevice, stream));
+    PCOB_CUDA_TRY(cudaMemsetAsync(d_stat, 0xff, size_t(mt) * 4, stream));
+    PCOB_CUDA_TRY(cudaMemsetAsync(d_ends, 0, size_t(mt) * 8, stream));
+    PCOB_CUDA_TRY(c.misc.reserve(sizeof(WalkResult)));
+    for (size_t w0 = 0; w0 < walked.size();) {  // one launch per flavour: its walked files' records are consecutive
+      const uint32_t fl = flavour(scan_file[walked[w0]]);
+      size_t w1 = w0 + 1;
+      while (w1 < walked.size() && flavour(scan_file[walked[w1]]) == fl) w1++;
+      const size_t r_lo = first_rec[w0], r_hi = w1 < walked.size() ? first_rec[w1] : recs.size();
+      const FileParams fp{d_src, src_len, dtype, fl >> 8, fl & 0xff};
+      profiler().begin("walk_kernel", stream);
+      walk_kernel<SMALL_MAX_SIZE_LOG><<<uint32_t(r_hi - r_lo), WALK_THREADS, sizeof(WalkSmem<SMALL_MAX_SIZE_LOG>), stream>>>(
+          fp, arena(), chunks_at + r_lo * sizeof(IndexChunk), uint32_t(r_hi - r_lo), 0, e_at, 0, 0, ~uint64_t(0), d_stat + r_lo, c.misc.as<WalkResult>(), 0,
+          d_ends + r_lo);
+      profiler().end(stream);
+      PCOB_CUDA_TRY(cudaGetLastError());
+      w0 = w1;
+    }
+    std::vector<uint32_t> st(mt);
+    std::vector<uint64_t> ends(mt);
+    PCOB_CUDA_TRY(cudaMemcpyAsync(st.data(), d_stat, size_t(mt) * 4, cudaMemcpyDeviceToHost, stream));
+    PCOB_CUDA_TRY(cudaMemcpyAsync(ends.data(), d_ends, size_t(mt) * 8, cudaMemcpyDeviceToHost, stream));
+    PCOB_CUDA_TRY(cudaMemcpyAsync(recs.data(), arena() + chunks_at, size_t(mt) * sizeof(IndexChunk), cudaMemcpyDeviceToHost, stream));  // n_vars as walked
+    PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
+    bool progress = false;
+    for (size_t w = 0; w < walked.size(); w++) {
+      const uint32_t s = walked[w], i = scan_file[s];
+      BatchFile& f = bf[i];
+      const size_t r0 = first_rec[w];
+      const uint32_t m = uint32_t(cand[s].size());
+      const uint32_t n0 = recs[r0].n;
+      uint64_t p = f.pos;
+      const std::vector<uint32_t> chain = follow_chunk_chain(cand[s].data(), st.data() + r0, ends.data() + r0, m, f.pos, n0, 0, ~uint64_t(0), f.end, &p);
+      if (chain.empty()) { tail[i] = 1; continue; }
+      for (uint32_t k : chain) {
+        IndexChunk ic = recs[r0 + k];
+        ic.out_offset = f.count;
+        f.count += n0;
+        f.recs.push_back(ic);
+      }
+      f.pos = p;
+      progress = true;
+    }
+    arena_end = e_at;
+    if (!progress) break;
+  }
+
+  // ---- 3. the terminator, or the serial walker
+  {
+    std::vector<uint32_t> ends_at;
+    std::vector<uint64_t> offs, lens;
+    for (uint32_t i = 0; i < n && i < limit; i++)
+      if (bf[i].walk && bf[i].pos < bf[i].end) {
+        ends_at.push_back(i);
+        offs.push_back(bf[i].pos);
+        lens.push_back(1);
+      }
+    std::vector<uint8_t> b;
+    if (PcoB200Error e = peek_src(offs, lens, 4, &b)) return e;
+    for (size_t k = 0; k < ends_at.size(); k++)
+      if (b[k * 4] == 0) bf[ends_at[k]].done = true;
+  }
+  PCOB_CUDA_TRY(c.misc.reserve(sizeof(WalkResult)));
+  for (uint32_t i = 0; i < n && i < limit; i++) {
+    BatchFile& f = bf[i];
+    if (!f.walk || f.done) continue;
+    const FileParams fpf{d_src + f.begin, f.end - f.begin, dtype, f.hdr.uniform_type, f.hdr.format_major};
+    const uint64_t len = f.end - f.begin;
+    const uint32_t max_chunks = uint32_t(std::min<uint64_t>(len / 5 + 2, 1u << 16));
+    uint64_t next = f.pos - f.begin;
+    for (;;) {
+      const uint64_t chunks_at = (arena_end + 15) & ~uint64_t(15);
+      const uint64_t entries_begin = chunks_at + uint64_t(max_chunks) * sizeof(IndexChunk);
+      uint64_t want_batches = (f.hdr.n_hint > f.count ? (f.hdr.n_hint - f.count) / BATCH_N : 0) + 2ull * max_chunks + 2;
+      want_batches = std::min<uint64_t>(want_batches, uint64_t(1) << 23);
+      const uint64_t entries_end = entries_begin + want_batches * MAX_VARS * sizeof(BatchEntry) + 16ull * max_chunks + 64;
+      PCOB_CUDA_TRY(c.files_arena.grow_preserve(entries_end + 64, arena_end, stream));
+      profiler().begin("walk_kernel", stream);
+      walk_kernel<12><<<1, WALK_THREADS, sizeof(WalkSmem<12>), stream>>>(fpf, arena(), chunks_at, max_chunks, entries_begin, entries_end, next, f.count, ~uint64_t(0),
+                                                                        nullptr, c.misc.as<WalkResult>(), 1);
+      profiler().end(stream);
+      PCOB_CUDA_TRY(cudaGetLastError());
+      WalkResult res;
+      PCOB_CUDA_TRY(readback_small_sync(&res, c.misc.p, sizeof(res), stream));
+      if (res.n_chunks > 0) {
+        std::vector<IndexChunk> got(res.n_chunks);
+        PCOB_CUDA_TRY(cudaMemcpyAsync(got.data(), arena() + chunks_at, got.size() * sizeof(IndexChunk), cudaMemcpyDeviceToHost, stream));
+        PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
+        for (IndexChunk& ic : got) {
+          ic.chunk_offset += f.begin;
+          f.recs.push_back(ic);
+        }
+        arena_end = std::max<uint64_t>(res.entries_end, entries_begin);
+      }
+      f.count += res.n_total;
+      next = res.next_byte;
+      if (res.status == ST_TERMINATOR) { f.done = true; break; }
+      if (res.status == ST_INDEX_FULL && res.n_chunks > 0) continue;
+      // a chunk the fast kernels decline (or one beyond the index scratch): the whole file goes to the catch-all decoder, as in
+      // decompress_ex
+      if ((res.status == ST_UNSUPPORTED || res.status == ST_INDEX_FULL) && cold_ok) { f.cold = true; f.staged = true; break; }
+      const PcoB200Error k = res.status == ST_INDEX_FULL ? fail(PCO_B200_UNSUPPORTED, "a single chunk exceeds the device index scratch")
+                                                         : status_to_error(res.status, ("chunk " + std::to_string(res.n_chunks) + " of this walk round").c_str());
+      fail_at(i, k, last_error_ref());
+      break;
+    }
+  }
+
+  // ---- indexed files: every record checked against its own file before anything is decoded.  A file whose records stay inside it joins
+  // the merged list; one with a record outside it decodes on its own with its own bounds (decompress_core, as decompress_ex), one whose
+  // chunk metas route it to the catch-all decoder is cold - both into scratch, since their count is only known once decoded
+  {
+    std::vector<uint32_t> ids;
+    std::vector<FileCheck> chk;
+    for (uint32_t i = 0; i < n && i < limit; i++)
+      if (bf[i].indexed && bf[i].n_idx_chunks > 0) {
+        ids.push_back(i);
+        chk.push_back(FileCheck{bf[i].idx_recs, bf[i].n_idx_chunks, bf[i].begin, bf[i].end - bf[i].begin, bf[i].idx_base, files[i].index_len, bf[i].count,
+                                bf[i].hdr.format_major, 0});
+      }
+    if (!ids.empty()) {
+      PCOB_CUDA_TRY(c.files_tab.reserve(chk.size() * sizeof(FileCheck) + 64));
+      PCOB_CUDA_TRY(c.files_res.reserve(chk.size() * 4 + 64));
+      PCOB_CUDA_TRY(cudaMemcpyAsync(c.files_tab.p, chk.data(), chk.size() * sizeof(FileCheck), cudaMemcpyHostToDevice, stream));
+      profiler().begin("check_index_kernel", stream);
+      check_index_kernel<<<uint32_t(ids.size()), 256, 0, stream>>>(d_src, arena(), dtype, c.files_tab.as<FileCheck>(), c.files_res.as<uint32_t>());
+      profiler().end(stream);
+      PCOB_CUDA_TRY(cudaGetLastError());
+      std::vector<uint32_t> verdict(ids.size());
+      PCOB_CUDA_TRY(readback_small_sync(verdict.data(), c.files_res.p, ids.size() * 4, stream));
+      for (size_t k = 0; k < ids.size(); k++) {
+        BatchFile& f = bf[ids[k]];
+        if (verdict[k] == IDX_MISALIGNED) fail_at(ids[k], PCO_B200_INVALID_ARGUMENT, "side index does not belong to this file (misaligned entries)");
+        else if (verdict[k] == IDX_OUTSIDE) f.alone = f.staged = true;
+        else if (verdict[k] == IDX_COLD && cold_ok) f.cold = f.staged = true;
+      }
+    }
+  }
+
+  // ---- cold files, and indexed files that decode on their own: their count is only known once decoded, so they decode into scratch first
+  auto cold_decode = [&](const BatchFile& f, void* out, uint64_t cap, ColdResult* res) -> PcoB200Error {
+    const FileParams fpf{d_src + f.begin, f.end - f.begin, dtype, f.hdr.uniform_type, f.hdr.format_major};
+    PCOB_CUDA_TRY(c.misc.reserve(256));
+    ColdResult* d_cres = reinterpret_cast<ColdResult*>(c.misc.as<uint8_t>() + 160);
+    for (uint32_t window_cap : {16u, COLD_MAX_WINDOW_LOG}) {  // lookback windows beyond 2^16 numbers get the large scratch on a second try
+      PCOB_CUDA_TRY(c.cold.reserve(cold_scratch_bytes(window_cap)));
+      profiler().begin("cold_decode_kernel", stream);
+      dispatch_latent(dtype, [&](auto tag) {
+        using L = decltype(tag);
+        cold_decode_kernel<L><<<1, 32, 0, stream>>>(fpf, f.hdr.first_chunk_byte, static_cast<L*>(out), cap, c.cold.as<uint8_t>(), window_cap, d_cres);
+        return 0;
+      });
+      profiler().end(stream);
+      PCOB_CUDA_TRY(cudaGetLastError());
+      PCOB_CUDA_TRY(cudaMemcpyAsync(res, d_cres, sizeof(*res), cudaMemcpyDeviceToHost, stream));
+      PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
+      if (res->status != ST_UNSUPPORTED) break;
+    }
+    return PCO_B200_OK;
+  };
+  uint64_t staged_end = 0;
+  for (uint32_t i = 0; i < n && i < limit; i++) {
+    BatchFile& f = bf[i];
+    if (!f.staged) continue;
+    if (f.alone) {
+      // decompress_ex's own path over this file and its index: the kernels' bounds are the file, the index and the count.  A count beyond
+      // dst is left to the placement below (IO).
+      if (f.count > dst_len) continue;
+      for (uint64_t cap = std::max<uint64_t>(f.count, 1);;) {
+        PCOB_CUDA_TRY(c.files_cold.grow_preserve((staged_end + cap) * elem + 64, staged_end * elem, stream));
+        DecodeOutcome oc;
+        const PcoB200Error e = decompress_core(d_src + f.begin, size_t(f.end - f.begin), dtype, c.files_cold.as<uint8_t>() + staged_end * elem, size_t(cap),
+                                               arena() + f.idx_base, size_t(files[i].index_len),
+                                               PCO_B200_SRC_ON_DEVICE | PCO_B200_DST_ON_DEVICE | PCO_B200_INDEX_ON_DEVICE, stream, &oc);
+        if (e == PCO_B200_CUDA) return e;
+        if (e != PCO_B200_OK) { fail_at(i, e, last_error_ref()); break; }
+        if (oc.n_total > cap && cap < dst_len) { cap = std::min<uint64_t>(oc.n_total, dst_len); continue; }  // the catch-all decoder found more
+        f.count = oc.n_total;
+        f.staged_at = staged_end;
+        staged_end += std::min<uint64_t>(oc.n_total, cap);
+        break;
+      }
+      continue;
+    }
+    uint64_t cap = std::max<uint64_t>(std::min<uint64_t>(f.hdr.n_hint, uint64_t(1) << 24), uint64_t(1) << 16);  // the hint is untrusted
+    for (;;) {
+      PCOB_CUDA_TRY(c.files_cold.grow_preserve((staged_end + cap) * elem + 64, staged_end * elem, stream));
+      ColdResult res;
+      if (PcoB200Error e = cold_decode(f, c.files_cold.as<uint8_t>() + staged_end * elem, cap, &res)) return e;
+      if (res.status == ST_DST_FULL) { cap = std::max<uint64_t>(2 * cap, res.n_total + (uint64_t(1) << 16)); continue; }
+      if (res.status != ST_TERMINATOR) fail_at(i, status_to_error(res.status, ("chunk " + std::to_string(res.n_chunks)).c_str()), last_error_ref());
+      f.count = res.n_total;
+      f.staged_at = staged_end;
+      f.recs.clear();
+      staged_end += res.n_total;
+      break;
+    }
+  }
+
+  // ---- placement
+  uint64_t total = 0;
+  for (uint32_t i = 0; i < n && i < limit; i++) {
+    if (bf[i].count > dst_len - std::min<uint64_t>(total, dst_len)) {
+      fail_at(i, PCO_B200_IO, "dst holds " + std::to_string(dst_len) + " numbers, the files up to this one " + std::to_string(total + bf[i].count));
+      break;
+    }
+    bf[i].out_base = total;
+    total += bf[i].count;
+  }
+  void* d_out = dst;
+  if (!dst_dev) {
+    PCOB_CUDA_TRY(c.out.reserve(total * elem + 64));
+    d_out = c.out.p;
+  }
+  const uint64_t out_len = dst_dev ? uint64_t(dst_len) : total;
+
+  // ---- 4. one chunk list for the fast kernels, grouped by (uniform type, format major)
+  std::map<uint32_t, std::vector<uint32_t>> flavours;
+  for (uint32_t i = 0; i < n && i < limit; i++)
+    if (!bf[i].cold && !bf[i].staged && (bf[i].indexed ? bf[i].n_idx_chunks : bf[i].recs.size()) > 0) flavours[(bf[i].hdr.uniform_type << 8) | bf[i].hdr.format_major].push_back(i);
+  struct Slot { uint32_t file; uint64_t at, n; };
+  std::vector<Slot> slots;
+  std::vector<FileMerge> merges;
+  uint64_t list_n = 0;
+  for (auto& kv : flavours)
+    for (uint32_t i : kv.second) {
+      const uint64_t k = bf[i].indexed ? bf[i].n_idx_chunks : bf[i].recs.size();
+      slots.push_back(Slot{i, list_n, k});
+      if (bf[i].indexed) merges.push_back(FileMerge{bf[i].idx_recs, list_n, files[i].offset, bf[i].idx_base, bf[i].out_base, k});
+      list_n += k;
+    }
+  if (list_n > 0xffffffffull) return fail(PCO_B200_UNSUPPORTED, "more than 2^32 chunks in one call");
+  const uint64_t list_at = (arena_end + 15) & ~uint64_t(15);
+  PCOB_CUDA_TRY(c.files_arena.grow_preserve(list_at + list_n * sizeof(IndexChunk) + 64, arena_end, stream));
+  if (list_n) {
+    std::vector<IndexChunk> list(list_n);
+    for (const Slot& s : slots)
+      if (!bf[s.file].indexed)
+        for (uint64_t k = 0; k < s.n; k++) {
+          list[s.at + k] = bf[s.file].recs[k];
+          list[s.at + k].out_offset += bf[s.file].out_base;
+        }
+    PCOB_CUDA_TRY(cudaMemcpyAsync(arena() + list_at, list.data(), list_n * sizeof(IndexChunk), cudaMemcpyHostToDevice, stream));
+    if (!merges.empty()) {
+      PCOB_CUDA_TRY(c.files_tab.reserve(merges.size() * sizeof(FileMerge) + 64));
+      PCOB_CUDA_TRY(cudaMemcpyAsync(c.files_tab.p, merges.data(), merges.size() * sizeof(FileMerge), cudaMemcpyHostToDevice, stream));
+      profiler().begin("merge_index_kernel", stream);
+      merge_index_kernel<<<uint32_t(merges.size()), 256, 0, stream>>>(arena(), c.files_tab.as<FileMerge>(), reinterpret_cast<IndexChunk*>(arena() + list_at));
+      profiler().end(stream);
+      PCOB_CUDA_TRY(cudaGetLastError());
+    }
+  }
+  const uint64_t arena_len = list_at + list_n * sizeof(IndexChunk);
+  {
+    size_t si = 0;
+    for (auto& kv : flavours) {
+      const BatchFile& f0 = bf[kv.second.front()];
+      const FileParams fp{d_src, src_len, dtype, f0.hdr.uniform_type, f0.hdr.format_major};
+      const size_t s_lo = si, s_hi = si + kv.second.size();  // this flavour's slots
+      si = s_hi;
+      std::vector<std::pair<size_t, size_t>> work{{s_lo, s_hi}};  // ranges of slots still to decode
+      while (!work.empty()) {
+        const auto [a, b] = work.back();
+        work.pop_back();
+        size_t hi = a;
+        while (hi < b && slots[hi].file < limit) hi++;  // files from the lowest failure on need no decoding
+        if (hi == a) continue;
+        const uint64_t first = slots[a].at, cnt = slots[hi - 1].at + slots[hi - 1].n - first;
+        const PcoB200Error e = launch_decode(c, fp, arena(), arena_len, list_at + first * sizeof(IndexChunk), uint32_t(cnt), d_out, out_len, stream);
+        if (e == PCO_B200_OK) continue;
+        if (e == PCO_B200_CUDA) return e;
+        // launch_decode names the first failing chunk of its launch ("... chunk k"): find its file
+        const std::string msg = last_error_ref();
+        const size_t at = msg.rfind("chunk ");
+        const uint64_t k = first + (at == std::string::npos ? 0 : std::strtoull(msg.c_str() + at + 6, nullptr, 10));
+        size_t s = a;
+        while (s + 1 < hi && slots[s + 1].at <= k) s++;
+        const uint32_t fi = slots[s].file;
+        if (e == PCO_B200_UNSUPPORTED && cold_ok) {
+          bf[fi].cold = true;
+          if (s + 1 < hi) work.push_back({s + 1, hi});
+        } else {
+          fail_at(fi, e, msg);
+        }
+        if (s > a) work.push_back({a, s});
+      }
+    }
+  }
+
+  // ---- 5. staged numbers moved into their slot; cold files found by the merged decode (an older format, whose chunk metas the check
+  // does not parse) through the catch-all decoder into their slot, sized by their index's count
+  for (uint32_t i = 0; i < n && i < limit; i++) {
+    BatchFile& f = bf[i];
+    uint8_t* slot = static_cast<uint8_t*>(d_out) + f.out_base * elem;
+    if (f.staged) {
+      if (f.count) PCOB_CUDA_TRY(cudaMemcpyAsync(slot, c.files_cold.as<uint8_t>() + f.staged_at * elem, f.count * elem, cudaMemcpyDeviceToDevice, stream));
+      continue;
+    }
+    if (!f.cold) continue;
+    ColdResult res;
+    if (PcoB200Error e = cold_decode(f, slot, f.count, &res)) return e;
+    if (res.status == ST_DST_FULL)  // the file holds more numbers than its index counts: refused rather than cut short
+      fail_at(i, PCO_B200_INVALID_ARGUMENT, "side index does not belong to this file (it counts " + std::to_string(f.count) + " numbers, the file holds more)");
+    else if (res.status != ST_TERMINATOR) fail_at(i, status_to_error(res.status, ("chunk " + std::to_string(res.n_chunks)).c_str()), last_error_ref());
+  }
+  if (limit < n_files) return file_fail(fkind, limit, fmsg);
+  if (!dst_dev && total) PCOB_CUDA_TRY(copy_sliced(dst, d_out, total * elem, cudaMemcpyDeviceToHost, stream));
+  PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
+  if (file_ns)
+    for (uint32_t i = 0; i < n; i++) file_ns[i] = bf[i].count;
+  if (n_written) *n_written = size_t(total);
+  return PCO_B200_OK;
+}
+
+PcoB200Error pco_b200_decompress_files(const void* src, size_t src_len, const void* index, size_t index_len, unsigned char dtype, const PcoB200FileRef* files,
+                                       size_t n_files, void* dst, size_t dst_len, uint64_t* file_ns, size_t* n_written, uint32_t flags, void* cuda_stream) {
+  const PcoB200Error e = decompress_files_impl(src, src_len, index, index_len, dtype, files, n_files, dst, dst_len, file_ns, n_written, flags,
+                                               static_cast<cudaStream_t>(cuda_stream));
   profiler().resolve();
   return e;
 }

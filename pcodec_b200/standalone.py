@@ -181,6 +181,152 @@ def decompress_chunks(src, dtype, chunk_offsets, chunk_ns):
     return dst[: n_written.value]
 
 
+# PcoB200FileRef (include/pco_b200.h): one standalone file of a batch, and its side index (index_len 0 = none)
+FILE_REF = np.dtype([("offset", "<u8"), ("len", "<u8"), ("index_offset", "<u8"), ("index_len", "<u8")])
+_INDEX_ON_DEVICE = 4
+
+
+def _lib_files():
+    L = _lib.lib()
+    if not getattr(L, "_files_ready", False):
+        L.pco_b200_compress_files.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_ubyte, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p,
+                                              C.c_size_t, C.c_void_p, C.c_uint32, C.c_void_p]
+        L.pco_b200_decompress_files.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_ubyte, C.c_void_p, C.c_size_t, C.c_void_p,
+                                                C.c_size_t, C.c_void_p, C.POINTER(C.c_size_t), C.c_uint32, C.c_void_p]
+        L._files_ready = True
+    return L
+
+
+def _is_cuda(x):
+    return getattr(x, "is_cuda", False)
+
+
+def _stream_of(t):
+    import torch
+
+    return C.c_void_p(torch.cuda.current_stream(t.device).cuda_stream)
+
+
+def compress_files(nums, file_ns, config=None, uniform_type=False, with_index=True):
+    """Compresses many arrays of one number type in one call (pco_b200_compress_files): file i is the next file_ns[i] numbers of
+    `nums`, written as its own standalone file, byte-identical to simple_compress (uniform_type=False) or simple_compress_into
+    (True) of those numbers.  Returns (data, files[, index]): the files back to back, one FILE_REF record per file, and - with
+    with_index - the files' side indexes at 16-byte aligned offsets.  A torch CUDA tensor gives uint8 CUDA tensors, computed on
+    the current stream."""
+    from .wrapped import _torch_dtypes
+
+    ns = np.ascontiguousarray(file_ns, dtype=np.uint64).reshape(-1)
+    cfg = (config or ChunkConfig())._to_c()
+    L = _lib_files()
+    if _is_cuda(nums):
+        import torch
+
+        t = nums.contiguous().reshape(-1)
+        dt = next(k for k, v in _torch_dtypes().items() if v == t.dtype)
+        src, flags, stream = C.c_void_p(t.data_ptr()), _lib.SRC_ON_DEVICE | _lib.DST_ON_DEVICE | _INDEX_ON_DEVICE, _stream_of(t)
+        total_n = t.numel()
+
+        def alloc(nbytes):
+            return torch.empty(max(nbytes, 1), dtype=torch.uint8, device=t.device)
+
+        def ptr(buf):
+            return C.c_void_p(buf.data_ptr())
+    else:
+        arr = np.ascontiguousarray(nums).reshape(-1)
+        dt, src, flags, stream, total_n = arr.dtype, arr.ctypes.data_as(C.c_void_p), 0, None, arr.size
+
+        def alloc(nbytes):
+            return np.empty(max(nbytes, 1), dtype=np.uint8)
+
+        def ptr(buf):
+            return buf.ctypes.data_as(C.c_void_p)
+    if int(ns.sum()) != total_n:
+        raise ValueError(f"file_ns add up to {int(ns.sum())} numbers, nums holds {total_n}")
+    dtb = _lib.dtype_byte(dt)
+    page_n = cfg.max_page_n or (1 << 18)
+    chunks = [int(cfg.n_exact_pages) if cfg.paging_spec == 1 else -(-int(n) // page_n) for n in ns]
+    cap = sum(L.pco_standalone_guarantee_file_size(int(n), dtb) + 160 * k for n, k in zip(ns, chunks))
+    icap = sum(L.pco_b200_index_size_bound(int(n), k) + 64 * k + 16 for n, k in zip(ns, chunks)) if with_index else 0
+    files = np.zeros(max(ns.size, 1), dtype=FILE_REF)
+    for attempt in range(2):  # a first guess of the capacities, then what the call reported it needs
+        data = alloc(cap)
+        index = alloc(icap) if with_index else None
+        rc = L.pco_b200_compress_files(src, ns.ctypes.data_as(C.c_void_p), C.c_size_t(ns.size), C.c_ubyte(dtb), C.byref(cfg), C.c_int(1 if uniform_type else 0),
+                                       ptr(data), C.c_size_t(cap), ptr(index) if with_index else None, C.c_size_t(icap), files.ctypes.data_as(C.c_void_p),
+                                       C.c_uint32(flags), stream)
+        if rc == 4 and attempt == 0 and ns.size:  # PCO_B200_IO: the refs report the sizes needed
+            last = files[ns.size - 1]
+            cap = max(cap, int(last["offset"] + last["len"]))
+            icap = max(icap, int(last["index_offset"] + last["index_len"]))
+            continue
+        _lib.check(rc)
+        break
+    files = files[: ns.size].copy()
+    used = int(files[-1]["offset"] + files[-1]["len"]) if ns.size else 0
+    iused = int(files[-1]["index_offset"] + files[-1]["index_len"]) if ns.size and with_index else 0
+    if _is_cuda(nums):
+        out = (data[:used], files)
+        return out + (index[:iused],) if with_index else out
+    out = (data[:used].tobytes(), files)
+    return out + (index[:iused].tobytes(),) if with_index else out
+
+
+def decompress_files(data, files, dtype, index=None):
+    """Decodes every standalone file `files` (FILE_REF records) names into one array, file after file in `files` order
+    (pco_b200_decompress_files).  Returns (values, file_ns).  Files with index_len > 0 are decoded through their side index in
+    `index`.  `data` and `index` are bytes / numpy, or torch CUDA tensors (then `values` is a CUDA tensor, computed on the current
+    stream)."""
+    from .wrapped import _host_u8, _torch_dtypes
+
+    dt = np.dtype(dtype)
+    r = np.ascontiguousarray(np.asarray(files).astype(FILE_REF, copy=False)).reshape(-1)
+    L = _lib_files()
+    nf = r.size
+    file_ns = np.zeros(max(nf, 1), dtype=np.uint64)
+    nw = C.c_size_t()
+    cuda = _is_cuda(data)
+    if cuda:
+        import torch
+
+        d = data.contiguous().reshape(-1)
+        ix = index.contiguous().reshape(-1) if index is not None else None
+        # the headers' count hints size the destination (grown if the files hold more)
+        pos = torch.as_tensor(r["offset"].astype(np.int64), device=d.device)[:, None] + torch.arange(32, device=d.device)[None, :]
+        heads = d[pos.clamp_(max=max(d.numel() - 1, 0))].cpu().numpy() if nf and d.numel() else np.zeros((nf, 32), np.uint8)
+        src_p, src_len = C.c_void_p(d.data_ptr()), d.numel()
+        idx_p, idx_len = (C.c_void_p(ix.data_ptr()), ix.numel()) if ix is not None else (None, 0)
+        flags, stream = _lib.SRC_ON_DEVICE | _lib.DST_ON_DEVICE | (_INDEX_ON_DEVICE if ix is not None else 0), _stream_of(d)
+
+        def alloc(n):
+            return torch.empty(max(n, 1), dtype=_torch_dtypes()[dt], device=d.device)
+
+        def ptr(buf):
+            return C.c_void_p(buf.data_ptr())
+    else:
+        d = _host_u8(data)
+        ix = _host_u8(index) if index is not None else None
+        heads = np.stack([np.frombuffer(d[int(o):int(o) + 32].tobytes().ljust(32, b"\0"), np.uint8) for o in r["offset"]]) if nf else np.zeros((0, 32), np.uint8)
+        src_p, src_len = d.ctypes.data_as(C.c_void_p), d.size
+        idx_p, idx_len = (ix.ctypes.data_as(C.c_void_p), ix.size) if ix is not None else (None, 0)
+        flags, stream = 0, None
+
+        def alloc(n):
+            return np.empty(max(n, 1), dtype=dt)
+
+        def ptr(buf):
+            return buf.ctypes.data_as(C.c_void_p)
+    cap = sum(n_hint(heads[k, : int(min(r["len"][k], 32))].tobytes()) for k in range(nf))
+    while True:
+        dst = alloc(cap)
+        rc = L.pco_b200_decompress_files(src_p, C.c_size_t(src_len), idx_p, C.c_size_t(idx_len), C.c_ubyte(_lib.dtype_byte(dt)), r.ctypes.data_as(C.c_void_p),
+                                         C.c_size_t(nf), ptr(dst), C.c_size_t(cap), file_ns.ctypes.data_as(C.c_void_p), C.byref(nw), C.c_uint32(flags), stream)
+        if rc == 4 and "dst holds" in _lib.lib().pco_b200_last_error_message().decode():  # the hints were short
+            cap = max(2 * cap, 1 << 16)
+            continue
+        _lib.check(rc)
+        return dst[: nw.value], file_ns[:nf].copy()
+
+
 class _CModeChoice(C.Structure):
     _fields_ = [("mode_spec", C.c_uint32), ("float_quant_k", C.c_uint32), ("float_mult_base", C.c_double), ("float_mult_inv_base", C.c_double),
                 ("int_mult_base", C.c_uint64), ("bits_saved_per_num", C.c_double)]
