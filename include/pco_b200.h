@@ -142,7 +142,8 @@ int pco_b200_profile_last(char *buf, size_t cap);
 /* Threading: the library keeps one scratch context per calling host thread (device buffers grown on demand and reused by that
  * thread's next call), so calls from different threads - each with its own cudaStream_t - run concurrently, e.g. compress of
  * chunk group g + 1 on one thread while group g decompresses on another (both PCIe directions busy).  A worker thread that is
- * about to exit returns its device scratch with pco_b200_thread_release(). */
+ * about to exit returns its device scratch with pco_b200_thread_release(); a thread that goes on calling the library afterwards gets
+ * fresh scratch on its next call. */
 void pco_b200_thread_release(void);
 /* Page-locked host buffers in place ("zero copy"): with bit 0 set, pco_b200_compress_ex (explicit Classic configs) reads a HOST `nums`
  * that is page-locked (cudaHostAlloc / cudaHostRegister, e.g. torch pin_memory) straight over PCIe in its one pass over the input; with
@@ -159,6 +160,13 @@ size_t pco_b200_debug_follow_chain(const uint64_t *cand, const uint32_t *statuse
 /* counts8[k] = chunks of the last decode launch served by decode class k (1, 2: general kernel with 1 / 2 latent vars;
  * 3, 4: narrow kernel, delta order 0 / 1); returns the number of chunks. */
 int pco_b200_profile_chunk_classes(unsigned *counts8);
+/* How the tANS encoder resolved the last compress call on this thread, if it ran with pco_b200_profile_enable(1) (for a call that
+ * compresses in several passes, e.g. pco_b200_compress_files with several groups: its last pass).  The encoder cuts each (chunk, latent
+ * var) page into segments, encoded in rounds of up to 64; counts8[k] = rounds resolved by k: 0 = the speculated segment inputs held,
+ * 1 = the fix-up iterations converged, 2 = transfer functions, 3 = in-order pass over the page (which ends the page's rounds);
+ * counts8[4 + k] = those of them that were not a page's first round (pages of more than 2^18 numbers).  Returns counts8[0] + ... +
+ * counts8[3]; 0 and all zeros when there is nothing to report. */
+int pco_b200_profile_ans_paths(unsigned *counts8);
 
 /* ---- sharded writers (no reference counterpart; SURVEY.md 8e): chunk c of the logical standalone file is compressed on rank
  * c mod G (PCO_B200_CHUNKS_ONLY); the page gather then leaves the WHOLE file - header | chunk_0 | chunk_1 | ... | 0x00, byte-identical

@@ -30,10 +30,14 @@ struct CompressScratch {
   bool plan_attr_set[4] = {false, false, false, false}, union_attr_set[4] = {false, false, false, false}, sort_attr_set[4] = {false, false, false, false};
   bool wide_attr_set[4] = {false, false, false, false};  // the wide (more than 256 bins) instantiations
   bool src_in_place = false;  // this call reads its numbers from the caller's page-locked host buffer (host_common.hpp, zero copy)
+  // ans_encode_kernel's round counters of the last call, kept only while profiling is on (pco_b200_profile_ans_paths)
+  DevBuf ans_paths;
+  bool ans_paths_valid = false;
   void release() {
     for (DevBuf* b : {&lat0, &lat1, &keys_a, &keys_b, &sym0, &sym1, &ans0, &ans1, &ob_sum, &ans_sum, &entries, &plans, &chunks, &starts, &seg, &out, &small,
-                      &index, &probes, &sample, &sample_starts, &key16_0, &key16_1, &idx_out, &lb_vals, &lb_resid, &lb_scratch})
+                      &index, &probes, &sample, &sample_starts, &key16_0, &key16_1, &idx_out, &lb_vals, &lb_resid, &lb_scratch, &ans_paths})
       b->release();
+    ans_paths_valid = false;
   }
 };
 
@@ -627,6 +631,7 @@ static PcoB200Error compress_typed(CompressScratch& S, const void* nums, size_t 
   const bool auto_mode = checked.auto_mode, auto_delta = checked.auto_delta;
   const uint32_t explicit_order = checked.explicit_order;
   const bool chunks_only = flags & PCO_B200_CHUNKS_ONLY;
+  S.ans_paths_valid = false;
   std::vector<uint8_t> header = make_standalone_header(n, uint8_t(uniform_type ? dtype : 0));
   if (chunks_only) header.clear();
   // empty input: header + terminator only (standalone/simple.rs:62-91)
@@ -704,6 +709,13 @@ static PcoB200Error compress_typed(CompressScratch& S, const void* nums, size_t 
   uint64_t* d_total = reinterpret_cast<uint64_t*>(d_small + 2);
   uint8_t* d_header = reinterpret_cast<uint8_t*>(d_small) + 64;
   if (!header.empty()) PCOB_CUDA_TRY(cudaMemcpyAsync(d_header, header.data(), header.size(), cudaMemcpyHostToDevice, stream));
+  uint32_t* d_ans_paths = nullptr;  // non-null only while profiling: the timed path launches ans_encode_kernel without counters
+  if (profiler_enabled().load(std::memory_order_relaxed)) {
+    PCOB_CUDA_TRY(S.ans_paths.reserve(ANS_PATH_SLOTS * sizeof(uint32_t)));
+    PCOB_CUDA_TRY(cudaMemsetAsync(S.ans_paths.p, 0, ANS_PATH_SLOTS * sizeof(uint32_t), stream));
+    d_ans_paths = S.ans_paths.as<uint32_t>();
+    S.ans_paths_valid = true;
+  }
 
   // ---- K1+K2 and the planner for one set of chunks (a run of the call's chunks, or the chunks' samples during the Auto delta search).
   // `e` describes the set (its own chunk_starts / row_base, counted from 0); plans and probes land in slots 0 .. e.n_chunks - 1.
@@ -1046,7 +1058,7 @@ static PcoB200Error compress_typed(CompressScratch& S, const void* nums, size_t 
       // the ans kernel indexes (chunk, var) by blockIdx; both vars share the launch via separate symbol arrays
       profiler().begin("ans_encode_kernel", stream);
       ans_encode_kernel<W><<<n_chunks * MAX_VARS, ANS_THREADS, 0, stream>>>(ep, bpc, d_plans, d_chunks, d_sym[0], d_sym[1], d_ans[0], d_ans[1], S.ans_sum.as<uint32_t>(),
-                                                                            S.entries.as<BatchEntry>());
+                                                                            S.entries.as<BatchEntry>(), d_ans_paths);
       profiler().end(stream);
       // ---- layout, offsets, K5
       profiler().begin("layout_kernel", stream);

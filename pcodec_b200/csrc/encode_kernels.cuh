@@ -1830,6 +1830,9 @@ constexpr int ANS_WARM_BATCHES = 2;         // batches of the preceding segment 
 constexpr uint32_t ANS_MAX_SEG_BATCHES = 16;
 constexpr uint32_t ANS_TF_MAX = 8;          // largest pivot weight the transfer-function path enumerates (a quiet replay of the segment per slot, ~0.12 ms each)
 constexpr int ANS_TF_LOOK = 4;              // it picks the lightest symbol among a chain's first ANS_TF_LOOK steps of the segment
+// slots of the round counters ans_encode_kernel keeps when profiling (pco_b200_profile_ans_paths, include/pco_b200.h): by resolution,
+// then the same four for the rounds after a page's first
+enum : uint32_t { ANS_PATH_SPECULATION = 0, ANS_PATH_FIXUP = 1, ANS_PATH_TRANSFER = 2, ANS_PATH_IN_ORDER = 3, ANS_PATH_LATER_ROUND = 4, ANS_PATH_SLOTS = 8 };
 
 template <bool WIDE>
 struct AnsSmemT {
@@ -1937,7 +1940,7 @@ __global__ void __launch_bounds__(ANS_THREADS, 4) ans_encode_kernel(EncParams ep
                                                                      ChunkEnc* __restrict__ chunks, const typename EncCap<WIDE>::Sym* __restrict__ sym0,
                                                                      const typename EncCap<WIDE>::Sym* __restrict__ sym1, uint16_t* __restrict__ ans0,
                                                                      uint16_t* __restrict__ ans1, uint32_t* __restrict__ ans_sum,
-                                                                     BatchEntry* __restrict__ entries) {
+                                                                     BatchEntry* __restrict__ entries, uint32_t* __restrict__ path_counts) {
   using Sym = typename EncCap<WIDE>::Sym;
   __shared__ AnsSmemT<WIDE> sm;
   const uint32_t c = blockIdx.x / MAX_VARS, v = blockIdx.x % MAX_VARS;
@@ -2160,7 +2163,8 @@ __global__ void __launch_bounds__(ANS_THREADS, 4) ans_encode_kernel(EncParams ep
     bool solved = false;
     {
       bool converged = false;
-      for (int iter = 0; iter < 24 && !converged; iter++) {
+      int iter = 0;
+      for (; iter < 24 && !converged; iter++) {
         const uint32_t in_true = (s == 0 || !active) ? my_in : uint32_t(sm.out_state[s - 1][j]);
         bool changed = false;
         if (in_true != my_in) {
@@ -2193,13 +2197,25 @@ __global__ void __launch_bounds__(ANS_THREADS, 4) ans_encode_kernel(EncParams ep
         converged = n_changed == 0;
         if (iter == 0 && n_changed > n_round) break;  // more than a quarter of the 4 n_round pairs (an eighth sent C5 float64 order 0 in-order, three times slower)
       }
+      // test hook (pco_b200_profile_ans_paths; null unless profiling): one count per round by resolution, and again in the upper half
+      // of the slots for rounds after the page's first
+      auto count_round = [&](uint32_t path) {
+        if (path_counts != nullptr && tid == 0) {
+          atomicAdd(&path_counts[path], 1u);
+          if (done > 0) atomicAdd(&path_counts[ANS_PATH_LATER_ROUND + path], 1u);
+        }
+      };
       if (!converged) {
         if (!pivots_enumerable()) {
+          count_round(ANS_PATH_IN_ORDER);
           serial_pass();
           return;
         }
+        count_round(ANS_PATH_TRANSFER);
         transfer_round();
         solved = true;
+      } else {
+        count_round(iter == 1 ? ANS_PATH_SPECULATION : ANS_PATH_FIXUP);  // iter: fix-up iterations run, the last one saw no output move
       }
     }
     if (solved) continue;  // transfer_round left the carry

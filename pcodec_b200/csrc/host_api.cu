@@ -922,7 +922,15 @@ int pco_b200_zero_copy(int mask) { return mask < 0 ? zero_copy_mask().load() : z
 // thread's next call).
 void pco_b200_thread_release(void) {
   Context& c = ctx();
-  if (c.initialized && c.device_ok) release_buffers(c);
+  if (c.initialized && c.device_ok) {
+    release_buffers(c);
+    // release_buffers also frees the binomial table that ensure_device builds once per context: mark the context uninitialised so that
+    // a later call on this thread builds it again.  Left initialised, the next decode that reached decode_kernel read a null table
+    // (an illegal address) - a thread that releases its scratch between calls instead of exiting.
+    c.initialized = false;
+    c.device_ok = false;
+    c.attrs_set = false;
+  }
   readback_bounce().release();
 }
 // Which decode instantiation served the chunks of the last decode launch: counts[k] = chunks of class k
@@ -935,6 +943,17 @@ int pco_b200_profile_chunk_classes(unsigned* counts8) {
   if (cudaMemcpy(cls.data(), c.d_cls, cls.size(), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
   for (uint8_t k : cls) counts8[(k & 0x7f) < 8 ? (k & 0x7f) : 0]++;
   return int(cls.size());
+}
+// How ans_encode_kernel resolved the tANS rounds of the last compress pass on this thread, when it ran with profiling on: counts[k] =
+// (chunk, var, round) triples resolved by k (0: speculation held, 1: fix-up converged, 2: transfer functions, 3: in-order pass),
+// counts[4 + k] = those among them that were not a page's first round.  Returns the number of rounds counted (0 and all zeros without a
+// profiled compress).
+int pco_b200_profile_ans_paths(unsigned* counts8) {
+  Context& c = ctx();
+  for (int i = 0; i < 8; i++) counts8[i] = 0;
+  if (!c.device_ok || !c.enc.ans_paths_valid) return 0;
+  if (cudaMemcpy(counts8, c.enc.ans_paths.p, ANS_PATH_SLOTS * sizeof(uint32_t), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
+  return int(counts8[ANS_PATH_SPECULATION] + counts8[ANS_PATH_FIXUP] + counts8[ANS_PATH_TRANSFER] + counts8[ANS_PATH_IN_ORDER]);
 }
 // Copies "name=ms;name=ms;..." of the last finished call into buf; returns the number of spans.
 int pco_b200_profile_last(char* buf, size_t cap) {

@@ -64,6 +64,26 @@ def test_no_gpu_means_loud_failure():
     assert e.value.kind == "Cuda"
 
 
+def test_ans_path_counters_without_a_compress_are_zero():
+    """pco_b200_profile_ans_paths on a thread that has compressed nothing (so also without a device): 0 rounds, every slot zeroed."""
+    import threading
+
+    from pcodec_b200 import _lib
+
+    L = _lib.lib()
+    out = {}
+
+    def probe():
+        counts = (C.c_uint * 8)(*([7] * 8))
+        out["rc"] = L.pco_b200_profile_ans_paths(counts)
+        out["counts"] = list(counts)
+
+    t = threading.Thread(target=probe)  # the library's scratch and counters are per thread: a new thread has none
+    t.start()
+    t.join()
+    assert out == {"rc": 0, "counts": [0] * 8}
+
+
 def test_decompress_chunks_argument_checks_need_no_device():
     """pco_b200_decompress_chunks validates its table before touching the device: nothing to do is fine, a missing table is not."""
     import ctypes as C
