@@ -306,6 +306,44 @@ PcoB200Error pco_b200_decompress_files(const void *src, size_t src_len, const vo
                                        void *dst, size_t dst_len, uint64_t *file_ns, size_t *n_written,
                                        uint32_t flags, void *cuda_stream);
 
+/* ---- ranges of an indexed standalone file (no reference counterpart): random access for a columnar reader that wants rows [a, b),
+ * a page cache answering point lookups, a checkpoint reader that wants one shard.  Only the chunks a range touches are decoded, and
+ * in chunks of delta order 0 only the batches it touches.
+ * One range: numbers [start, start + count) of the file, counted from its first number. */
+typedef struct PcoB200Range {
+  uint64_t start;  /* first number of the range, counted from the file's first number */
+  uint64_t count;  /* numbers in the range; 0 is allowed and writes nothing */
+} PcoB200Range;
+
+/* Decodes n_ranges ranges of one standalone file through its side index (`index`, as pco_b200_compress_ex or pco_b200_build_index
+ * write it): range i lands in dst right behind range i - 1, and *n_written = the sum of the counts.  Every number equals the same
+ * position of pco_b200_decompress_ex on the whole file.  Ranges may come in any order, may overlap and may repeat; a chunk is
+ * decoded once however many ranges touch it.  PCO_B200_SRC_ON_DEVICE covers `compressed`, PCO_B200_DST_ON_DEVICE covers dst,
+ * PCO_B200_INDEX_ON_DEVICE covers `index`; `ranges` is host memory.  Work runs on `cuda_stream`, and the call returns once it is done.
+ * Refused before any device work (headers and the chunk table in device memory are read back first, in at most two readbacks):
+ * an unknown dtype (PCO_B200_INVALID_TYPE); index == NULL or index_len == 0, ranges == NULL with n_ranges > 0, a range past the
+ * index's count of numbers or whose start + count overflows (message "range <i>: ..."), dst_len below the sum of the counts, an
+ * index whose header does not belong to the file (the check of pco_b200_decompress_ex), and an index whose chunk records do not tile
+ * the file's numbers in order (PCO_B200_INVALID_ARGUMENT).  n_ranges == 0 is OK.  A chunk that fails on the device fails the call
+ * with the kind pco_b200_decompress_ex gives, and the message names the lowest-index range with numbers in that chunk
+ * ("range 17: ...").  Chunks the fast kernels decline (tables above 2^10 states or 256 bins, f16 FloatMult, ...) are decoded by the
+ * single-thread catch-all decoder, from the chunk's start to the last number wanted.
+ * Like a short destination, a range decode reads only the chunks and batches it needs: it does not see corruption elsewhere in the
+ * file, including the end-of-page checks of chunks it stops early in. */
+PcoB200Error pco_b200_decompress_ranges(const void *compressed, size_t compressed_len, unsigned char dtype,
+                                        const void *index, size_t index_len,
+                                        const PcoB200Range *ranges, size_t n_ranges,
+                                        void *dst, size_t dst_len, size_t *n_written,
+                                        uint32_t flags, void *cuda_stream);
+/* Host logic of pco_b200_decompress_ranges, exposed for tests (needs no device): splits the ranges over `n_chunks` side-index chunk
+ * records (32 bytes each, as in the index) and groups the pieces into decode tasks, one per touched chunk.  pieces_out gets 6 words per
+ * piece (chunk, lo, hi, dst_off, range, task), in range order; tasks_out 6 per task (chunk, lo, hi, n_pieces, lowest range, staged),
+ * in chunk order.  Refuses what the call refuses (PCO_B200_INVALID_ARGUMENT); tables that are too small are PCO_B200_IO, with
+ * *n_pieces and *n_tasks still reporting the sizes needed. */
+PcoB200Error pco_b200_debug_plan_ranges(const void *chunk_table, size_t n_chunks, uint64_t n_total, const PcoB200Range *ranges,
+                                        size_t n_ranges, uint64_t *pieces_out, size_t pieces_cap, size_t *n_pieces,
+                                        uint64_t *tasks_out, size_t tasks_cap, size_t *n_tasks);
+
 #if defined(__cplusplus)
 }
 #endif

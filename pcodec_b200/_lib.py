@@ -170,6 +170,10 @@ def lib():
         L.pco_standalone_guarantee_file_size.argtypes = [C.c_size_t, C.c_ubyte]
         L.pco_b200_index_size_bound.restype = C.c_size_t
         L.pco_b200_index_size_bound.argtypes = [C.c_size_t, C.c_size_t]
+        L.pco_b200_decompress_ranges.argtypes = [C.c_void_p, C.c_size_t, C.c_ubyte, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
+                                                 C.c_size_t, C.POINTER(C.c_size_t), C.c_uint32, C.c_void_p]
+        L.pco_b200_debug_plan_ranges.argtypes = [C.c_void_p, C.c_size_t, C.c_uint64, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t,
+                                                 C.POINTER(C.c_size_t), C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
         _lib = L
     return _lib
 

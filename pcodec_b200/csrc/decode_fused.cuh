@@ -133,9 +133,9 @@ struct FusedSmem {
   };
 };
 
-// The walker warp: lane k walks batch 32 g + k of group g.
-__device__ __forceinline__ void fused_walker(FusedSmem& sm, const BitSrc& src, uint64_t chunk_bit0, const BatchEntry* __restrict__ entries, uint32_t nb_out,
-                                             uint32_t stored, uint32_t size_log, uint32_t rep_log, int walker, int lane) {
+// The walker warp: lane k walks batch first + 32 g + k of group g (groups, and so ring buffers and phases, count from batch `first`).
+__device__ __forceinline__ void fused_walker(FusedSmem& sm, const BitSrc& src, uint64_t chunk_bit0, const BatchEntry* __restrict__ entries, uint32_t first,
+                                             uint32_t nb_out, uint32_t stored, uint32_t size_log, uint32_t rep_log, int walker, int lane) {
   const uint64_t max_blk = (src.n_bits == 0 ? 0 : (src.n_bits - 1) >> 6) >> 1;
   const uint32_t node_sa = smem_addr(sm.node + (uint32_t(lane) & ((1u << rep_log) - 1)));  // this lane's copy
   const uint32_t sl = rep_log + 2;                                                           // states are byte offsets into the lane's copy
@@ -143,14 +143,14 @@ __device__ __forceinline__ void fused_walker(FusedSmem& sm, const BitSrc& src, u
   const uint32_t stg_sa = smem_addr(sm.run.stage[walker]);
   const uint32_t row_g = stg_sa + uint32_t(lane) * (FZ_ROW_BLOCKS * 16);
   const uint32_t* rowp = sm.run.stage[walker] + lane * (FZ_ROW_BLOCKS * 4);
-  const uint32_t groups = (nb_out + 31) / 32;
+  const uint32_t groups = (nb_out - first + 31) / 32;
   BatchEntry e_nxt;
   e_nxt.bit_pos = 0; e_nxt.st[0] = e_nxt.st[1] = e_nxt.st[2] = e_nxt.st[3] = 0;
-  if (uint32_t(walker) * 32 + lane < nb_out) e_nxt = entries[uint32_t(walker) * 32 + lane];
+  if (first + uint32_t(walker) * 32 + lane < nb_out) e_nxt = entries[first + uint32_t(walker) * 32 + lane];
   for (uint32_t g = walker; g < groups; g += FZ_WALKERS) {
     const uint32_t rb = g % FZ_NBUF, ph = g / FZ_NBUF;
     const BatchEntry e = e_nxt;
-    const uint32_t b = g * 32 + lane;
+    const uint32_t b = first + g * 32 + lane;
     const bool mine = b < nb_out;
     if (b + 32 * FZ_WALKERS < nb_out) e_nxt = entries[b + 32 * FZ_WALKERS];  // the walker's next entry is in flight while this group is walked
     if (ph > 0) mbar_wait(smem_addr(&sm.empty_bar[rb]), (ph - 1) & 1u);  // the decoders have taken group g - FZ_NBUF out of the buffer
@@ -285,10 +285,10 @@ __device__ __forceinline__ void fused_undelta(L (&x)[8], FusedSmem& sm, uint32_t
   }
 }
 
-// A decoder warp: batches d, d + FZ_DECODERS, ... of the chunk (K = consecutive delta order, 0 or 1).
-template <typename L, int K>
+// A decoder warp: batches first + d, first + d + FZ_DECODERS, ... of the chunk (K = consecutive delta order; first = 0 unless WIN and K = 0).
+template <typename L, int K, bool WIN>
 __device__ __forceinline__ void fused_decoder(FusedSmem& sm, const FileParams& fp, const BitSrc& src, const IndexChunk& task, uint64_t chunk_bit0, L* __restrict__ out,
-                                              uint32_t n, uint32_t n_out, int d, int lane) {
+                                              uint32_t n, uint32_t n_out, uint32_t first, const WinTask& win, int d, int lane) {
   const uint64_t max_blk = (src.n_bits == 0 ? 0 : (src.n_bits - 1) >> 6) >> 1;
   const uint64_t cblk0 = chunk_bit0 >> 7;
   const uint32_t cbr = uint32_t(chunk_bit0 & 127);
@@ -311,7 +311,7 @@ __device__ __forceinline__ void fused_decoder(FusedSmem& sm, const FileParams& f
     asm volatile("cp.async.commit_group;");
   };
   // symbols (8 per lane) and section start of batch bb out of the ring; non-blocking variant for the look-ahead
-  auto fetch = [&](uint32_t bb, uint32_t& off, uint2& sy, bool blocking) -> bool {
+  auto fetch = [&](uint32_t bb, uint32_t& off, uint2& sy, bool blocking) -> bool {  // bb counts from batch `first`
     const uint32_t g = bb >> 5, rb = g % FZ_NBUF, parity = (g / FZ_NBUF) & 1u;
     const uint32_t bar = smem_addr(&sm.full_bar[rb]);
     if (blocking) mbar_wait(bar, parity);
@@ -329,16 +329,16 @@ __device__ __forceinline__ void fused_decoder(FusedSmem& sm, const FileParams& f
   uint2 sy_cur = make_uint2(0u, 0u), sy_nxt = make_uint2(0u, 0u);
   bool have = false;
   uint32_t buf = 0;
-  for (uint32_t b = d; b < nb_out; b += FZ_DECODERS) {
+  for (uint32_t b = first + d; b < nb_out; b += FZ_DECODERS) {
     if (!have) {
-      fetch(b, off_cur, sy_cur, true);
+      fetch(b - first, off_cur, sy_cur, true);
       issue_window(off_cur, buf);
     }
     asm volatile("cp.async.wait_group 0;" ::: "memory");
     __syncwarp();  // this batch's window is visible to the warp; every lane is done with the other buffer
     const uint2 sy = sy_cur;
     have = false;
-    if (b + FZ_DECODERS < nb_out && fetch(b + FZ_DECODERS, off_nxt, sy_nxt, false)) {
+    if (b + FZ_DECODERS < nb_out && fetch(b - first + FZ_DECODERS, off_nxt, sy_nxt, false)) {
       issue_window(off_nxt, buf ^ 1u);
       have = true;
     }
@@ -440,15 +440,19 @@ __device__ __forceinline__ void fused_decoder(FusedSmem& sm, const FileParams& f
 #pragma unroll
       for (int e = 0; e < 8; e++) res[e] = from_latent_kind<L>(res[e], kind);
     }
-    const uint32_t out_cnt = min(uint32_t(BATCH_N), n_out - b * BATCH_N);
-    if (out_cnt == uint32_t(BATCH_N) && (reinterpret_cast<uintptr_t>(dst) & (sizeof(L) >= 4 ? 15 : sizeof(L) * 8 - 1)) == 0) {
-      store8<L>(dst, res);
+    if constexpr (WIN) {
+      win_store8<L>(win, b, lane, res);
     } else {
+      const uint32_t out_cnt = min(uint32_t(BATCH_N), n_out - b * BATCH_N);
+      if (out_cnt == uint32_t(BATCH_N) && (reinterpret_cast<uintptr_t>(dst) & (sizeof(L) >= 4 ? 15 : sizeof(L) * 8 - 1)) == 0) {
+        store8<L>(dst, res);
+      } else {
 #pragma unroll
-      for (int e = 0; e < 8; e++)
-        if (uint32_t(lane * 8 + e) < out_cnt) dst[e] = res[e];
+        for (int e = 0; e < 8; e++)
+          if (uint32_t(lane * 8 + e) < out_cnt) dst[e] = res[e];
+      }
+      dst += FZ_DECODERS * BATCH_N;
     }
-    dst += FZ_DECODERS * BATCH_N;
     if (b == nb_total - 1) {  // end-of-page checks by the warp that owns the last batch (page_decompressor.rs:184-188)
       const uint32_t total_bits = __shfl_sync(0xffffffffu, inc, 31);
       const uint64_t bit = (cblk0 << 7) + sec_rel + total_bits;
@@ -469,10 +473,13 @@ __device__ __forceinline__ void fused_decoder(FusedSmem& sm, const FileParams& f
 
 // d_cls[c] on return: CLS_DONE | class = the chunk is done (decoded here as narrow order 0 / 1, or refused with its status
 // written), 1 / 2 = it belongs to decode_kernel<L, 1 / 2> (symwalk_kernel + decode_kernel run for those).
-template <typename L>
+// WIN: window mode (decode_kernels.cuh, WinTask): task t stores only the numbers wins[t] names (out and out_len are unused), and the
+// status word of a chunk handed to the general pair holds its first batch, which sizes that task's scratch rows.
+template <typename L, bool WIN = false>
 __global__ void __launch_bounds__(FZ_THREADS, PCOB_FZ_MIN_BLOCKS)
 fused_narrow_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, const uint8_t* __restrict__ index_base, uint64_t index_len,
-                    uint32_t* __restrict__ statuses, uint8_t* __restrict__ d_cls, L* __restrict__ out, uint64_t out_len) {
+                    uint32_t* __restrict__ statuses, uint8_t* __restrict__ d_cls, L* __restrict__ out, uint64_t out_len,
+                    const WinTask* __restrict__ wins = nullptr) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   FusedSmem& sm = *reinterpret_cast<FusedSmem*>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -539,11 +546,16 @@ fused_narrow_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, const 
   }
   const uint32_t n_vars = sm.hdr.n_vars;
   const VarHdr vh0 = sm.hdr.var[0];
+  // status of a chunk handed to the general pair: not decoded yet (window mode: its first batch)
+  auto handed_over = [&]() -> uint32_t {
+    if constexpr (WIN) return win_first_batch(wins[blockIdx.x].lo, vh0.delta_order);
+    else return 0xffffffffu;
+  };
   // everything the general kernels serve is handed over untouched
   const bool candidate = n_vars == 1 && sm.hdr.mode == MODE_CLASSIC && vh0.n_bins >= 2 &&
                          task.entries_offset != 0 && index_base != nullptr;
   if (!candidate) {
-    if (tid == 0) { statuses[blockIdx.x] = 0xffffffffu; d_cls[blockIdx.x] = uint8_t(n_vars == 2 ? 2 : 1); }  // status: not decoded yet
+    if (tid == 0) { statuses[blockIdx.x] = handed_over(); d_cls[blockIdx.x] = uint8_t(n_vars == 2 ? 2 : 1); }
     return;
   }
   {
@@ -557,7 +569,7 @@ fused_narrow_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, const 
     return;
   }
   if (sm.hdr.var[0].max_offset_bits > NARROW_MAX_OB) {
-    if (tid == 0) { statuses[blockIdx.x] = 0xffffffffu; d_cls[blockIdx.x] = 1; }
+    if (tid == 0) { statuses[blockIdx.x] = handed_over(); d_cls[blockIdx.x] = 1; }
     return;
   }
   {
@@ -584,11 +596,19 @@ fused_narrow_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, const 
   }
   __syncthreads();  // q, nodes, base in place; the prologue scratch (aliased by ring, stage and windows) is dead
   if (sm.not_narrow) {
-    if (tid == 0) { statuses[blockIdx.x] = 0xffffffffu; d_cls[blockIdx.x] = 1; }
+    if (tid == 0) { statuses[blockIdx.x] = handed_over(); d_cls[blockIdx.x] = 1; }
     return;
   }
   const uint32_t n = sm.hdr.n;
-  const uint32_t n_out = task.out_offset >= out_len ? 0u : uint32_t(min(uint64_t(n), out_len - task.out_offset));
+  uint32_t n_out, first = 0;
+  WinTask win;
+  if constexpr (WIN) {
+    win = wins[blockIdx.x];
+    n_out = min(win.hi, n);
+    first = win_first_batch(win.lo, vh0.delta_order);
+  } else {
+    n_out = task.out_offset >= out_len ? 0u : uint32_t(min(uint64_t(n), out_len - task.out_offset));
+  }
   const uint32_t nb_total = n_batches_of(n), nb_out = n_batches_of(n_out);
   // an index that does not cover this chunk's batches cannot be walked (a stale or foreign index)
   if (task.entries_offset > index_len || uint64_t(nb_total) * sizeof(BatchEntry) > index_len - task.entries_offset) {
@@ -611,18 +631,18 @@ fused_narrow_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, const 
   if (role < FZ_WALKERS) {
     const BatchEntry* entries = reinterpret_cast<const BatchEntry*>(index_base + task.entries_offset);
     const uint32_t rep_log = min(5u, uint32_t(31 - __clz(uint32_t(FZ_NODE_WORDS) >> vh0.ans_size_log)));
-    fused_walker(sm, src, chunk_bit0, entries, nb_out, var_stored_n(n, K), vh0.ans_size_log, rep_log, role, lane);
+    fused_walker(sm, src, chunk_bit0, entries, first, nb_out, var_stored_n(n, K), vh0.ans_size_log, rep_log, role, lane);
   } else {
     const int d = role - FZ_WALKERS;
     switch (K) {
-      case 0: fused_decoder<L, 0>(sm, fp, src, task, chunk_bit0, out, n, n_out, d, lane); break;
-      case 1: fused_decoder<L, 1>(sm, fp, src, task, chunk_bit0, out, n, n_out, d, lane); break;
-      case 2: fused_decoder<L, 2>(sm, fp, src, task, chunk_bit0, out, n, n_out, d, lane); break;
-      case 3: fused_decoder<L, 3>(sm, fp, src, task, chunk_bit0, out, n, n_out, d, lane); break;
-      case 4: fused_decoder<L, 4>(sm, fp, src, task, chunk_bit0, out, n, n_out, d, lane); break;
-      case 5: fused_decoder<L, 5>(sm, fp, src, task, chunk_bit0, out, n, n_out, d, lane); break;
-      case 6: fused_decoder<L, 6>(sm, fp, src, task, chunk_bit0, out, n, n_out, d, lane); break;
-      default: fused_decoder<L, 7>(sm, fp, src, task, chunk_bit0, out, n, n_out, d, lane); break;
+      case 0: fused_decoder<L, 0, WIN>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane); break;
+      case 1: fused_decoder<L, 1, WIN>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane); break;
+      case 2: fused_decoder<L, 2, WIN>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane); break;
+      case 3: fused_decoder<L, 3, WIN>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane); break;
+      case 4: fused_decoder<L, 4, WIN>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane); break;
+      case 5: fused_decoder<L, 5, WIN>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane); break;
+      case 6: fused_decoder<L, 6, WIN>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane); break;
+      default: fused_decoder<L, 7, WIN>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane); break;
     }
   }
   __syncthreads();

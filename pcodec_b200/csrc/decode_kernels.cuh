@@ -114,6 +114,20 @@ __host__ __device__ inline uint64_t scratch_row0(uint64_t out_offset, uint32_t t
 __host__ __device__ inline uint64_t scratch_rows_total(uint64_t out_len, uint32_t n_tasks) { return uint64_t(MAX_VARS) * (out_len / BATCH_N + n_tasks + 1); }
 
 // ---------------------------------------------------------------------------
+// Window mode (the WIN instantiations, pco_b200_decompress_ranges): decode task t stores only the chunk's numbers [lo, hi), number lo
+// at address `dst`, and nothing else.  Its batches run from win_first_batch to ceil(hi / 256): a chunk of delta order 0 starts at
+// batch lo / 256 (every batch entry of the side index holds the batch's bit position and tANS states), higher orders at batch 0 (each
+// number depends on every earlier delta of the page, and a standalone chunk is one page).  The general pair places the task's
+// symbol and offset rows from row0 on: row (v, b) = row0 + v * (nb - first) + (b - first), nb = ceil(hi / 256).
+// ---------------------------------------------------------------------------
+struct WinTask {
+  uint32_t lo, hi;   // chunk-relative numbers to store
+  uint64_t dst;      // device address of number lo
+  uint64_t row0;     // general pair: first scratch row of the task
+};
+__device__ __forceinline__ uint32_t win_first_batch(uint32_t lo, uint32_t order) { return order == 0 ? lo / BATCH_N : 0u; }
+
+// ---------------------------------------------------------------------------
 // Chunk classes: symwalk_kernel parses and validates every chunk header anyway, so it also decides which decode
 // instantiation owns the chunk (d_cls, one byte per chunk): 1 / 2 = decode_kernel<L, 1 / 2> (any refusal is reported
 // by decode_kernel<L, 1>), 3 / 4 = decode_narrow_kernel (decode_narrow.cuh) with delta order 0 / 1.
@@ -810,6 +824,22 @@ __device__ __forceinline__ void store8(L* __restrict__ dst, const L (&r)[8]) {
     }
   }
 }
+// Window mode: the lane's 8 numbers of batch b (chunk numbers j0 .. j0 + 7) that fall inside the task's window.  A batch wholly inside
+// the window takes 16-byte stores when the address allows (the window may start at any element); the two edge batches store element
+// by element.
+template <typename L>
+__device__ __forceinline__ void win_store8(const WinTask& w, uint32_t b, int lane, const L (&r)[8]) {
+  L* __restrict__ out = reinterpret_cast<L*>(w.dst);
+  const uint32_t j0 = b * BATCH_N + uint32_t(lane) * 8;
+  const bool whole = b * BATCH_N >= w.lo && b * BATCH_N + BATCH_N <= w.hi;
+  if (whole && (reinterpret_cast<uintptr_t>(out + (j0 - w.lo)) & 15) == 0) {
+    store8<L>(out + (j0 - w.lo), r);
+  } else {
+#pragma unroll
+    for (int e = 0; e < 8; e++)
+      if (j0 + e >= w.lo && j0 + e < w.hi) out[j0 + e - w.lo] = r[e];
+  }
+}
 template <typename L>
 __device__ __forceinline__ void load8(const L* __restrict__ src, L (&r)[8]) {
   if (sizeof(L) == 8) {
@@ -890,9 +920,11 @@ struct SymWalkSmem {
   };
 };
 
+template <bool WIN = false>  // WIN: window mode, wins[t] says which numbers of task t are wanted (out_len is unused)
 __global__ void __launch_bounds__(SW_THREADS) symwalk_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, const uint8_t* __restrict__ index_base,
                                                               uint64_t index_len, uint64_t out_len, uint8_t* __restrict__ d_syms, uint32_t* __restrict__ d_offs,
-                                                              uint8_t* __restrict__ d_nvars, NarrowInfo* __restrict__ d_narrow, int classes_preset) {
+                                                              uint8_t* __restrict__ d_nvars, NarrowInfo* __restrict__ d_narrow, int classes_preset,
+                                                              const WinTask* __restrict__ wins = nullptr) {
   if (classes_preset && (d_nvars[blockIdx.x] & CLS_DONE)) return;  // fused_narrow_kernel has decoded (or refused) this chunk
   extern __shared__ __align__(16) unsigned char smem_raw[];
   SymWalkSmem& sm = *reinterpret_cast<SymWalkSmem*>(smem_raw);
@@ -964,20 +996,29 @@ __global__ void __launch_bounds__(SW_THREADS) symwalk_kernel(FileParams fp, cons
   }
   __syncthreads();  // the build scratch and plain tables (aliased by stage and tile) are dead
   const uint32_t n = sm.hdr.n;
-  const uint32_t n_out = task.out_offset >= out_len ? 0u : uint32_t(min(uint64_t(n), out_len - task.out_offset));
+  uint32_t n_out, first = 0;
+  uint64_t row0;
+  if constexpr (WIN) {
+    n_out = min(wins[blockIdx.x].hi, n);
+    first = win_first_batch(wins[blockIdx.x].lo, sm.hdr.var[0].delta_order);
+    row0 = wins[blockIdx.x].row0;
+  } else {
+    n_out = task.out_offset >= out_len ? 0u : uint32_t(min(uint64_t(n), out_len - task.out_offset));
+    row0 = scratch_row0(task.out_offset, blockIdx.x);
+  }
   const uint32_t nb_total = n_batches_of(n), nb_out = n_batches_of(n_out);
+  const uint32_t nb_rows = nb_out - first;  // batches walked, from `first` on
   const BatchEntry* entries = reinterpret_cast<const BatchEntry*>(index_base + task.entries_offset);
-  const uint64_t row0 = scratch_row0(task.out_offset, blockIdx.x);
-  const uint32_t groups = (nb_out + 31) / 32;
+  const uint32_t groups = (nb_rows + 31) / 32;
   uint32_t* stg = sm.w.stage[warp];
   uint32_t* tile = sm.w.tile[warp];
   const uint32_t stg_sa = uint32_t(__cvta_generic_to_shared(stg));
   for (uint32_t item = warp; item < n_vars * groups; item += SW_WARPS) {
-    const uint32_t v = item / groups, b0 = (item % groups) * 32;
+    const uint32_t v = item / groups, b0 = first + (item % groups) * 32;
     const VarHdr& vh = sm.hdr.var[v];
     const uint32_t stored = var_stored_n(n, vh.delta_order);
     const uint32_t nbg = min(32u, nb_out - b0);  // batches of this group
-    uint32_t* offs = d_offs + row0 + size_t(v) * nb_out;
+    uint32_t* offs = d_offs + row0 + size_t(v) * nb_rows - first;  // offs[b]: batch b >= first
     // lane k: entry of batch b0 + k
     BatchEntry e;
     e.bit_pos = 0; e.st[0] = e.st[1] = e.st[2] = e.st[3] = 0;
@@ -1003,7 +1044,7 @@ __global__ void __launch_bounds__(SW_THREADS) symwalk_kernel(FileParams fp, cons
       const uint32_t row_sa = smem_addr(row);
       const uint32_t* rowp = stg + lane * (SW_ROW_BLOCKS * 4);
       const uint32_t row_g = stg_sa + uint32_t(lane) * (SW_ROW_BLOCKS * 16);
-      uint8_t* sym_rows = d_syms + (row0 + size_t(v) * nb_out + b0) * BATCH_N;
+      uint8_t* sym_rows = d_syms + (row0 + size_t(v) * nb_rows + (b0 - first)) * BATCH_N;
       uint64_t bit = min(chunk_bit0 + e.bit_pos, src.n_bits);
       for (int part = 0; part < BATCH_N / SW_ROW_SYMS; part++) {
         const uint64_t blk = bit >> 7;
@@ -1097,11 +1138,12 @@ __global__ void __launch_bounds__(SW_THREADS) symwalk_kernel(FileParams fp, cons
 // NV = latent vars of the chunks this instantiation serves (1: classic, 2: int_mult / float_mult / float_quant); the
 // host launches both and a CTA leaves at once when its chunk belongs to the other (symwalk_kernel recorded each
 // chunk's var count) - one-var chunks then run with the registers of one var and a third CTA per SM.
-template <typename L, int NV>
+// WIN: window mode (symwalk_kernel<true> made the rows; wins[t] says which numbers of task t to store and where; out and out_len are unused).
+template <typename L, int NV, bool WIN = false>
 __global__ void __launch_bounds__(DEC_THREADS, NV == 1 ? PCOB_DEC_NV1_BLOCKS : 2)
 decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __restrict__ statuses, const uint8_t* __restrict__ index_base, uint64_t index_len,
               L* __restrict__ out, uint64_t out_len, const Binoms* __restrict__ binoms, const uint8_t* __restrict__ d_syms,
-              const uint32_t* __restrict__ d_offs, const uint8_t* __restrict__ d_nvars) {
+              const uint32_t* __restrict__ d_offs, const uint8_t* __restrict__ d_nvars, const WinTask* __restrict__ wins = nullptr) {
   if (d_nvars[blockIdx.x] != NV) return;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   DecodeSmem& sm = *reinterpret_cast<DecodeSmem*>(smem_raw);
@@ -1179,11 +1221,13 @@ decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __
   }
 
   const uint32_t n = sm.hdr.n;
-  // pco::standalone::simple_decompress_into semantics: emit only what fits in the destination
-  const uint32_t n_out = task.out_offset >= out_len ? 0u : uint32_t(min(uint64_t(n), out_len - task.out_offset));
+  // pco::standalone::simple_decompress_into semantics: emit only what fits in the destination (window mode: numbers below hi)
+  const uint32_t n_out = WIN ? min(wins[blockIdx.x].hi, n) : task.out_offset >= out_len ? 0u : uint32_t(min(uint64_t(n), out_len - task.out_offset));
   const uint32_t nb_total = n_batches_of(n);
   const uint32_t nb_out = n_batches_of(n_out);
   const uint32_t order = sm.hdr.var[0].delta_order;
+  const uint32_t first = WIN ? win_first_batch(wins[blockIdx.x].lo, order) : 0u;  // batches decoded: first .. nb_out - 1
+  const uint32_t nb_rows = nb_out - first;
   const bool need_index = (sm.hdr.var[0].n_bins > 1) || (n_vars > 1 && sm.hdr.var[1].n_bins > 1);
   const BatchEntry* entries = (task.entries_offset != 0 && index_base)
                                   ? reinterpret_cast<const BatchEntry*>(index_base + task.entries_offset) : nullptr;
@@ -1209,10 +1253,10 @@ decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __
   const int kind = is_float ? 2 : (is_signed ? 1 : 0);
   const uint32_t mode = sm.hdr.mode;
   uint32_t end_err = 0;
-  const uint64_t row0 = scratch_row0(task.out_offset, blockIdx.x);
+  const uint64_t row0 = WIN ? wins[blockIdx.x].row0 : scratch_row0(task.out_offset, blockIdx.x);
   // chunk-relative bit position of batch b's offsets section for var v
   auto off_of = [&](uint32_t v, uint32_t b) -> uint32_t {
-    if (need_index) return d_offs[row0 + size_t(v) * nb_out + b];
+    if (need_index) return d_offs[row0 + size_t(v) * nb_rows + (b - first)];
     // all vars trivial: batches before b contribute count0*ob0 + count1*ob1 bits
     const uint64_t c0 = min(uint64_t(b) * BATCH_N, uint64_t(stored0));
     const uint64_t c1 = min(uint64_t(b) * BATCH_N, uint64_t(stored1));
@@ -1245,20 +1289,21 @@ decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __
       for (uint32_t v = 0; v < NV; v++) {
         sy_nxt[v] = make_uint2(0u, 0u);
         if (v < n_vars && sm.hdr.var[v].n_bins > 1)
-          sy_nxt[v] = __ldg(reinterpret_cast<const uint2*>(d_syms + (row0 + size_t(v) * nb_out + b) * BATCH_N) + lane);
+          sy_nxt[v] = __ldg(reinterpret_cast<const uint2*>(d_syms + (row0 + size_t(v) * nb_rows + (b - first)) * BATCH_N) + lane);
       }
     };
-    if (uint32_t(warp) < nb_out) {
+    const uint32_t b_start = first + uint32_t(warp);
+    if (b_start < nb_out) {
 #pragma unroll
-      for (uint32_t v = 0; v < NV; v++) if (v < n_vars) off_cur[v] = off_of(v, warp);
+      for (uint32_t v = 0; v < NV; v++) if (v < n_vars) off_cur[v] = off_of(v, b_start);
       issue_window_loads(off_cur);
-      load_syms(warp);
-      if (uint32_t(warp) + DEC_WARPS < nb_out) {
+      load_syms(b_start);
+      if (b_start + DEC_WARPS < nb_out) {
 #pragma unroll
-        for (uint32_t v = 0; v < NV; v++) if (v < n_vars) off_nxt[v] = off_of(v, warp + DEC_WARPS);
+        for (uint32_t v = 0; v < NV; v++) if (v < n_vars) off_nxt[v] = off_of(v, b_start + DEC_WARPS);
       }
     }
-    for (uint32_t b = warp; b < nb_out; b += DEC_WARPS) {
+    for (uint32_t b = b_start; b < nb_out; b += DEC_WARPS) {
       const uint32_t out_cnt = min(uint32_t(BATCH_N), n_out - b * BATCH_N);  // numbers this batch emits
       __syncwarp();
 #pragma unroll
@@ -1468,7 +1513,9 @@ decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __
             res[e] = from_latent_kind<L>(L(L(pq << k) + lowest), 2);
           }
         }
-        if (out_cnt == BATCH_N && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+        if constexpr (WIN) {
+          win_store8<L>(wins[blockIdx.x], b, lane, res);
+        } else if (out_cnt == BATCH_N && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
           store8<L>(dst, res);  // 16-byte stores; a chunk that starts at an odd element offset takes the element-wise path
         } else {
 #pragma unroll

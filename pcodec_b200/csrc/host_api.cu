@@ -11,6 +11,7 @@
 #include "decode_cold.cuh"
 #include "files_kernels.cuh"
 #include "host_common.hpp"
+#include "ranges_kernels.cuh"
 #include "wrapped_kernels.cuh"
 
 namespace pcob200 {
@@ -28,6 +29,8 @@ struct Context {
   DevBuf src, out, index, statuses, misc, dec_syms, dec_offs, dec_narrow, gather, cold, spec;
   DevBuf wrap_metas, wrap_frames, wrap_tab, wrap_res, wrap_file, wrap_index, wrap_out;  // pco_b200_decompress_pages / pco_b200_compress_wrapped
   DevBuf files_tab, files_res, files_out, files_idx, files_arena, files_cold;            // pco_b200_compress_files / pco_b200_decompress_files
+  DevBuf rng_tab, rng_stage, rng_cold, rng_res, rng_copies;                             // pco_b200_decompress_ranges
+  bool ranges_attrs_set = false;
   CompressScratch enc;
   Binoms* d_binoms = nullptr;
   int sm_count = 0;
@@ -48,7 +51,7 @@ static Context& ctx() {
 static void release_buffers(Context& c) {
   for (DevBuf* b : {&c.src, &c.out, &c.index, &c.statuses, &c.misc, &c.dec_syms, &c.dec_offs, &c.dec_narrow, &c.gather, &c.cold, &c.spec, &c.wrap_metas, &c.wrap_frames,
                   &c.wrap_tab, &c.wrap_res, &c.wrap_file, &c.wrap_index, &c.wrap_out, &c.files_tab, &c.files_res, &c.files_out, &c.files_idx,
-                  &c.files_arena, &c.files_cold}) b->release();
+                  &c.files_arena, &c.files_cold, &c.rng_tab, &c.rng_stage, &c.rng_cold, &c.rng_res, &c.rng_copies}) b->release();
   c.enc.release();
   c.gather_err = nullptr;
   c.d_cls = nullptr;
@@ -70,6 +73,7 @@ static PcoB200Error ensure_device(Context& c) {
       c.initialized = false;
       c.device_ok = false;
       c.attrs_set = false;
+      c.ranges_attrs_set = false;
     }
   }
   if (!c.initialized) {
@@ -153,8 +157,8 @@ static PcoB200Error launch_decode(Context& c, const FileParams& fp, const uint8_
   const bool narrow_ok = true;  // the fused kernel serves every number width
   if (!c.attrs_set) {
     c.attrs_set = true;
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(symwalk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SymWalkSmem)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(symwalk_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(symwalk_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SymWalkSmem)));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(symwalk_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
     PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint64_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
     PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint32_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
     PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint64_t>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
@@ -930,6 +934,7 @@ void pco_b200_thread_release(void) {
     c.initialized = false;
     c.device_ok = false;
     c.attrs_set = false;
+    c.ranges_attrs_set = false;
   }
   readback_bounce().release();
 }
@@ -2216,6 +2221,390 @@ PcoB200Error pco_b200_decompress_files(const void* src, size_t src_len, const vo
                                                static_cast<cudaStream_t>(cuda_stream));
   profiler().resolve();
   return e;
+}
+
+// ---- ranges of an indexed standalone file (pco_b200_decompress_ranges)
+// A piece is the part of one range that lies in one chunk.  A task decodes one touched chunk, once, however many pieces it has: a
+// direct task (one piece) straight into the piece's place in the destination, a staged task (several pieces) as the window
+// [min lo, max hi) into a scratch slot, from which gather_ranges_kernel copies every piece to its place.
+struct RangePiece {
+  uint32_t chunk, task;
+  uint32_t lo, hi;    // chunk-relative numbers
+  uint64_t dst_off;   // element offset of number lo in dst
+  uint64_t range;     // the range it belongs to
+};
+struct RangeTask {
+  uint32_t chunk;
+  uint32_t lo, hi;          // the window: min lo and max hi of its pieces
+  uint32_t piece0, n_pieces;  // its pieces: pieces[by_chunk[piece0 .. piece0 + n_pieces)]
+  uint64_t first_range;     // the lowest-index range with numbers in the chunk
+};
+
+static PcoB200Error range_fail(PcoB200Error kind, uint64_t range, const std::string& what) {
+  return fail(kind, "range " + std::to_string(range) + ": " + what);
+}
+
+// Splits the ranges at chunk boundaries (a binary search over out_offset) and groups the pieces by chunk.  That search needs chunk
+// records that tile [0, n_total) in order, out_offset[k] = n[0] + ... + n[k - 1] with every n >= 1; an index is untrusted input, so
+// that is checked first.  Pieces come in range order, tasks in chunk order; *total = the sum of the counts.
+static PcoB200Error plan_ranges(const IndexChunk* recs, uint64_t n_chunks, uint64_t n_total, const PcoB200Range* ranges, size_t n_ranges,
+                                std::vector<RangePiece>& pieces, std::vector<RangeTask>& tasks, std::vector<uint32_t>& by_chunk, uint64_t* total) {
+  pieces.clear();
+  tasks.clear();
+  by_chunk.clear();
+  uint64_t sum = 0;
+  for (uint64_t k = 0; k < n_chunks; k++) {
+    if (recs[k].n == 0 || recs[k].out_offset != sum)
+      return fail(PCO_B200_INVALID_ARGUMENT, "side index: chunk " + std::to_string(k) + " does not start where the chunks before it end");
+    sum += recs[k].n;
+  }
+  if (sum != n_total)
+    return fail(PCO_B200_INVALID_ARGUMENT, "side index: its chunks hold " + std::to_string(sum) + " numbers, its header " + std::to_string(n_total));
+  uint64_t tot = 0;
+  for (size_t i = 0; i < n_ranges; i++) {
+    const uint64_t s = ranges[i].start, cnt = ranges[i].count;
+    if (cnt > n_total || s > n_total - cnt)
+      return range_fail(PCO_B200_INVALID_ARGUMENT, i, "start " + std::to_string(s) + " + count " + std::to_string(cnt) + " lies past the file's " +
+                                                          std::to_string(n_total) + " numbers");
+    if (cnt > ~uint64_t(0) - tot) return range_fail(PCO_B200_INVALID_ARGUMENT, i, "the counts add up to more than 2^64 numbers");
+    tot += cnt;
+  }
+  *total = tot;
+  uint64_t off = 0;
+  for (size_t i = 0; i < n_ranges; i++) {
+    uint64_t s = ranges[i].start, left = ranges[i].count;
+    while (left) {
+      uint64_t a = 0, b = n_chunks;  // the last chunk whose out_offset <= s
+      while (b - a > 1) {
+        const uint64_t m = a + (b - a) / 2;
+        if (recs[m].out_offset <= s) a = m;
+        else b = m;
+      }
+      const uint32_t lo = uint32_t(s - recs[a].out_offset);
+      const uint32_t take = uint32_t(std::min<uint64_t>(left, recs[a].n - lo));
+      pieces.push_back(RangePiece{uint32_t(a), 0, lo, lo + take, off, uint64_t(i)});
+      s += take;
+      left -= take;
+      off += take;
+    }
+  }
+  by_chunk.resize(pieces.size());
+  for (size_t p = 0; p < pieces.size(); p++) by_chunk[p] = uint32_t(p);
+  std::stable_sort(by_chunk.begin(), by_chunk.end(), [&](uint32_t x, uint32_t y) { return pieces[x].chunk < pieces[y].chunk; });
+  for (size_t p = 0; p < by_chunk.size();) {
+    RangeTask t{pieces[by_chunk[p]].chunk, ~0u, 0u, uint32_t(p), 0u, pieces[by_chunk[p]].range};  // stable: the first piece has the lowest range
+    size_t q = p;
+    for (; q < by_chunk.size() && pieces[by_chunk[q]].chunk == t.chunk; q++) {
+      RangePiece& pc = pieces[by_chunk[q]];
+      t.lo = std::min(t.lo, pc.lo);
+      t.hi = std::max(t.hi, pc.hi);
+      pc.task = uint32_t(tasks.size());
+    }
+    t.n_pieces = uint32_t(q - p);
+    tasks.push_back(t);
+    p = q;
+  }
+  return PCO_B200_OK;
+}
+
+static PcoB200Error decompress_ranges_impl(const void* compressed, size_t compressed_len, uint32_t dtype, const void* index, size_t index_len,
+                                           const PcoB200Range* ranges, size_t n_ranges, void* dst, size_t dst_len, size_t* n_written, uint32_t flags,
+                                           cudaStream_t stream) {
+  // ---- argument checks: host only, before any device work (headers in device memory are read back first)
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (n_written) *n_written = 0;
+  if (!index || index_len == 0) return fail(PCO_B200_INVALID_ARGUMENT, "a side index is required (pco_b200_build_index makes one)");
+  if (!ranges && n_ranges) return fail(PCO_B200_INVALID_ARGUMENT, "ranges are required");
+  if (n_ranges == 0) return PCO_B200_OK;
+  if (!compressed && compressed_len) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  const bool src_dev = flags & PCO_B200_SRC_ON_DEVICE, dst_dev = flags & PCO_B200_DST_ON_DEVICE, idx_dev = flags & PCO_B200_INDEX_ON_DEVICE;
+  const size_t elem = nt_bits(dtype) / 8;
+  Context& c = ctx();
+  if (src_dev || idx_dev)
+    if (PcoB200Error e = ensure_device(c)) return e;
+  // the file header and the index header: host copies, or one readback
+  uint8_t head[32] = {0};
+  const size_t avail = std::min<size_t>(compressed_len, sizeof(head));
+  IndexHeader ih;
+  std::memset(&ih, 0, sizeof(ih));
+  const bool ih_fits = index_len >= sizeof(IndexHeader);
+  bool need_sync = false;
+  if (avail) {
+    if (src_dev) { PCOB_CUDA_TRY(cudaMemcpyAsync(head, compressed, avail, cudaMemcpyDeviceToHost, stream)); need_sync = true; }
+    else std::memcpy(head, compressed, avail);
+  }
+  if (ih_fits) {
+    if (idx_dev) { PCOB_CUDA_TRY(cudaMemcpyAsync(&ih, index, sizeof(ih), cudaMemcpyDeviceToHost, stream)); need_sync = true; }
+    else std::memcpy(&ih, index, sizeof(ih));
+  }
+  if (need_sync) PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
+  StandaloneHeader hdr;
+  if (PcoB200Error e = parse_standalone_header(head, avail, compressed_len, &hdr)) return e;
+  // the same check as the side-index path of pco_b200_decompress_ex
+  if (!ih_fits || ih.magic != INDEX_MAGIC || ih.version != 1 || ih.file_len != compressed_len || ih.chunks_offset > index_len ||
+      ih.n_chunks > (index_len - ih.chunks_offset) / sizeof(IndexChunk))
+    return fail(PCO_B200_INVALID_ARGUMENT, "side index does not belong to this file");
+  if (ih.n_chunks > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "too many chunks");
+  // the chunk table: a host copy, or a second readback
+  std::vector<IndexChunk> recs(ih.n_chunks);
+  if (ih.n_chunks) {
+    const uint8_t* at = static_cast<const uint8_t*>(index) + ih.chunks_offset;
+    if (idx_dev) {
+      PCOB_CUDA_TRY(cudaMemcpyAsync(recs.data(), at, recs.size() * sizeof(IndexChunk), cudaMemcpyDeviceToHost, stream));
+      PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
+    } else {
+      std::memcpy(recs.data(), at, recs.size() * sizeof(IndexChunk));
+    }
+  }
+  std::vector<RangePiece> pieces;
+  std::vector<RangeTask> tasks;
+  std::vector<uint32_t> by_chunk;
+  uint64_t total = 0;
+  if (PcoB200Error e = plan_ranges(recs.data(), recs.size(), ih.n_total, ranges, n_ranges, pieces, tasks, by_chunk, &total)) return e;
+  if (total > dst_len) return fail(PCO_B200_INVALID_ARGUMENT, "dst holds " + std::to_string(dst_len) + " numbers, the ranges " + std::to_string(total));
+  if (total == 0) return PCO_B200_OK;
+  if (!dst) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (pieces.size() > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "the ranges make too many pieces");
+
+  // ---- the file, the index and the destination in HBM
+  if (PcoB200Error e = ensure_device(c)) return e;
+  const uint8_t* d_src = static_cast<const uint8_t*>(compressed);
+  if (!src_dev) {
+    PCOB_CUDA_TRY(c.src.reserve(compressed_len + 16));
+    PCOB_CUDA_TRY(copy_sliced(c.src.p, compressed, compressed_len, cudaMemcpyHostToDevice, stream));
+    d_src = c.src.as<uint8_t>();
+  }
+  const uint8_t* d_idx = static_cast<const uint8_t*>(index);
+  if (!idx_dev) {
+    PCOB_CUDA_TRY(c.index.reserve(index_len));
+    PCOB_CUDA_TRY(copy_sliced(c.index.p, index, index_len, cudaMemcpyHostToDevice, stream));
+    d_idx = c.index.as<uint8_t>();
+  }
+  uint8_t* d_out = static_cast<uint8_t*>(dst);
+  if (!dst_dev) {
+    PCOB_CUDA_TRY(c.out.reserve(total * elem + 64));
+    d_out = c.out.as<uint8_t>();
+  }
+  const FileParams fp{d_src, compressed_len, dtype, hdr.uniform_type, hdr.format_major};
+  const uint32_t T = uint32_t(tasks.size());
+  auto align16 = [](uint64_t x) { return (x + 15) & ~uint64_t(15); };
+  // scratch slots of the staged tasks
+  std::vector<uint64_t> slot(T, 0);
+  uint64_t stage_bytes = 0;
+  for (uint32_t t = 0; t < T; t++)
+    if (tasks[t].n_pieces > 1) {
+      slot[t] = stage_bytes;
+      stage_bytes += align16(uint64_t(tasks[t].hi - tasks[t].lo) * elem);
+    }
+  PCOB_CUDA_TRY(c.rng_stage.reserve(stage_bytes + 64));
+  uint8_t* d_stage = c.rng_stage.as<uint8_t>();
+  // task table: IndexChunk[T] (the chunks' own records) | WinTask[T]
+  const uint64_t wins_at = align16(uint64_t(T) * sizeof(IndexChunk));
+  PCOB_CUDA_TRY(c.rng_tab.reserve(wins_at + uint64_t(T) * sizeof(WinTask) + 64));
+  const IndexChunk* d_tasks = c.rng_tab.as<IndexChunk>();
+  WinTask* d_wins = reinterpret_cast<WinTask*>(c.rng_tab.as<uint8_t>() + wins_at);
+  std::vector<IndexChunk> trec(T);
+  std::vector<WinTask> wins(T);
+  for (uint32_t t = 0; t < T; t++) {
+    const RangeTask& k = tasks[t];
+    trec[t] = recs[k.chunk];
+    const uint8_t* at = k.n_pieces > 1 ? d_stage + slot[t] : d_out + pieces[by_chunk[k.piece0]].dst_off * elem;
+    wins[t] = WinTask{k.lo, k.hi, uint64_t(reinterpret_cast<uintptr_t>(at)), 0};
+  }
+  PCOB_CUDA_TRY(cudaMemcpyAsync(c.rng_tab.p, trec.data(), size_t(T) * sizeof(IndexChunk), cudaMemcpyHostToDevice, stream));
+  PCOB_CUDA_TRY(cudaMemcpyAsync(d_wins, wins.data(), size_t(T) * sizeof(WinTask), cudaMemcpyHostToDevice, stream));
+  // statuses and class bytes side by side: one readback brings both
+  const size_t res_bytes = (size_t(T) * (sizeof(uint32_t) + 1) + 3) & ~size_t(3);
+  PCOB_CUDA_TRY(c.statuses.reserve(res_bytes + 64));
+  uint32_t* d_st = c.statuses.as<uint32_t>();
+  uint8_t* d_cls = reinterpret_cast<uint8_t*>(d_st + T);
+  if (!c.ranges_attrs_set) {
+    c.ranges_attrs_set = true;
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(symwalk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SymWalkSmem)));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(symwalk_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint64_t, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint32_t, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint16_t, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint8_t, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint64_t, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint32_t, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint16_t, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint8_t, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+  }
+
+  // ---- 1. fused_narrow_kernel decodes the narrow chunks' windows and classifies the rest
+  profiler().begin("fused_narrow_kernel", stream);
+  dispatch_latent(dtype, [&](auto tag) {
+    using L = decltype(tag);
+    fused_narrow_kernel<L, true><<<T, FZ_THREADS, sizeof(FusedSmem), stream>>>(fp, d_tasks, d_idx, index_len, d_st, d_cls, nullptr, 0, d_wins);
+    return 0;
+  });
+  profiler().end(stream);
+  PCOB_CUDA_TRY(cudaGetLastError());
+  std::vector<uint32_t> res(res_bytes / 4);
+  PCOB_CUDA_TRY(readback_small_sync(res.data(), d_st, res_bytes, stream));
+  const uint8_t* cls = reinterpret_cast<const uint8_t*>(res.data() + T);
+  std::vector<uint32_t> st(T, ST_OK);
+  std::vector<uint32_t> general, cold;
+  uint64_t rows = 0;
+  for (uint32_t t = 0; t < T; t++) {
+    if (cls[t] & CLS_DONE) {
+      if (res[t] == ST_UNSUPPORTED) cold.push_back(t);
+      else st[t] = res[t];
+      continue;
+    }
+    // the general pair: the status word holds the task's first batch; it needs a row per var and batch from there on
+    general.push_back(t);
+    wins[t].row0 = rows;
+    rows += uint64_t(cls[t] == 2 ? 2 : 1) * (n_batches_of(tasks[t].hi) - std::min(res[t], n_batches_of(tasks[t].hi)));
+  }
+
+  // ---- 2. symwalk_kernel + decode_kernel for the others
+  if (!general.empty()) {
+    PCOB_CUDA_TRY(c.dec_syms.reserve(rows * BATCH_N + 64));
+    PCOB_CUDA_TRY(c.dec_offs.reserve(rows * sizeof(uint32_t) + 64));
+    PCOB_CUDA_TRY(cudaMemcpyAsync(d_wins, wins.data(), size_t(T) * sizeof(WinTask), cudaMemcpyHostToDevice, stream));
+    profiler().begin("symwalk_kernel", stream);
+    symwalk_kernel<true><<<T, SW_THREADS, sizeof(SymWalkSmem), stream>>>(fp, d_tasks, d_idx, index_len, 0, c.dec_syms.as<uint8_t>(), c.dec_offs.as<uint32_t>(),
+                                                                          d_cls, nullptr, 1, d_wins);
+    profiler().end(stream);
+    profiler().begin("decode_kernel", stream);
+    dispatch_latent(dtype, [&](auto tag) {
+      using L = decltype(tag);
+      decode_kernel<L, 1, true><<<T, DEC_THREADS, sizeof(DecodeSmem), stream>>>(fp, d_tasks, d_st, d_idx, index_len, nullptr, 0, c.d_binoms,
+                                                                                c.dec_syms.as<uint8_t>(), c.dec_offs.as<uint32_t>(), d_cls, d_wins);
+      decode_kernel<L, 2, true><<<T, DEC_THREADS, sizeof(DecodeSmem), stream>>>(fp, d_tasks, d_st, d_idx, index_len, nullptr, 0, c.d_binoms,
+                                                                                c.dec_syms.as<uint8_t>(), c.dec_offs.as<uint32_t>(), d_cls, d_wins);
+      return 0;
+    });
+    profiler().end(stream);
+    PCOB_CUDA_TRY(cudaGetLastError());
+    PCOB_CUDA_TRY(readback_small_sync(res.data(), d_st, size_t(T) * sizeof(uint32_t), stream));
+    for (uint32_t t : general) {
+      if (res[t] == ST_UNSUPPORTED) cold.push_back(t);
+      else st[t] = res[t];
+    }
+  }
+
+  // ---- 3. chunks only the catch-all decoder takes: one single-thread launch per chunk, from the chunk's start to max hi, into a slot
+  // of its own.  It stops there (ST_DST_FULL) or, when the window reaches the chunk's end, behind the chunk: the chunk is decoded once
+  // the decoder has counted it.
+  std::vector<uint64_t> cold_slot(T, 0);
+  uint8_t* d_cold = nullptr;
+  if (!cold.empty()) {
+    std::sort(cold.begin(), cold.end());
+    uint64_t cold_bytes = 0;
+    for (uint32_t t : cold) {
+      cold_slot[t] = cold_bytes;
+      cold_bytes += align16(uint64_t(tasks[t].hi) * elem);
+    }
+    PCOB_CUDA_TRY(c.rng_cold.reserve(cold_bytes + 64));
+    d_cold = c.rng_cold.as<uint8_t>();
+    const size_t nc = cold.size();
+    PCOB_CUDA_TRY(c.rng_res.reserve(nc * sizeof(ColdResult) + 64));
+    ColdResult* d_cres = c.rng_res.as<ColdResult>();
+    std::vector<ColdResult> cres(nc);
+    std::vector<size_t> todo(nc);
+    for (size_t k = 0; k < nc; k++) todo[k] = k;
+    for (uint32_t window_cap : {16u, COLD_MAX_WINDOW_LOG}) {  // lookback windows beyond 2^16 numbers get the large scratch on a second pass
+      if (todo.empty()) break;
+      PCOB_CUDA_TRY(c.cold.reserve(cold_scratch_bytes(window_cap)));
+      profiler().begin("cold_decode_kernel", stream);
+      for (size_t k : todo) {
+        const uint32_t t = cold[k];
+        dispatch_latent(dtype, [&](auto tag) {
+          using L = decltype(tag);
+          cold_decode_kernel<L><<<1, 32, 0, stream>>>(fp, trec[t].chunk_offset, reinterpret_cast<L*>(d_cold + cold_slot[t]), tasks[t].hi, c.cold.as<uint8_t>(),
+                                                      window_cap, d_cres + k);
+          return 0;
+        });
+      }
+      profiler().end(stream);
+      PCOB_CUDA_TRY(cudaGetLastError());
+      PCOB_CUDA_TRY(readback_small_sync(cres.data(), d_cres, nc * sizeof(ColdResult), stream));
+      std::vector<size_t> again;
+      for (size_t k : todo)
+        if (cres[k].n_chunks == 0 && cres[k].status == ST_UNSUPPORTED) again.push_back(k);
+      todo.swap(again);
+    }
+    for (size_t k = 0; k < nc; k++) {
+      const uint32_t s = cres[k].status;
+      st[cold[k]] = cres[k].n_chunks > 0 ? ST_OK : (s == ST_OK || s == ST_TERMINATOR || s == ST_DST_FULL) ? ST_CORRUPTION : s;
+    }
+  }
+
+  // ---- a failing chunk fails the call, named by the lowest-index range with numbers in it
+  {
+    uint32_t worst = T;
+    for (uint32_t t = 0; t < T; t++)
+      if (st[t] != ST_OK && (worst == T || tasks[t].first_range < tasks[worst].first_range)) worst = t;
+    if (worst < T) {
+      const PcoB200Error e = status_to_error(st[worst], ("chunk " + std::to_string(tasks[worst].chunk)).c_str());
+      return range_fail(e, tasks[worst].first_range, last_error_ref());
+    }
+  }
+
+  // ---- 4. pieces of staged and catch-all tasks: slot -> destination
+  std::vector<RangeCopy> copies;
+  for (uint32_t t = 0; t < T; t++) {
+    const RangeTask& k = tasks[t];
+    const bool is_cold = d_cold && std::binary_search(cold.begin(), cold.end(), t);
+    if (k.n_pieces == 1 && !is_cold) continue;
+    const uint8_t* base = is_cold ? d_cold + cold_slot[t] : d_stage + slot[t];
+    const uint32_t wlo = is_cold ? 0u : k.lo;
+    for (uint32_t q = 0; q < k.n_pieces; q++) {
+      const RangePiece& p = pieces[by_chunk[k.piece0 + q]];
+      copies.push_back(RangeCopy{uint64_t(reinterpret_cast<uintptr_t>(base + uint64_t(p.lo - wlo) * elem)),
+                                 uint64_t(reinterpret_cast<uintptr_t>(d_out + p.dst_off * elem)), uint64_t(p.hi - p.lo) * elem});
+    }
+  }
+  if (!copies.empty()) {
+    PCOB_CUDA_TRY(c.rng_copies.reserve(copies.size() * sizeof(RangeCopy) + 64));
+    PCOB_CUDA_TRY(cudaMemcpyAsync(c.rng_copies.p, copies.data(), copies.size() * sizeof(RangeCopy), cudaMemcpyHostToDevice, stream));
+    profiler().begin("gather_ranges_kernel", stream);
+    gather_ranges_kernel<<<uint32_t(copies.size()), RANGES_THREADS, 0, stream>>>(c.rng_copies.as<RangeCopy>());
+    profiler().end(stream);
+    PCOB_CUDA_TRY(cudaGetLastError());
+  }
+  if (!dst_dev) PCOB_CUDA_TRY(copy_sliced(dst, d_out, total * elem, cudaMemcpyDeviceToHost, stream));
+  PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
+  if (n_written) *n_written = size_t(total);
+  return PCO_B200_OK;
+}
+
+PcoB200Error pco_b200_decompress_ranges(const void* compressed, size_t compressed_len, unsigned char dtype, const void* index, size_t index_len,
+                                        const PcoB200Range* ranges, size_t n_ranges, void* dst, size_t dst_len, size_t* n_written, uint32_t flags,
+                                        void* cuda_stream) {
+  const PcoB200Error e = decompress_ranges_impl(compressed, compressed_len, dtype, index, index_len, ranges, n_ranges, dst, dst_len, n_written, flags,
+                                                static_cast<cudaStream_t>(cuda_stream));
+  profiler().resolve();
+  return e;
+}
+
+PcoB200Error pco_b200_debug_plan_ranges(const void* chunk_table, size_t n_chunks, uint64_t n_total, const PcoB200Range* ranges, size_t n_ranges,
+                                        uint64_t* pieces_out, size_t pieces_cap, size_t* n_pieces, uint64_t* tasks_out, size_t tasks_cap, size_t* n_tasks) {
+  if ((!chunk_table && n_chunks) || (!ranges && n_ranges)) return fail(PCO_B200_INVALID_ARGUMENT, "null table");
+  std::vector<IndexChunk> recs(n_chunks);
+  if (n_chunks) std::memcpy(recs.data(), chunk_table, n_chunks * sizeof(IndexChunk));
+  std::vector<RangePiece> pieces;
+  std::vector<RangeTask> tasks;
+  std::vector<uint32_t> by_chunk;
+  uint64_t total = 0;
+  if (PcoB200Error e = plan_ranges(recs.data(), n_chunks, n_total, ranges, n_ranges, pieces, tasks, by_chunk, &total)) return e;
+  if (n_pieces) *n_pieces = pieces.size();
+  if (n_tasks) *n_tasks = tasks.size();
+  if (pieces.size() > pieces_cap || tasks.size() > tasks_cap) return fail(PCO_B200_IO, "the tables are too small");
+  for (size_t p = 0; p < pieces.size(); p++) {
+    const RangePiece& x = pieces[p];
+    const uint64_t row[6] = {x.chunk, x.lo, x.hi, x.dst_off, x.range, x.task};
+    std::memcpy(pieces_out + 6 * p, row, sizeof(row));
+  }
+  for (size_t t = 0; t < tasks.size(); t++) {
+    const RangeTask& x = tasks[t];
+    const uint64_t row[6] = {x.chunk, x.lo, x.hi, x.n_pieces, x.first_range, x.n_pieces > 1 ? 1u : 0u};
+    std::memcpy(tasks_out + 6 * t, row, sizeof(row));
+  }
+  return PCO_B200_OK;
 }
 
 PcoB200Error pco_b200_build_index(const void* compressed, size_t compressed_len, unsigned char dtype, void* index, size_t index_cap,

@@ -327,6 +327,64 @@ def decompress_files(data, files, dtype, index=None):
         return dst[: nw.value], file_ns[:nf].copy()
 
 
+# PcoB200Range (include/pco_b200.h): numbers [start, start + count) of a file
+RANGE = np.dtype([("start", "<u8"), ("count", "<u8")])
+
+
+def _ranges_array(ranges):
+    a = np.asarray(ranges)
+    if a.dtype.names:
+        return np.ascontiguousarray(a.astype(RANGE, copy=False)).reshape(-1)
+    a = a.reshape(-1, 2) if a.size else a.reshape(0, 2)
+    if a.dtype.kind not in "iu":
+        raise TypeError(f"ranges must be integers, got {a.dtype}")
+    if a.dtype.kind == "i" and a.size and a.min() < 0:
+        raise ValueError("ranges must not be negative")
+    r = np.zeros(a.shape[0], dtype=RANGE)
+    r["start"], r["count"] = a[:, 0], a[:, 1]
+    return r
+
+
+def decompress_ranges(data, dtype, index, ranges):
+    """Decodes ranges of numbers of one standalone file (pco_b200_decompress_ranges): range i lands right behind range i - 1.  Only
+    the chunks a range touches are decoded, and in chunks of delta order 0 only the batches it touches.  `ranges` is a numpy array of
+    RANGE records or an (m, 2) integer array of (start, count); ranges may overlap, repeat and come in any order.  `index` is the
+    file's side index; index=None builds it first with build_index, which walks the whole file serially on the device (keep the index
+    from compress for repeated reads).  `data` and `index` are bytes / numpy, or torch CUDA tensors (then the result is a CUDA tensor,
+    computed on the current stream)."""
+    from .wrapped import _host_u8, _torch_dtypes
+
+    dt = np.dtype(dtype)
+    r = _ranges_array(ranges)
+    total = int(r["count"].sum(dtype=np.uint64)) if r.size else 0
+    L = _lib.lib()
+    nw = C.c_size_t()
+    if _is_cuda(data):
+        import torch
+
+        d = data.contiguous().reshape(-1)
+        if index is None:
+            index = torch.as_tensor(np.frombuffer(build_index(d.cpu().numpy().tobytes(), dt), np.uint8).copy(), device=d.device)
+        ix = index.contiguous().reshape(-1) if _is_cuda(index) else torch.as_tensor(_host_u8(index).copy(), device=d.device)
+        dst = torch.empty(max(total, 1), dtype=_torch_dtypes()[dt], device=d.device)
+        flags = _lib.SRC_ON_DEVICE | _lib.DST_ON_DEVICE | _INDEX_ON_DEVICE
+        rc = L.pco_b200_decompress_ranges(C.c_void_p(d.data_ptr()), C.c_size_t(d.numel()), C.c_ubyte(_lib.dtype_byte(dt)), C.c_void_p(ix.data_ptr()),
+                                          C.c_size_t(ix.numel()), r.ctypes.data_as(C.c_void_p), C.c_size_t(r.size), C.c_void_p(dst.data_ptr()),
+                                          C.c_size_t(total), C.byref(nw), C.c_uint32(flags), _stream_of(d))
+        _lib.check(rc)
+        return dst[: nw.value]
+    d = _host_u8(data)
+    if index is None:
+        index = build_index(d.tobytes(), dt)
+    ix = _host_u8(index)
+    dst = np.empty(max(total, 1), dtype=dt)
+    rc = L.pco_b200_decompress_ranges(d.ctypes.data_as(C.c_void_p), C.c_size_t(d.size), C.c_ubyte(_lib.dtype_byte(dt)), ix.ctypes.data_as(C.c_void_p),
+                                      C.c_size_t(ix.size), r.ctypes.data_as(C.c_void_p), C.c_size_t(r.size), dst.ctypes.data_as(C.c_void_p),
+                                      C.c_size_t(total), C.byref(nw), C.c_uint32(0), None)
+    _lib.check(rc)
+    return dst[: nw.value]
+
+
 class _CModeChoice(C.Structure):
     _fields_ = [("mode_spec", C.c_uint32), ("float_quant_k", C.c_uint32), ("float_mult_base", C.c_double), ("float_mult_inv_base", C.c_double),
                 ("int_mult_base", C.c_uint64), ("bits_saved_per_num", C.c_double)]
