@@ -344,6 +344,67 @@ PcoB200Error pco_b200_debug_plan_ranges(const void *chunk_table, size_t n_chunks
                                         size_t n_ranges, uint64_t *pieces_out, size_t pieces_cap, size_t *n_pieces,
                                         uint64_t *tasks_out, size_t tasks_cap, size_t *n_tasks);
 
+/* ---- asynchronous decompress of an indexed standalone file (no reference counterpart).  Every other device entry point returns once
+ * its work is done; this one only enqueues kernels on the caller's stream and returns at once, so it can be queued behind other GPU
+ * work while the host moves on, and captured in a CUDA graph.  It makes no synchronising or allocating CUDA call and refers to no
+ * memory of the library's per-thread scratch: a captured call may be replayed after pco_b200_thread_release or after any other call.
+ * A plan, made once outside any capture, fixes what the launches need by value; the file length, chunk count and n_total come from
+ * the side index on the device, so one plan (and one captured graph) decodes a different file of the same number type and header
+ * flavour on each call.  Device buffers only; the host reads the outcome back when it chooses. */
+typedef struct PcoB200AsyncPlan {      /* filled by pco_b200_decompress_async_plan; treat as opaque */
+  uint32_t dtype, uniform_type, format_major, reserved;
+  uint64_t src_cap, index_cap, dst_cap, max_chunks;
+  uint64_t workspace_bytes;            /* device workspace one in-flight call needs */
+} PcoB200AsyncPlan;
+
+typedef struct PcoB200AsyncStatus {    /* written on the device by every call */
+  uint32_t kind;                       /* PcoB200Error */
+  uint32_t device_status;              /* the device word behind it (for the message): a PcoB200Error kind of a chunk, or PCO_B200_ASYNC_* */
+  uint64_t chunk;                      /* lowest failing chunk, when kind != OK (UINT64_MAX for a PCO_B200_ASYNC_* refusal) */
+  uint64_t n_processed;                /* Progress, as pco_b200_decompress_ex reports it */
+  uint32_t finished;
+  uint32_t n_chunks;                   /* chunks in the file's side index (0 when the file was refused before decoding) */
+} PcoB200AsyncStatus;
+
+/* device_status of a file refused before any chunk is decoded */
+enum {
+  PCO_B200_ASYNC_HEADER_CORRUPT = 0x101,   /* the standalone header is corrupt (PCO_B200_CORRUPTION) */
+  PCO_B200_ASYNC_HEADER_SHORT = 0x102,     /* the file ends inside its standalone header (PCO_B200_INSUFFICIENT_DATA) */
+  PCO_B200_ASYNC_HEADER_MISMATCH = 0x103,  /* its uniform type or format major differs from the plan's (PCO_B200_INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_INDEX_FOREIGN = 0x104,    /* the side index does not belong to the file, or its file length exceeds src_cap (INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_TOO_MANY_CHUNKS = 0x105   /* the side index lists more than max_chunks chunks (PCO_B200_INVALID_ARGUMENT) */
+};
+
+/* Makes a plan.  `head` holds the first bytes of a standalone file in host memory (32 bytes, or the whole file if shorter, always
+ * suffice); the plan takes dtype, the header's uniform type and its format major from it.  src_cap, index_cap and dst_cap are the byte
+ * sizes of the file and index buffers and the element count of the destination that every call will pass; max_chunks bounds the
+ * chunks of any file decoded with the plan.  Checked before the device is touched: an unknown dtype (PCO_B200_INVALID_TYPE), a header
+ * that does not parse (the kind pco_b200_decompress_ex gives), a nonzero uniform type other than dtype and a max_chunks of 0 or above
+ * 2^32 - 1 (PCO_B200_INVALID_ARGUMENT).  Then *plan is filled, workspace_bytes included, and the one-time device set-up runs on the
+ * current device, which the calls must use; without a device that is PCO_B200_CUDA.  workspace_bytes grows with dst_cap and max_chunks
+ * (about 2.03 bytes per number of dst_cap and 557 bytes per chunk of max_chunks, plus 3.7 MB for the catch-all decoder). */
+PcoB200Error pco_b200_decompress_async_plan(const void *head, size_t head_len, unsigned char dtype,
+                                            size_t src_cap, size_t index_cap, size_t dst_cap, size_t max_chunks,
+                                            PcoB200AsyncPlan *plan);
+/* Enqueues the decode of the file in `src` through its side index `index` (as pco_b200_compress_ex or pco_b200_build_index write it)
+ * into `dst` on `cuda_stream`, and the outcome into *status; returns without waiting.  src, index, dst, workspace (plan->workspace_bytes,
+ * any 256-byte aligned device buffer) and status are device pointers; one workspace serves one call in flight, so calls on different
+ * streams need workspaces of their own.  Valid files decode to the numbers pco_b200_decompress_ex gives, whatever the spare capacity;
+ * a short dst_cap gives its Progress and its numbers.  Reads stay inside src_cap bytes of src and index_cap bytes of index, writes
+ * inside dst_cap numbers of dst.  The file length the index records must be at most src_cap, and a file of more than max_chunks chunks
+ * is refused (PCO_B200_INVALID_ARGUMENT) without a write to dst.  When src_cap equals the file's length, every error kind is the one
+ * pco_b200_decompress_ex gives for a single damaged chunk; with spare capacity a damaged chunk can read the stale bytes behind the file,
+ * which are still inside the buffer, and fail with another kind.  The return value covers the host side only: null pointers or a plan
+ * that was not filled (PCO_B200_INVALID_ARGUMENT), a launch the runtime refuses (PCO_B200_CUDA).  Chunks the fast kernels decline
+ * (tables above 2^10 states or 256 bins, f16 FloatMult) are decoded by the single-thread catch-all decoder; a Lookback window beyond
+ * 2^16 numbers is PCO_B200_UNSUPPORTED here.  With pco_b200_profile_enable(1), a call outside a stream capture records its kernel spans
+ * for pco_b200_profile_last (which then waits for them); a call inside a capture records none. */
+PcoB200Error pco_b200_decompress_async(const PcoB200AsyncPlan *plan, const void *src, const void *index, void *dst,
+                                       void *workspace, PcoB200AsyncStatus *status, void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory at a point of the caller's choosing.  Returns the kind,
+ * sets the last-error message ("chunk 17: ...") and, when the kind is OK, fills *progress (may be NULL). */
+PcoB200Error pco_b200_decompress_async_result(const PcoB200AsyncStatus *host_status, PcoB200Progress *progress);
+
 #if defined(__cplusplus)
 }
 #endif

@@ -278,11 +278,11 @@ __device__ inline uint32_t cold_join(const ColdChunk& ch, const ColdReader& r0, 
   return ST_OK;
 }
 
-// One thread decodes the file from `first_chunk_byte` on.  scratch: cold_scratch_bytes(COLD window cap) bytes.
+// The decoder one thread runs: the chunks from `first_chunk_byte` on, into out[0, out_len).  scratch: cold_scratch_bytes(COLD window cap)
+// bytes.  cold_decode_kernel runs it over a whole file; cold_chunks_kernel (async_kernels.cuh) over one chunk at a time.
 template <typename L>
-__global__ void cold_decode_kernel(FileParams fp, uint64_t first_chunk_byte, L* __restrict__ out, uint64_t out_len, uint8_t* __restrict__ scratch,
-                                   uint32_t window_log_cap, ColdResult* __restrict__ result) {
-  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+__device__ __forceinline__ void cold_decode_run(const FileParams& fp, uint64_t first_chunk_byte, L* __restrict__ out, uint64_t out_len,
+                                                uint8_t* __restrict__ scratch, uint32_t window_log_cap, ColdResult* __restrict__ result) {
   const BitSrc src = make_bitsrc(fp.src, fp.src_len);
   ColdReader r{src, src.mis_bits + first_chunk_byte * 8};
   // carve the scratch
@@ -498,6 +498,14 @@ __global__ void cold_decode_kernel(FileParams fp, uint64_t first_chunk_byte, L* 
   result->n_chunks = n_chunks;
   result->n_total = out_off;
   result->next_byte = (r.bit - src.mis_bits) >> 3;
+}
+
+// One thread decodes the file from `first_chunk_byte` on.  scratch: cold_scratch_bytes(COLD window cap) bytes.
+template <typename L>
+__global__ void cold_decode_kernel(FileParams fp, uint64_t first_chunk_byte, L* __restrict__ out, uint64_t out_len, uint8_t* __restrict__ scratch,
+                                   uint32_t window_log_cap, ColdResult* __restrict__ result) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  cold_decode_run<L>(fp, first_chunk_byte, out, out_len, scratch, window_log_cap, result);
 }
 
 }  // namespace pcob200

@@ -3,6 +3,7 @@
 // compute entry point fails with PCO_B200_CUDA.
 #include <algorithm>
 
+#include "async_kernels.cuh"
 #include "compress_host.cuh"
 #include "decode_kernels.cuh"
 #include "decode_narrow.cuh"
@@ -132,6 +133,23 @@ struct DecodeOutcome {
   bool terminated = false;
 };
 
+// Shared-memory attributes of the decode kernels, set once per context before their first launch.
+static PcoB200Error set_decode_attrs(Context& c) {
+  if (c.attrs_set) return PCO_B200_OK;
+  c.attrs_set = true;
+  PCOB_CUDA_TRY(cudaFuncSetAttribute(symwalk_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SymWalkSmem)));
+  PCOB_CUDA_TRY(cudaFuncSetAttribute(symwalk_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+  PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint64_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint32_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint64_t>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+  PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint32_t>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+  PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint16_t>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+  PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint8_t>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+  return PCO_B200_OK;
+}
+
 // Launch the decode over `n_chunks` IndexChunk records that live on the device.
 //   1. fused_narrow_kernel (decode_fused.cuh): parses and classifies every chunk and fully decodes the narrow class;
 //   2. only if some chunk is of another class: symwalk_kernel + decode_kernel<L, 1 / 2> for those.
@@ -155,19 +173,7 @@ static PcoB200Error launch_decode(Context& c, const FileParams& fp, const uint8_
   const IndexChunk* d_chunks = reinterpret_cast<const IndexChunk*>(d_index + chunks_offset);
   static const bool use_fused = [] { const char* e = std::getenv("PCOB200_FUSED"); return !(e && e[0] == '0'); }();
   const bool narrow_ok = true;  // the fused kernel serves every number width
-  if (!c.attrs_set) {
-    c.attrs_set = true;
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(symwalk_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SymWalkSmem)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(symwalk_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint64_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint32_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint64_t>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint32_t>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint16_t>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint8_t>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-  }
+  if (PcoB200Error e = set_decode_attrs(c)) return e;
   c.last_decode_chunks = n_chunks;
   const uint32_t* st = static_cast<const uint32_t*>(c.pinned_res);
   bool fused_ran = false;
@@ -962,6 +968,7 @@ int pco_b200_profile_ans_paths(unsigned* counts8) {
 }
 // Copies "name=ms;name=ms;..." of the last finished call into buf; returns the number of spans.
 int pco_b200_profile_last(char* buf, size_t cap) {
+  if (!profiler().spans.empty()) profiler().resolve();  // an asynchronous call leaves its spans pending: wait for them here
   std::string s;
   for (auto& kv : profiler().last) s += kv.first + "=" + std::to_string(kv.second) + ";";
   if (cap) {
@@ -2605,6 +2612,143 @@ PcoB200Error pco_b200_debug_plan_ranges(const void* chunk_table, size_t n_chunks
     std::memcpy(tasks_out + 6 * t, row, sizeof(row));
   }
   return PCO_B200_OK;
+}
+
+// ---- asynchronous decompress of an indexed standalone file (pco_b200_decompress_async; kernels in async_kernels.cuh)
+// The plan fixes what the launches take by value (FileParams' number type, uniform type and format major) and every grid size (from
+// max_chunks); the file's own length, chunk count and n_total are read from its side index on the device.  So a call is a fixed
+// sequence of seven launches and nothing else: check, fused, symwalk, decode<1>, decode<2>, cold, finish.  A kernel that has nothing
+// to do for a chunk leaves at its first line.
+
+PcoB200Error pco_b200_decompress_async_plan(const void* head, size_t head_len, unsigned char dtype, size_t src_cap, size_t index_cap, size_t dst_cap,
+                                            size_t max_chunks, PcoB200AsyncPlan* plan) {
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (!plan || (!head && head_len)) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  StandaloneHeader hdr;
+  if (PcoB200Error e = parse_standalone_header(static_cast<const uint8_t*>(head), std::min<size_t>(head_len, 32), head_len, &hdr)) return e;
+  if (hdr.uniform_type != 0 && hdr.uniform_type != dtype)
+    return fail(PCO_B200_INVALID_ARGUMENT, "the header's uniform type " + std::to_string(hdr.uniform_type) + " is not dtype " + std::to_string(dtype));
+  if (max_chunks == 0 || uint64_t(max_chunks) > 0xffffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_chunks must be 1 .. 2^32 - 1");
+  if (uint64_t(dst_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "dst_cap above 2^56 numbers");
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->uniform_type = hdr.uniform_type;
+  plan->format_major = hdr.format_major;
+  plan->src_cap = src_cap;
+  plan->index_cap = index_cap;
+  plan->dst_cap = dst_cap;
+  plan->max_chunks = max_chunks;
+  plan->workspace_bytes = async_layout(dst_cap, uint32_t(max_chunks)).total;
+  // the one-time device set-up, here and not in a call (which may be inside a capture): the decode kernels' attributes, and every kernel
+  // the call launches loaded now (with lazy module loading a kernel is otherwise loaded at its first launch)
+  Context& c = ctx();
+  if (PcoB200Error e = ensure_device(c)) return e;
+  if (PcoB200Error e = set_decode_attrs(c)) return e;
+  cudaFuncAttributes fa;
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, async_check_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, async_finish_kernel));
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
+    using L = decltype(tag);
+    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, fused_narrow_kernel<L>));
+    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, decode_kernel<L, 1>));
+    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, decode_kernel<L, 2>));
+    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, cold_chunks_kernel<L>));
+    return PCO_B200_OK;
+  });
+}
+
+PcoB200Error pco_b200_decompress_async(const PcoB200AsyncPlan* plan, const void* src, const void* index, void* dst, void* workspace,
+                                       PcoB200AsyncStatus* status, void* cuda_stream) {
+  if (!plan || !src || !index || !workspace || !status || (!dst && plan->dst_cap)) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (!nt_valid(plan->dtype) || plan->max_chunks == 0 || plan->max_chunks > 0xffffffffull || plan->dst_cap > (uint64_t(1) << 56) ||
+      plan->workspace_bytes != async_layout(plan->dst_cap, uint32_t(plan->max_chunks)).total)
+    return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_decompress_async_plan");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  PCOB_CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
+  // kernel spans only outside a capture (an event record would become part of the graph); those of an earlier call that nobody read go
+  const bool prof = cap == cudaStreamCaptureStatusNone && profiler_enabled().load(std::memory_order_relaxed);
+  if (prof) profiler().discard();
+  auto begin = [&](const char* name) { if (prof) profiler().begin(name, stream); };
+  auto end = [&]() { if (prof) profiler().end(stream); };
+
+  const uint32_t mc = uint32_t(plan->max_chunks);
+  const AsyncLayout lay = async_layout(plan->dst_cap, mc);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  AsyncCheck* chk = reinterpret_cast<AsyncCheck*>(ws);
+  IndexChunk* table = reinterpret_cast<IndexChunk*>(ws + lay.table);
+  uint32_t* d_st = reinterpret_cast<uint32_t*>(ws + lay.st);
+  uint8_t* d_cls = ws + lay.cls;
+  uint8_t* d_syms = ws + lay.syms;
+  uint32_t* d_offs = reinterpret_cast<uint32_t*>(ws + lay.offs);
+  uint8_t* d_cold = ws + lay.cold;
+  const uint8_t* d_idx = static_cast<const uint8_t*>(index);
+  AsyncArgs a;
+  a.fp = FileParams{src, plan->src_cap, plan->dtype, plan->uniform_type, plan->format_major};
+  a.index = d_idx;
+  a.index_cap = plan->index_cap;
+  a.dst_cap = plan->dst_cap;
+  a.max_chunks = mc;
+
+  begin("async_check_kernel");
+  async_check_kernel<<<(mc + ASYNC_CHECK_RECS - 1) / ASYNC_CHECK_RECS, ASYNC_THREADS, 0, stream>>>(a, chk, table);
+  end();
+  begin("fused_narrow_kernel");
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    fused_narrow_kernel<L><<<mc, FZ_THREADS, sizeof(FusedSmem), stream>>>(a.fp, table, d_idx, a.index_cap, d_st, d_cls, static_cast<L*>(dst), a.dst_cap);
+    return 0;
+  });
+  end();
+  begin("symwalk_kernel");
+  symwalk_kernel<false><<<mc, SW_THREADS, sizeof(SymWalkSmem), stream>>>(a.fp, table, d_idx, a.index_cap, a.dst_cap, d_syms, d_offs, d_cls, nullptr, 1);
+  end();
+  begin("decode_kernel");
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    decode_kernel<L, 1><<<mc, DEC_THREADS, sizeof(DecodeSmem), stream>>>(a.fp, table, d_st, d_idx, a.index_cap, static_cast<L*>(dst), a.dst_cap, &chk->binoms,
+                                                                          d_syms, d_offs, d_cls);
+    decode_kernel<L, 2><<<mc, DEC_THREADS, sizeof(DecodeSmem), stream>>>(a.fp, table, d_st, d_idx, a.index_cap, static_cast<L*>(dst), a.dst_cap, &chk->binoms,
+                                                                          d_syms, d_offs, d_cls);
+    return 0;
+  });
+  end();
+  begin("cold_chunks_kernel");
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    cold_chunks_kernel<L><<<1, ASYNC_THREADS, 0, stream>>>(a.fp, table, chk, d_st, static_cast<L*>(dst), a.dst_cap, d_cold);
+    return 0;
+  });
+  end();
+  begin("async_finish_kernel");
+  async_finish_kernel<<<1, 1024, 0, stream>>>(a.dst_cap, chk, d_st, status);
+  end();
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
+}
+
+PcoB200Error pco_b200_decompress_async_result(const PcoB200AsyncStatus* s, PcoB200Progress* progress) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200Error kind = s->kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(s->kind) : PCO_B200_CORRUPTION;
+  if (kind == PCO_B200_OK) {
+    if (progress) {
+      progress->n_processed = size_t(s->n_processed);
+      progress->finished = s->finished ? 1 : 0;
+    }
+    return PCO_B200_OK;
+  }
+  switch (s->device_status) {
+    case PCO_B200_ASYNC_HEADER_CORRUPT: return fail(kind, "corrupt standalone header (magic, version, type byte or size hint)");
+    case PCO_B200_ASYNC_HEADER_SHORT: return fail(kind, "insufficient data: the file ends inside its standalone header");
+    case PCO_B200_ASYNC_HEADER_MISMATCH: return fail(kind, "the file's uniform type or format version differs from the plan's");
+    case PCO_B200_ASYNC_INDEX_FOREIGN: return fail(kind, "side index does not belong to this file (or its file length exceeds src_cap)");
+    case PCO_B200_ASYNC_TOO_MANY_CHUNKS:
+      return fail(kind, "the side index lists " + std::to_string(s->n_chunks) + " chunks, more than the plan's max_chunks");
+    default:
+      status_to_error(s->device_status, "this chunk");
+      return fail(kind, "chunk " + std::to_string(s->chunk) + ": " + last_error_ref());
+  }
 }
 
 PcoB200Error pco_b200_build_index(const void* compressed, size_t compressed_len, unsigned char dtype, void* index, size_t index_cap,

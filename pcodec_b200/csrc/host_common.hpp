@@ -85,6 +85,13 @@ struct Profiler {
     }
     spans.clear();
   }
+  void discard() {  // drops pending spans unread (the events are released once the device has passed them)
+    for (auto& sp : spans) {
+      cudaEventDestroy(sp.e0);
+      cudaEventDestroy(sp.e1);
+    }
+    spans.clear();
+  }
 };
 inline Profiler& profiler() {
   static thread_local Profiler p;

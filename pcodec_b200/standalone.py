@@ -385,6 +385,91 @@ def decompress_ranges(data, dtype, index, ranges):
     return dst[: nw.value]
 
 
+class _CAsyncPlan(C.Structure):  # PcoB200AsyncPlan (include/pco_b200.h)
+    _fields_ = [("dtype", C.c_uint32), ("uniform_type", C.c_uint32), ("format_major", C.c_uint32), ("reserved", C.c_uint32),
+                ("src_cap", C.c_uint64), ("index_cap", C.c_uint64), ("dst_cap", C.c_uint64), ("max_chunks", C.c_uint64),
+                ("workspace_bytes", C.c_uint64)]
+
+
+class _CAsyncStatus(C.Structure):  # PcoB200AsyncStatus (include/pco_b200.h)
+    _fields_ = [("kind", C.c_uint32), ("device_status", C.c_uint32), ("chunk", C.c_uint64), ("n_processed", C.c_uint64),
+                ("finished", C.c_uint32), ("n_chunks", C.c_uint32)]
+
+
+def _lib_async():
+    L = _lib.lib()
+    if not getattr(L, "_async_ready", False):
+        L.pco_b200_decompress_async_plan.argtypes = [C.c_void_p, C.c_size_t, C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p]
+        L.pco_b200_decompress_async.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.pco_b200_decompress_async_result.argtypes = [C.c_void_p, C.c_void_p]
+        L._async_ready = True
+    return L
+
+
+class AsyncDecompressor:
+    """Decodes indexed standalone files on the current CUDA stream without waiting for the device (pco_b200_decompress_async): a call
+    only enqueues kernels, so it can run behind other GPU work while the host moves on, and it can be captured in a torch.cuda.CUDAGraph.
+
+    The plan comes from `head`, the first bytes of a file (32 suffice; bytes, numpy or a tensor): it fixes the number type `dtype`, the
+    header flavour (uniform type) and the format version of every file decoded with it.  src_cap, index_cap (bytes) and dst_cap (numbers)
+    are the sizes of the buffers every call passes, max_chunks the most chunks a file may have.  The file length, chunk count and number
+    count come from each file's side index on the device, so one captured call decodes whatever file its buffers hold on each replay.
+    The decompressor owns a device workspace and a status word; it serves one call in flight at a time (calls on one stream queue up)."""
+
+    def __init__(self, head, dtype, src_cap, index_cap, dst_cap, max_chunks, device=None):
+        import torch
+
+        from .wrapped import _host_u8
+
+        self.dtype = np.dtype(dtype)
+        if _is_cuda(head):
+            head = head.reshape(-1)[:32].cpu().numpy()
+        h = _host_u8(head)[:32].copy()
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        L = _lib_async()
+        self._plan = _CAsyncPlan()
+        with torch.cuda.device(self.device):
+            rc = L.pco_b200_decompress_async_plan(h.ctypes.data_as(C.c_void_p), C.c_size_t(h.size), C.c_ubyte(_lib.dtype_byte(self.dtype)),
+                                                  C.c_size_t(src_cap), C.c_size_t(index_cap), C.c_size_t(dst_cap), C.c_size_t(max_chunks),
+                                                  C.byref(self._plan))
+        _lib.check(rc)
+        self.workspace = torch.empty(self._plan.workspace_bytes, dtype=torch.uint8, device=self.device)
+        self.status = torch.zeros(C.sizeof(_CAsyncStatus), dtype=torch.uint8, device=self.device)
+
+    @property
+    def workspace_bytes(self):
+        return int(self._plan.workspace_bytes)
+
+    def __call__(self, src, index, dst):
+        """Enqueues the decode of the file in `src` (uint8 CUDA tensor of at least src_cap bytes) through its side index `index` (at least
+        index_cap bytes) into `dst` (a CUDA tensor of the plan's dtype, at least dst_cap numbers) on torch.cuda.current_stream().  Returns
+        nothing and does not wait; result() reports the outcome."""
+        import torch
+
+        from .wrapped import _torch_dtypes
+
+        p = self._plan
+        for name, t in (("src", src), ("index", index), ("dst", dst)):
+            if not _is_cuda(t) or t.device != self.device or not t.is_contiguous():
+                raise ValueError(f"{name} must be a contiguous CUDA tensor on {self.device}")
+        if src.numel() * src.element_size() < p.src_cap or index.numel() * index.element_size() < p.index_cap:
+            raise ValueError(f"src holds fewer than src_cap = {p.src_cap} bytes, or index fewer than index_cap = {p.index_cap}")
+        if dst.dtype != _torch_dtypes()[self.dtype] or dst.numel() < p.dst_cap:
+            raise ValueError(f"dst must hold at least dst_cap = {p.dst_cap} numbers of {self.dtype}")
+        rc = _lib_async().pco_b200_decompress_async(C.byref(p), C.c_void_p(src.data_ptr()), C.c_void_p(index.data_ptr()), C.c_void_p(dst.data_ptr()),
+                                                    C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()),
+                                                    C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+        _lib.check(rc)
+
+    def result(self):
+        """Copies the status of the last call back (waiting for it on the current stream) and returns its Progress, or raises PcoError
+        with the kind pco_b200_decompress_ex gives."""
+        s = _CAsyncStatus.from_buffer_copy(self.status.cpu().numpy().tobytes())
+        prog = _lib._CProgress()
+        _lib.check(_lib_async().pco_b200_decompress_async_result(C.byref(s), C.byref(prog)))
+        return Progress(prog.n_processed, bool(prog.finished))
+
+
 class _CModeChoice(C.Structure):
     _fields_ = [("mode_spec", C.c_uint32), ("float_quant_k", C.c_uint32), ("float_mult_base", C.c_double), ("float_mult_inv_base", C.c_double),
                 ("int_mult_base", C.c_uint64), ("bits_saved_per_num", C.c_double)]
