@@ -158,7 +158,7 @@ int pco_b200_zero_copy(int mask);
 size_t pco_b200_debug_follow_chain(const uint64_t *cand, const uint32_t *statuses, const uint64_t *ends, uint32_t m, uint64_t pos, uint64_t n0,
                                    uint64_t out_off, uint64_t dst_len, uint64_t src_len, uint32_t *verified, uint64_t *next_pos);
 /* counts8[k] = chunks of the last decode launch served by decode class k (1, 2: general kernel with 1 / 2 latent vars;
- * 3, 4: narrow kernel, delta order 0 / 1); returns the number of chunks. */
+ * 3, 4, 5: fused narrow kernel, delta order 0 / 1 / 2..7); returns the number of chunks. */
 int pco_b200_profile_chunk_classes(unsigned *counts8);
 /* How the tANS encoder resolved the last compress call on this thread, if it ran with pco_b200_profile_enable(1) (for a call that
  * compresses in several passes, e.g. pco_b200_compress_files with several groups: its last pass).  The encoder cuts each (chunk, latent

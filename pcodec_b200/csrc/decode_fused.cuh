@@ -1,6 +1,6 @@
 // fused_narrow_kernel: K7a + K7b + K8 + K9 in ONE kernel for the chunks that delta coding usually produces (the narrow
-// class of decode_narrow.cuh: classic mode, consecutive order 0 / 1, 2..256 bins whose lowers lie within 2^16 of the first
-// and whose offsets take <= 15 bits, 32- and 64-bit number types).
+// class: classic mode, consecutive delta of any order, 2..256 bins whose lowers lie within 2^16 of the first and whose
+// offsets take <= 15 bits, every number width).
 //
 // One CTA of 8 warps per chunk:
 //   * prologue: the chunk's first 4 KiB (header, bins, page meta) arrive in shared memory by ONE bulk copy
@@ -14,12 +14,37 @@
 //   * the other (FZ_DECODERS) warps decode, a warp per batch in batch order (page_latent_decompressor.rs:15-44, delta/consecutive.rs:35-50,
 //     mode/classic.rs:14-24): symbols from the ring, the offsets window by cp.async one batch ahead, fields peeled off
 //     register windows, the order-1 un-delta as one 32-bit scan + the fence-free carry record, 32-byte stores.
-// Compared with symwalk_kernel + decode_narrow_kernel the symbol bytes never leave the SM (no 0.27 GB scratch written and
-// read back), the section starts are not stored, the header is parsed once, and the compressed bytes are read by one kernel.
+// Compared with the two-kernel decode (symwalk_kernel + decode_kernel) the symbol bytes never leave the SM (no 0.27 GB scratch
+// written and read back), the section starts are not stored, the header is parsed once, and the compressed bytes are read by one kernel.
 #pragma once
-#include "decode_narrow.cuh"
+#include "decode_kernels.cuh"
 
 namespace pcob200 {
+
+constexpr int NW_WIN_WORDS = 128 + 4;  // a decoder warp's offsets window: 512 staged bytes + 16 of slack for the 3-word lane windows
+
+// one step of an inclusive warp scan: v += (value of lane - d) for lanes >= d; the shuffle's own range predicate guards the add
+__device__ __forceinline__ uint32_t scan_step_up(uint32_t v, int d) {
+  uint32_t r;
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .u32 t;\n\t"
+      "shfl.sync.up.b32 t|p, %1, %2, 0, 0xffffffff;\n\t"
+      "mov.u32 %0, %1;\n\t"
+      "@p add.u32 %0, %1, t;\n\t}"
+      : "=r"(r) : "r"(v), "r"(d));
+  return r;
+}
+// shifts that take the amount from the low 5 bits of `s` (the table entry itself: its bits 4..6 are zero)
+__device__ __forceinline__ uint32_t shr_wrap(uint32_t lo, uint32_t hi, uint32_t s) {
+  uint32_t r;
+  asm("shf.r.wrap.b32 %0, %1, %2, %3;" : "=r"(r) : "r"(lo), "r"(hi), "r"(s));
+  return r;
+}
+__device__ __forceinline__ uint32_t ones_shl_wrap(uint32_t s) {  // 0xffffffff << (s & 31)
+  uint32_t r;
+  asm("shf.l.wrap.b32 %0, %1, %2, %3;" : "=r"(r) : "r"(0u), "r"(0xffffffffu), "r"(s));
+  return r;
+}
 
 #ifndef PCOB_FZ_NBUF
 #define PCOB_FZ_NBUF 3

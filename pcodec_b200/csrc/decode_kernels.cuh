@@ -128,22 +128,14 @@ struct WinTask {
 __device__ __forceinline__ uint32_t win_first_batch(uint32_t lo, uint32_t order) { return order == 0 ? lo / BATCH_N : 0u; }
 
 // ---------------------------------------------------------------------------
-// Chunk classes: symwalk_kernel parses and validates every chunk header anyway, so it also decides which decode
-// instantiation owns the chunk (d_cls, one byte per chunk): 1 / 2 = decode_kernel<L, 1 / 2> (any refusal is reported
-// by decode_kernel<L, 1>), 3 / 4 = decode_narrow_kernel (decode_narrow.cuh) with delta order 0 / 1.
+// Chunk classes (d_cls, one byte per chunk): fused_narrow_kernel (decode_fused.cuh) decodes the narrow class itself and
+// reports 3 / 4 / 5 = delta order 0 / 1 / 2..7; for every other chunk symwalk_kernel, which parses and validates the header
+// anyway, decides which decode instantiation owns it: 1 / 2 = decode_kernel<L, 1 / 2> (any refusal is reported by
+// decode_kernel<L, 1>).
 // ---------------------------------------------------------------------------
 constexpr uint32_t CLS_NARROW0 = 3, CLS_NARROW1 = 4, CLS_NARROWK = 5;  // narrow class with delta order 0 / 1 / 2..7
 constexpr uint32_t CLS_DONE = 0x80;  // fused_narrow_kernel (decode_fused.cuh) has finished the chunk: the two-kernel path skips it
 constexpr uint32_t NARROW_MAX_OB = 15, NARROW_LOW_BITS = 16;
-
-struct NarrowInfo {   // one per chunk, in HBM scratch; only written for chunks of a narrow class
-  uint64_t base;      // lower of bin 0 (+ MID when the var is delta'd: folds toggle_center into the add)
-  uint64_t moment0;   // the page's delta moment (order 1)
-  uint32_t n;
-  uint32_t pad[3];
-  uint32_t q[SMALL_MAX_BINS];  // offset_bits | (lower - lower_0) << 7
-};
-static_assert(sizeof(NarrowInfo) % 16 == 0, "NarrowInfo rows are loaded with vector accesses");
 
 // ---------------------------------------------------------------------------
 // Cooperative table build for one latent var (all threads of the CTA call this).
@@ -907,7 +899,6 @@ struct SymWalkSmem {
   ChunkHdr hdr;
   uint32_t node[SW_NODE_WORDS];
   uint32_t err;
-  uint32_t not_narrow;
   union {
     struct {
       BuildScratch build;
@@ -923,9 +914,8 @@ struct SymWalkSmem {
 template <bool WIN = false>  // WIN: window mode, wins[t] says which numbers of task t are wanted (out_len is unused)
 __global__ void __launch_bounds__(SW_THREADS) symwalk_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, const uint8_t* __restrict__ index_base,
                                                               uint64_t index_len, uint64_t out_len, uint8_t* __restrict__ d_syms, uint32_t* __restrict__ d_offs,
-                                                              uint8_t* __restrict__ d_nvars, NarrowInfo* __restrict__ d_narrow, int classes_preset,
-                                                              const WinTask* __restrict__ wins = nullptr) {
-  if (classes_preset && (d_nvars[blockIdx.x] & CLS_DONE)) return;  // fused_narrow_kernel has decoded (or refused) this chunk
+                                                              uint8_t* __restrict__ d_nvars, const WinTask* __restrict__ wins = nullptr) {
+  if (d_nvars[blockIdx.x] & CLS_DONE) return;  // fused_narrow_kernel has decoded (or refused) this chunk
   extern __shared__ __align__(16) unsigned char smem_raw[];
   SymWalkSmem& sm = *reinterpret_cast<SymWalkSmem*>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -937,7 +927,6 @@ __global__ void __launch_bounds__(SW_THREADS) symwalk_kernel(FileParams fp, cons
   // every refusal below is reported by decode_kernel, which parses the same header
   if (tid == 0) {
     sm.err = 0;
-    sm.not_narrow = 0;
     parse_chunk_header(src, chunk_bit0, fp.dtype, fp.uniform_type, fp.format_major, true, sm.hdr);
     if (sm.hdr.status == ST_OK) {
       for (uint32_t v = 0; v < sm.hdr.n_vars; v++) {
@@ -962,29 +951,6 @@ __global__ void __launch_bounds__(SW_THREADS) symwalk_kernel(FileParams fp, cons
                             sm.b.build.bin_cum[v], sm.b.build.sym_of_state[v], sm.b.build.rank_counter[v], &sm.err, false);
   __syncthreads();
   if (sm.err) return;
-#ifndef PCOB_NO_NARROW
-  // narrow class (decode_narrow.cuh): the header and bins are parsed and validated at this point
-  if (d_narrow && n_vars == 1 && sm.hdr.mode == MODE_CLASSIC && sm.hdr.var[0].delta_order <= 1 && sm.hdr.var[0].latent_bits >= 32 &&
-      sm.hdr.var[0].n_bins >= 2 && sm.hdr.var[0].max_offset_bits <= NARROW_MAX_OB) {
-    const VarHdr& vh = sm.hdr.var[0];
-    const uint64_t lmask = vh.latent_bits == 64 ? ~uint64_t(0) : ((uint64_t(1) << vh.latent_bits) - 1);
-    const uint64_t lower0 = sm.b.build.bin_lower[0][0];
-    NarrowInfo* ni = d_narrow + blockIdx.x;
-    for (uint32_t i = tid; i < vh.n_bins; i += SW_THREADS) {
-      const uint64_t d = (sm.b.build.bin_lower[0][i] - lower0) & lmask;
-      if (d >> NARROW_LOW_BITS) sm.not_narrow = 1;
-      ni->q[i] = uint32_t(sm.b.build.bin_ob[0][i]) | (uint32_t(d) << 7);
-    }
-    __syncthreads();
-    if (tid == 0 && !sm.not_narrow) {
-      const uint64_t mid = uint64_t(1) << (vh.latent_bits - 1);
-      ni->base = vh.delta_order ? ((lower0 + mid) & lmask) : lower0;
-      ni->moment0 = sm.hdr.moments[0][0];
-      ni->n = sm.hdr.n;
-      d_nvars[blockIdx.x] = uint8_t(vh.delta_order ? CLS_NARROW1 : CLS_NARROW0);
-    }
-  }
-#endif
   // replicate: var v owns SW_NODE_WORDS / n_vars words (>= its 2^size_log); rep_log = log2 of its copy count
   const uint32_t region = SW_NODE_WORDS / n_vars;
   const uint32_t rep_log0 = min(5u, uint32_t(31 - __clz(region >> sm.hdr.var[0].ans_size_log)));

@@ -6,7 +6,6 @@
 #include "async_kernels.cuh"
 #include "compress_host.cuh"
 #include "decode_kernels.cuh"
-#include "decode_narrow.cuh"
 #include "decode_fused.cuh"
 #include "gather_kernels.cuh"
 #include "decode_cold.cuh"
@@ -17,31 +16,37 @@
 
 namespace pcob200 {
 
+// Every device scratch buffer of a context, listed once: Context declares them and reset_context frees them all.
+#define PCOB_CONTEXT_BUFFERS(X)                                                                                   \
+  X(src) X(out) X(index) X(statuses) X(misc) X(dec_syms) X(dec_offs) X(gather) X(cold) X(cold_res) X(spec)        \
+  /* pco_b200_decompress_pages / pco_b200_compress_wrapped */                                                     \
+  X(wrap_metas) X(wrap_frames) X(wrap_tab) X(wrap_res) X(wrap_file) X(wrap_index) X(wrap_out)                     \
+  /* pco_b200_compress_files / pco_b200_decompress_files */                                                       \
+  X(files_tab) X(files_res) X(files_out) X(files_idx) X(files_arena) X(files_cold)                                \
+  /* pco_b200_decompress_ranges */                                                                                \
+  X(rng_tab) X(rng_stage) X(rng_cold) X(rng_copies)
+
 // One Context per host thread (thread_local): its scratch buffers, events and the last call's profile belong to the calling
 // thread, so calls from different threads run concurrently (e.g. compress of chunk group g + 1 while group g decompresses, each
 // on its own stream) and the entry points are thread-safe the way the reference documents its own (pco_c/src/lib.rs:57-70).
 // The context follows the thread's current device: a cudaSetDevice between calls drops the scratch of the previous device.
 struct Context {
   int device = -1;
-  bool attrs_set = false;
+  bool attrs_set[2] = {false, false};  // set_decode_attrs<WIN> has run
   bool initialized = false;
   bool device_ok = false;
   std::string device_err;
-  DevBuf src, out, index, statuses, misc, dec_syms, dec_offs, dec_narrow, gather, cold, spec;
-  DevBuf wrap_metas, wrap_frames, wrap_tab, wrap_res, wrap_file, wrap_index, wrap_out;  // pco_b200_decompress_pages / pco_b200_compress_wrapped
-  DevBuf files_tab, files_res, files_out, files_idx, files_arena, files_cold;            // pco_b200_compress_files / pco_b200_decompress_files
-  DevBuf rng_tab, rng_stage, rng_cold, rng_res, rng_copies;                             // pco_b200_decompress_ranges
-  bool ranges_attrs_set = false;
+#define PCOB_DECLARE_BUFFER(name) DevBuf name;
+  PCOB_CONTEXT_BUFFERS(PCOB_DECLARE_BUFFER)
+#undef PCOB_DECLARE_BUFFER
   CompressScratch enc;
   Binoms* d_binoms = nullptr;
   int sm_count = 0;
   uint32_t last_decode_chunks = 0;  // chunks of the last decode launch (their class bytes are still at d_cls)
-  std::vector<uint8_t> host_cls;    // class bytes of the last fused launch as the kernel reported them (0 = decoded there)
   uint8_t* d_cls = nullptr;         // class bytes of the last decode launch (they live behind the status words in `statuses`)
   void* pinned_res = nullptr;       // page-locked landing buffer for the statuses + class bytes of a decode launch
   size_t pinned_cap = 0;
-  bool last_classes_fused = false;
-  uint32_t* gather_err = nullptr;   // error word of the last page gather (inside `gather`)  // every chunk of the last launch was served by fused_narrow_kernel
+  uint32_t* gather_err = nullptr;   // error word of the last page gather (inside `gather`)
 };
 
 static Context& ctx() {
@@ -49,10 +54,13 @@ static Context& ctx() {
   return c;
 }
 
-static void release_buffers(Context& c) {
-  for (DevBuf* b : {&c.src, &c.out, &c.index, &c.statuses, &c.misc, &c.dec_syms, &c.dec_offs, &c.dec_narrow, &c.gather, &c.cold, &c.spec, &c.wrap_metas, &c.wrap_frames,
-                  &c.wrap_tab, &c.wrap_res, &c.wrap_file, &c.wrap_index, &c.wrap_out, &c.files_tab, &c.files_res, &c.files_out, &c.files_idx,
-                  &c.files_arena, &c.files_cold, &c.rng_tab, &c.rng_stage, &c.rng_cold, &c.rng_res, &c.rng_copies}) b->release();
+// Frees the context's device memory and marks it uninitialised, so that the next call on this thread sets the device up again.  That
+// includes the binomial table ensure_device builds once per context: a context left initialised without it sent the next decode that
+// reached decode_kernel to a null table (an illegal address).
+static void reset_context(Context& c) {
+#define PCOB_RELEASE_BUFFER(name) c.name.release();
+  PCOB_CONTEXT_BUFFERS(PCOB_RELEASE_BUFFER)
+#undef PCOB_RELEASE_BUFFER
   c.enc.release();
   c.gather_err = nullptr;
   c.d_cls = nullptr;
@@ -61,20 +69,18 @@ static void release_buffers(Context& c) {
   c.pinned_cap = 0;
   if (c.d_binoms) cudaFree(c.d_binoms);
   c.d_binoms = nullptr;
+  c.initialized = false;
+  c.device_ok = false;
+  c.attrs_set[0] = c.attrs_set[1] = false;
 }
 
 static PcoB200Error ensure_device(Context& c) {
   if (c.initialized && c.device_ok) {
     int cur = -1;
     if (cudaGetDevice(&cur) == cudaSuccess && cur != c.device) {  // the thread moved to another device: start over there
-      const int now = cur;
       cudaSetDevice(c.device);
-      release_buffers(c);
-      cudaSetDevice(now);
-      c.initialized = false;
-      c.device_ok = false;
-      c.attrs_set = false;
-      c.ranges_attrs_set = false;
+      reset_context(c);
+      cudaSetDevice(cur);
     }
   }
   if (!c.initialized) {
@@ -133,29 +139,29 @@ struct DecodeOutcome {
   bool terminated = false;
 };
 
-// Shared-memory attributes of the decode kernels, set once per context before their first launch.
+// Shared-memory attributes of the decode kernels (the window-mode instantiations when WIN), set once per context before their first launch.
+template <bool WIN>
 static PcoB200Error set_decode_attrs(Context& c) {
-  if (c.attrs_set) return PCO_B200_OK;
-  c.attrs_set = true;
-  PCOB_CUDA_TRY(cudaFuncSetAttribute(symwalk_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SymWalkSmem)));
-  PCOB_CUDA_TRY(cudaFuncSetAttribute(symwalk_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-  PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint64_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
-  PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint32_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
-  PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint64_t>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-  PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint32_t>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-  PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
-  PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
-  PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint16_t>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-  PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint8_t>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+  if (c.attrs_set[WIN]) return PCO_B200_OK;
+  c.attrs_set[WIN] = true;
+  auto max_shared = [](auto* kernel, size_t smem) {
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+    return e != cudaSuccess ? e : cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, int(cudaSharedmemCarveoutMaxShared));
+  };
+  PCOB_CUDA_TRY(max_shared(symwalk_kernel<WIN>, sizeof(SymWalkSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint64_t, WIN>, sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint32_t, WIN>, sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint16_t, WIN>, sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint8_t, WIN>, sizeof(FusedSmem)));
   return PCO_B200_OK;
 }
 
 // Launch the decode over `n_chunks` IndexChunk records that live on the device.
 //   1. fused_narrow_kernel (decode_fused.cuh): parses and classifies every chunk and fully decodes the narrow class;
 //   2. only if some chunk is of another class: symwalk_kernel + decode_kernel<L, 1 / 2> for those.
-// PCOB200_FUSED=0 selects the round-1 pair symwalk_kernel + decode_narrow_kernel (kept for A/B measurements).
+// A failing chunk fails the launch ("... chunk k"); `bad_chunk`, when given, receives its position k among the launch's records.
 static PcoB200Error launch_decode(Context& c, const FileParams& fp, const uint8_t* d_index, uint64_t index_len, uint64_t chunks_offset, uint32_t n_chunks,
-                                  void* d_out, uint64_t out_len, cudaStream_t stream) {
+                                  void* d_out, uint64_t out_len, cudaStream_t stream, uint32_t* bad_chunk = nullptr) {
   if (n_chunks == 0) return PCO_B200_OK;
   // status words and class bytes side by side: one copy brings both back
   const size_t res_bytes = size_t(n_chunks) * (sizeof(uint32_t) + 1);
@@ -171,55 +177,39 @@ static PcoB200Error launch_decode(Context& c, const FileParams& fp, const uint8_
     c.pinned_cap = res_bytes + (res_bytes >> 1) + 4096;
   }
   const IndexChunk* d_chunks = reinterpret_cast<const IndexChunk*>(d_index + chunks_offset);
-  static const bool use_fused = [] { const char* e = std::getenv("PCOB200_FUSED"); return !(e && e[0] == '0'); }();
-  const bool narrow_ok = true;  // the fused kernel serves every number width
-  if (PcoB200Error e = set_decode_attrs(c)) return e;
+  if (PcoB200Error e = set_decode_attrs<false>(c)) return e;
   c.last_decode_chunks = n_chunks;
   const uint32_t* st = static_cast<const uint32_t*>(c.pinned_res);
-  bool fused_ran = false;
-  if (!(use_fused && narrow_ok)) PCOB_CUDA_TRY(cudaMemsetAsync(d_st, 0xff, size_t(n_chunks) * sizeof(uint32_t), stream));  // the fused kernel writes every word itself
-  if (use_fused && narrow_ok) {
-    fused_ran = true;
-    profiler().begin("fused_narrow_kernel", stream);
-    dispatch_latent(fp.dtype, [&](auto tag) {
-      using L = decltype(tag);
-      fused_narrow_kernel<L><<<n_chunks, FZ_THREADS, sizeof(FusedSmem), stream>>>(fp, d_chunks, d_index, index_len, d_st, d_cls, static_cast<L*>(d_out), out_len);
-      return 0;
-    });
-    profiler().end(stream);
-    PCOB_CUDA_TRY(cudaGetLastError());
-    // statuses and class bytes come back in one round trip; the general kernels only run if some chunk still needs them
-    PCOB_CUDA_TRY(readback_small_sync(c.pinned_res, d_st, (res_bytes + 3) & ~size_t(3), stream));  // the buffers hold res_bytes + 64
-    const uint8_t* cls = reinterpret_cast<const uint8_t*>(st + n_chunks);
-    c.host_cls.assign(cls, cls + n_chunks);
-    bool pending = false;
-    for (uint32_t i = 0; i < n_chunks; i++) {
-      if (!(cls[i] & CLS_DONE)) { pending = true; continue; }
-      if (st[i] != ST_OK) return status_to_error(st[i], ("chunk " + std::to_string(i)).c_str());
-    }
-    c.last_classes_fused = true;
-    if (!pending) return PCO_B200_OK;
+  auto chunk_fail = [&](uint32_t i) {
+    if (bad_chunk) *bad_chunk = i;
+    return status_to_error(st[i], ("chunk " + std::to_string(i)).c_str());
+  };
+  profiler().begin("fused_narrow_kernel", stream);
+  dispatch_latent(fp.dtype, [&](auto tag) {
+    using L = decltype(tag);
+    fused_narrow_kernel<L><<<n_chunks, FZ_THREADS, sizeof(FusedSmem), stream>>>(fp, d_chunks, d_index, index_len, d_st, d_cls, static_cast<L*>(d_out), out_len);
+    return 0;
+  });
+  profiler().end(stream);
+  PCOB_CUDA_TRY(cudaGetLastError());
+  // statuses and class bytes come back in one round trip; the general kernels only run if some chunk still needs them
+  PCOB_CUDA_TRY(readback_small_sync(c.pinned_res, d_st, (res_bytes + 3) & ~size_t(3), stream));  // the buffers hold res_bytes + 64
+  const uint8_t* cls = reinterpret_cast<const uint8_t*>(st + n_chunks);
+  bool pending = false;
+  for (uint32_t i = 0; i < n_chunks; i++) {
+    if (!(cls[i] & CLS_DONE)) { pending = true; continue; }
+    if (st[i] != ST_OK) return chunk_fail(i);
   }
-  c.last_classes_fused = false;
+  if (!pending) return PCO_B200_OK;
   // scratch between the two kernels: one symbol byte per latent the destination can take, one section start per batch
   const uint64_t rows = scratch_rows_total(out_len, n_chunks);
   PCOB_CUDA_TRY(c.dec_syms.reserve(rows * BATCH_N + 64));
   PCOB_CUDA_TRY(c.dec_offs.reserve(rows * sizeof(uint32_t) + 64));
-  const bool old_narrow = nt_bits(fp.dtype) >= 32 && !fused_ran;  // PCOB200_FUSED=0: the round-1 narrow kernel serves 32- and 64-bit types
-  if (old_narrow) PCOB_CUDA_TRY(c.dec_narrow.reserve(size_t(n_chunks) * sizeof(NarrowInfo)));
   profiler().begin("symwalk_kernel", stream);
   symwalk_kernel<<<n_chunks, SW_THREADS, sizeof(SymWalkSmem), stream>>>(fp, d_chunks, d_index, index_len, out_len, c.dec_syms.as<uint8_t>(), c.dec_offs.as<uint32_t>(),
-                                                                        d_cls, old_narrow ? c.dec_narrow.as<NarrowInfo>() : nullptr, fused_ran ? 1 : 0);
+                                                                        d_cls);
   profiler().end(stream);
   profiler().begin("decode_kernel", stream);  // the span covers every decode instantiation (a chunk runs in exactly one)
-  if (old_narrow) {
-    if (nt_bits(fp.dtype) == 64)
-      decode_narrow_kernel<uint64_t><<<n_chunks, NW_THREADS, 0, stream>>>(fp, d_chunks, d_st, static_cast<uint64_t*>(d_out), out_len, c.dec_syms.as<uint8_t>(),
-                                                                        c.dec_offs.as<uint32_t>(), d_cls, c.dec_narrow.as<NarrowInfo>());
-    else
-      decode_narrow_kernel<uint32_t><<<n_chunks, NW_THREADS, 0, stream>>>(fp, d_chunks, d_st, static_cast<uint32_t*>(d_out), out_len, c.dec_syms.as<uint8_t>(),
-                                                                        c.dec_offs.as<uint32_t>(), d_cls, c.dec_narrow.as<NarrowInfo>());
-  }
   dispatch_latent(fp.dtype, [&](auto tag) {
     using L = decltype(tag);
     decode_kernel<L, 1><<<n_chunks, DEC_THREADS, sizeof(DecodeSmem), stream>>>(fp, d_chunks, d_st, d_index, index_len, static_cast<L*>(d_out), out_len, c.d_binoms,
@@ -232,9 +222,112 @@ static PcoB200Error launch_decode(Context& c, const FileParams& fp, const uint8_
   PCOB_CUDA_TRY(cudaGetLastError());
   PCOB_CUDA_TRY(readback_small_sync(c.pinned_res, d_st, size_t(n_chunks) * sizeof(uint32_t), stream));
   for (uint32_t i = 0; i < n_chunks; i++)
-    if (st[i] != ST_OK) return status_to_error(st[i], ("chunk " + std::to_string(i)).c_str());
+    if (st[i] != ST_OK) return chunk_fail(i);
   return PCO_B200_OK;
 }
+
+// The file's first bytes (at most 32) and, when `ih` is given, the side index header (zeros when `index` holds none), from host or
+// device memory - one synchronisation for both - and the standalone header parsed from those bytes.
+static PcoB200Error read_heads(const void* src, size_t src_len, bool src_dev, const void* index, size_t index_len, bool idx_dev, IndexHeader* ih,
+                               StandaloneHeader* hdr, cudaStream_t stream) {
+  uint8_t head[32] = {0};
+  const size_t avail = std::min<size_t>(src_len, sizeof(head));
+  bool need_sync = false;
+  if (avail) {
+    if (src_dev) { PCOB_CUDA_TRY(cudaMemcpyAsync(head, src, avail, cudaMemcpyDeviceToHost, stream)); need_sync = true; }
+    else std::memcpy(head, src, avail);
+  }
+  if (ih) {
+    std::memset(ih, 0, sizeof(*ih));
+    if (index && index_len >= sizeof(IndexHeader)) {
+      if (idx_dev) { PCOB_CUDA_TRY(cudaMemcpyAsync(ih, index, sizeof(*ih), cudaMemcpyDeviceToHost, stream)); need_sync = true; }
+      else std::memcpy(ih, index, sizeof(*ih));
+    }
+  }
+  if (need_sync) PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
+  return parse_standalone_header(head, avail, src_len, hdr);
+}
+
+// A side index header made for a file of `file_len` bytes, whose chunk table lies inside the index's `index_len` bytes (overflow-safe;
+// the per-chunk fields are bounded on the device: entries inside the index, chunk_offset inside the file, writes inside the destination).
+static bool index_header_ok(const IndexHeader& ih, uint64_t file_len, uint64_t index_len) {
+  return ih.magic == INDEX_MAGIC && ih.version == 1 && ih.file_len == file_len && ih.chunks_offset <= index_len &&
+         ih.n_chunks <= (index_len - ih.chunks_offset) / sizeof(IndexChunk);
+}
+
+// A caller's buffer in HBM: the buffer itself when it is on the device, else its bytes copied into `buf`.
+static PcoB200Error stage_in(DevBuf& buf, const void* p, size_t len, bool on_device, cudaStream_t stream, const uint8_t** d_p) {
+  *d_p = static_cast<const uint8_t*>(p);
+  if (on_device) return PCO_B200_OK;
+  PCOB_CUDA_TRY(buf.reserve(len + 16));
+  if (len) PCOB_CUDA_TRY(copy_sliced(buf.p, p, len, cudaMemcpyHostToDevice, stream));
+  *d_p = buf.as<uint8_t>();
+  return PCO_B200_OK;
+}
+
+// Where the kernels write the output: the caller's device buffer, or `c.out` (at least `bytes`) for a host one.
+static PcoB200Error out_buffer(Context& c, void* dst, bool dst_dev, uint64_t bytes, void** d_out) {
+  *d_out = dst;
+  if (dst_dev) return PCO_B200_OK;
+  PCOB_CUDA_TRY(c.out.reserve(bytes + 64));
+  *d_out = c.out.p;
+  return PCO_B200_OK;
+}
+
+// Placeholder records for a walk: from `begin` on, each record gets room for MAX_VARS vars of batch entries for its `n` numbers
+// (16-byte aligned).  Returns where the entries end.
+static uint64_t lay_out_entries(IndexChunk* recs, size_t n_recs, uint64_t begin) {
+  for (size_t k = 0; k < n_recs; k++) {
+    recs[k].entries_offset = begin;
+    begin += (uint64_t(MAX_VARS) * n_batches_of(recs[k].n) * sizeof(BatchEntry) + 15) & ~uint64_t(15);
+  }
+  return begin;
+}
+
+// One catch-all decode: the chunks of `fp` from byte `first_byte` on, into `out`, which takes `cap` numbers.
+struct ColdJob {
+  FileParams fp;
+  uint64_t first_byte;
+  void* out;
+  uint64_t cap;
+};
+
+// cold_decode_kernel over every job (one single-thread launch each), the results read back into `res`.  Lookback windows beyond 2^16
+// numbers get the large scratch on a second pass, which takes the jobs whose result `retry` accepts.
+template <typename Retry>
+static PcoB200Error cold_decode_jobs(Context& c, uint32_t dtype, const std::vector<ColdJob>& jobs, Retry retry, std::vector<ColdResult>* res,
+                                     cudaStream_t stream) {
+  const size_t nj = jobs.size();
+  res->assign(nj, ColdResult{});
+  PCOB_CUDA_TRY(c.cold_res.reserve(nj * sizeof(ColdResult) + 64));
+  ColdResult* d_res = c.cold_res.as<ColdResult>();
+  std::vector<size_t> todo(nj);
+  for (size_t k = 0; k < nj; k++) todo[k] = k;
+  for (uint32_t window_cap : {16u, COLD_MAX_WINDOW_LOG}) {
+    if (todo.empty()) break;
+    PCOB_CUDA_TRY(c.cold.reserve(cold_scratch_bytes(window_cap)));
+    profiler().begin("cold_decode_kernel", stream);
+    for (size_t k : todo) {
+      const ColdJob& j = jobs[k];
+      dispatch_latent(dtype, [&](auto tag) {
+        using L = decltype(tag);
+        cold_decode_kernel<L><<<1, 32, 0, stream>>>(j.fp, j.first_byte, static_cast<L*>(j.out), j.cap, c.cold.as<uint8_t>(), window_cap, d_res + k);
+        return 0;
+      });
+    }
+    profiler().end(stream);
+    PCOB_CUDA_TRY(cudaGetLastError());
+    PCOB_CUDA_TRY(readback_small_sync(res->data(), d_res, nj * sizeof(ColdResult), stream));
+    std::vector<size_t> again;
+    for (size_t k : todo)
+      if (retry((*res)[k])) again.push_back(k);
+    todo.swap(again);
+  }
+  return PCO_B200_OK;
+}
+// A whole file is decoded again with the large window on any such refusal; a page or a range's chunk only if no chunk of it finished.
+static bool cold_retry_file(const ColdResult& r) { return r.status == ST_UNSUPPORTED; }
+static bool cold_retry_chunk(const ColdResult& r) { return r.n_chunks == 0 && r.status == ST_UNSUPPORTED; }
 
 // Index-free decompress, the parallel part (the reference's decompressor walks chunk after chunk, standalone/decompressor.rs:150-215;
 // so does this library's serial walk_kernel<<<1>>>, at one GPU thread's speed).  Chunk lengths are not in the file, but the chunks
@@ -303,16 +396,14 @@ static PcoB200Error speculative_walk_rounds(Context& c, const FileParams& fp, co
     m64 = std::min<uint64_t>(m64, fit + 8);  // a few more than fit: coincidences in front of the last chunk needed
     const uint32_t m = uint32_t(m64);
     const uint64_t chunks_offset = sizeof(IndexHeader);
-    const uint64_t entries_begin = (chunks_offset + uint64_t(m) * sizeof(IndexChunk) + 15) & ~uint64_t(15);
-    const uint64_t index_bytes = entries_begin + uint64_t(m) * stride;
     std::vector<IndexChunk> recs(m);
     for (uint32_t k = 0; k < m; k++) {
       recs[k].chunk_offset = cand[k];
       recs[k].n = n0;
       recs[k].n_vars = 0;
-      recs[k].entries_offset = entries_begin + uint64_t(k) * stride;
       recs[k].out_offset = 0;
     }
+    const uint64_t index_bytes = lay_out_entries(recs.data(), m, (chunks_offset + uint64_t(m) * sizeof(IndexChunk) + 15) & ~uint64_t(15));
     PCOB_CUDA_TRY(c.index.reserve(index_bytes + 64));
     uint8_t* d_index = c.index.as<uint8_t>();
     PCOB_CUDA_TRY(cudaMemcpyAsync(d_index + chunks_offset, recs.data(), size_t(m) * sizeof(IndexChunk), cudaMemcpyHostToDevice, stream));
@@ -370,72 +461,32 @@ static PcoB200Error decompress_fast(const void* compressed, size_t compressed_le
   const bool src_dev = flags & PCO_B200_SRC_ON_DEVICE, dst_dev = flags & PCO_B200_DST_ON_DEVICE;
   const size_t elem = nt_bits(dtype) / 8;
 
-  // 1. standalone header (host parse of the first bytes)
-  uint8_t head[32] = {0};
-  size_t avail = std::min<size_t>(compressed_len, sizeof(head));
-  // the file header and (when it lives on the device) the side index header come back in one round trip
+  // 1. standalone header (host parse of the first bytes); the side index header comes back in the same round trip
   const bool have_index = index != nullptr && index_len >= sizeof(IndexHeader);
   const bool idx_dev = flags & PCO_B200_INDEX_ON_DEVICE;
   IndexHeader ih;
-  std::memset(&ih, 0, sizeof(ih));
-  bool need_sync = false;
-  if (avail) {
-    if (src_dev) { PCOB_CUDA_TRY(cudaMemcpyAsync(head, compressed, avail, cudaMemcpyDeviceToHost, stream)); need_sync = true; }
-    else std::memcpy(head, compressed, avail);
-  }
-  if (have_index) {
-    if (idx_dev) { PCOB_CUDA_TRY(cudaMemcpyAsync(&ih, index, sizeof(ih), cudaMemcpyDeviceToHost, stream)); need_sync = true; }
-    else std::memcpy(&ih, index, sizeof(ih));
-  }
-  if (need_sync) PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
   StandaloneHeader hdr;
-  if (PcoB200Error e = parse_standalone_header(head, avail, compressed_len, &hdr)) return e;
+  if (PcoB200Error e = read_heads(compressed, compressed_len, src_dev, index, index_len, idx_dev, &ih, &hdr, stream)) return e;
 
   // 2. the file in HBM
   const uint8_t* d_src;
-  if (src_dev) d_src = static_cast<const uint8_t*>(compressed);
-  else {
-    PCOB_CUDA_TRY(c.src.reserve(compressed_len + 16));
-    call_trace().mark("d.begin");
-    PCOB_CUDA_TRY(copy_sliced(c.src.p, compressed, compressed_len, cudaMemcpyHostToDevice, stream));
-    call_trace().mark("d.h2d_submitted");
-    d_src = c.src.as<uint8_t>();
-  }
-  FileParams fp;
-  fp.src = d_src;
-  fp.src_len = compressed_len;
-  fp.dtype = dtype;
-  fp.uniform_type = hdr.uniform_type;
-  fp.format_major = hdr.format_major;
+  call_trace().mark("d.begin");
+  if (PcoB200Error e = stage_in(c.src, compressed, compressed_len, src_dev, stream, &d_src)) return e;
+  call_trace().mark("d.h2d_submitted");
+  const FileParams fp{d_src, compressed_len, dtype, hdr.uniform_type, hdr.format_major};
 
   // 3a. caller-supplied side index
   if (have_index) {
-    // overflow-safe: the chunk table must lie inside the index; per-chunk fields are bounded on the device (entries inside the
-    // index, chunk_offset inside the file, writes inside the destination)
-    if (ih.magic != INDEX_MAGIC || ih.version != 1 || ih.file_len != compressed_len || ih.chunks_offset > index_len ||
-        ih.n_chunks > (index_len - ih.chunks_offset) / sizeof(IndexChunk))
-      return fail(PCO_B200_INVALID_ARGUMENT, "side index does not belong to this file");
-    const uint8_t* d_idx = static_cast<const uint8_t*>(index);
-    if (!idx_dev) {
-      PCOB_CUDA_TRY(c.index.reserve(index_len));
-      PCOB_CUDA_TRY(copy_sliced(c.index.p, index, index_len, cudaMemcpyHostToDevice, stream));
-      d_idx = c.index.as<uint8_t>();
-    }
+    if (!index_header_ok(ih, compressed_len, index_len)) return fail(PCO_B200_INVALID_ARGUMENT, "side index does not belong to this file");
+    const uint8_t* d_idx;
+    if (PcoB200Error e = stage_in(c.index, index, index_len, idx_dev, stream, &d_idx)) return e;
     uint64_t n_emit = std::min<uint64_t>(ih.n_total, dst_len);
-    void* d_out = dst;
-    bool dst_in_place = false;
-    if (!dst_dev) {
-      // a page-locked destination is written in place by the decode kernels (every number is stored once, in 32-byte pieces that a
-      // warp lays down as 1 KiB runs): no staging buffer, no copy behind the kernel (host_common.hpp, zero copy)
-      void* in_place = (zero_copy_mask().load(std::memory_order_relaxed) & 2) ? mapped_host_ptr(dst) : nullptr;
-      if (in_place) {
-        d_out = in_place;
-        dst_in_place = true;
-      } else {
-        PCOB_CUDA_TRY(c.out.reserve(n_emit * elem + 64));
-        d_out = c.out.p;
-      }
-    }
+    // a page-locked destination is written in place by the decode kernels (every number is stored once, in 32-byte pieces that a
+    // warp lays down as 1 KiB runs): no staging buffer, no copy behind the kernel (host_common.hpp, zero copy)
+    void* d_out = !dst_dev && (zero_copy_mask().load(std::memory_order_relaxed) & 2) ? mapped_host_ptr(dst) : nullptr;
+    const bool dst_in_place = d_out != nullptr;
+    if (!dst_in_place)
+      if (PcoB200Error e = out_buffer(c, dst, dst_dev, n_emit * elem, &d_out)) return e;
     if (ih.n_chunks > 0xffffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "too many chunks");
     // a host destination holds (or is staged in c.out, which holds) n_emit numbers: that is the kernels' bound, whatever the index claims
     if (PcoB200Error e = launch_decode(c, fp, d_idx, index_len, ih.chunks_offset, uint32_t(ih.n_chunks), d_out, dst_dev ? uint64_t(dst_len) : n_emit, stream)) return e;
@@ -517,43 +568,16 @@ static PcoB200Error decompress_cold(const void* compressed, size_t compressed_le
   cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
   const bool src_dev = flags & PCO_B200_SRC_ON_DEVICE, dst_dev = flags & PCO_B200_DST_ON_DEVICE;
   const size_t elem = nt_bits(dtype) / 8;
-  uint8_t head[32] = {0};
-  const size_t avail = std::min<size_t>(compressed_len, sizeof(head));
-  if (avail) {
-    if (src_dev) { PCOB_CUDA_TRY(cudaMemcpyAsync(head, compressed, avail, cudaMemcpyDeviceToHost, stream)); PCOB_CUDA_TRY(cudaStreamSynchronize(stream)); }
-    else std::memcpy(head, compressed, avail);
-  }
   StandaloneHeader hdr;
-  if (PcoB200Error e = parse_standalone_header(head, avail, compressed_len, &hdr)) return e;
-  const uint8_t* d_src = static_cast<const uint8_t*>(compressed);
-  if (!src_dev) {
-    PCOB_CUDA_TRY(c.src.reserve(compressed_len + 16));
-    PCOB_CUDA_TRY(copy_sliced(c.src.p, compressed, compressed_len, cudaMemcpyHostToDevice, stream));
-    d_src = c.src.as<uint8_t>();
-  }
-  FileParams fp{d_src, compressed_len, dtype, hdr.uniform_type, hdr.format_major};
-  void* d_out = dst;
-  if (!dst_dev) {
-    PCOB_CUDA_TRY(c.out.reserve(dst_len * elem + 64));
-    d_out = c.out.p;
-  }
-  PCOB_CUDA_TRY(c.misc.reserve(256));
-  ColdResult* d_res = reinterpret_cast<ColdResult*>(c.misc.as<uint8_t>() + 160);
-  ColdResult res;
-  for (uint32_t window_cap : {16u, COLD_MAX_WINDOW_LOG}) {  // lookback windows beyond 2^16 numbers get the large scratch on a second try
-    PCOB_CUDA_TRY(c.cold.reserve(cold_scratch_bytes(window_cap)));
-    profiler().begin("cold_decode_kernel", stream);
-    dispatch_latent(dtype, [&](auto tag) {
-      using L = decltype(tag);
-      cold_decode_kernel<L><<<1, 32, 0, stream>>>(fp, hdr.first_chunk_byte, static_cast<L*>(d_out), uint64_t(dst_len), c.cold.as<uint8_t>(), window_cap, d_res);
-      return 0;
-    });
-    profiler().end(stream);
-    PCOB_CUDA_TRY(cudaGetLastError());
-    PCOB_CUDA_TRY(cudaMemcpyAsync(&res, d_res, sizeof(res), cudaMemcpyDeviceToHost, stream));
-    PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
-    if (res.status != ST_UNSUPPORTED) break;
-  }
+  if (PcoB200Error e = read_heads(compressed, compressed_len, src_dev, nullptr, 0, false, nullptr, &hdr, stream)) return e;
+  const uint8_t* d_src;
+  if (PcoB200Error e = stage_in(c.src, compressed, compressed_len, src_dev, stream, &d_src)) return e;
+  void* d_out;
+  if (PcoB200Error e = out_buffer(c, dst, dst_dev, uint64_t(dst_len) * elem, &d_out)) return e;
+  const FileParams fp{d_src, compressed_len, dtype, hdr.uniform_type, hdr.format_major};
+  std::vector<ColdResult> cres;
+  if (PcoB200Error e = cold_decode_jobs(c, dtype, {ColdJob{fp, hdr.first_chunk_byte, d_out, uint64_t(dst_len)}}, cold_retry_file, &cres, stream)) return e;
+  const ColdResult& res = cres[0];
   // like the walk path: the chunks before a failing one have been emitted (the reference's decoder stops where the error is)
   const uint64_t n_emit = std::min<uint64_t>(res.n_total, dst_len);
   if (!dst_dev && n_emit) {
@@ -932,20 +956,11 @@ int pco_b200_zero_copy(int mask) { return mask < 0 ? zero_copy_mask().load() : z
 // thread's next call).
 void pco_b200_thread_release(void) {
   Context& c = ctx();
-  if (c.initialized && c.device_ok) {
-    release_buffers(c);
-    // release_buffers also frees the binomial table that ensure_device builds once per context: mark the context uninitialised so that
-    // a later call on this thread builds it again.  Left initialised, the next decode that reached decode_kernel read a null table
-    // (an illegal address) - a thread that releases its scratch between calls instead of exiting.
-    c.initialized = false;
-    c.device_ok = false;
-    c.attrs_set = false;
-    c.ranges_attrs_set = false;
-  }
+  if (c.initialized && c.device_ok) reset_context(c);
   readback_bounce().release();
 }
 // Which decode instantiation served the chunks of the last decode launch: counts[k] = chunks of class k
-// (1, 2: decode_kernel<L, 1 / 2>; 3, 4: decode_narrow_kernel order 0 / 1).  Returns the number of chunks.
+// (1, 2: decode_kernel<L, 1 / 2>; 3, 4, 5: fused_narrow_kernel, delta order 0 / 1 / 2..7).  Returns the number of chunks.
 int pco_b200_profile_chunk_classes(unsigned* counts8) {
   Context& c = ctx();
   for (int i = 0; i < 8; i++) counts8[i] = 0;
@@ -1022,28 +1037,22 @@ PcoB200Error pco_b200_decompress_chunks(const void* compressed, size_t compresse
   // index skeleton: chunk records from the caller's table, room for 2 vars of entries per chunk
   const uint64_t chunks_offset = sizeof(IndexHeader);
   std::vector<IndexChunk> recs(n_chunks);
-  uint64_t off = (chunks_offset + uint64_t(n_chunks) * sizeof(IndexChunk) + 15) & ~uint64_t(15), out_off = 0;
+  uint64_t out_off = 0;
   for (size_t i = 0; i < n_chunks; i++) {
     if (chunk_offsets[i] >= compressed_len) return fail(PCO_B200_INVALID_ARGUMENT, "chunk offset " + std::to_string(i) + " lies outside the buffer");
     if (chunk_ns[i] == 0 || chunk_ns[i] > (1u << 24)) return fail(PCO_B200_INVALID_ARGUMENT, "chunk " + std::to_string(i) + ": count must be 1..2^24");
     recs[i].chunk_offset = chunk_offsets[i];
     recs[i].n = chunk_ns[i];
     recs[i].n_vars = 0;
-    recs[i].entries_offset = off;
     recs[i].out_offset = out_off;
-    off += (uint64_t(MAX_VARS) * n_batches_of(chunk_ns[i]) * sizeof(BatchEntry) + 15) & ~uint64_t(15);
     out_off += chunk_ns[i];
   }
+  const uint64_t off = lay_out_entries(recs.data(), n_chunks, (chunks_offset + uint64_t(n_chunks) * sizeof(IndexChunk) + 15) & ~uint64_t(15));
   const uint64_t n_total = out_off;
   if (n_total > dst_len) return fail(PCO_B200_INVALID_ARGUMENT, "dst holds " + std::to_string(dst_len) + " numbers, the chunks " + std::to_string(n_total));
   const uint8_t* d_src;
-  if (src_dev) d_src = static_cast<const uint8_t*>(compressed);
-  else {
-    PCOB_CUDA_TRY(c.src.reserve(compressed_len + 16));
-    PCOB_CUDA_TRY(copy_sliced(c.src.p, compressed, compressed_len, cudaMemcpyHostToDevice, stream));
-    d_src = c.src.as<uint8_t>();
-  }
-  FileParams fp{d_src, compressed_len, dtype, uniform_type, format_major};
+  if (PcoB200Error e = stage_in(c.src, compressed, compressed_len, src_dev, stream, &d_src)) return e;
+  const FileParams fp{d_src, compressed_len, dtype, uniform_type, format_major};
   PCOB_CUDA_TRY(c.index.reserve(off + 64));
   uint8_t* d_index = c.index.as<uint8_t>();
   PCOB_CUDA_TRY(cudaMemcpyAsync(d_index + chunks_offset, recs.data(), n_chunks * sizeof(IndexChunk), cudaMemcpyHostToDevice, stream));
@@ -1062,11 +1071,8 @@ PcoB200Error pco_b200_decompress_chunks(const void* compressed, size_t compresse
     for (size_t i = 0; i < n_chunks; i++)
       if (st[i] != ST_OK) { profiler().resolve(); return status_to_error(st[i], ("chunk " + std::to_string(i)).c_str()); }
   }
-  void* d_out = dst;
-  if (!dst_dev) {
-    PCOB_CUDA_TRY(c.out.reserve(n_total * elem + 64));
-    d_out = c.out.p;
-  }
+  void* d_out;
+  if (PcoB200Error e = out_buffer(c, dst, dst_dev, n_total * elem, &d_out)) return e;
   PcoB200Error e = launch_decode(c, fp, d_index, off, chunks_offset, uint32_t(n_chunks), d_out, dst_dev ? uint64_t(dst_len) : n_total, stream);
   profiler().resolve();
   if (e != PCO_B200_OK) return e;
@@ -1103,7 +1109,6 @@ static PcoB200Error decompress_pages_impl(const void* metas, size_t metas_len, c
   if ((!metas && metas_len) || (!pages && pages_len) || !dst) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
   // page table, and the index skeleton: one IndexChunk per page plus a spare one (a failing page walked on its own)
   const uint64_t chunks_offset = sizeof(IndexHeader);
-  uint64_t entries = (chunks_offset + (uint64_t(n_pages) + 1) * sizeof(IndexChunk) + 15) & ~uint64_t(15);
   std::vector<WrappedPage> tab(n_pages);
   std::vector<IndexChunk> recs(n_pages + 1);
   uint64_t frames_len = 0, n_total = 0;
@@ -1118,29 +1123,21 @@ static PcoB200Error decompress_pages_impl(const void* metas, size_t metas_len, c
     recs[i].chunk_offset = frames_len;
     recs[i].n = uint32_t(r.page_n);
     recs[i].n_vars = 0;
-    recs[i].entries_offset = entries;
     recs[i].out_offset = n_total;
-    entries += (uint64_t(MAX_VARS) * n_batches_of(uint32_t(r.page_n)) * sizeof(BatchEntry) + 15) & ~uint64_t(15);
     frames_len += (4 + r.meta_len + r.page_len + 15) & ~uint64_t(15);  // 16-byte aligned chunk starts for the kernels' block reads
     n_total += r.page_n;
   }
   if (n_total > dst_len) return fail(PCO_B200_INVALID_ARGUMENT, "dst holds " + std::to_string(dst_len) + " numbers, the pages " + std::to_string(n_total));
+  const uint64_t entries = lay_out_entries(recs.data(), n_pages, (chunks_offset + (uint64_t(n_pages) + 1) * sizeof(IndexChunk) + 15) & ~uint64_t(15));
 
   Context& c = ctx();
   if (PcoB200Error e = ensure_device(c)) return e;
   const bool src_dev = flags & PCO_B200_SRC_ON_DEVICE, dst_dev = flags & PCO_B200_DST_ON_DEVICE;
   const size_t elem = nt_bits(dtype) / 8;
   const uint32_t n = uint32_t(n_pages);
-  const uint8_t* d_metas = static_cast<const uint8_t*>(metas);
-  const uint8_t* d_pages = static_cast<const uint8_t*>(pages);
-  if (!src_dev) {
-    PCOB_CUDA_TRY(c.wrap_metas.reserve(metas_len + 16));
-    PCOB_CUDA_TRY(c.src.reserve(pages_len + 16));
-    if (metas_len) PCOB_CUDA_TRY(copy_sliced(c.wrap_metas.p, metas, metas_len, cudaMemcpyHostToDevice, stream));
-    if (pages_len) PCOB_CUDA_TRY(copy_sliced(c.src.p, pages, pages_len, cudaMemcpyHostToDevice, stream));
-    d_metas = c.wrap_metas.as<uint8_t>();
-    d_pages = c.src.as<uint8_t>();
-  }
+  const uint8_t *d_metas, *d_pages;
+  if (PcoB200Error e = stage_in(c.wrap_metas, metas, metas_len, src_dev, stream, &d_metas)) return e;
+  if (PcoB200Error e = stage_in(c.src, pages, pages_len, src_dev, stream, &d_pages)) return e;
   PCOB_CUDA_TRY(c.wrap_tab.reserve(n_pages * sizeof(WrappedPage)));
   PCOB_CUDA_TRY(cudaMemcpyAsync(c.wrap_tab.p, tab.data(), n_pages * sizeof(WrappedPage), cudaMemcpyHostToDevice, stream));
   PCOB_CUDA_TRY(c.index.reserve(entries + 64));
@@ -1211,11 +1208,8 @@ static PcoB200Error decompress_pages_impl(const void* metas, size_t metas_len, c
     break;
   }
 
-  void* d_out = dst;
-  if (!dst_dev) {
-    PCOB_CUDA_TRY(c.out.reserve(n_total * elem + 64));
-    d_out = c.out.p;
-  }
+  void* d_out;
+  if (PcoB200Error e = out_buffer(c, dst, dst_dev, n_total * elem, &d_out)) return e;
   const uint64_t out_len = dst_dev ? uint64_t(dst_len) : n_total;
   // ---- fast pages: the ordinary decode over their walked index records
   if (!fast.empty()) {
@@ -1227,17 +1221,13 @@ static PcoB200Error decompress_pages_impl(const void* metas, size_t metas_len, c
       for (uint32_t i : fast) sel.push_back(walked[i]);
       PCOB_CUDA_TRY(cudaMemcpyAsync(d_index + chunks_offset, sel.data(), sel.size() * sizeof(IndexChunk), cudaMemcpyHostToDevice, stream));
     }
-    if (PcoB200Error e = launch_decode(c, fp, d_index, entries, chunks_offset, uint32_t(fast.size()), d_out, out_len, stream)) {
+    uint32_t bad = 0;  // the first failing chunk of the launch: the bad-th fast page
+    if (PcoB200Error e = launch_decode(c, fp, d_index, entries, chunks_offset, uint32_t(fast.size()), d_out, out_len, stream, &bad)) {
       if (e == PCO_B200_CUDA) return e;
-      // launch_decode names the first failing chunk of its launch ("... in chunk k"): the k-th fast page
-      const std::string msg = last_error_ref();
-      const size_t at = msg.rfind("chunk ");
-      const size_t k = at == std::string::npos ? 0 : size_t(std::strtoull(msg.c_str() + at + 6, nullptr, 10));
-      const size_t page = fast[std::min(k, fast.size() - 1)];
-      if (page < fail_page) {
-        fail_page = page;
+      if (fast[bad] < fail_page) {
+        fail_page = fast[bad];
         decode_kind = e;
-        decode_msg = msg;
+        decode_msg = last_error_ref();
       }
     }
   }
@@ -1247,32 +1237,14 @@ static PcoB200Error decompress_pages_impl(const void* metas, size_t metas_len, c
   // decoder would read those as the next chunk.
   if (!cold.empty()) {
     const size_t nc = cold.size();
-    PCOB_CUDA_TRY(c.wrap_res.reserve(nc * sizeof(ColdResult) + 64));
-    ColdResult* d_cres = c.wrap_res.as<ColdResult>();
-    std::vector<ColdResult> cres(nc);
-    std::vector<size_t> todo(nc);
-    for (size_t k = 0; k < nc; k++) todo[k] = k;
-    for (uint32_t window_cap : {16u, COLD_MAX_WINDOW_LOG}) {  // lookback windows beyond 2^16 numbers get the large scratch on a second pass
-      if (todo.empty()) break;
-      PCOB_CUDA_TRY(c.cold.reserve(cold_scratch_bytes(window_cap)));
-      profiler().begin("cold_decode_kernel", stream);
-      for (size_t k : todo) {
-        const WrappedPage& w = tab[cold[k]];
-        const FileParams fpk{d_frames + w.frame_off, 4 + w.meta_len + w.page_len, dtype, 0, 4};
-        dispatch_latent(dtype, [&](auto tag) {
-          using L = decltype(tag);
-          cold_decode_kernel<L><<<1, 32, 0, stream>>>(fpk, 0, static_cast<L*>(d_out) + recs[cold[k]].out_offset, w.page_n, c.cold.as<uint8_t>(), window_cap, d_cres + k);
-          return 0;
-        });
-      }
-      profiler().end(stream);
-      PCOB_CUDA_TRY(cudaGetLastError());
-      PCOB_CUDA_TRY(readback_small_sync(cres.data(), d_cres, nc * sizeof(ColdResult), stream));
-      std::vector<size_t> again;
-      for (size_t k : todo)
-        if (cres[k].n_chunks == 0 && cres[k].status == ST_UNSUPPORTED) again.push_back(k);
-      todo.swap(again);
+    std::vector<ColdJob> jobs;
+    for (uint32_t i : cold) {
+      const WrappedPage& w = tab[i];
+      jobs.push_back(ColdJob{FileParams{d_frames + w.frame_off, 4 + w.meta_len + w.page_len, dtype, 0, 4}, 0,
+                             static_cast<uint8_t*>(d_out) + recs[i].out_offset * elem, w.page_n});
     }
+    std::vector<ColdResult> cres;
+    if (PcoB200Error e = cold_decode_jobs(c, dtype, jobs, cold_retry_chunk, &cres, stream)) return e;
     // the page is decoded once its chunk is (what the decoder reads behind it is not the page's)
     for (size_t k = 0; k < nc; k++)
       if (cres[k].n_chunks == 0) {
@@ -1714,12 +1686,8 @@ static PcoB200Error decompress_files_impl(const void* src, size_t src_len, const
   };
 
   // ---- the bytes in HBM: src, and the arena = [the caller's index | walked records and entries | the merged chunk list]
-  const uint8_t* d_src = static_cast<const uint8_t*>(src);
-  if (!src_dev) {
-    PCOB_CUDA_TRY(c.src.reserve(src_len + 16));
-    if (src_len) PCOB_CUDA_TRY(copy_sliced(c.src.p, src, src_len, cudaMemcpyHostToDevice, stream));
-    d_src = c.src.as<uint8_t>();
-  }
+  const uint8_t* d_src;
+  if (PcoB200Error e = stage_in(c.src, src, src_len, src_dev, stream, &d_src)) return e;
   uint64_t arena_end = any_index ? (uint64_t(index_len) + 15) & ~uint64_t(15) : 0;
   PCOB_CUDA_TRY(c.files_arena.reserve(arena_end + 64));
   if (any_index) PCOB_CUDA_TRY(copy_sliced(c.files_arena.p, index, index_len, idx_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, stream));
@@ -1783,8 +1751,7 @@ static PcoB200Error decompress_files_impl(const void* src, size_t src_len, const
         std::memcpy(&ih, iheads.data() + wi * sizeof(IndexHeader), sizeof(ih));
         wi++;
         // as decompress_ex checks it; the chunk table must also be 8-byte aligned for the kernels' loads
-        if (ih.magic != INDEX_MAGIC || ih.version != 1 || ih.file_len != r.len || ih.chunks_offset > r.index_len || ih.chunks_offset % 8 != 0 ||
-            ih.n_chunks > (r.index_len - ih.chunks_offset) / sizeof(IndexChunk)) {
+        if (!index_header_ok(ih, r.len, r.index_len) || ih.chunks_offset % 8 != 0) {
           fail_at(i, PCO_B200_INVALID_ARGUMENT, "side index does not belong to this file");
           break;
         }
@@ -1872,7 +1839,6 @@ static PcoB200Error decompress_files_impl(const void* src, size_t src_len, const
     std::vector<size_t> first_rec;          // its first record
     uint64_t budget = INDEX_BUDGET;
     const uint64_t chunks_at = (arena_end + 15) & ~uint64_t(15);
-    std::vector<uint64_t> strides;
     for (uint32_t s : scan_order) {
       const uint32_t i = scan_file[s];
       std::vector<uint64_t>& cs = cand[s];
@@ -1886,24 +1852,18 @@ static PcoB200Error decompress_files_impl(const void* src, size_t src_len, const
       cs.resize(m);
       walked.push_back(uint32_t(s));
       first_rec.push_back(recs.size());
-      strides.push_back(stride);
       for (uint64_t k = 0; k < m; k++) {
         IndexChunk ic;
         ic.chunk_offset = cs[k];
         ic.n = n0;
         ic.n_vars = 0;
-        ic.entries_offset = 0;  // below
         ic.out_offset = 0;
         recs.push_back(ic);
       }
     }
     if (recs.empty()) break;
     const uint32_t mt = uint32_t(recs.size());
-    uint64_t e_at = (chunks_at + uint64_t(mt) * sizeof(IndexChunk) + 15) & ~uint64_t(15);
-    for (size_t w = 0; w < walked.size(); w++) {
-      const size_t r1 = w + 1 < walked.size() ? first_rec[w + 1] : recs.size();
-      for (size_t r = first_rec[w]; r < r1; r++) { recs[r].entries_offset = e_at; e_at += strides[w]; }
-    }
+    const uint64_t e_at = lay_out_entries(recs.data(), mt, (chunks_at + uint64_t(mt) * sizeof(IndexChunk) + 15) & ~uint64_t(15));
     PCOB_CUDA_TRY(c.files_arena.grow_preserve(e_at + 64, arena_end, stream));
     PCOB_CUDA_TRY(c.spec.reserve(64 + size_t(CAND_CAP) * (8 + 4) + size_t(mt) * (4 + 8) + 64));
     uint32_t* d_stat = reinterpret_cast<uint32_t*>(c.spec.as<uint8_t>() + 64 + size_t(CAND_CAP) * 12);
@@ -2050,22 +2010,9 @@ static PcoB200Error decompress_files_impl(const void* src, size_t src_len, const
   // ---- cold files, and indexed files that decode on their own: their count is only known once decoded, so they decode into scratch first
   auto cold_decode = [&](const BatchFile& f, void* out, uint64_t cap, ColdResult* res) -> PcoB200Error {
     const FileParams fpf{d_src + f.begin, f.end - f.begin, dtype, f.hdr.uniform_type, f.hdr.format_major};
-    PCOB_CUDA_TRY(c.misc.reserve(256));
-    ColdResult* d_cres = reinterpret_cast<ColdResult*>(c.misc.as<uint8_t>() + 160);
-    for (uint32_t window_cap : {16u, COLD_MAX_WINDOW_LOG}) {  // lookback windows beyond 2^16 numbers get the large scratch on a second try
-      PCOB_CUDA_TRY(c.cold.reserve(cold_scratch_bytes(window_cap)));
-      profiler().begin("cold_decode_kernel", stream);
-      dispatch_latent(dtype, [&](auto tag) {
-        using L = decltype(tag);
-        cold_decode_kernel<L><<<1, 32, 0, stream>>>(fpf, f.hdr.first_chunk_byte, static_cast<L*>(out), cap, c.cold.as<uint8_t>(), window_cap, d_cres);
-        return 0;
-      });
-      profiler().end(stream);
-      PCOB_CUDA_TRY(cudaGetLastError());
-      PCOB_CUDA_TRY(cudaMemcpyAsync(res, d_cres, sizeof(*res), cudaMemcpyDeviceToHost, stream));
-      PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
-      if (res->status != ST_UNSUPPORTED) break;
-    }
+    std::vector<ColdResult> cres;
+    if (PcoB200Error e = cold_decode_jobs(c, dtype, {ColdJob{fpf, f.hdr.first_chunk_byte, out, cap}}, cold_retry_file, &cres, stream)) return e;
+    *res = cres[0];
     return PCO_B200_OK;
   };
   uint64_t staged_end = 0;
@@ -2117,11 +2064,8 @@ static PcoB200Error decompress_files_impl(const void* src, size_t src_len, const
     bf[i].out_base = total;
     total += bf[i].count;
   }
-  void* d_out = dst;
-  if (!dst_dev) {
-    PCOB_CUDA_TRY(c.out.reserve(total * elem + 64));
-    d_out = c.out.p;
-  }
+  void* d_out;
+  if (PcoB200Error e = out_buffer(c, dst, dst_dev, total * elem, &d_out)) return e;
   const uint64_t out_len = dst_dev ? uint64_t(dst_len) : total;
 
   // ---- 4. one chunk list for the fast kernels, grouped by (uniform type, format major)
@@ -2176,13 +2120,13 @@ static PcoB200Error decompress_files_impl(const void* src, size_t src_len, const
         while (hi < b && slots[hi].file < limit) hi++;  // files from the lowest failure on need no decoding
         if (hi == a) continue;
         const uint64_t first = slots[a].at, cnt = slots[hi - 1].at + slots[hi - 1].n - first;
-        const PcoB200Error e = launch_decode(c, fp, arena(), arena_len, list_at + first * sizeof(IndexChunk), uint32_t(cnt), d_out, out_len, stream);
+        uint32_t bad = 0;
+        const PcoB200Error e = launch_decode(c, fp, arena(), arena_len, list_at + first * sizeof(IndexChunk), uint32_t(cnt), d_out, out_len, stream, &bad);
         if (e == PCO_B200_OK) continue;
         if (e == PCO_B200_CUDA) return e;
-        // launch_decode names the first failing chunk of its launch ("... chunk k"): find its file
+        // the first failing chunk of the launch: find its file
         const std::string msg = last_error_ref();
-        const size_t at = msg.rfind("chunk ");
-        const uint64_t k = first + (at == std::string::npos ? 0 : std::strtoull(msg.c_str() + at + 6, nullptr, 10));
+        const uint64_t k = first + bad;
         size_t s = a;
         while (s + 1 < hi && slots[s + 1].at <= k) s++;
         const uint32_t fi = slots[s].file;
@@ -2330,27 +2274,11 @@ static PcoB200Error decompress_ranges_impl(const void* compressed, size_t compre
   if (src_dev || idx_dev)
     if (PcoB200Error e = ensure_device(c)) return e;
   // the file header and the index header: host copies, or one readback
-  uint8_t head[32] = {0};
-  const size_t avail = std::min<size_t>(compressed_len, sizeof(head));
   IndexHeader ih;
-  std::memset(&ih, 0, sizeof(ih));
-  const bool ih_fits = index_len >= sizeof(IndexHeader);
-  bool need_sync = false;
-  if (avail) {
-    if (src_dev) { PCOB_CUDA_TRY(cudaMemcpyAsync(head, compressed, avail, cudaMemcpyDeviceToHost, stream)); need_sync = true; }
-    else std::memcpy(head, compressed, avail);
-  }
-  if (ih_fits) {
-    if (idx_dev) { PCOB_CUDA_TRY(cudaMemcpyAsync(&ih, index, sizeof(ih), cudaMemcpyDeviceToHost, stream)); need_sync = true; }
-    else std::memcpy(&ih, index, sizeof(ih));
-  }
-  if (need_sync) PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
   StandaloneHeader hdr;
-  if (PcoB200Error e = parse_standalone_header(head, avail, compressed_len, &hdr)) return e;
+  if (PcoB200Error e = read_heads(compressed, compressed_len, src_dev, index, index_len, idx_dev, &ih, &hdr, stream)) return e;
   // the same check as the side-index path of pco_b200_decompress_ex
-  if (!ih_fits || ih.magic != INDEX_MAGIC || ih.version != 1 || ih.file_len != compressed_len || ih.chunks_offset > index_len ||
-      ih.n_chunks > (index_len - ih.chunks_offset) / sizeof(IndexChunk))
-    return fail(PCO_B200_INVALID_ARGUMENT, "side index does not belong to this file");
+  if (!index_header_ok(ih, compressed_len, index_len)) return fail(PCO_B200_INVALID_ARGUMENT, "side index does not belong to this file");
   if (ih.n_chunks > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "too many chunks");
   // the chunk table: a host copy, or a second readback
   std::vector<IndexChunk> recs(ih.n_chunks);
@@ -2375,23 +2303,12 @@ static PcoB200Error decompress_ranges_impl(const void* compressed, size_t compre
 
   // ---- the file, the index and the destination in HBM
   if (PcoB200Error e = ensure_device(c)) return e;
-  const uint8_t* d_src = static_cast<const uint8_t*>(compressed);
-  if (!src_dev) {
-    PCOB_CUDA_TRY(c.src.reserve(compressed_len + 16));
-    PCOB_CUDA_TRY(copy_sliced(c.src.p, compressed, compressed_len, cudaMemcpyHostToDevice, stream));
-    d_src = c.src.as<uint8_t>();
-  }
-  const uint8_t* d_idx = static_cast<const uint8_t*>(index);
-  if (!idx_dev) {
-    PCOB_CUDA_TRY(c.index.reserve(index_len));
-    PCOB_CUDA_TRY(copy_sliced(c.index.p, index, index_len, cudaMemcpyHostToDevice, stream));
-    d_idx = c.index.as<uint8_t>();
-  }
-  uint8_t* d_out = static_cast<uint8_t*>(dst);
-  if (!dst_dev) {
-    PCOB_CUDA_TRY(c.out.reserve(total * elem + 64));
-    d_out = c.out.as<uint8_t>();
-  }
+  const uint8_t *d_src, *d_idx;
+  if (PcoB200Error e = stage_in(c.src, compressed, compressed_len, src_dev, stream, &d_src)) return e;
+  if (PcoB200Error e = stage_in(c.index, index, index_len, idx_dev, stream, &d_idx)) return e;
+  void* d_out_v;
+  if (PcoB200Error e = out_buffer(c, dst, dst_dev, total * elem, &d_out_v)) return e;
+  uint8_t* d_out = static_cast<uint8_t*>(d_out_v);
   const FileParams fp{d_src, compressed_len, dtype, hdr.uniform_type, hdr.format_major};
   const uint32_t T = uint32_t(tasks.size());
   auto align16 = [](uint64_t x) { return (x + 15) & ~uint64_t(15); };
@@ -2425,19 +2342,7 @@ static PcoB200Error decompress_ranges_impl(const void* compressed, size_t compre
   PCOB_CUDA_TRY(c.statuses.reserve(res_bytes + 64));
   uint32_t* d_st = c.statuses.as<uint32_t>();
   uint8_t* d_cls = reinterpret_cast<uint8_t*>(d_st + T);
-  if (!c.ranges_attrs_set) {
-    c.ranges_attrs_set = true;
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(symwalk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SymWalkSmem)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(symwalk_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint64_t, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint32_t, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint16_t, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint8_t, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint64_t, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint32_t, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint16_t, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(fused_narrow_kernel<uint8_t, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-  }
+  if (PcoB200Error e = set_decode_attrs<true>(c)) return e;
 
   // ---- 1. fused_narrow_kernel decodes the narrow chunks' windows and classifies the rest
   profiler().begin("fused_narrow_kernel", stream);
@@ -2473,7 +2378,7 @@ static PcoB200Error decompress_ranges_impl(const void* compressed, size_t compre
     PCOB_CUDA_TRY(cudaMemcpyAsync(d_wins, wins.data(), size_t(T) * sizeof(WinTask), cudaMemcpyHostToDevice, stream));
     profiler().begin("symwalk_kernel", stream);
     symwalk_kernel<true><<<T, SW_THREADS, sizeof(SymWalkSmem), stream>>>(fp, d_tasks, d_idx, index_len, 0, c.dec_syms.as<uint8_t>(), c.dec_offs.as<uint32_t>(),
-                                                                          d_cls, nullptr, 1, d_wins);
+                                                                          d_cls, d_wins);
     profiler().end(stream);
     profiler().begin("decode_kernel", stream);
     dispatch_latent(dtype, [&](auto tag) {
@@ -2508,32 +2413,10 @@ static PcoB200Error decompress_ranges_impl(const void* compressed, size_t compre
     PCOB_CUDA_TRY(c.rng_cold.reserve(cold_bytes + 64));
     d_cold = c.rng_cold.as<uint8_t>();
     const size_t nc = cold.size();
-    PCOB_CUDA_TRY(c.rng_res.reserve(nc * sizeof(ColdResult) + 64));
-    ColdResult* d_cres = c.rng_res.as<ColdResult>();
-    std::vector<ColdResult> cres(nc);
-    std::vector<size_t> todo(nc);
-    for (size_t k = 0; k < nc; k++) todo[k] = k;
-    for (uint32_t window_cap : {16u, COLD_MAX_WINDOW_LOG}) {  // lookback windows beyond 2^16 numbers get the large scratch on a second pass
-      if (todo.empty()) break;
-      PCOB_CUDA_TRY(c.cold.reserve(cold_scratch_bytes(window_cap)));
-      profiler().begin("cold_decode_kernel", stream);
-      for (size_t k : todo) {
-        const uint32_t t = cold[k];
-        dispatch_latent(dtype, [&](auto tag) {
-          using L = decltype(tag);
-          cold_decode_kernel<L><<<1, 32, 0, stream>>>(fp, trec[t].chunk_offset, reinterpret_cast<L*>(d_cold + cold_slot[t]), tasks[t].hi, c.cold.as<uint8_t>(),
-                                                      window_cap, d_cres + k);
-          return 0;
-        });
-      }
-      profiler().end(stream);
-      PCOB_CUDA_TRY(cudaGetLastError());
-      PCOB_CUDA_TRY(readback_small_sync(cres.data(), d_cres, nc * sizeof(ColdResult), stream));
-      std::vector<size_t> again;
-      for (size_t k : todo)
-        if (cres[k].n_chunks == 0 && cres[k].status == ST_UNSUPPORTED) again.push_back(k);
-      todo.swap(again);
-    }
+    std::vector<ColdJob> jobs;
+    for (uint32_t t : cold) jobs.push_back(ColdJob{fp, trec[t].chunk_offset, d_cold + cold_slot[t], tasks[t].hi});
+    std::vector<ColdResult> cres;
+    if (PcoB200Error e = cold_decode_jobs(c, dtype, jobs, cold_retry_chunk, &cres, stream)) return e;
     for (size_t k = 0; k < nc; k++) {
       const uint32_t s = cres[k].status;
       st[cold[k]] = cres[k].n_chunks > 0 ? ST_OK : (s == ST_OK || s == ST_TERMINATOR || s == ST_DST_FULL) ? ST_CORRUPTION : s;
@@ -2643,7 +2526,7 @@ PcoB200Error pco_b200_decompress_async_plan(const void* head, size_t head_len, u
   // the call launches loaded now (with lazy module loading a kernel is otherwise loaded at its first launch)
   Context& c = ctx();
   if (PcoB200Error e = ensure_device(c)) return e;
-  if (PcoB200Error e = set_decode_attrs(c)) return e;
+  if (PcoB200Error e = set_decode_attrs<false>(c)) return e;
   cudaFuncAttributes fa;
   PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, async_check_kernel));
   PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, async_finish_kernel));
@@ -2702,7 +2585,7 @@ PcoB200Error pco_b200_decompress_async(const PcoB200AsyncPlan* plan, const void*
   });
   end();
   begin("symwalk_kernel");
-  symwalk_kernel<false><<<mc, SW_THREADS, sizeof(SymWalkSmem), stream>>>(a.fp, table, d_idx, a.index_cap, a.dst_cap, d_syms, d_offs, d_cls, nullptr, 1);
+  symwalk_kernel<false><<<mc, SW_THREADS, sizeof(SymWalkSmem), stream>>>(a.fp, table, d_idx, a.index_cap, a.dst_cap, d_syms, d_offs, d_cls);
   end();
   begin("decode_kernel");
   dispatch_latent(plan->dtype, [&](auto tag) {
@@ -2758,22 +2641,11 @@ PcoB200Error pco_b200_build_index(const void* compressed, size_t compressed_len,
   if (PcoB200Error e = ensure_device(c)) return e;
   cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
   const bool src_dev = flags & PCO_B200_SRC_ON_DEVICE;
-  uint8_t head[32] = {0};
-  size_t avail = std::min<size_t>(compressed_len, sizeof(head));
-  if (avail) {
-    if (src_dev) { PCOB_CUDA_TRY(cudaMemcpyAsync(head, compressed, avail, cudaMemcpyDeviceToHost, stream)); PCOB_CUDA_TRY(cudaStreamSynchronize(stream)); }
-    else std::memcpy(head, compressed, avail);
-  }
   StandaloneHeader hdr;
-  if (PcoB200Error e = parse_standalone_header(head, avail, compressed_len, &hdr)) return e;
+  if (PcoB200Error e = read_heads(compressed, compressed_len, src_dev, nullptr, 0, false, nullptr, &hdr, stream)) return e;
   const uint8_t* d_src;
-  if (src_dev) d_src = static_cast<const uint8_t*>(compressed);
-  else {
-    PCOB_CUDA_TRY(c.src.reserve(compressed_len + 16));
-    PCOB_CUDA_TRY(copy_sliced(c.src.p, compressed, compressed_len, cudaMemcpyHostToDevice, stream));
-    d_src = c.src.as<uint8_t>();
-  }
-  FileParams fp{d_src, compressed_len, dtype, hdr.uniform_type, hdr.format_major};
+  if (PcoB200Error e = stage_in(c.src, compressed, compressed_len, src_dev, stream, &d_src)) return e;
+  const FileParams fp{d_src, compressed_len, dtype, hdr.uniform_type, hdr.format_major};
   if (index_cap < sizeof(IndexHeader) + sizeof(IndexChunk) + 64) return fail(PCO_B200_IO, "index buffer too small");
   // Split the caller's capacity: chunk records sized from a lower bound on chunk bytes, the rest for entries.
   uint64_t max_chunks = std::min<uint64_t>(uint64_t(compressed_len) / 5 + 2, (index_cap - sizeof(IndexHeader)) / (4 * sizeof(IndexChunk)));

@@ -1,4 +1,4 @@
-"""GPU parity tests aimed at decode_narrow_kernel (pcodec_b200/csrc/decode_narrow.cuh): the lean decode instantiation
+"""GPU parity tests aimed at the narrow class of fused_narrow_kernel (pcodec_b200/csrc/decode_fused.cuh): the lean decode
 for classic-mode chunks with consecutive delta order 0 / 1, bin lowers within 2^16 of the first bin and offsets of
 <= 15 bits.  Streams come from the oracle; the GPU decode must equal the original numbers and the oracle's decode
 bit for bit, and pco_b200_profile_chunk_classes must show that the narrow kernel (class 3 / 4) really served them -
