@@ -405,6 +405,59 @@ PcoB200Error pco_b200_decompress_async(const PcoB200AsyncPlan *plan, const void 
  * sets the last-error message ("chunk 17: ...") and, when the kind is OK, fills *progress (may be NULL). */
 PcoB200Error pco_b200_decompress_async_result(const PcoB200AsyncStatus *host_status, PcoB200Progress *progress);
 
+/* ---- asynchronous compress (no reference counterpart): the other half of pco_b200_decompress_async.  The call only enqueues kernels on
+ * the caller's stream and returns at once; it makes no synchronising, allocating or host-to-device copy call and refers to no memory of
+ * the library's per-thread scratch, so it can be queued behind other GPU work and captured in a CUDA graph, and a captured call may be
+ * replayed after pco_b200_thread_release or after any other call.  A plan, made once outside any capture, fixes n, the config and the
+ * header flavour; the numbers are read from `nums` when the call runs, so one plan (and one captured graph) compresses whatever numbers
+ * the buffer holds on each run.  Every decision compress_ex makes on the host from the numbers (one-pass or two-kernel front end, counting
+ * or sorting planner, 16-bit keys or 64-bit latents in the packer) is made on the device.  Device buffers only. */
+typedef struct PcoB200AsyncCompressPlan {  /* filled by pco_b200_compress_async_plan; treat as opaque */
+  uint32_t dtype, uniform_type_header, mode, order;
+  uint32_t n_vars, bins_log, mode_k, reserved;
+  uint64_t n, max_page_n, dst_cap, index_cap;
+  uint64_t mode_base, base_bits, inv_base_bits;
+  uint64_t index_bytes;                    /* exact byte size of the side index for n (the call writes it when index != NULL) */
+  uint64_t workspace_bytes;                /* device workspace one in-flight call needs */
+} PcoB200AsyncCompressPlan;
+
+typedef struct PcoB200AsyncCompressStatus {  /* written on the device by every call */
+  uint32_t kind;                             /* PcoB200Error: OK, or PCO_B200_IO when the file does not fit dst_cap */
+  uint32_t device_status;                    /* 0, or PCO_B200_ASYNC_DST_FULL */
+  uint64_t file_bytes;                       /* bytes the file needs, also when it does not fit */
+  uint64_t n_written;                        /* bytes written to dst (0 when the file does not fit) */
+  uint64_t index_bytes;                      /* bytes written to index (0 when the call had none) */
+} PcoB200AsyncCompressStatus;
+enum { PCO_B200_ASYNC_DST_FULL = 0x106 };    /* device_status: the file is larger than dst_cap (PCO_B200_IO) */
+
+/* Makes a plan for compressing n numbers of dtype with `config` (NULL = the default config, whose Auto specs are refused) into a
+ * standalone file of the flavour uniform_type_header selects (as pco_b200_compress_ex), dst_cap bytes of destination and, when index_cap
+ * is not 0, a side index of up to index_cap bytes.  Runs on the host, before and outside any capture.  Refuses what pco_b200_compress_ex
+ * refuses, with the same kinds, and with PCO_B200_UNSUPPORTED also: ModeSpec::Auto and DeltaSpec::Auto (their searches run on host
+ * threads), runs wider than 256 unoptimized bins (levels 9-12 on chunks large enough to use them), PagingSpec::Exact, and chunk sizes that
+ * imply different unoptimized_bins_log (compress_ex encodes those in several runs).  An index_cap other than 0 below the exact index size
+ * (plan->index_bytes) is PCO_B200_IO.  Then *plan is filled, workspace_bytes included, and the one-time device set-up runs on the current
+ * device, which the calls must use (kernel attributes, and every kernel the call launches loaded); without a device that is
+ * PCO_B200_CUDA.  workspace_bytes = 256 + per number of the chunks' rows (each chunk rounded up to 256 numbers): 3 * sizeof(number) + 5
+ * bytes for one latent var (Classic), 4 * sizeof(number) + 10 for two; per chunk about 25 KB (the two vars' plans, the planner's probes,
+ * the chunk records) plus 20 bytes per batch of 256 numbers of the largest chunk, each region rounded up to 256 bytes. */
+PcoB200Error pco_b200_compress_async_plan(size_t n, unsigned char dtype, const PcoB200ChunkConfig *config, int uniform_type_header,
+                                          size_t dst_cap, size_t index_cap, PcoB200AsyncCompressPlan *plan);
+/* Enqueues the compress of the plan's n numbers in `nums` into `dst` (and the side index into `index`, which may be NULL) on
+ * `cuda_stream`, and the outcome into *status; returns without waiting.  nums, dst, index (16-byte aligned), workspace
+ * (plan->workspace_bytes, 256-byte aligned) and status are device pointers; one workspace serves one call in flight, so calls on different
+ * streams need workspaces of their own.  For every plan it accepts, the file bytes and the index bytes equal what pco_b200_compress_ex
+ * writes for the same numbers and config with PCO_B200_SRC_ON_DEVICE | PCO_B200_DST_ON_DEVICE | PCO_B200_INDEX_ON_DEVICE.  Nothing is
+ * written outside dst_cap bytes of dst; a file that does not fit is PCO_B200_IO in the status, which still reports the bytes it needs.
+ * The return value covers the host side only: null pointers, misaligned buffers, an index with a plan made without one, or a plan that was
+ * not filled (PCO_B200_INVALID_ARGUMENT), a launch the runtime refuses (PCO_B200_CUDA).  With pco_b200_profile_enable(1), a call outside a
+ * stream capture records its kernel spans for pco_b200_profile_last; a call inside a capture records none. */
+PcoB200Error pco_b200_compress_async(const PcoB200AsyncCompressPlan *plan, const void *nums, void *dst, void *index, void *workspace,
+                                     PcoB200AsyncCompressStatus *status, void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory at a point of the caller's choosing.  Returns the kind and
+ * sets the last-error message; when the kind is OK, fills *n_written and *index_len (either may be NULL). */
+PcoB200Error pco_b200_compress_async_result(const PcoB200AsyncCompressStatus *host_status, size_t *n_written, size_t *index_len);
+
 #if defined(__cplusplus)
 }
 #endif

@@ -1,0 +1,390 @@
+// Kernels and host steps of pco_b200_compress_async: an explicit-config compress with no host decision between launches, so the call can
+// be queued behind other work or captured in a CUDA graph.  The plan fixes n, the chunk layout (EqualPagesUpTo: the first `rem` chunks
+// hold low + 1 numbers, the others low), the mode, the delta order and one unoptimized_bins_log; everything that depends on the numbers
+// is decided on the device.  The ordinary encode kernels run unchanged.  Each choice compress_typed makes on the host from a readback
+// becomes a gate kernel that writes, per choice, a copy of the chunk starts that is either the real one or all zeros: a kernel launched
+// with the zero copy sees chunks of 0 numbers and leaves at its first lines.  Choices and their gates:
+//   one-pass or two-kernel front end (split_count_kernel's flag)  acomp_two_gate_kernel: split_delta_kernel's starts, ChunkEnc reset
+//   counting or sorting planner, per var (the range bits)           acomp_var_gate_kernel: the counting probe, the sort path, bin_lut_kernel,
+//                                                                   bin_kernel
+//   16-bit keys or 64-bit latents in pack_kernel, per var           acomp_pack_gate_kernel: one copy of the ChunkEnc table per choice, whose
+//                                                                   chunks the launches of the other choices find out of dst_cap
+// acomp_init_kernel lays out the chunks, the header and the index header; acomp_finish_kernel writes the PcoB200AsyncCompressStatus.
+#pragma once
+#include "../../include/pco_b200.h"
+#include "compress_host.cuh"
+
+namespace pcob200 {
+
+constexpr int ACOMP_THREADS = 256;
+constexpr uint32_t ACOMP_GATES_PER_VAR = 4;  // counting probe, sort path, bin_lut_kernel, bin_kernel
+
+// Chunk geometry of a plan (n_per_page's EqualPagesUpTo in closed form)
+struct AcompGeom {
+  uint64_t n, n_chunks, low, rem, max_n, slots;
+  uint32_t bpc, tiles;
+};
+__host__ __device__ inline uint64_t acomp_rows_of(uint64_t size) { return (size + BATCH_N - 1) / BATCH_N * BATCH_N; }
+inline AcompGeom acomp_geom(uint64_t n, uint64_t max_page_n) {
+  AcompGeom g = {};
+  g.n = n;
+  if (n == 0) return g;
+  const uint64_t mp = max_page_n == 0 ? (uint64_t(1) << 18) : max_page_n;
+  g.n_chunks = (n + mp - 1) / mp;
+  g.low = n / g.n_chunks;
+  g.rem = n % g.n_chunks;
+  g.max_n = g.low + (g.rem ? 1 : 0);
+  g.slots = g.rem * acomp_rows_of(g.low + 1) + (g.n_chunks - g.rem) * acomp_rows_of(g.low);
+  g.bpc = n_batches_of(uint32_t(g.max_n));
+  g.tiles = uint32_t((g.max_n + SPLIT_TILE - 1) / SPLIT_TILE);
+  return g;
+}
+__host__ __device__ inline uint64_t acomp_entries_bytes(uint32_t n_vars, uint64_t size) {
+  return (uint64_t(n_vars) * n_batches_of(uint32_t(size)) * sizeof(BatchEntry) + 15) & ~uint64_t(15);
+}
+// byte size of the side index compress_typed writes for this layout
+inline uint64_t acomp_index_bytes(const AcompGeom& g, uint32_t n_vars) {
+  if (g.n == 0) return sizeof(IndexHeader);
+  return ((sizeof(IndexHeader) + g.n_chunks * sizeof(IndexChunk) + 15) & ~uint64_t(15)) + g.rem * acomp_entries_bytes(n_vars, g.low + 1) +
+         (g.n_chunks - g.rem) * acomp_entries_bytes(n_vars, g.low);
+}
+
+// Workspace of one in-flight call, byte offsets of 256-byte aligned regions.  head: split_count_kernel's flags (2 words), the range bits
+// per var (2 words), the file size (u64 at byte 16), the standalone header (byte 64).
+struct AcompLayout {
+  uint64_t chunks, copies, starts, rows, gates, eoff, seg, plans, probes, ob_sum, ans_sum, entries;
+  uint64_t lat[MAX_VARS], keys_a, keys_b, key16[MAX_VARS], sym[MAX_VARS], ans[MAX_VARS];
+  uint64_t total;
+};
+inline uint64_t acomp_align(uint64_t x) { return (x + 255) & ~uint64_t(255); }
+inline AcompLayout acomp_layout(const AcompGeom& g, uint32_t lbytes, uint32_t n_vars) {
+  AcompLayout l = {};
+  uint64_t at = 256;
+  auto take = [&](uint64_t bytes) { const uint64_t o = at; at += acomp_align(bytes); return o; };
+  const uint64_t nc = g.n_chunks, cvb = nc * MAX_VARS * g.bpc;
+  l.chunks = take(nc * sizeof(ChunkEnc));
+  l.copies = take((uint64_t(1) << n_vars) * nc * sizeof(ChunkEnc));
+  l.starts = take((nc + 1) * 8);
+  l.rows = take((nc + 1) * 8);
+  l.gates = take((1 + ACOMP_GATES_PER_VAR * n_vars) * (nc + 1) * 8);
+  l.eoff = take(nc * 8);
+  l.seg = take(2 * nc * 8);
+  l.plans = take(nc * MAX_VARS * sizeof(VarPlan));
+  l.probes = take(nc * sizeof(PlanProbes));
+  l.ob_sum = take(cvb * 4);
+  l.ans_sum = take(cvb * 4);
+  l.entries = take(cvb * sizeof(BatchEntry));
+  // per number: the 64-bit path's latents and sort keys, the counting path's 16-bit keys, symbols and tANS fields (each + 64 bytes of
+  // slack, as compress_typed reserves them)
+  for (uint32_t v = 0; v < n_vars; v++) l.lat[v] = take(g.slots * lbytes + 64);
+  l.keys_a = take(g.slots * lbytes + 64);
+  l.keys_b = take(g.slots * lbytes + 64);
+  for (uint32_t v = 0; v < n_vars; v++) {
+    l.key16[v] = take(g.slots * 2 + 64);
+    l.sym[v] = take(g.slots + 64);
+    l.ans[v] = take(g.slots * 2 + 64);
+  }
+  l.total = at;
+  return l;
+}
+
+// What the launches take by value
+struct AcompArgs {
+  uint64_t n, n_chunks, low, rem;
+  uint64_t dst_cap, index_bytes;   // index_bytes: 0 = no index this call
+  uint32_t header_bytes, n_vars;
+  uint8_t* ws;
+  uint8_t* dst;
+  uint8_t* index;
+  AcompLayout lay;
+  uint8_t header[STANDALONE_HEADER_MAX];
+};
+struct AcompHead {
+  uint32_t flags[2];      // split_count_kernel: [0] range bits, [1] some chunk spans 2^15 or more
+  uint32_t range_bits[MAX_VARS];
+  uint64_t total;         // file bytes (chunk_offsets_kernel)
+};
+__device__ inline uint64_t* acomp_gate(const AcompArgs& a, uint32_t g) { return reinterpret_cast<uint64_t*>(a.ws + a.lay.gates) + uint64_t(g) * (a.n_chunks + 1); }
+__device__ inline uint64_t acomp_start(const AcompArgs& a, uint64_t c) { return c * a.low + (c < a.rem ? c : a.rem); }
+__device__ inline void acomp_reset_chunk(ChunkEnc* ch) {  // init_chunks_kernel's record
+  ChunkEnc z;
+  memset(&z, 0, sizeof(z));
+  z.vmin[0] = z.vmin[1] = ~uint64_t(0);
+  *ch = z;
+}
+
+// Grid-stride over every per-chunk and per-word job: ChunkEnc records, chunk starts and row bases, index entry offsets, the zeroed
+// offset-bit sums (fallback chunks leave their secondary var's untouched) and the zeroed index body; thread 0 writes the head, the
+// standalone header, the index header and, when n == 0, the whole file (header and terminator).
+__global__ void __launch_bounds__(ACOMP_THREADS) acomp_init_kernel(AcompArgs a, uint32_t bpc) {
+  const uint64_t nc = a.n_chunks;
+  ChunkEnc* chunks = reinterpret_cast<ChunkEnc*>(a.ws + a.lay.chunks);
+  uint64_t* starts = reinterpret_cast<uint64_t*>(a.ws + a.lay.starts);
+  uint64_t* rows = reinterpret_cast<uint64_t*>(a.ws + a.lay.rows);
+  uint64_t* eoff = reinterpret_cast<uint64_t*>(a.ws + a.lay.eoff);
+  uint32_t* ob_sum = reinterpret_cast<uint32_t*>(a.ws + a.lay.ob_sum);
+  const uint64_t r1 = acomp_rows_of(a.low + 1), r0 = acomp_rows_of(a.low);
+  const uint64_t e1 = acomp_entries_bytes(a.n_vars, a.low + 1), e0 = acomp_entries_bytes(a.n_vars, a.low);
+  const uint64_t ebase = (sizeof(IndexHeader) + nc * sizeof(IndexChunk) + 15) & ~uint64_t(15);
+  const uint64_t n_sums = nc * MAX_VARS * bpc;
+  const uint64_t idx_vecs = a.index_bytes > sizeof(IndexHeader) ? (a.index_bytes - sizeof(IndexHeader)) / 16 : 0;
+  const uint64_t jobs = max(max(nc + 1, n_sums), idx_vecs);
+  for (uint64_t t = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; t < jobs; t += uint64_t(gridDim.x) * blockDim.x) {
+    if (t <= nc) {
+      const uint64_t k = t < a.rem ? t : a.rem;
+      starts[t] = acomp_start(a, t);
+      rows[t] = k * r1 + (t - k) * r0;
+      if (t < nc) {
+        acomp_reset_chunk(&chunks[t]);
+        eoff[t] = ebase + k * e1 + (t - k) * e0;
+      }
+    }
+    if (t < n_sums) ob_sum[t] = 0;
+    if (t < idx_vecs) reinterpret_cast<uint4*>(a.index + sizeof(IndexHeader))[t] = make_uint4(0, 0, 0, 0);
+  }
+  if (blockIdx.x != 0 || threadIdx.x != 0) return;
+  AcompHead* h = reinterpret_cast<AcompHead*>(a.ws);
+  h->flags[0] = h->flags[1] = 0;
+  h->range_bits[0] = h->range_bits[1] = 0;
+  h->total = a.n == 0 ? a.header_bytes + 1 : 0;  // n == 0: header and terminator only (standalone/simple.rs:62-91)
+  for (uint32_t i = 0; i < a.header_bytes; i++) (a.ws + 64)[i] = a.header[i];
+  if (a.n == 0 && a.header_bytes + 1 <= a.dst_cap) {
+    for (uint32_t i = 0; i < a.header_bytes; i++) a.dst[i] = a.header[i];
+    a.dst[a.header_bytes] = 0;
+  }
+  if (a.index_bytes) {
+    IndexHeader ih;
+    memset(&ih, 0, sizeof(ih));
+    ih.magic = INDEX_MAGIC;
+    ih.version = 1;
+    ih.n_chunks = nc;
+    ih.n_total = a.n;
+    ih.chunks_offset = sizeof(IndexHeader);
+    if (a.n == 0) ih.file_len = ih.end_byte = a.header_bytes + 1;  // with chunks, emit_index_kernel writes both
+    *reinterpret_cast<IndexHeader*>(a.index) = ih;
+  }
+}
+
+// Behind split_count_kernel (or first, for the two-var modes: always_two): the two-kernel front end runs when some chunk's latents span
+// 2^15 or more.  Then the ChunkEnc records start over (init_chunks_kernel in plan_front) and split_delta_kernel sees the real starts.
+__global__ void __launch_bounds__(ACOMP_THREADS) acomp_two_gate_kernel(AcompArgs a, uint32_t always_two) {
+  const AcompHead* h = reinterpret_cast<const AcompHead*>(a.ws);
+  const bool two = always_two || h->flags[1] != 0;
+  ChunkEnc* chunks = reinterpret_cast<ChunkEnc*>(a.ws + a.lay.chunks);
+  uint64_t* g = acomp_gate(a, 0);
+  for (uint64_t c = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; c <= a.n_chunks; c += uint64_t(gridDim.x) * blockDim.x) {
+    g[c] = two ? acomp_start(a, c) : 0;
+    if (two && c < a.n_chunks) acomp_reset_chunk(&chunks[c]);
+  }
+}
+
+// One CTA, behind split_delta_kernel.  Per var: the range bits of the call (range_bits_kernel's maximum over the chunks, which also sets
+// key_base = vmin, on the two-kernel path; split_count_kernel's flags[0] on the one-pass path), then the starts of the four gated
+// launches: the counting probe (two-kernel path, range <= PLAN_MAX_COUNT_BITS), the sort path (range above), bin_lut_kernel (range <=)
+// and bin_kernel (above).
+__global__ void __launch_bounds__(1024) acomp_var_gate_kernel(AcompArgs a, uint32_t always_two) {
+  __shared__ uint32_t s_bits;
+  AcompHead* h = reinterpret_cast<AcompHead*>(a.ws);
+  ChunkEnc* chunks = reinterpret_cast<ChunkEnc*>(a.ws + a.lay.chunks);
+  const bool two = always_two || h->flags[1] != 0;
+  for (uint32_t v = 0; v < a.n_vars; v++) {
+    if (threadIdx.x == 0) s_bits = two ? 0u : h->flags[0];
+    __syncthreads();
+    if (two)
+      for (uint64_t c = threadIdx.x; c < a.n_chunks; c += blockDim.x) {
+        const uint64_t lo = chunks[c].vmin[v], hi = chunks[c].vmax[v];
+        atomicMax(&s_bits, hi > lo ? 64 - __clzll((long long)(hi - lo)) : 0u);
+        chunks[c].key_base[v] = lo;  // plan_probe_kernel's keys are latent - vmin
+      }
+    __syncthreads();
+    const uint32_t bits = s_bits;
+    if (threadIdx.x == 0) h->range_bits[v] = bits;
+    const bool narrow = bits <= PLAN_MAX_COUNT_BITS;
+    const bool on[ACOMP_GATES_PER_VAR] = {two && narrow, two && !narrow, narrow, !narrow};
+    for (uint64_t c = threadIdx.x; c <= a.n_chunks; c += blockDim.x) {
+      const uint64_t s = acomp_start(a, c);
+      for (uint32_t k = 0; k < ACOMP_GATES_PER_VAR; k++) acomp_gate(a, 1 + ACOMP_GATES_PER_VAR * v + k)[c] = on[k] ? s : 0;
+    }
+    __syncthreads();
+  }
+}
+
+// Behind chunk_offsets_kernel: copy k of the ChunkEnc table serves the pack_kernel launch whose var v reads 64-bit latents when bit v of k
+// is set and 16-bit keys otherwise.  In the copies of the choices the range bits did not make, every chunk lies past dst_cap.
+__global__ void __launch_bounds__(ACOMP_THREADS) acomp_pack_gate_kernel(AcompArgs a) {
+  const AcompHead* h = reinterpret_cast<const AcompHead*>(a.ws);
+  const ChunkEnc* chunks = reinterpret_cast<const ChunkEnc*>(a.ws + a.lay.chunks);
+  ChunkEnc* copies = reinterpret_cast<ChunkEnc*>(a.ws + a.lay.copies);
+  uint32_t live = 0;
+  for (uint32_t v = 0; v < a.n_vars; v++) live |= (h->range_bits[v] > PLAN_MAX_COUNT_BITS ? 1u : 0u) << v;
+  const uint64_t n_copies = uint64_t(1) << a.n_vars;
+  for (uint64_t t = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; t < n_copies * a.n_chunks; t += uint64_t(gridDim.x) * blockDim.x) {
+    const uint64_t k = t / a.n_chunks, c = t % a.n_chunks;
+    ChunkEnc ch = chunks[c];
+    if (k != live) ch.out_offset = ~uint64_t(0) - ch.chunk_bytes;  // out_offset + chunk_bytes exceeds any out_cap below 2^64 - 1
+    copies[t] = ch;
+  }
+}
+
+// One thread: the outcome.
+__global__ void acomp_finish_kernel(AcompArgs a, PcoB200AsyncCompressStatus* __restrict__ out) {
+  if (blockIdx.x != 0 || threadIdx.x != 0) return;
+  const uint64_t total = reinterpret_cast<const AcompHead*>(a.ws)->total;
+  PcoB200AsyncCompressStatus s;
+  const bool fits = total <= a.dst_cap;
+  s.kind = fits ? PCO_B200_OK : PCO_B200_IO;
+  s.device_status = fits ? 0u : uint32_t(PCO_B200_ASYNC_DST_FULL);
+  s.file_bytes = total;
+  s.n_written = fits ? total : 0;
+  s.index_bytes = a.index_bytes;
+  *out = s;
+}
+
+// ---- host steps
+
+inline PcoB200Error acomp_check_plan(const PcoB200AsyncCompressPlan* p, AcompGeom* g, AcompLayout* lay) {
+  if (!p || !nt_valid(p->dtype) || p->mode > MODE_FLOAT_QUANT || p->n_vars != (p->mode == MODE_CLASSIC ? 1u : 2u) || p->order > MAX_ORDER ||
+      p->bins_log > ENC_NARROW_BINS_LOG || (p->index_cap != 0 && p->index_bytes > p->index_cap))
+    return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_compress_async_plan");
+  *g = acomp_geom(p->n, p->max_page_n);
+  *lay = acomp_layout(*g, nt_bits(p->dtype) / 8, p->n_vars);
+  if (p->workspace_bytes != lay->total || p->index_bytes != acomp_index_bytes(*g, p->n_vars))
+    return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_compress_async_plan");
+  return PCO_B200_OK;
+}
+
+template <typename L>
+void acomp_launch(const PcoB200AsyncCompressPlan& p, const AcompGeom& g, const AcompArgs& a, const void* nums, PcoB200AsyncCompressStatus* status,
+                         cudaStream_t stream, bool prof) {
+  auto begin = [&](const char* name) { if (prof) profiler().begin(name, stream); };
+  auto end = [&]() { if (prof) profiler().end(stream); };
+  const uint32_t nc = uint32_t(g.n_chunks), bpc = g.bpc, tiles = g.tiles;
+  constexpr uint32_t LBITS = sizeof(L) * 8;
+  constexpr size_t RS_SMEM = size_t(RS_WARPS) * RS_BINS * sizeof(uint32_t);
+  uint8_t* ws = a.ws;
+  const AcompLayout& l = a.lay;
+  const uint32_t init_ctas = uint32_t(std::min<uint64_t>(1024, std::max<uint64_t>({g.n_chunks + 1, g.n_chunks * MAX_VARS * bpc, a.index_bytes / 16}) / ACOMP_THREADS + 1));
+  begin("acomp_init_kernel");
+  acomp_init_kernel<<<init_ctas, ACOMP_THREADS, 0, stream>>>(a, bpc);
+  end();
+  if (p.n > 0) {
+    ChunkEnc* chunks = reinterpret_cast<ChunkEnc*>(ws + l.chunks);
+    VarPlan* plans = reinterpret_cast<VarPlan*>(ws + l.plans);
+    PlanProbes* probes = reinterpret_cast<PlanProbes*>(ws + l.probes);
+    AcompHead* head = reinterpret_cast<AcompHead*>(ws);
+    uint64_t* gates = reinterpret_cast<uint64_t*>(ws + l.gates);
+    L* lat[MAX_VARS] = {reinterpret_cast<L*>(ws + l.lat[0]), p.n_vars > 1 ? reinterpret_cast<L*>(ws + l.lat[1]) : nullptr};
+    uint16_t* key16[MAX_VARS] = {reinterpret_cast<uint16_t*>(ws + l.key16[0]), p.n_vars > 1 ? reinterpret_cast<uint16_t*>(ws + l.key16[1]) : nullptr};
+    uint8_t* sym[MAX_VARS] = {ws + l.sym[0], p.n_vars > 1 ? ws + l.sym[1] : nullptr};
+    uint16_t* ans[MAX_VARS] = {reinterpret_cast<uint16_t*>(ws + l.ans[0]), p.n_vars > 1 ? reinterpret_cast<uint16_t*>(ws + l.ans[1]) : nullptr};
+    L* keys_a = reinterpret_cast<L*>(ws + l.keys_a);
+    L* keys_b = reinterpret_cast<L*>(ws + l.keys_b);
+    uint64_t* seg_begin = reinterpret_cast<uint64_t*>(ws + l.seg);
+    uint64_t* seg_end = seg_begin + nc;
+    uint32_t* ob_sum = reinterpret_cast<uint32_t*>(ws + l.ob_sum);
+    uint32_t* ans_sum = reinterpret_cast<uint32_t*>(ws + l.ans_sum);
+    BatchEntry* entries = reinterpret_cast<BatchEntry*>(ws + l.entries);
+    EncParams ep;
+    std::memset(&ep, 0, sizeof(ep));
+    ep.dtype = p.dtype;
+    ep.uniform_type = p.uniform_type_header ? p.dtype : 0;
+    ep.mode = p.mode;
+    ep.mode_base = p.mode_base;
+    ep.base_bits = p.base_bits;
+    ep.inv_base_bits = p.inv_base_bits;
+    ep.mode_k = p.mode_k;
+    ep.order = p.order;
+    ep.n_vars = p.n_vars;
+    ep.n_total = p.n;
+    ep.n_chunks = nc;
+    ep.max_chunk_n = uint32_t(g.max_n);
+    ep.bins_log[0] = p.bins_log;
+    ep.bins_log[1] = std::min<uint32_t>(p.bins_log, 6);  // LIMITED_UNOPTIMIZED_BINS_LOG (chunk_compressor.rs:238-248)
+    ep.nums = nums;
+    ep.chunk_starts = reinterpret_cast<const uint64_t*>(ws + l.starts);
+    ep.row_base = reinterpret_cast<const uint64_t*>(ws + l.rows);
+    auto gated = [&](uint32_t gate) { EncParams e = ep; e.chunk_starts = gates + uint64_t(gate) * (g.n_chunks + 1); return e; };
+    const uint32_t always_two = p.n_vars > 1 ? 1u : 0u;
+    // ---- front end: the one-pass kernel for Classic, then the two-kernel path behind its flag (always, for the two-var modes)
+    if (!always_two) {
+      begin("split_count_kernel");
+      split_count_kernel<L><<<nc, SC_THREADS, size_t(SC_N) * 4, stream>>>(ep, chunks, probes, key16[0], head->flags);
+      end();
+    }
+    acomp_two_gate_kernel<<<(nc + ACOMP_THREADS) / ACOMP_THREADS, ACOMP_THREADS, 0, stream>>>(a, always_two);
+    const EncParams e_two = gated(0);
+    begin("split_delta_kernel");
+    switch (p.mode) {
+      case MODE_CLASSIC: split_delta_kernel<L, MODE_CLASSIC><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
+      case MODE_INT_MULT: split_delta_kernel<L, MODE_INT_MULT><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
+      case MODE_FLOAT_QUANT: split_delta_kernel<L, MODE_FLOAT_QUANT><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
+      default: split_delta_kernel<L, MODE_FLOAT_MULT><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
+    }
+    end();
+    acomp_var_gate_kernel<<<1, 1024, 0, stream>>>(a, always_two);
+    // ---- planner per var: counting probe or sort path (whichever the range bits gate on), then the solver on the probes either left
+    // (the one-pass kernel writes var 0's probes itself).  The counting probe takes the counters of PLAN_MAX_COUNT_BITS and the sort all
+    // bits of the number type: both give the probes of the narrower range, and the number of sort passes - so the buffer the sorted keys
+    // end in - is fixed.
+    const L* sorted = ((LBITS + RS_BITS - 1) / RS_BITS) & 1 ? keys_b : keys_a;
+    for (uint32_t v = 0; v < p.n_vars; v++) {
+      const EncParams e_count = gated(1 + ACOMP_GATES_PER_VAR * v), e_sort = gated(2 + ACOMP_GATES_PER_VAR * v);
+      begin("plan_probe_kernel_counting");
+      plan_probe_kernel<L, true><<<nc, PLAN_THREADS, ((size_t(1) << PLAN_MAX_COUNT_BITS) + 1) * 4 + 16, stream>>>(e_count, lat[v], chunks, probes, int(v),
+                                                                                                                    PLAN_MAX_COUNT_BITS, key16[v]);
+      end();
+      begin("sort_keys_kernel");
+      sort_keys_kernel<L><<<nc * tiles, 256, 0, stream>>>(e_sort, tiles, lat[v], keys_a, chunks, int(v));
+      end();
+      segment_offsets_kernel<<<(nc + 255) / 256, 256, 0, stream>>>(e_sort, v == 0 ? p.order : 0, seg_begin, seg_end);
+      begin("radix_sort_segments_kernel");
+      radix_sort_segments_kernel<L><<<nc, RS_THREADS, RS_SMEM, stream>>>(keys_a, keys_b, seg_begin, seg_end, LBITS);
+      end();
+      begin("plan_probe_kernel_sorted");
+      plan_probe_kernel<L, false><<<nc, PLAN_THREADS, 16, stream>>>(e_sort, sorted, chunks, probes, int(v), LBITS, nullptr);
+      end();
+      begin("plan_solve_kernel");
+      plan_solve_kernel<L><<<nc, SOLVE_THREADS, 0, stream>>>(ep, probes, chunks, plans, int(v));
+      end();
+    }
+    fallback_kernel<false><<<(nc + 255) / 256, 256, 0, stream>>>(ep, plans, chunks, 0u);
+    // ---- K3 per var: the lookup-table binning on the 16-bit keys, or the search over the 64-bit latents
+    const uint32_t parts = (bpc + BINL_BATCHES - 1) / BINL_BATCHES, groups = (bpc + 7) / 8;
+    for (uint32_t v = 0; v < p.n_vars; v++) {
+      begin("bin_lut_kernel");
+      bin_lut_kernel<L><<<nc * parts, BINL_THREADS, (size_t(1) << PLAN_MAX_COUNT_BITS) + 16, stream>>>(gated(3 + ACOMP_GATES_PER_VAR * v), bpc, parts, key16[v], plans,
+                                                                                                      chunks, sym[v], ob_sum, int(v), PLAN_MAX_COUNT_BITS);
+      end();
+      begin("bin_kernel");
+      bin_kernel<L, false><<<nc * groups, BIN_THREADS, 0, stream>>>(gated(4 + ACOMP_GATES_PER_VAR * v), bpc, lat[v], plans, chunks, sym[v], ob_sum, int(v));
+      end();
+    }
+    begin("ans_encode_kernel");
+    ans_encode_kernel<false><<<nc * MAX_VARS, ANS_THREADS, 0, stream>>>(ep, bpc, plans, chunks, sym[0], sym[1], ans[0], ans[1], ans_sum, entries, nullptr);
+    end();
+    begin("layout_kernel");
+    layout_kernel<false><<<nc, LAYOUT_THREADS, 0, stream>>>(ep, bpc, plans, chunks, ans_sum, ob_sum, entries);
+    end();
+    chunk_offsets_kernel<<<1, 1024, 0, stream>>>(chunks, nc, a.header_bytes, 1u, &head->total);
+    // ---- K5: one launch per choice of keys or latents; only the one the range bits made finds its chunks inside dst_cap
+    const uint64_t n_copies = uint64_t(1) << p.n_vars;
+    acomp_pack_gate_kernel<<<uint32_t(std::min<uint64_t>(1024, (n_copies * g.n_chunks + ACOMP_THREADS - 1) / ACOMP_THREADS)), ACOMP_THREADS, 0, stream>>>(a);
+    const uint64_t out_cap = std::min<uint64_t>(p.dst_cap, ~uint64_t(0) - 1);
+    begin("pack_kernel");
+    for (uint64_t k = 0; k < n_copies; k++) {
+      const ChunkEnc* copy = reinterpret_cast<const ChunkEnc*>(ws + l.copies) + k * g.n_chunks;
+      pack_kernel<L><<<nc, PACK_THREADS, sizeof(PackSmem), stream>>>(ep, bpc, lat[0], lat[1], plans, copy, sym[0], sym[1], ans[0], ans[1], entries, a.dst, out_cap,
+                                                                     (k & 1) ? nullptr : key16[0], (p.n_vars > 1 && !(k & 2)) ? key16[1] : nullptr);
+    }
+    end();
+    header_footer_kernel<<<1, 32, 0, stream>>>(a.dst, out_cap, ws + 64, a.header_bytes, &head->total);
+    if (a.index_bytes)
+      emit_index_kernel<<<nc, 256, 0, stream>>>(ep, bpc, chunks, entries, a.index, sizeof(IndexHeader), reinterpret_cast<const uint64_t*>(ws + l.eoff), &head->total,
+                                                1u, 0u, 0, 1u);
+  }
+  begin("acomp_finish_kernel");
+  acomp_finish_kernel<<<1, 32, 0, stream>>>(a, status);
+  end();
+}
+
+}  // namespace pcob200

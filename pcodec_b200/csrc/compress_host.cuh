@@ -71,16 +71,23 @@ inline PcoB200Error n_per_page(const PcoB200ChunkConfig& cfg, size_t n, std::vec
   return PCO_B200_OK;
 }
 
-// standalone header bytes (pco/src/standalone/compressor.rs:12-16,85-105)
+// standalone header bytes (pco/src/standalone/compressor.rs:12-16,85-105) into out[0 .. STANDALONE_HEADER_MAX); returns their count.
+// The size hint is a varint: 6 bits (power - 1), then the `power` bits of n_hint.
+constexpr uint32_t STANDALONE_HEADER_MAX = 17;
+__host__ __device__ inline uint32_t standalone_header_into(uint64_t n_hint, uint8_t uniform_type, uint8_t* out) {
+  const uint8_t magic[6] = {112, 99, 111, 33, 3, uniform_type};
+  for (int i = 0; i < 6; i++) out[i] = magic[i];
+  uint32_t power = 1;
+  while (power < 64 && (n_hint >> power) != 0) power++;
+  const uint32_t nbytes = (6 + power + 7) / 8;
+  for (uint32_t i = 0; i < nbytes; i++) out[6 + i] = uint8_t(i == 0 ? ((power - 1) | (n_hint << 6)) : (n_hint >> (8 * i - 6)));
+  out[6 + nbytes] = 4;
+  out[7 + nbytes] = 1;
+  return 8 + nbytes;
+}
 inline std::vector<uint8_t> make_standalone_header(uint64_t n_hint, uint8_t uniform_type) {
-  std::vector<uint8_t> h = {112, 99, 111, 33, 3, uniform_type};
-  uint32_t power = n_hint == 0 ? 1 : 64 - uint32_t(__builtin_clzll(n_hint));
-  unsigned __int128 v = (unsigned __int128)(power - 1) | ((unsigned __int128)(power >= 64 ? n_hint : (n_hint & ((uint64_t(1) << power) - 1))) << 6);
-  uint32_t nbytes = (6 + power + 7) / 8;
-  for (uint32_t i = 0; i < nbytes; i++) h.push_back(uint8_t(v >> (8 * i)));
-  h.push_back(4);
-  h.push_back(1);
-  return h;
+  uint8_t h[STANDALONE_HEADER_MAX];
+  return std::vector<uint8_t>(h, h + standalone_header_into(n_hint, uniform_type, h));
 }
 
 __global__ void range_bits_kernel(ChunkEnc* chunks, uint32_t n_chunks, int v, uint32_t* out_bits) {

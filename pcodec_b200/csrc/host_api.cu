@@ -3,6 +3,7 @@
 // compute entry point fails with PCO_B200_CUDA.
 #include <algorithm>
 
+#include "async_compress.cuh"
 #include "async_kernels.cuh"
 #include "compress_host.cuh"
 #include "decode_kernels.cuh"
@@ -2632,6 +2633,133 @@ PcoB200Error pco_b200_decompress_async_result(const PcoB200AsyncStatus* s, PcoB2
       status_to_error(s->device_status, "this chunk");
       return fail(kind, "chunk " + std::to_string(s->chunk) + ": " + last_error_ref());
   }
+}
+
+// ---- asynchronous compress (pco_b200_compress_async; gate kernels in async_compress.cuh).  The plan fixes the layout and the config;
+// the call is a fixed sequence of launches: init, [split_count, two-kernel gate], split_delta, range gate, per var (counting probe, sort
+// keys, segment offsets, radix sort, sorted probe, solve), fallback, per var (bin_lut, bin), ans, layout, chunk offsets, pack gate, one
+// pack per choice of keys, header, [index], finish.  n == 0 is init and finish only.
+
+PcoB200Error pco_b200_compress_async_plan(size_t n, unsigned char dtype, const PcoB200ChunkConfig* config, int uniform_type_header, size_t dst_cap,
+                                          size_t index_cap, PcoB200AsyncCompressPlan* plan) {
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (!plan) return fail(PCO_B200_INVALID_ARGUMENT, "null plan");
+  PcoB200ChunkConfig cfg;
+  if (config) cfg = *config;
+  else {
+    std::memset(&cfg, 0, sizeof(cfg));  // pco::ChunkConfig::default(): level 8, Auto, Auto, EqualPagesUpTo(2^18)
+    cfg.compression_level = 8;
+  }
+  ConfigCheck ck;
+  if (PcoB200Error e = check_config(cfg, dtype, n, &ck)) return e;
+  if (ck.auto_mode || ck.auto_delta)
+    return fail(PCO_B200_UNSUPPORTED, "ModeSpec::Auto and DeltaSpec::Auto search on host threads: the asynchronous compress takes explicit specs only");
+  if (cfg.paging_spec == PCO_B200_PAGING_EXACT) return fail(PCO_B200_UNSUPPORTED, "PagingSpec::Exact: the asynchronous compress takes EqualPagesUpTo only");
+  const AcompGeom g = acomp_geom(n, cfg.max_page_n);
+  uint32_t bins_log = 0;
+  if (n > 0) {
+    bins_log = choose_unoptimized_bins_log(cfg.compression_level, size_t(g.max_n));
+    if (bins_log > ENC_NARROW_BINS_LOG)
+      return fail(PCO_B200_UNSUPPORTED, "more than 256 unoptimized bins (levels 9-12): the asynchronous compress runs the narrow kernels only");
+    if (g.rem != 0 && g.low > 0 && choose_unoptimized_bins_log(cfg.compression_level, size_t(g.low)) != bins_log)
+      return fail(PCO_B200_UNSUPPORTED, "the chunk sizes imply different unoptimized_bins_log (compress_ex encodes them in several runs)");
+  }
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->uniform_type_header = uniform_type_header ? 1 : 0;
+  plan->mode = ck.explicit_mode.mode;
+  plan->order = ck.explicit_order;
+  plan->n_vars = ck.explicit_mode.mode == MODE_CLASSIC ? 1 : 2;
+  plan->bins_log = bins_log;
+  plan->mode_k = ck.explicit_mode.mode_k;
+  plan->n = n;
+  plan->max_page_n = cfg.max_page_n;
+  plan->dst_cap = dst_cap;
+  plan->index_cap = index_cap;
+  plan->mode_base = ck.explicit_mode.mode_base;
+  plan->base_bits = ck.explicit_mode.base_bits;
+  plan->inv_base_bits = ck.explicit_mode.inv_base_bits;
+  plan->index_bytes = acomp_index_bytes(g, plan->n_vars);
+  plan->workspace_bytes = acomp_layout(g, nt_bits(dtype) / 8, plan->n_vars).total;
+  if (index_cap != 0 && index_cap < plan->index_bytes)
+    return fail(PCO_B200_IO, "index buffer too small (need " + std::to_string(plan->index_bytes) + " bytes)");
+  // the one-time device set-up, here and not in a call (which may be inside a capture): the attributes compress_typed sets on first
+  // use, and every kernel the call launches loaded now (with lazy module loading a kernel is otherwise loaded at its first launch)
+  Context& c = ctx();
+  if (PcoB200Error e = ensure_device(c)) return e;
+  cudaFuncAttributes fa;
+  for (const void* k : {(const void*)acomp_init_kernel, (const void*)acomp_two_gate_kernel, (const void*)acomp_var_gate_kernel,
+                        (const void*)acomp_pack_gate_kernel, (const void*)acomp_finish_kernel, (const void*)init_chunks_kernel,
+                        (const void*)segment_offsets_kernel, (const void*)fallback_kernel<false>, (const void*)ans_encode_kernel<false>,
+                        (const void*)layout_kernel<false>, (const void*)chunk_offsets_kernel, (const void*)header_footer_kernel,
+                        (const void*)emit_index_kernel})
+    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, k));
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
+    using L = decltype(tag);
+    constexpr size_t RS_SMEM = size_t(RS_WARPS) * RS_BINS * sizeof(uint32_t);
+    const int count_smem = int(((size_t(1) << PLAN_MAX_COUNT_BITS) + 1) * 4 + 16);
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, count_smem));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(split_count_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(size_t(SC_N) * 4)));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PackSmem)));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(radix_sort_segments_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RS_SMEM));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(bin_lut_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    for (const void* k : {(const void*)split_count_kernel<L>, (const void*)split_delta_kernel<L, MODE_CLASSIC>, (const void*)split_delta_kernel<L, MODE_INT_MULT>,
+                          (const void*)split_delta_kernel<L, MODE_FLOAT_QUANT>, (const void*)split_delta_kernel<L, MODE_FLOAT_MULT>,
+                          (const void*)plan_probe_kernel<L, false>, (const void*)sort_keys_kernel<L>, (const void*)plan_solve_kernel<L>,
+                          (const void*)bin_kernel<L, false>})
+      PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, k));
+    return PCO_B200_OK;
+  });
+}
+
+PcoB200Error pco_b200_compress_async(const PcoB200AsyncCompressPlan* plan, const void* nums, void* dst, void* index, void* workspace,
+                                     PcoB200AsyncCompressStatus* status, void* cuda_stream) {
+  if (!plan || !workspace || !status || (!nums && plan->n) || (!dst && plan->dst_cap)) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  AcompGeom g;
+  AcompArgs a;
+  std::memset(&a, 0, sizeof(a));
+  if (PcoB200Error e = acomp_check_plan(plan, &g, &a.lay)) return e;
+  if (index && plan->index_cap == 0) return fail(PCO_B200_INVALID_ARGUMENT, "an index with a plan made without one (index_cap 0)");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  if (reinterpret_cast<uintptr_t>(index) & 15) return fail(PCO_B200_INVALID_ARGUMENT, "the index is not 16-byte aligned");
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  PCOB_CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
+  // kernel spans only outside a capture (an event record would become part of the graph); those of an earlier call that nobody read go
+  const bool prof = cap == cudaStreamCaptureStatusNone && profiler_enabled().load(std::memory_order_relaxed);
+  if (prof) profiler().discard();
+  a.n = plan->n;
+  a.n_chunks = g.n_chunks;
+  a.low = g.low;
+  a.rem = g.rem;
+  a.dst_cap = plan->dst_cap;
+  a.index_bytes = index ? plan->index_bytes : 0;
+  a.n_vars = plan->n_vars;
+  a.ws = static_cast<uint8_t*>(workspace);
+  a.dst = static_cast<uint8_t*>(dst);
+  a.index = static_cast<uint8_t*>(index);
+  a.header_bytes = standalone_header_into(plan->n, uint8_t(plan->uniform_type_header ? plan->dtype : 0), a.header);
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    acomp_launch<decltype(tag)>(*plan, g, a, nums, status, stream, prof);
+    return 0;
+  });
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
+}
+
+PcoB200Error pco_b200_compress_async_result(const PcoB200AsyncCompressStatus* s, size_t* n_written, size_t* index_len) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200Error kind = s->kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(s->kind) : PCO_B200_CORRUPTION;
+  if (kind == PCO_B200_OK) {
+    if (n_written) *n_written = size_t(s->n_written);
+    if (index_len) *index_len = size_t(s->index_bytes);
+    return PCO_B200_OK;
+  }
+  if (s->device_status == PCO_B200_ASYNC_DST_FULL)
+    return fail(kind, "failed to write whole buffer (need " + std::to_string(s->file_bytes) + " bytes)");
+  return fail(kind, "asynchronous compress failed (device status " + std::to_string(s->device_status) + ")");
 }
 
 PcoB200Error pco_b200_build_index(const void* compressed, size_t compressed_len, unsigned char dtype, void* index, size_t index_cap,

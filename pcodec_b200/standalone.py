@@ -470,6 +470,109 @@ class AsyncDecompressor:
         return Progress(prog.n_processed, bool(prog.finished))
 
 
+class _CAsyncCompressPlan(C.Structure):  # PcoB200AsyncCompressPlan (include/pco_b200.h)
+    _fields_ = [("dtype", C.c_uint32), ("uniform_type_header", C.c_uint32), ("mode", C.c_uint32), ("order", C.c_uint32),
+                ("n_vars", C.c_uint32), ("bins_log", C.c_uint32), ("mode_k", C.c_uint32), ("reserved", C.c_uint32),
+                ("n", C.c_uint64), ("max_page_n", C.c_uint64), ("dst_cap", C.c_uint64), ("index_cap", C.c_uint64),
+                ("mode_base", C.c_uint64), ("base_bits", C.c_uint64), ("inv_base_bits", C.c_uint64),
+                ("index_bytes", C.c_uint64), ("workspace_bytes", C.c_uint64)]
+
+
+class _CAsyncCompressStatus(C.Structure):  # PcoB200AsyncCompressStatus (include/pco_b200.h)
+    _fields_ = [("kind", C.c_uint32), ("device_status", C.c_uint32), ("file_bytes", C.c_uint64), ("n_written", C.c_uint64),
+                ("index_bytes", C.c_uint64)]
+
+
+def _lib_async_compress():
+    L = _lib.lib()
+    if not getattr(L, "_async_compress_ready", False):
+        L.pco_b200_compress_async_plan.argtypes = [C.c_size_t, C.c_ubyte, C.c_void_p, C.c_int, C.c_size_t, C.c_size_t, C.c_void_p]
+        L.pco_b200_compress_async.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.pco_b200_compress_async_result.argtypes = [C.c_void_p, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
+        L._async_compress_ready = True
+    return L
+
+
+class AsyncCompressor:
+    """Compresses n numbers on the current CUDA stream without waiting for the device (pco_b200_compress_async): a call only enqueues
+    kernels, so it can run behind other GPU work while the host moves on, and it can be captured in a torch.cuda.CUDAGraph.
+
+    The plan fixes n, the number type `dtype`, the config (explicit mode and delta specs, levels up to 8, EqualPagesUpTo paging), the
+    header flavour (uniform_type_header: as simple_compress_into) and the capacities: dst_cap bytes of file (default: the size guarantee
+    pco_standalone_guarantee_file_size) and, with index=True, the exact size of the side index.  The numbers are read when the call runs,
+    so a captured call compresses whatever its input tensor holds on each replay.  The bytes equal what compress_ex writes for the same
+    numbers and config.  The compressor owns a device workspace and a status word; it serves one call in flight at a time (calls on one
+    stream queue up)."""
+
+    def __init__(self, n, dtype, config=None, dst_cap=None, index=True, uniform_type_header=False, device=None):
+        import torch
+
+        self.dtype = np.dtype(dtype)
+        self.n = int(n)
+        dtb = _lib.dtype_byte(self.dtype)
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        L = _lib_async_compress()
+        if dst_cap is None:
+            dst_cap = L.pco_standalone_guarantee_file_size(self.n, dtb)
+        cfg = (config or ChunkConfig())._to_c()
+        self._plan = _CAsyncCompressPlan()
+        with torch.cuda.device(self.device):
+            if index:  # the exact index size is known once the plan exists: a first plan without an index reports it
+                rc = L.pco_b200_compress_async_plan(C.c_size_t(self.n), C.c_ubyte(dtb), C.byref(cfg), C.c_int(1 if uniform_type_header else 0),
+                                                    C.c_size_t(dst_cap), C.c_size_t(0), C.byref(self._plan))
+                _lib.check(rc)
+            rc = L.pco_b200_compress_async_plan(C.c_size_t(self.n), C.c_ubyte(dtb), C.byref(cfg), C.c_int(1 if uniform_type_header else 0),
+                                                C.c_size_t(dst_cap), C.c_size_t(self._plan.index_bytes if index else 0), C.byref(self._plan))
+        _lib.check(rc)
+        self.workspace = torch.empty(max(self._plan.workspace_bytes, 1), dtype=torch.uint8, device=self.device)
+        self.status = torch.zeros(C.sizeof(_CAsyncCompressStatus), dtype=torch.uint8, device=self.device)
+
+    @property
+    def dst_cap(self):
+        return int(self._plan.dst_cap)
+
+    @property
+    def index_bytes(self):
+        """Bytes of the side index each call writes (0 without one)."""
+        return int(self._plan.index_cap and self._plan.index_bytes)
+
+    @property
+    def workspace_bytes(self):
+        return int(self._plan.workspace_bytes)
+
+    def __call__(self, nums, dst, index=None):
+        """Enqueues the compress of `nums` (a CUDA tensor of the plan's dtype and n numbers) into `dst` (uint8 CUDA tensor of at least dst_cap
+        bytes) and, when given, the side index into `index` (uint8 CUDA tensor of at least index_bytes bytes) on torch.cuda.current_stream().
+        Returns nothing and does not wait; result() reports the outcome."""
+        import torch
+
+        from .wrapped import _torch_dtypes
+
+        p = self._plan
+        for name, t in (("nums", nums), ("dst", dst)) + ((("index", index),) if index is not None else ()):
+            if not _is_cuda(t) or t.device != self.device or not t.is_contiguous():
+                raise ValueError(f"{name} must be a contiguous CUDA tensor on {self.device}")
+        if nums.dtype != _torch_dtypes()[self.dtype] or nums.numel() != self.n:
+            raise ValueError(f"nums must hold n = {self.n} numbers of {self.dtype}")
+        if dst.numel() * dst.element_size() < p.dst_cap:
+            raise ValueError(f"dst holds fewer than dst_cap = {p.dst_cap} bytes")
+        if index is not None and (not p.index_cap or index.numel() * index.element_size() < p.index_bytes):
+            raise ValueError(f"index needs a compressor made with index=True and at least {p.index_bytes} bytes")
+        rc = _lib_async_compress().pco_b200_compress_async(C.byref(p), C.c_void_p(nums.data_ptr()), C.c_void_p(dst.data_ptr()),
+                                                          C.c_void_p(index.data_ptr()) if index is not None else None,
+                                                          C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()),
+                                                          C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+        _lib.check(rc)
+
+    def result(self):
+        """Copies the status of the last call back (waiting for it on the current stream) and returns (file_bytes, index_bytes), or raises
+        PcoError (Io when the file does not fit dst_cap)."""
+        s = _CAsyncCompressStatus.from_buffer_copy(self.status.cpu().numpy().tobytes())
+        nw, il = C.c_size_t(), C.c_size_t()
+        _lib.check(_lib_async_compress().pco_b200_compress_async_result(C.byref(s), C.byref(nw), C.byref(il)))
+        return int(nw.value), int(il.value)
+
+
 class _CModeChoice(C.Structure):
     _fields_ = [("mode_spec", C.c_uint32), ("float_quant_k", C.c_uint32), ("float_mult_base", C.c_double), ("float_mult_inv_base", C.c_double),
                 ("int_mult_base", C.c_uint64), ("bits_saved_per_num", C.c_double)]
