@@ -526,34 +526,6 @@ __global__ void __launch_bounds__(WALK_THREADS, PCOB_WALK_MIN_BLOCKS) walk_kerne
 }
 
 // ---------------------------------------------------------------------------
-// find_chunk_starts_kernel: every byte position in [begin, end) whose 4 bytes equal `pattern` (a chunk's type byte and its 24-bit
-// count - 1, docs/format.md:186-192), appended to `out` in no particular order.  Chunk lengths are not in a standalone file, so the
-// index-free decompressor cannot know where chunk k + 1 starts before it has walked chunk k - but chunks of one file almost always
-// share their first 4 bytes (same type, same count), so every position that LOOKS like such a chunk start is walked speculatively,
-// all in parallel, and the host then follows the chain of (start, end) pairs from the first chunk: a candidate is a real chunk
-// start exactly when a verified chunk ends on it (host_api.cu, decompress_fast 3b).  A thread takes 8 positions.
-// ---------------------------------------------------------------------------
-constexpr int FIND_THREADS = 256;
-constexpr int FIND_PER_THREAD = 8;
-__global__ void __launch_bounds__(FIND_THREADS) find_chunk_starts_kernel(const uint8_t* __restrict__ src, uint64_t begin, uint64_t end, uint32_t pattern,
-                                                                        uint64_t* __restrict__ out, uint32_t cap, uint32_t* __restrict__ count) {
-  const uint64_t p0 = begin + (uint64_t(blockIdx.x) * FIND_THREADS + threadIdx.x) * FIND_PER_THREAD;
-  if (p0 >= end) return;
-  // positions p0 .. p0 + 7 need bytes p0 .. p0 + 10; `end` already leaves room for the 4 bytes of the last position
-  uint32_t b[FIND_PER_THREAD + 3];
-#pragma unroll
-  for (int i = 0; i < FIND_PER_THREAD + 3; i++) b[i] = (p0 + i < end + 3) ? uint32_t(src[p0 + i]) : 0x100u;  // 0x100 never matches
-#pragma unroll
-  for (int i = 0; i < FIND_PER_THREAD; i++) {
-    const uint32_t w = b[i] | (b[i + 1] << 8) | (b[i + 2] << 16) | (b[i + 3] << 24);
-    if (w == pattern && (b[i] | b[i + 1] | b[i + 2] | b[i + 3]) < 0x100u && p0 + i < end) {
-      const uint32_t k = atomicAdd(count, 1u);
-      if (k < cap) out[k] = p0 + i;
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------
 // Latent-type helpers
 // ---------------------------------------------------------------------------
 template <typename L> struct LT;

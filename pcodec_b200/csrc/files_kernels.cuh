@@ -151,8 +151,15 @@ struct FileScan {
   uint32_t pattern, block0;
 };
 
-// As find_chunk_starts_kernel (decode_kernels.cuh), over many files at once: a block finds its file by binary search over block0 and
-// appends (position, file) pairs in no particular order.  Positions past `cap` are counted but not stored.
+// Every byte position in each file's [begin, end) whose 4 bytes equal its `pattern` (a chunk's type byte and its 24-bit count - 1,
+// docs/format.md:186-192).  Chunk lengths are not in a standalone file, so the index-free decompressor cannot know where chunk k + 1
+// starts before it has walked chunk k - but chunks of one file almost always share their first 4 bytes (same type, same count), so
+// every position that LOOKS like such a chunk start is walked speculatively, all in parallel, and the host then follows the chain of
+// (start, end) pairs from the first chunk: a candidate is a real chunk start exactly when a verified chunk ends on it (host_api.cu,
+// speculative_walk_rounds).  A block finds its file by binary search over block0; a thread takes 8 positions.  (position, file) pairs
+// are appended in no particular order; positions past `cap` are counted but not stored.
+constexpr int FIND_THREADS = 256;
+constexpr int FIND_PER_THREAD = 8;
 __global__ void __launch_bounds__(FIND_THREADS) find_file_starts_kernel(const uint8_t* __restrict__ src, const FileScan* __restrict__ scans, uint32_t n_scans,
                                                                        uint64_t* __restrict__ out_pos, uint32_t* __restrict__ out_file, uint32_t cap,
                                                                        uint32_t* __restrict__ count) {

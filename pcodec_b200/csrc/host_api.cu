@@ -275,12 +275,14 @@ static PcoB200Error out_buffer(Context& c, void* dst, bool dst_dev, uint64_t byt
   return PCO_B200_OK;
 }
 
-// Placeholder records for a walk: from `begin` on, each record gets room for MAX_VARS vars of batch entries for its `n` numbers
-// (16-byte aligned).  Returns where the entries end.
+// Room for MAX_VARS vars of batch entries for a chunk of `n` numbers, 16-byte aligned.
+static uint64_t entries_room(uint32_t n) { return (uint64_t(MAX_VARS) * n_batches_of(n) * sizeof(BatchEntry) + 15) & ~uint64_t(15); }
+
+// Placeholder records for a walk: from `begin` on, each record gets entries_room of its `n` numbers.  Returns where the entries end.
 static uint64_t lay_out_entries(IndexChunk* recs, size_t n_recs, uint64_t begin) {
   for (size_t k = 0; k < n_recs; k++) {
     recs[k].entries_offset = begin;
-    begin += (uint64_t(MAX_VARS) * n_batches_of(recs[k].n) * sizeof(BatchEntry) + 15) & ~uint64_t(15);
+    begin += entries_room(recs[k].n);
   }
   return begin;
 }
@@ -330,120 +332,301 @@ static PcoB200Error cold_decode_jobs(Context& c, uint32_t dtype, const std::vect
 static bool cold_retry_file(const ColdResult& r) { return r.status == ST_UNSUPPORTED; }
 static bool cold_retry_chunk(const ColdResult& r) { return r.n_chunks == 0 && r.status == ST_UNSUPPORTED; }
 
-// Index-free decompress, the parallel part (the reference's decompressor walks chunk after chunk, standalone/decompressor.rs:150-215;
-// so does this library's serial walk_kernel<<<1>>>, at one GPU thread's speed).  Chunk lengths are not in the file, but the chunks
-// of a file nearly always start with the same 4 bytes - the type byte and count - 1 (docs/format.md:186-192).  So, from the first
-// unread chunk at `*next_byte`:
-//   1. find_chunk_starts_kernel lists every position behind it that carries the same 4 bytes (the real chunk starts of that size
-//      plus, once per ~4 GB of compressed bytes, a coincidence);
-//   2. walk_kernel walks ALL of them at once, one thread each, as if each were a chunk start: index entries, status, end position;
-//   3. the host follows the chain from the first chunk: the chunk at p is real, it ends at e(p), and if e(p) is on the list the chunk
-//      there is real too (a coincidence is never reached: no verified chunk ends on it).  The verified chunks are decoded by the
-//      ordinary kernels, their output offsets being k * n.
-// The loop repeats from where the chain stopped (chunks of another size - typically the file's last one - start a new pattern) and
-// hands over to the serial walker as soon as a round verifies nothing: the terminator, a chunk that does not fit `dst`, a corrupt or
-// truncated chunk and every other special case keep the serial path's semantics and error reporting.
-// `host_src` is the file in host memory (nullptr when it only lives on the device).  PCOB200_SPECULATIVE_WALK=0 turns this off.
-static PcoB200Error speculative_walk_rounds(Context& c, const FileParams& fp, const uint8_t* host_src, void* dst, uint64_t dst_len, bool dst_dev, size_t elem,
-                                            cudaStream_t stream, uint64_t* next_byte, uint64_t* out_off, void** d_out_io) {
-  {  // read per call: tests of the serial walk switch it off in-process
-    const char* e = std::getenv("PCOB200_SPECULATIVE_WALK");
-    if (e && e[0] == '0') return PCO_B200_OK;
+// Bytes at many positions of `base`, a buffer in host memory or, when `on_device`, in device memory (one readback):
+// out[k * width + j] = base[offs[k] + j] for j < min(width, lens[k]), 0 behind that.
+static PcoB200Error peek(Context& c, const void* base, bool on_device, const std::vector<uint64_t>& offs, const std::vector<uint64_t>& lens, uint32_t width,
+                         std::vector<uint8_t>* out, cudaStream_t stream) {
+  const size_t m = offs.size();
+  out->assign(m * width, 0);
+  if (m == 0) return PCO_B200_OK;
+  if (!on_device) {
+    for (size_t k = 0; k < m; k++) std::memcpy(out->data() + k * width, static_cast<const uint8_t*>(base) + offs[k], std::min<uint64_t>(lens[k], width));
+    return PCO_B200_OK;
   }
-  constexpr uint32_t CAND_CAP = 1u << 16;                  // candidates listed per round
-  constexpr uint64_t INDEX_BUDGET = uint64_t(768) << 20;   // bytes of index scratch per round
+  if (m == 1) {  // a one-file walk: a plain copy costs less than uploading the table
+    PCOB_CUDA_TRY(cudaMemcpyAsync(out->data(), static_cast<const uint8_t*>(base) + offs[0], std::min<uint64_t>(lens[0], width), cudaMemcpyDeviceToHost, stream));
+    PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
+    return PCO_B200_OK;
+  }
+  PCOB_CUDA_TRY(c.files_tab.reserve(m * 16 + 64));
+  PCOB_CUDA_TRY(c.files_res.reserve(m * width + 64));
+  uint64_t* d_offs = c.files_tab.as<uint64_t>();
+  PCOB_CUDA_TRY(cudaMemcpyAsync(d_offs, offs.data(), m * 8, cudaMemcpyHostToDevice, stream));
+  PCOB_CUDA_TRY(cudaMemcpyAsync(d_offs + m, lens.data(), m * 8, cudaMemcpyHostToDevice, stream));
+  peek_bytes_kernel<<<uint32_t((m + 7) / 8), 256, 0, stream>>>(static_cast<const uint8_t*>(base), d_offs, d_offs + m, uint32_t(m), width, c.files_res.as<uint8_t>());
+  PCOB_CUDA_TRY(cudaGetLastError());
+  PCOB_CUDA_TRY(readback_small_sync(out->data(), c.files_res.p, (m * width + 3) & ~size_t(3), stream));
+  return PCO_B200_OK;
+}
+
+// How the walk of an index-free file ended.  COLD: a chunk the fast kernels decline, or one beyond the index scratch (the catch-all
+// decoder still reads such a file); FAILED: any other error.  Both leave the error's kind and message.  OPEN: not walked to an end,
+// because a file in front of it failed.
+enum class WalkEnd { OPEN, TERMINATED, DST_FULL, COLD, FAILED };
+
+// An index-free file for walk_index_free: its bytes src[begin, end), its header, the walk cursor and a cap on its numbers.  The walk
+// stops behind the chunk that takes the count past `cap` (DST_FULL: simple_decompress_into's short destination).  `expect` is the
+// count the serial walker's scratch is sized for: the destination's room for one file, the header's count hint in a batch.  The walk
+// appends the file's chunk records - chunk_offset in src, entries_offset in the arena, out_offset from the file's first number - and
+// counts their numbers.
+struct WalkFile {
+  StandaloneHeader hdr;
+  uint64_t begin = 0, end = 0;
+  uint64_t pos = 0;
+  uint64_t cap = ~uint64_t(0);
+  uint64_t expect = 0;
+  uint64_t count = 0;
+  std::vector<IndexChunk> recs;
+  WalkEnd how = WalkEnd::OPEN;
+  PcoB200Error err = PCO_B200_OK;
+  std::string msg;
+};
+
+// Index-free files, the parallel part (the reference's decompressor walks chunk after chunk, standalone/decompressor.rs:150-215; so does
+// the serial walk_kernel<<<1>>>, at one GPU thread's speed).  Chunk lengths are not in a file, but its chunks nearly always start with
+// the same 4 bytes - the type byte and count - 1 (docs/format.md:186-192).  So in each round, from every file's first unread chunk:
+//   1. find_file_starts_kernel lists every position behind it, inside its file, that carries the same 4 bytes (the real chunk starts
+//      of that size plus, once per ~4 GB of compressed bytes, a coincidence), for all files in one launch;
+//   2. walk_kernel walks ALL of them at once, one CTA each, as if each were a chunk start: index entries, status, end position;
+//   3. the host follows each file's chain from its first chunk: the chunk at p is real, it ends at e(p), and if e(p) is on the list
+//      the chunk there is real too (a coincidence is never reached: no verified chunk ends on it).
+// The rounds repeat from where the chains stopped (chunks of another size - typically a file's last one - start a new pattern).  A
+// file leaves them at its terminator, at a chunk past its cap, with too many candidates, or once a round verifies nothing for it:
+// walk_index_free finishes it.  A round lays out its candidates' entries, then their records, from *arena_end on, and moves *arena_end
+// behind the entries of the last chunk a chain took: the next round reuses the rest.
+static PcoB200Error speculative_walk_rounds(Context& c, const uint8_t* src, bool src_dev, const uint8_t* d_src, size_t src_len, uint32_t dtype,
+                                            const std::vector<WalkFile*>& files, DevBuf& arena, uint64_t* arena_end, cudaStream_t stream) {
+  constexpr uint64_t FILE_CAND_CAP = 1u << 16;             // a file with more candidates is not worth speculating on
+  constexpr uint64_t INDEX_BUDGET = uint64_t(768) << 20;   // bytes of walked records and entries per round
+  const uint32_t n = uint32_t(files.size());
+  const uint32_t cand_cap = uint32_t(std::min<uint64_t>(uint64_t(1) << 22, n * FILE_CAND_CAP));  // candidates listed per round, all files together
+  std::vector<uint8_t> tail(n, 0);                         // 1: the file has left the rounds
+  for (uint32_t i = 0; i < n; i++)
+    if (files[i]->hdr.uniform_type != 0 && files[i]->hdr.uniform_type != dtype) tail[i] = 1;  // no chunk can pass
   for (int round = 0; round < 4096; round++) {
-    const uint64_t pos = *next_byte;
-    if (pos + 4 > fp.src_len) return PCO_B200_OK;
-    uint8_t h4[4];
-    if (host_src) std::memcpy(h4, host_src + pos, 4);
-    else {
-      PCOB_CUDA_TRY(cudaMemcpyAsync(h4, static_cast<const uint8_t*>(fp.src) + pos, 4, cudaMemcpyDeviceToHost, stream));
-      PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
+    std::vector<uint32_t> act;
+    std::vector<uint64_t> offs, lens;
+    for (uint32_t i = 0; i < n; i++)
+      if (!tail[i]) {
+        if (files[i]->pos + 4 > files[i]->end) { tail[i] = 1; continue; }
+        act.push_back(i);
+        offs.push_back(files[i]->pos);
+        lens.push_back(4);
+      }
+    if (act.empty()) break;
+    std::vector<uint8_t> h4;
+    if (PcoB200Error e = peek(c, src, src_dev, offs, lens, 4, &h4, stream)) return e;
+    std::vector<FileScan> scans;
+    std::vector<uint32_t> scan_file;
+    uint64_t blocks = 0;
+    const uint64_t per_block = uint64_t(FIND_THREADS) * FIND_PER_THREAD;
+    for (size_t k = 0; k < act.size(); k++) {
+      const uint32_t i = act[k];
+      const uint8_t* b = h4.data() + k * 4;
+      // the terminator, or a type byte the serial walker reports; or a chunk past the cap, whose semantics the serial walker owns
+      if (b[0] != dtype || files[i]->count + ((uint32_t(b[1]) | (uint32_t(b[2]) << 8) | (uint32_t(b[3]) << 16)) + 1) > files[i]->cap) {
+        tail[i] = 1;
+        continue;
+      }
+      FileScan s;
+      s.begin = files[i]->pos;
+      s.end = files[i]->end - 3;  // last position + 1 whose 4 bytes lie inside the file
+      s.pattern = uint32_t(b[0]) | (uint32_t(b[1]) << 8) | (uint32_t(b[2]) << 16) | (uint32_t(b[3]) << 24);
+      s.block0 = uint32_t(blocks);
+      blocks += (s.end - s.begin + per_block - 1) / per_block;
+      scans.push_back(s);
+      scan_file.push_back(i);
     }
-    if (h4[0] != fp.dtype) return PCO_B200_OK;  // the terminator (0), or a type byte the serial path will report
-    const uint32_t n0 = (uint32_t(h4[1]) | (uint32_t(h4[2]) << 8) | (uint32_t(h4[3]) << 16)) + 1;
-    if (*out_off + n0 > dst_len) return PCO_B200_OK;  // the serial path owns the too-small-destination semantics
-    const uint32_t pattern = uint32_t(h4[0]) | (uint32_t(h4[1]) << 8) | (uint32_t(h4[2]) << 16) | (uint32_t(h4[3]) << 24);
-    // scratch: count | candidate positions | chunk ends | statuses
-    PCOB_CUDA_TRY(c.spec.reserve(64 + size_t(CAND_CAP) * (8 + 8 + 4)));
+    if (scans.empty()) break;
+    if (blocks > 0x7fffffffull) { for (uint32_t i : scan_file) tail[i] = 1; break; }
+    // scratch: count | candidate positions | their files | statuses | chunk ends
+    PCOB_CUDA_TRY(c.spec.reserve(64 + size_t(cand_cap) * (8 + 4)));
+    PCOB_CUDA_TRY(c.files_tab.reserve(scans.size() * sizeof(FileScan) + 64));
     uint32_t* d_count = c.spec.as<uint32_t>();
     uint64_t* d_cand = reinterpret_cast<uint64_t*>(c.spec.as<uint8_t>() + 64);
-    uint64_t* d_ends = d_cand + CAND_CAP;
-    uint32_t* d_stat = reinterpret_cast<uint32_t*>(d_ends + CAND_CAP);
+    uint32_t* d_cfile = reinterpret_cast<uint32_t*>(d_cand + cand_cap);
+    PCOB_CUDA_TRY(cudaMemcpyAsync(c.files_tab.p, scans.data(), scans.size() * sizeof(FileScan), cudaMemcpyHostToDevice, stream));
     PCOB_CUDA_TRY(cudaMemsetAsync(d_count, 0, 4, stream));
-    const uint64_t scan_end = fp.src_len - 3;  // last position + 1 whose 4 bytes lie inside the file
-    const uint64_t per_block = uint64_t(FIND_THREADS) * FIND_PER_THREAD;
-    const uint64_t blocks = (scan_end - pos + per_block - 1) / per_block;
-    if (blocks > 0x7fffffffull) return PCO_B200_OK;
-    profiler().begin("find_chunk_starts_kernel", stream);
-    find_chunk_starts_kernel<<<uint32_t(blocks), FIND_THREADS, 0, stream>>>(static_cast<const uint8_t*>(fp.src), pos, scan_end, pattern, d_cand, CAND_CAP, d_count);
+    profiler().begin("find_file_starts_kernel", stream);
+    find_file_starts_kernel<<<uint32_t(blocks), FIND_THREADS, 0, stream>>>(d_src, c.files_tab.as<FileScan>(), uint32_t(scans.size()), d_cand, d_cfile, cand_cap, d_count);
     profiler().end(stream);
     PCOB_CUDA_TRY(cudaGetLastError());
     uint32_t count = 0;
-    PCOB_CUDA_TRY(cudaMemcpyAsync(&count, d_count, 4, cudaMemcpyDeviceToHost, stream));
+    PCOB_CUDA_TRY(readback_small_sync(&count, d_count, 4, stream));
+    if (count > cand_cap) { for (uint32_t i : scan_file) tail[i] = 1; break; }
+    std::vector<uint64_t> cpos(count);
+    std::vector<uint32_t> cfile(count);
+    PCOB_CUDA_TRY(cudaMemcpyAsync(cpos.data(), d_cand, size_t(count) * 8, cudaMemcpyDeviceToHost, stream));
+    PCOB_CUDA_TRY(cudaMemcpyAsync(cfile.data(), d_cfile, size_t(count) * 4, cudaMemcpyDeviceToHost, stream));
     PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
-    if (count == 0 || count > CAND_CAP) return PCO_B200_OK;  // a file full of the pattern: not worth speculating on
-    std::vector<uint64_t> cand(count);
-    PCOB_CUDA_TRY(cudaMemcpyAsync(cand.data(), d_cand, size_t(count) * 8, cudaMemcpyDeviceToHost, stream));
-    PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
-    std::sort(cand.begin(), cand.end());
-    if (cand[0] != pos) return PCO_B200_OK;
-    // walk as many candidates (in file order) as the index budget and the destination allow
-    const uint32_t nb0 = n_batches_of(n0);
-    const uint64_t stride = (uint64_t(MAX_VARS) * nb0 * sizeof(BatchEntry) + 15) & ~uint64_t(15);
-    const uint64_t fit = (dst_len - *out_off) / n0;  // chunks of this size the destination can still take (>= 1)
-    uint64_t m64 = std::min<uint64_t>(count, std::max<uint64_t>(1, INDEX_BUDGET / (stride + sizeof(IndexChunk))));
-    m64 = std::min<uint64_t>(m64, fit + 8);  // a few more than fit: coincidences in front of the last chunk needed
-    const uint32_t m = uint32_t(m64);
-    const uint64_t chunks_offset = sizeof(IndexHeader);
-    std::vector<IndexChunk> recs(m);
-    for (uint32_t k = 0; k < m; k++) {
-      recs[k].chunk_offset = cand[k];
-      recs[k].n = n0;
-      recs[k].n_vars = 0;
-      recs[k].out_offset = 0;
+    std::vector<std::vector<uint64_t>> cand(scans.size());
+    for (uint32_t k = 0; k < count; k++) cand[cfile[k]].push_back(cpos[k]);
+    // the round's walk: every file's candidates (as many as its budget share and its cap allow), one CTA each.  FileParams carries one
+    // uniform type and format version per launch, so the records are laid out flavour by flavour and each flavour present is one launch.
+    auto flavour = [&](uint32_t i) { return (files[i]->hdr.uniform_type << 8) | files[i]->hdr.format_major; };
+    std::vector<uint32_t> scan_order(scans.size());
+    for (size_t s = 0; s < scans.size(); s++) scan_order[s] = uint32_t(s);
+    std::stable_sort(scan_order.begin(), scan_order.end(), [&](uint32_t a, uint32_t b) { return flavour(scan_file[a]) < flavour(scan_file[b]); });
+    std::vector<IndexChunk> recs;
+    std::vector<uint32_t> walked;           // scan index of each file walked this round
+    std::vector<size_t> first_rec;          // its first record
+    uint64_t budget = INDEX_BUDGET;
+    for (uint32_t s : scan_order) {
+      const uint32_t i = scan_file[s];
+      const WalkFile& f = *files[i];
+      std::vector<uint64_t>& cs = cand[s];
+      std::sort(cs.begin(), cs.end());
+      if (cs.empty() || cs.size() > FILE_CAND_CAP || cs[0] != f.pos) { tail[i] = 1; continue; }
+      const uint32_t n0 = ((scans[s].pattern >> 8) & 0xffffffu) + 1;
+      const uint64_t stride = entries_room(n0);
+      const uint64_t fit = std::min((f.cap - f.count) / n0, FILE_CAND_CAP);  // chunks of this size the cap still takes (>= 1)
+      // a few more candidates than fit: coincidences may lie in front of the last chunk that does
+      uint64_t m = std::min<uint64_t>({cs.size(), std::max<uint64_t>(1, INDEX_BUDGET / (stride + sizeof(IndexChunk))), fit + 8});
+      if (!walked.empty() && m * (stride + sizeof(IndexChunk)) > budget) continue;  // waits for the next round
+      budget -= std::min(budget, m * (stride + sizeof(IndexChunk)));
+      cs.resize(m);
+      walked.push_back(uint32_t(s));
+      first_rec.push_back(recs.size());
+      for (uint64_t k = 0; k < m; k++) {
+        IndexChunk ic;
+        ic.chunk_offset = cs[k];
+        ic.n = n0;
+        ic.n_vars = 0;
+        ic.out_offset = 0;
+        recs.push_back(ic);
+      }
     }
-    const uint64_t index_bytes = lay_out_entries(recs.data(), m, (chunks_offset + uint64_t(m) * sizeof(IndexChunk) + 15) & ~uint64_t(15));
-    PCOB_CUDA_TRY(c.index.reserve(index_bytes + 64));
-    uint8_t* d_index = c.index.as<uint8_t>();
-    PCOB_CUDA_TRY(cudaMemcpyAsync(d_index + chunks_offset, recs.data(), size_t(m) * sizeof(IndexChunk), cudaMemcpyHostToDevice, stream));
-    PCOB_CUDA_TRY(cudaMemsetAsync(d_stat, 0xff, size_t(m) * 4, stream));
-    PCOB_CUDA_TRY(cudaMemsetAsync(d_ends, 0, size_t(m) * 8, stream));
+    if (recs.empty()) break;
+    const uint32_t mt = uint32_t(recs.size());
+    const uint64_t chunks_at = lay_out_entries(recs.data(), mt, (*arena_end + 15) & ~uint64_t(15));  // the records behind the entries
+    PCOB_CUDA_TRY(arena.grow_preserve(chunks_at + uint64_t(mt) * sizeof(IndexChunk) + 64, *arena_end, stream));
+    PCOB_CUDA_TRY(c.spec.reserve(64 + size_t(cand_cap) * (8 + 4) + size_t(mt) * (4 + 8) + 64));
+    uint32_t* d_stat = reinterpret_cast<uint32_t*>(c.spec.as<uint8_t>() + 64 + size_t(cand_cap) * 12);
+    uint64_t* d_ends = reinterpret_cast<uint64_t*>(c.spec.as<uint8_t>() + 64 + size_t(cand_cap) * 12 + ((size_t(mt) * 4 + 15) & ~size_t(15)));
+    PCOB_CUDA_TRY(cudaMemcpyAsync(arena.as<uint8_t>() + chunks_at, recs.data(), size_t(mt) * sizeof(IndexChunk), cudaMemcpyHostToDevice, stream));
+    PCOB_CUDA_TRY(cudaMemsetAsync(d_stat, 0xff, size_t(mt) * 4, stream));
+    PCOB_CUDA_TRY(cudaMemsetAsync(d_ends, 0, size_t(mt) * 8, stream));
     PCOB_CUDA_TRY(c.misc.reserve(sizeof(WalkResult)));
-    profiler().begin("walk_kernel", stream);
-    walk_kernel<SMALL_MAX_SIZE_LOG><<<m, WALK_THREADS, sizeof(WalkSmem<SMALL_MAX_SIZE_LOG>), stream>>>(
-        fp, d_index, chunks_offset, m, 0, index_bytes, 0, 0, ~uint64_t(0), d_stat, c.misc.as<WalkResult>(), 0, d_ends);
-    profiler().end(stream);
-    PCOB_CUDA_TRY(cudaGetLastError());
-    std::vector<uint32_t> st(m);
-    std::vector<uint64_t> ends(m);
-    PCOB_CUDA_TRY(cudaMemcpyAsync(st.data(), d_stat, size_t(m) * 4, cudaMemcpyDeviceToHost, stream));
-    PCOB_CUDA_TRY(cudaMemcpyAsync(ends.data(), d_ends, size_t(m) * 8, cudaMemcpyDeviceToHost, stream));
-    PCOB_CUDA_TRY(cudaMemcpyAsync(recs.data(), d_index + chunks_offset, size_t(m) * sizeof(IndexChunk), cudaMemcpyDeviceToHost, stream));  // n_vars as walked
+    for (size_t w0 = 0; w0 < walked.size();) {  // one launch per flavour: its walked files' records are consecutive
+      const uint32_t fl = flavour(scan_file[walked[w0]]);
+      size_t w1 = w0 + 1;
+      while (w1 < walked.size() && flavour(scan_file[walked[w1]]) == fl) w1++;
+      const size_t r_lo = first_rec[w0], r_hi = w1 < walked.size() ? first_rec[w1] : recs.size();
+      const FileParams fp{d_src, src_len, dtype, fl >> 8, fl & 0xff};
+      profiler().begin("walk_kernel", stream);
+      walk_kernel<SMALL_MAX_SIZE_LOG><<<uint32_t(r_hi - r_lo), WALK_THREADS, sizeof(WalkSmem<SMALL_MAX_SIZE_LOG>), stream>>>(
+          fp, arena.as<uint8_t>(), chunks_at + r_lo * sizeof(IndexChunk), uint32_t(r_hi - r_lo), 0, chunks_at, 0, 0, ~uint64_t(0), d_stat + r_lo,
+          c.misc.as<WalkResult>(), 0, d_ends + r_lo);
+      profiler().end(stream);
+      PCOB_CUDA_TRY(cudaGetLastError());
+      w0 = w1;
+    }
+    std::vector<uint32_t> st(mt);
+    std::vector<uint64_t> ends(mt);
+    PCOB_CUDA_TRY(cudaMemcpyAsync(st.data(), d_stat, size_t(mt) * 4, cudaMemcpyDeviceToHost, stream));
+    PCOB_CUDA_TRY(cudaMemcpyAsync(ends.data(), d_ends, size_t(mt) * 8, cudaMemcpyDeviceToHost, stream));
+    PCOB_CUDA_TRY(cudaMemcpyAsync(recs.data(), arena.as<uint8_t>() + chunks_at, size_t(mt) * sizeof(IndexChunk), cudaMemcpyDeviceToHost, stream));  // n_vars as walked
     PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
-    // the chain of real chunks
-    uint64_t p = pos;
-    const std::vector<uint32_t> chain = follow_chunk_chain(cand.data(), st.data(), ends.data(), m, pos, n0, *out_off, dst_len, fp.src_len, &p);
-    std::vector<IndexChunk> real;
-    real.reserve(chain.size());
-    for (uint32_t k : chain) {
-      IndexChunk ic = recs[k];
-      ic.out_offset = *out_off + uint64_t(real.size()) * n0;
-      real.push_back(ic);
+    bool progress = false;
+    uint64_t kept_end = *arena_end;
+    for (size_t w = 0; w < walked.size(); w++) {
+      const uint32_t s = walked[w], i = scan_file[s];
+      WalkFile& f = *files[i];
+      const size_t r0 = first_rec[w];
+      const uint32_t m = uint32_t(cand[s].size());
+      const uint32_t n0 = recs[r0].n;
+      uint64_t p = f.pos;
+      const std::vector<uint32_t> chain = follow_chunk_chain(cand[s].data(), st.data() + r0, ends.data() + r0, m, f.pos, n0, f.count, f.cap, f.end, &p);
+      if (chain.empty()) { tail[i] = 1; continue; }
+      for (uint32_t k : chain) {
+        IndexChunk ic = recs[r0 + k];
+        ic.out_offset = f.count;
+        f.count += n0;
+        f.recs.push_back(ic);
+        kept_end = std::max(kept_end, ic.entries_offset + entries_room(n0));
+      }
+      f.pos = p;
+      progress = true;
     }
-    if (real.empty()) return PCO_B200_OK;
-    PCOB_CUDA_TRY(cudaMemcpyAsync(d_index + chunks_offset, real.data(), real.size() * sizeof(IndexChunk), cudaMemcpyHostToDevice, stream));
-    const uint64_t emit_end = *out_off + uint64_t(real.size()) * n0;
-    void* d_out = dst;
-    if (!dst_dev) {
-      PCOB_CUDA_TRY(c.out.grow_preserve(emit_end * elem + 64, *out_off * elem, stream));
-      d_out = c.out.p;
+    *arena_end = kept_end;
+    if (!progress) break;
+  }
+  return PCO_B200_OK;
+}
+
+// Walks index-free files to their end: the speculative rounds (PCOB200_SPECULATIVE_WALK=0 skips them), then a peek at every file's
+// next byte - a file the rounds walked to its terminator is done - and the serial walker, one file at a time, for every other file.
+// So the terminator, a chunk past the cap, a corrupt or truncated chunk and every other special case keep the serial walker's semantics
+// and error reporting.  The serial walks go in list order and stop at the first file that fails: a caller that reports the lowest
+// failing file needs nothing behind it, and those files stay OPEN.  `src` is the caller's buffer (in device memory when src_dev),
+// `d_src` its bytes in HBM; the walked chunks' entries go into `arena` from *arena_end on, which moves behind them.
+static PcoB200Error walk_index_free(Context& c, const uint8_t* src, bool src_dev, const uint8_t* d_src, size_t src_len, uint32_t dtype,
+                                    const std::vector<WalkFile*>& files, DevBuf& arena, uint64_t* arena_end, cudaStream_t stream) {
+  *arena_end = std::max<uint64_t>(*arena_end, 16);  // entries_offset 0 means "no entries" to the decode kernels
+  const char* spec = std::getenv("PCOB200_SPECULATIVE_WALK");  // read per call: tests of the serial walk switch it off in-process
+  if (!(spec && spec[0] == '0'))
+    if (PcoB200Error e = speculative_walk_rounds(c, src, src_dev, d_src, src_len, dtype, files, arena, arena_end, stream)) return e;
+  std::vector<uint8_t> done(files.size(), 0);
+  {
+    std::vector<size_t> at;
+    std::vector<uint64_t> offs, lens;
+    for (size_t k = 0; k < files.size(); k++)
+      if (files[k]->pos < files[k]->end) {
+        at.push_back(k);
+        offs.push_back(files[k]->pos);
+        lens.push_back(1);
+      }
+    std::vector<uint8_t> b;
+    if (PcoB200Error e = peek(c, src, src_dev, offs, lens, 4, &b, stream)) return e;
+    for (size_t j = 0; j < at.size(); j++)
+      if (b[j * 4] == 0) done[at[j]] = 1;
+  }
+  PCOB_CUDA_TRY(c.misc.reserve(sizeof(WalkResult)));
+  for (size_t k = 0; k < files.size(); k++) {
+    WalkFile& f = *files[k];
+    f.how = WalkEnd::TERMINATED;
+    if (done[k]) continue;
+    const FileParams fpf{d_src + f.begin, f.end - f.begin, dtype, f.hdr.uniform_type, f.hdr.format_major};
+    const uint32_t max_chunks = uint32_t(std::min<uint64_t>((f.end - f.begin) / 5 + 2, 1u << 16));
+    uint64_t next = f.pos - f.begin;
+    for (;;) {
+      // entries for the batches still to come (by `expect`) plus 2 per chunk, for 2 vars; then room for the records, which the next
+      // round reuses
+      const uint64_t entries_begin = (*arena_end + 15) & ~uint64_t(15);
+      uint64_t want_batches = (f.expect > f.count ? (f.expect - f.count) / BATCH_N : 0) + 2ull * max_chunks + 2;
+      want_batches = std::min<uint64_t>(want_batches, uint64_t(1) << 23);
+      const uint64_t entries_end = entries_begin + want_batches * MAX_VARS * sizeof(BatchEntry) + 16ull * max_chunks + 64;
+      const uint64_t chunks_at = (entries_end + 15) & ~uint64_t(15);
+      PCOB_CUDA_TRY(arena.grow_preserve(chunks_at + uint64_t(max_chunks) * sizeof(IndexChunk) + 64, *arena_end, stream));
+      profiler().begin("walk_kernel", stream);
+      walk_kernel<12><<<1, WALK_THREADS, sizeof(WalkSmem<12>), stream>>>(fpf, arena.as<uint8_t>(), chunks_at, max_chunks, entries_begin, entries_end, next, f.count,
+                                                                        f.cap, nullptr, c.misc.as<WalkResult>(), 1);
+      profiler().end(stream);
+      PCOB_CUDA_TRY(cudaGetLastError());
+      WalkResult res;
+      PCOB_CUDA_TRY(readback_small_sync(&res, c.misc.p, sizeof(res), stream));
+      if (res.n_chunks > 0) {
+        std::vector<IndexChunk> got(res.n_chunks);
+        PCOB_CUDA_TRY(cudaMemcpyAsync(got.data(), arena.as<uint8_t>() + chunks_at, got.size() * sizeof(IndexChunk), cudaMemcpyDeviceToHost, stream));
+        PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
+        for (IndexChunk& ic : got) {
+          ic.chunk_offset += f.begin;
+          f.recs.push_back(ic);
+        }
+        *arena_end = res.entries_end;
+      }
+      f.count += res.n_total;
+      next = res.next_byte;
+      if (res.status == ST_TERMINATOR) break;
+      if (res.status == ST_DST_FULL) { f.how = WalkEnd::DST_FULL; break; }
+      if (res.status == ST_INDEX_FULL && res.n_chunks > 0) continue;
+      f.how = res.status == ST_UNSUPPORTED || res.status == ST_INDEX_FULL ? WalkEnd::COLD : WalkEnd::FAILED;
+      f.err = res.status == ST_INDEX_FULL ? fail(PCO_B200_UNSUPPORTED, "a single chunk exceeds the device index scratch")
+                                          : status_to_error(res.status, ("chunk " + std::to_string(res.n_chunks) + " of this walk round").c_str());
+      f.msg = last_error_ref();
+      break;
     }
-    if (PcoB200Error e = launch_decode(c, fp, d_index, index_bytes, chunks_offset, uint32_t(real.size()), d_out, dst_dev ? dst_len : emit_end, stream)) return e;
-    *d_out_io = d_out;
-    *out_off = emit_end;
-    *next_byte = p;
+    if (f.how == WalkEnd::FAILED) break;
   }
   return PCO_B200_OK;
 }
@@ -506,54 +689,28 @@ static PcoB200Error decompress_fast(const void* compressed, size_t compressed_le
     return PCO_B200_OK;
   }
 
-  // 3b. no index: walk the file on the device in rounds, decoding each round's chunks.
-  // Chunk boundaries are not in the stream, so this is one serial tANS walk (cold path).
-  const uint32_t max_chunks = uint32_t(std::min<uint64_t>(uint64_t(compressed_len) / 5 + 2, 1u << 16));
-  uint64_t next_byte = hdr.first_chunk_byte;
-  uint64_t out_off = 0;
-  void* d_out = dst;
-  // runs of same-sized chunks are found, walked and decoded in parallel; what is left (the terminator at least) goes through the serial walk
-  if (PcoB200Error e = speculative_walk_rounds(c, fp, src_dev ? nullptr : static_cast<const uint8_t*>(compressed), dst, uint64_t(dst_len), dst_dev, elem, stream,
-                                               &next_byte, &out_off, &d_out))
+  // 3b. no index: walk the file (walk_index_free), then decode every chunk walked in one launch.  The kernels write no number past dst_len:
+  // a destination that ends inside a chunk gets that chunk's first numbers.
+  WalkFile f;
+  f.hdr = hdr;
+  f.end = compressed_len;
+  f.pos = hdr.first_chunk_byte;
+  f.cap = f.expect = dst_len;
+  uint64_t arena_end = 0;
+  if (PcoB200Error e = walk_index_free(c, static_cast<const uint8_t*>(compressed), src_dev, d_src, compressed_len, dtype, {&f}, c.index, &arena_end, stream)) return e;
+  const uint64_t n_emit = std::min<uint64_t>(f.count, dst_len);
+  void* d_out;
+  if (PcoB200Error e = out_buffer(c, dst, dst_dev, n_emit * elem, &d_out)) return e;
+  const uint64_t list_at = (arena_end + 15) & ~uint64_t(15), list_end = list_at + f.recs.size() * sizeof(IndexChunk);
+  PCOB_CUDA_TRY(c.index.grow_preserve(list_end + 64, arena_end, stream));
+  if (!f.recs.empty())
+    PCOB_CUDA_TRY(cudaMemcpyAsync(c.index.as<uint8_t>() + list_at, f.recs.data(), f.recs.size() * sizeof(IndexChunk), cudaMemcpyHostToDevice, stream));
+  // the chunks in front of a failing one are decoded too, as the reference emits them; a failing decode is the error that wins
+  if (PcoB200Error e = launch_decode(c, fp, c.index.as<uint8_t>(), list_end, list_at, uint32_t(f.recs.size()), d_out, dst_dev ? uint64_t(dst_len) : n_emit, stream))
     return e;
-  PCOB_CUDA_TRY(c.misc.reserve(sizeof(WalkResult)));
-  WalkResult* d_res = c.misc.as<WalkResult>();
-  for (;;) {
-    // scratch index: header | IndexChunk[max_chunks] | entries for the batches dst can still take (+2 per chunk) x 2 vars
-    const uint64_t chunks_offset = sizeof(IndexHeader);
-    const uint64_t entries_begin = chunks_offset + uint64_t(max_chunks) * sizeof(IndexChunk);
-    uint64_t want_batches = (dst_len > out_off ? (dst_len - out_off) / BATCH_N : 0) + 2ull * max_chunks + 2;
-    want_batches = std::min<uint64_t>(want_batches, uint64_t(1) << 23);
-    const uint64_t entries_bytes = want_batches * MAX_VARS * sizeof(BatchEntry) + 16ull * max_chunks + 64;
-    PCOB_CUDA_TRY(c.index.reserve(entries_begin + entries_bytes));
-    uint8_t* d_index = c.index.as<uint8_t>();
-    profiler().begin("walk_kernel", stream);
-    walk_kernel<12><<<1, WALK_THREADS, sizeof(WalkSmem<12>), stream>>>(fp, d_index, chunks_offset, max_chunks, entries_begin, entries_begin + entries_bytes,
-                                                      next_byte, out_off, uint64_t(dst_len), nullptr, d_res, 1);
-    profiler().end(stream);
-    PCOB_CUDA_TRY(cudaGetLastError());
-    WalkResult res;
-    PCOB_CUDA_TRY(cudaMemcpyAsync(&res, d_res, sizeof(res), cudaMemcpyDeviceToHost, stream));
-    PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
-    const bool soft = res.status == ST_TERMINATOR || res.status == ST_INDEX_FULL || res.status == ST_DST_FULL;
-    // decode what was indexed this round (the reference also emits the chunks before a failing one)
-    if (res.n_chunks > 0) {
-      uint64_t round_emit_end = std::min<uint64_t>(out_off + res.n_total, dst_len);
-      if (!dst_dev) {
-        PCOB_CUDA_TRY(c.out.grow_preserve(round_emit_end * elem + 64, std::min<uint64_t>(out_off, dst_len) * elem, stream));
-        d_out = c.out.p;
-      }
-      if (PcoB200Error e = launch_decode(c, fp, d_index, entries_begin + entries_bytes, chunks_offset, res.n_chunks, d_out, dst_dev ? uint64_t(dst_len) : round_emit_end, stream)) return e;
-    }
-    out_off += res.n_total;
-    next_byte = res.next_byte;
-    if (!soft) return status_to_error(res.status, ("chunk " + std::to_string(res.n_chunks) + " of this walk round").c_str());
-    if (res.status == ST_TERMINATOR) { outcome->terminated = true; break; }
-    if (res.status == ST_DST_FULL) break;
-    if (res.n_chunks == 0) return fail(PCO_B200_UNSUPPORTED, "a single chunk exceeds the device index scratch");
-  }
-  outcome->n_total = out_off;
-  uint64_t n_emit = std::min<uint64_t>(out_off, dst_len);
+  if (f.how == WalkEnd::COLD || f.how == WalkEnd::FAILED) return fail(f.err, f.msg);  // decompress_core takes a cold file to the catch-all decoder
+  outcome->n_total = f.count;
+  outcome->terminated = f.how == WalkEnd::TERMINATED;
   if (!dst_dev && n_emit) {
     PCOB_CUDA_TRY(copy_sliced(dst, d_out, n_emit * elem, cudaMemcpyDeviceToHost, stream));
     PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
@@ -1625,28 +1782,22 @@ PcoB200Error pco_b200_compress_files(const void* nums, const uint64_t* file_ns, 
 // in place and the whole batch is ONE chunk list for the ordinary decode kernels (one launch_decode per header flavour and format
 // version, which FileParams carries per launch):
 //   1. the files' heads (and index headers) come back in one readback and are parsed on the host;
-//   2. index-free files are walked together: each round peeks every unfinished file's next 4 bytes, finds every file's candidate
-//      chunk starts in one find_file_starts_kernel launch, walks all candidates in one walk_kernel launch and follows each file's
-//      chain on the host (speculative_walk_rounds, for many files).  The walked records stay in an arena beside the staged indexes;
-//   3. a file whose next byte is then its terminator is done; any other (a chunk of odd size, corruption, truncation, an older
-//      format, a cold chunk) finishes on the serial walker, one file at a time, with the single-file semantics;
-//   4. check_index_kernel tests every indexed file's records against its own file (a file that fails decodes on its own, through
+//   2. index-free files are walked together (walk_index_free): speculative rounds over all of them, then the serial walker for each
+//      file the rounds did not take to its terminator.  The walked records stay in an arena beside the staged indexes; a file whose
+//      walk meets a chunk the fast kernels decline is cold;
+//   3. check_index_kernel tests every indexed file's records against its own file (a file that fails decodes on its own, through
 //      decompress_core) and marks cold files; then
 //      merge_index_kernel writes the indexed files' records, rebased, into the list beside the walked ones; launch_decode runs over
 //      it.  A failing chunk names its file: a chunk the fast kernels decline makes that file cold and the list is decoded again
 //      without it; any other failure drops the files from it on and the rest is decoded again, so that the lowest failure is found;
-//   5. cold files go through cold_decode_kernel, one launch per file.
-struct BatchFile {
-  StandaloneHeader hdr;
-  bool indexed = false, walk = false, done = false, cold = false, staged = false;
+//   4. cold files go through cold_decode_kernel, one launch per file.
+// A file of the batch.  An indexed file uses hdr, begin, end and count (from its index) of WalkFile; an index-free one all of it.
+struct BatchFile : WalkFile {
+  bool indexed = false, walk = false, cold = false, staged = false;
   bool alone = false;            // indexed, with a record outside its own file: decoded by itself, as decompress_ex decodes it
-  uint64_t count = 0;            // numbers: from the index, or walked so far
-  uint64_t begin = 0, end = 0;   // the file's bytes in src
-  uint64_t pos = 0;              // walk cursor (byte in src)
   uint64_t idx_recs = 0;         // indexed: byte offset of its IndexChunk[0] in the arena
   uint64_t idx_base = 0;         // indexed: byte offset of its index in the arena
   uint64_t n_idx_chunks = 0;
-  std::vector<IndexChunk> recs;  // walked: chunk_offset in src, entries_offset in the arena, out_offset from the file's first number
   uint64_t out_base = 0;
   uint64_t staged_at = 0;        // cold without index: element offset of its numbers in files_cold
 };
@@ -1674,7 +1825,6 @@ static PcoB200Error decompress_files_impl(const void* src, size_t src_len, const
   Context& c = ctx();
   if (PcoB200Error e = ensure_device(c)) return e;
   static const bool cold_ok = [] { const char* v = std::getenv("PCOB200_COLD_DECODE"); return !(v && v[0] == '0'); }();
-  const bool spec_ok = [] { const char* v = std::getenv("PCOB200_SPECULATIVE_WALK"); return !(v && v[0] == '0'); }();
   const bool src_dev = flags & PCO_B200_SRC_ON_DEVICE, dst_dev = flags & PCO_B200_DST_ON_DEVICE, idx_dev = flags & PCO_B200_INDEX_ON_DEVICE;
   const size_t elem = nt_bits(dtype) / 8;
   const uint32_t n = uint32_t(n_files);
@@ -1693,27 +1843,6 @@ static PcoB200Error decompress_files_impl(const void* src, size_t src_len, const
   PCOB_CUDA_TRY(c.files_arena.reserve(arena_end + 64));
   if (any_index) PCOB_CUDA_TRY(copy_sliced(c.files_arena.p, index, index_len, idx_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, stream));
   auto arena = [&]() { return c.files_arena.as<uint8_t>(); };
-  // bytes at many positions of a device buffer, in one readback
-  auto peek = [&](const uint8_t* d_base, const std::vector<uint64_t>& offs, const std::vector<uint64_t>& lens, uint32_t width, std::vector<uint8_t>* out) -> PcoB200Error {
-    const size_t m = offs.size();
-    out->assign(m * width, 0);
-    if (m == 0) return PCO_B200_OK;
-    PCOB_CUDA_TRY(c.files_tab.reserve(m * 16 + 64));
-    PCOB_CUDA_TRY(c.files_res.reserve(m * width + 64));
-    uint64_t* d_offs = c.files_tab.as<uint64_t>();
-    PCOB_CUDA_TRY(cudaMemcpyAsync(d_offs, offs.data(), m * 8, cudaMemcpyHostToDevice, stream));
-    PCOB_CUDA_TRY(cudaMemcpyAsync(d_offs + m, lens.data(), m * 8, cudaMemcpyHostToDevice, stream));
-    peek_bytes_kernel<<<uint32_t((m + 7) / 8), 256, 0, stream>>>(d_base, d_offs, d_offs + m, uint32_t(m), width, c.files_res.as<uint8_t>());
-    PCOB_CUDA_TRY(cudaGetLastError());
-    PCOB_CUDA_TRY(readback_small_sync(out->data(), c.files_res.p, (m * width + 3) & ~size_t(3), stream));
-    return PCO_B200_OK;
-  };
-  auto peek_src = [&](const std::vector<uint64_t>& offs, const std::vector<uint64_t>& lens, uint32_t width, std::vector<uint8_t>* out) -> PcoB200Error {
-    if (src_dev) return peek(d_src, offs, lens, width, out);
-    out->assign(offs.size() * width, 0);
-    for (size_t k = 0; k < offs.size(); k++) std::memcpy(out->data() + k * width, static_cast<const uint8_t*>(src) + offs[k], std::min<uint64_t>(lens[k], width));
-    return PCO_B200_OK;
-  };
 
   // ---- 1. heads and index headers
   std::vector<BatchFile> bf(n_files);
@@ -1730,13 +1859,8 @@ static PcoB200Error decompress_files_impl(const void* src, size_t src_len, const
       }
     }
     std::vector<uint8_t> heads, iheads;
-    if (PcoB200Error e = peek_src(offs, lens, 32, &heads)) return e;
-    if (idx_dev) {
-      if (PcoB200Error e = peek(arena(), ioffs, ilens, sizeof(IndexHeader), &iheads)) return e;
-    } else {
-      iheads.assign(ioffs.size() * sizeof(IndexHeader), 0);
-      for (size_t k = 0; k < ioffs.size(); k++) std::memcpy(iheads.data() + k * sizeof(IndexHeader), static_cast<const uint8_t*>(index) + ioffs[k], sizeof(IndexHeader));
-    }
+    if (PcoB200Error e = peek(c, src, src_dev, offs, lens, 32, &heads, stream)) return e;
+    if (PcoB200Error e = peek(c, index, idx_dev, ioffs, ilens, sizeof(IndexHeader), &iheads, stream)) return e;
     size_t wi = 0;
     for (uint32_t i = 0; i < n; i++) {
       BatchFile& f = bf[i];
@@ -1764,216 +1888,22 @@ static PcoB200Error decompress_files_impl(const void* src, size_t src_len, const
       } else {
         f.walk = true;
         f.pos = r.offset + f.hdr.first_chunk_byte;
+        f.expect = f.hdr.n_hint;
       }
     }
   }
 
-  // ---- 2. index-free files: speculative rounds over all of them at once
-  constexpr uint32_t CAND_CAP = 1u << 22;                  // candidates listed per round, all files together
-  constexpr uint32_t FILE_CAND_CAP = 1u << 16;             // a file with more is not worth speculating on (as for one file)
-  constexpr uint64_t INDEX_BUDGET = uint64_t(768) << 20;   // bytes of walked records and entries per round
-  std::vector<uint8_t> tail(n_files, 0);                   // 1: this file finishes on the serial walker
-  for (uint32_t i = 0; i < n; i++)
-    if (bf[i].walk && (!spec_ok || (bf[i].hdr.uniform_type != 0 && bf[i].hdr.uniform_type != dtype))) tail[i] = 1;  // the latter: no chunk can pass
-  for (int round = 0; round < 4096; round++) {
-    std::vector<uint32_t> act;
-    std::vector<uint64_t> offs, lens;
-    for (uint32_t i = 0; i < n && i < limit; i++)
-      if (bf[i].walk && !bf[i].done && !tail[i]) {
-        if (bf[i].pos + 4 > bf[i].end) { tail[i] = 1; continue; }
-        act.push_back(i);
-        offs.push_back(bf[i].pos);
-        lens.push_back(4);
-      }
-    if (act.empty()) break;
-    std::vector<uint8_t> h4;
-    if (PcoB200Error e = peek_src(offs, lens, 4, &h4)) return e;
-    std::vector<FileScan> scans;
-    std::vector<uint32_t> scan_file;
-    uint64_t blocks = 0;
-    const uint64_t per_block = uint64_t(FIND_THREADS) * FIND_PER_THREAD;
-    for (size_t k = 0; k < act.size(); k++) {
-      const uint32_t i = act[k];
-      const uint8_t* b = h4.data() + k * 4;
-      if (b[0] != dtype) { tail[i] = 1; continue; }  // the terminator, or a type byte the serial walker reports
-      FileScan s;
-      s.begin = bf[i].pos;
-      s.end = bf[i].end - 3;
-      s.pattern = uint32_t(b[0]) | (uint32_t(b[1]) << 8) | (uint32_t(b[2]) << 16) | (uint32_t(b[3]) << 24);
-      s.block0 = uint32_t(blocks);
-      blocks += (s.end - s.begin + per_block - 1) / per_block;
-      scans.push_back(s);
-      scan_file.push_back(i);
-    }
-    if (scans.empty()) break;
-    if (blocks > 0x7fffffffull) { for (uint32_t i : scan_file) tail[i] = 1; break; }
-    // scratch: count | candidate positions | their files | statuses | chunk ends
-    PCOB_CUDA_TRY(c.spec.reserve(64 + size_t(CAND_CAP) * (8 + 4)));
-    PCOB_CUDA_TRY(c.files_tab.reserve(scans.size() * sizeof(FileScan) + 64));
-    uint32_t* d_count = c.spec.as<uint32_t>();
-    uint64_t* d_cand = reinterpret_cast<uint64_t*>(c.spec.as<uint8_t>() + 64);
-    uint32_t* d_cfile = reinterpret_cast<uint32_t*>(d_cand + CAND_CAP);
-    PCOB_CUDA_TRY(cudaMemcpyAsync(c.files_tab.p, scans.data(), scans.size() * sizeof(FileScan), cudaMemcpyHostToDevice, stream));
-    PCOB_CUDA_TRY(cudaMemsetAsync(d_count, 0, 4, stream));
-    profiler().begin("find_file_starts_kernel", stream);
-    find_file_starts_kernel<<<uint32_t(blocks), FIND_THREADS, 0, stream>>>(d_src, c.files_tab.as<FileScan>(), uint32_t(scans.size()), d_cand, d_cfile, CAND_CAP, d_count);
-    profiler().end(stream);
-    PCOB_CUDA_TRY(cudaGetLastError());
-    uint32_t count = 0;
-    PCOB_CUDA_TRY(readback_small_sync(&count, d_count, 4, stream));
-    if (count > CAND_CAP) { for (uint32_t i : scan_file) tail[i] = 1; break; }
-    std::vector<uint64_t> cpos(count);
-    std::vector<uint32_t> cfile(count);
-    PCOB_CUDA_TRY(cudaMemcpyAsync(cpos.data(), d_cand, size_t(count) * 8, cudaMemcpyDeviceToHost, stream));
-    PCOB_CUDA_TRY(cudaMemcpyAsync(cfile.data(), d_cfile, size_t(count) * 4, cudaMemcpyDeviceToHost, stream));
-    PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
-    std::vector<std::vector<uint64_t>> cand(scans.size());
-    for (uint32_t k = 0; k < count; k++) cand[cfile[k]].push_back(cpos[k]);
-    // the round's walk: every file's candidates (as many as its budget share allows), one CTA each.  FileParams carries one uniform type
-    // and format version per launch, so the records are laid out flavour by flavour and each flavour present is one launch.
-    auto flavour = [&](uint32_t i) { return (bf[i].hdr.uniform_type << 8) | bf[i].hdr.format_major; };
-    std::vector<uint32_t> scan_order(scans.size());
-    for (size_t s = 0; s < scans.size(); s++) scan_order[s] = uint32_t(s);
-    std::stable_sort(scan_order.begin(), scan_order.end(), [&](uint32_t a, uint32_t b) { return flavour(scan_file[a]) < flavour(scan_file[b]); });
-    std::vector<IndexChunk> recs;
-    std::vector<uint32_t> walked;           // scan index of each file walked this round
-    std::vector<size_t> first_rec;          // its first record
-    uint64_t budget = INDEX_BUDGET;
-    const uint64_t chunks_at = (arena_end + 15) & ~uint64_t(15);
-    for (uint32_t s : scan_order) {
-      const uint32_t i = scan_file[s];
-      std::vector<uint64_t>& cs = cand[s];
-      std::sort(cs.begin(), cs.end());
-      if (cs.empty() || cs.size() > FILE_CAND_CAP || cs[0] != bf[i].pos) { tail[i] = 1; continue; }
-      const uint32_t n0 = ((scans[s].pattern >> 8) & 0xffffffu) + 1;
-      const uint64_t stride = (uint64_t(MAX_VARS) * n_batches_of(n0) * sizeof(BatchEntry) + 15) & ~uint64_t(15);
-      uint64_t m = std::min<uint64_t>(cs.size(), std::max<uint64_t>(1, INDEX_BUDGET / (stride + sizeof(IndexChunk))));
-      if (!walked.empty() && m * (stride + sizeof(IndexChunk)) > budget) continue;  // waits for the next round
-      budget -= std::min(budget, m * (stride + sizeof(IndexChunk)));
-      cs.resize(m);
-      walked.push_back(uint32_t(s));
-      first_rec.push_back(recs.size());
-      for (uint64_t k = 0; k < m; k++) {
-        IndexChunk ic;
-        ic.chunk_offset = cs[k];
-        ic.n = n0;
-        ic.n_vars = 0;
-        ic.out_offset = 0;
-        recs.push_back(ic);
-      }
-    }
-    if (recs.empty()) break;
-    const uint32_t mt = uint32_t(recs.size());
-    const uint64_t e_at = lay_out_entries(recs.data(), mt, (chunks_at + uint64_t(mt) * sizeof(IndexChunk) + 15) & ~uint64_t(15));
-    PCOB_CUDA_TRY(c.files_arena.grow_preserve(e_at + 64, arena_end, stream));
-    PCOB_CUDA_TRY(c.spec.reserve(64 + size_t(CAND_CAP) * (8 + 4) + size_t(mt) * (4 + 8) + 64));
-    uint32_t* d_stat = reinterpret_cast<uint32_t*>(c.spec.as<uint8_t>() + 64 + size_t(CAND_CAP) * 12);
-    uint64_t* d_ends = reinterpret_cast<uint64_t*>(c.spec.as<uint8_t>() + 64 + size_t(CAND_CAP) * 12 + ((size_t(mt) * 4 + 15) & ~size_t(15)));
-    PCOB_CUDA_TRY(cudaMemcpyAsync(arena() + chunks_at, recs.data(), size_t(mt) * sizeof(IndexChunk), cudaMemcpyHostToDevice, stream));
-    PCOB_CUDA_TRY(cudaMemsetAsync(d_stat, 0xff, size_t(mt) * 4, stream));
-    PCOB_CUDA_TRY(cudaMemsetAsync(d_ends, 0, size_t(mt) * 8, stream));
-    PCOB_CUDA_TRY(c.misc.reserve(sizeof(WalkResult)));
-    for (size_t w0 = 0; w0 < walked.size();) {  // one launch per flavour: its walked files' records are consecutive
-      const uint32_t fl = flavour(scan_file[walked[w0]]);
-      size_t w1 = w0 + 1;
-      while (w1 < walked.size() && flavour(scan_file[walked[w1]]) == fl) w1++;
-      const size_t r_lo = first_rec[w0], r_hi = w1 < walked.size() ? first_rec[w1] : recs.size();
-      const FileParams fp{d_src, src_len, dtype, fl >> 8, fl & 0xff};
-      profiler().begin("walk_kernel", stream);
-      walk_kernel<SMALL_MAX_SIZE_LOG><<<uint32_t(r_hi - r_lo), WALK_THREADS, sizeof(WalkSmem<SMALL_MAX_SIZE_LOG>), stream>>>(
-          fp, arena(), chunks_at + r_lo * sizeof(IndexChunk), uint32_t(r_hi - r_lo), 0, e_at, 0, 0, ~uint64_t(0), d_stat + r_lo, c.misc.as<WalkResult>(), 0,
-          d_ends + r_lo);
-      profiler().end(stream);
-      PCOB_CUDA_TRY(cudaGetLastError());
-      w0 = w1;
-    }
-    std::vector<uint32_t> st(mt);
-    std::vector<uint64_t> ends(mt);
-    PCOB_CUDA_TRY(cudaMemcpyAsync(st.data(), d_stat, size_t(mt) * 4, cudaMemcpyDeviceToHost, stream));
-    PCOB_CUDA_TRY(cudaMemcpyAsync(ends.data(), d_ends, size_t(mt) * 8, cudaMemcpyDeviceToHost, stream));
-    PCOB_CUDA_TRY(cudaMemcpyAsync(recs.data(), arena() + chunks_at, size_t(mt) * sizeof(IndexChunk), cudaMemcpyDeviceToHost, stream));  // n_vars as walked
-    PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
-    bool progress = false;
-    for (size_t w = 0; w < walked.size(); w++) {
-      const uint32_t s = walked[w], i = scan_file[s];
-      BatchFile& f = bf[i];
-      const size_t r0 = first_rec[w];
-      const uint32_t m = uint32_t(cand[s].size());
-      const uint32_t n0 = recs[r0].n;
-      uint64_t p = f.pos;
-      const std::vector<uint32_t> chain = follow_chunk_chain(cand[s].data(), st.data() + r0, ends.data() + r0, m, f.pos, n0, 0, ~uint64_t(0), f.end, &p);
-      if (chain.empty()) { tail[i] = 1; continue; }
-      for (uint32_t k : chain) {
-        IndexChunk ic = recs[r0 + k];
-        ic.out_offset = f.count;
-        f.count += n0;
-        f.recs.push_back(ic);
-      }
-      f.pos = p;
-      progress = true;
-    }
-    arena_end = e_at;
-    if (!progress) break;
-  }
-
-  // ---- 3. the terminator, or the serial walker
+  // ---- 2. index-free files, walked together; a cold one goes to the catch-all decoder, as in decompress_ex
   {
-    std::vector<uint32_t> ends_at;
-    std::vector<uint64_t> offs, lens;
+    std::vector<WalkFile*> walks;
     for (uint32_t i = 0; i < n && i < limit; i++)
-      if (bf[i].walk && bf[i].pos < bf[i].end) {
-        ends_at.push_back(i);
-        offs.push_back(bf[i].pos);
-        lens.push_back(1);
-      }
-    std::vector<uint8_t> b;
-    if (PcoB200Error e = peek_src(offs, lens, 4, &b)) return e;
-    for (size_t k = 0; k < ends_at.size(); k++)
-      if (b[k * 4] == 0) bf[ends_at[k]].done = true;
-  }
-  PCOB_CUDA_TRY(c.misc.reserve(sizeof(WalkResult)));
-  for (uint32_t i = 0; i < n && i < limit; i++) {
-    BatchFile& f = bf[i];
-    if (!f.walk || f.done) continue;
-    const FileParams fpf{d_src + f.begin, f.end - f.begin, dtype, f.hdr.uniform_type, f.hdr.format_major};
-    const uint64_t len = f.end - f.begin;
-    const uint32_t max_chunks = uint32_t(std::min<uint64_t>(len / 5 + 2, 1u << 16));
-    uint64_t next = f.pos - f.begin;
-    for (;;) {
-      const uint64_t chunks_at = (arena_end + 15) & ~uint64_t(15);
-      const uint64_t entries_begin = chunks_at + uint64_t(max_chunks) * sizeof(IndexChunk);
-      uint64_t want_batches = (f.hdr.n_hint > f.count ? (f.hdr.n_hint - f.count) / BATCH_N : 0) + 2ull * max_chunks + 2;
-      want_batches = std::min<uint64_t>(want_batches, uint64_t(1) << 23);
-      const uint64_t entries_end = entries_begin + want_batches * MAX_VARS * sizeof(BatchEntry) + 16ull * max_chunks + 64;
-      PCOB_CUDA_TRY(c.files_arena.grow_preserve(entries_end + 64, arena_end, stream));
-      profiler().begin("walk_kernel", stream);
-      walk_kernel<12><<<1, WALK_THREADS, sizeof(WalkSmem<12>), stream>>>(fpf, arena(), chunks_at, max_chunks, entries_begin, entries_end, next, f.count, ~uint64_t(0),
-                                                                        nullptr, c.misc.as<WalkResult>(), 1);
-      profiler().end(stream);
-      PCOB_CUDA_TRY(cudaGetLastError());
-      WalkResult res;
-      PCOB_CUDA_TRY(readback_small_sync(&res, c.misc.p, sizeof(res), stream));
-      if (res.n_chunks > 0) {
-        std::vector<IndexChunk> got(res.n_chunks);
-        PCOB_CUDA_TRY(cudaMemcpyAsync(got.data(), arena() + chunks_at, got.size() * sizeof(IndexChunk), cudaMemcpyDeviceToHost, stream));
-        PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
-        for (IndexChunk& ic : got) {
-          ic.chunk_offset += f.begin;
-          f.recs.push_back(ic);
-        }
-        arena_end = std::max<uint64_t>(res.entries_end, entries_begin);
-      }
-      f.count += res.n_total;
-      next = res.next_byte;
-      if (res.status == ST_TERMINATOR) { f.done = true; break; }
-      if (res.status == ST_INDEX_FULL && res.n_chunks > 0) continue;
-      // a chunk the fast kernels decline (or one beyond the index scratch): the whole file goes to the catch-all decoder, as in
-      // decompress_ex
-      if ((res.status == ST_UNSUPPORTED || res.status == ST_INDEX_FULL) && cold_ok) { f.cold = true; f.staged = true; break; }
-      const PcoB200Error k = res.status == ST_INDEX_FULL ? fail(PCO_B200_UNSUPPORTED, "a single chunk exceeds the device index scratch")
-                                                         : status_to_error(res.status, ("chunk " + std::to_string(res.n_chunks) + " of this walk round").c_str());
-      fail_at(i, k, last_error_ref());
-      break;
+      if (bf[i].walk) walks.push_back(&bf[i]);
+    if (PcoB200Error e = walk_index_free(c, static_cast<const uint8_t*>(src), src_dev, d_src, src_len, dtype, walks, c.files_arena, &arena_end, stream)) return e;
+    for (uint32_t i = 0; i < n && i < limit; i++) {
+      BatchFile& f = bf[i];
+      if (!f.walk || f.how == WalkEnd::TERMINATED) continue;
+      if (f.how == WalkEnd::COLD && cold_ok) f.cold = f.staged = true;
+      else fail_at(i, f.err, f.msg);
     }
   }
 
@@ -2069,7 +1999,7 @@ static PcoB200Error decompress_files_impl(const void* src, size_t src_len, const
   if (PcoB200Error e = out_buffer(c, dst, dst_dev, total * elem, &d_out)) return e;
   const uint64_t out_len = dst_dev ? uint64_t(dst_len) : total;
 
-  // ---- 4. one chunk list for the fast kernels, grouped by (uniform type, format major)
+  // ---- 3. one chunk list for the fast kernels, grouped by (uniform type, format major)
   std::map<uint32_t, std::vector<uint32_t>> flavours;
   for (uint32_t i = 0; i < n && i < limit; i++)
     if (!bf[i].cold && !bf[i].staged && (bf[i].indexed ? bf[i].n_idx_chunks : bf[i].recs.size()) > 0) flavours[(bf[i].hdr.uniform_type << 8) | bf[i].hdr.format_major].push_back(i);
@@ -2142,7 +2072,7 @@ static PcoB200Error decompress_files_impl(const void* src, size_t src_len, const
     }
   }
 
-  // ---- 5. staged numbers moved into their slot; cold files found by the merged decode (an older format, whose chunk metas the check
+  // ---- 4. staged numbers moved into their slot; cold files found by the merged decode (an older format, whose chunk metas the check
   // does not parse) through the catch-all decoder into their slot, sized by their index's count
   for (uint32_t i = 0; i < n && i < limit; i++) {
     BatchFile& f = bf[i];

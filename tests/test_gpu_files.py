@@ -365,7 +365,8 @@ def _walk_launches(fn):
 
 
 def test_walk_bound():
-    """300 index-free files of 3 chunks each launch walk_kernel no more often than decompress_ex does on one of them."""
+    """300 index-free files of 3 chunks each launch walk_kernel no more often than decompress_ex does on one of them, which launches it
+    at most twice: the speculative round, and the serial walker if the round does not end at the terminator."""
     from pcodec_b200 import ChunkConfig, DeltaSpec, ModeSpec, PagingSpec
 
     sa = _sa()
@@ -379,7 +380,7 @@ def test_walk_bound():
     got = {}
     batch = _walk_launches(lambda: got.update(v=sa.decompress_files(data, files, np.uint64)[0]))
     np.testing.assert_array_equal(got["v"], x)
-    assert 0 < batch <= single, (batch, single)
+    assert 0 < batch <= single <= 2, (batch, single)
 
 
 @pytest.mark.parametrize("name", ["v0_0_0_classic", "v0_1_0_delta_int_mult", "v0_3_0_f16", "v0_4_5_uniform_type", "v1_0_0_u8"])

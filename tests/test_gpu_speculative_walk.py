@@ -1,8 +1,9 @@
 """Index-free decompress (what pco_standalone_simple_decompress_into receives: no side index, no chunk offsets) finds runs of
 same-sized chunks by their first 4 bytes, walks every candidate in parallel and follows the chain of verified (start, end) pairs
-(host_api.cu speculative_walk_rounds, decode_kernels.cuh find_chunk_starts_kernel).  The numbers must be the oracle's whatever the
-candidates look like: coincidences inside chunk bodies, chunks of changing sizes, short last chunks, short destinations, corrupt and
-truncated files (reference semantics: pco/src/standalone/simple.rs:100-143, decompressor.rs:150-215)."""
+(host_api.cu walk_index_free and speculative_walk_rounds, the walker pco_b200_decompress_files shares; files_kernels.cuh
+find_file_starts_kernel).  The numbers must be the oracle's whatever the candidates look like: coincidences inside chunk bodies, chunks
+of changing sizes, short last chunks, short destinations, corrupt and truncated files (reference semantics:
+pco/src/standalone/simple.rs:100-143, decompressor.rs:150-215)."""
 import ctypes as C
 
 import numpy as np
@@ -143,6 +144,35 @@ def test_corrupt_and_truncated_files_fail_like_the_serial_walk():
     with pytest.raises(PcoError) as e:
         standalone.simple_decompress(data[: starts[6]], np.uint64)
     assert e.value.kind == "InsufficientData"
+
+
+@pytest.mark.parametrize("speculative", [None, "0"])
+def test_chunks_before_a_failing_chunk_reach_a_device_destination(monkeypatch, speculative):
+    """The call fails at a corrupt chunk, and a device destination holds the numbers of the chunks in front of it, as the reference's
+    decoder emits them - with the speculative rounds and with the serial walk alone."""
+    if speculative is None:
+        monkeypatch.delenv("PCOB200_SPECULATIVE_WALK", raising=False)
+    else:
+        monkeypatch.setenv("PCOB200_SPECULATIVE_WALK", speculative)
+    rng = np.random.default_rng(7)
+    page_n = 2048
+    n = 9 * page_n
+    x = np.cumsum(rng.geometric(0.01, size=n)).astype(np.uint64)
+    data = oracle.simple_compress(x, oracle.make_config(mode=oracle.MODE_CLASSIC, delta=oracle.DELTA_CONSECUTIVE, delta_order=1, max_page_n=page_n))
+    starts = [c["chunk_start"] for c in oracle.inspect(data, np.uint64)["chunks"]]
+    bad = bytearray(data)
+    bad[starts[4]] = 0x37
+    L = _lib.lib()
+    dev = torch.device("cuda")
+    d_src = torch.from_numpy(np.frombuffer(bytes(bad), dtype=np.uint8).copy()).to(dev)
+    d_out = torch.zeros(n, dtype=torch.int64, device=dev)
+    prog = _lib._CProgress()
+    rc = L.pco_b200_decompress_ex(C.c_void_p(d_src.data_ptr()), C.c_size_t(d_src.numel()), C.c_ubyte(2), C.c_void_p(d_out.data_ptr()), C.c_size_t(n), C.byref(prog),
+                                  None, C.c_size_t(0), C.c_uint32(3), None)
+    with pytest.raises(PcoError) as e:
+        _lib.check(rc)
+    assert e.value.kind in ("Corruption", "InvalidType", "InvalidArgument")
+    assert np.array_equal(d_out.cpu().numpy().view(np.uint64)[: 4 * page_n], x[: 4 * page_n])
 
 
 def test_many_chunks_in_one_call():
