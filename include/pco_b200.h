@@ -458,6 +458,81 @@ PcoB200Error pco_b200_compress_async(const PcoB200AsyncCompressPlan *plan, const
  * sets the last-error message; when the kind is OK, fills *n_written and *index_len (either may be NULL). */
 PcoB200Error pco_b200_compress_async_result(const PcoB200AsyncCompressStatus *host_status, size_t *n_written, size_t *index_len);
 
+/* ---- asynchronous ranges of an indexed standalone file (no reference counterpart): pco_b200_decompress_ranges with the ranges, their
+ * count and every buffer in device memory.  Positions a kernel produced (a sampler's row ids, a batch of embedding keys, a page cache's
+ * misses) are decoded behind the step that produced them, with no copy to the host: the call only enqueues kernels on the caller's
+ * stream and returns at once.  It makes no synchronising, allocating or host-to-device copy call and refers to no memory of the
+ * library's per-thread scratch, so it can be captured in a CUDA graph, and a captured call may be replayed after
+ * pco_b200_thread_release or after any other call.  The pieces of the ranges are planned on the device: a plan made once outside any
+ * capture fixes the grids from its capacities, and the number of ranges is read from device memory, so one captured graph serves a
+ * different count, a different set of ranges and a different file (same number type and header flavour) on each replay. */
+typedef struct PcoB200AsyncRangesPlan {  /* filled by pco_b200_decompress_ranges_async_plan; treat as opaque */
+  uint32_t dtype, uniform_type, format_major, reserved;
+  uint64_t src_cap, index_cap, max_chunks, max_ranges, dst_cap, window_cap;
+  uint64_t workspace_bytes;              /* device workspace one in-flight call needs */
+} PcoB200AsyncRangesPlan;
+
+typedef struct PcoB200AsyncRangesStatus {  /* written on the device by every call */
+  uint32_t kind;                           /* PcoB200Error */
+  uint32_t device_status;                  /* the device word behind it: a chunk's PcoB200Error kind, or PCO_B200_ASYNC_* */
+  uint64_t range;                          /* the range the failure is named by (UINT64_MAX if none) */
+  uint64_t chunk;                          /* the failing chunk, or the chunk that breaks the tiling (UINT64_MAX if none) */
+  uint64_t n_written;                      /* the sum of the counts, once the ranges passed their checks (0 before) */
+  uint64_t window_needed;                  /* the window the ranges need (the rule below), also when above window_cap; 0 when refused earlier */
+} PcoB200AsyncRangesStatus;
+
+/* device_status of a call refused before any decoding, beyond the PCO_B200_ASYNC_* codes of pco_b200_decompress_async */
+enum {
+  PCO_B200_ASYNC_INDEX_TILING = 0x107,    /* chunk `chunk` does not start where the chunks before it end, or holds no numbers (INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_INDEX_TOTAL = 0x108,     /* the chunk records tile, but not up to the index header's n_total (INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_TOO_MANY_RANGES = 0x109, /* *n_ranges is above the plan's max_ranges (INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_RANGE_PAST = 0x10a,      /* range `range` lies past the file's numbers (INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_RANGE_OVERFLOW = 0x10b,  /* the counts up to range `range` add up to more than 2^64 numbers (INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_DST_SHORT = 0x10c,       /* the sum of the counts (n_written) is above dst_cap (INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_WINDOW = 0x10d           /* window_needed is above the plan's window_cap (PCO_B200_IO) */
+};
+
+/* Makes a plan.  `head`, dtype, src_cap, index_cap, max_chunks and dst_cap are those of pco_b200_decompress_async_plan (dst_cap: numbers
+ * of dst); max_ranges bounds *n_ranges of every call, window_cap the window a call may need (numbers).  Checked before the device is
+ * touched, with the kinds of pco_b200_decompress_async_plan: dtype, the header, the uniform type, max_chunks in 1 .. 2^32 - 1, max_ranges
+ * in 1 .. 2^32 - 1, dst_cap and window_cap at most 2^56 (PCO_B200_INVALID_ARGUMENT).  Then *plan is filled and the one-time device set-up
+ * runs on the current device, which the calls must use; without a device that is PCO_B200_CUDA.
+ * Window rule: a chunk touched by the ranges needs a window of (the chunk-relative end of the last number wanted of it, rounded up to
+ * 256) numbers, and window_needed is the sum of the windows of the touched chunks.  It holds the staged windows of chunks several pieces
+ * share, the catch-all decoder's output and the two-var decode's scratch rows, whichever route a chunk takes.  Whole-chunk ranges over a
+ * file of chunks of 2^18 numbers need about the numbers they cover; a point lookup needs up to a chunk's length.
+ * workspace_bytes is the sum of these regions, each rounded up to 256 bytes: 1880 (the check and the binomial table), 48 (state),
+ * 32 max_chunks (chunk table), 32 max_chunks (marks), 24 ceil(max_chunks / 256) and 32 ceil(max_ranges / 256) (CTA sums),
+ * 8 max_ranges (destination offsets), 8 max_ranges (chunk
+ * spans), 32 max_chunks (task records), 24 max_chunks (windows), 24 max_chunks (routes and slots), 4 max_chunks (statuses), max_chunks
+ * (classes), 2 floor(window_cap / 256) rows of 256 bytes and of 4 bytes (scratch rows), window_cap numbers (slots), and the catch-all
+ * decoder's 3.7 MB (the last two as in pco_b200_decompress_async_plan). */
+PcoB200Error pco_b200_decompress_ranges_async_plan(const void *head, size_t head_len, unsigned char dtype, size_t src_cap,
+                                                   size_t index_cap, size_t max_chunks, size_t max_ranges, size_t dst_cap,
+                                                   size_t window_cap, PcoB200AsyncRangesPlan *plan);
+/* Enqueues the decode of ranges[0 : *n_ranges) of the file in `src` through its side index `index` into dst on `cuda_stream`, and the
+ * outcome into *status; returns without waiting.  src (src_cap bytes), index (index_cap bytes), ranges (PcoB200Range[max_ranges]),
+ * n_ranges (one uint64_t), dst (dst_cap numbers), workspace (plan->workspace_bytes, 256-byte aligned) and status are device pointers;
+ * one workspace serves one call in flight.  For a valid file, dst[0 : total) equals what pco_b200_decompress_ranges writes for the same
+ * file, index and ranges: range i lands right behind range i - 1, and ranges may overlap, repeat, come in any order, have count 0 and
+ * span any number of chunks.  Refusals, in this order, with the kind pco_b200_decompress_ranges gives where it has one: *n_ranges above
+ * max_ranges; the header and index check of pco_b200_decompress_async (file length at most src_cap, at most max_chunks chunks); chunk
+ * records that do not tile the numbers in order; a range past the file or where the counts overflow (the lowest such range); a sum of
+ * the counts above dst_cap; window_needed above window_cap (PCO_B200_IO).  Every refusal is decided before any write to dst.  A chunk
+ * that fails gives the kind pco_b200_decompress_ranges gives, named by the lowest-index range with numbers in it, and nothing is written
+ * outside dst[0 : total).  Reads stay inside the capacities.  Chunks the fast kernels decline are decoded by the catch-all decoder from
+ * the chunk's start to the last number wanted; a Lookback window beyond 2^16 numbers is PCO_B200_UNSUPPORTED here.  The return value
+ * covers the host side only: null pointers, an unaligned workspace or a plan that was not filled (PCO_B200_INVALID_ARGUMENT), a launch
+ * the runtime refuses (PCO_B200_CUDA).  With pco_b200_profile_enable(1), a call outside a stream capture records its kernel spans for
+ * pco_b200_profile_last; a call inside a capture records none. */
+PcoB200Error pco_b200_decompress_ranges_async(const PcoB200AsyncRangesPlan *plan, const void *src, const void *index,
+                                              const PcoB200Range *ranges, const uint64_t *n_ranges, void *dst, void *workspace,
+                                              PcoB200AsyncRangesStatus *status, void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory at a point of the caller's choosing.  Returns the kind,
+ * sets the last-error message as pco_b200_decompress_ranges words it ("range 17: corrupt data in chunk 3") and, when the kind is OK,
+ * sets *n_written (may be NULL) to the sum of the counts. */
+PcoB200Error pco_b200_decompress_ranges_async_result(const PcoB200AsyncRangesStatus *host_status, size_t *n_written);
+
 #if defined(__cplusplus)
 }
 #endif

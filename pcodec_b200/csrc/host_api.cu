@@ -5,6 +5,7 @@
 
 #include "async_compress.cuh"
 #include "async_kernels.cuh"
+#include "async_ranges_kernels.cuh"
 #include "compress_host.cuh"
 #include "decode_kernels.cuh"
 #include "decode_fused.cuh"
@@ -2562,6 +2563,205 @@ PcoB200Error pco_b200_decompress_async_result(const PcoB200AsyncStatus* s, PcoB2
     default:
       status_to_error(s->device_status, "this chunk");
       return fail(kind, "chunk " + std::to_string(s->chunk) + ": " + last_error_ref());
+  }
+}
+
+// ---- asynchronous ranges of an indexed standalone file (pco_b200_decompress_ranges_async; kernels in async_ranges_kernels.cuh)
+// The plan fixes every grid size (from max_chunks and max_ranges) and the byte layout of the workspace; the file's length, chunk count and
+// n_total come from its side index, and the number of ranges from *n_ranges, on the device.  A call is a fixed sequence of fifteen
+// launches: check, chunks, count, scan, mark, window, gate, tasks, fused, symwalk, decode<1>, decode<2>, cold, gather, finish.
+
+static bool ar_plan_ok(const PcoB200AsyncRangesPlan* p) {
+  return nt_valid(p->dtype) && p->max_chunks >= 1 && p->max_chunks <= 0xffffffffull && p->max_ranges >= 1 && p->max_ranges <= 0xffffffffull &&
+         p->dst_cap <= (uint64_t(1) << 56) && p->window_cap <= (uint64_t(1) << 56) &&
+         p->workspace_bytes == ar_layout(p->max_chunks, p->max_ranges, p->window_cap, nt_bits(p->dtype) / 8).total;
+}
+
+PcoB200Error pco_b200_decompress_ranges_async_plan(const void* head, size_t head_len, unsigned char dtype, size_t src_cap, size_t index_cap,
+                                                   size_t max_chunks, size_t max_ranges, size_t dst_cap, size_t window_cap, PcoB200AsyncRangesPlan* plan) {
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (!plan || (!head && head_len)) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  StandaloneHeader hdr;
+  if (PcoB200Error e = parse_standalone_header(static_cast<const uint8_t*>(head), std::min<size_t>(head_len, 32), head_len, &hdr)) return e;
+  if (hdr.uniform_type != 0 && hdr.uniform_type != dtype)
+    return fail(PCO_B200_INVALID_ARGUMENT, "the header's uniform type " + std::to_string(hdr.uniform_type) + " is not dtype " + std::to_string(dtype));
+  if (max_chunks == 0 || uint64_t(max_chunks) > 0xffffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_chunks must be 1 .. 2^32 - 1");
+  if (max_ranges == 0 || uint64_t(max_ranges) > 0xffffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_ranges must be 1 .. 2^32 - 1");
+  if (uint64_t(dst_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "dst_cap above 2^56 numbers");
+  if (uint64_t(window_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "window_cap above 2^56 numbers");
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->uniform_type = hdr.uniform_type;
+  plan->format_major = hdr.format_major;
+  plan->src_cap = src_cap;
+  plan->index_cap = index_cap;
+  plan->max_chunks = max_chunks;
+  plan->max_ranges = max_ranges;
+  plan->dst_cap = dst_cap;
+  plan->window_cap = window_cap;
+  plan->workspace_bytes = ar_layout(max_chunks, max_ranges, window_cap, nt_bits(dtype) / 8).total;
+  // the one-time device set-up, as in pco_b200_decompress_async_plan: the window-mode decode kernels' attributes, and every kernel the
+  // call launches loaded now
+  Context& c = ctx();
+  if (PcoB200Error e = ensure_device(c)) return e;
+  if (PcoB200Error e = set_decode_attrs<true>(c)) return e;
+  cudaFuncAttributes fa;
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, async_check_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_chunks_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_count_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_scan_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_mark_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_window_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_gate_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_tasks_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, symwalk_kernel<true>));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_gather_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_finish_kernel));
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
+    using L = decltype(tag);
+    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, fused_narrow_kernel<L, true>));
+    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, decode_kernel<L, 1, true>));
+    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, decode_kernel<L, 2, true>));
+    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_cold_kernel<L>));
+    return PCO_B200_OK;
+  });
+}
+
+PcoB200Error pco_b200_decompress_ranges_async(const PcoB200AsyncRangesPlan* plan, const void* src, const void* index, const PcoB200Range* ranges,
+                                              const uint64_t* n_ranges, void* dst, void* workspace, PcoB200AsyncRangesStatus* status, void* cuda_stream) {
+  if (!plan || !src || !index || !ranges || !n_ranges || !workspace || !status || (!dst && plan->dst_cap))
+    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (!ar_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_decompress_ranges_async_plan");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  PCOB_CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
+  const bool prof = cap == cudaStreamCaptureStatusNone && profiler_enabled().load(std::memory_order_relaxed);
+  if (prof) profiler().discard();
+  auto begin = [&](const char* name) { if (prof) profiler().begin(name, stream); };
+  auto end = [&]() { if (prof) profiler().end(stream); };
+
+  const uint32_t mc = uint32_t(plan->max_chunks), mr = uint32_t(plan->max_ranges), elem = nt_bits(plan->dtype) / 8;
+  const ArLayout lay = ar_layout(mc, mr, plan->window_cap, elem);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  AsyncCheck* chk = reinterpret_cast<AsyncCheck*>(ws);
+  ArState* state = reinterpret_cast<ArState*>(ws + lay.state);
+  IndexChunk* table = reinterpret_cast<IndexChunk*>(ws + lay.table);
+  ArMark* marks = reinterpret_cast<ArMark*>(ws + lay.marks);
+  ArChunkPart* cparts = reinterpret_cast<ArChunkPart*>(ws + lay.cparts);
+  ArRangePart* rparts = reinterpret_cast<ArRangePart*>(ws + lay.rparts);
+  uint64_t* roff = reinterpret_cast<uint64_t*>(ws + lay.roff);
+  uint2* rspan = reinterpret_cast<uint2*>(ws + lay.rspan);
+  IndexChunk* tasks = reinterpret_cast<IndexChunk*>(ws + lay.tasks);
+  WinTask* wins = reinterpret_cast<WinTask*>(ws + lay.wins);
+  ArTask* tinfo = reinterpret_cast<ArTask*>(ws + lay.tinfo);
+  uint32_t* d_st = reinterpret_cast<uint32_t*>(ws + lay.st);
+  uint8_t* d_cls = ws + lay.cls;
+  uint8_t* d_syms = ws + lay.syms;
+  uint32_t* d_offs = reinterpret_cast<uint32_t*>(ws + lay.offs);
+  uint8_t* d_stage = ws + lay.stage;
+  uint8_t* d_cold = ws + lay.cold;
+  const uint8_t* d_idx = static_cast<const uint8_t*>(index);
+  ArArgs g;
+  g.a.fp = FileParams{src, plan->src_cap, plan->dtype, plan->uniform_type, plan->format_major};
+  g.a.index = d_idx;
+  g.a.index_cap = plan->index_cap;
+  g.a.dst_cap = plan->dst_cap;
+  g.a.max_chunks = mc;
+  g.ranges = ranges;
+  g.n_ranges = n_ranges;
+  g.window_cap = plan->window_cap;
+  g.max_ranges = mr;
+  g.elem = elem;
+  const uint32_t cb = uint32_t(ar_ctas(mc)), rb = uint32_t(ar_ctas(mr));
+
+  begin("async_check_kernel");
+  async_check_kernel<<<(mc + ASYNC_CHECK_RECS - 1) / ASYNC_CHECK_RECS, ASYNC_THREADS, 0, stream>>>(g.a, chk, table);
+  end();
+  begin("ar_chunks_kernel");
+  ar_chunks_kernel<<<cb, AR_THREADS, 0, stream>>>(chk, table, marks, cparts);
+  end();
+  begin("ar_count_kernel");
+  ar_count_kernel<<<rb, AR_THREADS, 0, stream>>>(g, chk, rparts);
+  end();
+  begin("ar_scan_kernel");
+  ar_scan_kernel<<<1, AR_SCAN_THREADS, 0, stream>>>(g, chk, cparts, rparts, state);
+  end();
+  begin("ar_mark_kernel");
+  ar_mark_kernel<<<rb, AR_THREADS, 0, stream>>>(g, chk, table, rparts, state, marks, roff, rspan);
+  end();
+  begin("ar_window_kernel");
+  ar_window_kernel<<<cb, AR_THREADS, 0, stream>>>(chk, state, marks, cparts);
+  end();
+  begin("ar_gate_kernel");
+  ar_gate_kernel<<<1, AR_SCAN_THREADS, 0, stream>>>(g, cparts, state);
+  end();
+  begin("ar_tasks_kernel");
+  ar_tasks_kernel<<<cb, AR_THREADS, 0, stream>>>(g, chk, state, table, marks, cparts, tasks, wins, tinfo, static_cast<uint8_t*>(dst), d_stage);
+  end();
+  begin("fused_narrow_kernel");
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    fused_narrow_kernel<L, true><<<mc, FZ_THREADS, sizeof(FusedSmem), stream>>>(g.a.fp, tasks, d_idx, g.a.index_cap, d_st, d_cls, nullptr, 0, wins);
+    return 0;
+  });
+  end();
+  begin("symwalk_kernel");
+  symwalk_kernel<true><<<mc, SW_THREADS, sizeof(SymWalkSmem), stream>>>(g.a.fp, tasks, d_idx, g.a.index_cap, 0, d_syms, d_offs, d_cls, wins);
+  end();
+  begin("decode_kernel");
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    decode_kernel<L, 1, true><<<mc, DEC_THREADS, sizeof(DecodeSmem), stream>>>(g.a.fp, tasks, d_st, d_idx, g.a.index_cap, nullptr, 0, &chk->binoms, d_syms,
+                                                                                d_offs, d_cls, wins);
+    decode_kernel<L, 2, true><<<mc, DEC_THREADS, sizeof(DecodeSmem), stream>>>(g.a.fp, tasks, d_st, d_idx, g.a.index_cap, nullptr, 0, &chk->binoms, d_syms,
+                                                                                d_offs, d_cls, wins);
+    return 0;
+  });
+  end();
+  begin("ar_cold_kernel");
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    ar_cold_kernel<L><<<1, AR_THREADS, 0, stream>>>(g.a.fp, state, tasks, wins, tinfo, d_st, reinterpret_cast<L*>(d_stage), d_cold);
+    return 0;
+  });
+  end();
+  begin("ar_gather_kernel");
+  ar_gather_kernel<<<std::min(mr, AR_GATHER_MAX_CTAS), AR_THREADS, 0, stream>>>(g, state, table, marks, wins, tinfo, d_st, roff, rspan,
+                                                                                  static_cast<uint8_t*>(dst), d_stage);
+  end();
+  begin("ar_finish_kernel");
+  ar_finish_kernel<<<1, AR_SCAN_THREADS, 0, stream>>>(state, tinfo, d_st, status);
+  end();
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
+}
+
+PcoB200Error pco_b200_decompress_ranges_async_result(const PcoB200AsyncRangesStatus* s, size_t* n_written) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200Error kind = s->kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(s->kind) : PCO_B200_CORRUPTION;
+  if (kind == PCO_B200_OK) {
+    if (n_written) *n_written = size_t(s->n_written);
+    return PCO_B200_OK;
+  }
+  switch (s->device_status) {
+    case PCO_B200_ASYNC_HEADER_CORRUPT: return fail(kind, "corrupt standalone header (magic, version, type byte or size hint)");
+    case PCO_B200_ASYNC_HEADER_SHORT: return fail(kind, "insufficient data: the file ends inside its standalone header");
+    case PCO_B200_ASYNC_HEADER_MISMATCH: return fail(kind, "the file's uniform type or format version differs from the plan's");
+    case PCO_B200_ASYNC_INDEX_FOREIGN: return fail(kind, "side index does not belong to this file (or its file length exceeds src_cap)");
+    case PCO_B200_ASYNC_TOO_MANY_CHUNKS: return fail(kind, "the side index lists more chunks than the plan's max_chunks");
+    case PCO_B200_ASYNC_INDEX_TILING:
+      return fail(kind, "side index: chunk " + std::to_string(s->chunk) + " does not start where the chunks before it end");
+    case PCO_B200_ASYNC_INDEX_TOTAL: return fail(kind, "side index: its chunks do not hold the number of numbers its header states");
+    case PCO_B200_ASYNC_TOO_MANY_RANGES: return fail(kind, "*n_ranges is above the plan's max_ranges");
+    case PCO_B200_ASYNC_RANGE_PAST: return range_fail(kind, s->range, "start + count lies past the file's numbers");
+    case PCO_B200_ASYNC_RANGE_OVERFLOW: return range_fail(kind, s->range, "the counts add up to more than 2^64 numbers");
+    case PCO_B200_ASYNC_DST_SHORT: return fail(kind, "dst_cap is below the ranges' " + std::to_string(s->n_written) + " numbers");
+    case PCO_B200_ASYNC_WINDOW:
+      return fail(kind, "the ranges need a window of " + std::to_string(s->window_needed) + " numbers, more than the plan's window_cap");
+    default:
+      status_to_error(s->device_status, ("chunk " + std::to_string(s->chunk)).c_str());
+      return range_fail(kind, s->range, last_error_ref());
   }
 }
 

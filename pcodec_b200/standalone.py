@@ -470,6 +470,103 @@ class AsyncDecompressor:
         return Progress(prog.n_processed, bool(prog.finished))
 
 
+class _CAsyncRangesPlan(C.Structure):  # PcoB200AsyncRangesPlan (include/pco_b200.h)
+    _fields_ = [("dtype", C.c_uint32), ("uniform_type", C.c_uint32), ("format_major", C.c_uint32), ("reserved", C.c_uint32),
+                ("src_cap", C.c_uint64), ("index_cap", C.c_uint64), ("max_chunks", C.c_uint64), ("max_ranges", C.c_uint64),
+                ("dst_cap", C.c_uint64), ("window_cap", C.c_uint64), ("workspace_bytes", C.c_uint64)]
+
+
+class _CAsyncRangesStatus(C.Structure):  # PcoB200AsyncRangesStatus (include/pco_b200.h)
+    _fields_ = [("kind", C.c_uint32), ("device_status", C.c_uint32), ("range", C.c_uint64), ("chunk", C.c_uint64), ("n_written", C.c_uint64),
+                ("window_needed", C.c_uint64)]
+
+
+def _lib_async_ranges():
+    L = _lib.lib()
+    if not getattr(L, "_async_ranges_ready", False):
+        L.pco_b200_decompress_ranges_async_plan.argtypes = [C.c_void_p, C.c_size_t, C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                                            C.c_size_t, C.c_size_t, C.c_void_p]
+        L.pco_b200_decompress_ranges_async.argtypes = [C.c_void_p] * 9
+        L.pco_b200_decompress_ranges_async_result.argtypes = [C.c_void_p, C.POINTER(C.c_size_t)]
+        L._async_ranges_ready = True
+    return L
+
+
+class AsyncRangeDecompressor:
+    """Decodes ranges of indexed standalone files on the current CUDA stream with the ranges in device memory and without waiting for the
+    device (pco_b200_decompress_ranges_async): positions a kernel produced need no trip to the host, and a call can be captured in a
+    torch.cuda.CUDAGraph.
+
+    The plan comes from `head`, the first bytes of a file (as AsyncDecompressor).  src_cap, index_cap (bytes) and dst_cap (numbers) are the
+    sizes of the buffers every call passes, max_chunks the most chunks a file may have, max_ranges the most ranges of a call, and
+    window_cap the most window numbers a call may need (include/pco_b200.h: the sum over touched chunks of the end of the last number
+    wanted, rounded up to 256).  The number of ranges is read from a device tensor, so one captured call serves a different count, different
+    ranges and a different file on each replay.  The decompressor owns a device workspace and a status; it serves one call in flight."""
+
+    def __init__(self, head, dtype, src_cap, index_cap, max_chunks, max_ranges, dst_cap, window_cap, device=None):
+        import torch
+
+        from .wrapped import _host_u8
+
+        self.dtype = np.dtype(dtype)
+        if _is_cuda(head):
+            head = head.reshape(-1)[:32].cpu().numpy()
+        h = _host_u8(head)[:32].copy()
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        L = _lib_async_ranges()
+        self._plan = _CAsyncRangesPlan()
+        with torch.cuda.device(self.device):
+            rc = L.pco_b200_decompress_ranges_async_plan(h.ctypes.data_as(C.c_void_p), C.c_size_t(h.size), C.c_ubyte(_lib.dtype_byte(self.dtype)),
+                                                         C.c_size_t(src_cap), C.c_size_t(index_cap), C.c_size_t(max_chunks), C.c_size_t(max_ranges),
+                                                         C.c_size_t(dst_cap), C.c_size_t(window_cap), C.byref(self._plan))
+        _lib.check(rc)
+        self.workspace = torch.empty(self._plan.workspace_bytes, dtype=torch.uint8, device=self.device)
+        self.status = torch.zeros(C.sizeof(_CAsyncRangesStatus), dtype=torch.uint8, device=self.device)
+
+    @property
+    def workspace_bytes(self):
+        return int(self._plan.workspace_bytes)
+
+    def __call__(self, src, index, ranges, n_ranges, dst):
+        """Enqueues the decode of ranges[: n_ranges[0]] of the file in `src` (uint8 CUDA tensor of at least src_cap bytes) through its side
+        index `index` (at least index_cap bytes) into `dst` (a CUDA tensor of the plan's dtype, at least dst_cap numbers) on
+        torch.cuda.current_stream().  `ranges` is an int64 CUDA tensor of shape (max_ranges, 2) of (start, count), `n_ranges` a 1-element
+        int64 CUDA tensor.  Returns nothing and does not wait; result() reports the outcome."""
+        import torch
+
+        from .wrapped import _torch_dtypes
+
+        p = self._plan
+        for name, t in (("src", src), ("index", index), ("ranges", ranges), ("n_ranges", n_ranges), ("dst", dst)):
+            if not _is_cuda(t) or t.device != self.device or not t.is_contiguous():
+                raise ValueError(f"{name} must be a contiguous CUDA tensor on {self.device}")
+        if src.numel() * src.element_size() < p.src_cap or index.numel() * index.element_size() < p.index_cap:
+            raise ValueError(f"src holds fewer than src_cap = {p.src_cap} bytes, or index fewer than index_cap = {p.index_cap}")
+        if ranges.dtype != torch.int64 or ranges.dim() != 2 or ranges.shape[1] != 2 or ranges.shape[0] < p.max_ranges:
+            raise ValueError(f"ranges must be an int64 tensor of shape ({p.max_ranges}, 2)")
+        if n_ranges.dtype != torch.int64 or n_ranges.numel() != 1:
+            raise ValueError("n_ranges must be a 1-element int64 tensor")
+        if dst.dtype != _torch_dtypes()[self.dtype] or dst.numel() < p.dst_cap:
+            raise ValueError(f"dst must hold at least dst_cap = {p.dst_cap} numbers of {self.dtype}")
+        rc = _lib_async_ranges().pco_b200_decompress_ranges_async(
+            C.byref(p), C.c_void_p(src.data_ptr()), C.c_void_p(index.data_ptr()), C.c_void_p(ranges.data_ptr()), C.c_void_p(n_ranges.data_ptr()),
+            C.c_void_p(dst.data_ptr()), C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()),
+            C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+        _lib.check(rc)
+
+    def status_record(self):
+        """The last call's PcoB200AsyncRangesStatus, copied back (waiting for it on the current stream)."""
+        return _CAsyncRangesStatus.from_buffer_copy(self.status.cpu().numpy().tobytes())
+
+    def result(self):
+        """Copies the status of the last call back (waiting for it on the current stream) and returns the number of numbers written, or
+        raises PcoError with the kind pco_b200_decompress_ranges gives."""
+        s = self.status_record()
+        nw = C.c_size_t()
+        _lib.check(_lib_async_ranges().pco_b200_decompress_ranges_async_result(C.byref(s), C.byref(nw)))
+        return int(nw.value)
+
+
 class _CAsyncCompressPlan(C.Structure):  # PcoB200AsyncCompressPlan (include/pco_b200.h)
     _fields_ = [("dtype", C.c_uint32), ("uniform_type_header", C.c_uint32), ("mode", C.c_uint32), ("order", C.c_uint32),
                 ("n_vars", C.c_uint32), ("bins_log", C.c_uint32), ("mode_k", C.c_uint32), ("reserved", C.c_uint32),
