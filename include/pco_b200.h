@@ -533,6 +533,88 @@ PcoB200Error pco_b200_decompress_ranges_async(const PcoB200AsyncRangesPlan *plan
  * sets *n_written (may be NULL) to the sum of the counts. */
 PcoB200Error pco_b200_decompress_ranges_async_result(const PcoB200AsyncRangesStatus *host_status, size_t *n_written);
 
+/* ---- asynchronous batch of indexed standalone files (no reference counterpart): pco_b200_decompress_files with the file list, its
+ * count and every buffer in device memory.  A data loader or a page cache in HBM holds thousands of small compressed files, each with its
+ * side index; a kernel (a sampler, a cache lookup) picks the ones the next step needs, and this call decodes them behind that kernel
+ * with no copy to the host.  It only enqueues kernels on the caller's stream and returns at once; it makes no synchronising, allocating
+ * or host-to-device copy call and refers to no memory of the library's per-thread scratch, so it can be captured in a CUDA graph, and a
+ * captured call may be replayed after pco_b200_thread_release or after any other call.  A plan made once outside any capture fixes the
+ * grids from its capacities; the refs and their count are read on the device, so one captured graph serves different refs, a different
+ * count and different files (same number type and header flavour) on each replay. */
+typedef struct PcoB200AsyncFilesPlan {  /* filled by pco_b200_decompress_files_async_plan; treat as opaque */
+  uint32_t dtype, uniform_type, format_major, reserved;
+  uint64_t src_cap, index_cap, max_files, max_chunks, dst_cap;
+  uint64_t workspace_bytes;             /* device workspace one in-flight call needs */
+} PcoB200AsyncFilesPlan;
+
+typedef struct PcoB200AsyncFilesStatus {  /* written on the device by every call */
+  uint32_t kind;                          /* PcoB200Error */
+  uint32_t device_status;                 /* the device word behind it: a chunk's PcoB200Error kind, or PCO_B200_ASYNC_* */
+  uint64_t file;                          /* the file the outcome names (UINT64_MAX if none) */
+  uint64_t chunk;                         /* the failing chunk, counted from that file's first chunk (UINT64_MAX if none) */
+  uint64_t n_written;                     /* the sum of the files' counts, once every file passed its checks and placement (0 before) */
+  uint64_t n_files;                       /* *n_files as the call read it */
+} PcoB200AsyncFilesStatus;
+
+/* device_status of a batch refused before any decoding, beyond the PCO_B200_ASYNC_* codes above (which name file `file` here) */
+enum {
+  PCO_B200_ASYNC_TOO_MANY_FILES = 0x10e,       /* *n_files is above the plan's max_files (INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_FILE_OUTSIDE = 0x10f,         /* the file's bytes lie outside src_cap (INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_INDEX_OFFSET = 0x110,         /* its index_offset is not a multiple of 16 (INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_INDEX_OUTSIDE = 0x111,        /* its side index lies outside index_cap (INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_NO_INDEX = 0x112,             /* its index_len is below a side index header's 64 bytes (PCO_B200_UNSUPPORTED) */
+  PCO_B200_ASYNC_ENTRIES_MISALIGNED = 0x113,   /* its batch entries are not 4-byte aligned (INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_RECORDS_OUTSIDE = 0x114,      /* a record points outside its file, its index or its count (INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_FILES_DST = 0x115             /* the files up to this one hold more than dst_cap numbers (PCO_B200_IO) */
+};
+
+/* Makes a plan.  `head`, dtype, src_cap, index_cap and dst_cap (numbers) are those of pco_b200_decompress_async_plan; `head` is the first
+ * bytes of any file of the batch, and every file must have its header flavour.  max_files bounds *n_files of every call, max_chunks the
+ * chunks of the whole batch.  Checked before the device is touched, with the kinds of pco_b200_decompress_async_plan: dtype, the header,
+ * the uniform type, max_files in 1 .. 2^31 - 1, max_chunks in 1 .. 2^32 - 1, dst_cap at most 2^56 (PCO_B200_INVALID_ARGUMENT).  Then
+ * *plan is filled and the one-time device set-up runs on the current device, which the calls must use (kernel attributes, and every
+ * kernel the call launches loaded); without a device that is PCO_B200_CUDA.
+ * workspace_bytes is the sum of these regions, each rounded up to 256 bytes: 1880 (the binomial table and the chunk count), 64 (state),
+ * 4 max_files (file verdicts), 64 max_files (check rows), 4 max_files (record verdicts), 48 max_files (merge rows),
+ * 48 ceil(max_files / 256) (CTA sums), 32 max_chunks (chunk table), 4 max_chunks (statuses), max_chunks (classes), 2 (dst_cap / 256 +
+ * max_chunks + 1) rows of 256 bytes and of 4 bytes (the general pair's scratch, as pco_b200_decompress_async_plan), and the catch-all
+ * decoder's 3.7 MB. */
+PcoB200Error pco_b200_decompress_files_async_plan(const void *head, size_t head_len, unsigned char dtype, size_t src_cap,
+                                                  size_t index_cap, size_t max_files, size_t max_chunks, size_t dst_cap,
+                                                  PcoB200AsyncFilesPlan *plan);
+/* Enqueues the decode of files[0 : *n_files) into dst on `cuda_stream`, and the outcome into *status; returns without waiting.  src
+ * (src_cap bytes), index (index_cap bytes), files (PcoB200FileRef[max_files], offsets counted from src and index), n_files (one
+ * uint64_t), dst (dst_cap numbers), file_ns (uint64_t[max_files]; may be NULL), workspace (plan->workspace_bytes, 256-byte aligned) and
+ * status are device pointers; one workspace serves one call in flight.  File i's numbers land right behind file i - 1's, in `files` order,
+ * and file_ns[i] gets its count; files may repeat and come in any order.  For every batch pco_b200_decompress_files accepts with
+ * src_len = src_cap, index_len = index_cap and dst_len = dst_cap, dst[0 : total), file_ns and the total equal its output.
+ * Refusals, with the kind pco_b200_decompress_files gives and naming the same file: *n_files above max_files; then, over all files first,
+ * the lowest file whose ref lies outside src_cap or index_cap or whose index_offset is not a multiple of 16; then the lowest file that
+ * fails its header, its index header, the check of its records (misaligned entries), its placement (PCO_B200_IO when the running total
+ * passes dst_cap) or its decode.  Every refusal up to placement is decided before any write to dst.  A batch refused before the files
+ * (too many of them, a ref outside the buffers) writes nothing to dst; one whose lowest refused file is j decodes only the files before j,
+ * as pco_b200_decompress_files does, so that a decode failure in one of them is the one reported, and writes nothing at or behind file
+ * j's place.  file_ns is written only on success.
+ * Where this call differs from pco_b200_decompress_files, on purpose:
+ *   - a file with no side index (index_len below 64 bytes) is PCO_B200_UNSUPPORTED (PCO_B200_ASYNC_NO_INDEX): a walk needs the host;
+ *   - a file whose uniform type or format major differs from the plan's is PCO_B200_ASYNC_HEADER_MISMATCH (INVALID_ARGUMENT);
+ *   - a file whose index records point outside its bytes, its index or its count is refused as an index that does not belong to its file
+ *     (PCO_B200_ASYNC_RECORDS_OUTSIDE), where pco_b200_decompress_files decodes it on its own;
+ *   - a batch of more than max_chunks chunks is refused (PCO_B200_ASYNC_TOO_MANY_CHUNKS), naming the first file that takes the running
+ *     chunk count past max_chunks;
+ *   - a chunk the fast kernels decline is decoded by itself with the catch-all decoder, as pco_b200_decompress_async does, and a Lookback
+ *     window beyond 2^16 numbers is PCO_B200_UNSUPPORTED.
+ * The return value covers the host side only: null pointers, an unaligned workspace or a plan that was not filled
+ * (PCO_B200_INVALID_ARGUMENT), a launch the runtime refuses (PCO_B200_CUDA).  With pco_b200_profile_enable(1), a call outside a stream
+ * capture records its kernel spans for pco_b200_profile_last; a call inside a capture records none. */
+PcoB200Error pco_b200_decompress_files_async(const PcoB200AsyncFilesPlan *plan, const void *src, const void *index,
+                                             const PcoB200FileRef *files, const uint64_t *n_files, void *dst, uint64_t *file_ns,
+                                             void *workspace, PcoB200AsyncFilesStatus *status, void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory at a point of the caller's choosing.  Returns the kind,
+ * sets the last-error message as pco_b200_decompress_files words it ("file 17: ...") and, when the kind is OK, sets *n_written (may be
+ * NULL) to the sum of the files' counts. */
+PcoB200Error pco_b200_decompress_files_async_result(const PcoB200AsyncFilesStatus *host_status, size_t *n_written);
+
 #if defined(__cplusplus)
 }
 #endif

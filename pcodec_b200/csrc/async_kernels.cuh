@@ -111,6 +111,21 @@ __device__ inline uint32_t async_parse_header(const uint8_t* b, uint64_t file_le
   return ST_OK;
 }
 
+// C(n, j) mod 2^64 by Pascal additions, n = 0 .. 256 (ensure_device builds the same table on the host), by one thread, into the Binoms
+// lvalue B.  A macro rather than a function: expanded in async_check_kernel, it compiles to the instructions the loop written there gave.
+#define PCOB_ASYNC_FILL_BINOMS(B)                                                    \
+  do {                                                                               \
+    uint64_t row[MAX_ORDER] = {1, 0, 0, 0, 0, 0, 0};                                 \
+    for (int n = 0; n <= 256; n++) {                                                 \
+      if (n > 0)                                                                     \
+        for (int j = MAX_ORDER - 1; j >= 1; j--) row[j] += row[j - 1];               \
+      if ((n & 7) == 0 && n < 256)                                                   \
+        for (int j = 0; j < MAX_ORDER; j++) (B).lane8[n >> 3][j] = row[j];           \
+      if (n == 256)                                                                  \
+        for (int j = 0; j < MAX_ORDER; j++) (B).full[j] = row[j];                    \
+    }                                                                                \
+  } while (0)
+
 // ceil(max_chunks / ASYNC_CHECK_RECS) CTAs.  Each CTA checks the headers (a few dozen bytes, from L2 after the first CTA) and writes its
 // share of the table; CTA 0 also writes the AsyncCheck.  The check is decompress_ex's (host_api.cu, decompress_fast) with
 // file_len <= src_cap in place of equality, plus n_chunks <= max_chunks.  A refused file leaves a table of pads only.
@@ -141,16 +156,7 @@ __global__ void __launch_bounds__(ASYNC_THREADS) async_check_kernel(AsyncArgs a,
       chk->reserved = 0;
     }
   } else if (tid == 32 && blockIdx.x == 0) {
-    // C(n, j) mod 2^64 by Pascal additions, n = 0 .. 256 (ensure_device builds the same table on the host)
-    uint64_t row[MAX_ORDER] = {1, 0, 0, 0, 0, 0, 0};
-    for (int n = 0; n <= 256; n++) {
-      if (n > 0)
-        for (int j = MAX_ORDER - 1; j >= 1; j--) row[j] += row[j - 1];
-      if ((n & 7) == 0 && n < 256)
-        for (int j = 0; j < MAX_ORDER; j++) chk->binoms.lane8[n >> 3][j] = row[j];
-      if (n == 256)
-        for (int j = 0; j < MAX_ORDER; j++) chk->binoms.full[j] = row[j];
-    }
+    PCOB_ASYNC_FILL_BINOMS(chk->binoms);
   }
   __syncthreads();
   const uint64_t w = uint64_t(blockIdx.x) * ASYNC_THREADS + tid;  // word w of the table: record w / 4, field word w % 4

@@ -63,6 +63,13 @@ struct BatchEntry {
 };
 static_assert(sizeof(IndexHeader) == 64 && sizeof(IndexChunk) == 32 && sizeof(BatchEntry) == 12, "index layout");
 
+// A side index header made for a file of `file_len` bytes, whose chunk table lies inside the index's `index_len` bytes (overflow-safe;
+// the per-chunk fields are bounded on the device: entries inside the index, chunk_offset inside the file, writes inside the destination).
+__host__ __device__ inline bool index_header_ok(const IndexHeader& ih, uint64_t file_len, uint64_t index_len) {
+  return ih.magic == INDEX_MAGIC && ih.version == 1 && ih.file_len == file_len && ih.chunks_offset <= index_len &&
+         ih.n_chunks <= (index_len - ih.chunks_offset) / sizeof(IndexChunk);
+}
+
 // ---------------------------------------------------------------------------
 // Bit stream view: a byte range addressed through 8-byte aligned words.
 // ---------------------------------------------------------------------------

@@ -4,6 +4,7 @@
 #include <algorithm>
 
 #include "async_compress.cuh"
+#include "async_files_kernels.cuh"
 #include "async_kernels.cuh"
 #include "async_ranges_kernels.cuh"
 #include "compress_host.cuh"
@@ -248,13 +249,6 @@ static PcoB200Error read_heads(const void* src, size_t src_len, bool src_dev, co
   }
   if (need_sync) PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
   return parse_standalone_header(head, avail, src_len, hdr);
-}
-
-// A side index header made for a file of `file_len` bytes, whose chunk table lies inside the index's `index_len` bytes (overflow-safe;
-// the per-chunk fields are bounded on the device: entries inside the index, chunk_offset inside the file, writes inside the destination).
-static bool index_header_ok(const IndexHeader& ih, uint64_t file_len, uint64_t index_len) {
-  return ih.magic == INDEX_MAGIC && ih.version == 1 && ih.file_len == file_len && ih.chunks_offset <= index_len &&
-         ih.n_chunks <= (index_len - ih.chunks_offset) / sizeof(IndexChunk);
 }
 
 // A caller's buffer in HBM: the buffer itself when it is on the device, else its bytes copied into `buf`.
@@ -2762,6 +2756,185 @@ PcoB200Error pco_b200_decompress_ranges_async_result(const PcoB200AsyncRangesSta
     default:
       status_to_error(s->device_status, ("chunk " + std::to_string(s->chunk)).c_str());
       return range_fail(kind, s->range, last_error_ref());
+  }
+}
+
+// ---- asynchronous batch of indexed standalone files (pco_b200_decompress_files_async; kernels in async_files_kernels.cuh)
+// The plan fixes every grid size (from max_files and max_chunks) and the byte layout of the workspace; the refs and their count are read
+// on the device.  A call is a fixed sequence of twelve launches: files, check_index, scan, place, table, merge_index, fused, symwalk,
+// decode<1>, decode<2>, cold, finish.
+
+static bool af_plan_ok(const PcoB200AsyncFilesPlan* p) {
+  return nt_valid(p->dtype) && p->max_files >= 1 && p->max_files <= 0x7fffffffull && p->max_chunks >= 1 && p->max_chunks <= 0xffffffffull &&
+         p->dst_cap <= (uint64_t(1) << 56) && p->workspace_bytes == af_layout(p->max_files, p->max_chunks, p->dst_cap).total;
+}
+
+PcoB200Error pco_b200_decompress_files_async_plan(const void* head, size_t head_len, unsigned char dtype, size_t src_cap, size_t index_cap,
+                                                  size_t max_files, size_t max_chunks, size_t dst_cap, PcoB200AsyncFilesPlan* plan) {
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (!plan || (!head && head_len)) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  StandaloneHeader hdr;
+  if (PcoB200Error e = parse_standalone_header(static_cast<const uint8_t*>(head), std::min<size_t>(head_len, 32), head_len, &hdr)) return e;
+  if (hdr.uniform_type != 0 && hdr.uniform_type != dtype)
+    return fail(PCO_B200_INVALID_ARGUMENT, "the header's uniform type " + std::to_string(hdr.uniform_type) + " is not dtype " + std::to_string(dtype));
+  if (max_files == 0 || uint64_t(max_files) > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_files must be 1 .. 2^31 - 1");
+  if (max_chunks == 0 || uint64_t(max_chunks) > 0xffffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_chunks must be 1 .. 2^32 - 1");
+  if (uint64_t(dst_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "dst_cap above 2^56 numbers");
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->uniform_type = hdr.uniform_type;
+  plan->format_major = hdr.format_major;
+  plan->src_cap = src_cap;
+  plan->index_cap = index_cap;
+  plan->max_files = max_files;
+  plan->max_chunks = max_chunks;
+  plan->dst_cap = dst_cap;
+  plan->workspace_bytes = af_layout(max_files, max_chunks, dst_cap).total;
+  // the one-time device set-up, as in pco_b200_decompress_async_plan
+  Context& c = ctx();
+  if (PcoB200Error e = ensure_device(c)) return e;
+  if (PcoB200Error e = set_decode_attrs<false>(c)) return e;
+  cudaFuncAttributes fa;
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, af_files_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, check_index_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, af_scan_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, af_place_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, af_table_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, merge_index_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, symwalk_kernel<false>));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, af_finish_kernel));
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
+    using L = decltype(tag);
+    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, fused_narrow_kernel<L>));
+    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, decode_kernel<L, 1>));
+    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, decode_kernel<L, 2>));
+    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, cold_chunks_kernel<L>));
+    return PCO_B200_OK;
+  });
+}
+
+PcoB200Error pco_b200_decompress_files_async(const PcoB200AsyncFilesPlan* plan, const void* src, const void* index, const PcoB200FileRef* files,
+                                             const uint64_t* n_files, void* dst, uint64_t* file_ns, void* workspace, PcoB200AsyncFilesStatus* status,
+                                             void* cuda_stream) {
+  if (!plan || !src || !index || !files || !n_files || !workspace || !status || (!dst && plan->dst_cap))
+    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (!af_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_decompress_files_async_plan");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  PCOB_CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
+  const bool prof = cap == cudaStreamCaptureStatusNone && profiler_enabled().load(std::memory_order_relaxed);
+  if (prof) profiler().discard();
+  auto begin = [&](const char* name) { if (prof) profiler().begin(name, stream); };
+  auto end = [&]() { if (prof) profiler().end(stream); };
+
+  const uint32_t mf = uint32_t(plan->max_files), mc = uint32_t(plan->max_chunks);
+  const AfLayout lay = af_layout(mf, mc, plan->dst_cap);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  AsyncCheck* chk = reinterpret_cast<AsyncCheck*>(ws);
+  AfState* state = reinterpret_cast<AfState*>(ws + lay.state);
+  uint32_t* fst = reinterpret_cast<uint32_t*>(ws + lay.fst);
+  FileCheck* fchk = reinterpret_cast<FileCheck*>(ws + lay.fchk);
+  uint32_t* verdict = reinterpret_cast<uint32_t*>(ws + lay.verdict);
+  FileMerge* merges = reinterpret_cast<FileMerge*>(ws + lay.merges);
+  AfPart* parts = reinterpret_cast<AfPart*>(ws + lay.parts);
+  IndexChunk* table = reinterpret_cast<IndexChunk*>(ws + lay.table);
+  uint32_t* d_st = reinterpret_cast<uint32_t*>(ws + lay.st);
+  uint8_t* d_cls = ws + lay.cls;
+  uint8_t* d_syms = ws + lay.syms;
+  uint32_t* d_offs = reinterpret_cast<uint32_t*>(ws + lay.offs);
+  uint8_t* d_cold = ws + lay.cold;
+  const uint8_t* d_idx = static_cast<const uint8_t*>(index);
+  AfArgs g;
+  g.fp = FileParams{src, plan->src_cap, plan->dtype, plan->uniform_type, plan->format_major};
+  g.index = d_idx;
+  g.index_cap = plan->index_cap;
+  g.dst_cap = plan->dst_cap;
+  g.files = files;
+  g.n_files = n_files;
+  g.max_files = mf;
+  g.max_chunks = mc;
+  const uint32_t fb = uint32_t(af_ctas(mf)), tb = uint32_t(std::max(af_ctas(mf), af_ctas(mc)));
+
+  begin("af_files_kernel");
+  af_files_kernel<<<fb, AF_THREADS, 0, stream>>>(g, chk, fst, fchk, merges, parts);
+  end();
+  begin("check_index_kernel");
+  check_index_kernel<<<mf, 256, 0, stream>>>(static_cast<const uint8_t*>(src), d_idx, plan->dtype, fchk, verdict);
+  end();
+  begin("af_scan_kernel");
+  af_scan_kernel<<<1, AF_SCAN_THREADS, 0, stream>>>(g, parts, state);
+  end();
+  begin("af_place_kernel");
+  af_place_kernel<<<fb, AF_THREADS, 0, stream>>>(g, fst, fchk, verdict, parts, merges, state);
+  end();
+  begin("af_table_kernel");
+  af_table_kernel<<<tb, AF_THREADS, 0, stream>>>(g, state, chk, merges, table);
+  end();
+  begin("merge_index_kernel");
+  merge_index_kernel<<<mf, 256, 0, stream>>>(d_idx, merges, table);
+  end();
+  begin("fused_narrow_kernel");
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    fused_narrow_kernel<L><<<mc, FZ_THREADS, sizeof(FusedSmem), stream>>>(g.fp, table, d_idx, g.index_cap, d_st, d_cls, static_cast<L*>(dst), g.dst_cap);
+    return 0;
+  });
+  end();
+  begin("symwalk_kernel");
+  symwalk_kernel<false><<<mc, SW_THREADS, sizeof(SymWalkSmem), stream>>>(g.fp, table, d_idx, g.index_cap, g.dst_cap, d_syms, d_offs, d_cls);
+  end();
+  begin("decode_kernel");
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    decode_kernel<L, 1><<<mc, DEC_THREADS, sizeof(DecodeSmem), stream>>>(g.fp, table, d_st, d_idx, g.index_cap, static_cast<L*>(dst), g.dst_cap, &chk->binoms,
+                                                                          d_syms, d_offs, d_cls);
+    decode_kernel<L, 2><<<mc, DEC_THREADS, sizeof(DecodeSmem), stream>>>(g.fp, table, d_st, d_idx, g.index_cap, static_cast<L*>(dst), g.dst_cap, &chk->binoms,
+                                                                          d_syms, d_offs, d_cls);
+    return 0;
+  });
+  end();
+  begin("cold_chunks_kernel");
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    cold_chunks_kernel<L><<<1, ASYNC_THREADS, 0, stream>>>(g.fp, table, chk, d_st, static_cast<L*>(dst), g.dst_cap, d_cold);
+    return 0;
+  });
+  end();
+  begin("af_finish_kernel");
+  af_finish_kernel<<<1, AF_SCAN_THREADS, 0, stream>>>(state, chk, merges, fchk, d_st, file_ns, status);
+  end();
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
+}
+
+PcoB200Error pco_b200_decompress_files_async_result(const PcoB200AsyncFilesStatus* s, size_t* n_written) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200Error kind = s->kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(s->kind) : PCO_B200_CORRUPTION;
+  if (kind == PCO_B200_OK) {
+    if (n_written) *n_written = size_t(s->n_written);
+    return PCO_B200_OK;
+  }
+  const uint64_t f = s->file;
+  switch (s->device_status) {
+    case PCO_B200_ASYNC_TOO_MANY_FILES:
+      return fail(kind, "*n_files is " + std::to_string(s->n_files) + ", above the plan's max_files");
+    case PCO_B200_ASYNC_FILE_OUTSIDE: return file_fail(kind, f, "file lies outside src");
+    case PCO_B200_ASYNC_INDEX_OFFSET: return file_fail(kind, f, "index offset is not a multiple of 16");
+    case PCO_B200_ASYNC_INDEX_OUTSIDE: return file_fail(kind, f, "side index lies outside index");
+    case PCO_B200_ASYNC_HEADER_CORRUPT: return file_fail(kind, f, "corrupt standalone header (magic, version, type byte or size hint)");
+    case PCO_B200_ASYNC_HEADER_SHORT: return file_fail(kind, f, "insufficient data: the file ends inside its standalone header");
+    case PCO_B200_ASYNC_HEADER_MISMATCH: return file_fail(kind, f, "the file's uniform type or format version differs from the plan's");
+    case PCO_B200_ASYNC_NO_INDEX: return file_fail(kind, f, "no side index (files without one are walked, which needs the host)");
+    case PCO_B200_ASYNC_INDEX_FOREIGN: return file_fail(kind, f, "side index does not belong to this file");
+    case PCO_B200_ASYNC_ENTRIES_MISALIGNED: return file_fail(kind, f, "side index does not belong to this file (misaligned entries)");
+    case PCO_B200_ASYNC_RECORDS_OUTSIDE:
+      return file_fail(kind, f, "side index does not belong to this file (a record points outside the file, its index or its count)");
+    case PCO_B200_ASYNC_FILES_DST: return file_fail(kind, f, "dst holds fewer numbers than the files up to this one");
+    case PCO_B200_ASYNC_TOO_MANY_CHUNKS: return file_fail(kind, f, "the files up to this one hold more chunks than the plan's max_chunks");
+    default:
+      status_to_error(s->device_status, ("chunk " + std::to_string(s->chunk)).c_str());
+      return file_fail(kind, f, last_error_ref());
   }
 }
 

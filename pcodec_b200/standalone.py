@@ -670,6 +670,106 @@ class AsyncCompressor:
         return int(nw.value), int(il.value)
 
 
+class _CAsyncFilesPlan(C.Structure):  # PcoB200AsyncFilesPlan (include/pco_b200.h)
+    _fields_ = [("dtype", C.c_uint32), ("uniform_type", C.c_uint32), ("format_major", C.c_uint32), ("reserved", C.c_uint32),
+                ("src_cap", C.c_uint64), ("index_cap", C.c_uint64), ("max_files", C.c_uint64), ("max_chunks", C.c_uint64),
+                ("dst_cap", C.c_uint64), ("workspace_bytes", C.c_uint64)]
+
+
+class _CAsyncFilesStatus(C.Structure):  # PcoB200AsyncFilesStatus (include/pco_b200.h)
+    _fields_ = [("kind", C.c_uint32), ("device_status", C.c_uint32), ("file", C.c_uint64), ("chunk", C.c_uint64), ("n_written", C.c_uint64),
+                ("n_files", C.c_uint64)]
+
+
+def _lib_async_files():
+    L = _lib.lib()
+    if not getattr(L, "_async_files_ready", False):
+        L.pco_b200_decompress_files_async_plan.argtypes = [C.c_void_p, C.c_size_t, C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                                           C.c_size_t, C.c_void_p]
+        L.pco_b200_decompress_files_async.argtypes = [C.c_void_p] * 10
+        L.pco_b200_decompress_files_async_result.argtypes = [C.c_void_p, C.POINTER(C.c_size_t)]
+        L._async_files_ready = True
+    return L
+
+
+class AsyncFilesDecompressor:
+    """Decodes a batch of indexed standalone files on the current CUDA stream with the file list in device memory and without waiting for
+    the device (pco_b200_decompress_files_async): refs a kernel picked (a sampler, a cache lookup) need no trip to the host, and a call can
+    be captured in a torch.cuda.CUDAGraph.
+
+    The plan comes from `head`, the first bytes of any file of the batch (as AsyncDecompressor): every file must share its number type and
+    header flavour.  src_cap, index_cap (bytes) and dst_cap (numbers) are the sizes of the buffers every call passes, max_files the most
+    files of a call and max_chunks the most chunks of a whole batch.  The number of files is read from a device tensor, so one captured call
+    serves different refs, a different count and different files on each replay.  The decompressor owns a device workspace and a status;
+    it serves one call in flight."""
+
+    def __init__(self, head, dtype, src_cap, index_cap, max_files, max_chunks, dst_cap, device=None):
+        import torch
+
+        from .wrapped import _host_u8
+
+        self.dtype = np.dtype(dtype)
+        if _is_cuda(head):
+            head = head.reshape(-1)[:32].cpu().numpy()
+        h = _host_u8(head)[:32].copy()
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        L = _lib_async_files()
+        self._plan = _CAsyncFilesPlan()
+        with torch.cuda.device(self.device):
+            rc = L.pco_b200_decompress_files_async_plan(h.ctypes.data_as(C.c_void_p), C.c_size_t(h.size), C.c_ubyte(_lib.dtype_byte(self.dtype)),
+                                                        C.c_size_t(src_cap), C.c_size_t(index_cap), C.c_size_t(max_files), C.c_size_t(max_chunks),
+                                                        C.c_size_t(dst_cap), C.byref(self._plan))
+        _lib.check(rc)
+        self.workspace = torch.empty(self._plan.workspace_bytes, dtype=torch.uint8, device=self.device)
+        self.status = torch.zeros(C.sizeof(_CAsyncFilesStatus), dtype=torch.uint8, device=self.device)
+
+    @property
+    def workspace_bytes(self):
+        return int(self._plan.workspace_bytes)
+
+    def __call__(self, src, index, files, n_files, dst, file_ns):
+        """Enqueues the decode of files[: n_files[0]] into `dst` (a CUDA tensor of the plan's dtype, at least dst_cap numbers) on
+        torch.cuda.current_stream(): file i lands right behind file i - 1 and file_ns[i] gets its count.  `src` and `index` are uint8 CUDA
+        tensors of at least src_cap and index_cap bytes; `files` is an int64 CUDA tensor of shape (max_files, 4) holding the FILE_REF
+        fields (offset, len, index_offset, index_len), `n_files` a 1-element int64 CUDA tensor, `file_ns` an int64 CUDA tensor of at least
+        max_files elements.  Returns nothing and does not wait; result() reports the outcome."""
+        import torch
+
+        from .wrapped import _torch_dtypes
+
+        p = self._plan
+        for name, t in (("src", src), ("index", index), ("files", files), ("n_files", n_files), ("dst", dst), ("file_ns", file_ns)):
+            if not _is_cuda(t) or t.device != self.device or not t.is_contiguous():
+                raise ValueError(f"{name} must be a contiguous CUDA tensor on {self.device}")
+        if src.numel() * src.element_size() < p.src_cap or index.numel() * index.element_size() < p.index_cap:
+            raise ValueError(f"src holds fewer than src_cap = {p.src_cap} bytes, or index fewer than index_cap = {p.index_cap}")
+        if files.dtype != torch.int64 or files.dim() != 2 or files.shape[1] != 4 or files.shape[0] < p.max_files:
+            raise ValueError(f"files must be an int64 tensor of shape ({p.max_files}, 4)")
+        if n_files.dtype != torch.int64 or n_files.numel() != 1:
+            raise ValueError("n_files must be a 1-element int64 tensor")
+        if file_ns.dtype != torch.int64 or file_ns.numel() < p.max_files:
+            raise ValueError(f"file_ns must be an int64 tensor of at least max_files = {p.max_files} elements")
+        if dst.dtype != _torch_dtypes()[self.dtype] or dst.numel() < p.dst_cap:
+            raise ValueError(f"dst must hold at least dst_cap = {p.dst_cap} numbers of {self.dtype}")
+        rc = _lib_async_files().pco_b200_decompress_files_async(
+            C.byref(p), C.c_void_p(src.data_ptr()), C.c_void_p(index.data_ptr()), C.c_void_p(files.data_ptr()), C.c_void_p(n_files.data_ptr()),
+            C.c_void_p(dst.data_ptr()), C.c_void_p(file_ns.data_ptr()), C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()),
+            C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+        _lib.check(rc)
+
+    def status_record(self):
+        """The last call's PcoB200AsyncFilesStatus, copied back (waiting for it on the current stream)."""
+        return _CAsyncFilesStatus.from_buffer_copy(self.status.cpu().numpy().tobytes())
+
+    def result(self):
+        """Copies the status of the last call back (waiting for it on the current stream) and returns the number of numbers written, or
+        raises PcoError with the kind pco_b200_decompress_files gives ("file 17: ...")."""
+        s = self.status_record()
+        nw = C.c_size_t()
+        _lib.check(_lib_async_files().pco_b200_decompress_files_async_result(C.byref(s), C.byref(nw)))
+        return int(nw.value)
+
+
 class _CModeChoice(C.Structure):
     _fields_ = [("mode_spec", C.c_uint32), ("float_quant_k", C.c_uint32), ("float_mult_base", C.c_double), ("float_mult_inv_base", C.c_double),
                 ("int_mult_base", C.c_uint64), ("bits_saved_per_num", C.c_double)]
