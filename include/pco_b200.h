@@ -615,6 +615,90 @@ PcoB200Error pco_b200_decompress_files_async(const PcoB200AsyncFilesPlan *plan, 
  * NULL) to the sum of the files' counts. */
 PcoB200Error pco_b200_decompress_files_async_result(const PcoB200AsyncFilesStatus *host_status, size_t *n_written);
 
+/* ---- asynchronous batch compress of standalone files (no reference counterpart): pco_b200_compress_files with the file sizes, their
+ * count and every buffer in device memory.  A checkpoint writer compresses every tensor of a model, an offload compresses the blocks a
+ * step evicted, a columnar writer its column chunks: a kernel decides how many files there are and how large each is, and this call
+ * compresses them behind it with no copy to the host.  It only enqueues kernels on the caller's stream and returns at once; it makes no
+ * synchronising, allocating or host-to-device copy call and refers to no memory of the library's per-thread scratch, so it can be
+ * captured in a CUDA graph, and a captured call may be replayed after pco_b200_thread_release or after any other call.  A plan made once
+ * outside any capture fixes the config and the grids from its capacities; the sizes and their count are read on the device, so one
+ * captured graph serves a different count, different sizes and different numbers on each replay.  The whole batch is one pass of the
+ * encode kernels, whatever unoptimized_bins_log its chunks' sizes imply. */
+typedef struct PcoB200AsyncCompressFilesPlan {  /* filled by pco_b200_compress_files_async_plan; treat as opaque */
+  uint32_t dtype, uniform_type_header, mode, order;
+  uint32_t n_vars, level, mode_k, reserved;
+  uint64_t max_files, nums_cap, max_file_n, max_page_n, max_chunks, dst_cap, index_cap;
+  uint64_t mode_base, base_bits, inv_base_bits;
+  uint64_t dst_bound;                           /* bytes of dst every batch within the capacities fits in */
+  uint64_t index_bound;                         /* bytes of index every batch within the capacities fits in */
+  uint64_t workspace_bytes;                     /* device workspace one in-flight call needs */
+} PcoB200AsyncCompressFilesPlan;
+
+typedef struct PcoB200AsyncCompressFilesStatus {  /* written on the device by every call */
+  uint32_t kind;                                  /* PcoB200Error */
+  uint32_t device_status;                         /* 0, or the PCO_B200_ASYNC_* code behind the kind */
+  uint64_t file;                                  /* the file a refusal names (UINT64_MAX if none) */
+  uint64_t n_files;                               /* *n_files as the call read it */
+  uint64_t dst_bytes;                             /* bytes of dst the batch needs, also when above dst_cap (0 when refused earlier) */
+  uint64_t index_bytes;                           /* bytes of index it needs (0 without an index, or when refused earlier) */
+  uint64_t dst_written;                           /* bytes written to dst (0 unless OK) */
+  uint64_t index_written;                         /* bytes written to index (0 unless OK) */
+} PcoB200AsyncCompressFilesStatus;
+
+/* device_status of a refused batch, beyond PCO_B200_ASYNC_TOO_MANY_FILES (*n_files above max_files, INVALID_ARGUMENT) */
+enum {
+  PCO_B200_ASYNC_FILE_TOO_LARGE = 0x116,    /* file `file` holds more than max_file_n numbers (PCO_B200_INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_NUMS_CAP = 0x117,          /* the counts up to file `file` add up to more than nums_cap (PCO_B200_INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_FILES_DST_FULL = 0x118,    /* the files need more than dst_cap bytes (PCO_B200_IO) */
+  PCO_B200_ASYNC_FILES_INDEX_FULL = 0x119   /* their side indexes need more than index_cap bytes (PCO_B200_IO) */
+};
+
+/* Makes a plan for batches of up to max_files files of dtype, compressed with `config` (NULL = the default config, whose Auto specs are
+ * refused) into standalone files of the flavour uniform_type_header selects: at most nums_cap numbers in all, at most max_file_n per
+ * file, dst_cap bytes of destination and, when index_cap is not 0, side indexes in up to index_cap bytes.  Runs on the host, before and
+ * outside any capture.  Refuses what pco_b200_compress_async_plan refuses, with the same kinds (pco_b200_compress_ex's config checks;
+ * ModeSpec::Auto, DeltaSpec::Auto and PagingSpec::Exact; more than 256 unoptimized bins at the largest chunk, min(max_page_n,
+ * max_file_n, nums_cap) numbers, PCO_B200_UNSUPPORTED), but not chunk sizes that imply different unoptimized_bins_log: each chunk gets
+ * its own.  max_files outside 1 .. 2^31 - 1, max_file_n of 0, nums_cap above 2^56, or capacities whose chunk slots times the largest
+ * chunk's tiles of numbers pass 2^31 - 1 CTAs are PCO_B200_INVALID_ARGUMENT.  Then *plan is filled and the one-time device set-up runs on
+ * the current device, which the calls must use; without a device that is PCO_B200_CUDA.
+ * The plan's bounds, with m = min(max_page_n (0: 2^18), max_file_n, nums_cap) (at least 1), L the number type's bits and V the latent vars
+ * of the mode (1 for Classic, else 2):
+ *   max_chunks  = floor(nums_cap / m) + max_files                                  (chunks of any batch within the capacities)
+ *   dst_bound   = max_files * 18 + max_chunks * (5 + meta) + ceil(nums_cap * L / 8)  (18: the largest header and a terminator; per
+ *                 chunk its 4 framing bytes, 1 for the rounding of its body and meta, a baseline chunk's metadata: (1125 + L + the bits of
+ *                 L's offset width) / 8 rounded up, 150 bytes for 64-bit numbers; the size pco_standalone_guarantee_file_size assumes)
+ *   index_bound = max_files * 64 + max_chunks * (32 + 12 V + 15) + 12 V * ceil(nums_cap / 256)
+ * workspace_bytes is pco_b200_compress_async_plan's formula for max_chunks chunks of m numbers and nums_cap + 255 max_chunks rows, plus
+ * these regions, each rounded up to 256 bytes: 136 (state), 56 max_files (file table), 80 ceil(max_files / 256) (CTA sums),
+ * 4 max_chunks (chunk files), 8 ceil((max_chunks + 1) / 256) (chunk CTA sums) and 8 (max_chunks + 1) (chunk byte offsets). */
+PcoB200Error pco_b200_compress_files_async_plan(unsigned char dtype, const PcoB200ChunkConfig *config, int uniform_type_header,
+                                                size_t max_files, size_t nums_cap, size_t max_file_n, size_t dst_cap, size_t index_cap,
+                                                PcoB200AsyncCompressFilesPlan *plan);
+/* Enqueues the compress of files[0 : *n_files) on `cuda_stream`, and the outcome into *status; returns without waiting.  File i is the
+ * next file_ns[i] numbers of `nums`, as in pco_b200_compress_files.  nums (nums_cap numbers), file_ns (uint64_t[max_files]), n_files (one
+ * uint64_t), dst (dst_cap bytes), index (index_cap bytes, 16-byte aligned; may be NULL), files (PcoB200FileRef[max_files]), workspace
+ * (plan->workspace_bytes, 256-byte aligned) and status are device pointers; one workspace serves one call in flight.  For every batch
+ * within the capacities, dst[0 : total), each file's side index at its 16-byte aligned offset and files[0 : *n_files) equal what
+ * pco_b200_compress_files writes for the same numbers, sizes and config with every buffer on the device; *n_files = 0 writes nothing.
+ * Refusals, in this order: *n_files above max_files (PCO_B200_ASYNC_TOO_MANY_FILES); the lowest file above max_file_n or that takes the
+ * running sum of the counts past nums_cap (PCO_B200_INVALID_ARGUMENT); the files or their indexes above dst_cap or index_cap (PCO_B200_IO,
+ * with `files` and the status reporting the sizes needed).  The first two are decided before anything is written to dst, index or files,
+ * and write nothing there; a batch that does not fit writes only `files`.  The return value covers the host side only: null pointers, an
+ * unaligned workspace or index, an index with a plan made without one, or a plan that was not filled (PCO_B200_INVALID_ARGUMENT), a launch
+ * the runtime refuses (PCO_B200_CUDA).  With pco_b200_profile_enable(1), a call outside a stream capture records its kernel spans for
+ * pco_b200_profile_last; a call inside a capture records none. */
+PcoB200Error pco_b200_compress_files_async(const PcoB200AsyncCompressFilesPlan *plan, const void *nums, const uint64_t *file_ns,
+                                           const uint64_t *n_files, void *dst, void *index, PcoB200FileRef *files, void *workspace,
+                                           PcoB200AsyncCompressFilesStatus *status, void *cuda_stream);
+/* Testing aid, host only: writes the standalone header for a size hint of n_hint (uniform_type 0, or the number type byte) into out (at
+ * least 17 bytes) with the function the device framing uses, and returns its length (0 if the length the placement assumed differs). */
+size_t pco_b200_debug_standalone_header(uint64_t n_hint, unsigned char uniform_type, unsigned char *out);
+/* Host only: the outcome of a call, from its status copied back to host memory at a point of the caller's choosing.  Returns the kind,
+ * sets the last-error message as pco_b200_compress_files words it ("file 17: ...") and, when the kind is OK, sets *dst_len and *index_len
+ * (either may be NULL) to the bytes written. */
+PcoB200Error pco_b200_compress_files_async_result(const PcoB200AsyncCompressFilesStatus *host_status, size_t *dst_len, size_t *index_len);
+
 #if defined(__cplusplus)
 }
 #endif

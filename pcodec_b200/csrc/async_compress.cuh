@@ -106,6 +106,8 @@ struct AcompHead {
 };
 __device__ inline uint64_t* acomp_gate(const AcompArgs& a, uint32_t g) { return reinterpret_cast<uint64_t*>(a.ws + a.lay.gates) + uint64_t(g) * (a.n_chunks + 1); }
 __device__ inline uint64_t acomp_start(const AcompArgs& a, uint64_t c) { return c * a.low + (c < a.rem ? c : a.rem); }
+// the chunk starts the init kernel wrote (acomp_init_kernel, or acf_init_kernel for a batch of files): the gates copy them
+__device__ inline const uint64_t* acomp_starts(const AcompArgs& a) { return reinterpret_cast<const uint64_t*>(a.ws + a.lay.starts); }
 __device__ inline void acomp_reset_chunk(ChunkEnc* ch) {  // init_chunks_kernel's record
   ChunkEnc z;
   memset(&z, 0, sizeof(z));
@@ -172,8 +174,9 @@ __global__ void __launch_bounds__(ACOMP_THREADS) acomp_two_gate_kernel(AcompArgs
   const bool two = always_two || h->flags[1] != 0;
   ChunkEnc* chunks = reinterpret_cast<ChunkEnc*>(a.ws + a.lay.chunks);
   uint64_t* g = acomp_gate(a, 0);
+  const uint64_t* starts = acomp_starts(a);
   for (uint64_t c = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; c <= a.n_chunks; c += uint64_t(gridDim.x) * blockDim.x) {
-    g[c] = two ? acomp_start(a, c) : 0;
+    g[c] = two ? starts[c] : 0;
     if (two && c < a.n_chunks) acomp_reset_chunk(&chunks[c]);
   }
 }
@@ -202,7 +205,7 @@ __global__ void __launch_bounds__(1024) acomp_var_gate_kernel(AcompArgs a, uint3
     const bool narrow = bits <= PLAN_MAX_COUNT_BITS;
     const bool on[ACOMP_GATES_PER_VAR] = {two && narrow, two && !narrow, narrow, !narrow};
     for (uint64_t c = threadIdx.x; c <= a.n_chunks; c += blockDim.x) {
-      const uint64_t s = acomp_start(a, c);
+      const uint64_t s = acomp_starts(a)[c];
       for (uint32_t k = 0; k < ACOMP_GATES_PER_VAR; k++) acomp_gate(a, 1 + ACOMP_GATES_PER_VAR * v + k)[c] = on[k] ? s : 0;
     }
     __syncthreads();

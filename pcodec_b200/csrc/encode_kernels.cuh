@@ -67,6 +67,17 @@ struct EncParams {
   uint32_t uniform_type;   // header flavour
 };
 
+// unoptimized_bins_log of var v of a chunk of n >= 1 numbers at compression level `level` (choose_unoptimized_bins_log,
+// chunk_compressor.rs:362-371; the secondary var takes at most 6, LIMITED_UNOPTIMIZED_BINS_LOG, chunk_compressor.rs:238-248).  The
+// CHUNK_BINS instantiations of the planner kernels take the level in ep.bins_log[0] and compute each chunk's value with this, so one
+// launch serves chunks whose sizes imply different values.
+__device__ __forceinline__ uint32_t chunk_bins_log(uint32_t level, uint64_t n, int v) {
+  const uint32_t log_n = 63u - uint32_t(__clzll((long long)n));
+  const uint32_t fast = log_n >= 4 ? log_n - 4 : 0;
+  const uint32_t b = level <= fast ? level : fast + (level - fast) / 2;
+  return v == 0 ? b : min(b, 6u);
+}
+
 template <bool WIDE>
 struct VarPlanT {
   static constexpr int MAXB = EncCap<WIDE>::MAXB;
@@ -557,7 +568,7 @@ struct PlanSmem {
 // COUNTING = true : `keys` holds the raw (unsorted) latents and the key range is < 2^range_bits <= 2^15: the CTA counts
 //                   every key into shared memory, prefix-sums the counters, and reads ranks / run extents off the
 //                   cumulative counts -- the planner only ever needs order statistics, never the sorted array.
-template <typename L, bool COUNTING, bool WIDE = false>
+template <typename L, bool COUNTING, bool WIDE = false, bool CHUNK_BINS = false>
 __global__ void __launch_bounds__(PLAN_THREADS) plan_probe_kernel(EncParams ep, const L* __restrict__ keys, const ChunkEnc* __restrict__ chunks,
                                                                    PlanProbesT<WIDE>* __restrict__ probes, int v, uint32_t range_bits,
                                                                    uint16_t* __restrict__ keys16, uint32_t n_override = 0) {
@@ -641,7 +652,7 @@ __global__ void __launch_bounds__(PLAN_THREADS) plan_probe_kernel(EncParams ep, 
     return lo;
   };
   PlanProbesT<WIDE>& pr = probes[c];
-  const uint32_t n_bins_log = ep.bins_log[v];
+  const uint32_t n_bins_log = CHUNK_BINS ? chunk_bins_log(ep.bins_log[0], ce - cs, v) : ep.bins_log[v];
   const uint32_t nbk = 1u << n_bins_log;
   auto c_count_of = [&](uint32_t b) -> uint32_t { return uint32_t((uint64_t(b + 1) * n + nbk - 1) >> n_bins_log); };
   if (tid == 0) pr.first = s_at(0);
@@ -745,7 +756,7 @@ __device__ __forceinline__ void sc_stream(const L* __restrict__ nums, uint32_t n
   }
 }
 
-template <typename L>
+template <typename L, bool CHUNK_BINS = false>
 __global__ void __launch_bounds__(SC_THREADS, 1) split_count_kernel(EncParams ep, ChunkEnc* __restrict__ chunks, PlanProbes* __restrict__ probes,
                                                                    uint16_t* __restrict__ keys16, uint32_t* __restrict__ flags) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -864,7 +875,7 @@ __global__ void __launch_bounds__(SC_THREADS, 1) split_count_kernel(EncParams ep
     return lo;
   };
   PlanProbes& pr = probes[c];
-  const uint32_t n_bins_log = ep.bins_log[0];
+  const uint32_t n_bins_log = CHUNK_BINS ? chunk_bins_log(ep.bins_log[0], n, 0) : ep.bins_log[0];
   const uint32_t nbk = 1u << n_bins_log;
   auto c_count_of = [&](uint32_t b) -> uint32_t { return uint32_t((uint64_t(b + 1) * stored + nbk - 1) >> n_bins_log); };
   if (tid == 0) pr.first = s_at(0);
@@ -992,7 +1003,7 @@ __global__ void broadcast_plan_kernel(VarPlanT<WIDE>* __restrict__ plans, uint32
   for (uint32_t i = threadIdx.x; i < sizeof(VarPlanT<WIDE>) / 16; i += blockDim.x) dst[i] = src[i];
 }
 
-template <typename L>
+template <typename L, bool CHUNK_BINS = false>
 __global__ void __launch_bounds__(SOLVE_THREADS) plan_solve_kernel(EncParams ep, const PlanProbes* __restrict__ probes,
                                                                     const ChunkEnc* __restrict__ chunks, VarPlan* __restrict__ plans, int v,
                                                                     uint32_t n_override = 0) {
@@ -1011,7 +1022,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS) plan_solve_kernel(EncParams ep,
     return;
   }
   ENC_TICK_INIT();
-  const uint32_t n_bins_log = ep.bins_log[v];
+  const uint32_t n_bins_log = CHUNK_BINS ? chunk_bins_log(ep.bins_log[0], ce - cs, v) : ep.bins_log[v];
   const uint32_t nbk = 1u << n_bins_log;
   const bool small_n = n <= (1u << 20);  // (cc << n_bins_log) fits 32 bits (n_bins_log <= 8)
   // (cc << n_bins_log) / n, cc <= n: the quotient is at most 2^n_bins_log <= 256, so a float estimate is within 1 of it and one

@@ -4,6 +4,7 @@
 #include <algorithm>
 
 #include "async_compress.cuh"
+#include "async_compress_files.cuh"
 #include "async_files_kernels.cuh"
 #include "async_kernels.cuh"
 #include "async_ranges_kernels.cuh"
@@ -3063,6 +3064,163 @@ PcoB200Error pco_b200_compress_async_result(const PcoB200AsyncCompressStatus* s,
   if (s->device_status == PCO_B200_ASYNC_DST_FULL)
     return fail(kind, "failed to write whole buffer (need " + std::to_string(s->file_bytes) + " bytes)");
   return fail(kind, "asynchronous compress failed (device status " + std::to_string(s->device_status) + ")");
+}
+
+// ---- asynchronous batch compress (pco_b200_compress_files_async; kernels in async_compress_files.cuh).  The plan fixes the config and the
+// grids from the capacities; the call is a fixed sequence of launches: files, scan, place, init, the encode kernels of
+// pco_b200_compress_async (split_count and the planner kernels in their CHUNK_BINS instantiations), bytes, bytes scan, offsets, pack gate,
+// one pack per choice of keys, frame, [index], finish.
+
+PcoB200Error pco_b200_compress_files_async_plan(unsigned char dtype, const PcoB200ChunkConfig* config, int uniform_type_header, size_t max_files,
+                                                size_t nums_cap, size_t max_file_n, size_t dst_cap, size_t index_cap,
+                                                PcoB200AsyncCompressFilesPlan* plan) {
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (!plan) return fail(PCO_B200_INVALID_ARGUMENT, "null plan");
+  PcoB200ChunkConfig cfg;
+  if (config) cfg = *config;
+  else {
+    std::memset(&cfg, 0, sizeof(cfg));  // pco::ChunkConfig::default(): level 8, Auto, Auto, EqualPagesUpTo(2^18)
+    cfg.compression_level = 8;
+  }
+  if (max_files == 0 || max_files > 0x7fffffffu) return fail(PCO_B200_INVALID_ARGUMENT, "max_files must be in 1 .. 2^31 - 1");
+  if (max_file_n == 0) return fail(PCO_B200_INVALID_ARGUMENT, "max_file_n must be at least 1");
+  if (uint64_t(nums_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "nums_cap must be at most 2^56");
+  // the config as compress_async_plan checks it, at the largest chunk (a file of min(max_page_n, max_file_n, nums_cap) numbers is one chunk)
+  // (Exact paging first: its page sizes are checked against a count, and a batch has none)
+  if (cfg.paging_spec == PCO_B200_PAGING_EXACT) return fail(PCO_B200_UNSUPPORTED, "PagingSpec::Exact: the asynchronous compress takes EqualPagesUpTo only");
+  const uint64_t chunk_n = acf_chunk_n(cfg.max_page_n, max_file_n, nums_cap);
+  ConfigCheck ck;
+  if (PcoB200Error e = check_config(cfg, dtype, size_t(chunk_n), &ck)) return e;
+  if (ck.auto_mode || ck.auto_delta)
+    return fail(PCO_B200_UNSUPPORTED, "ModeSpec::Auto and DeltaSpec::Auto search on host threads: the asynchronous compress takes explicit specs only");
+  if (choose_unoptimized_bins_log(cfg.compression_level, size_t(chunk_n)) > ENC_NARROW_BINS_LOG)
+    return fail(PCO_B200_UNSUPPORTED, "more than 256 unoptimized bins (levels 9-12): the asynchronous compress runs the narrow kernels only");
+  const uint64_t max_chunks = uint64_t(nums_cap) / chunk_n + max_files;
+  const uint64_t tiles = (chunk_n + SPLIT_TILE - 1) / SPLIT_TILE, bpc = n_batches_of(uint32_t(chunk_n));
+  const uint64_t per_chunk = std::max<uint64_t>({tiles, (bpc + BINL_BATCHES - 1) / BINL_BATCHES, (bpc + 7) / 8, uint64_t(MAX_VARS)});
+  if (max_chunks > 0x7fffffffu / per_chunk)
+    return fail(PCO_B200_INVALID_ARGUMENT, "the capacities give " + std::to_string(max_chunks) + " chunk slots, more than one launch can cover");
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->uniform_type_header = uniform_type_header ? 1 : 0;
+  plan->mode = ck.explicit_mode.mode;
+  plan->order = ck.explicit_order;
+  plan->n_vars = ck.explicit_mode.mode == MODE_CLASSIC ? 1 : 2;
+  plan->level = cfg.compression_level;
+  plan->mode_k = ck.explicit_mode.mode_k;
+  plan->max_files = max_files;
+  plan->nums_cap = nums_cap;
+  plan->max_file_n = max_file_n;
+  plan->max_page_n = cfg.max_page_n;
+  plan->max_chunks = max_chunks;
+  plan->dst_cap = dst_cap;
+  plan->index_cap = index_cap;
+  plan->mode_base = ck.explicit_mode.mode_base;
+  plan->base_bits = ck.explicit_mode.base_bits;
+  plan->inv_base_bits = ck.explicit_mode.inv_base_bits;
+  const uint64_t lbits = nt_bits(dtype);
+  plan->dst_bound = uint64_t(max_files) * (standalone_header_size() + 1) + max_chunks * (5 + baseline_chunk_meta_size(uint32_t(lbits))) +
+                    (uint64_t(nums_cap) * lbits + 7) / 8;
+  plan->index_bound = uint64_t(max_files) * sizeof(IndexHeader) + max_chunks * (sizeof(IndexChunk) + plan->n_vars * sizeof(BatchEntry) + 15) +
+                      plan->n_vars * sizeof(BatchEntry) * ((uint64_t(nums_cap) + BATCH_N - 1) / BATCH_N);
+  plan->workspace_bytes = acf_plan_geom(*plan).l.total;
+  // the one-time device set-up (compress_async_plan's, for this call's kernels)
+  Context& c = ctx();
+  if (PcoB200Error e = ensure_device(c)) return e;
+  cudaFuncAttributes fa;
+  for (const void* k : {(const void*)acf_files_kernel, (const void*)acf_scan_kernel, (const void*)acf_place_kernel, (const void*)acf_init_kernel,
+                        (const void*)acf_bytes_kernel, (const void*)acf_bytes_scan_kernel, (const void*)acf_offsets_kernel, (const void*)acf_frame_kernel,
+                        (const void*)acf_index_kernel, (const void*)acf_finish_kernel, (const void*)acomp_two_gate_kernel, (const void*)acomp_var_gate_kernel,
+                        (const void*)acomp_pack_gate_kernel, (const void*)segment_offsets_kernel, (const void*)fallback_kernel<false>,
+                        (const void*)ans_encode_kernel<false>, (const void*)layout_kernel<false>})
+    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, k));
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
+    using L = decltype(tag);
+    constexpr size_t RS_SMEM = size_t(RS_WARPS) * RS_BINS * sizeof(uint32_t);
+    const int count_smem = int(((size_t(1) << PLAN_MAX_COUNT_BITS) + 1) * 4 + 16);
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, count_smem));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(split_count_kernel<L, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(size_t(SC_N) * 4)));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PackSmem)));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(radix_sort_segments_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RS_SMEM));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true, false, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(bin_lut_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    for (const void* k : {(const void*)split_count_kernel<L, true>, (const void*)split_delta_kernel<L, MODE_CLASSIC>, (const void*)split_delta_kernel<L, MODE_INT_MULT>,
+                          (const void*)split_delta_kernel<L, MODE_FLOAT_QUANT>, (const void*)split_delta_kernel<L, MODE_FLOAT_MULT>,
+                          (const void*)plan_probe_kernel<L, false, false, true>, (const void*)sort_keys_kernel<L>, (const void*)plan_solve_kernel<L, true>,
+                          (const void*)bin_kernel<L, false>})
+      PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, k));
+    return PCO_B200_OK;
+  });
+}
+
+PcoB200Error pco_b200_compress_files_async(const PcoB200AsyncCompressFilesPlan* plan, const void* nums, const uint64_t* file_ns, const uint64_t* n_files,
+                                           void* dst, void* index, PcoB200FileRef* files, void* workspace, PcoB200AsyncCompressFilesStatus* status,
+                                           void* cuda_stream) {
+  if (!plan || !file_ns || !n_files || !files || !workspace || !status || (!nums && plan->nums_cap) || (!dst && plan->dst_cap))
+    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  AcfPlanGeom pg;
+  if (PcoB200Error e = acf_check_plan(plan, &pg)) return e;
+  if (index && plan->index_cap == 0) return fail(PCO_B200_INVALID_ARGUMENT, "an index with a plan made without one (index_cap 0)");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  if (reinterpret_cast<uintptr_t>(index) & 15) return fail(PCO_B200_INVALID_ARGUMENT, "the index is not 16-byte aligned");
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  PCOB_CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
+  const bool prof = cap == cudaStreamCaptureStatusNone && profiler_enabled().load(std::memory_order_relaxed);
+  if (prof) profiler().discard();
+  AcfArgs fa;
+  std::memset(&fa, 0, sizeof(fa));
+  fa.a.n_chunks = pg.g.n_chunks;
+  fa.a.dst_cap = plan->dst_cap;
+  fa.a.n_vars = plan->n_vars;
+  fa.a.ws = static_cast<uint8_t*>(workspace);
+  fa.a.dst = static_cast<uint8_t*>(dst);
+  fa.a.index = static_cast<uint8_t*>(index);
+  fa.a.lay = pg.l.enc;
+  fa.l = pg.l;
+  fa.file_ns = file_ns;
+  fa.n_files = n_files;
+  fa.files = files;
+  fa.max_files = plan->max_files;
+  fa.max_file_n = plan->max_file_n;
+  fa.nums_cap = plan->nums_cap;
+  fa.max_page_n = plan->max_page_n == 0 ? (uint64_t(1) << 18) : plan->max_page_n;
+  fa.index_cap = index ? plan->index_cap : 0;
+  fa.uniform_type = plan->uniform_type_header ? plan->dtype : 0;
+  fa.bpc = pg.g.bpc;
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    acf_launch<decltype(tag)>(*plan, pg.g, fa, nums, status, stream, prof);
+    return 0;
+  });
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;
+}
+
+size_t pco_b200_debug_standalone_header(uint64_t n_hint, unsigned char uniform_type, unsigned char* out) {
+  const uint32_t len = standalone_header_into(n_hint, uniform_type, out);
+  return len == standalone_header_len(n_hint) ? len : 0;
+}
+
+PcoB200Error pco_b200_compress_files_async_result(const PcoB200AsyncCompressFilesStatus* s, size_t* dst_len, size_t* index_len) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200Error kind = s->kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(s->kind) : PCO_B200_CORRUPTION;
+  if (kind == PCO_B200_OK) {
+    if (dst_len) *dst_len = size_t(s->dst_written);
+    if (index_len) *index_len = size_t(s->index_written);
+    return PCO_B200_OK;
+  }
+  switch (s->device_status) {
+    case PCO_B200_ASYNC_TOO_MANY_FILES:
+      return fail(kind, std::to_string(s->n_files) + " files, more than the plan's max_files");
+    case PCO_B200_ASYNC_FILE_TOO_LARGE: return file_fail(kind, size_t(s->file), "more numbers than the plan's max_file_n");
+    case PCO_B200_ASYNC_NUMS_CAP: return file_fail(kind, size_t(s->file), "the files up to this one hold more numbers than the plan's nums_cap");
+    case PCO_B200_ASYNC_FILES_DST_FULL:
+    case PCO_B200_ASYNC_FILES_INDEX_FULL:
+      return fail(kind, "failed to write whole buffer (need " + std::to_string(s->dst_bytes) + " file bytes and " + std::to_string(s->index_bytes) +
+                            " index bytes)");
+    default: return fail(kind, "asynchronous batch compress failed (device status " + std::to_string(s->device_status) + ")");
+  }
 }
 
 PcoB200Error pco_b200_build_index(const void* compressed, size_t compressed_len, unsigned char dtype, void* index, size_t index_cap,

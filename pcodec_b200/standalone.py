@@ -770,6 +770,127 @@ class AsyncFilesDecompressor:
         return int(nw.value)
 
 
+class _CAsyncCompressFilesPlan(C.Structure):  # PcoB200AsyncCompressFilesPlan (include/pco_b200.h)
+    _fields_ = [("dtype", C.c_uint32), ("uniform_type_header", C.c_uint32), ("mode", C.c_uint32), ("order", C.c_uint32),
+                ("n_vars", C.c_uint32), ("level", C.c_uint32), ("mode_k", C.c_uint32), ("reserved", C.c_uint32),
+                ("max_files", C.c_uint64), ("nums_cap", C.c_uint64), ("max_file_n", C.c_uint64), ("max_page_n", C.c_uint64),
+                ("max_chunks", C.c_uint64), ("dst_cap", C.c_uint64), ("index_cap", C.c_uint64),
+                ("mode_base", C.c_uint64), ("base_bits", C.c_uint64), ("inv_base_bits", C.c_uint64),
+                ("dst_bound", C.c_uint64), ("index_bound", C.c_uint64), ("workspace_bytes", C.c_uint64)]
+
+
+class _CAsyncCompressFilesStatus(C.Structure):  # PcoB200AsyncCompressFilesStatus (include/pco_b200.h)
+    _fields_ = [("kind", C.c_uint32), ("device_status", C.c_uint32), ("file", C.c_uint64), ("n_files", C.c_uint64),
+                ("dst_bytes", C.c_uint64), ("index_bytes", C.c_uint64), ("dst_written", C.c_uint64), ("index_written", C.c_uint64)]
+
+
+def _lib_async_compress_files():
+    L = _lib.lib()
+    if not getattr(L, "_async_compress_files_ready", False):
+        L.pco_b200_compress_files_async_plan.argtypes = [C.c_ubyte, C.c_void_p, C.c_int, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                                         C.c_size_t, C.c_void_p]
+        L.pco_b200_compress_files_async.argtypes = [C.c_void_p] * 10
+        L.pco_b200_compress_files_async_result.argtypes = [C.c_void_p, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
+        L._async_compress_files_ready = True
+    return L
+
+
+class AsyncFilesCompressor:
+    """Compresses a batch of standalone files on the current CUDA stream, with the file sizes in device memory and without waiting for the
+    device (pco_b200_compress_files_async): sizes a kernel decided (the tensors of a checkpoint, the blocks a step evicted) need no trip to
+    the host, and a call can be captured in a torch.cuda.CUDAGraph.
+
+    The plan fixes the number type `dtype`, the config (explicit mode and delta specs, EqualPagesUpTo paging), the header flavour
+    (uniform_type_header: as simple_compress_into) and the capacities: at most max_files files, nums_cap numbers in all and max_file_n per
+    file, dst_cap bytes of files (default: the plan's dst_bound, which every batch within the capacities fits in) and, with index=True,
+    the plan's index_bound bytes of side indexes.  The sizes and their count are read when the call runs, so one captured call compresses
+    a different count, different sizes and different numbers on each replay.  The bytes, the indexes and the refs equal what compress_files
+    writes.  The compressor owns a device workspace and a status; it serves one call in flight."""
+
+    def __init__(self, dtype, config, max_files, nums_cap, max_file_n, dst_cap=None, index=True, uniform_type_header=False, device=None):
+        import torch
+
+        self.dtype = np.dtype(dtype)
+        dtb = _lib.dtype_byte(self.dtype)
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        L = _lib_async_compress_files()
+        cfg = (config or ChunkConfig())._to_c()
+        self._plan = _CAsyncCompressFilesPlan()
+
+        def plan(dcap, icap):
+            with torch.cuda.device(self.device):
+                return L.pco_b200_compress_files_async_plan(C.c_ubyte(dtb), C.byref(cfg), C.c_int(1 if uniform_type_header else 0), C.c_size_t(max_files),
+                                                            C.c_size_t(nums_cap), C.c_size_t(max_file_n), C.c_size_t(dcap), C.c_size_t(icap),
+                                                            C.byref(self._plan))
+
+        if dst_cap is None or index:  # the bounds are known once a plan exists: a first plan reports them
+            _lib.check(plan(dst_cap or 0, 0))
+        _lib.check(plan(self._plan.dst_bound if dst_cap is None else dst_cap, self._plan.index_bound if index else 0))
+        self.workspace = torch.empty(self._plan.workspace_bytes, dtype=torch.uint8, device=self.device)
+        self.status = torch.zeros(C.sizeof(_CAsyncCompressFilesStatus), dtype=torch.uint8, device=self.device)
+
+    @property
+    def dst_cap(self):
+        return int(self._plan.dst_cap)
+
+    @property
+    def index_cap(self):
+        """Bytes of side indexes a call may write (0 without an index)."""
+        return int(self._plan.index_cap)
+
+    @property
+    def max_files(self):
+        return int(self._plan.max_files)
+
+    @property
+    def workspace_bytes(self):
+        return int(self._plan.workspace_bytes)
+
+    def __call__(self, nums, file_ns, n_files, dst, index, files):
+        """Enqueues the compress of the first n_files[0] files on torch.cuda.current_stream(): file i is the next file_ns[i] numbers of
+        `nums` (a CUDA tensor of the plan's dtype, at least nums_cap numbers).  `file_ns` is an int64 CUDA tensor of at least max_files
+        elements, `n_files` a 1-element int64 CUDA tensor, `dst` a uint8 CUDA tensor of at least dst_cap bytes, `index` one of at least
+        index_cap bytes (or None), and `files` the int64 (max_files, 4) CUDA tensor of FILE_REF fields that AsyncFilesDecompressor takes.
+        Returns nothing and does not wait; result() reports the outcome."""
+        import torch
+
+        from .wrapped import _torch_dtypes
+
+        p = self._plan
+        for name, t in (("nums", nums), ("file_ns", file_ns), ("n_files", n_files), ("dst", dst), ("files", files)) + ((("index", index),) if index is not None else ()):
+            if not _is_cuda(t) or t.device != self.device or not t.is_contiguous():
+                raise ValueError(f"{name} must be a contiguous CUDA tensor on {self.device}")
+        if nums.dtype != _torch_dtypes()[self.dtype] or nums.numel() < p.nums_cap:
+            raise ValueError(f"nums must hold at least nums_cap = {p.nums_cap} numbers of {self.dtype}")
+        if file_ns.dtype != torch.int64 or file_ns.numel() < p.max_files:
+            raise ValueError(f"file_ns must be an int64 tensor of at least max_files = {p.max_files} elements")
+        if n_files.dtype != torch.int64 or n_files.numel() != 1:
+            raise ValueError("n_files must be a 1-element int64 tensor")
+        if dst.numel() * dst.element_size() < p.dst_cap:
+            raise ValueError(f"dst holds fewer than dst_cap = {p.dst_cap} bytes")
+        if index is not None and (not p.index_cap or index.numel() * index.element_size() < p.index_cap):
+            raise ValueError(f"index needs a compressor made with index=True and at least index_cap = {p.index_cap} bytes")
+        if files.dtype != torch.int64 or files.dim() != 2 or files.shape[1] != 4 or files.shape[0] < p.max_files:
+            raise ValueError(f"files must be an int64 tensor of shape ({p.max_files}, 4)")
+        rc = _lib_async_compress_files().pco_b200_compress_files_async(
+            C.byref(p), C.c_void_p(nums.data_ptr()), C.c_void_p(file_ns.data_ptr()), C.c_void_p(n_files.data_ptr()), C.c_void_p(dst.data_ptr()),
+            C.c_void_p(index.data_ptr()) if index is not None else None, C.c_void_p(files.data_ptr()), C.c_void_p(self.workspace.data_ptr()),
+            C.c_void_p(self.status.data_ptr()), C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+        _lib.check(rc)
+
+    def status_record(self):
+        """The last call's PcoB200AsyncCompressFilesStatus, copied back (waiting for it on the current stream)."""
+        return _CAsyncCompressFilesStatus.from_buffer_copy(self.status.cpu().numpy().tobytes())
+
+    def result(self):
+        """Copies the status of the last call back (waiting for it on the current stream) and returns (dst_len, index_len), the bytes
+        written, or raises PcoError with the kind pco_b200_compress_files gives ("file 17: ...")."""
+        s = self.status_record()
+        dl, il = C.c_size_t(), C.c_size_t()
+        _lib.check(_lib_async_compress_files().pco_b200_compress_files_async_result(C.byref(s), C.byref(dl), C.byref(il)))
+        return int(dl.value), int(il.value)
+
+
 class _CModeChoice(C.Structure):
     _fields_ = [("mode_spec", C.c_uint32), ("float_quant_k", C.c_uint32), ("float_mult_base", C.c_double), ("float_mult_inv_base", C.c_double),
                 ("int_mult_base", C.c_uint64), ("bits_saved_per_num", C.c_double)]
