@@ -13,7 +13,8 @@
 //     section starts.  full/empty mbarriers carry the hand-over.
 //   * the other (FZ_DECODERS) warps decode, a warp per batch in batch order (page_latent_decompressor.rs:15-44, delta/consecutive.rs:35-50,
 //     mode/classic.rs:14-24): symbols from the ring, the offsets window by cp.async one batch ahead, fields peeled off
-//     register windows, the order-1 un-delta as one 32-bit scan + the fence-free carry record, 32-byte stores.
+//     register windows, the order-1 un-delta as one 32-bit scan + the fence-free carry record, 16-byte stores that write whole
+//     128-byte lines after a transpose across 8 lanes (store8).
 // Compared with the two-kernel decode (symwalk_kernel + decode_kernel) the symbol bytes never leave the SM (no 0.27 GB scratch
 // written and read back), the section starts are not stored, the header is parsed once, and the compressed bytes are read by one kernel.
 #pragma once
@@ -52,8 +53,10 @@ __device__ __forceinline__ uint32_t ones_shl_wrap(uint32_t s) {  // 0xffffffff <
 #ifndef PCOB_FZ_WALKERS
 #define PCOB_FZ_WALKERS 2
 #endif
-// walkers, ring buffers and staged symbols per row are build-time knobs (-D); the defaults were chosen by timing C2 (1024 chunks x 2^18
-// u64) over 1..3 walkers, 2..3 buffers and rows of 64..256 symbols.
+// walkers, ring buffers, staged symbols per row and the launch bounds' CTAs per SM are build-time knobs (-D); the defaults were chosen by
+// timing fused_narrow_kernel on bench.py's data (C2, 1024 chunks x 2^18 u64) on an H100 SXM at 700 W over 2..3 walkers, 2..4 buffers,
+// rows of 64..256 symbols and 2..4 CTAs per SM.  2 CTAs per SM (up to 128 registers, no spills) beat 3 by 2 % and 4 by 18 %: at 4 (64
+// registers) the kernel spills, and store8's transpose only pays once it does not; 3 walkers or rows of 64 or 256 symbols were slower.
 #ifndef PCOB_FZ_ROW_SYMS
 #define PCOB_FZ_ROW_SYMS 128
 #endif
@@ -61,7 +64,7 @@ __device__ __forceinline__ uint32_t ones_shl_wrap(uint32_t s) {  // 0xffffffff <
 #define PCOB_FZ_NODE_WORDS 2048
 #endif
 #ifndef PCOB_FZ_MIN_BLOCKS
-#define PCOB_FZ_MIN_BLOCKS 4
+#define PCOB_FZ_MIN_BLOCKS 2
 #endif
 #ifndef PCOB_FZ_THREADS
 #define PCOB_FZ_THREADS 256
@@ -470,7 +473,7 @@ __device__ __forceinline__ void fused_decoder(FusedSmem& sm, const FileParams& f
     } else {
       const uint32_t out_cnt = min(uint32_t(BATCH_N), n_out - b * BATCH_N);
       if (out_cnt == uint32_t(BATCH_N) && (reinterpret_cast<uintptr_t>(dst) & (sizeof(L) >= 4 ? 15 : sizeof(L) * 8 - 1)) == 0) {
-        store8<L>(dst, res);
+        store8<L>(dst, res, lane);
       } else {
 #pragma unroll
         for (int e = 0; e < 8; e++)

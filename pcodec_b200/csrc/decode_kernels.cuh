@@ -757,19 +757,66 @@ __device__ __forceinline__ void undelta_chain_cold(L (&x)[8], DecodeSmem& sm, ui
   for (int e = 0; e < 8; e++) x[e] = tmp[e];
 }
 
+// One butterfly step of a transpose across lanes: the lanes that differ in lane bit M swap their pieces whose slot bit C differs from
+// that lane bit, so the piece that sat at (lane bit x, slot bit y) moves to (lane bit y, slot bit x).  4 shuffles per piece sent.
+template <int NP, int M, int C>
+__device__ __forceinline__ void swap_pieces(uint4 (&w)[NP], bool hi) {
+#pragma unroll
+  for (int i = 0; i < NP; i++) {
+    if (i & C) continue;
+    const int j = i | C;
+    const uint4 s = hi ? w[i] : w[j];
+    uint4 v;
+    v.x = __shfl_xor_sync(0xffffffffu, s.x, M);
+    v.y = __shfl_xor_sync(0xffffffffu, s.y, M);
+    v.z = __shfl_xor_sync(0xffffffffu, s.z, M);
+    v.w = __shfl_xor_sync(0xffffffffu, s.w, M);
+    if (hi) w[i] = v;
+    else w[j] = v;
+  }
+}
+__device__ __forceinline__ void st_cs_v4(char* p, const uint4& v) {  // evict-first: nothing on the decode path reads the output back
+  asm volatile("st.global.cs.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+
 // 8 consecutive numbers of a lane -> global memory.  16 bytes is the widest store sm_90 has (32-byte stores arrived with
-// sm_100), so 4- and 8-byte types take two or four of them; callers pass a 16-byte-aligned dst for those types.
+// sm_100), so 4- and 8-byte types take two or four of them; callers pass a 16-byte-aligned dst for those types.  Stored where
+// each lane holds them (64 or 32 bytes apart), every warp store would write half of each 32-byte sector it touches.  So each group
+// of 8 lanes first transposes its 16-byte pieces by shuffles (two butterfly steps for 8-byte types, one for 4-byte ones), and
+// then every store instruction writes whole 128-byte lines, one per group.  All 32 lanes must take this path together: the callers'
+// conditions (a whole batch, a 16-byte-aligned dst) are the same for every lane of a warp, as lane offsets are multiples of 32 bytes.
+// On H100 this took fused_narrow_kernel on bench.py's data from 1.33 to 1.10 ms, together with the register budget of its
+// launch bounds (decode_fused.cuh): at 64 registers the transpose spilled and gained only 1-2 %.
 template <typename L>
-__device__ __forceinline__ void store8(L* __restrict__ dst, const L (&r)[8]) {
-  if (sizeof(L) == 8) {
+__device__ __forceinline__ void store8(L* __restrict__ dst, const L (&r)[8], int lane) {
+  if constexpr (sizeof(L) >= 4) {
+    constexpr int NP = sizeof(L) / 2;  // 16-byte pieces per lane; the group's 8 NP pieces are NP lines
+    uint4 w[NP];
 #pragma unroll
-    for (int q = 0; q < 4; q++)
-      asm volatile("st.global.v2.u64 [%0], {%1, %2};" ::"l"(dst + 2 * q), "l"(uint64_t(r[2 * q])), "l"(uint64_t(r[2 * q + 1])) : "memory");
-  } else if (sizeof(L) == 4) {
+    for (int p = 0; p < NP; p++) {
+      uint32_t u[4];
 #pragma unroll
-    for (int q = 0; q < 2; q++)
-      asm volatile("st.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(dst + 4 * q), "r"(uint32_t(r[4 * q])), "r"(uint32_t(r[4 * q + 1])),
-                   "r"(uint32_t(r[4 * q + 2])), "r"(uint32_t(r[4 * q + 3])) : "memory");
+      for (int k = 0; k < 4; k++) {
+        const int e = p * (16 / sizeof(L)) + (sizeof(L) == 8 ? k / 2 : k);
+        u[k] = sizeof(L) == 8 ? uint32_t(uint64_t(r[e]) >> (32 * (k & 1))) : uint32_t(r[e]);
+      }
+      w[p] = make_uint4(u[0], u[1], u[2], u[3]);
+    }
+    // piece p of group lane s is the group's piece s NP + p; its line is the top bits of that index, and the swaps move those bits into
+    // the slot: after them slot t holds line t, and the lane holds piece `at` of every line
+    const int s = lane & 7;
+    if constexpr (NP == 4) {  // piece index (s2 s1 s0 p1 p0) -> lane (p1 p0 s0), slot (s2 s1)
+      swap_pieces<NP, 4, 2>(w, s & 4);
+      swap_pieces<NP, 2, 1>(w, s & 2);
+    } else {  // piece index (s2 s1 s0 p0) -> lane (p0 s1 s0), slot (s2)
+      swap_pieces<NP, 4, 1>(w, s & 4);
+    }
+    const int at = NP == 4 ? 4 * (s & 1) + (s >> 1) : 2 * (s & 3) + (s >> 2);
+    char* const line0 = reinterpret_cast<char*>(dst) - 16 * NP * s;  // the group's first line
+#pragma unroll
+    for (int t = 0; t < NP; t++) {
+      st_cs_v4(line0 + 128 * t + 16 * at, w[t]);
+    }
   } else if (sizeof(L) == 2) {  // 8 numbers = 16 bytes: one store when aligned
     if ((reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
       asm volatile("st.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "r"(uint32_t(r[0]) | (uint32_t(r[1]) << 16)), "r"(uint32_t(r[2]) | (uint32_t(r[3]) << 16)),
@@ -797,7 +844,7 @@ __device__ __forceinline__ void win_store8(const WinTask& w, uint32_t b, int lan
   const uint32_t j0 = b * BATCH_N + uint32_t(lane) * 8;
   const bool whole = b * BATCH_N >= w.lo && b * BATCH_N + BATCH_N <= w.hi;
   if (whole && (reinterpret_cast<uintptr_t>(out + (j0 - w.lo)) & 15) == 0) {
-    store8<L>(out + (j0 - w.lo), r);
+    store8<L>(out + (j0 - w.lo), r, lane);
   } else {
 #pragma unroll
     for (int e = 0; e < 8; e++)
@@ -1454,7 +1501,7 @@ decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __
         if constexpr (WIN) {
           win_store8<L>(wins[blockIdx.x], b, lane, res);
         } else if (out_cnt == BATCH_N && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
-          store8<L>(dst, res);  // 16-byte stores; a chunk that starts at an odd element offset takes the element-wise path
+          store8<L>(dst, res, lane);  // 16-byte stores; a chunk that starts at an odd element offset takes the element-wise path
         } else {
 #pragma unroll
           for (int e = 0; e < 8; e++)

@@ -749,10 +749,18 @@ __device__ __forceinline__ void sc_stream(const L* __restrict__ nums, uint32_t n
       kw[u] = w & 0xffffu;
       if (live) atomicAdd(&cnt[w & SC_MASK], 1u);
     }
-    // rows are 256-aligned and padded: vector stores of the keys
+    // rows are 256-aligned and padded: vector stores of the keys.  16-byte ones when SC_PER allows, so that a warp's stores fill
+    // whole 32-byte sectors (two 8-byte stores would each leave every sector half written)
+    if (SC_PER % 8 == 0) {
 #pragma unroll
-    for (int g = 0; g < SC_PER / 4; g++)
-      *reinterpret_cast<uint2*>(k16 + s + 4 * g) = make_uint2(kw[4 * g] | (kw[4 * g + 1] << 16), kw[4 * g + 2] | (kw[4 * g + 3] << 16));
+      for (int g = 0; g < SC_PER / 8; g++)
+        *reinterpret_cast<uint4*>(k16 + s + 8 * g) = make_uint4(kw[8 * g] | (kw[8 * g + 1] << 16), kw[8 * g + 2] | (kw[8 * g + 3] << 16),
+                                                               kw[8 * g + 4] | (kw[8 * g + 5] << 16), kw[8 * g + 6] | (kw[8 * g + 7] << 16));
+    } else {
+#pragma unroll
+      for (int g = 0; g < SC_PER / 4; g++)
+        *reinterpret_cast<uint2*>(k16 + s + 4 * g) = make_uint2(kw[4 * g] | (kw[4 * g + 1] << 16), kw[4 * g + 2] | (kw[4 * g + 3] << 16));
+    }
   }
 }
 
