@@ -390,6 +390,8 @@ int pco_oracle_kat_histogram_u64(const uint64_t* latents, size_t n, uint32_t n_b
     *n_out = bins.size();
   });
 }
+// histograms.rs:250-258: heapsort fallbacks taken by every histogram built in this process so far
+uint64_t pco_oracle_heapsort_fallbacks(void) { return heapsort_fallbacks().load(std::memory_order_relaxed); }
 // histograms.rs apply_sorted over several pre-sorted slices (tests :375-386)
 int pco_oracle_kat_histogram_sorted_u32(const uint32_t* latents, const size_t* slice_lens, size_t n_slices, size_t n, uint32_t n_bins_log,
                                         uint64_t* out, size_t* n_out, uint64_t* incomplete_out, int* has_incomplete) {

@@ -2,6 +2,8 @@
 // Chunk planner: equal-count histogram (partial quicksort), bin optimisation DP,
 // tANS weight quantisation.  Bit-exactness of "same bins" rests on this file.
 #pragma once
+#include <atomic>
+
 #include "pco_format.hpp"
 
 namespace pco_oracle {
@@ -93,6 +95,14 @@ inline void heapsort(L* x, size_t len) {
 // ---------------------------------------------------------------------------
 // pco/src/histograms.rs
 // ---------------------------------------------------------------------------
+// How often apply_quicksort_recurse ran out of good pivots and took the heapsort + apply_sorted fallback (:250-258), over the
+// process.  Test infrastructure: the GPU planner does not reproduce that fallback, so the tests that compare it with the oracle
+// check that their inputs never reach it.
+inline std::atomic<uint64_t>& heapsort_fallbacks() {
+  static std::atomic<uint64_t> count{0};
+  return count;
+}
+
 template <typename L>
 struct HistogramBin {
   size_t count;
@@ -209,6 +219,7 @@ struct HistogramBuilder {
     if (pr.second) {
       bad_pivot_limit -= 1;
       if (bad_pivot_limit == 0) {
+        heapsort_fallbacks().fetch_add(1, std::memory_order_relaxed);
         heapsort(v, lhs_count);
         heapsort(v + lhs_count, len - lhs_count);
         apply_sorted(v, len);

@@ -437,14 +437,18 @@ static PcoB200Error plan_front(CompressScratch& S, cudaStream_t stream, EncParam
           PCOB_CUDA_TRY(cudaFuncSetAttribute(union_probe_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(size_t(SC_N) * 4)));
         }
         PCOB_CUDA_TRY(cudaMemsetAsync(d_small, 0, 8, stream));
+        profiler().begin("union_probe_kernel", stream);
         union_probe_kernel<L><<<1, SC_THREADS, size_t(SC_N) * 4, stream>>>(e, n_chunks, d_chunks, d_probes, S.key16_0.as<uint16_t>(), d_small);
+        profiler().end(stream);
         PCOB_CUDA_TRY(cudaMemcpyAsync(fl, d_small, 8, cudaMemcpyDeviceToHost, stream));
         PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
         if (fl[1] == 0) {
           vrb[0] = fl[0];
           uint64_t stored_total = 0;
           for (uint64_t pn : sizes) stored_total += pn > e.order ? pn - e.order : 0;
+          profiler().begin("plan_solve_kernel", stream);
           plan_solve_kernel<L><<<1, SOLVE_THREADS, 0, stream>>>(e, d_probes, d_chunks, d_plans, 0, uint32_t(stored_total));
+          profiler().end(stream);
           broadcast_plan_kernel<<<n_chunks, 128, 0, stream>>>(d_plans, n_chunks);
           return PCO_B200_OK;
         }
@@ -481,7 +485,9 @@ static PcoB200Error plan_front(CompressScratch& S, cudaStream_t stream, EncParam
       // pages of one wrapped chunk on the sort path: common minimum, the pages' keys as one gap-free segment, one sort,
       // the union's probes and plan, copied to every page's slot (classic mode: one latent var)
       PCOB_CUDA_TRY(cudaMemsetAsync(d_small, 0, 4, stream));
+      profiler().begin("union_range_kernel", stream);
       union_range_kernel<<<1, 32, 0, stream>>>(e, n_chunks, d_chunks, d_small);
+      profiler().end(stream);
       uint32_t range_bits = 0;
       PCOB_CUDA_TRY(cudaMemcpyAsync(&range_bits, d_small, 4, cudaMemcpyDeviceToHost, stream));
       PCOB_CUDA_TRY(cudaStreamSynchronize(stream));
@@ -497,15 +503,22 @@ static PcoB200Error plan_front(CompressScratch& S, cudaStream_t stream, EncParam
       const uint64_t seg_host[2] = {0, stored_total};
       uint64_t* d_seg = d_prefix + prefix.size();
       PCOB_CUDA_TRY(cudaMemcpyAsync(d_seg, seg_host, 16, cudaMemcpyHostToDevice, stream));
+      // (span names prefixed union_: one segment holding every page, told apart from the per-chunk sort below)
+      profiler().begin("union_sort_keys_kernel", stream);
       sort_keys_kernel<L><<<n_chunks * tiles, 256, 0, stream>>>(e, tiles, d_lat[0], S.keys_a.as<L>(), d_chunks, 0, d_prefix);
+      profiler().end(stream);
       const L* sorted = S.keys_a.as<L>();
       if (stored_total > 1) {
         const uint32_t sort_bits = std::max<uint32_t>(range_bits, 1);
         PCOB_CUDA_TRY(ensure_sort_attr());
+        profiler().begin("union_radix_sort_kernel", stream);
         radix_sort_segments_kernel<L><<<1, RS_THREADS, RS_SMEM, stream>>>(S.keys_a.as<L>(), S.keys_b.as<L>(), d_seg, d_seg + 1, sort_bits);
+        profiler().end(stream);
         if (((sort_bits + RS_BITS - 1) / RS_BITS) & 1) sorted = S.keys_b.as<L>();
       }
+      profiler().begin("union_plan_probe_kernel_sorted", stream);
       plan_probe_kernel<L, false, WIDE><<<1, PLAN_THREADS, 16, stream>>>(e, sorted, d_chunks, d_probes, 0, range_bits, nullptr, uint32_t(stored_total));
+      profiler().end(stream);
       solve(1, 0, uint32_t(stored_total));
       broadcast_plan_kernel<WIDE><<<n_chunks, 128, 0, stream>>>(d_plans, n_chunks);
       return PCO_B200_OK;
