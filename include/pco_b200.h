@@ -699,6 +699,79 @@ size_t pco_b200_debug_standalone_header(uint64_t n_hint, unsigned char uniform_t
  * (either may be NULL) to the bytes written. */
 PcoB200Error pco_b200_compress_files_async_result(const PcoB200AsyncCompressFilesStatus *host_status, size_t *dst_len, size_t *index_len);
 
+/* ---- asynchronous batch of wrapped-format pages (no reference counterpart): pco_b200_decompress_pages with the page refs, their count
+ * and every buffer in device memory.  A GPU reader of a container that embeds pco (a columnar file whose column chunks carry pco metas
+ * and pages, a store that keeps page bytes apart from their chunk metadata) prunes pages on the device - a filter on page statistics, a
+ * row-group selection, a join's probe side - and this call decodes the surviving pages behind that kernel with no copy to the host.  It
+ * only enqueues kernels on the caller's stream and returns at once; it makes no synchronising, allocating or host-to-device copy call and
+ * refers to no memory of the library's per-thread scratch, so it can be captured in a CUDA graph, and a captured call may be replayed
+ * after pco_b200_thread_release or after any other call.  A plan made once outside any capture fixes the grids from its capacities; the
+ * refs and their count are read on the device, so one captured graph serves different refs, a different count and different bytes on
+ * each replay.  Pages carry no uniform type and are wrapped format 4.x, as pco_b200_decompress_pages assumes. */
+typedef struct PcoB200AsyncPagesPlan {  /* filled by pco_b200_decompress_pages_async_plan; treat as opaque */
+  uint32_t dtype, reserved;
+  uint64_t metas_cap, pages_cap, max_pages, dst_cap, frame_cap;
+  uint64_t workspace_bytes;             /* device workspace one in-flight call needs */
+} PcoB200AsyncPagesPlan;
+
+typedef struct PcoB200AsyncPagesStatus {  /* written on the device by every call */
+  uint32_t kind;                          /* PcoB200Error */
+  uint32_t device_status;                 /* the device word behind it: a page's PcoB200Error kind, or PCO_B200_ASYNC_* */
+  uint64_t page;                          /* the page the outcome names (UINT64_MAX if none) */
+  uint64_t n_written;                     /* the sum of page_n, once every page passed its checks (0 before, and on a failure) */
+  uint64_t n_pages;                       /* *n_pages as the call read it */
+  uint64_t frames_needed;                 /* bytes of framed pages the batch needs, also when above frame_cap (0 when refused earlier) */
+} PcoB200AsyncPagesStatus;
+
+/* device_status of a batch refused before any decoding */
+enum {
+  PCO_B200_ASYNC_TOO_MANY_PAGES = 0x11a,  /* *n_pages is above the plan's max_pages (INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_META_OUTSIDE = 0x11b,    /* page `page`'s chunk meta lies outside metas_cap (INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_PAGE_OUTSIDE = 0x11c,    /* page `page`'s bytes lie outside pages_cap (INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_PAGE_N = 0x11d,          /* page `page`'s page_n is outside 1 .. 2^24 (INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_PAGES_DST = 0x11e,       /* the pages up to page `page` hold more than dst_cap numbers (INVALID_ARGUMENT) */
+  PCO_B200_ASYNC_FRAMES = 0x11f           /* the framed pages need more than frame_cap bytes, frames_needed (PCO_B200_IO) */
+};
+
+/* Makes a plan for batches of up to max_pages pages of dtype, whose refs point into metas_cap bytes of metas and pages_cap bytes of pages,
+ * decoded into dst_cap numbers.  Each page is decoded as a standalone chunk framed in the workspace ([dtype][page_n - 1][meta][page], 16-byte
+ * aligned: ceil((4 + meta_len + page_len) / 16) * 16 bytes); frame_cap bounds the sum of those frames.  Checked before the device is
+ * touched: dtype (PCO_B200_INVALID_TYPE), max_pages in 1 .. 2^31 - 1, dst_cap and frame_cap at most 2^56 (PCO_B200_INVALID_ARGUMENT).
+ * Then *plan is filled and the one-time device set-up runs on the current device, which the calls must use (kernel attributes, and every
+ * kernel the call launches loaded); without a device that is PCO_B200_CUDA.
+ * workspace_bytes is the sum of these regions, each rounded up to 256 bytes, with m = max_pages: 1880 (the binomial table), 136 (state),
+ * 48 m (page table), 32 (m + 1) + 24 floor(dst_cap / 256) + 32 m (placeholder records and batch entries), ceil(frame_cap / 16) * 16 + 64
+ * (frames and a pad frame), 4 m, 4 m and 8 m (meta statuses, walk statuses, walk ends), 56 ceil(m / 256) (CTA sums), 32 m (decode table),
+ * 4 m (its pages), 4 m (cold list), 4 m (statuses), m (classes), 2 (dst_cap / 256 + m + 1) rows of 256 bytes and of 4 bytes (the
+ * general pair's scratch, as pco_b200_decompress_async_plan), and the catch-all decoder's 3.7 MB. */
+PcoB200Error pco_b200_decompress_pages_async_plan(unsigned char dtype, size_t metas_cap, size_t pages_cap, size_t max_pages,
+                                                  size_t dst_cap, size_t frame_cap, PcoB200AsyncPagesPlan *plan);
+/* Enqueues the decode of the pages refs[0 : *n_pages) names into dst on `cuda_stream`, and the outcome into *status; returns without
+ * waiting.  metas (metas_cap bytes), pages (pages_cap bytes; may be the same buffer as metas), refs (PcoB200PageRef[max_pages]), n_pages
+ * (one uint64_t), dst (dst_cap numbers), workspace (plan->workspace_bytes, 256-byte aligned) and status are device pointers; one workspace
+ * serves one call in flight.  Page i lands right behind page i - 1, in refs order; pages may repeat, come in any order and share a meta.
+ * For every batch pco_b200_decompress_pages accepts with metas_len = metas_cap, pages_len = pages_cap and dst_len = dst_cap, dst[0 : total)
+ * and the total (n_written) equal its output.
+ * Refusals, in this order, with the kind pco_b200_decompress_pages gives and naming the same page: *n_pages above max_pages; the lowest
+ * page whose ref lies outside metas_cap or pages_cap or whose page_n is outside 1 .. 2^24; the page whose running sum of page_n passes
+ * dst_cap (pco_b200_decompress_pages reports that without a page); then, on the device, the lowest page that fails its meta length
+ * (INVALID_ARGUMENT), its meta layout (CORRUPTION), its walk (with the kind its walk over its own frame alone gives) or its decode.  A batch
+ * refused before the device touches a page writes nothing to dst; one whose lowest failing page is j writes nothing at or behind j's slot.
+ * Where this call differs from pco_b200_decompress_pages, on purpose:
+ *   - framed pages that need more than frame_cap bytes are PCO_B200_IO (PCO_B200_ASYNC_FRAMES), with frames_needed reported;
+ *   - a Lookback window beyond 2^16 numbers is PCO_B200_UNSUPPORTED, as in the other asynchronous calls (pco 1.0.3 writes windows of at
+ *     most 2^15, so its pages always decode).
+ * The return value covers the host side only: null pointers, an unaligned workspace or a plan that was not filled
+ * (PCO_B200_INVALID_ARGUMENT), a launch the runtime refuses (PCO_B200_CUDA).  With pco_b200_profile_enable(1), a call outside a stream
+ * capture records its kernel spans for pco_b200_profile_last; a call inside a capture records none. */
+PcoB200Error pco_b200_decompress_pages_async(const PcoB200AsyncPagesPlan *plan, const void *metas, const void *pages,
+                                             const PcoB200PageRef *refs, const uint64_t *n_pages, void *dst, void *workspace,
+                                             PcoB200AsyncPagesStatus *status, void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory at a point of the caller's choosing.  Returns the kind,
+ * sets the last-error message as pco_b200_decompress_pages words it ("page 17: ...") and, when the kind is OK, sets *n_written (may be
+ * NULL) to the sum of page_n. */
+PcoB200Error pco_b200_decompress_pages_async_result(const PcoB200AsyncPagesStatus *host_status, size_t *n_written);
+
 #if defined(__cplusplus)
 }
 #endif

@@ -439,11 +439,12 @@ __device__ inline uint32_t walk_chunk_serial(const BitSrc& src, const ChunkHdr& 
 #define PCOB_WALK_MIN_BLOCKS 8
 #endif
 constexpr int WALK_THREADS = PCOB_WALK_THREADS;
+// The body of walk_kernel, for kernels that build their FileParams on the device (ap_rewalk_kernel, async_pages_kernels.cuh).  The
+// caller launches it as walk_kernel is launched: WALK_THREADS threads, sizeof(WalkSmem<CAP_LOG>) bytes of dynamic shared memory.
 template <int CAP_LOG>
-__global__ void __launch_bounds__(WALK_THREADS, PCOB_WALK_MIN_BLOCKS) walk_kernel(FileParams fp, uint8_t* index_base, uint64_t chunks_offset, uint32_t max_chunks,
-                                                   uint64_t entries_begin, uint64_t entries_cap_end, uint64_t first_chunk_byte,
-                                                   uint64_t first_out_offset, uint64_t stop_after_total, uint32_t* statuses, WalkResult* result,
-                                                   int serial_file_mode, uint64_t* chunk_ends = nullptr) {
+__device__ __forceinline__ void walk_run(FileParams fp, uint8_t* index_base, uint64_t chunks_offset, uint32_t max_chunks, uint64_t entries_begin,
+                                         uint64_t entries_cap_end, uint64_t first_chunk_byte, uint64_t first_out_offset, uint64_t stop_after_total,
+                                         uint32_t* statuses, WalkResult* result, int serial_file_mode, uint64_t* chunk_ends) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   WalkSmem<CAP_LOG>& sm = *reinterpret_cast<WalkSmem<CAP_LOG>*>(smem_raw);
   const BitSrc src = make_bitsrc(fp.src, fp.src_len);
@@ -523,6 +524,15 @@ __global__ void __launch_bounds__(WALK_THREADS, PCOB_WALK_MIN_BLOCKS) walk_kerne
     result->entries_end = entries_off;
     result->n_total = out_off - first_out_offset;
   }
+}
+
+template <int CAP_LOG>
+__global__ void __launch_bounds__(WALK_THREADS, PCOB_WALK_MIN_BLOCKS) walk_kernel(FileParams fp, uint8_t* index_base, uint64_t chunks_offset, uint32_t max_chunks,
+                                                   uint64_t entries_begin, uint64_t entries_cap_end, uint64_t first_chunk_byte,
+                                                   uint64_t first_out_offset, uint64_t stop_after_total, uint32_t* statuses, WalkResult* result,
+                                                   int serial_file_mode, uint64_t* chunk_ends = nullptr) {
+  walk_run<CAP_LOG>(fp, index_base, chunks_offset, max_chunks, entries_begin, entries_cap_end, first_chunk_byte, first_out_offset, stop_after_total,
+                    statuses, result, serial_file_mode, chunk_ends);
 }
 
 // ---------------------------------------------------------------------------

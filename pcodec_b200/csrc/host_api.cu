@@ -7,6 +7,7 @@
 #include "async_compress_files.cuh"
 #include "async_files_kernels.cuh"
 #include "async_kernels.cuh"
+#include "async_pages_kernels.cuh"
 #include "async_ranges_kernels.cuh"
 #include "compress_host.cuh"
 #include "decode_kernels.cuh"
@@ -2936,6 +2937,183 @@ PcoB200Error pco_b200_decompress_files_async_result(const PcoB200AsyncFilesStatu
     default:
       status_to_error(s->device_status, ("chunk " + std::to_string(s->chunk)).c_str());
       return file_fail(kind, f, last_error_ref());
+  }
+}
+
+// ---- asynchronous batch of wrapped pages (pco_b200_decompress_pages_async; kernels in async_pages_kernels.cuh)
+// The plan fixes every grid size (from max_pages) and the byte layout of the workspace; the refs and their count are read on the device.
+// A call is a fixed sequence of thirteen launches: pages, scan, place, frame_pages, walk, route, rewalk, fused, symwalk, decode<1>,
+// decode<2>, cold, finish.
+
+static bool ap_plan_ok(const PcoB200AsyncPagesPlan* p) {
+  return nt_valid(p->dtype) && p->max_pages >= 1 && p->max_pages <= 0x7fffffffull && p->dst_cap <= (uint64_t(1) << 56) &&
+         p->frame_cap <= (uint64_t(1) << 56) && p->workspace_bytes == ap_layout(p->max_pages, p->dst_cap, p->frame_cap).total;
+}
+
+PcoB200Error pco_b200_decompress_pages_async_plan(unsigned char dtype, size_t metas_cap, size_t pages_cap, size_t max_pages, size_t dst_cap,
+                                                  size_t frame_cap, PcoB200AsyncPagesPlan* plan) {
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (!plan) return fail(PCO_B200_INVALID_ARGUMENT, "null plan");
+  if (max_pages == 0 || uint64_t(max_pages) > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_pages must be 1 .. 2^31 - 1");
+  if (uint64_t(dst_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "dst_cap above 2^56 numbers");
+  if (uint64_t(frame_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "frame_cap above 2^56 bytes");
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->metas_cap = metas_cap;
+  plan->pages_cap = pages_cap;
+  plan->max_pages = max_pages;
+  plan->dst_cap = dst_cap;
+  plan->frame_cap = frame_cap;
+  plan->workspace_bytes = ap_layout(max_pages, dst_cap, frame_cap).total;
+  // the one-time device set-up, as in pco_b200_decompress_async_plan
+  Context& c = ctx();
+  if (PcoB200Error e = ensure_device(c)) return e;
+  if (PcoB200Error e = set_decode_attrs<false>(c)) return e;
+  cudaFuncAttributes fa;
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ap_pages_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ap_scan_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ap_place_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, frame_pages_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, walk_kernel<SMALL_MAX_SIZE_LOG>));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ap_route_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ap_rewalk_kernel));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, symwalk_kernel<false>));
+  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ap_finish_kernel));
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
+    using L = decltype(tag);
+    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, fused_narrow_kernel<L>));
+    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, decode_kernel<L, 1>));
+    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, decode_kernel<L, 2>));
+    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ap_cold_kernel<L>));
+    return PCO_B200_OK;
+  });
+}
+
+PcoB200Error pco_b200_decompress_pages_async(const PcoB200AsyncPagesPlan* plan, const void* metas, const void* pages, const PcoB200PageRef* refs,
+                                             const uint64_t* n_pages, void* dst, void* workspace, PcoB200AsyncPagesStatus* status, void* cuda_stream) {
+  if (!plan || !metas || !pages || !refs || !n_pages || !workspace || !status || (!dst && plan->dst_cap))
+    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (!ap_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_decompress_pages_async_plan");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  PCOB_CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
+  const bool prof = cap == cudaStreamCaptureStatusNone && profiler_enabled().load(std::memory_order_relaxed);
+  if (prof) profiler().discard();
+  auto begin = [&](const char* name) { if (prof) profiler().begin(name, stream); };
+  auto end = [&]() { if (prof) profiler().end(stream); };
+
+  const uint32_t mp = uint32_t(plan->max_pages);
+  const ApLayout lay = ap_layout(mp, plan->dst_cap, plan->frame_cap);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  AsyncCheck* chk = reinterpret_cast<AsyncCheck*>(ws);
+  ApState* state = reinterpret_cast<ApState*>(ws + lay.state);
+  WrappedPage* tab = reinterpret_cast<WrappedPage*>(ws + lay.tab);
+  uint8_t* d_idx = ws + lay.index;
+  IndexChunk* recs = reinterpret_cast<IndexChunk*>(d_idx);
+  uint8_t* d_frames = ws + lay.frames;
+  uint32_t* pstat = reinterpret_cast<uint32_t*>(ws + lay.pstat);
+  uint32_t* wst = reinterpret_cast<uint32_t*>(ws + lay.wst);
+  uint64_t* ends = reinterpret_cast<uint64_t*>(ws + lay.ends);
+  ApPart* parts = reinterpret_cast<ApPart*>(ws + lay.parts);
+  IndexChunk* table = reinterpret_cast<IndexChunk*>(ws + lay.table);
+  uint32_t* fast_page = reinterpret_cast<uint32_t*>(ws + lay.fast_page);
+  uint32_t* cold_list = reinterpret_cast<uint32_t*>(ws + lay.cold_list);
+  uint32_t* d_st = reinterpret_cast<uint32_t*>(ws + lay.st);
+  uint8_t* d_cls = ws + lay.cls;
+  uint8_t* d_syms = ws + lay.syms;
+  uint32_t* d_offs = reinterpret_cast<uint32_t*>(ws + lay.offs);
+  uint8_t* d_cold = ws + lay.cold;
+  ApArgs g;
+  g.metas = static_cast<const uint8_t*>(metas);
+  g.pages = static_cast<const uint8_t*>(pages);
+  g.refs = refs;
+  g.n_pages = n_pages;
+  g.metas_cap = plan->metas_cap;
+  g.pages_cap = plan->pages_cap;
+  g.dst_cap = plan->dst_cap;
+  g.frame_cap = plan->frame_cap;
+  g.dtype = plan->dtype;
+  g.max_pages = mp;
+  // the frames as one file: every page's frame below frame_cap, the pad frame behind them
+  const FileParams fp{d_frames, lay.pad_frame + 64, plan->dtype, 0, 4};
+  const uint32_t pb = uint32_t(ap_ctas(mp));
+
+  begin("ap_pages_kernel");
+  ap_pages_kernel<<<pb, AP_THREADS, 0, stream>>>(g, chk, parts);
+  end();
+  begin("ap_scan_kernel");
+  ap_scan_kernel<<<1, AP_SCAN_THREADS, 0, stream>>>(g, parts, state);
+  end();
+  begin("ap_place_kernel");
+  ap_place_kernel<<<pb, AP_THREADS, 0, stream>>>(g, parts, state, tab, recs, d_frames, lay.pad_frame, (uint64_t(mp) + 1) * sizeof(IndexChunk));
+  end();
+  begin("frame_pages_kernel");
+  frame_pages_kernel<<<mp, WRAP_THREADS, 0, stream>>>(g.metas, g.metas_cap, g.pages, g.dtype, tab, d_frames, pstat);
+  end();
+  begin("walk_kernel");
+  walk_kernel<SMALL_MAX_SIZE_LOG><<<mp, WALK_THREADS, sizeof(WalkSmem<SMALL_MAX_SIZE_LOG>), stream>>>(
+      fp, d_idx, 0, mp, 0, lay.index_len, 0, 0, ~uint64_t(0), wst, &state->walk, 0, ends);
+  end();
+  begin("ap_route_kernel");
+  ap_route_kernel<<<1, AP_SCAN_THREADS, 0, stream>>>(g, state, tab, recs, pstat, wst, ends, table, fast_page, cold_list, fp.src_len);
+  end();
+  begin("ap_rewalk_kernel");
+  ap_rewalk_kernel<<<1, WALK_THREADS, sizeof(WalkSmem<SMALL_MAX_SIZE_LOG>), stream>>>(g, state, tab, d_frames, d_idx, lay.index_len);
+  end();
+  begin("fused_narrow_kernel");
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    fused_narrow_kernel<L><<<mp, FZ_THREADS, sizeof(FusedSmem), stream>>>(fp, table, d_idx, lay.index_len, d_st, d_cls, static_cast<L*>(dst), g.dst_cap);
+    return 0;
+  });
+  end();
+  begin("symwalk_kernel");
+  symwalk_kernel<false><<<mp, SW_THREADS, sizeof(SymWalkSmem), stream>>>(fp, table, d_idx, lay.index_len, g.dst_cap, d_syms, d_offs, d_cls);
+  end();
+  begin("decode_kernel");
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    decode_kernel<L, 1><<<mp, DEC_THREADS, sizeof(DecodeSmem), stream>>>(fp, table, d_st, d_idx, lay.index_len, static_cast<L*>(dst), g.dst_cap, &chk->binoms,
+                                                                          d_syms, d_offs, d_cls);
+    decode_kernel<L, 2><<<mp, DEC_THREADS, sizeof(DecodeSmem), stream>>>(fp, table, d_st, d_idx, lay.index_len, static_cast<L*>(dst), g.dst_cap, &chk->binoms,
+                                                                          d_syms, d_offs, d_cls);
+    return 0;
+  });
+  end();
+  begin("ap_cold_kernel");
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    ap_cold_kernel<L><<<1, ASYNC_THREADS, 0, stream>>>(g, state, tab, recs, d_st, fast_page, cold_list, d_frames, static_cast<L*>(dst), d_cold);
+    return 0;
+  });
+  end();
+  begin("ap_finish_kernel");
+  ap_finish_kernel<<<1, 32, 0, stream>>>(state, status);
+  end();
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
+}
+
+PcoB200Error pco_b200_decompress_pages_async_result(const PcoB200AsyncPagesStatus* s, size_t* n_written) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200Error kind = s->kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(s->kind) : PCO_B200_CORRUPTION;
+  if (kind == PCO_B200_OK) {
+    if (n_written) *n_written = size_t(s->n_written);
+    return PCO_B200_OK;
+  }
+  const size_t p = size_t(s->page);
+  switch (s->device_status) {
+    case PCO_B200_ASYNC_TOO_MANY_PAGES: return fail(kind, "*n_pages is " + std::to_string(s->n_pages) + ", above the plan's max_pages");
+    case PCO_B200_ASYNC_META_OUTSIDE: return page_fail(kind, p, "chunk meta lies outside metas");
+    case PCO_B200_ASYNC_PAGE_OUTSIDE: return page_fail(kind, p, "page lies outside pages");
+    case PCO_B200_ASYNC_PAGE_N: return page_fail(kind, p, "page n must be 1..2^24");
+    case PCO_B200_ASYNC_PAGES_DST: return page_fail(kind, p, "dst holds fewer numbers than the pages up to this one");
+    case PCO_B200_ASYNC_FRAMES:
+      return fail(kind, "the framed pages need " + std::to_string(s->frames_needed) + " bytes, more than the plan's frame_cap");
+    default:
+      status_to_error(s->device_status, "the page");
+      return page_fail(kind, p, last_error_ref());
   }
 }
 
