@@ -694,6 +694,9 @@ PcoB200Error pco_b200_compress_files_async(const PcoB200AsyncCompressFilesPlan *
 /* Testing aid, host only: writes the standalone header for a size hint of n_hint (uniform_type 0, or the number type byte) into out (at
  * least 17 bytes) with the function the device framing uses, and returns its length (0 if the length the placement assumed differs). */
 size_t pco_b200_debug_standalone_header(uint64_t n_hint, unsigned char uniform_type, unsigned char *out);
+/* Testing aid, host only: the kind (a PcoB200Error) that the finish kernels of every asynchronous call write for device_status, a chunk's
+ * status or a PCO_B200_ASYNC_* code, from the one table they share. */
+unsigned pco_b200_debug_async_kind(unsigned device_status);
 /* Host only: the outcome of a call, from its status copied back to host memory at a point of the caller's choosing.  Returns the kind,
  * sets the last-error message as pco_b200_compress_files words it ("file 17: ...") and, when the kind is OK, sets *dst_len and *index_len
  * (either may be NULL) to the bytes written. */

@@ -188,3 +188,69 @@ def dtype_byte(dtype):
     if dt not in NP_TO_BYTE:
         raise TypeError(f"unsupported dtype {dt}")
     return NP_TO_BYTE[dt]
+
+
+def bind(flag, **argtypes):
+    """The library, with the argtypes of the named functions set the first time a binder asks (the library attribute `flag` marks it)."""
+    L = lib()
+    if not getattr(L, flag, False):
+        for name, types in argtypes.items():
+            getattr(L, name).argtypes = types
+        setattr(L, flag, True)
+    return L
+
+
+class _AsyncCall:
+    """What the wrappers of the asynchronous calls share: the device, the plan (a ctypes struct of class _Plan, made under that device),
+    the device workspace and the status (of class _Status) a call writes, the checks of the tensors a call takes and the stream it runs
+    on.  One call in flight at a time; calls on one stream queue up."""
+
+    _Plan = _Status = None
+
+    def _make_plan(self, device, plan_fn):
+        """Resolves the device and fills the plan with plan_fn(pointer to the plan), which returns the library's error code."""
+        import torch
+
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self._plan = self._Plan()
+        self._replan(plan_fn)
+
+    def _replan(self, plan_fn):
+        import torch
+
+        with torch.cuda.device(self.device):
+            rc = plan_fn(C.byref(self._plan))
+        check(rc)
+
+    def _alloc(self):
+        import torch
+
+        self.workspace = torch.empty(max(self._plan.workspace_bytes, 1), dtype=torch.uint8, device=self.device)
+        self.status = torch.zeros(C.sizeof(self._Status), dtype=torch.uint8, device=self.device)
+
+    @staticmethod
+    def _head(head):
+        """The first 32 bytes of a file (bytes, numpy or a tensor) as host memory."""
+        from .wrapped import _host_u8
+
+        if getattr(head, "is_cuda", False):
+            head = head.reshape(-1)[:32].cpu().numpy()
+        return _host_u8(head)[:32].copy()
+
+    def _check_tensors(self, **tensors):
+        for name, t in tensors.items():
+            if not getattr(t, "is_cuda", False) or t.device != self.device or not t.is_contiguous():
+                raise ValueError(f"{name} must be a contiguous CUDA tensor on {self.device}")
+
+    def _stream(self):
+        import torch
+
+        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    @property
+    def workspace_bytes(self):
+        return int(self._plan.workspace_bytes)
+
+    def status_record(self):
+        """The last call's status struct, copied back (waiting for it on the current stream)."""
+        return self._Status.from_buffer_copy(self.status.cpu().numpy().tobytes())

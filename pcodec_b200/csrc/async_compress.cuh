@@ -258,18 +258,17 @@ inline PcoB200Error acomp_check_plan(const PcoB200AsyncCompressPlan* p, AcompGeo
 
 template <typename L>
 void acomp_launch(const PcoB200AsyncCompressPlan& p, const AcompGeom& g, const AcompArgs& a, const void* nums, PcoB200AsyncCompressStatus* status,
-                         cudaStream_t stream, bool prof) {
-  auto begin = [&](const char* name) { if (prof) profiler().begin(name, stream); };
-  auto end = [&]() { if (prof) profiler().end(stream); };
+                         const AsyncLaunch& ln) {
+  const cudaStream_t stream = ln.stream;
   const uint32_t nc = uint32_t(g.n_chunks), bpc = g.bpc, tiles = g.tiles;
   constexpr uint32_t LBITS = sizeof(L) * 8;
   constexpr size_t RS_SMEM = size_t(RS_WARPS) * RS_BINS * sizeof(uint32_t);
   uint8_t* ws = a.ws;
   const AcompLayout& l = a.lay;
   const uint32_t init_ctas = uint32_t(std::min<uint64_t>(1024, std::max<uint64_t>({g.n_chunks + 1, g.n_chunks * MAX_VARS * bpc, a.index_bytes / 16}) / ACOMP_THREADS + 1));
-  begin("acomp_init_kernel");
+  ln.begin("acomp_init_kernel");
   acomp_init_kernel<<<init_ctas, ACOMP_THREADS, 0, stream>>>(a, bpc);
-  end();
+  ln.end();
   if (p.n > 0) {
     ChunkEnc* chunks = reinterpret_cast<ChunkEnc*>(ws + l.chunks);
     VarPlan* plans = reinterpret_cast<VarPlan*>(ws + l.plans);
@@ -310,20 +309,20 @@ void acomp_launch(const PcoB200AsyncCompressPlan& p, const AcompGeom& g, const A
     const uint32_t always_two = p.n_vars > 1 ? 1u : 0u;
     // ---- front end: the one-pass kernel for Classic, then the two-kernel path behind its flag (always, for the two-var modes)
     if (!always_two) {
-      begin("split_count_kernel");
+      ln.begin("split_count_kernel");
       split_count_kernel<L><<<nc, SC_THREADS, size_t(SC_N) * 4, stream>>>(ep, chunks, probes, key16[0], head->flags);
-      end();
+      ln.end();
     }
     acomp_two_gate_kernel<<<(nc + ACOMP_THREADS) / ACOMP_THREADS, ACOMP_THREADS, 0, stream>>>(a, always_two);
     const EncParams e_two = gated(0);
-    begin("split_delta_kernel");
+    ln.begin("split_delta_kernel");
     switch (p.mode) {
       case MODE_CLASSIC: split_delta_kernel<L, MODE_CLASSIC><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
       case MODE_INT_MULT: split_delta_kernel<L, MODE_INT_MULT><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
       case MODE_FLOAT_QUANT: split_delta_kernel<L, MODE_FLOAT_QUANT><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
       default: split_delta_kernel<L, MODE_FLOAT_MULT><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
     }
-    end();
+    ln.end();
     acomp_var_gate_kernel<<<1, 1024, 0, stream>>>(a, always_two);
     // ---- planner per var: counting probe or sort path (whichever the range bits gate on), then the solver on the probes either left
     // (the one-pass kernel writes var 0's probes itself).  The counting probe takes the counters of PLAN_MAX_COUNT_BITS and the sort all
@@ -332,62 +331,62 @@ void acomp_launch(const PcoB200AsyncCompressPlan& p, const AcompGeom& g, const A
     const L* sorted = ((LBITS + RS_BITS - 1) / RS_BITS) & 1 ? keys_b : keys_a;
     for (uint32_t v = 0; v < p.n_vars; v++) {
       const EncParams e_count = gated(1 + ACOMP_GATES_PER_VAR * v), e_sort = gated(2 + ACOMP_GATES_PER_VAR * v);
-      begin("plan_probe_kernel_counting");
+      ln.begin("plan_probe_kernel_counting");
       plan_probe_kernel<L, true><<<nc, PLAN_THREADS, ((size_t(1) << PLAN_MAX_COUNT_BITS) + 1) * 4 + 16, stream>>>(e_count, lat[v], chunks, probes, int(v),
                                                                                                                     PLAN_MAX_COUNT_BITS, key16[v]);
-      end();
-      begin("sort_keys_kernel");
+      ln.end();
+      ln.begin("sort_keys_kernel");
       sort_keys_kernel<L><<<nc * tiles, 256, 0, stream>>>(e_sort, tiles, lat[v], keys_a, chunks, int(v));
-      end();
+      ln.end();
       segment_offsets_kernel<<<(nc + 255) / 256, 256, 0, stream>>>(e_sort, v == 0 ? p.order : 0, seg_begin, seg_end);
-      begin("radix_sort_segments_kernel");
+      ln.begin("radix_sort_segments_kernel");
       radix_sort_segments_kernel<L><<<nc, RS_THREADS, RS_SMEM, stream>>>(keys_a, keys_b, seg_begin, seg_end, LBITS);
-      end();
-      begin("plan_probe_kernel_sorted");
+      ln.end();
+      ln.begin("plan_probe_kernel_sorted");
       plan_probe_kernel<L, false><<<nc, PLAN_THREADS, 16, stream>>>(e_sort, sorted, chunks, probes, int(v), LBITS, nullptr);
-      end();
-      begin("plan_solve_kernel");
+      ln.end();
+      ln.begin("plan_solve_kernel");
       plan_solve_kernel<L><<<nc, SOLVE_THREADS, 0, stream>>>(ep, probes, chunks, plans, int(v));
-      end();
+      ln.end();
     }
     fallback_kernel<false><<<(nc + 255) / 256, 256, 0, stream>>>(ep, plans, chunks, 0u);
     // ---- K3 per var: the lookup-table binning on the 16-bit keys, or the search over the 64-bit latents
     const uint32_t parts = (bpc + BINL_BATCHES - 1) / BINL_BATCHES, groups = (bpc + 7) / 8;
     for (uint32_t v = 0; v < p.n_vars; v++) {
-      begin("bin_lut_kernel");
+      ln.begin("bin_lut_kernel");
       bin_lut_kernel<L><<<nc * parts, BINL_THREADS, (size_t(1) << PLAN_MAX_COUNT_BITS) + 16, stream>>>(gated(3 + ACOMP_GATES_PER_VAR * v), bpc, parts, key16[v], plans,
                                                                                                       chunks, sym[v], ob_sum, int(v), PLAN_MAX_COUNT_BITS);
-      end();
-      begin("bin_kernel");
+      ln.end();
+      ln.begin("bin_kernel");
       bin_kernel<L, false><<<nc * groups, BIN_THREADS, 0, stream>>>(gated(4 + ACOMP_GATES_PER_VAR * v), bpc, lat[v], plans, chunks, sym[v], ob_sum, int(v));
-      end();
+      ln.end();
     }
-    begin("ans_encode_kernel");
+    ln.begin("ans_encode_kernel");
     ans_encode_kernel<false><<<nc * MAX_VARS, ANS_THREADS, 0, stream>>>(ep, bpc, plans, chunks, sym[0], sym[1], ans[0], ans[1], ans_sum, entries, nullptr);
-    end();
-    begin("layout_kernel");
+    ln.end();
+    ln.begin("layout_kernel");
     layout_kernel<false><<<nc, LAYOUT_THREADS, 0, stream>>>(ep, bpc, plans, chunks, ans_sum, ob_sum, entries);
-    end();
+    ln.end();
     chunk_offsets_kernel<<<1, 1024, 0, stream>>>(chunks, nc, a.header_bytes, 1u, &head->total);
     // ---- K5: one launch per choice of keys or latents; only the one the range bits made finds its chunks inside dst_cap
     const uint64_t n_copies = uint64_t(1) << p.n_vars;
     acomp_pack_gate_kernel<<<uint32_t(std::min<uint64_t>(1024, (n_copies * g.n_chunks + ACOMP_THREADS - 1) / ACOMP_THREADS)), ACOMP_THREADS, 0, stream>>>(a);
     const uint64_t out_cap = std::min<uint64_t>(p.dst_cap, ~uint64_t(0) - 1);
-    begin("pack_kernel");
+    ln.begin("pack_kernel");
     for (uint64_t k = 0; k < n_copies; k++) {
       const ChunkEnc* copy = reinterpret_cast<const ChunkEnc*>(ws + l.copies) + k * g.n_chunks;
       pack_kernel<L><<<nc, PACK_THREADS, sizeof(PackSmem), stream>>>(ep, bpc, lat[0], lat[1], plans, copy, sym[0], sym[1], ans[0], ans[1], entries, a.dst, out_cap,
                                                                      (k & 1) ? nullptr : key16[0], (p.n_vars > 1 && !(k & 2)) ? key16[1] : nullptr);
     }
-    end();
+    ln.end();
     header_footer_kernel<<<1, 32, 0, stream>>>(a.dst, out_cap, ws + 64, a.header_bytes, &head->total);
     if (a.index_bytes)
       emit_index_kernel<<<nc, 256, 0, stream>>>(ep, bpc, chunks, entries, a.index, sizeof(IndexHeader), reinterpret_cast<const uint64_t*>(ws + l.eoff), &head->total,
                                                 1u, 0u, 0, 1u);
   }
-  begin("acomp_finish_kernel");
+  ln.begin("acomp_finish_kernel");
   acomp_finish_kernel<<<1, 32, 0, stream>>>(a, status);
-  end();
+  ln.end();
 }
 
 }  // namespace pcob200

@@ -34,15 +34,6 @@ constexpr int ACF_SCAN_THREADS = 1024;  // the one-CTA launches
 constexpr int ACF_INDEX_THREADS = 128;
 enum { ACF_NUMS = 0, ACF_CHUNKS, ACF_ROWS, ACF_FRAME, ACF_IDX, ACF_SUMS };
 
-// the PcoB200Error kind of a device_status of this call
-__host__ __device__ inline uint32_t acf_kind_of(uint32_t st) {
-  switch (st) {
-    case PCO_B200_ASYNC_TOO_MANY_FILES: case PCO_B200_ASYNC_FILE_TOO_LARGE: case PCO_B200_ASYNC_NUMS_CAP: return PCO_B200_INVALID_ARGUMENT;
-    case PCO_B200_ASYNC_FILES_DST_FULL: case PCO_B200_ASYNC_FILES_INDEX_FULL: return PCO_B200_IO;
-    default: return PCO_B200_CORRUPTION;
-  }
-}
-
 // standalone_header_into's length for a size hint of n
 __host__ __device__ inline uint32_t standalone_header_len(uint64_t n) {
   uint32_t power = 1;
@@ -426,7 +417,7 @@ __global__ void acf_finish_kernel(AcfArgs g, PcoB200AsyncCompressFilesStatus* __
       s.device_status = st->dst_bytes > g.a.dst_cap ? uint32_t(PCO_B200_ASYNC_FILES_DST_FULL) : uint32_t(PCO_B200_ASYNC_FILES_INDEX_FULL);
     }
   }
-  s.kind = s.device_status == 0 ? uint32_t(PCO_B200_OK) : acf_kind_of(s.device_status);
+  s.kind = async_kind_of(s.device_status);
   *out = s;
 }
 
@@ -460,9 +451,8 @@ inline PcoB200Error acf_check_plan(const PcoB200AsyncCompressFilesPlan* p, AcfPl
 
 template <typename L>
 void acf_launch(const PcoB200AsyncCompressFilesPlan& p, const AcompGeom& g, const AcfArgs& fa, const void* nums, PcoB200AsyncCompressFilesStatus* status,
-                cudaStream_t stream, bool prof) {
-  auto begin = [&](const char* name) { if (prof) profiler().begin(name, stream); };
-  auto end = [&]() { if (prof) profiler().end(stream); };
+                const AsyncLaunch& ln) {
+  const cudaStream_t stream = ln.stream;
   const AcompArgs& a = fa.a;
   const uint32_t nc = uint32_t(g.n_chunks), bpc = g.bpc, tiles = g.tiles;
   constexpr uint32_t LBITS = sizeof(L) * 8;
@@ -470,19 +460,19 @@ void acf_launch(const PcoB200AsyncCompressFilesPlan& p, const AcompGeom& g, cons
   uint8_t* ws = a.ws;
   const AcompLayout& l = a.lay;
   const uint32_t file_ctas = uint32_t(acf_ctas(p.max_files)), chunk_ctas = uint32_t(acf_ctas(g.n_chunks + 1));
-  begin("acf_files_kernel");
+  ln.begin("acf_files_kernel");
   acf_files_kernel<<<file_ctas, ACF_THREADS, 0, stream>>>(fa);
-  end();
-  begin("acf_scan_kernel");
+  ln.end();
+  ln.begin("acf_scan_kernel");
   acf_scan_kernel<<<1, ACF_SCAN_THREADS, 0, stream>>>(fa);
-  end();
-  begin("acf_place_kernel");
+  ln.end();
+  ln.begin("acf_place_kernel");
   acf_place_kernel<<<file_ctas, ACF_THREADS, 0, stream>>>(fa);
-  end();
+  ln.end();
   const uint32_t init_ctas = uint32_t(std::min<uint64_t>(1024, std::max<uint64_t>(g.n_chunks + 1, g.n_chunks * MAX_VARS * bpc) / ACF_THREADS + 1));
-  begin("acf_init_kernel");
+  ln.begin("acf_init_kernel");
   acf_init_kernel<<<init_ctas, ACF_THREADS, 0, stream>>>(fa);
-  end();
+  ln.end();
   ChunkEnc* chunks = reinterpret_cast<ChunkEnc*>(ws + l.chunks);
   VarPlan* plans = reinterpret_cast<VarPlan*>(ws + l.plans);
   PlanProbes* probes = reinterpret_cast<PlanProbes*>(ws + l.probes);
@@ -521,91 +511,91 @@ void acf_launch(const PcoB200AsyncCompressFilesPlan& p, const AcompGeom& g, cons
   const uint32_t always_two = p.n_vars > 1 ? 1u : 0u;
   // ---- the encode kernels, as acomp_launch runs them
   if (!always_two) {
-    begin("split_count_kernel");
+    ln.begin("split_count_kernel");
     split_count_kernel<L, true><<<nc, SC_THREADS, size_t(SC_N) * 4, stream>>>(ep, chunks, probes, key16[0], head->flags);
-    end();
+    ln.end();
   }
   acomp_two_gate_kernel<<<(nc + ACOMP_THREADS) / ACOMP_THREADS, ACOMP_THREADS, 0, stream>>>(a, always_two);
   const EncParams e_two = gated(0);
-  begin("split_delta_kernel");
+  ln.begin("split_delta_kernel");
   switch (p.mode) {
     case MODE_CLASSIC: split_delta_kernel<L, MODE_CLASSIC><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
     case MODE_INT_MULT: split_delta_kernel<L, MODE_INT_MULT><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
     case MODE_FLOAT_QUANT: split_delta_kernel<L, MODE_FLOAT_QUANT><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
     default: split_delta_kernel<L, MODE_FLOAT_MULT><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
   }
-  end();
+  ln.end();
   acomp_var_gate_kernel<<<1, 1024, 0, stream>>>(a, always_two);
   const L* sorted = ((LBITS + RS_BITS - 1) / RS_BITS) & 1 ? keys_b : keys_a;
   for (uint32_t v = 0; v < p.n_vars; v++) {
     const EncParams e_count = gated(1 + ACOMP_GATES_PER_VAR * v), e_sort = gated(2 + ACOMP_GATES_PER_VAR * v);
-    begin("plan_probe_kernel_counting");
+    ln.begin("plan_probe_kernel_counting");
     plan_probe_kernel<L, true, false, true><<<nc, PLAN_THREADS, ((size_t(1) << PLAN_MAX_COUNT_BITS) + 1) * 4 + 16, stream>>>(
         e_count, lat[v], chunks, probes, int(v), PLAN_MAX_COUNT_BITS, key16[v]);
-    end();
-    begin("sort_keys_kernel");
+    ln.end();
+    ln.begin("sort_keys_kernel");
     sort_keys_kernel<L><<<nc * tiles, 256, 0, stream>>>(e_sort, tiles, lat[v], keys_a, chunks, int(v));
-    end();
+    ln.end();
     segment_offsets_kernel<<<(nc + 255) / 256, 256, 0, stream>>>(e_sort, v == 0 ? p.order : 0, seg_begin, seg_end);
-    begin("radix_sort_segments_kernel");
+    ln.begin("radix_sort_segments_kernel");
     radix_sort_segments_kernel<L><<<nc, RS_THREADS, RS_SMEM, stream>>>(keys_a, keys_b, seg_begin, seg_end, LBITS);
-    end();
-    begin("plan_probe_kernel_sorted");
+    ln.end();
+    ln.begin("plan_probe_kernel_sorted");
     plan_probe_kernel<L, false, false, true><<<nc, PLAN_THREADS, 16, stream>>>(e_sort, sorted, chunks, probes, int(v), LBITS, nullptr);
-    end();
-    begin("plan_solve_kernel");
+    ln.end();
+    ln.begin("plan_solve_kernel");
     plan_solve_kernel<L, true><<<nc, SOLVE_THREADS, 0, stream>>>(ep, probes, chunks, plans, int(v));
-    end();
+    ln.end();
   }
   fallback_kernel<false><<<(nc + 255) / 256, 256, 0, stream>>>(ep, plans, chunks, 0u);
   const uint32_t parts = (bpc + BINL_BATCHES - 1) / BINL_BATCHES, groups = (bpc + 7) / 8;
   for (uint32_t v = 0; v < p.n_vars; v++) {
-    begin("bin_lut_kernel");
+    ln.begin("bin_lut_kernel");
     bin_lut_kernel<L><<<nc * parts, BINL_THREADS, (size_t(1) << PLAN_MAX_COUNT_BITS) + 16, stream>>>(gated(3 + ACOMP_GATES_PER_VAR * v), bpc, parts, key16[v], plans,
                                                                                                     chunks, sym[v], ob_sum, int(v), PLAN_MAX_COUNT_BITS);
-    end();
-    begin("bin_kernel");
+    ln.end();
+    ln.begin("bin_kernel");
     bin_kernel<L, false><<<nc * groups, BIN_THREADS, 0, stream>>>(gated(4 + ACOMP_GATES_PER_VAR * v), bpc, lat[v], plans, chunks, sym[v], ob_sum, int(v));
-    end();
+    ln.end();
   }
-  begin("ans_encode_kernel");
+  ln.begin("ans_encode_kernel");
   ans_encode_kernel<false><<<nc * MAX_VARS, ANS_THREADS, 0, stream>>>(ep, bpc, plans, chunks, sym[0], sym[1], ans[0], ans[1], ans_sum, entries, nullptr);
-  end();
-  begin("layout_kernel");
+  ln.end();
+  ln.begin("layout_kernel");
   layout_kernel<false><<<nc, LAYOUT_THREADS, 0, stream>>>(ep, bpc, plans, chunks, ans_sum, ob_sum, entries);
-  end();
+  ln.end();
   // ---- placement: every chunk's final place in dst, behind its file's header
-  begin("acf_bytes_kernel");
+  ln.begin("acf_bytes_kernel");
   acf_bytes_kernel<<<chunk_ctas, ACF_THREADS, 0, stream>>>(fa);
-  end();
-  begin("acf_bytes_scan_kernel");
+  ln.end();
+  ln.begin("acf_bytes_scan_kernel");
   acf_bytes_scan_kernel<<<1, ACF_SCAN_THREADS, 0, stream>>>(fa);
-  end();
-  begin("acf_offsets_kernel");
+  ln.end();
+  ln.begin("acf_offsets_kernel");
   acf_offsets_kernel<<<chunk_ctas, ACF_THREADS, 0, stream>>>(fa);
-  end();
+  ln.end();
   const uint64_t n_copies = uint64_t(1) << p.n_vars;
   acomp_pack_gate_kernel<<<uint32_t(std::min<uint64_t>(1024, (n_copies * g.n_chunks + ACOMP_THREADS - 1) / ACOMP_THREADS)), ACOMP_THREADS, 0, stream>>>(a);
   const uint64_t out_cap = std::min<uint64_t>(p.dst_cap, ~uint64_t(0) - 1);
-  begin("pack_kernel");
+  ln.begin("pack_kernel");
   for (uint64_t k = 0; k < n_copies; k++) {
     const ChunkEnc* copy = reinterpret_cast<const ChunkEnc*>(ws + l.copies) + k * g.n_chunks;
     pack_kernel<L><<<nc, PACK_THREADS, sizeof(PackSmem), stream>>>(ep, bpc, lat[0], lat[1], plans, copy, sym[0], sym[1], ans[0], ans[1], entries, a.dst, out_cap,
                                                                    (k & 1) ? nullptr : key16[0], (p.n_vars > 1 && !(k & 2)) ? key16[1] : nullptr);
   }
-  end();
+  ln.end();
   // ---- framing
-  begin("acf_frame_kernel");
+  ln.begin("acf_frame_kernel");
   acf_frame_kernel<<<file_ctas, ACF_THREADS, 0, stream>>>(fa);
-  end();
+  ln.end();
   if (a.index) {
-    begin("acf_index_kernel");
+    ln.begin("acf_index_kernel");
     acf_index_kernel<<<nc, ACF_INDEX_THREADS, 0, stream>>>(fa);
-    end();
+    ln.end();
   }
-  begin("acf_finish_kernel");
+  ln.begin("acf_finish_kernel");
   acf_finish_kernel<<<1, 32, 0, stream>>>(fa, status);
-  end();
+  ln.end();
 }
 
 }  // namespace pcob200

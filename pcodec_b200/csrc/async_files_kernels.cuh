@@ -56,13 +56,12 @@ struct AfArgs {
 
 // Workspace of one in-flight call, byte offsets, each region 256-byte aligned:
 // AsyncCheck (binomials, chunk count) | AfState | per file: status, FileCheck, verdict, FileMerge | CTA sums | IndexChunk[max_chunks] |
-// statuses | class bytes | the general pair's symbol and offset rows | the catch-all decoder's scratch.
-struct AfLayout {
-  uint64_t state, fst, fchk, verdict, merges, parts, table, st, cls, syms, offs, cold, total;
+// the decode tail.
+struct AfLayout : AsyncDecodeTail {
+  uint64_t state, fst, fchk, verdict, merges, parts, table;
 };
 __host__ __device__ inline uint64_t af_ctas(uint64_t n) { return (n + AF_THREADS - 1) / AF_THREADS; }
 __host__ __device__ inline AfLayout af_layout(uint64_t max_files, uint64_t max_chunks, uint64_t dst_cap) {
-  const uint64_t rows = scratch_rows_total(dst_cap, uint32_t(max_chunks));
   AfLayout l;
   l.state = async_align(sizeof(AsyncCheck));
   l.fst = l.state + async_align(sizeof(AfState));
@@ -71,24 +70,9 @@ __host__ __device__ inline AfLayout af_layout(uint64_t max_files, uint64_t max_c
   l.merges = l.verdict + async_align(max_files * sizeof(uint32_t));
   l.parts = l.merges + async_align(max_files * sizeof(FileMerge));
   l.table = l.parts + async_align(af_ctas(max_files) * sizeof(AfPart));
-  l.st = l.table + async_align(max_chunks * sizeof(IndexChunk));
-  l.cls = l.st + async_align(max_chunks * sizeof(uint32_t));
-  l.syms = l.cls + async_align(max_chunks);
-  l.offs = l.syms + async_align(rows * BATCH_N);
-  l.cold = l.offs + async_align(rows * sizeof(uint32_t));
-  l.total = l.cold + async_align(cold_scratch_bytes(ASYNC_COLD_WINDOW_LOG));
+  static_cast<AsyncDecodeTail&>(l) =
+      async_decode_tail(l.table + async_align(max_chunks * sizeof(IndexChunk)), max_chunks, scratch_rows_total(dst_cap, uint32_t(max_chunks)), 0);
   return l;
-}
-
-// the PcoB200Error kind of a status word of this call
-__host__ __device__ inline uint32_t af_kind_of(uint32_t st) {
-  switch (st) {
-    case PCO_B200_ASYNC_TOO_MANY_FILES: case PCO_B200_ASYNC_FILE_OUTSIDE: case PCO_B200_ASYNC_INDEX_OFFSET: case PCO_B200_ASYNC_INDEX_OUTSIDE:
-    case PCO_B200_ASYNC_ENTRIES_MISALIGNED: case PCO_B200_ASYNC_RECORDS_OUTSIDE: return PCO_B200_INVALID_ARGUMENT;
-    case PCO_B200_ASYNC_NO_INDEX: return PCO_B200_UNSUPPORTED;
-    case PCO_B200_ASYNC_FILES_DST: return PCO_B200_IO;
-    default: return async_kind_of(st);
-  }
 }
 
 __device__ __forceinline__ uint64_t af_n_files(const AfArgs& g) {
@@ -301,12 +285,12 @@ __global__ void __launch_bounds__(AF_SCAN_THREADS) af_finish_kernel(const AfStat
       else b = m;
     }
     const uint32_t st = statuses[s_min];
-    r.kind = af_kind_of(st);
+    r.kind = async_kind_of(st);
     r.device_status = st;
     r.file = a;
     r.chunk = s_min - merges[a].list_at;
   } else if (pending != ST_OK) {
-    r.kind = af_kind_of(pending);
+    r.kind = async_kind_of(pending);
     r.device_status = pending;
     if (pending != PCO_B200_ASYNC_TOO_MANY_FILES) r.file = state->bad >> 32;
   }

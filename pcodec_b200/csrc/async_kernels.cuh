@@ -35,32 +35,52 @@ struct AsyncArgs {
   uint32_t max_chunks;
 };
 
-// Workspace of one in-flight call: AsyncCheck | IndexChunk[max_chunks] | statuses | class bytes | the general pair's symbol and offset
-// rows | the catch-all decoder's scratch.  Byte offsets, each region 256-byte aligned.
-struct AsyncLayout {
-  uint64_t table, st, cls, syms, offs, cold, total;
+// The regions every asynchronous decompress workspace ends with, from byte offset `at`: the statuses and class bytes of `slots` decode
+// slots | the general pair's `rows` symbol and offset rows | `stage_bytes` of staging (none but the ranges call's) | the catch-all
+// decoder's scratch.  Byte offsets, each region 256-byte aligned.
+struct AsyncDecodeTail {
+  uint64_t st, cls, syms, offs, stage, cold, total;
 };
 __host__ __device__ inline uint64_t async_align(uint64_t x) { return (x + 255) & ~uint64_t(255); }
+__host__ __device__ inline AsyncDecodeTail async_decode_tail(uint64_t at, uint64_t slots, uint64_t rows, uint64_t stage_bytes) {
+  AsyncDecodeTail t;
+  t.st = at;
+  t.cls = t.st + async_align(slots * sizeof(uint32_t));
+  t.syms = t.cls + async_align(slots);
+  t.offs = t.syms + async_align(rows * BATCH_N);
+  t.stage = t.offs + async_align(rows * sizeof(uint32_t));
+  t.cold = t.stage + async_align(stage_bytes);
+  t.total = t.cold + async_align(cold_scratch_bytes(ASYNC_COLD_WINDOW_LOG));
+  return t;
+}
+
+// Workspace of one in-flight call: AsyncCheck | IndexChunk[max_chunks] | the decode tail.
+struct AsyncLayout : AsyncDecodeTail {
+  uint64_t table;
+};
 __host__ __device__ inline AsyncLayout async_layout(uint64_t dst_cap, uint32_t max_chunks) {
-  const uint64_t rows = scratch_rows_total(dst_cap, max_chunks);
   AsyncLayout l;
   l.table = async_align(sizeof(AsyncCheck));
-  l.st = l.table + async_align(uint64_t(max_chunks) * sizeof(IndexChunk));
-  l.cls = l.st + async_align(uint64_t(max_chunks) * sizeof(uint32_t));
-  l.syms = l.cls + async_align(max_chunks);
-  l.offs = l.syms + async_align(rows * BATCH_N);
-  l.cold = l.offs + async_align(rows * sizeof(uint32_t));
-  l.total = l.cold + async_align(cold_scratch_bytes(ASYNC_COLD_WINDOW_LOG));
+  static_cast<AsyncDecodeTail&>(l) =
+      async_decode_tail(l.table + async_align(uint64_t(max_chunks) * sizeof(IndexChunk)), max_chunks, scratch_rows_total(dst_cap, max_chunks), 0);
   return l;
 }
 
-// the PcoB200Error kind of a chunk status or file-level refusal (status_to_error, host_common.hpp)
+// The PcoB200Error kind of a chunk status (as status_to_error, host_common.hpp, gives it) or of any PCO_B200_ASYNC_* code (as its comment
+// in pco_b200.h states it).  Every asynchronous call's status goes through this one table; the codes of the calls are disjoint.
 __host__ __device__ inline uint32_t async_kind_of(uint32_t st) {
   switch (st) {
     case ST_OK: return PCO_B200_OK;
     case ST_INSUFFICIENT_DATA: case PCO_B200_ASYNC_HEADER_SHORT: return PCO_B200_INSUFFICIENT_DATA;
-    case ST_INVALID_ARGUMENT: case PCO_B200_ASYNC_HEADER_MISMATCH: case PCO_B200_ASYNC_INDEX_FOREIGN: case PCO_B200_ASYNC_TOO_MANY_CHUNKS: return PCO_B200_INVALID_ARGUMENT;
-    case ST_UNSUPPORTED: return PCO_B200_UNSUPPORTED;
+    case ST_INVALID_ARGUMENT: case PCO_B200_ASYNC_HEADER_MISMATCH: case PCO_B200_ASYNC_INDEX_FOREIGN: case PCO_B200_ASYNC_TOO_MANY_CHUNKS:
+    case PCO_B200_ASYNC_INDEX_TILING: case PCO_B200_ASYNC_INDEX_TOTAL: case PCO_B200_ASYNC_TOO_MANY_RANGES: case PCO_B200_ASYNC_RANGE_PAST:
+    case PCO_B200_ASYNC_RANGE_OVERFLOW: case PCO_B200_ASYNC_DST_SHORT: case PCO_B200_ASYNC_TOO_MANY_FILES: case PCO_B200_ASYNC_FILE_OUTSIDE:
+    case PCO_B200_ASYNC_INDEX_OFFSET: case PCO_B200_ASYNC_INDEX_OUTSIDE: case PCO_B200_ASYNC_ENTRIES_MISALIGNED: case PCO_B200_ASYNC_RECORDS_OUTSIDE:
+    case PCO_B200_ASYNC_FILE_TOO_LARGE: case PCO_B200_ASYNC_NUMS_CAP: case PCO_B200_ASYNC_TOO_MANY_PAGES: case PCO_B200_ASYNC_META_OUTSIDE:
+    case PCO_B200_ASYNC_PAGE_OUTSIDE: case PCO_B200_ASYNC_PAGE_N: case PCO_B200_ASYNC_PAGES_DST: return PCO_B200_INVALID_ARGUMENT;
+    case PCO_B200_ASYNC_DST_FULL: case PCO_B200_ASYNC_WINDOW: case PCO_B200_ASYNC_FILES_DST: case PCO_B200_ASYNC_FILES_DST_FULL:
+    case PCO_B200_ASYNC_FILES_INDEX_FULL: case PCO_B200_ASYNC_FRAMES: return PCO_B200_IO;
+    case ST_UNSUPPORTED: case PCO_B200_ASYNC_NO_INDEX: return PCO_B200_UNSUPPORTED;
     default: return PCO_B200_CORRUPTION;
   }
 }
@@ -193,7 +213,7 @@ __global__ void __launch_bounds__(ASYNC_THREADS) cold_chunks_kernel(FileParams f
         if (rec.out_offset < out_len) {
           ColdResult res;
           cold_decode_run<L>(fp, rec.chunk_offset, out + rec.out_offset, min(uint64_t(rec.n), out_len - rec.out_offset), scratch, ASYNC_COLD_WINDOW_LOG, &res);
-          st = res.n_chunks > 0 ? uint32_t(ST_OK) : (res.status == ST_OK || res.status == ST_TERMINATOR || res.status == ST_DST_FULL) ? uint32_t(ST_CORRUPTION) : res.status;
+          st = cold_status(res);
         }
         statuses[c] = st;
       }

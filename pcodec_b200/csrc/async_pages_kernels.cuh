@@ -60,17 +60,15 @@ struct ApArgs {
 
 // Workspace of one in-flight call, byte offsets, each region 256-byte aligned:
 // AsyncCheck (binomials) | ApState | WrappedPage[max_pages] | IndexChunk[max_pages + 1] and the batch entries | frames and a pad frame |
-// per page: meta status, walk status, walk end | CTA sums | decode table | its pages | cold list | decode statuses | class bytes | the
-// general pair's symbol and offset rows | the catch-all decoder's scratch.
-struct ApLayout {
-  uint64_t state, tab, index, index_len, frames, pad_frame, pstat, wst, ends, parts, table, fast_page, cold_list, st, cls, syms, offs, cold, total;
+// per page: meta status, walk status, walk end | CTA sums | decode table | its pages | cold list | the decode tail.
+struct ApLayout : AsyncDecodeTail {
+  uint64_t state, tab, index, index_len, frames, pad_frame, pstat, wst, ends, parts, table, fast_page, cold_list;
 };
 __host__ __device__ inline uint64_t ap_ctas(uint64_t n) { return (n + AP_THREADS - 1) / AP_THREADS; }
 // Batch entries of an accepted batch: each page's entries_room (16-byte aligned room for MAX_VARS x ceil(n / 256) entries of 12 bytes)
 // is at most 24 floor(n / 256) + 32 bytes, and the pages hold at most dst_cap numbers.
 __host__ __device__ inline uint64_t ap_entries_bound(uint64_t max_pages, uint64_t dst_cap) { return 24 * (dst_cap / BATCH_N) + 32 * max_pages; }
 __host__ __device__ inline ApLayout ap_layout(uint64_t max_pages, uint64_t dst_cap, uint64_t frame_cap) {
-  const uint64_t rows = scratch_rows_total(dst_cap, uint32_t(max_pages));
   ApLayout l;
   l.state = async_align(sizeof(AsyncCheck));
   l.tab = l.state + async_align(sizeof(ApState));
@@ -85,23 +83,9 @@ __host__ __device__ inline ApLayout ap_layout(uint64_t max_pages, uint64_t dst_c
   l.table = l.parts + async_align(ap_ctas(max_pages) * sizeof(ApPart));
   l.fast_page = l.table + async_align(max_pages * sizeof(IndexChunk));
   l.cold_list = l.fast_page + async_align(max_pages * sizeof(uint32_t));
-  l.st = l.cold_list + async_align(max_pages * sizeof(uint32_t));
-  l.cls = l.st + async_align(max_pages * sizeof(uint32_t));
-  l.syms = l.cls + async_align(max_pages);
-  l.offs = l.syms + async_align(rows * BATCH_N);
-  l.cold = l.offs + async_align(rows * sizeof(uint32_t));
-  l.total = l.cold + async_align(cold_scratch_bytes(ASYNC_COLD_WINDOW_LOG));
+  static_cast<AsyncDecodeTail&>(l) =
+      async_decode_tail(l.cold_list + async_align(max_pages * sizeof(uint32_t)), max_pages, scratch_rows_total(dst_cap, uint32_t(max_pages)), 0);
   return l;
-}
-
-// the PcoB200Error kind of a status word of this call
-__host__ __device__ inline uint32_t ap_kind_of(uint32_t st) {
-  switch (st) {
-    case PCO_B200_ASYNC_TOO_MANY_PAGES: case PCO_B200_ASYNC_META_OUTSIDE: case PCO_B200_ASYNC_PAGE_OUTSIDE: case PCO_B200_ASYNC_PAGE_N:
-    case PCO_B200_ASYNC_PAGES_DST: return PCO_B200_INVALID_ARGUMENT;
-    case PCO_B200_ASYNC_FRAMES: return PCO_B200_IO;
-    default: return async_kind_of(st);
-  }
 }
 
 __device__ __forceinline__ uint64_t ap_n_pages(const ApArgs& g) {
@@ -378,8 +362,7 @@ __global__ void __launch_bounds__(ASYNC_THREADS) ap_cold_kernel(ApArgs g, ApStat
     ColdResult res;
     cold_decode_run<L>(fp, 0, out + recs[p].out_offset, w.page_n, scratch, ASYNC_COLD_WINDOW_LOG, &res);
     if (res.n_chunks == 0) {  // the page is decoded once its chunk is (what the decoder reads behind it is not the page's)
-      const uint32_t st = (res.status == ST_OK || res.status == ST_TERMINATOR || res.status == ST_DST_FULL) ? uint32_t(ST_CORRUPTION) : res.status;
-      fail = (uint64_t(p) << 32) | st;
+      fail = (uint64_t(p) << 32) | cold_status(res);
       break;
     }
   }
@@ -400,7 +383,7 @@ __global__ void __launch_bounds__(32) ap_finish_kernel(const ApState* __restrict
   r.n_pages = s.n_read;
   r.frames_needed = refs_ok || s.status == PCO_B200_ASYNC_PAGES_DST ? (s.frames.ovf ? AR_NONE64 : s.frames.s) : 0;
   if (s.status != ST_OK) {
-    r.kind = ap_kind_of(s.status);
+    r.kind = async_kind_of(s.status);
     r.device_status = s.status;
     r.n_written = 0;
     if (s.status != PCO_B200_ASYNC_TOO_MANY_PAGES && s.status != PCO_B200_ASYNC_FRAMES) r.page = s.bad >> 32;
@@ -413,7 +396,7 @@ __global__ void __launch_bounds__(32) ap_finish_kernel(const ApState* __restrict
       r.page = s.decode_fail >> 32;
       st = uint32_t(s.decode_fail);
     }
-    r.kind = ap_kind_of(st);
+    r.kind = async_kind_of(st);
     r.device_status = st;
     r.n_written = 0;
   }

@@ -85,9 +85,10 @@ struct ArArgs {
   uint32_t elem;          // bytes per number
 };
 
-// Workspace of one in-flight call, byte offsets, each region 256-byte aligned.
-struct ArLayout {
-  uint64_t state, table, marks, cparts, rparts, roff, rspan, tasks, wins, tinfo, st, cls, syms, offs, stage, cold, total;
+// Workspace of one in-flight call, byte offsets, each region 256-byte aligned; the decode tail stages the window between the offset rows
+// and the catch-all decoder's scratch.
+struct ArLayout : AsyncDecodeTail {
+  uint64_t state, table, marks, cparts, rparts, roff, rspan, tasks, wins, tinfo;
 };
 __host__ __device__ inline uint64_t ar_ctas(uint64_t n) { return (n + AR_THREADS - 1) / AR_THREADS; }
 __host__ __device__ inline uint64_t ar_rows(uint64_t window_cap) { return 2 * (window_cap / BATCH_N); }
@@ -103,24 +104,9 @@ __host__ __device__ inline ArLayout ar_layout(uint64_t max_chunks, uint64_t max_
   l.tasks = l.rspan + async_align(max_ranges * sizeof(uint2));
   l.wins = l.tasks + async_align(max_chunks * sizeof(IndexChunk));
   l.tinfo = l.wins + async_align(max_chunks * sizeof(WinTask));
-  l.st = l.tinfo + async_align(max_chunks * sizeof(ArTask));
-  l.cls = l.st + async_align(max_chunks * sizeof(uint32_t));
-  l.syms = l.cls + async_align(max_chunks);
-  l.offs = l.syms + async_align(ar_rows(window_cap) * BATCH_N);
-  l.stage = l.offs + async_align(ar_rows(window_cap) * sizeof(uint32_t));
-  l.cold = l.stage + async_align(window_cap * elem);
-  l.total = l.cold + async_align(cold_scratch_bytes(ASYNC_COLD_WINDOW_LOG));
+  static_cast<AsyncDecodeTail&>(l) =
+      async_decode_tail(l.tinfo + async_align(max_chunks * sizeof(ArTask)), max_chunks, ar_rows(window_cap), window_cap * elem);
   return l;
-}
-
-// the PcoB200Error kind of a status word of this call
-__host__ __device__ inline uint32_t ar_kind_of(uint32_t st) {
-  switch (st) {
-    case PCO_B200_ASYNC_INDEX_TILING: case PCO_B200_ASYNC_INDEX_TOTAL: case PCO_B200_ASYNC_TOO_MANY_RANGES: case PCO_B200_ASYNC_RANGE_PAST:
-    case PCO_B200_ASYNC_RANGE_OVERFLOW: case PCO_B200_ASYNC_DST_SHORT: return PCO_B200_INVALID_ARGUMENT;
-    case PCO_B200_ASYNC_WINDOW: return PCO_B200_IO;
-    default: return async_kind_of(st);
-  }
 }
 
 __device__ __forceinline__ ArSum ar_add(ArSum a, ArSum b) {
@@ -426,7 +412,7 @@ __global__ void __launch_bounds__(AR_THREADS) ar_cold_kernel(FileParams fp, cons
         const uint32_t c = s_list[i];
         ColdResult res;
         cold_decode_run<L>(fp, tasks[c].chunk_offset, stage + tinfo[c].slot, wins[c].hi, scratch, ASYNC_COLD_WINDOW_LOG, &res);
-        statuses[c] = res.n_chunks > 0 ? uint32_t(ST_OK) : (res.status == ST_OK || res.status == ST_TERMINATOR || res.status == ST_DST_FULL) ? uint32_t(ST_CORRUPTION) : res.status;
+        statuses[c] = cold_status(res);
         tinfo[c].route = AR_COLD;
       }
     }
@@ -496,14 +482,14 @@ __global__ void __launch_bounds__(AR_SCAN_THREADS) ar_finish_kernel(const ArStat
   const bool known = s.status == ST_OK || s.status == PCO_B200_ASYNC_DST_SHORT || s.status == PCO_B200_ASYNC_WINDOW;
   if (known) r.n_written = s.total;
   if (s.status != ST_OK) {
-    r.kind = ar_kind_of(s.status);
+    r.kind = async_kind_of(s.status);
     r.device_status = s.status;
     if (s.status == PCO_B200_ASYNC_RANGE_PAST || s.status == PCO_B200_ASYNC_RANGE_OVERFLOW) r.range = s.bad >> 1;
     if (s.status == PCO_B200_ASYNC_INDEX_TILING) r.chunk = s.bad_chunk;
   } else if (s_min != AR_NONE64) {
     const uint32_t t = uint32_t(s_min);
     const uint32_t st = statuses[t];
-    r.kind = ar_kind_of(st);
+    r.kind = async_kind_of(st);
     r.device_status = st;
     r.range = s_min >> 32;
     r.chunk = tinfo[t].chunk;

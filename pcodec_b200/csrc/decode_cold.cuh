@@ -48,6 +48,12 @@ struct ColdResult {
   uint64_t next_byte;
 };
 
+// The status of one chunk the catch-all decoder was run on: ST_OK once the decoder has counted the chunk, else its error, where a run
+// that ended cleanly (or at the destination's end) before the chunk is corrupt data.
+__device__ __forceinline__ uint32_t cold_status(const ColdResult& res) {
+  return res.n_chunks > 0 ? uint32_t(ST_OK) : (res.status == ST_OK || res.status == ST_TERMINATOR || res.status == ST_DST_FULL) ? uint32_t(ST_CORRUPTION) : res.status;
+}
+
 __host__ __device__ inline size_t cold_scratch_bytes(uint32_t window_n_log_cap) {
   const size_t per_var = (size_t(1) << COLD_MAX_SIZE_LOG) * (4 + 2) + size_t(COLD_MAX_BINS) * (8 + 1 + 4) + (256 + 32) * 8 + 256 * 4 + 64;
   const size_t win = 2 * (size_t(1) << (window_n_log_cap > 8 ? window_n_log_cap : 8)) * 8;  // buffer_n = 2 max(window_n, 256) for each delta-coded var

@@ -2,6 +2,7 @@
 // There is no CPU implementation of the hot path in this library: without a CUDA device every
 // compute entry point fails with PCO_B200_CUDA.
 #include <algorithm>
+#include <initializer_list>
 
 #include "async_compress.cuh"
 #include "async_compress_files.cuh"
@@ -756,6 +757,97 @@ static PcoB200Error decompress_core(const void* compressed, size_t compressed_le
     e = decompress_cold(compressed, compressed_len, dtype, dst, dst_len, flags, cuda_stream, outcome);
   }
   return e;
+}
+
+// ---- the asynchronous calls' shared host steps.  Each call enqueues a fixed sequence of launches on the caller's stream (AsyncLaunch,
+// host_common.hpp) and makes no host decision between them; its plan does the one-time device set-up, here and not in a call (which may
+// be inside a capture).
+
+// Every kernel in `kernels` loaded now (with lazy module loading a kernel is otherwise loaded at its first launch).
+static PcoB200Error load_kernels(std::initializer_list<const void*> kernels) {
+  cudaFuncAttributes fa;
+  for (const void* k : kernels) PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, k));
+  return PCO_B200_OK;
+}
+
+// The set-up of an asynchronous decompress plan: the device, the decode kernels' attributes (the window-mode instantiations when WIN),
+// and loaded: the decode stage's kernels for dtype, the call's catch-all kernel (cold(tag) for a latent type tag) and the call's `kernels`.
+template <bool WIN, typename Cold>
+static PcoB200Error async_decode_setup(unsigned char dtype, Cold cold, std::initializer_list<const void*> kernels) {
+  Context& c = ctx();
+  if (PcoB200Error e = ensure_device(c)) return e;
+  if (PcoB200Error e = set_decode_attrs<WIN>(c)) return e;
+  if (PcoB200Error e = load_kernels(kernels)) return e;
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
+    using L = decltype(tag);
+    return load_kernels({(const void*)fused_narrow_kernel<L, WIN>, (const void*)symwalk_kernel<WIN>, (const void*)decode_kernel<L, 1, WIN>,
+                         (const void*)decode_kernel<L, 2, WIN>, cold(tag)});
+  });
+}
+
+// The checks of a plan that takes the first bytes of a file: dtype, the buffers (`plan` is the caller's output), the standalone header
+// in head, and its uniform type against dtype.
+static PcoB200Error check_async_head(const void* head, size_t head_len, unsigned char dtype, const void* plan, StandaloneHeader* hdr) {
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (!plan || (!head && head_len)) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (PcoB200Error e = parse_standalone_header(static_cast<const uint8_t*>(head), std::min<size_t>(head_len, 32), head_len, hdr)) return e;
+  if (hdr->uniform_type != 0 && hdr->uniform_type != dtype)
+    return fail(PCO_B200_INVALID_ARGUMENT, "the header's uniform type " + std::to_string(hdr->uniform_type) + " is not dtype " + std::to_string(dtype));
+  return PCO_B200_OK;
+}
+
+// The decode stage of an asynchronous decompress: fused_narrow_kernel, symwalk_kernel and decode_kernel<L, 1 / 2> over the `slots`
+// records of `table`, one CTA each, in window mode when WIN (wins says which numbers of each task are wanted, and dst is unused).
+struct DecodeStage {
+  FileParams fp;
+  const IndexChunk* table;
+  const uint8_t* index;
+  uint64_t index_len;
+  uint32_t slots;
+  uint32_t* st;
+  uint8_t* cls;
+  uint8_t* syms;
+  uint32_t* offs;
+  const Binoms* binoms;
+  void* dst;
+  uint64_t dst_cap;
+  const WinTask* wins;
+};
+template <bool WIN>
+static void enqueue_decode_stage(const AsyncLaunch& ln, const DecodeStage& d) {
+  const cudaStream_t stream = ln.stream;
+  ln.begin("fused_narrow_kernel");
+  dispatch_latent(d.fp.dtype, [&](auto tag) {
+    using L = decltype(tag);
+    fused_narrow_kernel<L, WIN><<<d.slots, FZ_THREADS, sizeof(FusedSmem), stream>>>(d.fp, d.table, d.index, d.index_len, d.st, d.cls, static_cast<L*>(d.dst),
+                                                                                   d.dst_cap, d.wins);
+    return 0;
+  });
+  ln.end();
+  ln.begin("symwalk_kernel");
+  symwalk_kernel<WIN><<<d.slots, SW_THREADS, sizeof(SymWalkSmem), stream>>>(d.fp, d.table, d.index, d.index_len, d.dst_cap, d.syms, d.offs, d.cls, d.wins);
+  ln.end();
+  ln.begin("decode_kernel");
+  dispatch_latent(d.fp.dtype, [&](auto tag) {
+    using L = decltype(tag);
+    decode_kernel<L, 1, WIN><<<d.slots, DEC_THREADS, sizeof(DecodeSmem), stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst), d.dst_cap,
+                                                                                  d.binoms, d.syms, d.offs, d.cls, d.wins);
+    decode_kernel<L, 2, WIN><<<d.slots, DEC_THREADS, sizeof(DecodeSmem), stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst), d.dst_cap,
+                                                                                  d.binoms, d.syms, d.offs, d.cls, d.wins);
+    return 0;
+  });
+  ln.end();
+}
+
+// The message of a standalone-header refusal of a decompress call (the file's own words: pco_b200_decompress_files_async names the file
+// in front), or nullptr for any other status.
+static const char* async_header_refusal(uint32_t device_status) {
+  switch (device_status) {
+    case PCO_B200_ASYNC_HEADER_CORRUPT: return "corrupt standalone header (magic, version, type byte or size hint)";
+    case PCO_B200_ASYNC_HEADER_SHORT: return "insufficient data: the file ends inside its standalone header";
+    case PCO_B200_ASYNC_HEADER_MISMATCH: return "the file's uniform type or format version differs from the plan's";
+    default: return nullptr;
+  }
 }
 
 }  // namespace pcob200
@@ -2425,20 +2517,23 @@ PcoB200Error pco_b200_debug_plan_ranges(const void* chunk_table, size_t n_chunks
   return PCO_B200_OK;
 }
 
+unsigned pco_b200_debug_async_kind(unsigned device_status) { return async_kind_of(device_status); }
+
 // ---- asynchronous decompress of an indexed standalone file (pco_b200_decompress_async; kernels in async_kernels.cuh)
 // The plan fixes what the launches take by value (FileParams' number type, uniform type and format major) and every grid size (from
 // max_chunks); the file's own length, chunk count and n_total are read from its side index on the device.  So a call is a fixed
 // sequence of seven launches and nothing else: check, fused, symwalk, decode<1>, decode<2>, cold, finish.  A kernel that has nothing
 // to do for a chunk leaves at its first line.
 
+static bool async_plan_ok(const PcoB200AsyncPlan* p) {
+  return nt_valid(p->dtype) && p->max_chunks >= 1 && p->max_chunks <= 0xffffffffull && p->dst_cap <= (uint64_t(1) << 56) &&
+         p->workspace_bytes == async_layout(p->dst_cap, uint32_t(p->max_chunks)).total;
+}
+
 PcoB200Error pco_b200_decompress_async_plan(const void* head, size_t head_len, unsigned char dtype, size_t src_cap, size_t index_cap, size_t dst_cap,
                                             size_t max_chunks, PcoB200AsyncPlan* plan) {
-  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
-  if (!plan || (!head && head_len)) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
   StandaloneHeader hdr;
-  if (PcoB200Error e = parse_standalone_header(static_cast<const uint8_t*>(head), std::min<size_t>(head_len, 32), head_len, &hdr)) return e;
-  if (hdr.uniform_type != 0 && hdr.uniform_type != dtype)
-    return fail(PCO_B200_INVALID_ARGUMENT, "the header's uniform type " + std::to_string(hdr.uniform_type) + " is not dtype " + std::to_string(dtype));
+  if (PcoB200Error e = check_async_head(head, head_len, dtype, plan, &hdr)) return e;
   if (max_chunks == 0 || uint64_t(max_chunks) > 0xffffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_chunks must be 1 .. 2^32 - 1");
   if (uint64_t(dst_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "dst_cap above 2^56 numbers");
   std::memset(plan, 0, sizeof(*plan));
@@ -2450,39 +2545,18 @@ PcoB200Error pco_b200_decompress_async_plan(const void* head, size_t head_len, u
   plan->dst_cap = dst_cap;
   plan->max_chunks = max_chunks;
   plan->workspace_bytes = async_layout(dst_cap, uint32_t(max_chunks)).total;
-  // the one-time device set-up, here and not in a call (which may be inside a capture): the decode kernels' attributes, and every kernel
-  // the call launches loaded now (with lazy module loading a kernel is otherwise loaded at its first launch)
-  Context& c = ctx();
-  if (PcoB200Error e = ensure_device(c)) return e;
-  if (PcoB200Error e = set_decode_attrs<false>(c)) return e;
-  cudaFuncAttributes fa;
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, async_check_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, async_finish_kernel));
-  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
-    using L = decltype(tag);
-    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, fused_narrow_kernel<L>));
-    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, decode_kernel<L, 1>));
-    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, decode_kernel<L, 2>));
-    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, cold_chunks_kernel<L>));
-    return PCO_B200_OK;
-  });
+  return async_decode_setup<false>(dtype, [](auto tag) { return (const void*)cold_chunks_kernel<decltype(tag)>; },
+                                   {(const void*)async_check_kernel, (const void*)async_finish_kernel});
 }
 
 PcoB200Error pco_b200_decompress_async(const PcoB200AsyncPlan* plan, const void* src, const void* index, void* dst, void* workspace,
                                        PcoB200AsyncStatus* status, void* cuda_stream) {
   if (!plan || !src || !index || !workspace || !status || (!dst && plan->dst_cap)) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
-  if (!nt_valid(plan->dtype) || plan->max_chunks == 0 || plan->max_chunks > 0xffffffffull || plan->dst_cap > (uint64_t(1) << 56) ||
-      plan->workspace_bytes != async_layout(plan->dst_cap, uint32_t(plan->max_chunks)).total)
-    return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_decompress_async_plan");
+  if (!async_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_decompress_async_plan");
   if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
-  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  PCOB_CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
-  // kernel spans only outside a capture (an event record would become part of the graph); those of an earlier call that nobody read go
-  const bool prof = cap == cudaStreamCaptureStatusNone && profiler_enabled().load(std::memory_order_relaxed);
-  if (prof) profiler().discard();
-  auto begin = [&](const char* name) { if (prof) profiler().begin(name, stream); };
-  auto end = [&]() { if (prof) profiler().end(stream); };
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+  const cudaStream_t stream = ln.stream;
 
   const uint32_t mc = uint32_t(plan->max_chunks);
   const AsyncLayout lay = async_layout(plan->dst_cap, mc);
@@ -2490,51 +2564,28 @@ PcoB200Error pco_b200_decompress_async(const PcoB200AsyncPlan* plan, const void*
   AsyncCheck* chk = reinterpret_cast<AsyncCheck*>(ws);
   IndexChunk* table = reinterpret_cast<IndexChunk*>(ws + lay.table);
   uint32_t* d_st = reinterpret_cast<uint32_t*>(ws + lay.st);
-  uint8_t* d_cls = ws + lay.cls;
-  uint8_t* d_syms = ws + lay.syms;
-  uint32_t* d_offs = reinterpret_cast<uint32_t*>(ws + lay.offs);
-  uint8_t* d_cold = ws + lay.cold;
-  const uint8_t* d_idx = static_cast<const uint8_t*>(index);
   AsyncArgs a;
   a.fp = FileParams{src, plan->src_cap, plan->dtype, plan->uniform_type, plan->format_major};
-  a.index = d_idx;
+  a.index = static_cast<const uint8_t*>(index);
   a.index_cap = plan->index_cap;
   a.dst_cap = plan->dst_cap;
   a.max_chunks = mc;
 
-  begin("async_check_kernel");
+  ln.begin("async_check_kernel");
   async_check_kernel<<<(mc + ASYNC_CHECK_RECS - 1) / ASYNC_CHECK_RECS, ASYNC_THREADS, 0, stream>>>(a, chk, table);
-  end();
-  begin("fused_narrow_kernel");
+  ln.end();
+  enqueue_decode_stage<false>(ln, DecodeStage{a.fp, table, a.index, a.index_cap, mc, d_st, ws + lay.cls, ws + lay.syms,
+                                              reinterpret_cast<uint32_t*>(ws + lay.offs), &chk->binoms, dst, a.dst_cap, nullptr});
+  ln.begin("cold_chunks_kernel");
   dispatch_latent(plan->dtype, [&](auto tag) {
     using L = decltype(tag);
-    fused_narrow_kernel<L><<<mc, FZ_THREADS, sizeof(FusedSmem), stream>>>(a.fp, table, d_idx, a.index_cap, d_st, d_cls, static_cast<L*>(dst), a.dst_cap);
+    cold_chunks_kernel<L><<<1, ASYNC_THREADS, 0, stream>>>(a.fp, table, chk, d_st, static_cast<L*>(dst), a.dst_cap, ws + lay.cold);
     return 0;
   });
-  end();
-  begin("symwalk_kernel");
-  symwalk_kernel<false><<<mc, SW_THREADS, sizeof(SymWalkSmem), stream>>>(a.fp, table, d_idx, a.index_cap, a.dst_cap, d_syms, d_offs, d_cls);
-  end();
-  begin("decode_kernel");
-  dispatch_latent(plan->dtype, [&](auto tag) {
-    using L = decltype(tag);
-    decode_kernel<L, 1><<<mc, DEC_THREADS, sizeof(DecodeSmem), stream>>>(a.fp, table, d_st, d_idx, a.index_cap, static_cast<L*>(dst), a.dst_cap, &chk->binoms,
-                                                                          d_syms, d_offs, d_cls);
-    decode_kernel<L, 2><<<mc, DEC_THREADS, sizeof(DecodeSmem), stream>>>(a.fp, table, d_st, d_idx, a.index_cap, static_cast<L*>(dst), a.dst_cap, &chk->binoms,
-                                                                          d_syms, d_offs, d_cls);
-    return 0;
-  });
-  end();
-  begin("cold_chunks_kernel");
-  dispatch_latent(plan->dtype, [&](auto tag) {
-    using L = decltype(tag);
-    cold_chunks_kernel<L><<<1, ASYNC_THREADS, 0, stream>>>(a.fp, table, chk, d_st, static_cast<L*>(dst), a.dst_cap, d_cold);
-    return 0;
-  });
-  end();
-  begin("async_finish_kernel");
+  ln.end();
+  ln.begin("async_finish_kernel");
   async_finish_kernel<<<1, 1024, 0, stream>>>(a.dst_cap, chk, d_st, status);
-  end();
+  ln.end();
   PCOB_CUDA_TRY(cudaGetLastError());
   return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
 }
@@ -2549,10 +2600,8 @@ PcoB200Error pco_b200_decompress_async_result(const PcoB200AsyncStatus* s, PcoB2
     }
     return PCO_B200_OK;
   }
+  if (const char* h = async_header_refusal(s->device_status)) return fail(kind, h);
   switch (s->device_status) {
-    case PCO_B200_ASYNC_HEADER_CORRUPT: return fail(kind, "corrupt standalone header (magic, version, type byte or size hint)");
-    case PCO_B200_ASYNC_HEADER_SHORT: return fail(kind, "insufficient data: the file ends inside its standalone header");
-    case PCO_B200_ASYNC_HEADER_MISMATCH: return fail(kind, "the file's uniform type or format version differs from the plan's");
     case PCO_B200_ASYNC_INDEX_FOREIGN: return fail(kind, "side index does not belong to this file (or its file length exceeds src_cap)");
     case PCO_B200_ASYNC_TOO_MANY_CHUNKS:
       return fail(kind, "the side index lists " + std::to_string(s->n_chunks) + " chunks, more than the plan's max_chunks");
@@ -2575,12 +2624,8 @@ static bool ar_plan_ok(const PcoB200AsyncRangesPlan* p) {
 
 PcoB200Error pco_b200_decompress_ranges_async_plan(const void* head, size_t head_len, unsigned char dtype, size_t src_cap, size_t index_cap,
                                                    size_t max_chunks, size_t max_ranges, size_t dst_cap, size_t window_cap, PcoB200AsyncRangesPlan* plan) {
-  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
-  if (!plan || (!head && head_len)) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
   StandaloneHeader hdr;
-  if (PcoB200Error e = parse_standalone_header(static_cast<const uint8_t*>(head), std::min<size_t>(head_len, 32), head_len, &hdr)) return e;
-  if (hdr.uniform_type != 0 && hdr.uniform_type != dtype)
-    return fail(PCO_B200_INVALID_ARGUMENT, "the header's uniform type " + std::to_string(hdr.uniform_type) + " is not dtype " + std::to_string(dtype));
+  if (PcoB200Error e = check_async_head(head, head_len, dtype, plan, &hdr)) return e;
   if (max_chunks == 0 || uint64_t(max_chunks) > 0xffffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_chunks must be 1 .. 2^32 - 1");
   if (max_ranges == 0 || uint64_t(max_ranges) > 0xffffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_ranges must be 1 .. 2^32 - 1");
   if (uint64_t(dst_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "dst_cap above 2^56 numbers");
@@ -2596,31 +2641,10 @@ PcoB200Error pco_b200_decompress_ranges_async_plan(const void* head, size_t head
   plan->dst_cap = dst_cap;
   plan->window_cap = window_cap;
   plan->workspace_bytes = ar_layout(max_chunks, max_ranges, window_cap, nt_bits(dtype) / 8).total;
-  // the one-time device set-up, as in pco_b200_decompress_async_plan: the window-mode decode kernels' attributes, and every kernel the
-  // call launches loaded now
-  Context& c = ctx();
-  if (PcoB200Error e = ensure_device(c)) return e;
-  if (PcoB200Error e = set_decode_attrs<true>(c)) return e;
-  cudaFuncAttributes fa;
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, async_check_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_chunks_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_count_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_scan_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_mark_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_window_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_gate_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_tasks_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, symwalk_kernel<true>));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_gather_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_finish_kernel));
-  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
-    using L = decltype(tag);
-    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, fused_narrow_kernel<L, true>));
-    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, decode_kernel<L, 1, true>));
-    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, decode_kernel<L, 2, true>));
-    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ar_cold_kernel<L>));
-    return PCO_B200_OK;
-  });
+  return async_decode_setup<true>(dtype, [](auto tag) { return (const void*)ar_cold_kernel<decltype(tag)>; },
+                                  {(const void*)async_check_kernel, (const void*)ar_chunks_kernel, (const void*)ar_count_kernel, (const void*)ar_scan_kernel,
+                                   (const void*)ar_mark_kernel, (const void*)ar_window_kernel, (const void*)ar_gate_kernel, (const void*)ar_tasks_kernel,
+                                   (const void*)ar_gather_kernel, (const void*)ar_finish_kernel});
 }
 
 PcoB200Error pco_b200_decompress_ranges_async(const PcoB200AsyncRangesPlan* plan, const void* src, const void* index, const PcoB200Range* ranges,
@@ -2629,13 +2653,9 @@ PcoB200Error pco_b200_decompress_ranges_async(const PcoB200AsyncRangesPlan* plan
     return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
   if (!ar_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_decompress_ranges_async_plan");
   if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
-  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  PCOB_CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
-  const bool prof = cap == cudaStreamCaptureStatusNone && profiler_enabled().load(std::memory_order_relaxed);
-  if (prof) profiler().discard();
-  auto begin = [&](const char* name) { if (prof) profiler().begin(name, stream); };
-  auto end = [&]() { if (prof) profiler().end(stream); };
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+  const cudaStream_t stream = ln.stream;
 
   const uint32_t mc = uint32_t(plan->max_chunks), mr = uint32_t(plan->max_ranges), elem = nt_bits(plan->dtype) / 8;
   const ArLayout lay = ar_layout(mc, mr, plan->window_cap, elem);
@@ -2652,15 +2672,10 @@ PcoB200Error pco_b200_decompress_ranges_async(const PcoB200AsyncRangesPlan* plan
   WinTask* wins = reinterpret_cast<WinTask*>(ws + lay.wins);
   ArTask* tinfo = reinterpret_cast<ArTask*>(ws + lay.tinfo);
   uint32_t* d_st = reinterpret_cast<uint32_t*>(ws + lay.st);
-  uint8_t* d_cls = ws + lay.cls;
-  uint8_t* d_syms = ws + lay.syms;
-  uint32_t* d_offs = reinterpret_cast<uint32_t*>(ws + lay.offs);
   uint8_t* d_stage = ws + lay.stage;
-  uint8_t* d_cold = ws + lay.cold;
-  const uint8_t* d_idx = static_cast<const uint8_t*>(index);
   ArArgs g;
   g.a.fp = FileParams{src, plan->src_cap, plan->dtype, plan->uniform_type, plan->format_major};
-  g.a.index = d_idx;
+  g.a.index = static_cast<const uint8_t*>(index);
   g.a.index_cap = plan->index_cap;
   g.a.dst_cap = plan->dst_cap;
   g.a.max_chunks = mc;
@@ -2671,64 +2686,47 @@ PcoB200Error pco_b200_decompress_ranges_async(const PcoB200AsyncRangesPlan* plan
   g.elem = elem;
   const uint32_t cb = uint32_t(ar_ctas(mc)), rb = uint32_t(ar_ctas(mr));
 
-  begin("async_check_kernel");
+  ln.begin("async_check_kernel");
   async_check_kernel<<<(mc + ASYNC_CHECK_RECS - 1) / ASYNC_CHECK_RECS, ASYNC_THREADS, 0, stream>>>(g.a, chk, table);
-  end();
-  begin("ar_chunks_kernel");
+  ln.end();
+  ln.begin("ar_chunks_kernel");
   ar_chunks_kernel<<<cb, AR_THREADS, 0, stream>>>(chk, table, marks, cparts);
-  end();
-  begin("ar_count_kernel");
+  ln.end();
+  ln.begin("ar_count_kernel");
   ar_count_kernel<<<rb, AR_THREADS, 0, stream>>>(g, chk, rparts);
-  end();
-  begin("ar_scan_kernel");
+  ln.end();
+  ln.begin("ar_scan_kernel");
   ar_scan_kernel<<<1, AR_SCAN_THREADS, 0, stream>>>(g, chk, cparts, rparts, state);
-  end();
-  begin("ar_mark_kernel");
+  ln.end();
+  ln.begin("ar_mark_kernel");
   ar_mark_kernel<<<rb, AR_THREADS, 0, stream>>>(g, chk, table, rparts, state, marks, roff, rspan);
-  end();
-  begin("ar_window_kernel");
+  ln.end();
+  ln.begin("ar_window_kernel");
   ar_window_kernel<<<cb, AR_THREADS, 0, stream>>>(chk, state, marks, cparts);
-  end();
-  begin("ar_gate_kernel");
+  ln.end();
+  ln.begin("ar_gate_kernel");
   ar_gate_kernel<<<1, AR_SCAN_THREADS, 0, stream>>>(g, cparts, state);
-  end();
-  begin("ar_tasks_kernel");
+  ln.end();
+  ln.begin("ar_tasks_kernel");
   ar_tasks_kernel<<<cb, AR_THREADS, 0, stream>>>(g, chk, state, table, marks, cparts, tasks, wins, tinfo, static_cast<uint8_t*>(dst), d_stage);
-  end();
-  begin("fused_narrow_kernel");
+  ln.end();
+  // window mode: the decode writes to the tasks' destinations or slots (wins), not to a dst of its own
+  enqueue_decode_stage<true>(ln, DecodeStage{g.a.fp, tasks, g.a.index, g.a.index_cap, mc, d_st, ws + lay.cls, ws + lay.syms,
+                                             reinterpret_cast<uint32_t*>(ws + lay.offs), &chk->binoms, nullptr, 0, wins});
+  ln.begin("ar_cold_kernel");
   dispatch_latent(plan->dtype, [&](auto tag) {
     using L = decltype(tag);
-    fused_narrow_kernel<L, true><<<mc, FZ_THREADS, sizeof(FusedSmem), stream>>>(g.a.fp, tasks, d_idx, g.a.index_cap, d_st, d_cls, nullptr, 0, wins);
+    ar_cold_kernel<L><<<1, AR_THREADS, 0, stream>>>(g.a.fp, state, tasks, wins, tinfo, d_st, reinterpret_cast<L*>(d_stage), ws + lay.cold);
     return 0;
   });
-  end();
-  begin("symwalk_kernel");
-  symwalk_kernel<true><<<mc, SW_THREADS, sizeof(SymWalkSmem), stream>>>(g.a.fp, tasks, d_idx, g.a.index_cap, 0, d_syms, d_offs, d_cls, wins);
-  end();
-  begin("decode_kernel");
-  dispatch_latent(plan->dtype, [&](auto tag) {
-    using L = decltype(tag);
-    decode_kernel<L, 1, true><<<mc, DEC_THREADS, sizeof(DecodeSmem), stream>>>(g.a.fp, tasks, d_st, d_idx, g.a.index_cap, nullptr, 0, &chk->binoms, d_syms,
-                                                                                d_offs, d_cls, wins);
-    decode_kernel<L, 2, true><<<mc, DEC_THREADS, sizeof(DecodeSmem), stream>>>(g.a.fp, tasks, d_st, d_idx, g.a.index_cap, nullptr, 0, &chk->binoms, d_syms,
-                                                                                d_offs, d_cls, wins);
-    return 0;
-  });
-  end();
-  begin("ar_cold_kernel");
-  dispatch_latent(plan->dtype, [&](auto tag) {
-    using L = decltype(tag);
-    ar_cold_kernel<L><<<1, AR_THREADS, 0, stream>>>(g.a.fp, state, tasks, wins, tinfo, d_st, reinterpret_cast<L*>(d_stage), d_cold);
-    return 0;
-  });
-  end();
-  begin("ar_gather_kernel");
+  ln.end();
+  ln.begin("ar_gather_kernel");
   ar_gather_kernel<<<std::min(mr, AR_GATHER_MAX_CTAS), AR_THREADS, 0, stream>>>(g, state, table, marks, wins, tinfo, d_st, roff, rspan,
                                                                                   static_cast<uint8_t*>(dst), d_stage);
-  end();
-  begin("ar_finish_kernel");
+  ln.end();
+  ln.begin("ar_finish_kernel");
   ar_finish_kernel<<<1, AR_SCAN_THREADS, 0, stream>>>(state, tinfo, d_st, status);
-  end();
+  ln.end();
   PCOB_CUDA_TRY(cudaGetLastError());
   return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
 }
@@ -2740,10 +2738,8 @@ PcoB200Error pco_b200_decompress_ranges_async_result(const PcoB200AsyncRangesSta
     if (n_written) *n_written = size_t(s->n_written);
     return PCO_B200_OK;
   }
+  if (const char* h = async_header_refusal(s->device_status)) return fail(kind, h);
   switch (s->device_status) {
-    case PCO_B200_ASYNC_HEADER_CORRUPT: return fail(kind, "corrupt standalone header (magic, version, type byte or size hint)");
-    case PCO_B200_ASYNC_HEADER_SHORT: return fail(kind, "insufficient data: the file ends inside its standalone header");
-    case PCO_B200_ASYNC_HEADER_MISMATCH: return fail(kind, "the file's uniform type or format version differs from the plan's");
     case PCO_B200_ASYNC_INDEX_FOREIGN: return fail(kind, "side index does not belong to this file (or its file length exceeds src_cap)");
     case PCO_B200_ASYNC_TOO_MANY_CHUNKS: return fail(kind, "the side index lists more chunks than the plan's max_chunks");
     case PCO_B200_ASYNC_INDEX_TILING:
@@ -2773,12 +2769,8 @@ static bool af_plan_ok(const PcoB200AsyncFilesPlan* p) {
 
 PcoB200Error pco_b200_decompress_files_async_plan(const void* head, size_t head_len, unsigned char dtype, size_t src_cap, size_t index_cap,
                                                   size_t max_files, size_t max_chunks, size_t dst_cap, PcoB200AsyncFilesPlan* plan) {
-  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
-  if (!plan || (!head && head_len)) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
   StandaloneHeader hdr;
-  if (PcoB200Error e = parse_standalone_header(static_cast<const uint8_t*>(head), std::min<size_t>(head_len, 32), head_len, &hdr)) return e;
-  if (hdr.uniform_type != 0 && hdr.uniform_type != dtype)
-    return fail(PCO_B200_INVALID_ARGUMENT, "the header's uniform type " + std::to_string(hdr.uniform_type) + " is not dtype " + std::to_string(dtype));
+  if (PcoB200Error e = check_async_head(head, head_len, dtype, plan, &hdr)) return e;
   if (max_files == 0 || uint64_t(max_files) > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_files must be 1 .. 2^31 - 1");
   if (max_chunks == 0 || uint64_t(max_chunks) > 0xffffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_chunks must be 1 .. 2^32 - 1");
   if (uint64_t(dst_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "dst_cap above 2^56 numbers");
@@ -2792,27 +2784,9 @@ PcoB200Error pco_b200_decompress_files_async_plan(const void* head, size_t head_
   plan->max_chunks = max_chunks;
   plan->dst_cap = dst_cap;
   plan->workspace_bytes = af_layout(max_files, max_chunks, dst_cap).total;
-  // the one-time device set-up, as in pco_b200_decompress_async_plan
-  Context& c = ctx();
-  if (PcoB200Error e = ensure_device(c)) return e;
-  if (PcoB200Error e = set_decode_attrs<false>(c)) return e;
-  cudaFuncAttributes fa;
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, af_files_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, check_index_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, af_scan_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, af_place_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, af_table_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, merge_index_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, symwalk_kernel<false>));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, af_finish_kernel));
-  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
-    using L = decltype(tag);
-    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, fused_narrow_kernel<L>));
-    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, decode_kernel<L, 1>));
-    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, decode_kernel<L, 2>));
-    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, cold_chunks_kernel<L>));
-    return PCO_B200_OK;
-  });
+  return async_decode_setup<false>(dtype, [](auto tag) { return (const void*)cold_chunks_kernel<decltype(tag)>; },
+                                   {(const void*)af_files_kernel, (const void*)check_index_kernel, (const void*)af_scan_kernel, (const void*)af_place_kernel,
+                                    (const void*)af_table_kernel, (const void*)merge_index_kernel, (const void*)af_finish_kernel});
 }
 
 PcoB200Error pco_b200_decompress_files_async(const PcoB200AsyncFilesPlan* plan, const void* src, const void* index, const PcoB200FileRef* files,
@@ -2822,13 +2796,9 @@ PcoB200Error pco_b200_decompress_files_async(const PcoB200AsyncFilesPlan* plan, 
     return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
   if (!af_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_decompress_files_async_plan");
   if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
-  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  PCOB_CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
-  const bool prof = cap == cudaStreamCaptureStatusNone && profiler_enabled().load(std::memory_order_relaxed);
-  if (prof) profiler().discard();
-  auto begin = [&](const char* name) { if (prof) profiler().begin(name, stream); };
-  auto end = [&]() { if (prof) profiler().end(stream); };
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+  const cudaStream_t stream = ln.stream;
 
   const uint32_t mf = uint32_t(plan->max_files), mc = uint32_t(plan->max_chunks);
   const AfLayout lay = af_layout(mf, mc, plan->dst_cap);
@@ -2842,10 +2812,6 @@ PcoB200Error pco_b200_decompress_files_async(const PcoB200AsyncFilesPlan* plan, 
   AfPart* parts = reinterpret_cast<AfPart*>(ws + lay.parts);
   IndexChunk* table = reinterpret_cast<IndexChunk*>(ws + lay.table);
   uint32_t* d_st = reinterpret_cast<uint32_t*>(ws + lay.st);
-  uint8_t* d_cls = ws + lay.cls;
-  uint8_t* d_syms = ws + lay.syms;
-  uint32_t* d_offs = reinterpret_cast<uint32_t*>(ws + lay.offs);
-  uint8_t* d_cold = ws + lay.cold;
   const uint8_t* d_idx = static_cast<const uint8_t*>(index);
   AfArgs g;
   g.fp = FileParams{src, plan->src_cap, plan->dtype, plan->uniform_type, plan->format_major};
@@ -2858,54 +2824,36 @@ PcoB200Error pco_b200_decompress_files_async(const PcoB200AsyncFilesPlan* plan, 
   g.max_chunks = mc;
   const uint32_t fb = uint32_t(af_ctas(mf)), tb = uint32_t(std::max(af_ctas(mf), af_ctas(mc)));
 
-  begin("af_files_kernel");
+  ln.begin("af_files_kernel");
   af_files_kernel<<<fb, AF_THREADS, 0, stream>>>(g, chk, fst, fchk, merges, parts);
-  end();
-  begin("check_index_kernel");
+  ln.end();
+  ln.begin("check_index_kernel");
   check_index_kernel<<<mf, 256, 0, stream>>>(static_cast<const uint8_t*>(src), d_idx, plan->dtype, fchk, verdict);
-  end();
-  begin("af_scan_kernel");
+  ln.end();
+  ln.begin("af_scan_kernel");
   af_scan_kernel<<<1, AF_SCAN_THREADS, 0, stream>>>(g, parts, state);
-  end();
-  begin("af_place_kernel");
+  ln.end();
+  ln.begin("af_place_kernel");
   af_place_kernel<<<fb, AF_THREADS, 0, stream>>>(g, fst, fchk, verdict, parts, merges, state);
-  end();
-  begin("af_table_kernel");
+  ln.end();
+  ln.begin("af_table_kernel");
   af_table_kernel<<<tb, AF_THREADS, 0, stream>>>(g, state, chk, merges, table);
-  end();
-  begin("merge_index_kernel");
+  ln.end();
+  ln.begin("merge_index_kernel");
   merge_index_kernel<<<mf, 256, 0, stream>>>(d_idx, merges, table);
-  end();
-  begin("fused_narrow_kernel");
+  ln.end();
+  enqueue_decode_stage<false>(ln, DecodeStage{g.fp, table, d_idx, g.index_cap, mc, d_st, ws + lay.cls, ws + lay.syms,
+                                              reinterpret_cast<uint32_t*>(ws + lay.offs), &chk->binoms, dst, g.dst_cap, nullptr});
+  ln.begin("cold_chunks_kernel");
   dispatch_latent(plan->dtype, [&](auto tag) {
     using L = decltype(tag);
-    fused_narrow_kernel<L><<<mc, FZ_THREADS, sizeof(FusedSmem), stream>>>(g.fp, table, d_idx, g.index_cap, d_st, d_cls, static_cast<L*>(dst), g.dst_cap);
+    cold_chunks_kernel<L><<<1, ASYNC_THREADS, 0, stream>>>(g.fp, table, chk, d_st, static_cast<L*>(dst), g.dst_cap, ws + lay.cold);
     return 0;
   });
-  end();
-  begin("symwalk_kernel");
-  symwalk_kernel<false><<<mc, SW_THREADS, sizeof(SymWalkSmem), stream>>>(g.fp, table, d_idx, g.index_cap, g.dst_cap, d_syms, d_offs, d_cls);
-  end();
-  begin("decode_kernel");
-  dispatch_latent(plan->dtype, [&](auto tag) {
-    using L = decltype(tag);
-    decode_kernel<L, 1><<<mc, DEC_THREADS, sizeof(DecodeSmem), stream>>>(g.fp, table, d_st, d_idx, g.index_cap, static_cast<L*>(dst), g.dst_cap, &chk->binoms,
-                                                                          d_syms, d_offs, d_cls);
-    decode_kernel<L, 2><<<mc, DEC_THREADS, sizeof(DecodeSmem), stream>>>(g.fp, table, d_st, d_idx, g.index_cap, static_cast<L*>(dst), g.dst_cap, &chk->binoms,
-                                                                          d_syms, d_offs, d_cls);
-    return 0;
-  });
-  end();
-  begin("cold_chunks_kernel");
-  dispatch_latent(plan->dtype, [&](auto tag) {
-    using L = decltype(tag);
-    cold_chunks_kernel<L><<<1, ASYNC_THREADS, 0, stream>>>(g.fp, table, chk, d_st, static_cast<L*>(dst), g.dst_cap, d_cold);
-    return 0;
-  });
-  end();
-  begin("af_finish_kernel");
+  ln.end();
+  ln.begin("af_finish_kernel");
   af_finish_kernel<<<1, AF_SCAN_THREADS, 0, stream>>>(state, chk, merges, fchk, d_st, file_ns, status);
-  end();
+  ln.end();
   PCOB_CUDA_TRY(cudaGetLastError());
   return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
 }
@@ -2918,15 +2866,13 @@ PcoB200Error pco_b200_decompress_files_async_result(const PcoB200AsyncFilesStatu
     return PCO_B200_OK;
   }
   const uint64_t f = s->file;
+  if (const char* h = async_header_refusal(s->device_status)) return file_fail(kind, f, h);
   switch (s->device_status) {
     case PCO_B200_ASYNC_TOO_MANY_FILES:
       return fail(kind, "*n_files is " + std::to_string(s->n_files) + ", above the plan's max_files");
     case PCO_B200_ASYNC_FILE_OUTSIDE: return file_fail(kind, f, "file lies outside src");
     case PCO_B200_ASYNC_INDEX_OFFSET: return file_fail(kind, f, "index offset is not a multiple of 16");
     case PCO_B200_ASYNC_INDEX_OUTSIDE: return file_fail(kind, f, "side index lies outside index");
-    case PCO_B200_ASYNC_HEADER_CORRUPT: return file_fail(kind, f, "corrupt standalone header (magic, version, type byte or size hint)");
-    case PCO_B200_ASYNC_HEADER_SHORT: return file_fail(kind, f, "insufficient data: the file ends inside its standalone header");
-    case PCO_B200_ASYNC_HEADER_MISMATCH: return file_fail(kind, f, "the file's uniform type or format version differs from the plan's");
     case PCO_B200_ASYNC_NO_INDEX: return file_fail(kind, f, "no side index (files without one are walked, which needs the host)");
     case PCO_B200_ASYNC_INDEX_FOREIGN: return file_fail(kind, f, "side index does not belong to this file");
     case PCO_B200_ASYNC_ENTRIES_MISALIGNED: return file_fail(kind, f, "side index does not belong to this file (misaligned entries)");
@@ -2965,28 +2911,10 @@ PcoB200Error pco_b200_decompress_pages_async_plan(unsigned char dtype, size_t me
   plan->dst_cap = dst_cap;
   plan->frame_cap = frame_cap;
   plan->workspace_bytes = ap_layout(max_pages, dst_cap, frame_cap).total;
-  // the one-time device set-up, as in pco_b200_decompress_async_plan
-  Context& c = ctx();
-  if (PcoB200Error e = ensure_device(c)) return e;
-  if (PcoB200Error e = set_decode_attrs<false>(c)) return e;
-  cudaFuncAttributes fa;
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ap_pages_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ap_scan_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ap_place_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, frame_pages_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, walk_kernel<SMALL_MAX_SIZE_LOG>));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ap_route_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ap_rewalk_kernel));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, symwalk_kernel<false>));
-  PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ap_finish_kernel));
-  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
-    using L = decltype(tag);
-    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, fused_narrow_kernel<L>));
-    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, decode_kernel<L, 1>));
-    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, decode_kernel<L, 2>));
-    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, ap_cold_kernel<L>));
-    return PCO_B200_OK;
-  });
+  return async_decode_setup<false>(dtype, [](auto tag) { return (const void*)ap_cold_kernel<decltype(tag)>; },
+                                   {(const void*)ap_pages_kernel, (const void*)ap_scan_kernel, (const void*)ap_place_kernel, (const void*)frame_pages_kernel,
+                                    (const void*)walk_kernel<SMALL_MAX_SIZE_LOG>, (const void*)ap_route_kernel, (const void*)ap_rewalk_kernel,
+                                    (const void*)ap_finish_kernel});
 }
 
 PcoB200Error pco_b200_decompress_pages_async(const PcoB200AsyncPagesPlan* plan, const void* metas, const void* pages, const PcoB200PageRef* refs,
@@ -2995,13 +2923,9 @@ PcoB200Error pco_b200_decompress_pages_async(const PcoB200AsyncPagesPlan* plan, 
     return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
   if (!ap_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_decompress_pages_async_plan");
   if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
-  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  PCOB_CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
-  const bool prof = cap == cudaStreamCaptureStatusNone && profiler_enabled().load(std::memory_order_relaxed);
-  if (prof) profiler().discard();
-  auto begin = [&](const char* name) { if (prof) profiler().begin(name, stream); };
-  auto end = [&]() { if (prof) profiler().end(stream); };
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+  const cudaStream_t stream = ln.stream;
 
   const uint32_t mp = uint32_t(plan->max_pages);
   const ApLayout lay = ap_layout(mp, plan->dst_cap, plan->frame_cap);
@@ -3020,10 +2944,6 @@ PcoB200Error pco_b200_decompress_pages_async(const PcoB200AsyncPagesPlan* plan, 
   uint32_t* fast_page = reinterpret_cast<uint32_t*>(ws + lay.fast_page);
   uint32_t* cold_list = reinterpret_cast<uint32_t*>(ws + lay.cold_list);
   uint32_t* d_st = reinterpret_cast<uint32_t*>(ws + lay.st);
-  uint8_t* d_cls = ws + lay.cls;
-  uint8_t* d_syms = ws + lay.syms;
-  uint32_t* d_offs = reinterpret_cast<uint32_t*>(ws + lay.offs);
-  uint8_t* d_cold = ws + lay.cold;
   ApArgs g;
   g.metas = static_cast<const uint8_t*>(metas);
   g.pages = static_cast<const uint8_t*>(pages);
@@ -3039,58 +2959,40 @@ PcoB200Error pco_b200_decompress_pages_async(const PcoB200AsyncPagesPlan* plan, 
   const FileParams fp{d_frames, lay.pad_frame + 64, plan->dtype, 0, 4};
   const uint32_t pb = uint32_t(ap_ctas(mp));
 
-  begin("ap_pages_kernel");
+  ln.begin("ap_pages_kernel");
   ap_pages_kernel<<<pb, AP_THREADS, 0, stream>>>(g, chk, parts);
-  end();
-  begin("ap_scan_kernel");
+  ln.end();
+  ln.begin("ap_scan_kernel");
   ap_scan_kernel<<<1, AP_SCAN_THREADS, 0, stream>>>(g, parts, state);
-  end();
-  begin("ap_place_kernel");
+  ln.end();
+  ln.begin("ap_place_kernel");
   ap_place_kernel<<<pb, AP_THREADS, 0, stream>>>(g, parts, state, tab, recs, d_frames, lay.pad_frame, (uint64_t(mp) + 1) * sizeof(IndexChunk));
-  end();
-  begin("frame_pages_kernel");
+  ln.end();
+  ln.begin("frame_pages_kernel");
   frame_pages_kernel<<<mp, WRAP_THREADS, 0, stream>>>(g.metas, g.metas_cap, g.pages, g.dtype, tab, d_frames, pstat);
-  end();
-  begin("walk_kernel");
+  ln.end();
+  ln.begin("walk_kernel");
   walk_kernel<SMALL_MAX_SIZE_LOG><<<mp, WALK_THREADS, sizeof(WalkSmem<SMALL_MAX_SIZE_LOG>), stream>>>(
       fp, d_idx, 0, mp, 0, lay.index_len, 0, 0, ~uint64_t(0), wst, &state->walk, 0, ends);
-  end();
-  begin("ap_route_kernel");
+  ln.end();
+  ln.begin("ap_route_kernel");
   ap_route_kernel<<<1, AP_SCAN_THREADS, 0, stream>>>(g, state, tab, recs, pstat, wst, ends, table, fast_page, cold_list, fp.src_len);
-  end();
-  begin("ap_rewalk_kernel");
+  ln.end();
+  ln.begin("ap_rewalk_kernel");
   ap_rewalk_kernel<<<1, WALK_THREADS, sizeof(WalkSmem<SMALL_MAX_SIZE_LOG>), stream>>>(g, state, tab, d_frames, d_idx, lay.index_len);
-  end();
-  begin("fused_narrow_kernel");
+  ln.end();
+  enqueue_decode_stage<false>(ln, DecodeStage{fp, table, d_idx, lay.index_len, mp, d_st, ws + lay.cls, ws + lay.syms,
+                                              reinterpret_cast<uint32_t*>(ws + lay.offs), &chk->binoms, dst, g.dst_cap, nullptr});
+  ln.begin("ap_cold_kernel");
   dispatch_latent(plan->dtype, [&](auto tag) {
     using L = decltype(tag);
-    fused_narrow_kernel<L><<<mp, FZ_THREADS, sizeof(FusedSmem), stream>>>(fp, table, d_idx, lay.index_len, d_st, d_cls, static_cast<L*>(dst), g.dst_cap);
+    ap_cold_kernel<L><<<1, ASYNC_THREADS, 0, stream>>>(g, state, tab, recs, d_st, fast_page, cold_list, d_frames, static_cast<L*>(dst), ws + lay.cold);
     return 0;
   });
-  end();
-  begin("symwalk_kernel");
-  symwalk_kernel<false><<<mp, SW_THREADS, sizeof(SymWalkSmem), stream>>>(fp, table, d_idx, lay.index_len, g.dst_cap, d_syms, d_offs, d_cls);
-  end();
-  begin("decode_kernel");
-  dispatch_latent(plan->dtype, [&](auto tag) {
-    using L = decltype(tag);
-    decode_kernel<L, 1><<<mp, DEC_THREADS, sizeof(DecodeSmem), stream>>>(fp, table, d_st, d_idx, lay.index_len, static_cast<L*>(dst), g.dst_cap, &chk->binoms,
-                                                                          d_syms, d_offs, d_cls);
-    decode_kernel<L, 2><<<mp, DEC_THREADS, sizeof(DecodeSmem), stream>>>(fp, table, d_st, d_idx, lay.index_len, static_cast<L*>(dst), g.dst_cap, &chk->binoms,
-                                                                          d_syms, d_offs, d_cls);
-    return 0;
-  });
-  end();
-  begin("ap_cold_kernel");
-  dispatch_latent(plan->dtype, [&](auto tag) {
-    using L = decltype(tag);
-    ap_cold_kernel<L><<<1, ASYNC_THREADS, 0, stream>>>(g, state, tab, recs, d_st, fast_page, cold_list, d_frames, static_cast<L*>(dst), d_cold);
-    return 0;
-  });
-  end();
-  begin("ap_finish_kernel");
+  ln.end();
+  ln.begin("ap_finish_kernel");
   ap_finish_kernel<<<1, 32, 0, stream>>>(state, status);
-  end();
+  ln.end();
   PCOB_CUDA_TRY(cudaGetLastError());
   return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
 }
@@ -3169,13 +3071,11 @@ PcoB200Error pco_b200_compress_async_plan(size_t n, unsigned char dtype, const P
   // use, and every kernel the call launches loaded now (with lazy module loading a kernel is otherwise loaded at its first launch)
   Context& c = ctx();
   if (PcoB200Error e = ensure_device(c)) return e;
-  cudaFuncAttributes fa;
-  for (const void* k : {(const void*)acomp_init_kernel, (const void*)acomp_two_gate_kernel, (const void*)acomp_var_gate_kernel,
-                        (const void*)acomp_pack_gate_kernel, (const void*)acomp_finish_kernel, (const void*)init_chunks_kernel,
-                        (const void*)segment_offsets_kernel, (const void*)fallback_kernel<false>, (const void*)ans_encode_kernel<false>,
-                        (const void*)layout_kernel<false>, (const void*)chunk_offsets_kernel, (const void*)header_footer_kernel,
-                        (const void*)emit_index_kernel})
-    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, k));
+  if (PcoB200Error e = load_kernels({(const void*)acomp_init_kernel, (const void*)acomp_two_gate_kernel, (const void*)acomp_var_gate_kernel,
+                                     (const void*)acomp_pack_gate_kernel, (const void*)acomp_finish_kernel, (const void*)init_chunks_kernel,
+                                     (const void*)segment_offsets_kernel, (const void*)fallback_kernel<false>, (const void*)ans_encode_kernel<false>,
+                                     (const void*)layout_kernel<false>, (const void*)chunk_offsets_kernel, (const void*)header_footer_kernel,
+                                     (const void*)emit_index_kernel})) return e;
   return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
     using L = decltype(tag);
     constexpr size_t RS_SMEM = size_t(RS_WARPS) * RS_BINS * sizeof(uint32_t);
@@ -3187,12 +3087,10 @@ PcoB200Error pco_b200_compress_async_plan(size_t n, unsigned char dtype, const P
     PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
     PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
     PCOB_CUDA_TRY(cudaFuncSetAttribute(bin_lut_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    for (const void* k : {(const void*)split_count_kernel<L>, (const void*)split_delta_kernel<L, MODE_CLASSIC>, (const void*)split_delta_kernel<L, MODE_INT_MULT>,
-                          (const void*)split_delta_kernel<L, MODE_FLOAT_QUANT>, (const void*)split_delta_kernel<L, MODE_FLOAT_MULT>,
-                          (const void*)plan_probe_kernel<L, false>, (const void*)sort_keys_kernel<L>, (const void*)plan_solve_kernel<L>,
-                          (const void*)bin_kernel<L, false>})
-      PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, k));
-    return PCO_B200_OK;
+    return load_kernels({(const void*)split_count_kernel<L>, (const void*)split_delta_kernel<L, MODE_CLASSIC>, (const void*)split_delta_kernel<L, MODE_INT_MULT>,
+                         (const void*)split_delta_kernel<L, MODE_FLOAT_QUANT>, (const void*)split_delta_kernel<L, MODE_FLOAT_MULT>,
+                         (const void*)plan_probe_kernel<L, false>, (const void*)sort_keys_kernel<L>, (const void*)plan_solve_kernel<L>,
+                         (const void*)bin_kernel<L, false>});
   });
 }
 
@@ -3206,12 +3104,8 @@ PcoB200Error pco_b200_compress_async(const PcoB200AsyncCompressPlan* plan, const
   if (index && plan->index_cap == 0) return fail(PCO_B200_INVALID_ARGUMENT, "an index with a plan made without one (index_cap 0)");
   if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
   if (reinterpret_cast<uintptr_t>(index) & 15) return fail(PCO_B200_INVALID_ARGUMENT, "the index is not 16-byte aligned");
-  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  PCOB_CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
-  // kernel spans only outside a capture (an event record would become part of the graph); those of an earlier call that nobody read go
-  const bool prof = cap == cudaStreamCaptureStatusNone && profiler_enabled().load(std::memory_order_relaxed);
-  if (prof) profiler().discard();
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
   a.n = plan->n;
   a.n_chunks = g.n_chunks;
   a.low = g.low;
@@ -3224,7 +3118,7 @@ PcoB200Error pco_b200_compress_async(const PcoB200AsyncCompressPlan* plan, const
   a.index = static_cast<uint8_t*>(index);
   a.header_bytes = standalone_header_into(plan->n, uint8_t(plan->uniform_type_header ? plan->dtype : 0), a.header);
   dispatch_latent(plan->dtype, [&](auto tag) {
-    acomp_launch<decltype(tag)>(*plan, g, a, nums, status, stream, prof);
+    acomp_launch<decltype(tag)>(*plan, g, a, nums, status, ln);
     return 0;
   });
   PCOB_CUDA_TRY(cudaGetLastError());
@@ -3305,13 +3199,11 @@ PcoB200Error pco_b200_compress_files_async_plan(unsigned char dtype, const PcoB2
   // the one-time device set-up (compress_async_plan's, for this call's kernels)
   Context& c = ctx();
   if (PcoB200Error e = ensure_device(c)) return e;
-  cudaFuncAttributes fa;
-  for (const void* k : {(const void*)acf_files_kernel, (const void*)acf_scan_kernel, (const void*)acf_place_kernel, (const void*)acf_init_kernel,
-                        (const void*)acf_bytes_kernel, (const void*)acf_bytes_scan_kernel, (const void*)acf_offsets_kernel, (const void*)acf_frame_kernel,
-                        (const void*)acf_index_kernel, (const void*)acf_finish_kernel, (const void*)acomp_two_gate_kernel, (const void*)acomp_var_gate_kernel,
-                        (const void*)acomp_pack_gate_kernel, (const void*)segment_offsets_kernel, (const void*)fallback_kernel<false>,
-                        (const void*)ans_encode_kernel<false>, (const void*)layout_kernel<false>})
-    PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, k));
+  if (PcoB200Error e = load_kernels({(const void*)acf_files_kernel, (const void*)acf_scan_kernel, (const void*)acf_place_kernel, (const void*)acf_init_kernel,
+                                     (const void*)acf_bytes_kernel, (const void*)acf_bytes_scan_kernel, (const void*)acf_offsets_kernel, (const void*)acf_frame_kernel,
+                                     (const void*)acf_index_kernel, (const void*)acf_finish_kernel, (const void*)acomp_two_gate_kernel, (const void*)acomp_var_gate_kernel,
+                                     (const void*)acomp_pack_gate_kernel, (const void*)segment_offsets_kernel, (const void*)fallback_kernel<false>,
+                                     (const void*)ans_encode_kernel<false>, (const void*)layout_kernel<false>})) return e;
   return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
     using L = decltype(tag);
     constexpr size_t RS_SMEM = size_t(RS_WARPS) * RS_BINS * sizeof(uint32_t);
@@ -3323,12 +3215,10 @@ PcoB200Error pco_b200_compress_files_async_plan(unsigned char dtype, const PcoB2
     PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true, false, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
     PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
     PCOB_CUDA_TRY(cudaFuncSetAttribute(bin_lut_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    for (const void* k : {(const void*)split_count_kernel<L, true>, (const void*)split_delta_kernel<L, MODE_CLASSIC>, (const void*)split_delta_kernel<L, MODE_INT_MULT>,
-                          (const void*)split_delta_kernel<L, MODE_FLOAT_QUANT>, (const void*)split_delta_kernel<L, MODE_FLOAT_MULT>,
-                          (const void*)plan_probe_kernel<L, false, false, true>, (const void*)sort_keys_kernel<L>, (const void*)plan_solve_kernel<L, true>,
-                          (const void*)bin_kernel<L, false>})
-      PCOB_CUDA_TRY(cudaFuncGetAttributes(&fa, k));
-    return PCO_B200_OK;
+    return load_kernels({(const void*)split_count_kernel<L, true>, (const void*)split_delta_kernel<L, MODE_CLASSIC>, (const void*)split_delta_kernel<L, MODE_INT_MULT>,
+                         (const void*)split_delta_kernel<L, MODE_FLOAT_QUANT>, (const void*)split_delta_kernel<L, MODE_FLOAT_MULT>,
+                         (const void*)plan_probe_kernel<L, false, false, true>, (const void*)sort_keys_kernel<L>, (const void*)plan_solve_kernel<L, true>,
+                         (const void*)bin_kernel<L, false>});
   });
 }
 
@@ -3342,11 +3232,8 @@ PcoB200Error pco_b200_compress_files_async(const PcoB200AsyncCompressFilesPlan* 
   if (index && plan->index_cap == 0) return fail(PCO_B200_INVALID_ARGUMENT, "an index with a plan made without one (index_cap 0)");
   if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
   if (reinterpret_cast<uintptr_t>(index) & 15) return fail(PCO_B200_INVALID_ARGUMENT, "the index is not 16-byte aligned");
-  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  PCOB_CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
-  const bool prof = cap == cudaStreamCaptureStatusNone && profiler_enabled().load(std::memory_order_relaxed);
-  if (prof) profiler().discard();
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
   AcfArgs fa;
   std::memset(&fa, 0, sizeof(fa));
   fa.a.n_chunks = pg.g.n_chunks;
@@ -3368,7 +3255,7 @@ PcoB200Error pco_b200_compress_files_async(const PcoB200AsyncCompressFilesPlan* 
   fa.uniform_type = plan->uniform_type_header ? plan->dtype : 0;
   fa.bpc = pg.g.bpc;
   dispatch_latent(plan->dtype, [&](auto tag) {
-    acf_launch<decltype(tag)>(*plan, pg.g, fa, nums, status, stream, prof);
+    acf_launch<decltype(tag)>(*plan, pg.g, fa, nums, status, ln);
     return 0;
   });
   PCOB_CUDA_TRY(cudaGetLastError());

@@ -98,6 +98,24 @@ inline Profiler& profiler() {
   return p;
 }
 
+// The caller's stream of an asynchronous call, and whether its launches record kernel spans: only outside a capture (an event record
+// would become part of the graph).  Opening it drops the spans of an earlier call that nobody read.
+struct AsyncLaunch {
+  cudaStream_t stream;
+  bool prof;
+  void begin(const char* name) const { if (prof) profiler().begin(name, stream); }
+  void end() const { if (prof) profiler().end(stream); }
+};
+inline PcoB200Error open_async_launch(void* cuda_stream, AsyncLaunch* ln) {
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  PCOB_CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
+  ln->stream = stream;
+  ln->prof = cap == cudaStreamCaptureStatusNone && profiler_enabled().load(std::memory_order_relaxed);
+  if (ln->prof) profiler().discard();
+  return PCO_B200_OK;
+}
+
 // ---- PCOB200_TRACE=1: host-clock marks of a call's phases on stderr (one line per call; all threads share the epoch) ------------------
 inline bool trace_enabled() {
   static const bool on = std::getenv("PCOB200_TRACE") != nullptr;

@@ -397,16 +397,13 @@ class _CAsyncStatus(C.Structure):  # PcoB200AsyncStatus (include/pco_b200.h)
 
 
 def _lib_async():
-    L = _lib.lib()
-    if not getattr(L, "_async_ready", False):
-        L.pco_b200_decompress_async_plan.argtypes = [C.c_void_p, C.c_size_t, C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p]
-        L.pco_b200_decompress_async.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.pco_b200_decompress_async_result.argtypes = [C.c_void_p, C.c_void_p]
-        L._async_ready = True
-    return L
+    return _lib.bind("_async_ready",
+                     pco_b200_decompress_async_plan=[C.c_void_p, C.c_size_t, C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p],
+                     pco_b200_decompress_async=[C.c_void_p] * 7,
+                     pco_b200_decompress_async_result=[C.c_void_p, C.c_void_p])
 
 
-class AsyncDecompressor:
+class AsyncDecompressor(_lib._AsyncCall):
     """Decodes indexed standalone files on the current CUDA stream without waiting for the device (pco_b200_decompress_async): a call
     only enqueues kernels, so it can run behind other GPU work while the host moves on, and it can be captured in a torch.cuda.CUDAGraph.
 
@@ -416,55 +413,36 @@ class AsyncDecompressor:
     count come from each file's side index on the device, so one captured call decodes whatever file its buffers hold on each replay.
     The decompressor owns a device workspace and a status word; it serves one call in flight at a time (calls on one stream queue up)."""
 
+    _Plan, _Status = _CAsyncPlan, _CAsyncStatus
+
     def __init__(self, head, dtype, src_cap, index_cap, dst_cap, max_chunks, device=None):
-        import torch
-
-        from .wrapped import _host_u8
-
         self.dtype = np.dtype(dtype)
-        if _is_cuda(head):
-            head = head.reshape(-1)[:32].cpu().numpy()
-        h = _host_u8(head)[:32].copy()
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        L = _lib_async()
-        self._plan = _CAsyncPlan()
-        with torch.cuda.device(self.device):
-            rc = L.pco_b200_decompress_async_plan(h.ctypes.data_as(C.c_void_p), C.c_size_t(h.size), C.c_ubyte(_lib.dtype_byte(self.dtype)),
-                                                  C.c_size_t(src_cap), C.c_size_t(index_cap), C.c_size_t(dst_cap), C.c_size_t(max_chunks),
-                                                  C.byref(self._plan))
-        _lib.check(rc)
-        self.workspace = torch.empty(self._plan.workspace_bytes, dtype=torch.uint8, device=self.device)
-        self.status = torch.zeros(C.sizeof(_CAsyncStatus), dtype=torch.uint8, device=self.device)
-
-    @property
-    def workspace_bytes(self):
-        return int(self._plan.workspace_bytes)
+        h = self._head(head)
+        self._make_plan(device, lambda plan: _lib_async().pco_b200_decompress_async_plan(
+            h.ctypes.data_as(C.c_void_p), C.c_size_t(h.size), C.c_ubyte(_lib.dtype_byte(self.dtype)), C.c_size_t(src_cap), C.c_size_t(index_cap),
+            C.c_size_t(dst_cap), C.c_size_t(max_chunks), plan))
+        self._alloc()
 
     def __call__(self, src, index, dst):
         """Enqueues the decode of the file in `src` (uint8 CUDA tensor of at least src_cap bytes) through its side index `index` (at least
         index_cap bytes) into `dst` (a CUDA tensor of the plan's dtype, at least dst_cap numbers) on torch.cuda.current_stream().  Returns
         nothing and does not wait; result() reports the outcome."""
-        import torch
-
         from .wrapped import _torch_dtypes
 
         p = self._plan
-        for name, t in (("src", src), ("index", index), ("dst", dst)):
-            if not _is_cuda(t) or t.device != self.device or not t.is_contiguous():
-                raise ValueError(f"{name} must be a contiguous CUDA tensor on {self.device}")
+        self._check_tensors(src=src, index=index, dst=dst)
         if src.numel() * src.element_size() < p.src_cap or index.numel() * index.element_size() < p.index_cap:
             raise ValueError(f"src holds fewer than src_cap = {p.src_cap} bytes, or index fewer than index_cap = {p.index_cap}")
         if dst.dtype != _torch_dtypes()[self.dtype] or dst.numel() < p.dst_cap:
             raise ValueError(f"dst must hold at least dst_cap = {p.dst_cap} numbers of {self.dtype}")
         rc = _lib_async().pco_b200_decompress_async(C.byref(p), C.c_void_p(src.data_ptr()), C.c_void_p(index.data_ptr()), C.c_void_p(dst.data_ptr()),
-                                                    C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()),
-                                                    C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+                                                    C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()), self._stream())
         _lib.check(rc)
 
     def result(self):
         """Copies the status of the last call back (waiting for it on the current stream) and returns its Progress, or raises PcoError
         with the kind pco_b200_decompress_ex gives."""
-        s = _CAsyncStatus.from_buffer_copy(self.status.cpu().numpy().tobytes())
+        s = self.status_record()
         prog = _lib._CProgress()
         _lib.check(_lib_async().pco_b200_decompress_async_result(C.byref(s), C.byref(prog)))
         return Progress(prog.n_processed, bool(prog.finished))
@@ -482,17 +460,14 @@ class _CAsyncRangesStatus(C.Structure):  # PcoB200AsyncRangesStatus (include/pco
 
 
 def _lib_async_ranges():
-    L = _lib.lib()
-    if not getattr(L, "_async_ranges_ready", False):
-        L.pco_b200_decompress_ranges_async_plan.argtypes = [C.c_void_p, C.c_size_t, C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
-                                                            C.c_size_t, C.c_size_t, C.c_void_p]
-        L.pco_b200_decompress_ranges_async.argtypes = [C.c_void_p] * 9
-        L.pco_b200_decompress_ranges_async_result.argtypes = [C.c_void_p, C.POINTER(C.c_size_t)]
-        L._async_ranges_ready = True
-    return L
+    return _lib.bind("_async_ranges_ready",
+                     pco_b200_decompress_ranges_async_plan=[C.c_void_p, C.c_size_t, C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                                            C.c_size_t, C.c_size_t, C.c_void_p],
+                     pco_b200_decompress_ranges_async=[C.c_void_p] * 9,
+                     pco_b200_decompress_ranges_async_result=[C.c_void_p, C.POINTER(C.c_size_t)])
 
 
-class AsyncRangeDecompressor:
+class AsyncRangeDecompressor(_lib._AsyncCall):
     """Decodes ranges of indexed standalone files on the current CUDA stream with the ranges in device memory and without waiting for the
     device (pco_b200_decompress_ranges_async): positions a kernel produced need no trip to the host, and a call can be captured in a
     torch.cuda.CUDAGraph.
@@ -503,29 +478,15 @@ class AsyncRangeDecompressor:
     wanted, rounded up to 256).  The number of ranges is read from a device tensor, so one captured call serves a different count, different
     ranges and a different file on each replay.  The decompressor owns a device workspace and a status; it serves one call in flight."""
 
+    _Plan, _Status = _CAsyncRangesPlan, _CAsyncRangesStatus
+
     def __init__(self, head, dtype, src_cap, index_cap, max_chunks, max_ranges, dst_cap, window_cap, device=None):
-        import torch
-
-        from .wrapped import _host_u8
-
         self.dtype = np.dtype(dtype)
-        if _is_cuda(head):
-            head = head.reshape(-1)[:32].cpu().numpy()
-        h = _host_u8(head)[:32].copy()
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        L = _lib_async_ranges()
-        self._plan = _CAsyncRangesPlan()
-        with torch.cuda.device(self.device):
-            rc = L.pco_b200_decompress_ranges_async_plan(h.ctypes.data_as(C.c_void_p), C.c_size_t(h.size), C.c_ubyte(_lib.dtype_byte(self.dtype)),
-                                                         C.c_size_t(src_cap), C.c_size_t(index_cap), C.c_size_t(max_chunks), C.c_size_t(max_ranges),
-                                                         C.c_size_t(dst_cap), C.c_size_t(window_cap), C.byref(self._plan))
-        _lib.check(rc)
-        self.workspace = torch.empty(self._plan.workspace_bytes, dtype=torch.uint8, device=self.device)
-        self.status = torch.zeros(C.sizeof(_CAsyncRangesStatus), dtype=torch.uint8, device=self.device)
-
-    @property
-    def workspace_bytes(self):
-        return int(self._plan.workspace_bytes)
+        h = self._head(head)
+        self._make_plan(device, lambda plan: _lib_async_ranges().pco_b200_decompress_ranges_async_plan(
+            h.ctypes.data_as(C.c_void_p), C.c_size_t(h.size), C.c_ubyte(_lib.dtype_byte(self.dtype)), C.c_size_t(src_cap), C.c_size_t(index_cap),
+            C.c_size_t(max_chunks), C.c_size_t(max_ranges), C.c_size_t(dst_cap), C.c_size_t(window_cap), plan))
+        self._alloc()
 
     def __call__(self, src, index, ranges, n_ranges, dst):
         """Enqueues the decode of ranges[: n_ranges[0]] of the file in `src` (uint8 CUDA tensor of at least src_cap bytes) through its side
@@ -537,9 +498,7 @@ class AsyncRangeDecompressor:
         from .wrapped import _torch_dtypes
 
         p = self._plan
-        for name, t in (("src", src), ("index", index), ("ranges", ranges), ("n_ranges", n_ranges), ("dst", dst)):
-            if not _is_cuda(t) or t.device != self.device or not t.is_contiguous():
-                raise ValueError(f"{name} must be a contiguous CUDA tensor on {self.device}")
+        self._check_tensors(src=src, index=index, ranges=ranges, n_ranges=n_ranges, dst=dst)
         if src.numel() * src.element_size() < p.src_cap or index.numel() * index.element_size() < p.index_cap:
             raise ValueError(f"src holds fewer than src_cap = {p.src_cap} bytes, or index fewer than index_cap = {p.index_cap}")
         if ranges.dtype != torch.int64 or ranges.dim() != 2 or ranges.shape[1] != 2 or ranges.shape[0] < p.max_ranges:
@@ -550,13 +509,8 @@ class AsyncRangeDecompressor:
             raise ValueError(f"dst must hold at least dst_cap = {p.dst_cap} numbers of {self.dtype}")
         rc = _lib_async_ranges().pco_b200_decompress_ranges_async(
             C.byref(p), C.c_void_p(src.data_ptr()), C.c_void_p(index.data_ptr()), C.c_void_p(ranges.data_ptr()), C.c_void_p(n_ranges.data_ptr()),
-            C.c_void_p(dst.data_ptr()), C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()),
-            C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+            C.c_void_p(dst.data_ptr()), C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()), self._stream())
         _lib.check(rc)
-
-    def status_record(self):
-        """The last call's PcoB200AsyncRangesStatus, copied back (waiting for it on the current stream)."""
-        return _CAsyncRangesStatus.from_buffer_copy(self.status.cpu().numpy().tobytes())
 
     def result(self):
         """Copies the status of the last call back (waiting for it on the current stream) and returns the number of numbers written, or
@@ -581,16 +535,13 @@ class _CAsyncCompressStatus(C.Structure):  # PcoB200AsyncCompressStatus (include
 
 
 def _lib_async_compress():
-    L = _lib.lib()
-    if not getattr(L, "_async_compress_ready", False):
-        L.pco_b200_compress_async_plan.argtypes = [C.c_size_t, C.c_ubyte, C.c_void_p, C.c_int, C.c_size_t, C.c_size_t, C.c_void_p]
-        L.pco_b200_compress_async.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.pco_b200_compress_async_result.argtypes = [C.c_void_p, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
-        L._async_compress_ready = True
-    return L
+    return _lib.bind("_async_compress_ready",
+                     pco_b200_compress_async_plan=[C.c_size_t, C.c_ubyte, C.c_void_p, C.c_int, C.c_size_t, C.c_size_t, C.c_void_p],
+                     pco_b200_compress_async=[C.c_void_p] * 7,
+                     pco_b200_compress_async_result=[C.c_void_p, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)])
 
 
-class AsyncCompressor:
+class AsyncCompressor(_lib._AsyncCall):
     """Compresses n numbers on the current CUDA stream without waiting for the device (pco_b200_compress_async): a call only enqueues
     kernels, so it can run behind other GPU work while the host moves on, and it can be captured in a torch.cuda.CUDAGraph.
 
@@ -601,28 +552,26 @@ class AsyncCompressor:
     numbers and config.  The compressor owns a device workspace and a status word; it serves one call in flight at a time (calls on one
     stream queue up)."""
 
-    def __init__(self, n, dtype, config=None, dst_cap=None, index=True, uniform_type_header=False, device=None):
-        import torch
+    _Plan, _Status = _CAsyncCompressPlan, _CAsyncCompressStatus
 
+    def __init__(self, n, dtype, config=None, dst_cap=None, index=True, uniform_type_header=False, device=None):
         self.dtype = np.dtype(dtype)
         self.n = int(n)
         dtb = _lib.dtype_byte(self.dtype)
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         L = _lib_async_compress()
         if dst_cap is None:
             dst_cap = L.pco_standalone_guarantee_file_size(self.n, dtb)
         cfg = (config or ChunkConfig())._to_c()
-        self._plan = _CAsyncCompressPlan()
-        with torch.cuda.device(self.device):
-            if index:  # the exact index size is known once the plan exists: a first plan without an index reports it
-                rc = L.pco_b200_compress_async_plan(C.c_size_t(self.n), C.c_ubyte(dtb), C.byref(cfg), C.c_int(1 if uniform_type_header else 0),
-                                                    C.c_size_t(dst_cap), C.c_size_t(0), C.byref(self._plan))
-                _lib.check(rc)
-            rc = L.pco_b200_compress_async_plan(C.c_size_t(self.n), C.c_ubyte(dtb), C.byref(cfg), C.c_int(1 if uniform_type_header else 0),
-                                                C.c_size_t(dst_cap), C.c_size_t(self._plan.index_bytes if index else 0), C.byref(self._plan))
-        _lib.check(rc)
-        self.workspace = torch.empty(max(self._plan.workspace_bytes, 1), dtype=torch.uint8, device=self.device)
-        self.status = torch.zeros(C.sizeof(_CAsyncCompressStatus), dtype=torch.uint8, device=self.device)
+
+        def plan_fn(index_cap):
+            return lambda plan: L.pco_b200_compress_async_plan(C.c_size_t(self.n), C.c_ubyte(dtb), C.byref(cfg), C.c_int(1 if uniform_type_header else 0),
+                                                               C.c_size_t(dst_cap), C.c_size_t(index_cap), plan)
+
+        # the exact index size is known once the plan exists: a first plan without an index reports it
+        self._make_plan(device, plan_fn(0))
+        if index:
+            self._replan(plan_fn(self._plan.index_bytes))
+        self._alloc()
 
     @property
     def dst_cap(self):
@@ -633,22 +582,14 @@ class AsyncCompressor:
         """Bytes of the side index each call writes (0 without one)."""
         return int(self._plan.index_cap and self._plan.index_bytes)
 
-    @property
-    def workspace_bytes(self):
-        return int(self._plan.workspace_bytes)
-
     def __call__(self, nums, dst, index=None):
         """Enqueues the compress of `nums` (a CUDA tensor of the plan's dtype and n numbers) into `dst` (uint8 CUDA tensor of at least dst_cap
         bytes) and, when given, the side index into `index` (uint8 CUDA tensor of at least index_bytes bytes) on torch.cuda.current_stream().
         Returns nothing and does not wait; result() reports the outcome."""
-        import torch
-
         from .wrapped import _torch_dtypes
 
         p = self._plan
-        for name, t in (("nums", nums), ("dst", dst)) + ((("index", index),) if index is not None else ()):
-            if not _is_cuda(t) or t.device != self.device or not t.is_contiguous():
-                raise ValueError(f"{name} must be a contiguous CUDA tensor on {self.device}")
+        self._check_tensors(nums=nums, dst=dst, **({"index": index} if index is not None else {}))
         if nums.dtype != _torch_dtypes()[self.dtype] or nums.numel() != self.n:
             raise ValueError(f"nums must hold n = {self.n} numbers of {self.dtype}")
         if dst.numel() * dst.element_size() < p.dst_cap:
@@ -657,14 +598,13 @@ class AsyncCompressor:
             raise ValueError(f"index needs a compressor made with index=True and at least {p.index_bytes} bytes")
         rc = _lib_async_compress().pco_b200_compress_async(C.byref(p), C.c_void_p(nums.data_ptr()), C.c_void_p(dst.data_ptr()),
                                                           C.c_void_p(index.data_ptr()) if index is not None else None,
-                                                          C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()),
-                                                          C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+                                                          C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()), self._stream())
         _lib.check(rc)
 
     def result(self):
         """Copies the status of the last call back (waiting for it on the current stream) and returns (file_bytes, index_bytes), or raises
         PcoError (Io when the file does not fit dst_cap)."""
-        s = _CAsyncCompressStatus.from_buffer_copy(self.status.cpu().numpy().tobytes())
+        s = self.status_record()
         nw, il = C.c_size_t(), C.c_size_t()
         _lib.check(_lib_async_compress().pco_b200_compress_async_result(C.byref(s), C.byref(nw), C.byref(il)))
         return int(nw.value), int(il.value)
@@ -682,17 +622,14 @@ class _CAsyncFilesStatus(C.Structure):  # PcoB200AsyncFilesStatus (include/pco_b
 
 
 def _lib_async_files():
-    L = _lib.lib()
-    if not getattr(L, "_async_files_ready", False):
-        L.pco_b200_decompress_files_async_plan.argtypes = [C.c_void_p, C.c_size_t, C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
-                                                           C.c_size_t, C.c_void_p]
-        L.pco_b200_decompress_files_async.argtypes = [C.c_void_p] * 10
-        L.pco_b200_decompress_files_async_result.argtypes = [C.c_void_p, C.POINTER(C.c_size_t)]
-        L._async_files_ready = True
-    return L
+    return _lib.bind("_async_files_ready",
+                     pco_b200_decompress_files_async_plan=[C.c_void_p, C.c_size_t, C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                                           C.c_size_t, C.c_void_p],
+                     pco_b200_decompress_files_async=[C.c_void_p] * 10,
+                     pco_b200_decompress_files_async_result=[C.c_void_p, C.POINTER(C.c_size_t)])
 
 
-class AsyncFilesDecompressor:
+class AsyncFilesDecompressor(_lib._AsyncCall):
     """Decodes a batch of indexed standalone files on the current CUDA stream with the file list in device memory and without waiting for
     the device (pco_b200_decompress_files_async): refs a kernel picked (a sampler, a cache lookup) need no trip to the host, and a call can
     be captured in a torch.cuda.CUDAGraph.
@@ -703,29 +640,15 @@ class AsyncFilesDecompressor:
     serves different refs, a different count and different files on each replay.  The decompressor owns a device workspace and a status;
     it serves one call in flight."""
 
+    _Plan, _Status = _CAsyncFilesPlan, _CAsyncFilesStatus
+
     def __init__(self, head, dtype, src_cap, index_cap, max_files, max_chunks, dst_cap, device=None):
-        import torch
-
-        from .wrapped import _host_u8
-
         self.dtype = np.dtype(dtype)
-        if _is_cuda(head):
-            head = head.reshape(-1)[:32].cpu().numpy()
-        h = _host_u8(head)[:32].copy()
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        L = _lib_async_files()
-        self._plan = _CAsyncFilesPlan()
-        with torch.cuda.device(self.device):
-            rc = L.pco_b200_decompress_files_async_plan(h.ctypes.data_as(C.c_void_p), C.c_size_t(h.size), C.c_ubyte(_lib.dtype_byte(self.dtype)),
-                                                        C.c_size_t(src_cap), C.c_size_t(index_cap), C.c_size_t(max_files), C.c_size_t(max_chunks),
-                                                        C.c_size_t(dst_cap), C.byref(self._plan))
-        _lib.check(rc)
-        self.workspace = torch.empty(self._plan.workspace_bytes, dtype=torch.uint8, device=self.device)
-        self.status = torch.zeros(C.sizeof(_CAsyncFilesStatus), dtype=torch.uint8, device=self.device)
-
-    @property
-    def workspace_bytes(self):
-        return int(self._plan.workspace_bytes)
+        h = self._head(head)
+        self._make_plan(device, lambda plan: _lib_async_files().pco_b200_decompress_files_async_plan(
+            h.ctypes.data_as(C.c_void_p), C.c_size_t(h.size), C.c_ubyte(_lib.dtype_byte(self.dtype)), C.c_size_t(src_cap), C.c_size_t(index_cap),
+            C.c_size_t(max_files), C.c_size_t(max_chunks), C.c_size_t(dst_cap), plan))
+        self._alloc()
 
     def __call__(self, src, index, files, n_files, dst, file_ns):
         """Enqueues the decode of files[: n_files[0]] into `dst` (a CUDA tensor of the plan's dtype, at least dst_cap numbers) on
@@ -738,9 +661,7 @@ class AsyncFilesDecompressor:
         from .wrapped import _torch_dtypes
 
         p = self._plan
-        for name, t in (("src", src), ("index", index), ("files", files), ("n_files", n_files), ("dst", dst), ("file_ns", file_ns)):
-            if not _is_cuda(t) or t.device != self.device or not t.is_contiguous():
-                raise ValueError(f"{name} must be a contiguous CUDA tensor on {self.device}")
+        self._check_tensors(src=src, index=index, files=files, n_files=n_files, dst=dst, file_ns=file_ns)
         if src.numel() * src.element_size() < p.src_cap or index.numel() * index.element_size() < p.index_cap:
             raise ValueError(f"src holds fewer than src_cap = {p.src_cap} bytes, or index fewer than index_cap = {p.index_cap}")
         if files.dtype != torch.int64 or files.dim() != 2 or files.shape[1] != 4 or files.shape[0] < p.max_files:
@@ -754,12 +675,8 @@ class AsyncFilesDecompressor:
         rc = _lib_async_files().pco_b200_decompress_files_async(
             C.byref(p), C.c_void_p(src.data_ptr()), C.c_void_p(index.data_ptr()), C.c_void_p(files.data_ptr()), C.c_void_p(n_files.data_ptr()),
             C.c_void_p(dst.data_ptr()), C.c_void_p(file_ns.data_ptr()), C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()),
-            C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+            self._stream())
         _lib.check(rc)
-
-    def status_record(self):
-        """The last call's PcoB200AsyncFilesStatus, copied back (waiting for it on the current stream)."""
-        return _CAsyncFilesStatus.from_buffer_copy(self.status.cpu().numpy().tobytes())
 
     def result(self):
         """Copies the status of the last call back (waiting for it on the current stream) and returns the number of numbers written, or
@@ -785,17 +702,14 @@ class _CAsyncCompressFilesStatus(C.Structure):  # PcoB200AsyncCompressFilesStatu
 
 
 def _lib_async_compress_files():
-    L = _lib.lib()
-    if not getattr(L, "_async_compress_files_ready", False):
-        L.pco_b200_compress_files_async_plan.argtypes = [C.c_ubyte, C.c_void_p, C.c_int, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
-                                                         C.c_size_t, C.c_void_p]
-        L.pco_b200_compress_files_async.argtypes = [C.c_void_p] * 10
-        L.pco_b200_compress_files_async_result.argtypes = [C.c_void_p, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
-        L._async_compress_files_ready = True
-    return L
+    return _lib.bind("_async_compress_files_ready",
+                     pco_b200_compress_files_async_plan=[C.c_ubyte, C.c_void_p, C.c_int, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                                         C.c_size_t, C.c_void_p],
+                     pco_b200_compress_files_async=[C.c_void_p] * 10,
+                     pco_b200_compress_files_async_result=[C.c_void_p, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)])
 
 
-class AsyncFilesCompressor:
+class AsyncFilesCompressor(_lib._AsyncCall):
     """Compresses a batch of standalone files on the current CUDA stream, with the file sizes in device memory and without waiting for the
     device (pco_b200_compress_files_async): sizes a kernel decided (the tensors of a checkpoint, the blocks a step evicted) need no trip to
     the host, and a call can be captured in a torch.cuda.CUDAGraph.
@@ -807,27 +721,24 @@ class AsyncFilesCompressor:
     a different count, different sizes and different numbers on each replay.  The bytes, the indexes and the refs equal what compress_files
     writes.  The compressor owns a device workspace and a status; it serves one call in flight."""
 
-    def __init__(self, dtype, config, max_files, nums_cap, max_file_n, dst_cap=None, index=True, uniform_type_header=False, device=None):
-        import torch
+    _Plan, _Status = _CAsyncCompressFilesPlan, _CAsyncCompressFilesStatus
 
+    def __init__(self, dtype, config, max_files, nums_cap, max_file_n, dst_cap=None, index=True, uniform_type_header=False, device=None):
         self.dtype = np.dtype(dtype)
         dtb = _lib.dtype_byte(self.dtype)
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         L = _lib_async_compress_files()
         cfg = (config or ChunkConfig())._to_c()
-        self._plan = _CAsyncCompressFilesPlan()
 
-        def plan(dcap, icap):
-            with torch.cuda.device(self.device):
-                return L.pco_b200_compress_files_async_plan(C.c_ubyte(dtb), C.byref(cfg), C.c_int(1 if uniform_type_header else 0), C.c_size_t(max_files),
-                                                            C.c_size_t(nums_cap), C.c_size_t(max_file_n), C.c_size_t(dcap), C.c_size_t(icap),
-                                                            C.byref(self._plan))
+        def plan_fn(dcap, icap):
+            return lambda plan: L.pco_b200_compress_files_async_plan(C.c_ubyte(dtb), C.byref(cfg), C.c_int(1 if uniform_type_header else 0),
+                                                                     C.c_size_t(max_files), C.c_size_t(nums_cap), C.c_size_t(max_file_n),
+                                                                     C.c_size_t(dcap), C.c_size_t(icap), plan)
 
-        if dst_cap is None or index:  # the bounds are known once a plan exists: a first plan reports them
-            _lib.check(plan(dst_cap or 0, 0))
-        _lib.check(plan(self._plan.dst_bound if dst_cap is None else dst_cap, self._plan.index_bound if index else 0))
-        self.workspace = torch.empty(self._plan.workspace_bytes, dtype=torch.uint8, device=self.device)
-        self.status = torch.zeros(C.sizeof(_CAsyncCompressFilesStatus), dtype=torch.uint8, device=self.device)
+        # the bounds are known once a plan exists: a first plan reports them
+        self._make_plan(device, plan_fn(dst_cap or 0, 0))
+        if dst_cap is None or index:
+            self._replan(plan_fn(self._plan.dst_bound if dst_cap is None else dst_cap, self._plan.index_bound if index else 0))
+        self._alloc()
 
     @property
     def dst_cap(self):
@@ -842,10 +753,6 @@ class AsyncFilesCompressor:
     def max_files(self):
         return int(self._plan.max_files)
 
-    @property
-    def workspace_bytes(self):
-        return int(self._plan.workspace_bytes)
-
     def __call__(self, nums, file_ns, n_files, dst, index, files):
         """Enqueues the compress of the first n_files[0] files on torch.cuda.current_stream(): file i is the next file_ns[i] numbers of
         `nums` (a CUDA tensor of the plan's dtype, at least nums_cap numbers).  `file_ns` is an int64 CUDA tensor of at least max_files
@@ -857,9 +764,7 @@ class AsyncFilesCompressor:
         from .wrapped import _torch_dtypes
 
         p = self._plan
-        for name, t in (("nums", nums), ("file_ns", file_ns), ("n_files", n_files), ("dst", dst), ("files", files)) + ((("index", index),) if index is not None else ()):
-            if not _is_cuda(t) or t.device != self.device or not t.is_contiguous():
-                raise ValueError(f"{name} must be a contiguous CUDA tensor on {self.device}")
+        self._check_tensors(nums=nums, file_ns=file_ns, n_files=n_files, dst=dst, files=files, **({"index": index} if index is not None else {}))
         if nums.dtype != _torch_dtypes()[self.dtype] or nums.numel() < p.nums_cap:
             raise ValueError(f"nums must hold at least nums_cap = {p.nums_cap} numbers of {self.dtype}")
         if file_ns.dtype != torch.int64 or file_ns.numel() < p.max_files:
@@ -875,12 +780,8 @@ class AsyncFilesCompressor:
         rc = _lib_async_compress_files().pco_b200_compress_files_async(
             C.byref(p), C.c_void_p(nums.data_ptr()), C.c_void_p(file_ns.data_ptr()), C.c_void_p(n_files.data_ptr()), C.c_void_p(dst.data_ptr()),
             C.c_void_p(index.data_ptr()) if index is not None else None, C.c_void_p(files.data_ptr()), C.c_void_p(self.workspace.data_ptr()),
-            C.c_void_p(self.status.data_ptr()), C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+            C.c_void_p(self.status.data_ptr()), self._stream())
         _lib.check(rc)
-
-    def status_record(self):
-        """The last call's PcoB200AsyncCompressFilesStatus, copied back (waiting for it on the current stream)."""
-        return _CAsyncCompressFilesStatus.from_buffer_copy(self.status.cpu().numpy().tobytes())
 
     def result(self):
         """Copies the status of the last call back (waiting for it on the current stream) and returns (dst_len, index_len), the bytes

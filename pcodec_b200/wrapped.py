@@ -245,16 +245,13 @@ class _CAsyncPagesStatus(C.Structure):  # PcoB200AsyncPagesStatus (include/pco_b
 
 
 def _lib_async_pages():
-    L = _lib.lib()
-    if not getattr(L, "_async_pages_ready", False):
-        L.pco_b200_decompress_pages_async_plan.argtypes = [C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p]
-        L.pco_b200_decompress_pages_async.argtypes = [C.c_void_p] * 9
-        L.pco_b200_decompress_pages_async_result.argtypes = [C.c_void_p, C.POINTER(C.c_size_t)]
-        L._async_pages_ready = True
-    return L
+    return _lib.bind("_async_pages_ready",
+                     pco_b200_decompress_pages_async_plan=[C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p],
+                     pco_b200_decompress_pages_async=[C.c_void_p] * 9,
+                     pco_b200_decompress_pages_async_result=[C.c_void_p, C.POINTER(C.c_size_t)])
 
 
-class AsyncPagesDecompressor:
+class AsyncPagesDecompressor(_lib._AsyncCall):
     """Decodes a batch of wrapped-format pages on the current CUDA stream with the page refs in device memory and without waiting for the
     device (pco_b200_decompress_pages_async): pages a kernel kept (a filter on page statistics, a row-group selection) need no trip to the
     host, and a call can be captured in a torch.cuda.CUDAGraph.
@@ -266,25 +263,16 @@ class AsyncPagesDecompressor:
     from a device tensor, so one captured call serves different refs, a different count and different bytes on each replay.  The
     decompressor owns a device workspace and a status; it serves one call in flight."""
 
-    def __init__(self, dtype, metas_cap, pages_cap, max_pages, dst_cap, frame_cap=None, device=None):
-        import torch
+    _Plan, _Status = _CAsyncPagesPlan, _CAsyncPagesStatus
 
+    def __init__(self, dtype, metas_cap, pages_cap, max_pages, dst_cap, frame_cap=None, device=None):
         self.dtype = np.dtype(dtype)
         if frame_cap is None:
             frame_cap = metas_cap + pages_cap + 20 * max_pages
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        L = _lib_async_pages()
-        self._plan = _CAsyncPagesPlan()
-        with torch.cuda.device(self.device):
-            rc = L.pco_b200_decompress_pages_async_plan(C.c_ubyte(_lib.dtype_byte(self.dtype)), C.c_size_t(metas_cap), C.c_size_t(pages_cap),
-                                                        C.c_size_t(max_pages), C.c_size_t(dst_cap), C.c_size_t(frame_cap), C.byref(self._plan))
-        _lib.check(rc)
-        self.workspace = torch.empty(self._plan.workspace_bytes, dtype=torch.uint8, device=self.device)
-        self.status = torch.zeros(C.sizeof(_CAsyncPagesStatus), dtype=torch.uint8, device=self.device)
-
-    @property
-    def workspace_bytes(self):
-        return int(self._plan.workspace_bytes)
+        self._make_plan(device, lambda plan: _lib_async_pages().pco_b200_decompress_pages_async_plan(
+            C.c_ubyte(_lib.dtype_byte(self.dtype)), C.c_size_t(metas_cap), C.c_size_t(pages_cap), C.c_size_t(max_pages), C.c_size_t(dst_cap),
+            C.c_size_t(frame_cap), plan))
+        self._alloc()
 
     def __call__(self, metas, pages, refs, n_pages, dst):
         """Enqueues the decode of the pages refs[: n_pages[0]] names into `dst` (a CUDA tensor of the plan's dtype, at least dst_cap
@@ -295,9 +283,7 @@ class AsyncPagesDecompressor:
         import torch
 
         p = self._plan
-        for name, t in (("metas", metas), ("pages", pages), ("refs", refs), ("n_pages", n_pages), ("dst", dst)):
-            if not _is_cuda(t) or t.device != self.device or not t.is_contiguous():
-                raise ValueError(f"{name} must be a contiguous CUDA tensor on {self.device}")
+        self._check_tensors(metas=metas, pages=pages, refs=refs, n_pages=n_pages, dst=dst)
         if metas.numel() * metas.element_size() < p.metas_cap or pages.numel() * pages.element_size() < p.pages_cap:
             raise ValueError(f"metas holds fewer than metas_cap = {p.metas_cap} bytes, or pages fewer than pages_cap = {p.pages_cap}")
         if refs.dtype != torch.int64 or refs.dim() != 2 or refs.shape[1] != 5 or refs.shape[0] < p.max_pages:
@@ -308,13 +294,8 @@ class AsyncPagesDecompressor:
             raise ValueError(f"dst must hold at least dst_cap = {p.dst_cap} numbers of {self.dtype}")
         rc = _lib_async_pages().pco_b200_decompress_pages_async(
             C.byref(p), C.c_void_p(metas.data_ptr()), C.c_void_p(pages.data_ptr()), C.c_void_p(refs.data_ptr()), C.c_void_p(n_pages.data_ptr()),
-            C.c_void_p(dst.data_ptr()), C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()),
-            C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+            C.c_void_p(dst.data_ptr()), C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()), self._stream())
         _lib.check(rc)
-
-    def status_record(self):
-        """The last call's PcoB200AsyncPagesStatus, copied back (waiting for it on the current stream)."""
-        return _CAsyncPagesStatus.from_buffer_copy(self.status.cpu().numpy().tobytes())
 
     def result(self):
         """Copies the status of the last call back (waiting for it on the current stream) and returns the number of numbers written, or
