@@ -775,6 +775,92 @@ PcoB200Error pco_b200_decompress_pages_async(const PcoB200AsyncPagesPlan *plan, 
  * NULL) to the sum of page_n. */
 PcoB200Error pco_b200_decompress_pages_async_result(const PcoB200AsyncPagesStatus *host_status, size_t *n_written);
 
+/* ---- asynchronous batch compress into wrapped-format chunks (no reference counterpart): pco_b200_compress_wrapped over a batch of
+ * arrays, with the array sizes, their count and every buffer in device memory.  A GPU writer of a container that embeds pco (a columnar
+ * file whose column chunks a kernel sized, a page store) compresses every column chunk behind the step that produced it, with no copy to
+ * the host, and writes its metas and pages where it keeps them.  It only enqueues kernels on the caller's stream and returns at once; it
+ * makes no synchronising, allocating or host-to-device copy call and refers to no memory of the library's per-thread scratch, so it can be
+ * captured in a CUDA graph, and a captured call may be replayed after pco_b200_thread_release or after any other call.  A plan made once
+ * outside any capture fixes the config and the grids from its capacities; the sizes and their count are read on the device, so one
+ * captured graph serves a different count, different sizes and different numbers on each replay.  The refs come out in the layout
+ * pco_b200_decompress_pages_async reads, so one graph can hold a compress and a decode of the same pages.  The whole batch is one pass of
+ * the encode kernels of pco_b200_compress_files_async, whatever unoptimized_bins_log its chunks' sizes imply. */
+typedef struct PcoB200AsyncCompressWrappedPlan {  /* filled by pco_b200_compress_wrapped_async_plan; treat as opaque */
+  uint32_t dtype, mode, order, n_vars;
+  uint32_t level, mode_k, reserved0, reserved1;
+  uint64_t max_arrays, nums_cap, max_array_n, max_page_n, max_chunks, metas_cap, pages_cap;
+  uint64_t mode_base, base_bits, inv_base_bits;
+  uint64_t metas_bound;                           /* bytes of metas every batch within the capacities fits in */
+  uint64_t pages_bound;                           /* bytes of pages every batch within the capacities fits in */
+  uint64_t workspace_bytes;                       /* device workspace one in-flight call needs */
+} PcoB200AsyncCompressWrappedPlan;
+
+typedef struct PcoB200AsyncCompressWrappedStatus {  /* written on the device by every call */
+  uint32_t kind;                                    /* PcoB200Error */
+  uint32_t device_status;                           /* 0, or the PCO_B200_ASYNC_* code behind the kind */
+  uint64_t array;                                   /* the array a refusal names (UINT64_MAX if none) */
+  uint64_t n_arrays;                                /* *n_arrays as the call read it */
+  uint64_t n_chunks;                                /* chunks of the batch (0 when refused before placement) */
+  uint64_t metas_bytes;                             /* bytes of metas the batch needs, also when above metas_cap (0 when refused earlier) */
+  uint64_t pages_bytes;                             /* bytes of pages it needs, also when above pages_cap (0 when refused earlier) */
+  uint64_t metas_written;                           /* bytes written to metas (0 unless OK) */
+  uint64_t pages_written;                           /* bytes written to pages (0 unless OK) */
+} PcoB200AsyncCompressWrappedStatus;
+
+/* Makes a plan for batches of up to max_arrays arrays of dtype, compressed with `config` (NULL = the default config, whose Auto specs are
+ * refused) into wrapped chunks of one page each: at most nums_cap numbers in all, at most max_array_n per array, metas_cap bytes of metas
+ * and pages_cap bytes of pages.  Runs on the host, before and outside any capture.  Refuses what pco_b200_compress_files_async_plan
+ * refuses, with the same kinds and in the same order (max_array_n and max_arrays standing for max_file_n and max_files).  Then *plan is
+ * filled and the one-time device set-up runs on the current device, which the calls must use (kernel attributes, and every kernel the call
+ * launches loaded); without a device that is PCO_B200_CUDA.
+ * The plan's bounds, with m = min(max_page_n (0: 2^18), max_array_n, nums_cap) (at least 1), L the number type's bits, O = log2(L) + 1 the
+ * bits of L's offset width, V the latent vars of the mode (1 for Classic, else 2), P the bits of the mode's parameter (0 for Classic, 8 for
+ * FloatQuant, L for IntMult and FloatMult) and B = ceil((1125 + L + O) / 8) a baseline chunk's metadata (150 bytes for 64-bit numbers):
+ *   max_chunks  = floor(nums_cap / m) + max_arrays                      (chunks of any batch within the capacities)
+ *   pages_bound = max_chunks * (1 + B) + ceil(nums_cap * L / 8)
+ *   metas_bound = min(max_chunks * M, pages_bound), M = ceil((1106 + P + V * (19 + 256 * (15 + L + O))) / 8)
+ * A chunk with its 4 framing bytes is at most 4 + B + ceil(n * L / 8) bytes (pco's size guarantee: a chunk that would be larger is written
+ * in the baseline encoding), so its meta and its page are each at most B + ceil(n * L / 8), and summed over the chunks those are at most
+ * pages_bound (1 per chunk for the rounding).  A meta is also at most M: 4 bits of mode, P, DeltaEncoding's largest encoding (1102 bits),
+ * and per latent var 19 bits of header and at most 256 bins (the plan refuses more unoptimized bins, and a chunk never has more bins than
+ * that) of at most 15 + L + O bits each.
+ * workspace_bytes is pco_b200_compress_files_async_plan's for the same config and capacities (max_files = max_arrays, max_file_n =
+ * max_array_n), plus these regions, each rounded up to 256 bytes: max_chunks * (5 + B) + ceil(nums_cap * L / 8) (the chunks as
+ * pco_b200_compress_wrapped stages them, with their 4 framing bytes), 32 (state), 4 max_chunks (meta lengths) and 32 ceil((max_chunks + 1)
+ * / 256) (CTA sums). */
+PcoB200Error pco_b200_compress_wrapped_async_plan(unsigned char dtype, const PcoB200ChunkConfig *config, size_t max_arrays, size_t nums_cap,
+                                                  size_t max_array_n, size_t metas_cap, size_t pages_cap,
+                                                  PcoB200AsyncCompressWrappedPlan *plan);
+/* Enqueues the compress of arrays[0 : *n_arrays) on `cuda_stream`, and the outcome into *status; returns without waiting.  Array i is the
+ * next array_ns[i] numbers of `nums`; it is cut into the chunks pco_b200_compress_wrapped writes for it alone (the config's
+ * EqualPagesUpTo), and each chunk is one wrapped chunk of one page.  nums (nums_cap numbers), array_ns (uint64_t[max_arrays]), n_arrays
+ * (one uint64_t), metas (metas_cap bytes), pages (pages_cap bytes), refs (PcoB200PageRef[max_chunks]), first_chunk (uint64_t[max_arrays +
+ * 1]), workspace (plan->workspace_bytes, 256-byte aligned) and status are device pointers; one workspace serves one call in flight.  The
+ * metas go back to back into metas, the pages into pages, one ref per chunk into refs, all in array order; array i's chunks are
+ * refs[first_chunk[i] : first_chunk[i + 1]), and first_chunk[*n_arrays] is the number of chunks.  An array of 0 numbers has no chunks, and
+ * *n_arrays = 0 writes first_chunk[0] = 0 and the status only.  For every batch within the capacities, array i's metas and pages equal
+ * what pco_b200_compress_wrapped writes for its numbers alone with the same config and every buffer on the device, right behind array
+ * i - 1's, and its refs equal that call's refs with meta_offset and page_offset moved by the bytes of the arrays before it.
+ * Refusals, in this order, with these PCO_B200_ASYNC_* codes:
+ *   - PCO_B200_ASYNC_TOO_MANY_FILES: *n_arrays is above max_arrays (PCO_B200_INVALID_ARGUMENT);
+ *   - PCO_B200_ASYNC_FILE_TOO_LARGE: array `array` holds more than max_array_n numbers (PCO_B200_INVALID_ARGUMENT);
+ *   - PCO_B200_ASYNC_NUMS_CAP: the counts up to array `array` add up to more than nums_cap (PCO_B200_INVALID_ARGUMENT); of these two, the
+ *     lowest array is named;
+ *   - PCO_B200_ASYNC_FILES_DST_FULL: the metas need more than metas_cap bytes or the pages more than pages_cap (PCO_B200_IO), with the status
+ *     reporting the sizes needed.
+ * The first three are decided before anything is written and write only the status; a batch that does not fit writes refs, first_chunk
+ * and the status, and not a byte of metas or pages.  The return value covers the host side only: null pointers, an unaligned workspace or a
+ * plan that was not filled (PCO_B200_INVALID_ARGUMENT), a launch the runtime refuses (PCO_B200_CUDA).  With pco_b200_profile_enable(1), a
+ * call outside a stream capture records its kernel spans for pco_b200_profile_last; a call inside a capture records none. */
+PcoB200Error pco_b200_compress_wrapped_async(const PcoB200AsyncCompressWrappedPlan *plan, const void *nums, const uint64_t *array_ns,
+                                             const uint64_t *n_arrays, void *metas, void *pages, PcoB200PageRef *refs, uint64_t *first_chunk,
+                                             void *workspace, PcoB200AsyncCompressWrappedStatus *status, void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory at a point of the caller's choosing.  Returns the kind,
+ * sets the last-error message as pco_b200_compress_wrapped words it ("array 17: ...") and, when the kind is OK, sets *metas_len, *pages_len
+ * and *n_chunks (any may be NULL). */
+PcoB200Error pco_b200_compress_wrapped_async_result(const PcoB200AsyncCompressWrappedStatus *host_status, size_t *metas_len, size_t *pages_len,
+                                                    size_t *n_chunks);
+
 #if defined(__cplusplus)
 }
 #endif

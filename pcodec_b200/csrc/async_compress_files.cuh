@@ -118,6 +118,8 @@ struct AcfArgs {
   PcoB200FileRef* files;
   uint64_t max_files, max_file_n, nums_cap, max_page_n, index_cap;
   uint32_t uniform_type, bpc;
+  uint32_t framed;  // 1: standalone files (a header and a terminator around each file's chunks); 0: bare chunks (async_compress_wrapped.cuh)
+  uint32_t reserved;
 };
 __device__ __forceinline__ AcfState* acf_state(const AcfArgs& g) { return reinterpret_cast<AcfState*>(g.a.ws + g.l.state); }
 __device__ __forceinline__ AcfFile* acf_files(const AcfArgs& g) { return reinterpret_cast<AcfFile*>(g.a.ws + g.l.files); }
@@ -132,7 +134,7 @@ __device__ __forceinline__ void acf_file_sums(const AcfArgs& g, uint64_t f, uint
   s[ACF_NUMS] = ar_sum(n);
   s[ACF_CHUNKS] = ar_sum(fg.k);
   s[ACF_ROWS] = ar_sum(fg.rows);
-  s[ACF_FRAME] = ar_sum(f < nf ? standalone_header_len(nn) + 1 : 0);
+  s[ACF_FRAME] = ar_sum(f < nf && g.framed ? standalone_header_len(nn) + 1 : 0);
   s[ACF_IDX] = ar_sum(f < nf ? fg.idx : 0);
   *n_out = n;
 }
@@ -199,7 +201,7 @@ __global__ void __launch_bounds__(ACF_THREADS) acf_place_kernel(AcfArgs g) {
   AcfFile r;
   r.n = n;
   for (int k = 0; k < ACF_SUMS; k++) r.first[k] = ex[k].s;
-  r.hdr_len = standalone_header_len(n);
+  r.hdr_len = g.framed ? standalone_header_len(n) : 0;
   acf_files(g)[f] = r;
   const ArSum end = ar_add(ex[ACF_NUMS], s[ACF_NUMS]);
   uint32_t code = ST_OK;
@@ -449,9 +451,9 @@ inline PcoB200Error acf_check_plan(const PcoB200AsyncCompressFilesPlan* p, AcfPl
   return PCO_B200_OK;
 }
 
+// The launches up to and including pack_kernel, which every call of this layout shares: each chunk lands at its place in a.dst.
 template <typename L>
-void acf_launch(const PcoB200AsyncCompressFilesPlan& p, const AcompGeom& g, const AcfArgs& fa, const void* nums, PcoB200AsyncCompressFilesStatus* status,
-                const AsyncLaunch& ln) {
+void acf_launch_encode(const PcoB200AsyncCompressFilesPlan& p, const AcompGeom& g, const AcfArgs& fa, const void* nums, const AsyncLaunch& ln) {
   const cudaStream_t stream = ln.stream;
   const AcompArgs& a = fa.a;
   const uint32_t nc = uint32_t(g.n_chunks), bpc = g.bpc, tiles = g.tiles;
@@ -584,11 +586,19 @@ void acf_launch(const PcoB200AsyncCompressFilesPlan& p, const AcompGeom& g, cons
                                                                    (k & 1) ? nullptr : key16[0], (p.n_vars > 1 && !(k & 2)) ? key16[1] : nullptr);
   }
   ln.end();
+}
+
+template <typename L>
+void acf_launch(const PcoB200AsyncCompressFilesPlan& p, const AcompGeom& g, const AcfArgs& fa, const void* nums, PcoB200AsyncCompressFilesStatus* status,
+                const AsyncLaunch& ln) {
+  acf_launch_encode<L>(p, g, fa, nums, ln);
+  const cudaStream_t stream = ln.stream;
+  const uint32_t nc = uint32_t(g.n_chunks), file_ctas = uint32_t(acf_ctas(p.max_files));
   // ---- framing
   ln.begin("acf_frame_kernel");
   acf_frame_kernel<<<file_ctas, ACF_THREADS, 0, stream>>>(fa);
   ln.end();
-  if (a.index) {
+  if (fa.a.index) {
     ln.begin("acf_index_kernel");
     acf_index_kernel<<<nc, ACF_INDEX_THREADS, 0, stream>>>(fa);
     ln.end();

@@ -6,6 +6,7 @@
 
 #include "async_compress.cuh"
 #include "async_compress_files.cuh"
+#include "async_compress_wrapped.cuh"
 #include "async_files_kernels.cuh"
 #include "async_kernels.cuh"
 #include "async_pages_kernels.cuh"
@@ -3143,35 +3144,78 @@ PcoB200Error pco_b200_compress_async_result(const PcoB200AsyncCompressStatus* s,
 // pco_b200_compress_async (split_count and the planner kernels in their CHUNK_BINS instantiations), bytes, bytes scan, offsets, pack gate,
 // one pack per choice of keys, frame, [index], finish.
 
-PcoB200Error pco_b200_compress_files_async_plan(unsigned char dtype, const PcoB200ChunkConfig* config, int uniform_type_header, size_t max_files,
-                                                size_t nums_cap, size_t max_file_n, size_t dst_cap, size_t index_cap,
-                                                PcoB200AsyncCompressFilesPlan* plan) {
-  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
-  if (!plan) return fail(PCO_B200_INVALID_ARGUMENT, "null plan");
+// The refusals of the asynchronous batch compress plans, in their order, with `item` naming what the batch holds ("file" or "array"):
+// the capacities, PagingSpec::Exact, the config, Auto specs, more than 256 unoptimized bins at the largest chunk, the CTA limit.  Fills
+// the config, its check and the chunk slots.
+static PcoB200Error acf_plan_checks(unsigned char dtype, const PcoB200ChunkConfig* config, size_t max_items, size_t nums_cap, size_t max_item_n,
+                                    const std::string& item, PcoB200ChunkConfig* cfg_out, ConfigCheck* ck_out, uint64_t* max_chunks_out) {
   PcoB200ChunkConfig cfg;
   if (config) cfg = *config;
   else {
     std::memset(&cfg, 0, sizeof(cfg));  // pco::ChunkConfig::default(): level 8, Auto, Auto, EqualPagesUpTo(2^18)
     cfg.compression_level = 8;
   }
-  if (max_files == 0 || max_files > 0x7fffffffu) return fail(PCO_B200_INVALID_ARGUMENT, "max_files must be in 1 .. 2^31 - 1");
-  if (max_file_n == 0) return fail(PCO_B200_INVALID_ARGUMENT, "max_file_n must be at least 1");
+  if (max_items == 0 || max_items > 0x7fffffffu) return fail(PCO_B200_INVALID_ARGUMENT, "max_" + item + "s must be in 1 .. 2^31 - 1");
+  if (max_item_n == 0) return fail(PCO_B200_INVALID_ARGUMENT, "max_" + item + "_n must be at least 1");
   if (uint64_t(nums_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "nums_cap must be at most 2^56");
   // the config as compress_async_plan checks it, at the largest chunk (a file of min(max_page_n, max_file_n, nums_cap) numbers is one chunk)
   // (Exact paging first: its page sizes are checked against a count, and a batch has none)
   if (cfg.paging_spec == PCO_B200_PAGING_EXACT) return fail(PCO_B200_UNSUPPORTED, "PagingSpec::Exact: the asynchronous compress takes EqualPagesUpTo only");
-  const uint64_t chunk_n = acf_chunk_n(cfg.max_page_n, max_file_n, nums_cap);
+  const uint64_t chunk_n = acf_chunk_n(cfg.max_page_n, max_item_n, nums_cap);
   ConfigCheck ck;
   if (PcoB200Error e = check_config(cfg, dtype, size_t(chunk_n), &ck)) return e;
   if (ck.auto_mode || ck.auto_delta)
     return fail(PCO_B200_UNSUPPORTED, "ModeSpec::Auto and DeltaSpec::Auto search on host threads: the asynchronous compress takes explicit specs only");
   if (choose_unoptimized_bins_log(cfg.compression_level, size_t(chunk_n)) > ENC_NARROW_BINS_LOG)
     return fail(PCO_B200_UNSUPPORTED, "more than 256 unoptimized bins (levels 9-12): the asynchronous compress runs the narrow kernels only");
-  const uint64_t max_chunks = uint64_t(nums_cap) / chunk_n + max_files;
+  const uint64_t max_chunks = uint64_t(nums_cap) / chunk_n + max_items;
   const uint64_t tiles = (chunk_n + SPLIT_TILE - 1) / SPLIT_TILE, bpc = n_batches_of(uint32_t(chunk_n));
   const uint64_t per_chunk = std::max<uint64_t>({tiles, (bpc + BINL_BATCHES - 1) / BINL_BATCHES, (bpc + 7) / 8, uint64_t(MAX_VARS)});
   if (max_chunks > 0x7fffffffu / per_chunk)
     return fail(PCO_B200_INVALID_ARGUMENT, "the capacities give " + std::to_string(max_chunks) + " chunk slots, more than one launch can cover");
+  *cfg_out = cfg;
+  *ck_out = ck;
+  *max_chunks_out = max_chunks;
+  return PCO_B200_OK;
+}
+
+// The one-time device set-up of the asynchronous batch compress calls (compress_async_plan's, for their kernels), plus `extra`.
+static PcoB200Error acf_plan_setup(unsigned char dtype, std::initializer_list<const void*> extra) {
+  Context& c = ctx();
+  if (PcoB200Error e = ensure_device(c)) return e;
+  if (PcoB200Error e = load_kernels(extra)) return e;
+  if (PcoB200Error e = load_kernels({(const void*)acf_files_kernel, (const void*)acf_scan_kernel, (const void*)acf_place_kernel, (const void*)acf_init_kernel,
+                                     (const void*)acf_bytes_kernel, (const void*)acf_bytes_scan_kernel, (const void*)acf_offsets_kernel,
+                                     (const void*)acomp_two_gate_kernel, (const void*)acomp_var_gate_kernel,
+                                     (const void*)acomp_pack_gate_kernel, (const void*)segment_offsets_kernel, (const void*)fallback_kernel<false>,
+                                     (const void*)ans_encode_kernel<false>, (const void*)layout_kernel<false>})) return e;
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
+    using L = decltype(tag);
+    constexpr size_t RS_SMEM = size_t(RS_WARPS) * RS_BINS * sizeof(uint32_t);
+    const int count_smem = int(((size_t(1) << PLAN_MAX_COUNT_BITS) + 1) * 4 + 16);
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, count_smem));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(split_count_kernel<L, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(size_t(SC_N) * 4)));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PackSmem)));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(radix_sort_segments_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RS_SMEM));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true, false, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(bin_lut_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    return load_kernels({(const void*)split_count_kernel<L, true>, (const void*)split_delta_kernel<L, MODE_CLASSIC>, (const void*)split_delta_kernel<L, MODE_INT_MULT>,
+                         (const void*)split_delta_kernel<L, MODE_FLOAT_QUANT>, (const void*)split_delta_kernel<L, MODE_FLOAT_MULT>,
+                         (const void*)plan_probe_kernel<L, false, false, true>, (const void*)sort_keys_kernel<L>, (const void*)plan_solve_kernel<L, true>,
+                         (const void*)bin_kernel<L, false>});
+  });
+}
+
+PcoB200Error pco_b200_compress_files_async_plan(unsigned char dtype, const PcoB200ChunkConfig* config, int uniform_type_header, size_t max_files,
+                                                size_t nums_cap, size_t max_file_n, size_t dst_cap, size_t index_cap,
+                                                PcoB200AsyncCompressFilesPlan* plan) {
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (!plan) return fail(PCO_B200_INVALID_ARGUMENT, "null plan");
+  PcoB200ChunkConfig cfg;
+  ConfigCheck ck;
+  uint64_t max_chunks = 0;
+  if (PcoB200Error e = acf_plan_checks(dtype, config, max_files, nums_cap, max_file_n, "file", &cfg, &ck, &max_chunks)) return e;
   std::memset(plan, 0, sizeof(*plan));
   plan->dtype = dtype;
   plan->uniform_type_header = uniform_type_header ? 1 : 0;
@@ -3197,29 +3241,34 @@ PcoB200Error pco_b200_compress_files_async_plan(unsigned char dtype, const PcoB2
                       plan->n_vars * sizeof(BatchEntry) * ((uint64_t(nums_cap) + BATCH_N - 1) / BATCH_N);
   plan->workspace_bytes = acf_plan_geom(*plan).l.total;
   // the one-time device set-up (compress_async_plan's, for this call's kernels)
-  Context& c = ctx();
-  if (PcoB200Error e = ensure_device(c)) return e;
-  if (PcoB200Error e = load_kernels({(const void*)acf_files_kernel, (const void*)acf_scan_kernel, (const void*)acf_place_kernel, (const void*)acf_init_kernel,
-                                     (const void*)acf_bytes_kernel, (const void*)acf_bytes_scan_kernel, (const void*)acf_offsets_kernel, (const void*)acf_frame_kernel,
-                                     (const void*)acf_index_kernel, (const void*)acf_finish_kernel, (const void*)acomp_two_gate_kernel, (const void*)acomp_var_gate_kernel,
-                                     (const void*)acomp_pack_gate_kernel, (const void*)segment_offsets_kernel, (const void*)fallback_kernel<false>,
-                                     (const void*)ans_encode_kernel<false>, (const void*)layout_kernel<false>})) return e;
-  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
-    using L = decltype(tag);
-    constexpr size_t RS_SMEM = size_t(RS_WARPS) * RS_BINS * sizeof(uint32_t);
-    const int count_smem = int(((size_t(1) << PLAN_MAX_COUNT_BITS) + 1) * 4 + 16);
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, count_smem));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(split_count_kernel<L, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(size_t(SC_N) * 4)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PackSmem)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(radix_sort_segments_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RS_SMEM));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true, false, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(bin_lut_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    return load_kernels({(const void*)split_count_kernel<L, true>, (const void*)split_delta_kernel<L, MODE_CLASSIC>, (const void*)split_delta_kernel<L, MODE_INT_MULT>,
-                         (const void*)split_delta_kernel<L, MODE_FLOAT_QUANT>, (const void*)split_delta_kernel<L, MODE_FLOAT_MULT>,
-                         (const void*)plan_probe_kernel<L, false, false, true>, (const void*)sort_keys_kernel<L>, (const void*)plan_solve_kernel<L, true>,
-                         (const void*)bin_kernel<L, false>});
-  });
+  return acf_plan_setup(dtype, {(const void*)acf_frame_kernel, (const void*)acf_index_kernel, (const void*)acf_finish_kernel});
+}
+
+// What the launches of a batch compress take by value (framed: 1 for standalone files, 0 for bare chunks)
+static AcfArgs acf_args(const PcoB200AsyncCompressFilesPlan& p, const AcfPlanGeom& pg, void* workspace, void* dst, void* index, const uint64_t* ns,
+                        const uint64_t* n_items, PcoB200FileRef* files, uint32_t framed) {
+  AcfArgs fa;
+  std::memset(&fa, 0, sizeof(fa));
+  fa.a.n_chunks = pg.g.n_chunks;
+  fa.a.dst_cap = p.dst_cap;
+  fa.a.n_vars = p.n_vars;
+  fa.a.ws = static_cast<uint8_t*>(workspace);
+  fa.a.dst = static_cast<uint8_t*>(dst);
+  fa.a.index = static_cast<uint8_t*>(index);
+  fa.a.lay = pg.l.enc;
+  fa.l = pg.l;
+  fa.file_ns = ns;
+  fa.n_files = n_items;
+  fa.files = files;
+  fa.max_files = p.max_files;
+  fa.max_file_n = p.max_file_n;
+  fa.nums_cap = p.nums_cap;
+  fa.max_page_n = p.max_page_n == 0 ? (uint64_t(1) << 18) : p.max_page_n;
+  fa.index_cap = index ? p.index_cap : 0;
+  fa.uniform_type = p.uniform_type_header ? p.dtype : 0;
+  fa.bpc = pg.g.bpc;
+  fa.framed = framed;
+  return fa;
 }
 
 PcoB200Error pco_b200_compress_files_async(const PcoB200AsyncCompressFilesPlan* plan, const void* nums, const uint64_t* file_ns, const uint64_t* n_files,
@@ -3234,26 +3283,7 @@ PcoB200Error pco_b200_compress_files_async(const PcoB200AsyncCompressFilesPlan* 
   if (reinterpret_cast<uintptr_t>(index) & 15) return fail(PCO_B200_INVALID_ARGUMENT, "the index is not 16-byte aligned");
   AsyncLaunch ln;
   if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
-  AcfArgs fa;
-  std::memset(&fa, 0, sizeof(fa));
-  fa.a.n_chunks = pg.g.n_chunks;
-  fa.a.dst_cap = plan->dst_cap;
-  fa.a.n_vars = plan->n_vars;
-  fa.a.ws = static_cast<uint8_t*>(workspace);
-  fa.a.dst = static_cast<uint8_t*>(dst);
-  fa.a.index = static_cast<uint8_t*>(index);
-  fa.a.lay = pg.l.enc;
-  fa.l = pg.l;
-  fa.file_ns = file_ns;
-  fa.n_files = n_files;
-  fa.files = files;
-  fa.max_files = plan->max_files;
-  fa.max_file_n = plan->max_file_n;
-  fa.nums_cap = plan->nums_cap;
-  fa.max_page_n = plan->max_page_n == 0 ? (uint64_t(1) << 18) : plan->max_page_n;
-  fa.index_cap = index ? plan->index_cap : 0;
-  fa.uniform_type = plan->uniform_type_header ? plan->dtype : 0;
-  fa.bpc = pg.g.bpc;
+  const AcfArgs fa = acf_args(*plan, pg, workspace, dst, index, file_ns, n_files, files, 1);
   dispatch_latent(plan->dtype, [&](auto tag) {
     acf_launch<decltype(tag)>(*plan, pg.g, fa, nums, status, ln);
     return 0;
@@ -3285,6 +3315,101 @@ PcoB200Error pco_b200_compress_files_async_result(const PcoB200AsyncCompressFile
       return fail(kind, "failed to write whole buffer (need " + std::to_string(s->dst_bytes) + " file bytes and " + std::to_string(s->index_bytes) +
                             " index bytes)");
     default: return fail(kind, "asynchronous batch compress failed (device status " + std::to_string(s->device_status) + ")");
+  }
+}
+
+// ---- asynchronous batch compress into wrapped chunks (pco_b200_compress_wrapped_async; kernels in async_compress_wrapped.cuh).  The
+// launches of pco_b200_compress_files_async up to pack_kernel with bare chunks staged in the workspace, then lens, scan, refs, split,
+// finish.
+
+PcoB200Error pco_b200_compress_wrapped_async_plan(unsigned char dtype, const PcoB200ChunkConfig* config, size_t max_arrays, size_t nums_cap,
+                                                  size_t max_array_n, size_t metas_cap, size_t pages_cap, PcoB200AsyncCompressWrappedPlan* plan) {
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (!plan) return fail(PCO_B200_INVALID_ARGUMENT, "null plan");
+  PcoB200ChunkConfig cfg;
+  ConfigCheck ck;
+  uint64_t max_chunks = 0;
+  if (PcoB200Error e = acf_plan_checks(dtype, config, max_arrays, nums_cap, max_array_n, "array", &cfg, &ck, &max_chunks)) return e;
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->mode = ck.explicit_mode.mode;
+  plan->order = ck.explicit_order;
+  plan->n_vars = ck.explicit_mode.mode == MODE_CLASSIC ? 1 : 2;
+  plan->level = cfg.compression_level;
+  plan->mode_k = ck.explicit_mode.mode_k;
+  plan->max_arrays = max_arrays;
+  plan->nums_cap = nums_cap;
+  plan->max_array_n = max_array_n;
+  plan->max_page_n = cfg.max_page_n;
+  plan->max_chunks = max_chunks;
+  plan->metas_cap = metas_cap;
+  plan->pages_cap = pages_cap;
+  plan->mode_base = ck.explicit_mode.mode_base;
+  plan->base_bits = ck.explicit_mode.base_bits;
+  plan->inv_base_bits = ck.explicit_mode.inv_base_bits;
+  // the bounds the header comment derives
+  const uint64_t lbits = nt_bits(dtype), obb = offset_bits_bits(uint32_t(lbits));
+  const uint64_t mode_bits = plan->mode == MODE_CLASSIC ? 0 : plan->mode == MODE_FLOAT_QUANT ? 8 : lbits;
+  const uint64_t meta_max = (4 + mode_bits + (4 + 5 + 5 + 64 + 32 * 32) + plan->n_vars * (4 + 15 + 256 * (15 + lbits + obb)) + 7) / 8;
+  plan->pages_bound = max_chunks * (1 + baseline_chunk_meta_size(uint32_t(lbits))) + (uint64_t(nums_cap) * lbits + 7) / 8;
+  plan->metas_bound = std::min<uint64_t>(max_chunks * meta_max, plan->pages_bound);
+  plan->workspace_bytes = acw_plan_geom(*plan).l.total;
+  return acf_plan_setup(dtype, {(const void*)acw_lens_kernel, (const void*)acw_scan_kernel, (const void*)acw_refs_kernel, (const void*)acw_split_kernel,
+                                (const void*)acw_finish_kernel});
+}
+
+PcoB200Error pco_b200_compress_wrapped_async(const PcoB200AsyncCompressWrappedPlan* plan, const void* nums, const uint64_t* array_ns,
+                                             const uint64_t* n_arrays, void* metas, void* pages, PcoB200PageRef* refs, uint64_t* first_chunk,
+                                             void* workspace, PcoB200AsyncCompressWrappedStatus* status, void* cuda_stream) {
+  if (!plan || !array_ns || !n_arrays || !refs || !first_chunk || !workspace || !status || (!nums && plan->nums_cap) || (!metas && plan->metas_cap) ||
+      (!pages && plan->pages_cap))
+    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  AcwPlanGeom pg;
+  if (PcoB200Error e = acw_check_plan(plan, &pg)) return e;
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  if (reinterpret_cast<uintptr_t>(refs) & 7 || reinterpret_cast<uintptr_t>(first_chunk) & 7)
+    return fail(PCO_B200_INVALID_ARGUMENT, "refs and first_chunk must be 8-byte aligned");
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+  const PcoB200AsyncCompressFilesPlan fp = acw_files_plan(*plan);
+  AcwArgs w;
+  std::memset(&w, 0, sizeof(w));
+  w.f = acf_args(fp, pg.f, workspace, static_cast<uint8_t*>(workspace) + pg.l.stage, nullptr, array_ns, n_arrays, nullptr, 0);
+  w.l = pg.l;
+  w.metas = static_cast<uint8_t*>(metas);
+  w.pages = static_cast<uint8_t*>(pages);
+  w.refs = refs;
+  w.first_chunk = first_chunk;
+  w.metas_cap = plan->metas_cap;
+  w.pages_cap = plan->pages_cap;
+  w.dtype = plan->dtype;
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    acw_launch<decltype(tag)>(*plan, pg, w, nums, status, ln);
+    return 0;
+  });
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
+}
+
+PcoB200Error pco_b200_compress_wrapped_async_result(const PcoB200AsyncCompressWrappedStatus* s, size_t* metas_len, size_t* pages_len, size_t* n_chunks) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200Error kind = s->kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(s->kind) : PCO_B200_CORRUPTION;
+  if (kind == PCO_B200_OK) {
+    if (metas_len) *metas_len = size_t(s->metas_written);
+    if (pages_len) *pages_len = size_t(s->pages_written);
+    if (n_chunks) *n_chunks = size_t(s->n_chunks);
+    return PCO_B200_OK;
+  }
+  const std::string array = "array " + std::to_string(s->array) + ": ";
+  switch (s->device_status) {
+    case PCO_B200_ASYNC_TOO_MANY_FILES: return fail(kind, std::to_string(s->n_arrays) + " arrays, more than the plan's max_arrays");
+    case PCO_B200_ASYNC_FILE_TOO_LARGE: return fail(kind, array + "more numbers than the plan's max_array_n");
+    case PCO_B200_ASYNC_NUMS_CAP: return fail(kind, array + "the arrays up to this one hold more numbers than the plan's nums_cap");
+    case PCO_B200_ASYNC_FILES_DST_FULL:
+      return fail(kind, "failed to write whole buffer (need " + std::to_string(s->metas_bytes) + " meta bytes and " + std::to_string(s->pages_bytes) +
+                            " page bytes)");
+    case ST_CORRUPTION: return fail(kind, "compressor returned chunks that do not split into meta and page");
+    default: return fail(kind, "asynchronous wrapped compress failed (device status " + std::to_string(s->device_status) + ")");
   }
 }
 

@@ -6,7 +6,9 @@ PcoError("Unsupported") when their PagingSpec would give several (DESIGN.md sect
 
 Batched forms for containers that keep chunk metas and pages themselves: `compress_chunks` writes a whole array as wrapped
 chunks of one page each, `decompress_pages` decodes any number of pages in one call.  Both take host buffers (bytes / numpy)
-or torch CUDA tensors; with CUDA tensors the work runs on torch.cuda.current_stream() and the outputs are CUDA tensors."""
+or torch CUDA tensors; with CUDA tensors the work runs on torch.cuda.current_stream() and the outputs are CUDA tensors.
+`AsyncChunksCompressor` and `AsyncPagesDecompressor` are their forms with the sizes or refs in device memory, which do not wait for the
+device and can be captured in a CUDA graph."""
 import ctypes as C
 
 import numpy as np
@@ -304,3 +306,110 @@ class AsyncPagesDecompressor(_lib._AsyncCall):
         nw = C.c_size_t()
         _lib.check(_lib_async_pages().pco_b200_decompress_pages_async_result(C.byref(s), C.byref(nw)))
         return int(nw.value)
+
+
+class _CAsyncCompressWrappedPlan(C.Structure):  # PcoB200AsyncCompressWrappedPlan (include/pco_b200.h)
+    _fields_ = [("dtype", C.c_uint32), ("mode", C.c_uint32), ("order", C.c_uint32), ("n_vars", C.c_uint32),
+                ("level", C.c_uint32), ("mode_k", C.c_uint32), ("reserved0", C.c_uint32), ("reserved1", C.c_uint32),
+                ("max_arrays", C.c_uint64), ("nums_cap", C.c_uint64), ("max_array_n", C.c_uint64), ("max_page_n", C.c_uint64),
+                ("max_chunks", C.c_uint64), ("metas_cap", C.c_uint64), ("pages_cap", C.c_uint64),
+                ("mode_base", C.c_uint64), ("base_bits", C.c_uint64), ("inv_base_bits", C.c_uint64),
+                ("metas_bound", C.c_uint64), ("pages_bound", C.c_uint64), ("workspace_bytes", C.c_uint64)]
+
+
+class _CAsyncCompressWrappedStatus(C.Structure):  # PcoB200AsyncCompressWrappedStatus (include/pco_b200.h)
+    _fields_ = [("kind", C.c_uint32), ("device_status", C.c_uint32), ("array", C.c_uint64), ("n_arrays", C.c_uint64), ("n_chunks", C.c_uint64),
+                ("metas_bytes", C.c_uint64), ("pages_bytes", C.c_uint64), ("metas_written", C.c_uint64), ("pages_written", C.c_uint64)]
+
+
+def _lib_async_compress_wrapped():
+    return _lib.bind("_async_compress_wrapped_ready",
+                     pco_b200_compress_wrapped_async_plan=[C.c_ubyte, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                                           C.c_void_p],
+                     pco_b200_compress_wrapped_async=[C.c_void_p] * 11,
+                     pco_b200_compress_wrapped_async_result=[C.c_void_p, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)])
+
+
+class AsyncChunksCompressor(_lib._AsyncCall):
+    """Compresses a batch of arrays into wrapped chunks of one page each on the current CUDA stream, with the array sizes in device memory
+    and without waiting for the device (pco_b200_compress_wrapped_async): column chunks a kernel sized need no trip to the host, and a call
+    can be captured in a torch.cuda.CUDAGraph.  Each array is cut into the chunks compress_chunks writes for it alone, and its metas, pages
+    and refs equal compress_chunks's, placed behind the arrays before it.
+
+    The plan fixes the number type `dtype`, the config (explicit mode and delta specs, EqualPagesUpTo paging) and the capacities: at most
+    max_arrays arrays, nums_cap numbers in all and max_array_n per array, metas_cap bytes of metas and pages_cap bytes of pages (default:
+    the plan's metas_bound and pages_bound, which every batch within the capacities fits in).  The refs come out as the int64
+    (max_chunks, 5) tensor AsyncPagesDecompressor takes, so one graph can compress pages and decode them.  The compressor owns a device
+    workspace and a status; it serves one call in flight."""
+
+    _Plan, _Status = _CAsyncCompressWrappedPlan, _CAsyncCompressWrappedStatus
+
+    def __init__(self, dtype, config, max_arrays, nums_cap, max_array_n, metas_cap=None, pages_cap=None, device=None):
+        self.dtype = np.dtype(dtype)
+        dtb = _lib.dtype_byte(self.dtype)
+        L = _lib_async_compress_wrapped()
+        cfg = (config or ChunkConfig())._to_c()
+
+        def plan_fn(mcap, pcap):
+            return lambda plan: L.pco_b200_compress_wrapped_async_plan(C.c_ubyte(dtb), C.byref(cfg), C.c_size_t(max_arrays), C.c_size_t(nums_cap),
+                                                                       C.c_size_t(max_array_n), C.c_size_t(mcap), C.c_size_t(pcap), plan)
+
+        # the bounds are known once a plan exists: a first plan reports them
+        self._make_plan(device, plan_fn(metas_cap or 0, pages_cap or 0))
+        if metas_cap is None or pages_cap is None:
+            self._replan(plan_fn(self._plan.metas_bound if metas_cap is None else metas_cap, self._plan.pages_bound if pages_cap is None else pages_cap))
+        self._alloc()
+
+    @property
+    def metas_cap(self):
+        return int(self._plan.metas_cap)
+
+    @property
+    def pages_cap(self):
+        return int(self._plan.pages_cap)
+
+    @property
+    def max_arrays(self):
+        return int(self._plan.max_arrays)
+
+    @property
+    def max_chunks(self):
+        """Rows of `refs` a call takes: the most chunks of any batch within the capacities."""
+        return int(self._plan.max_chunks)
+
+    def __call__(self, nums, array_ns, n_arrays, metas, pages, refs, first_chunk):
+        """Enqueues the compress of the first n_arrays[0] arrays on torch.cuda.current_stream(): array i is the next array_ns[i] numbers of
+        `nums` (a CUDA tensor of the plan's dtype, at least nums_cap numbers).  `array_ns` is an int64 CUDA tensor of at least max_arrays
+        elements, `n_arrays` a 1-element int64 CUDA tensor, `metas` and `pages` uint8 CUDA tensors of at least metas_cap and pages_cap
+        bytes, `refs` the int64 (max_chunks, 5) CUDA tensor of PAGE_REF fields that AsyncPagesDecompressor takes, and `first_chunk` an int64
+        CUDA tensor of max_arrays + 1 elements: array i's chunks are refs[first_chunk[i] : first_chunk[i + 1]].  Returns nothing and does
+        not wait; result() reports the outcome."""
+        import torch
+
+        p = self._plan
+        self._check_tensors(nums=nums, array_ns=array_ns, n_arrays=n_arrays, metas=metas, pages=pages, refs=refs, first_chunk=first_chunk)
+        if nums.dtype != _torch_dtypes()[self.dtype] or nums.numel() < p.nums_cap:
+            raise ValueError(f"nums must hold at least nums_cap = {p.nums_cap} numbers of {self.dtype}")
+        if array_ns.dtype != torch.int64 or array_ns.numel() < p.max_arrays:
+            raise ValueError(f"array_ns must be an int64 tensor of at least max_arrays = {p.max_arrays} elements")
+        if n_arrays.dtype != torch.int64 or n_arrays.numel() != 1:
+            raise ValueError("n_arrays must be a 1-element int64 tensor")
+        if metas.numel() * metas.element_size() < p.metas_cap or pages.numel() * pages.element_size() < p.pages_cap:
+            raise ValueError(f"metas holds fewer than metas_cap = {p.metas_cap} bytes, or pages fewer than pages_cap = {p.pages_cap}")
+        if refs.dtype != torch.int64 or refs.dim() != 2 or refs.shape[1] != 5 or refs.shape[0] < p.max_chunks:
+            raise ValueError(f"refs must be an int64 tensor of shape ({p.max_chunks}, 5)")
+        if first_chunk.dtype != torch.int64 or first_chunk.numel() < p.max_arrays + 1:
+            raise ValueError(f"first_chunk must be an int64 tensor of at least max_arrays + 1 = {p.max_arrays + 1} elements")
+        rc = _lib_async_compress_wrapped().pco_b200_compress_wrapped_async(
+            C.byref(p), C.c_void_p(nums.data_ptr()), C.c_void_p(array_ns.data_ptr()), C.c_void_p(n_arrays.data_ptr()), C.c_void_p(metas.data_ptr()),
+            C.c_void_p(pages.data_ptr()), C.c_void_p(refs.data_ptr()), C.c_void_p(first_chunk.data_ptr()), C.c_void_p(self.workspace.data_ptr()),
+            C.c_void_p(self.status.data_ptr()), self._stream())
+        _lib.check(rc)
+
+    def result(self):
+        """Copies the status of the last call back (waiting for it on the current stream) and returns (metas_len, pages_len, n_chunks), or
+        raises PcoError with the kind compress_chunks gives ("array 17: ...")."""
+        s = self.status_record()
+        ml, pl, nc = C.c_size_t(), C.c_size_t(), C.c_size_t()
+        _lib.check(_lib_async_compress_wrapped().pco_b200_compress_wrapped_async_result(C.byref(s), C.byref(ml), C.byref(pl), C.byref(nc)))
+        return int(ml.value), int(pl.value), int(nc.value)
