@@ -10,6 +10,7 @@
 //   16-bit keys or 64-bit latents in pack_kernel, per var           acomp_pack_gate_kernel: one copy of the ChunkEnc table per choice, whose
 //                                                                   chunks the launches of the other choices find out of dst_cap
 // acomp_init_kernel lays out the chunks, the header and the index header; acomp_finish_kernel writes the PcoB200AsyncCompressStatus.
+// enqueue_encode_kernels and enqueue_pack make the gated launches, which the batch calls (async_compress_files.cuh) share.
 #pragma once
 #include "../../include/pco_b200.h"
 #include "compress_host.cuh"
@@ -245,9 +246,14 @@ __global__ void acomp_finish_kernel(AcompArgs a, PcoB200AsyncCompressStatus* __r
 
 // ---- host steps
 
+// The clause every asynchronous compress plan check shares: the spec fields as the plan functions fill them (P: any of the three plans)
+template <typename P>
+inline bool acomp_spec_ok(const P* p) {
+  return p && nt_valid(p->dtype) && p->mode <= MODE_FLOAT_QUANT && p->n_vars == (p->mode == MODE_CLASSIC ? 1u : 2u) && p->order <= MAX_ORDER;
+}
+
 inline PcoB200Error acomp_check_plan(const PcoB200AsyncCompressPlan* p, AcompGeom* g, AcompLayout* lay) {
-  if (!p || !nt_valid(p->dtype) || p->mode > MODE_FLOAT_QUANT || p->n_vars != (p->mode == MODE_CLASSIC ? 1u : 2u) || p->order > MAX_ORDER ||
-      p->bins_log > ENC_NARROW_BINS_LOG || (p->index_cap != 0 && p->index_bytes > p->index_cap))
+  if (!acomp_spec_ok(p) || p->bins_log > ENC_NARROW_BINS_LOG || (p->index_cap != 0 && p->index_bytes > p->index_cap))
     return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_compress_async_plan");
   *g = acomp_geom(p->n, p->max_page_n);
   *lay = acomp_layout(*g, nt_bits(p->dtype) / 8, p->n_vars);
@@ -256,133 +262,187 @@ inline PcoB200Error acomp_check_plan(const PcoB200AsyncCompressPlan* p, AcompGeo
   return PCO_B200_OK;
 }
 
+// The workspace regions of an AcompLayout as the encode kernels take them; the secondary var's are null for one var.
 template <typename L>
-void acomp_launch(const PcoB200AsyncCompressPlan& p, const AcompGeom& g, const AcompArgs& a, const void* nums, PcoB200AsyncCompressStatus* status,
-                         const AsyncLaunch& ln) {
-  const cudaStream_t stream = ln.stream;
-  const uint32_t nc = uint32_t(g.n_chunks), bpc = g.bpc, tiles = g.tiles;
-  constexpr uint32_t LBITS = sizeof(L) * 8;
-  constexpr size_t RS_SMEM = size_t(RS_WARPS) * RS_BINS * sizeof(uint32_t);
+struct AcompRegions {
+  AcompHead* head;
+  ChunkEnc *chunks, *copies;
+  VarPlan* plans;
+  PlanProbes* probes;
+  uint64_t *gates, *seg_begin, *seg_end;
+  L *lat[MAX_VARS], *keys_a, *keys_b;
+  uint16_t *key16[MAX_VARS], *ans[MAX_VARS];
+  uint8_t* sym[MAX_VARS];
+  uint32_t *ob_sum, *ans_sum;
+  BatchEntry* entries;
+};
+template <typename L>
+AcompRegions<L> acomp_regions(const AcompArgs& a) {
   uint8_t* ws = a.ws;
   const AcompLayout& l = a.lay;
-  const uint32_t init_ctas = uint32_t(std::min<uint64_t>(1024, std::max<uint64_t>({g.n_chunks + 1, g.n_chunks * MAX_VARS * bpc, a.index_bytes / 16}) / ACOMP_THREADS + 1));
+  const bool two = a.n_vars > 1;
+  AcompRegions<L> r;
+  r.head = reinterpret_cast<AcompHead*>(ws);
+  r.chunks = reinterpret_cast<ChunkEnc*>(ws + l.chunks);
+  r.copies = reinterpret_cast<ChunkEnc*>(ws + l.copies);
+  r.plans = reinterpret_cast<VarPlan*>(ws + l.plans);
+  r.probes = reinterpret_cast<PlanProbes*>(ws + l.probes);
+  r.gates = reinterpret_cast<uint64_t*>(ws + l.gates);
+  for (uint32_t v = 0; v < MAX_VARS; v++) {
+    const bool on = v == 0 || two;
+    r.lat[v] = on ? reinterpret_cast<L*>(ws + l.lat[v]) : nullptr;
+    r.key16[v] = on ? reinterpret_cast<uint16_t*>(ws + l.key16[v]) : nullptr;
+    r.sym[v] = on ? ws + l.sym[v] : nullptr;
+    r.ans[v] = on ? reinterpret_cast<uint16_t*>(ws + l.ans[v]) : nullptr;
+  }
+  r.keys_a = reinterpret_cast<L*>(ws + l.keys_a);
+  r.keys_b = reinterpret_cast<L*>(ws + l.keys_b);
+  r.seg_begin = reinterpret_cast<uint64_t*>(ws + l.seg);
+  r.seg_end = r.seg_begin + a.n_chunks;
+  r.ob_sum = reinterpret_cast<uint32_t*>(ws + l.ob_sum);
+  r.ans_sum = reinterpret_cast<uint32_t*>(ws + l.ans_sum);
+  r.entries = reinterpret_cast<BatchEntry*>(ws + l.entries);
+  return r;
+}
+
+// The EncParams of the encode stage: the spec fields of the plan (P: a compress_async or compress_files_async plan), the chunks of g,
+// the starts and row bases the init kernel wrote, and the caller's n_total and unoptimized_bins_log per var.
+template <typename P>
+EncParams acomp_enc_params(const P& p, const AcompGeom& g, const AcompArgs& a, const void* nums, uint64_t n_total, uint32_t bins_log0,
+                           uint32_t bins_log1) {
+  EncParams ep;
+  std::memset(&ep, 0, sizeof(ep));
+  ep.dtype = p.dtype;
+  ep.uniform_type = p.uniform_type_header ? p.dtype : 0;
+  ep.mode = p.mode;
+  ep.mode_base = p.mode_base;
+  ep.base_bits = p.base_bits;
+  ep.inv_base_bits = p.inv_base_bits;
+  ep.mode_k = p.mode_k;
+  ep.order = p.order;
+  ep.n_vars = p.n_vars;
+  ep.n_total = n_total;
+  ep.n_chunks = uint32_t(g.n_chunks);
+  ep.max_chunk_n = uint32_t(g.max_n);
+  ep.bins_log[0] = bins_log0;
+  ep.bins_log[1] = bins_log1;
+  ep.nums = nums;
+  ep.chunk_starts = reinterpret_cast<const uint64_t*>(a.ws + a.lay.starts);
+  ep.row_base = reinterpret_cast<const uint64_t*>(a.ws + a.lay.rows);
+  return ep;
+}
+
+// The gated encode kernels of every asynchronous compress, from the front end to layout_kernel, behind the init kernel that wrote the
+// starts, row bases and head.  CHUNK_BINS: split_count_kernel and the planner kernels compute each chunk's unoptimized_bins_log from
+// the level in ep.bins_log[0] and its n (a batch); otherwise they take ep.bins_log as it is.
+template <typename L, bool CHUNK_BINS>
+void enqueue_encode_kernels(const AcompGeom& g, const AcompArgs& a, const EncParams& ep, const AsyncLaunch& ln) {
+  const cudaStream_t stream = ln.stream;
+  const uint32_t nc = uint32_t(g.n_chunks), bpc = g.bpc, tiles = g.tiles, n_vars = ep.n_vars;
+  constexpr uint32_t LBITS = sizeof(L) * 8;
+  constexpr size_t RS_SMEM = size_t(RS_WARPS) * RS_BINS * sizeof(uint32_t);
+  const AcompRegions<L> r = acomp_regions<L>(a);
+  auto gated = [&](uint32_t gate) { EncParams e = ep; e.chunk_starts = r.gates + uint64_t(gate) * (g.n_chunks + 1); return e; };
+  const uint32_t always_two = n_vars > 1 ? 1u : 0u;
+  // ---- front end: the one-pass kernel for Classic, then the two-kernel path behind its flag (always, for the two-var modes)
+  if (!always_two) {
+    ln.begin("split_count_kernel");
+    split_count_kernel<L, CHUNK_BINS><<<nc, SC_THREADS, size_t(SC_N) * 4, stream>>>(ep, r.chunks, r.probes, r.key16[0], r.head->flags);
+    ln.end();
+  }
+  acomp_two_gate_kernel<<<(nc + ACOMP_THREADS) / ACOMP_THREADS, ACOMP_THREADS, 0, stream>>>(a, always_two);
+  const EncParams e_two = gated(0);
+  ln.begin("split_delta_kernel");
+  switch (ep.mode) {
+    case MODE_CLASSIC: split_delta_kernel<L, MODE_CLASSIC><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, r.lat[0], r.lat[1], r.chunks); break;
+    case MODE_INT_MULT: split_delta_kernel<L, MODE_INT_MULT><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, r.lat[0], r.lat[1], r.chunks); break;
+    case MODE_FLOAT_QUANT: split_delta_kernel<L, MODE_FLOAT_QUANT><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, r.lat[0], r.lat[1], r.chunks); break;
+    default: split_delta_kernel<L, MODE_FLOAT_MULT><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, r.lat[0], r.lat[1], r.chunks); break;
+  }
+  ln.end();
+  acomp_var_gate_kernel<<<1, 1024, 0, stream>>>(a, always_two);
+  // ---- planner per var: counting probe or sort path (whichever the range bits gate on), then the solver on the probes either left
+  // (the one-pass kernel writes var 0's probes itself).  The counting probe takes the counters of PLAN_MAX_COUNT_BITS and the sort all
+  // bits of the number type: both give the probes of the narrower range, and the number of sort passes - so the buffer the sorted keys
+  // end in - is fixed.
+  const L* sorted = ((LBITS + RS_BITS - 1) / RS_BITS) & 1 ? r.keys_b : r.keys_a;
+  for (uint32_t v = 0; v < n_vars; v++) {
+    const EncParams e_count = gated(1 + ACOMP_GATES_PER_VAR * v), e_sort = gated(2 + ACOMP_GATES_PER_VAR * v);
+    ln.begin("plan_probe_kernel_counting");
+    plan_probe_kernel<L, true, false, CHUNK_BINS><<<nc, PLAN_THREADS, ((size_t(1) << PLAN_MAX_COUNT_BITS) + 1) * 4 + 16, stream>>>(
+        e_count, r.lat[v], r.chunks, r.probes, int(v), PLAN_MAX_COUNT_BITS, r.key16[v]);
+    ln.end();
+    ln.begin("sort_keys_kernel");
+    sort_keys_kernel<L><<<nc * tiles, 256, 0, stream>>>(e_sort, tiles, r.lat[v], r.keys_a, r.chunks, int(v));
+    ln.end();
+    segment_offsets_kernel<<<(nc + 255) / 256, 256, 0, stream>>>(e_sort, v == 0 ? ep.order : 0, r.seg_begin, r.seg_end);
+    ln.begin("radix_sort_segments_kernel");
+    radix_sort_segments_kernel<L><<<nc, RS_THREADS, RS_SMEM, stream>>>(r.keys_a, r.keys_b, r.seg_begin, r.seg_end, LBITS);
+    ln.end();
+    ln.begin("plan_probe_kernel_sorted");
+    plan_probe_kernel<L, false, false, CHUNK_BINS><<<nc, PLAN_THREADS, 16, stream>>>(e_sort, sorted, r.chunks, r.probes, int(v), LBITS, nullptr);
+    ln.end();
+    ln.begin("plan_solve_kernel");
+    plan_solve_kernel<L, CHUNK_BINS><<<nc, SOLVE_THREADS, 0, stream>>>(ep, r.probes, r.chunks, r.plans, int(v));
+    ln.end();
+  }
+  fallback_kernel<false><<<(nc + 255) / 256, 256, 0, stream>>>(ep, r.plans, r.chunks, 0u);
+  // ---- K3 per var: the lookup-table binning on the 16-bit keys, or the search over the 64-bit latents
+  const uint32_t parts = (bpc + BINL_BATCHES - 1) / BINL_BATCHES, groups = (bpc + 7) / 8;
+  for (uint32_t v = 0; v < n_vars; v++) {
+    ln.begin("bin_lut_kernel");
+    bin_lut_kernel<L><<<nc * parts, BINL_THREADS, (size_t(1) << PLAN_MAX_COUNT_BITS) + 16, stream>>>(gated(3 + ACOMP_GATES_PER_VAR * v), bpc, parts, r.key16[v],
+                                                                                                    r.plans, r.chunks, r.sym[v], r.ob_sum, int(v), PLAN_MAX_COUNT_BITS);
+    ln.end();
+    ln.begin("bin_kernel");
+    bin_kernel<L, false><<<nc * groups, BIN_THREADS, 0, stream>>>(gated(4 + ACOMP_GATES_PER_VAR * v), bpc, r.lat[v], r.plans, r.chunks, r.sym[v], r.ob_sum, int(v));
+    ln.end();
+  }
+  ln.begin("ans_encode_kernel");
+  ans_encode_kernel<false><<<nc * MAX_VARS, ANS_THREADS, 0, stream>>>(ep, bpc, r.plans, r.chunks, r.sym[0], r.sym[1], r.ans[0], r.ans[1], r.ans_sum, r.entries, nullptr);
+  ln.end();
+  ln.begin("layout_kernel");
+  layout_kernel<false><<<nc, LAYOUT_THREADS, 0, stream>>>(ep, bpc, r.plans, r.chunks, r.ans_sum, r.ob_sum, r.entries);
+  ln.end();
+}
+
+// K5, behind the launches that place each chunk (ChunkEnc::out_offset): the pack gate, then one pack_kernel per choice of keys or
+// latents; only the one the range bits made finds its chunks inside dst_cap.
+template <typename L>
+void enqueue_pack(const AcompGeom& g, const AcompArgs& a, const EncParams& ep, const AsyncLaunch& ln) {
+  const cudaStream_t stream = ln.stream;
+  const AcompRegions<L> r = acomp_regions<L>(a);
+  const uint64_t n_copies = uint64_t(1) << a.n_vars;
+  acomp_pack_gate_kernel<<<uint32_t(std::min<uint64_t>(1024, (n_copies * g.n_chunks + ACOMP_THREADS - 1) / ACOMP_THREADS)), ACOMP_THREADS, 0, stream>>>(a);
+  const uint64_t out_cap = std::min<uint64_t>(a.dst_cap, ~uint64_t(0) - 1);
+  ln.begin("pack_kernel");
+  for (uint64_t k = 0; k < n_copies; k++)
+    pack_kernel<L><<<uint32_t(g.n_chunks), PACK_THREADS, sizeof(PackSmem), stream>>>(ep, g.bpc, r.lat[0], r.lat[1], r.plans, r.copies + k * g.n_chunks, r.sym[0],
+                                                                                     r.sym[1], r.ans[0], r.ans[1], r.entries, a.dst, out_cap,
+                                                                                     (k & 1) ? nullptr : r.key16[0], (a.n_vars > 1 && !(k & 2)) ? r.key16[1] : nullptr);
+  ln.end();
+}
+
+template <typename L>
+void acomp_launch(const PcoB200AsyncCompressPlan& p, const AcompGeom& g, const AcompArgs& a, const void* nums, PcoB200AsyncCompressStatus* status,
+                  const AsyncLaunch& ln) {
+  const cudaStream_t stream = ln.stream;
+  const uint32_t nc = uint32_t(g.n_chunks);
+  const uint32_t init_ctas = uint32_t(std::min<uint64_t>(1024, std::max<uint64_t>({g.n_chunks + 1, g.n_chunks * MAX_VARS * g.bpc, a.index_bytes / 16}) / ACOMP_THREADS + 1));
   ln.begin("acomp_init_kernel");
-  acomp_init_kernel<<<init_ctas, ACOMP_THREADS, 0, stream>>>(a, bpc);
+  acomp_init_kernel<<<init_ctas, ACOMP_THREADS, 0, stream>>>(a, g.bpc);
   ln.end();
   if (p.n > 0) {
-    ChunkEnc* chunks = reinterpret_cast<ChunkEnc*>(ws + l.chunks);
-    VarPlan* plans = reinterpret_cast<VarPlan*>(ws + l.plans);
-    PlanProbes* probes = reinterpret_cast<PlanProbes*>(ws + l.probes);
-    AcompHead* head = reinterpret_cast<AcompHead*>(ws);
-    uint64_t* gates = reinterpret_cast<uint64_t*>(ws + l.gates);
-    L* lat[MAX_VARS] = {reinterpret_cast<L*>(ws + l.lat[0]), p.n_vars > 1 ? reinterpret_cast<L*>(ws + l.lat[1]) : nullptr};
-    uint16_t* key16[MAX_VARS] = {reinterpret_cast<uint16_t*>(ws + l.key16[0]), p.n_vars > 1 ? reinterpret_cast<uint16_t*>(ws + l.key16[1]) : nullptr};
-    uint8_t* sym[MAX_VARS] = {ws + l.sym[0], p.n_vars > 1 ? ws + l.sym[1] : nullptr};
-    uint16_t* ans[MAX_VARS] = {reinterpret_cast<uint16_t*>(ws + l.ans[0]), p.n_vars > 1 ? reinterpret_cast<uint16_t*>(ws + l.ans[1]) : nullptr};
-    L* keys_a = reinterpret_cast<L*>(ws + l.keys_a);
-    L* keys_b = reinterpret_cast<L*>(ws + l.keys_b);
-    uint64_t* seg_begin = reinterpret_cast<uint64_t*>(ws + l.seg);
-    uint64_t* seg_end = seg_begin + nc;
-    uint32_t* ob_sum = reinterpret_cast<uint32_t*>(ws + l.ob_sum);
-    uint32_t* ans_sum = reinterpret_cast<uint32_t*>(ws + l.ans_sum);
-    BatchEntry* entries = reinterpret_cast<BatchEntry*>(ws + l.entries);
-    EncParams ep;
-    std::memset(&ep, 0, sizeof(ep));
-    ep.dtype = p.dtype;
-    ep.uniform_type = p.uniform_type_header ? p.dtype : 0;
-    ep.mode = p.mode;
-    ep.mode_base = p.mode_base;
-    ep.base_bits = p.base_bits;
-    ep.inv_base_bits = p.inv_base_bits;
-    ep.mode_k = p.mode_k;
-    ep.order = p.order;
-    ep.n_vars = p.n_vars;
-    ep.n_total = p.n;
-    ep.n_chunks = nc;
-    ep.max_chunk_n = uint32_t(g.max_n);
-    ep.bins_log[0] = p.bins_log;
-    ep.bins_log[1] = std::min<uint32_t>(p.bins_log, 6);  // LIMITED_UNOPTIMIZED_BINS_LOG (chunk_compressor.rs:238-248)
-    ep.nums = nums;
-    ep.chunk_starts = reinterpret_cast<const uint64_t*>(ws + l.starts);
-    ep.row_base = reinterpret_cast<const uint64_t*>(ws + l.rows);
-    auto gated = [&](uint32_t gate) { EncParams e = ep; e.chunk_starts = gates + uint64_t(gate) * (g.n_chunks + 1); return e; };
-    const uint32_t always_two = p.n_vars > 1 ? 1u : 0u;
-    // ---- front end: the one-pass kernel for Classic, then the two-kernel path behind its flag (always, for the two-var modes)
-    if (!always_two) {
-      ln.begin("split_count_kernel");
-      split_count_kernel<L><<<nc, SC_THREADS, size_t(SC_N) * 4, stream>>>(ep, chunks, probes, key16[0], head->flags);
-      ln.end();
-    }
-    acomp_two_gate_kernel<<<(nc + ACOMP_THREADS) / ACOMP_THREADS, ACOMP_THREADS, 0, stream>>>(a, always_two);
-    const EncParams e_two = gated(0);
-    ln.begin("split_delta_kernel");
-    switch (p.mode) {
-      case MODE_CLASSIC: split_delta_kernel<L, MODE_CLASSIC><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
-      case MODE_INT_MULT: split_delta_kernel<L, MODE_INT_MULT><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
-      case MODE_FLOAT_QUANT: split_delta_kernel<L, MODE_FLOAT_QUANT><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
-      default: split_delta_kernel<L, MODE_FLOAT_MULT><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
-    }
-    ln.end();
-    acomp_var_gate_kernel<<<1, 1024, 0, stream>>>(a, always_two);
-    // ---- planner per var: counting probe or sort path (whichever the range bits gate on), then the solver on the probes either left
-    // (the one-pass kernel writes var 0's probes itself).  The counting probe takes the counters of PLAN_MAX_COUNT_BITS and the sort all
-    // bits of the number type: both give the probes of the narrower range, and the number of sort passes - so the buffer the sorted keys
-    // end in - is fixed.
-    const L* sorted = ((LBITS + RS_BITS - 1) / RS_BITS) & 1 ? keys_b : keys_a;
-    for (uint32_t v = 0; v < p.n_vars; v++) {
-      const EncParams e_count = gated(1 + ACOMP_GATES_PER_VAR * v), e_sort = gated(2 + ACOMP_GATES_PER_VAR * v);
-      ln.begin("plan_probe_kernel_counting");
-      plan_probe_kernel<L, true><<<nc, PLAN_THREADS, ((size_t(1) << PLAN_MAX_COUNT_BITS) + 1) * 4 + 16, stream>>>(e_count, lat[v], chunks, probes, int(v),
-                                                                                                                    PLAN_MAX_COUNT_BITS, key16[v]);
-      ln.end();
-      ln.begin("sort_keys_kernel");
-      sort_keys_kernel<L><<<nc * tiles, 256, 0, stream>>>(e_sort, tiles, lat[v], keys_a, chunks, int(v));
-      ln.end();
-      segment_offsets_kernel<<<(nc + 255) / 256, 256, 0, stream>>>(e_sort, v == 0 ? p.order : 0, seg_begin, seg_end);
-      ln.begin("radix_sort_segments_kernel");
-      radix_sort_segments_kernel<L><<<nc, RS_THREADS, RS_SMEM, stream>>>(keys_a, keys_b, seg_begin, seg_end, LBITS);
-      ln.end();
-      ln.begin("plan_probe_kernel_sorted");
-      plan_probe_kernel<L, false><<<nc, PLAN_THREADS, 16, stream>>>(e_sort, sorted, chunks, probes, int(v), LBITS, nullptr);
-      ln.end();
-      ln.begin("plan_solve_kernel");
-      plan_solve_kernel<L><<<nc, SOLVE_THREADS, 0, stream>>>(ep, probes, chunks, plans, int(v));
-      ln.end();
-    }
-    fallback_kernel<false><<<(nc + 255) / 256, 256, 0, stream>>>(ep, plans, chunks, 0u);
-    // ---- K3 per var: the lookup-table binning on the 16-bit keys, or the search over the 64-bit latents
-    const uint32_t parts = (bpc + BINL_BATCHES - 1) / BINL_BATCHES, groups = (bpc + 7) / 8;
-    for (uint32_t v = 0; v < p.n_vars; v++) {
-      ln.begin("bin_lut_kernel");
-      bin_lut_kernel<L><<<nc * parts, BINL_THREADS, (size_t(1) << PLAN_MAX_COUNT_BITS) + 16, stream>>>(gated(3 + ACOMP_GATES_PER_VAR * v), bpc, parts, key16[v], plans,
-                                                                                                      chunks, sym[v], ob_sum, int(v), PLAN_MAX_COUNT_BITS);
-      ln.end();
-      ln.begin("bin_kernel");
-      bin_kernel<L, false><<<nc * groups, BIN_THREADS, 0, stream>>>(gated(4 + ACOMP_GATES_PER_VAR * v), bpc, lat[v], plans, chunks, sym[v], ob_sum, int(v));
-      ln.end();
-    }
-    ln.begin("ans_encode_kernel");
-    ans_encode_kernel<false><<<nc * MAX_VARS, ANS_THREADS, 0, stream>>>(ep, bpc, plans, chunks, sym[0], sym[1], ans[0], ans[1], ans_sum, entries, nullptr);
-    ln.end();
-    ln.begin("layout_kernel");
-    layout_kernel<false><<<nc, LAYOUT_THREADS, 0, stream>>>(ep, bpc, plans, chunks, ans_sum, ob_sum, entries);
-    ln.end();
-    chunk_offsets_kernel<<<1, 1024, 0, stream>>>(chunks, nc, a.header_bytes, 1u, &head->total);
-    // ---- K5: one launch per choice of keys or latents; only the one the range bits made finds its chunks inside dst_cap
-    const uint64_t n_copies = uint64_t(1) << p.n_vars;
-    acomp_pack_gate_kernel<<<uint32_t(std::min<uint64_t>(1024, (n_copies * g.n_chunks + ACOMP_THREADS - 1) / ACOMP_THREADS)), ACOMP_THREADS, 0, stream>>>(a);
-    const uint64_t out_cap = std::min<uint64_t>(p.dst_cap, ~uint64_t(0) - 1);
-    ln.begin("pack_kernel");
-    for (uint64_t k = 0; k < n_copies; k++) {
-      const ChunkEnc* copy = reinterpret_cast<const ChunkEnc*>(ws + l.copies) + k * g.n_chunks;
-      pack_kernel<L><<<nc, PACK_THREADS, sizeof(PackSmem), stream>>>(ep, bpc, lat[0], lat[1], plans, copy, sym[0], sym[1], ans[0], ans[1], entries, a.dst, out_cap,
-                                                                     (k & 1) ? nullptr : key16[0], (p.n_vars > 1 && !(k & 2)) ? key16[1] : nullptr);
-    }
-    ln.end();
-    header_footer_kernel<<<1, 32, 0, stream>>>(a.dst, out_cap, ws + 64, a.header_bytes, &head->total);
+    // the secondary var takes at most LIMITED_UNOPTIMIZED_BINS_LOG (chunk_compressor.rs:238-248)
+    const EncParams ep = acomp_enc_params(p, g, a, nums, p.n, p.bins_log, std::min<uint32_t>(p.bins_log, 6));
+    const AcompRegions<L> r = acomp_regions<L>(a);
+    enqueue_encode_kernels<L, false>(g, a, ep, ln);
+    chunk_offsets_kernel<<<1, 1024, 0, stream>>>(r.chunks, nc, a.header_bytes, 1u, &r.head->total);
+    enqueue_pack<L>(g, a, ep, ln);
+    header_footer_kernel<<<1, 32, 0, stream>>>(a.dst, std::min<uint64_t>(a.dst_cap, ~uint64_t(0) - 1), a.ws + 64, a.header_bytes, &r.head->total);
     if (a.index_bytes)
-      emit_index_kernel<<<nc, 256, 0, stream>>>(ep, bpc, chunks, entries, a.index, sizeof(IndexHeader), reinterpret_cast<const uint64_t*>(ws + l.eoff), &head->total,
-                                                1u, 0u, 0, 1u);
+      emit_index_kernel<<<nc, 256, 0, stream>>>(ep, g.bpc, r.chunks, r.entries, a.index, sizeof(IndexHeader), reinterpret_cast<const uint64_t*>(a.ws + a.lay.eoff),
+                                                &r.head->total, 1u, 0u, 0, 1u);
   }
   ln.begin("acomp_finish_kernel");
   acomp_finish_kernel<<<1, 32, 0, stream>>>(a, status);

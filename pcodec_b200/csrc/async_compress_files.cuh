@@ -10,9 +10,9 @@
 //                           max_file_n, or the running sum of the counts past nums_cap, with exact 64-bit overflow detection);
 //   acf_init_kernel         per chunk slot: its start and row base (EqualPagesUpTo per file in closed form; the chunks of a refused batch
 //                           and the pad slots up to max_chunks hold 0 numbers), its file, its ChunkEnc reset; the zeroed offset-bit sums;
-//   the encode kernels      as pco_b200_compress_async runs them, behind the same gates (async_compress.cuh, which read the starts table
-//                           this init kernel wrote); split_count_kernel, plan_probe_kernel and plan_solve_kernel in their CHUNK_BINS
-//                           instantiations, which compute each chunk's unoptimized_bins_log from its n;
+//   the encode kernels      enqueue_encode_kernels (async_compress.cuh), as pco_b200_compress_async runs them behind the same gates
+//                           (which read the starts table this init kernel wrote); split_count_kernel, plan_probe_kernel and
+//                           plan_solve_kernel in their CHUNK_BINS instantiations, which compute each chunk's unoptimized_bins_log from its n;
 //   acf_bytes_kernel, acf_bytes_scan_kernel, acf_offsets_kernel
 //                           a multi-CTA exclusive scan of the chunk sizes layout_kernel wrote: each chunk's place in dst behind its file's
 //                           header, every file's place and length, and whether the batch fits dst_cap and index_cap.  A chunk that is not
@@ -442,8 +442,7 @@ inline AcfPlanGeom acf_plan_geom(const PcoB200AsyncCompressFilesPlan& p) {
 }
 
 inline PcoB200Error acf_check_plan(const PcoB200AsyncCompressFilesPlan* p, AcfPlanGeom* pg) {
-  if (!p || !nt_valid(p->dtype) || p->mode > MODE_FLOAT_QUANT || p->n_vars != (p->mode == MODE_CLASSIC ? 1u : 2u) || p->order > MAX_ORDER ||
-      p->level > 12 || p->max_files == 0 || p->max_files > 0x7fffffffu || p->max_file_n == 0 || p->nums_cap > (uint64_t(1) << 56) ||
+  if (!acomp_spec_ok(p) || p->level > 12 || p->max_files == 0 || p->max_files > 0x7fffffffu || p->max_file_n == 0 || p->nums_cap > (uint64_t(1) << 56) ||
       p->max_chunks != p->nums_cap / acf_chunk_n(p->max_page_n, p->max_file_n, p->nums_cap) + p->max_files || p->max_chunks > 0x7fffffffu)
     return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_compress_files_async_plan");
   *pg = acf_plan_geom(*p);
@@ -455,12 +454,6 @@ inline PcoB200Error acf_check_plan(const PcoB200AsyncCompressFilesPlan* p, AcfPl
 template <typename L>
 void acf_launch_encode(const PcoB200AsyncCompressFilesPlan& p, const AcompGeom& g, const AcfArgs& fa, const void* nums, const AsyncLaunch& ln) {
   const cudaStream_t stream = ln.stream;
-  const AcompArgs& a = fa.a;
-  const uint32_t nc = uint32_t(g.n_chunks), bpc = g.bpc, tiles = g.tiles;
-  constexpr uint32_t LBITS = sizeof(L) * 8;
-  constexpr size_t RS_SMEM = size_t(RS_WARPS) * RS_BINS * sizeof(uint32_t);
-  uint8_t* ws = a.ws;
-  const AcompLayout& l = a.lay;
   const uint32_t file_ctas = uint32_t(acf_ctas(p.max_files)), chunk_ctas = uint32_t(acf_ctas(g.n_chunks + 1));
   ln.begin("acf_files_kernel");
   acf_files_kernel<<<file_ctas, ACF_THREADS, 0, stream>>>(fa);
@@ -471,101 +464,13 @@ void acf_launch_encode(const PcoB200AsyncCompressFilesPlan& p, const AcompGeom& 
   ln.begin("acf_place_kernel");
   acf_place_kernel<<<file_ctas, ACF_THREADS, 0, stream>>>(fa);
   ln.end();
-  const uint32_t init_ctas = uint32_t(std::min<uint64_t>(1024, std::max<uint64_t>(g.n_chunks + 1, g.n_chunks * MAX_VARS * bpc) / ACF_THREADS + 1));
+  const uint32_t init_ctas = uint32_t(std::min<uint64_t>(1024, std::max<uint64_t>(g.n_chunks + 1, g.n_chunks * MAX_VARS * g.bpc) / ACF_THREADS + 1));
   ln.begin("acf_init_kernel");
   acf_init_kernel<<<init_ctas, ACF_THREADS, 0, stream>>>(fa);
   ln.end();
-  ChunkEnc* chunks = reinterpret_cast<ChunkEnc*>(ws + l.chunks);
-  VarPlan* plans = reinterpret_cast<VarPlan*>(ws + l.plans);
-  PlanProbes* probes = reinterpret_cast<PlanProbes*>(ws + l.probes);
-  AcompHead* head = reinterpret_cast<AcompHead*>(ws);
-  uint64_t* gates = reinterpret_cast<uint64_t*>(ws + l.gates);
-  L* lat[MAX_VARS] = {reinterpret_cast<L*>(ws + l.lat[0]), p.n_vars > 1 ? reinterpret_cast<L*>(ws + l.lat[1]) : nullptr};
-  uint16_t* key16[MAX_VARS] = {reinterpret_cast<uint16_t*>(ws + l.key16[0]), p.n_vars > 1 ? reinterpret_cast<uint16_t*>(ws + l.key16[1]) : nullptr};
-  uint8_t* sym[MAX_VARS] = {ws + l.sym[0], p.n_vars > 1 ? ws + l.sym[1] : nullptr};
-  uint16_t* ans[MAX_VARS] = {reinterpret_cast<uint16_t*>(ws + l.ans[0]), p.n_vars > 1 ? reinterpret_cast<uint16_t*>(ws + l.ans[1]) : nullptr};
-  L* keys_a = reinterpret_cast<L*>(ws + l.keys_a);
-  L* keys_b = reinterpret_cast<L*>(ws + l.keys_b);
-  uint64_t* seg_begin = reinterpret_cast<uint64_t*>(ws + l.seg);
-  uint64_t* seg_end = seg_begin + nc;
-  uint32_t* ob_sum = reinterpret_cast<uint32_t*>(ws + l.ob_sum);
-  uint32_t* ans_sum = reinterpret_cast<uint32_t*>(ws + l.ans_sum);
-  BatchEntry* entries = reinterpret_cast<BatchEntry*>(ws + l.entries);
-  EncParams ep;
-  std::memset(&ep, 0, sizeof(ep));
-  ep.dtype = p.dtype;
-  ep.uniform_type = p.uniform_type_header ? p.dtype : 0;
-  ep.mode = p.mode;
-  ep.mode_base = p.mode_base;
-  ep.base_bits = p.base_bits;
-  ep.inv_base_bits = p.inv_base_bits;
-  ep.mode_k = p.mode_k;
-  ep.order = p.order;
-  ep.n_vars = p.n_vars;
-  ep.n_total = p.nums_cap;
-  ep.n_chunks = nc;
-  ep.max_chunk_n = uint32_t(g.max_n);
-  ep.bins_log[0] = p.level;  // the CHUNK_BINS kernels compute each chunk's unoptimized_bins_log from the level and its n
-  ep.nums = nums;
-  ep.chunk_starts = reinterpret_cast<const uint64_t*>(ws + l.starts);
-  ep.row_base = reinterpret_cast<const uint64_t*>(ws + l.rows);
-  auto gated = [&](uint32_t gate) { EncParams e = ep; e.chunk_starts = gates + uint64_t(gate) * (g.n_chunks + 1); return e; };
-  const uint32_t always_two = p.n_vars > 1 ? 1u : 0u;
-  // ---- the encode kernels, as acomp_launch runs them
-  if (!always_two) {
-    ln.begin("split_count_kernel");
-    split_count_kernel<L, true><<<nc, SC_THREADS, size_t(SC_N) * 4, stream>>>(ep, chunks, probes, key16[0], head->flags);
-    ln.end();
-  }
-  acomp_two_gate_kernel<<<(nc + ACOMP_THREADS) / ACOMP_THREADS, ACOMP_THREADS, 0, stream>>>(a, always_two);
-  const EncParams e_two = gated(0);
-  ln.begin("split_delta_kernel");
-  switch (p.mode) {
-    case MODE_CLASSIC: split_delta_kernel<L, MODE_CLASSIC><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
-    case MODE_INT_MULT: split_delta_kernel<L, MODE_INT_MULT><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
-    case MODE_FLOAT_QUANT: split_delta_kernel<L, MODE_FLOAT_QUANT><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
-    default: split_delta_kernel<L, MODE_FLOAT_MULT><<<nc * tiles, SPLIT_THREADS, 0, stream>>>(e_two, tiles, lat[0], lat[1], chunks); break;
-  }
-  ln.end();
-  acomp_var_gate_kernel<<<1, 1024, 0, stream>>>(a, always_two);
-  const L* sorted = ((LBITS + RS_BITS - 1) / RS_BITS) & 1 ? keys_b : keys_a;
-  for (uint32_t v = 0; v < p.n_vars; v++) {
-    const EncParams e_count = gated(1 + ACOMP_GATES_PER_VAR * v), e_sort = gated(2 + ACOMP_GATES_PER_VAR * v);
-    ln.begin("plan_probe_kernel_counting");
-    plan_probe_kernel<L, true, false, true><<<nc, PLAN_THREADS, ((size_t(1) << PLAN_MAX_COUNT_BITS) + 1) * 4 + 16, stream>>>(
-        e_count, lat[v], chunks, probes, int(v), PLAN_MAX_COUNT_BITS, key16[v]);
-    ln.end();
-    ln.begin("sort_keys_kernel");
-    sort_keys_kernel<L><<<nc * tiles, 256, 0, stream>>>(e_sort, tiles, lat[v], keys_a, chunks, int(v));
-    ln.end();
-    segment_offsets_kernel<<<(nc + 255) / 256, 256, 0, stream>>>(e_sort, v == 0 ? p.order : 0, seg_begin, seg_end);
-    ln.begin("radix_sort_segments_kernel");
-    radix_sort_segments_kernel<L><<<nc, RS_THREADS, RS_SMEM, stream>>>(keys_a, keys_b, seg_begin, seg_end, LBITS);
-    ln.end();
-    ln.begin("plan_probe_kernel_sorted");
-    plan_probe_kernel<L, false, false, true><<<nc, PLAN_THREADS, 16, stream>>>(e_sort, sorted, chunks, probes, int(v), LBITS, nullptr);
-    ln.end();
-    ln.begin("plan_solve_kernel");
-    plan_solve_kernel<L, true><<<nc, SOLVE_THREADS, 0, stream>>>(ep, probes, chunks, plans, int(v));
-    ln.end();
-  }
-  fallback_kernel<false><<<(nc + 255) / 256, 256, 0, stream>>>(ep, plans, chunks, 0u);
-  const uint32_t parts = (bpc + BINL_BATCHES - 1) / BINL_BATCHES, groups = (bpc + 7) / 8;
-  for (uint32_t v = 0; v < p.n_vars; v++) {
-    ln.begin("bin_lut_kernel");
-    bin_lut_kernel<L><<<nc * parts, BINL_THREADS, (size_t(1) << PLAN_MAX_COUNT_BITS) + 16, stream>>>(gated(3 + ACOMP_GATES_PER_VAR * v), bpc, parts, key16[v], plans,
-                                                                                                    chunks, sym[v], ob_sum, int(v), PLAN_MAX_COUNT_BITS);
-    ln.end();
-    ln.begin("bin_kernel");
-    bin_kernel<L, false><<<nc * groups, BIN_THREADS, 0, stream>>>(gated(4 + ACOMP_GATES_PER_VAR * v), bpc, lat[v], plans, chunks, sym[v], ob_sum, int(v));
-    ln.end();
-  }
-  ln.begin("ans_encode_kernel");
-  ans_encode_kernel<false><<<nc * MAX_VARS, ANS_THREADS, 0, stream>>>(ep, bpc, plans, chunks, sym[0], sym[1], ans[0], ans[1], ans_sum, entries, nullptr);
-  ln.end();
-  ln.begin("layout_kernel");
-  layout_kernel<false><<<nc, LAYOUT_THREADS, 0, stream>>>(ep, bpc, plans, chunks, ans_sum, ob_sum, entries);
-  ln.end();
+  // the CHUNK_BINS kernels compute each chunk's unoptimized_bins_log from the level and its n
+  const EncParams ep = acomp_enc_params(p, g, fa.a, nums, p.nums_cap, p.level, 0);
+  enqueue_encode_kernels<L, true>(g, fa.a, ep, ln);
   // ---- placement: every chunk's final place in dst, behind its file's header
   ln.begin("acf_bytes_kernel");
   acf_bytes_kernel<<<chunk_ctas, ACF_THREADS, 0, stream>>>(fa);
@@ -576,16 +481,7 @@ void acf_launch_encode(const PcoB200AsyncCompressFilesPlan& p, const AcompGeom& 
   ln.begin("acf_offsets_kernel");
   acf_offsets_kernel<<<chunk_ctas, ACF_THREADS, 0, stream>>>(fa);
   ln.end();
-  const uint64_t n_copies = uint64_t(1) << p.n_vars;
-  acomp_pack_gate_kernel<<<uint32_t(std::min<uint64_t>(1024, (n_copies * g.n_chunks + ACOMP_THREADS - 1) / ACOMP_THREADS)), ACOMP_THREADS, 0, stream>>>(a);
-  const uint64_t out_cap = std::min<uint64_t>(p.dst_cap, ~uint64_t(0) - 1);
-  ln.begin("pack_kernel");
-  for (uint64_t k = 0; k < n_copies; k++) {
-    const ChunkEnc* copy = reinterpret_cast<const ChunkEnc*>(ws + l.copies) + k * g.n_chunks;
-    pack_kernel<L><<<nc, PACK_THREADS, sizeof(PackSmem), stream>>>(ep, bpc, lat[0], lat[1], plans, copy, sym[0], sym[1], ans[0], ans[1], entries, a.dst, out_cap,
-                                                                   (k & 1) ? nullptr : key16[0], (p.n_vars > 1 && !(k & 2)) ? key16[1] : nullptr);
-  }
-  ln.end();
+  enqueue_pack<L>(g, fa.a, ep, ln);
 }
 
 template <typename L>

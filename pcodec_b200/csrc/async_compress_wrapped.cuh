@@ -249,8 +249,7 @@ inline AcwPlanGeom acw_plan_geom(const PcoB200AsyncCompressWrappedPlan& p) {
 
 inline PcoB200Error acw_check_plan(const PcoB200AsyncCompressWrappedPlan* p, AcwPlanGeom* pg) {
   const char* what = "the plan was not made by pco_b200_compress_wrapped_async_plan";
-  if (!p || !nt_valid(p->dtype) || p->mode > MODE_FLOAT_QUANT || p->n_vars != (p->mode == MODE_CLASSIC ? 1u : 2u) || p->order > MAX_ORDER ||
-      p->level > 12 || p->max_arrays == 0 || p->max_arrays > 0x7fffffffu || p->max_array_n == 0 || p->nums_cap > (uint64_t(1) << 56) ||
+  if (!acomp_spec_ok(p) || p->level > 12 || p->max_arrays == 0 || p->max_arrays > 0x7fffffffu || p->max_array_n == 0 || p->nums_cap > (uint64_t(1) << 56) ||
       p->max_chunks != p->nums_cap / acf_chunk_n(p->max_page_n, p->max_array_n, p->nums_cap) + p->max_arrays || p->max_chunks > 0x7fffffffu)
     return fail(PCO_B200_INVALID_ARGUMENT, what);
   *pg = acw_plan_geom(*p);

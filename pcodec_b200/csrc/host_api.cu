@@ -771,6 +771,9 @@ static PcoB200Error load_kernels(std::initializer_list<const void*> kernels) {
   return PCO_B200_OK;
 }
 
+// The PcoB200Error of an asynchronous call's status kind, as its *_result function returns it (a kind no call writes reads as Corruption)
+static PcoB200Error async_result_kind(uint32_t kind) { return kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(kind) : PCO_B200_CORRUPTION; }
+
 // The set-up of an asynchronous decompress plan: the device, the decode kernels' attributes (the window-mode instantiations when WIN),
 // and loaded: the decode stage's kernels for dtype, the call's catch-all kernel (cold(tag) for a latent type tag) and the call's `kernels`.
 template <bool WIN, typename Cold>
@@ -783,6 +786,47 @@ static PcoB200Error async_decode_setup(unsigned char dtype, Cold cold, std::init
     using L = decltype(tag);
     return load_kernels({(const void*)fused_narrow_kernel<L, WIN>, (const void*)symwalk_kernel<WIN>, (const void*)decode_kernel<L, 1, WIN>,
                          (const void*)decode_kernel<L, 2, WIN>, cold(tag)});
+  });
+}
+
+// The plan fields an explicit ModeSpec and DeltaSpec fix (P: any of the three asynchronous compress plans)
+template <typename P>
+static void fill_explicit_spec(P* plan, const ConfigCheck& ck) {
+  plan->mode = ck.explicit_mode.mode;
+  plan->order = ck.explicit_order;
+  plan->n_vars = ck.explicit_mode.mode == MODE_CLASSIC ? 1 : 2;
+  plan->mode_k = ck.explicit_mode.mode_k;
+  plan->mode_base = ck.explicit_mode.mode_base;
+  plan->base_bits = ck.explicit_mode.base_bits;
+  plan->inv_base_bits = ck.explicit_mode.inv_base_bits;
+}
+
+// The one-time device set-up of an asynchronous compress plan, here and not in a call (which may be inside a capture): the device, the
+// attributes compress_typed sets on first use, and loaded: the encode stage's kernels for dtype (split_count_kernel and the planner
+// kernels in their CHUNK_BINS instantiations when CHUNK_BINS) and the call's `extra` kernels.
+template <bool CHUNK_BINS>
+static PcoB200Error async_encode_setup(unsigned char dtype, std::initializer_list<const void*> extra) {
+  Context& c = ctx();
+  if (PcoB200Error e = ensure_device(c)) return e;
+  if (PcoB200Error e = load_kernels(extra)) return e;
+  if (PcoB200Error e = load_kernels({(const void*)acomp_two_gate_kernel, (const void*)acomp_var_gate_kernel, (const void*)acomp_pack_gate_kernel,
+                                     (const void*)segment_offsets_kernel, (const void*)fallback_kernel<false>, (const void*)ans_encode_kernel<false>,
+                                     (const void*)layout_kernel<false>})) return e;
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
+    using L = decltype(tag);
+    constexpr size_t RS_SMEM = size_t(RS_WARPS) * RS_BINS * sizeof(uint32_t);
+    const int count_smem = int(((size_t(1) << PLAN_MAX_COUNT_BITS) + 1) * 4 + 16);
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true, false, CHUNK_BINS>, cudaFuncAttributeMaxDynamicSharedMemorySize, count_smem));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(split_count_kernel<L, CHUNK_BINS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(size_t(SC_N) * 4)));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PackSmem)));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(radix_sort_segments_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RS_SMEM));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true, false, CHUNK_BINS>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    PCOB_CUDA_TRY(cudaFuncSetAttribute(bin_lut_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    return load_kernels({(const void*)split_count_kernel<L, CHUNK_BINS>, (const void*)split_delta_kernel<L, MODE_CLASSIC>, (const void*)split_delta_kernel<L, MODE_INT_MULT>,
+                         (const void*)split_delta_kernel<L, MODE_FLOAT_QUANT>, (const void*)split_delta_kernel<L, MODE_FLOAT_MULT>,
+                         (const void*)plan_probe_kernel<L, false, false, CHUNK_BINS>, (const void*)sort_keys_kernel<L>, (const void*)plan_solve_kernel<L, CHUNK_BINS>,
+                         (const void*)bin_kernel<L, false>});
   });
 }
 
@@ -911,16 +955,20 @@ PcoB200Error pco_b200_simple_decompress_into(const void* compressed, size_t comp
   return pco_b200_decompress_ex(compressed, compressed_len, dtype, dst, dst_len, progress, nullptr, 0, 0, nullptr);
 }
 
+// The config a call runs: *config, or pco::ChunkConfig::default() (level 8, Auto, Auto, EqualPagesUpTo(2^18)) when config is null
+static PcoB200ChunkConfig default_chunk_config(const PcoB200ChunkConfig* config) {
+  if (config) return *config;
+  PcoB200ChunkConfig cfg;
+  std::memset(&cfg, 0, sizeof(cfg));
+  cfg.compression_level = 8;
+  return cfg;
+}
+
 static PcoB200Error compress_dispatch(const void* nums, size_t n, unsigned char dtype, const PcoB200ChunkConfig* config, bool uniform, void* dst,
                                       size_t dst_cap, size_t* n_written, void* index, size_t index_cap, size_t* index_len, uint32_t flags,
                                       void* cuda_stream) {
   if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
-  PcoB200ChunkConfig cfg;
-  if (config) cfg = *config;
-  else {
-    std::memset(&cfg, 0, sizeof(cfg));  // pco::ChunkConfig::default(): level 8, Auto, Auto, EqualPagesUpTo(2^18)
-    cfg.compression_level = 8;
-  }
+  const PcoB200ChunkConfig cfg = default_chunk_config(config);
   Context& c = ctx();
   if (PcoB200Error e = ensure_device(c)) return e;
   CompressResult res;
@@ -1046,9 +1094,7 @@ PcoB200Error pco_b200_chunk_compressor_new(const void* nums, size_t n, unsigned 
   *out = nullptr;
   if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
   if (n == 0) return fail(PCO_B200_INVALID_ARGUMENT, "cannot compress empty chunk");  // chunk_compressor.rs:113-127
-  PcoB200ChunkConfig cfg;
-  if (config) cfg = *config;
-  else { std::memset(&cfg, 0, sizeof(cfg)); cfg.compression_level = 8; }
+  const PcoB200ChunkConfig cfg = default_chunk_config(config);
   std::vector<uint64_t> pages;
   if (PcoB200Error e = n_per_page(cfg, n, &pages)) return e;
   auto cc = std::make_unique<PcoB200ChunkCompressor>();
@@ -1526,12 +1572,7 @@ static PcoB200Error compress_wrapped_impl(const void* nums, size_t n, uint32_t d
   if (metas_len) *metas_len = 0;
   if (pages_len) *pages_len = 0;
   if (n_chunks_out) *n_chunks_out = 0;
-  PcoB200ChunkConfig cfg;
-  if (config) cfg = *config;
-  else {
-    std::memset(&cfg, 0, sizeof(cfg));  // pco::ChunkConfig::default()
-    cfg.compression_level = 8;
-  }
+  const PcoB200ChunkConfig cfg = default_chunk_config(config);
   Context& c = ctx();
   if (PcoB200Error e = ensure_device(c)) return e;
   // the chunks simple_compress would write; a paging spec that does not fit is reported by the pipeline, with its other checks
@@ -1665,12 +1706,7 @@ static PcoB200Error compress_files_impl(const void* nums, const uint64_t* file_n
   if (n_files == 0) return PCO_B200_OK;
   if (!file_ns || !files) return fail(PCO_B200_INVALID_ARGUMENT, "file_ns and files are required");
   if ((!dst && dst_cap) || (!index && index_cap)) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
-  PcoB200ChunkConfig cfg;
-  if (config) cfg = *config;
-  else {
-    std::memset(&cfg, 0, sizeof(cfg));  // pco::ChunkConfig::default()
-    cfg.compression_level = 8;
-  }
+  const PcoB200ChunkConfig cfg = default_chunk_config(config);
   // ---- every file's config check, on the host and in file order
   const uint32_t lbits = nt_bits(dtype);
   size_t first_bad = n_files;
@@ -2593,7 +2629,7 @@ PcoB200Error pco_b200_decompress_async(const PcoB200AsyncPlan* plan, const void*
 
 PcoB200Error pco_b200_decompress_async_result(const PcoB200AsyncStatus* s, PcoB200Progress* progress) {
   if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
-  const PcoB200Error kind = s->kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(s->kind) : PCO_B200_CORRUPTION;
+  const PcoB200Error kind = async_result_kind(s->kind);
   if (kind == PCO_B200_OK) {
     if (progress) {
       progress->n_processed = size_t(s->n_processed);
@@ -2734,7 +2770,7 @@ PcoB200Error pco_b200_decompress_ranges_async(const PcoB200AsyncRangesPlan* plan
 
 PcoB200Error pco_b200_decompress_ranges_async_result(const PcoB200AsyncRangesStatus* s, size_t* n_written) {
   if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
-  const PcoB200Error kind = s->kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(s->kind) : PCO_B200_CORRUPTION;
+  const PcoB200Error kind = async_result_kind(s->kind);
   if (kind == PCO_B200_OK) {
     if (n_written) *n_written = size_t(s->n_written);
     return PCO_B200_OK;
@@ -2861,7 +2897,7 @@ PcoB200Error pco_b200_decompress_files_async(const PcoB200AsyncFilesPlan* plan, 
 
 PcoB200Error pco_b200_decompress_files_async_result(const PcoB200AsyncFilesStatus* s, size_t* n_written) {
   if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
-  const PcoB200Error kind = s->kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(s->kind) : PCO_B200_CORRUPTION;
+  const PcoB200Error kind = async_result_kind(s->kind);
   if (kind == PCO_B200_OK) {
     if (n_written) *n_written = size_t(s->n_written);
     return PCO_B200_OK;
@@ -3000,7 +3036,7 @@ PcoB200Error pco_b200_decompress_pages_async(const PcoB200AsyncPagesPlan* plan, 
 
 PcoB200Error pco_b200_decompress_pages_async_result(const PcoB200AsyncPagesStatus* s, size_t* n_written) {
   if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
-  const PcoB200Error kind = s->kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(s->kind) : PCO_B200_CORRUPTION;
+  const PcoB200Error kind = async_result_kind(s->kind);
   if (kind == PCO_B200_OK) {
     if (n_written) *n_written = size_t(s->n_written);
     return PCO_B200_OK;
@@ -3021,20 +3057,16 @@ PcoB200Error pco_b200_decompress_pages_async_result(const PcoB200AsyncPagesStatu
 }
 
 // ---- asynchronous compress (pco_b200_compress_async; gate kernels in async_compress.cuh).  The plan fixes the layout and the config;
-// the call is a fixed sequence of launches: init, [split_count, two-kernel gate], split_delta, range gate, per var (counting probe, sort
-// keys, segment offsets, radix sort, sorted probe, solve), fallback, per var (bin_lut, bin), ans, layout, chunk offsets, pack gate, one
-// pack per choice of keys, header, [index], finish.  n == 0 is init and finish only.
+// the call is a fixed sequence of launches: init, the encode stage (enqueue_encode_kernels: [split_count], two-kernel gate, split_delta,
+// range gate, per var (counting probe, sort keys, segment offsets, radix sort, sorted probe, solve), fallback, per var (bin_lut, bin),
+// ans, layout), chunk offsets, pack gate, one pack per choice of keys (enqueue_pack), header, [index], finish.  n == 0 is init and
+// finish only.
 
 PcoB200Error pco_b200_compress_async_plan(size_t n, unsigned char dtype, const PcoB200ChunkConfig* config, int uniform_type_header, size_t dst_cap,
                                           size_t index_cap, PcoB200AsyncCompressPlan* plan) {
   if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
   if (!plan) return fail(PCO_B200_INVALID_ARGUMENT, "null plan");
-  PcoB200ChunkConfig cfg;
-  if (config) cfg = *config;
-  else {
-    std::memset(&cfg, 0, sizeof(cfg));  // pco::ChunkConfig::default(): level 8, Auto, Auto, EqualPagesUpTo(2^18)
-    cfg.compression_level = 8;
-  }
+  const PcoB200ChunkConfig cfg = default_chunk_config(config);
   ConfigCheck ck;
   if (PcoB200Error e = check_config(cfg, dtype, n, &ck)) return e;
   if (ck.auto_mode || ck.auto_delta)
@@ -3052,47 +3084,18 @@ PcoB200Error pco_b200_compress_async_plan(size_t n, unsigned char dtype, const P
   std::memset(plan, 0, sizeof(*plan));
   plan->dtype = dtype;
   plan->uniform_type_header = uniform_type_header ? 1 : 0;
-  plan->mode = ck.explicit_mode.mode;
-  plan->order = ck.explicit_order;
-  plan->n_vars = ck.explicit_mode.mode == MODE_CLASSIC ? 1 : 2;
+  fill_explicit_spec(plan, ck);
   plan->bins_log = bins_log;
-  plan->mode_k = ck.explicit_mode.mode_k;
   plan->n = n;
   plan->max_page_n = cfg.max_page_n;
   plan->dst_cap = dst_cap;
   plan->index_cap = index_cap;
-  plan->mode_base = ck.explicit_mode.mode_base;
-  plan->base_bits = ck.explicit_mode.base_bits;
-  plan->inv_base_bits = ck.explicit_mode.inv_base_bits;
   plan->index_bytes = acomp_index_bytes(g, plan->n_vars);
   plan->workspace_bytes = acomp_layout(g, nt_bits(dtype) / 8, plan->n_vars).total;
   if (index_cap != 0 && index_cap < plan->index_bytes)
     return fail(PCO_B200_IO, "index buffer too small (need " + std::to_string(plan->index_bytes) + " bytes)");
-  // the one-time device set-up, here and not in a call (which may be inside a capture): the attributes compress_typed sets on first
-  // use, and every kernel the call launches loaded now (with lazy module loading a kernel is otherwise loaded at its first launch)
-  Context& c = ctx();
-  if (PcoB200Error e = ensure_device(c)) return e;
-  if (PcoB200Error e = load_kernels({(const void*)acomp_init_kernel, (const void*)acomp_two_gate_kernel, (const void*)acomp_var_gate_kernel,
-                                     (const void*)acomp_pack_gate_kernel, (const void*)acomp_finish_kernel, (const void*)init_chunks_kernel,
-                                     (const void*)segment_offsets_kernel, (const void*)fallback_kernel<false>, (const void*)ans_encode_kernel<false>,
-                                     (const void*)layout_kernel<false>, (const void*)chunk_offsets_kernel, (const void*)header_footer_kernel,
-                                     (const void*)emit_index_kernel})) return e;
-  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
-    using L = decltype(tag);
-    constexpr size_t RS_SMEM = size_t(RS_WARPS) * RS_BINS * sizeof(uint32_t);
-    const int count_smem = int(((size_t(1) << PLAN_MAX_COUNT_BITS) + 1) * 4 + 16);
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, count_smem));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(split_count_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(size_t(SC_N) * 4)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PackSmem)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(radix_sort_segments_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RS_SMEM));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(bin_lut_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    return load_kernels({(const void*)split_count_kernel<L>, (const void*)split_delta_kernel<L, MODE_CLASSIC>, (const void*)split_delta_kernel<L, MODE_INT_MULT>,
-                         (const void*)split_delta_kernel<L, MODE_FLOAT_QUANT>, (const void*)split_delta_kernel<L, MODE_FLOAT_MULT>,
-                         (const void*)plan_probe_kernel<L, false>, (const void*)sort_keys_kernel<L>, (const void*)plan_solve_kernel<L>,
-                         (const void*)bin_kernel<L, false>});
-  });
+  return async_encode_setup<false>(dtype, {(const void*)acomp_init_kernel, (const void*)acomp_finish_kernel, (const void*)chunk_offsets_kernel,
+                                           (const void*)header_footer_kernel, (const void*)emit_index_kernel});
 }
 
 PcoB200Error pco_b200_compress_async(const PcoB200AsyncCompressPlan* plan, const void* nums, void* dst, void* index, void* workspace,
@@ -3128,7 +3131,7 @@ PcoB200Error pco_b200_compress_async(const PcoB200AsyncCompressPlan* plan, const
 
 PcoB200Error pco_b200_compress_async_result(const PcoB200AsyncCompressStatus* s, size_t* n_written, size_t* index_len) {
   if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
-  const PcoB200Error kind = s->kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(s->kind) : PCO_B200_CORRUPTION;
+  const PcoB200Error kind = async_result_kind(s->kind);
   if (kind == PCO_B200_OK) {
     if (n_written) *n_written = size_t(s->n_written);
     if (index_len) *index_len = size_t(s->index_bytes);
@@ -3140,21 +3143,16 @@ PcoB200Error pco_b200_compress_async_result(const PcoB200AsyncCompressStatus* s,
 }
 
 // ---- asynchronous batch compress (pco_b200_compress_files_async; kernels in async_compress_files.cuh).  The plan fixes the config and the
-// grids from the capacities; the call is a fixed sequence of launches: files, scan, place, init, the encode kernels of
-// pco_b200_compress_async (split_count and the planner kernels in their CHUNK_BINS instantiations), bytes, bytes scan, offsets, pack gate,
-// one pack per choice of keys, frame, [index], finish.
+// grids from the capacities; the call is a fixed sequence of launches: files, scan, place, init, the encode stage of
+// pco_b200_compress_async (enqueue_encode_kernels, with split_count and the planner kernels in their CHUNK_BINS instantiations), bytes,
+// bytes scan, offsets, pack gate, one pack per choice of keys (enqueue_pack), frame, [index], finish.
 
 // The refusals of the asynchronous batch compress plans, in their order, with `item` naming what the batch holds ("file" or "array"):
 // the capacities, PagingSpec::Exact, the config, Auto specs, more than 256 unoptimized bins at the largest chunk, the CTA limit.  Fills
 // the config, its check and the chunk slots.
 static PcoB200Error acf_plan_checks(unsigned char dtype, const PcoB200ChunkConfig* config, size_t max_items, size_t nums_cap, size_t max_item_n,
                                     const std::string& item, PcoB200ChunkConfig* cfg_out, ConfigCheck* ck_out, uint64_t* max_chunks_out) {
-  PcoB200ChunkConfig cfg;
-  if (config) cfg = *config;
-  else {
-    std::memset(&cfg, 0, sizeof(cfg));  // pco::ChunkConfig::default(): level 8, Auto, Auto, EqualPagesUpTo(2^18)
-    cfg.compression_level = 8;
-  }
+  const PcoB200ChunkConfig cfg = default_chunk_config(config);
   if (max_items == 0 || max_items > 0x7fffffffu) return fail(PCO_B200_INVALID_ARGUMENT, "max_" + item + "s must be in 1 .. 2^31 - 1");
   if (max_item_n == 0) return fail(PCO_B200_INVALID_ARGUMENT, "max_" + item + "_n must be at least 1");
   if (uint64_t(nums_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "nums_cap must be at most 2^56");
@@ -3179,34 +3177,6 @@ static PcoB200Error acf_plan_checks(unsigned char dtype, const PcoB200ChunkConfi
   return PCO_B200_OK;
 }
 
-// The one-time device set-up of the asynchronous batch compress calls (compress_async_plan's, for their kernels), plus `extra`.
-static PcoB200Error acf_plan_setup(unsigned char dtype, std::initializer_list<const void*> extra) {
-  Context& c = ctx();
-  if (PcoB200Error e = ensure_device(c)) return e;
-  if (PcoB200Error e = load_kernels(extra)) return e;
-  if (PcoB200Error e = load_kernels({(const void*)acf_files_kernel, (const void*)acf_scan_kernel, (const void*)acf_place_kernel, (const void*)acf_init_kernel,
-                                     (const void*)acf_bytes_kernel, (const void*)acf_bytes_scan_kernel, (const void*)acf_offsets_kernel,
-                                     (const void*)acomp_two_gate_kernel, (const void*)acomp_var_gate_kernel,
-                                     (const void*)acomp_pack_gate_kernel, (const void*)segment_offsets_kernel, (const void*)fallback_kernel<false>,
-                                     (const void*)ans_encode_kernel<false>, (const void*)layout_kernel<false>})) return e;
-  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
-    using L = decltype(tag);
-    constexpr size_t RS_SMEM = size_t(RS_WARPS) * RS_BINS * sizeof(uint32_t);
-    const int count_smem = int(((size_t(1) << PLAN_MAX_COUNT_BITS) + 1) * 4 + 16);
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, count_smem));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(split_count_kernel<L, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(size_t(SC_N) * 4)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PackSmem)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(radix_sort_segments_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RS_SMEM));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true, false, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(bin_lut_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    return load_kernels({(const void*)split_count_kernel<L, true>, (const void*)split_delta_kernel<L, MODE_CLASSIC>, (const void*)split_delta_kernel<L, MODE_INT_MULT>,
-                         (const void*)split_delta_kernel<L, MODE_FLOAT_QUANT>, (const void*)split_delta_kernel<L, MODE_FLOAT_MULT>,
-                         (const void*)plan_probe_kernel<L, false, false, true>, (const void*)sort_keys_kernel<L>, (const void*)plan_solve_kernel<L, true>,
-                         (const void*)bin_kernel<L, false>});
-  });
-}
-
 PcoB200Error pco_b200_compress_files_async_plan(unsigned char dtype, const PcoB200ChunkConfig* config, int uniform_type_header, size_t max_files,
                                                 size_t nums_cap, size_t max_file_n, size_t dst_cap, size_t index_cap,
                                                 PcoB200AsyncCompressFilesPlan* plan) {
@@ -3219,11 +3189,8 @@ PcoB200Error pco_b200_compress_files_async_plan(unsigned char dtype, const PcoB2
   std::memset(plan, 0, sizeof(*plan));
   plan->dtype = dtype;
   plan->uniform_type_header = uniform_type_header ? 1 : 0;
-  plan->mode = ck.explicit_mode.mode;
-  plan->order = ck.explicit_order;
-  plan->n_vars = ck.explicit_mode.mode == MODE_CLASSIC ? 1 : 2;
+  fill_explicit_spec(plan, ck);
   plan->level = cfg.compression_level;
-  plan->mode_k = ck.explicit_mode.mode_k;
   plan->max_files = max_files;
   plan->nums_cap = nums_cap;
   plan->max_file_n = max_file_n;
@@ -3231,17 +3198,15 @@ PcoB200Error pco_b200_compress_files_async_plan(unsigned char dtype, const PcoB2
   plan->max_chunks = max_chunks;
   plan->dst_cap = dst_cap;
   plan->index_cap = index_cap;
-  plan->mode_base = ck.explicit_mode.mode_base;
-  plan->base_bits = ck.explicit_mode.base_bits;
-  plan->inv_base_bits = ck.explicit_mode.inv_base_bits;
   const uint64_t lbits = nt_bits(dtype);
   plan->dst_bound = uint64_t(max_files) * (standalone_header_size() + 1) + max_chunks * (5 + baseline_chunk_meta_size(uint32_t(lbits))) +
                     (uint64_t(nums_cap) * lbits + 7) / 8;
   plan->index_bound = uint64_t(max_files) * sizeof(IndexHeader) + max_chunks * (sizeof(IndexChunk) + plan->n_vars * sizeof(BatchEntry) + 15) +
                       plan->n_vars * sizeof(BatchEntry) * ((uint64_t(nums_cap) + BATCH_N - 1) / BATCH_N);
   plan->workspace_bytes = acf_plan_geom(*plan).l.total;
-  // the one-time device set-up (compress_async_plan's, for this call's kernels)
-  return acf_plan_setup(dtype, {(const void*)acf_frame_kernel, (const void*)acf_index_kernel, (const void*)acf_finish_kernel});
+  return async_encode_setup<true>(dtype, {(const void*)acf_files_kernel, (const void*)acf_scan_kernel, (const void*)acf_place_kernel, (const void*)acf_init_kernel,
+                                          (const void*)acf_bytes_kernel, (const void*)acf_bytes_scan_kernel, (const void*)acf_offsets_kernel,
+                                          (const void*)acf_frame_kernel, (const void*)acf_index_kernel, (const void*)acf_finish_kernel});
 }
 
 // What the launches of a batch compress take by value (framed: 1 for standalone files, 0 for bare chunks)
@@ -3299,7 +3264,7 @@ size_t pco_b200_debug_standalone_header(uint64_t n_hint, unsigned char uniform_t
 
 PcoB200Error pco_b200_compress_files_async_result(const PcoB200AsyncCompressFilesStatus* s, size_t* dst_len, size_t* index_len) {
   if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
-  const PcoB200Error kind = s->kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(s->kind) : PCO_B200_CORRUPTION;
+  const PcoB200Error kind = async_result_kind(s->kind);
   if (kind == PCO_B200_OK) {
     if (dst_len) *dst_len = size_t(s->dst_written);
     if (index_len) *index_len = size_t(s->index_written);
@@ -3332,11 +3297,8 @@ PcoB200Error pco_b200_compress_wrapped_async_plan(unsigned char dtype, const Pco
   if (PcoB200Error e = acf_plan_checks(dtype, config, max_arrays, nums_cap, max_array_n, "array", &cfg, &ck, &max_chunks)) return e;
   std::memset(plan, 0, sizeof(*plan));
   plan->dtype = dtype;
-  plan->mode = ck.explicit_mode.mode;
-  plan->order = ck.explicit_order;
-  plan->n_vars = ck.explicit_mode.mode == MODE_CLASSIC ? 1 : 2;
+  fill_explicit_spec(plan, ck);
   plan->level = cfg.compression_level;
-  plan->mode_k = ck.explicit_mode.mode_k;
   plan->max_arrays = max_arrays;
   plan->nums_cap = nums_cap;
   plan->max_array_n = max_array_n;
@@ -3344,9 +3306,6 @@ PcoB200Error pco_b200_compress_wrapped_async_plan(unsigned char dtype, const Pco
   plan->max_chunks = max_chunks;
   plan->metas_cap = metas_cap;
   plan->pages_cap = pages_cap;
-  plan->mode_base = ck.explicit_mode.mode_base;
-  plan->base_bits = ck.explicit_mode.base_bits;
-  plan->inv_base_bits = ck.explicit_mode.inv_base_bits;
   // the bounds the header comment derives
   const uint64_t lbits = nt_bits(dtype), obb = offset_bits_bits(uint32_t(lbits));
   const uint64_t mode_bits = plan->mode == MODE_CLASSIC ? 0 : plan->mode == MODE_FLOAT_QUANT ? 8 : lbits;
@@ -3354,8 +3313,10 @@ PcoB200Error pco_b200_compress_wrapped_async_plan(unsigned char dtype, const Pco
   plan->pages_bound = max_chunks * (1 + baseline_chunk_meta_size(uint32_t(lbits))) + (uint64_t(nums_cap) * lbits + 7) / 8;
   plan->metas_bound = std::min<uint64_t>(max_chunks * meta_max, plan->pages_bound);
   plan->workspace_bytes = acw_plan_geom(*plan).l.total;
-  return acf_plan_setup(dtype, {(const void*)acw_lens_kernel, (const void*)acw_scan_kernel, (const void*)acw_refs_kernel, (const void*)acw_split_kernel,
-                                (const void*)acw_finish_kernel});
+  return async_encode_setup<true>(dtype, {(const void*)acf_files_kernel, (const void*)acf_scan_kernel, (const void*)acf_place_kernel, (const void*)acf_init_kernel,
+                                          (const void*)acf_bytes_kernel, (const void*)acf_bytes_scan_kernel, (const void*)acf_offsets_kernel,
+                                          (const void*)acw_lens_kernel, (const void*)acw_scan_kernel, (const void*)acw_refs_kernel,
+                                          (const void*)acw_split_kernel, (const void*)acw_finish_kernel});
 }
 
 PcoB200Error pco_b200_compress_wrapped_async(const PcoB200AsyncCompressWrappedPlan* plan, const void* nums, const uint64_t* array_ns,
@@ -3393,7 +3354,7 @@ PcoB200Error pco_b200_compress_wrapped_async(const PcoB200AsyncCompressWrappedPl
 
 PcoB200Error pco_b200_compress_wrapped_async_result(const PcoB200AsyncCompressWrappedStatus* s, size_t* metas_len, size_t* pages_len, size_t* n_chunks) {
   if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
-  const PcoB200Error kind = s->kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(s->kind) : PCO_B200_CORRUPTION;
+  const PcoB200Error kind = async_result_kind(s->kind);
   if (kind == PCO_B200_OK) {
     if (metas_len) *metas_len = size_t(s->metas_written);
     if (pages_len) *pages_len = size_t(s->pages_written);
