@@ -32,6 +32,32 @@ struct pco_oracle_config {
   uint32_t reserved;
 };
 
+// One latent variable of a chunk written by pco_oracle_write_explicit_file: the bins as the chunk meta lists them, and the stored
+// latents as (bin index, offset) pairs.  `moments` holds the delta state (`delta_order` latents) when the var uses the delta.
+struct pco_oracle_explicit_var {
+  uint32_t ans_size_log;
+  uint32_t n_bins;
+  const uint32_t* weights;
+  const uint64_t* lowers;
+  const uint32_t* offset_bits;
+  uint64_t n_stored;
+  const uint32_t* symbols;
+  const uint64_t* offsets;
+  const uint64_t* moments;
+};
+
+// One chunk: mode (ModeKind: 0 Classic, 1 IntMult, 2 FloatMult, 3 FloatQuant) with its parameter (IntMult base, FloatMult base as
+// latent-ordered bits, FloatQuant k), consecutive delta of `delta_order` (0 = NoOp), and the primary and secondary vars.
+struct pco_oracle_explicit_chunk {
+  uint64_t n;
+  uint32_t mode;
+  uint32_t float_quant_k;
+  uint64_t mode_base_latent;
+  uint32_t delta_order;
+  uint32_t secondary_uses_delta;
+  pco_oracle_explicit_var vars[2];
+};
+
 }  // extern "C"
 
 static thread_local std::string g_last_error;
@@ -112,7 +138,151 @@ static void with_cc(void* handle, Fn&& fn) {
   }
 }
 
+// ----- explicit streams: a chunk built from given bins and (bin, offset) pairs ----------------------------------------------------
+// The chunk meta of an explicit chunk, checked against everything the format's reader requires (metadata/chunk_latent_var.rs:102-157,
+// mode validity, delta order); anything else is a valid stream, so whatever passes decodes.
+static ChunkMeta explicit_chunk_meta(uint8_t dtype, const pco_oracle_explicit_chunk& c) {
+  if (!number_type_valid(dtype)) invalid_argument("unknown number type byte");
+  const Bitlen bits = number_type_bits(dtype);
+  if (c.n == 0 || c.n > MAX_ENTRIES) invalid_argument("chunk count must be in 1..2^24");
+  if (c.mode > uint32_t(ModeKind::FloatQuant)) invalid_argument("mode must be Classic, IntMult, FloatMult or FloatQuant");
+  if (c.delta_order > MAX_CONSECUTIVE_DELTA_ORDER) invalid_argument("consecutive delta order exceeds 7");
+  ChunkMeta m;
+  m.number_bits = bits;
+  m.mode.kind = ModeKind(c.mode);
+  m.mode.base_latent = bits == 64 ? c.mode_base_latent : c.mode_base_latent & ((uint64_t(1) << bits) - 1);
+  if (c.mode_base_latent != m.mode.base_latent) invalid_argument("mode base exceeds the number type");
+  m.mode.k = c.float_quant_k;
+  if (!mode_is_valid(m.mode, dtype)) invalid_argument("mode or mode parameter invalid for the number type");
+  if (c.delta_order) {
+    m.delta.kind = DeltaKind::Consecutive;
+    m.delta.order = c.delta_order;
+    m.delta.secondary_uses_delta = c.secondary_uses_delta != 0;
+  } else if (c.secondary_uses_delta) {
+    invalid_argument("secondary_uses_delta without a delta encoding");
+  }
+  m.has_secondary = mode_has_secondary(m.mode);
+  for (int v = 0; v < (m.has_secondary ? 2 : 1); v++) {
+    const pco_oracle_explicit_var& s = c.vars[v];
+    LatentVarMeta& vm = v == 0 ? m.primary : m.secondary;
+    vm.latent_bits = bits;
+    vm.ans_size_log = s.ans_size_log;
+    if (s.ans_size_log > MAX_ANS_BITS) invalid_argument("ans_size_log exceeds 14");
+    if (s.n_bins > (uint64_t(1) << s.ans_size_log)) invalid_argument("more bins than tANS states");
+    if (s.n_bins == 1 && s.ans_size_log > 0) invalid_argument("one bin with ans_size_log > 0");
+    uint64_t total = 0;
+    for (uint32_t i = 0; i < s.n_bins; i++) {
+      if (s.weights[i] == 0) invalid_argument("bin weight 0");
+      if (s.offset_bits[i] > bits) invalid_argument("offset_bits exceeds the latent type");
+      if (bits < 64 && s.lowers[i] >> bits) invalid_argument("bin lower exceeds the latent type");
+      total += s.weights[i];
+      vm.bins.push_back(Bin{s.weights[i], s.lowers[i], s.offset_bits[i]});
+    }
+    if (s.n_bins > 0 && total != (uint64_t(1) << s.ans_size_log)) invalid_argument("weights do not sum to 2^ans_size_log");
+    const size_t n_state = delta_for_latent_var(m.delta, v == 0 ? VarKey::Primary : VarKey::Secondary).n_latents_per_state();
+    if (s.n_stored != (c.n > n_state ? c.n - n_state : 0)) invalid_argument("stored count must be n minus the var's delta order");
+    if (s.n_stored > 0 && s.n_bins == 0) invalid_argument("stored latents without bins");
+    for (uint64_t i = 0; i < s.n_stored; i++) {
+      if (s.symbols[i] >= s.n_bins) invalid_argument("symbol is not a bin");
+      if (s.offset_bits[s.symbols[i]] < 64 && s.offsets[i] >> s.offset_bits[s.symbols[i]]) invalid_argument("offset does not fit its bin's offset_bits");
+    }
+    for (size_t i = 0; i < n_state; i++)
+      if (bits < 64 && s.moments[i] >> bits) invalid_argument("moment exceeds the latent type");
+  }
+  return m;
+}
+
+// The page of an explicit chunk (chunk_compressor.rs:624-705): the interleaved tANS states come from encoding each var's symbols in
+// reverse, batch by batch, as the compressor does; the page meta holds the moments and the final states.
+static void write_explicit_page(const ChunkMeta& m, const pco_oracle_explicit_chunk& c, std::vector<uint8_t>& dst) {
+  struct Var {
+    const pco_oracle_explicit_var* s;
+    Bitlen size_log;
+    std::vector<AnsState> vals;
+    std::vector<Bitlen> nbits;
+    AnsState finals[ANS_INTERLEAVING];
+  };
+  std::vector<Var> vars;
+  for (int v = 0; v < (m.has_secondary ? 2 : 1); v++) {
+    const pco_oracle_explicit_var& s = c.vars[v];
+    Var x{&s, s.ans_size_log, std::vector<AnsState>(s.n_stored), std::vector<Bitlen>(s.n_stored, 0), {}};
+    const AnsState table = AnsState(1) << s.ans_size_log;
+    for (size_t j = 0; j < ANS_INTERLEAVING; j++) x.finals[j] = table;
+    if (s.n_bins > 1) {
+      AnsEncoder enc(ans_spec_from_weights(s.ans_size_log, std::vector<Weight>(s.weights, s.weights + s.n_bins)));
+      const size_t n_batches = (s.n_stored + FULL_BATCH_N - 1) / FULL_BATCH_N;
+      for (size_t b = n_batches; b-- > 0;) {
+        const size_t start = b * FULL_BATCH_N, end = std::min<size_t>(start + FULL_BATCH_N, s.n_stored);
+        for (size_t i = end; i-- > start;) {
+          AnsState& st = x.finals[(i - start) % ANS_INTERLEAVING];
+          Bitlen nb;
+          const AnsState ns = enc.encode(st, s.symbols[i], &nb);
+          x.vals[i] = AnsState(lowest_bits_u64(st, nb));
+          x.nbits[i] = nb;
+          st = ns;
+        }
+      }
+    }
+    vars.push_back(std::move(x));
+  }
+  BitWriter w(dst);
+  for (size_t v = 0; v < vars.size(); v++) {
+    const LatentVarMeta& vm = v == 0 ? m.primary : m.secondary;
+    const size_t n_state = delta_for_latent_var(m.delta, v == 0 ? VarKey::Primary : VarKey::Secondary).n_latents_per_state();
+    for (size_t i = 0; i < n_state; i++) w.write_uint(vars[v].s->moments[i], vm.latent_bits);
+    for (size_t j = 0; j < ANS_INTERLEAVING; j++) w.write_uint(vars[v].finals[j] - (AnsState(1) << vars[v].size_log), vm.ans_size_log);
+  }
+  w.finish_byte();
+  for (uint64_t start = 0; start < c.n; start += FULL_BATCH_N) {
+    for (const Var& x : vars) {
+      const pco_oracle_explicit_var& s = *x.s;
+      const uint64_t end = std::min<uint64_t>(start + FULL_BATCH_N, s.n_stored);
+      if (s.n_bins > 1)
+        for (uint64_t i = start; i < end; i++) w.write_uint(x.vals[i], x.nbits[i]);
+      for (uint64_t i = start; i < end; i++) w.write_uint(s.offsets[i], s.offset_bits[s.symbols[i]]);
+    }
+  }
+  w.finish();
+}
+
 extern "C" {
+
+// A standalone file (header, each chunk's type byte, count, meta and page, terminator) of chunks with explicit bins and stored latents.
+// `metas` / `pages`, when not null, receive each chunk's wrapped meta and page bytes back to back, with their lengths in
+// meta_lens / page_lens (n_chunks entries each).  An invalid spec is InvalidArgument.
+int pco_oracle_write_explicit_file(uint8_t dtype, const pco_oracle_explicit_chunk* chunks, size_t n_chunks, uint8_t** out, size_t* out_len,
+                                   uint8_t** metas, size_t* meta_lens, uint8_t** pages, size_t* page_lens) {
+  return guarded([&] {
+    uint64_t total = 0;
+    std::vector<ChunkMeta> cms;
+    for (size_t i = 0; i < n_chunks; i++) {
+      cms.push_back(explicit_chunk_meta(dtype, chunks[i]));
+      total += chunks[i].n;
+    }
+    std::vector<uint8_t> dst, all_metas, all_pages;
+    write_standalone_header(dst, total, 0);
+    for (size_t i = 0; i < n_chunks; i++) {
+      BitWriter w(dst);
+      w.write_aligned_bytes(&dtype, 1);
+      w.write_uint(chunks[i].n - 1, BITS_TO_ENCODE_N_ENTRIES);
+      w.finish();
+      std::vector<uint8_t> meta, page;
+      write_chunk_meta(cms[i], meta);
+      write_explicit_page(cms[i], chunks[i], page);
+      dst.insert(dst.end(), meta.begin(), meta.end());
+      dst.insert(dst.end(), page.begin(), page.end());
+      all_metas.insert(all_metas.end(), meta.begin(), meta.end());
+      all_pages.insert(all_pages.end(), page.begin(), page.end());
+      if (meta_lens) meta_lens[i] = meta.size();
+      if (page_lens) page_lens[i] = page.size();
+    }
+    dst.push_back(MAGIC_TERMINATION_BYTE);
+    size_t unused;
+    if (metas) *metas = dup_bytes(all_metas, &unused);
+    if (pages) *pages = dup_bytes(all_pages, &unused);
+    *out = dup_bytes(dst, out_len);
+  });
+}
 
 const char* pco_oracle_last_error() { return g_last_error.c_str(); }
 void pco_oracle_free(void* p) { std::free(p); }

@@ -226,6 +226,65 @@ def wrapped_decompress_page(meta, page, dtype, page_n):
     return dst, mc.value, pc.value
 
 
+class _ExplicitVar(C.Structure):  # pco_oracle_explicit_var (c_api.cpp)
+    _fields_ = [("ans_size_log", C.c_uint32), ("n_bins", C.c_uint32), ("weights", C.c_void_p), ("lowers", C.c_void_p), ("offset_bits", C.c_void_p),
+                ("n_stored", C.c_uint64), ("symbols", C.c_void_p), ("offsets", C.c_void_p), ("moments", C.c_void_p)]
+
+
+class _ExplicitChunk(C.Structure):  # pco_oracle_explicit_chunk (c_api.cpp)
+    _fields_ = [("n", C.c_uint64), ("mode", C.c_uint32), ("float_quant_k", C.c_uint32), ("mode_base_latent", C.c_uint64), ("delta_order", C.c_uint32),
+                ("secondary_uses_delta", C.c_uint32), ("vars", _ExplicitVar * 2)]
+
+
+EXPLICIT_MODES = {"classic": 0, "int_mult": 1, "float_mult": 2, "float_quant": 3}
+
+
+def write_explicit_file(dtype, chunks):
+    """A standalone file of chunks with explicit bins and stored latents (pco_oracle_write_explicit_file).  Each chunk is a dict:
+    n; mode ("classic", "int_mult", "float_mult", "float_quant") with `base` (IntMult base, or FloatMult base as latent-ordered bits)
+    or `k`; `order` (consecutive delta, 0 = none) and `secondary_uses_delta`; `vars`: one dict per latent var (primary, then secondary)
+    with ans_size_log, bins [(weight, lower, offset_bits), ...], symbols and offsets (the stored latents), and moments (the delta
+    state) when the var uses the delta.  Returns (file, [(meta, page) per chunk])."""
+    dt = NP_TO_BYTE[np.dtype(dtype)]
+    arr = (_ExplicitChunk * max(len(chunks), 1))()
+    keep = []
+
+    def buf(values, ctype):
+        a = np.ascontiguousarray(np.asarray(values, dtype=np.uint64).astype(ctype).reshape(-1))
+        keep.append(a)
+        return a.ctypes.data_as(C.c_void_p) if a.size else None
+
+    for c, spec in zip(arr, chunks):
+        c.n = spec["n"]
+        c.mode = EXPLICIT_MODES[spec.get("mode", "classic")]
+        c.mode_base_latent = spec.get("base", 0)
+        c.float_quant_k = spec.get("k", 0)
+        c.delta_order = spec.get("order", 0)
+        c.secondary_uses_delta = 1 if spec.get("secondary_uses_delta") else 0
+        for v, var in zip(c.vars, spec["vars"]):
+            bins = np.asarray(var["bins"], dtype=np.uint64).reshape(-1, 3)
+            v.ans_size_log = var["ans_size_log"]
+            v.n_bins = bins.shape[0]
+            v.weights, v.lowers, v.offset_bits = buf(bins[:, 0], np.uint32), buf(bins[:, 1], np.uint64), buf(bins[:, 2], np.uint32)
+            v.n_stored = len(var["symbols"])
+            v.symbols, v.offsets = buf(var["symbols"], np.uint32), buf(var["offsets"], np.uint64)
+            v.moments = buf(var.get("moments", []), np.uint64)
+    out, n = C.c_void_p(), C.c_size_t()
+    metas, pages = C.c_void_p(), C.c_void_p()
+    mlens, plens = (C.c_size_t * max(len(chunks), 1))(), (C.c_size_t * max(len(chunks), 1))()
+    f = lib().pco_oracle_write_explicit_file
+    f.argtypes = [C.c_uint8, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    _check(f(dt, C.cast(arr, C.c_void_p), len(chunks), C.byref(out), C.byref(n), C.byref(metas), mlens, C.byref(pages), plens))
+    data = _take_bytes(out, n)
+    mall = _take_bytes(metas, C.c_size_t(sum(mlens[:len(chunks)])))
+    pall = _take_bytes(pages, C.c_size_t(sum(plens[:len(chunks)])))
+    parts, mo, po = [], 0, 0
+    for i in range(len(chunks)):
+        parts.append((mall[mo:mo + mlens[i]], pall[po:po + plens[i]]))
+        mo, po = mo + mlens[i], po + plens[i]
+    return data, parts
+
+
 def bench_roundtrip(nums, n_chunks, chunk_n, config, threads):
     """Compress + decompress `n_chunks` chunks of `chunk_n` numbers (contiguous in `nums`) on `threads` native threads, one chunk
     per task, verifying the round trip.  Returns (compress seconds, decompress seconds, compressed bytes).  bench.py's CPU arm."""
