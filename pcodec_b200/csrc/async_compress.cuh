@@ -20,34 +20,23 @@ namespace pcob200 {
 constexpr int ACOMP_THREADS = 256;
 constexpr uint32_t ACOMP_GATES_PER_VAR = 4;  // counting probe, sort path, bin_lut_kernel, bin_kernel
 
-// Chunk geometry of a plan (n_per_page's EqualPagesUpTo in closed form)
+// Chunk geometry of a plan: its EqualPages chunks, the largest chunk's size and the latent slots
 struct AcompGeom {
   uint64_t n, n_chunks, low, rem, max_n, slots;
   uint32_t bpc, tiles;
 };
-__host__ __device__ inline uint64_t acomp_rows_of(uint64_t size) { return (size + BATCH_N - 1) / BATCH_N * BATCH_N; }
 inline AcompGeom acomp_geom(uint64_t n, uint64_t max_page_n) {
+  const EqualPages ep = equal_pages(n, max_page_n);
   AcompGeom g = {};
   g.n = n;
-  if (n == 0) return g;
-  const uint64_t mp = max_page_n == 0 ? (uint64_t(1) << 18) : max_page_n;
-  g.n_chunks = (n + mp - 1) / mp;
-  g.low = n / g.n_chunks;
-  g.rem = n % g.n_chunks;
-  g.max_n = g.low + (g.rem ? 1 : 0);
-  g.slots = g.rem * acomp_rows_of(g.low + 1) + (g.n_chunks - g.rem) * acomp_rows_of(g.low);
+  g.n_chunks = ep.n_chunks;
+  g.low = ep.low;
+  g.rem = ep.rem;
+  g.max_n = ep.size(0);
+  g.slots = ep.row_start(ep.n_chunks);
   g.bpc = n_batches_of(uint32_t(g.max_n));
   g.tiles = uint32_t((g.max_n + SPLIT_TILE - 1) / SPLIT_TILE);
   return g;
-}
-__host__ __device__ inline uint64_t acomp_entries_bytes(uint32_t n_vars, uint64_t size) {
-  return (uint64_t(n_vars) * n_batches_of(uint32_t(size)) * sizeof(BatchEntry) + 15) & ~uint64_t(15);
-}
-// byte size of the side index compress_typed writes for this layout
-inline uint64_t acomp_index_bytes(const AcompGeom& g, uint32_t n_vars) {
-  if (g.n == 0) return sizeof(IndexHeader);
-  return ((sizeof(IndexHeader) + g.n_chunks * sizeof(IndexChunk) + 15) & ~uint64_t(15)) + g.rem * acomp_entries_bytes(n_vars, g.low + 1) +
-         (g.n_chunks - g.rem) * acomp_entries_bytes(n_vars, g.low);
 }
 
 // Workspace of one in-flight call, byte offsets of 256-byte aligned regions.  head: split_count_kernel's flags (2 words), the range bits
@@ -106,15 +95,8 @@ struct AcompHead {
   uint64_t total;         // file bytes (chunk_offsets_kernel)
 };
 __device__ inline uint64_t* acomp_gate(const AcompArgs& a, uint32_t g) { return reinterpret_cast<uint64_t*>(a.ws + a.lay.gates) + uint64_t(g) * (a.n_chunks + 1); }
-__device__ inline uint64_t acomp_start(const AcompArgs& a, uint64_t c) { return c * a.low + (c < a.rem ? c : a.rem); }
 // the chunk starts the init kernel wrote (acomp_init_kernel, or acf_init_kernel for a batch of files): the gates copy them
 __device__ inline const uint64_t* acomp_starts(const AcompArgs& a) { return reinterpret_cast<const uint64_t*>(a.ws + a.lay.starts); }
-__device__ inline void acomp_reset_chunk(ChunkEnc* ch) {  // init_chunks_kernel's record
-  ChunkEnc z;
-  memset(&z, 0, sizeof(z));
-  z.vmin[0] = z.vmin[1] = ~uint64_t(0);
-  *ch = z;
-}
 
 // Grid-stride over every per-chunk and per-word job: ChunkEnc records, chunk starts and row bases, index entry offsets, the zeroed
 // offset-bit sums (fallback chunks leave their secondary var's untouched) and the zeroed index body; thread 0 writes the head, the
@@ -126,20 +108,17 @@ __global__ void __launch_bounds__(ACOMP_THREADS) acomp_init_kernel(AcompArgs a, 
   uint64_t* rows = reinterpret_cast<uint64_t*>(a.ws + a.lay.rows);
   uint64_t* eoff = reinterpret_cast<uint64_t*>(a.ws + a.lay.eoff);
   uint32_t* ob_sum = reinterpret_cast<uint32_t*>(a.ws + a.lay.ob_sum);
-  const uint64_t r1 = acomp_rows_of(a.low + 1), r0 = acomp_rows_of(a.low);
-  const uint64_t e1 = acomp_entries_bytes(a.n_vars, a.low + 1), e0 = acomp_entries_bytes(a.n_vars, a.low);
-  const uint64_t ebase = (sizeof(IndexHeader) + nc * sizeof(IndexChunk) + 15) & ~uint64_t(15);
+  const EqualPages ep = {nc, a.low, a.rem};
   const uint64_t n_sums = nc * MAX_VARS * bpc;
   const uint64_t idx_vecs = a.index_bytes > sizeof(IndexHeader) ? (a.index_bytes - sizeof(IndexHeader)) / 16 : 0;
   const uint64_t jobs = max(max(nc + 1, n_sums), idx_vecs);
   for (uint64_t t = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; t < jobs; t += uint64_t(gridDim.x) * blockDim.x) {
     if (t <= nc) {
-      const uint64_t k = t < a.rem ? t : a.rem;
-      starts[t] = acomp_start(a, t);
-      rows[t] = k * r1 + (t - k) * r0;
+      starts[t] = ep.start(t);
+      rows[t] = ep.row_start(t);
       if (t < nc) {
-        acomp_reset_chunk(&chunks[t]);
-        eoff[t] = ebase + k * e1 + (t - k) * e0;
+        reset_chunk_enc(&chunks[t]);
+        eoff[t] = ep.entries_offset(a.n_vars, t);
       }
     }
     if (t < n_sums) ob_sum[t] = 0;
@@ -178,7 +157,7 @@ __global__ void __launch_bounds__(ACOMP_THREADS) acomp_two_gate_kernel(AcompArgs
   const uint64_t* starts = acomp_starts(a);
   for (uint64_t c = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; c <= a.n_chunks; c += uint64_t(gridDim.x) * blockDim.x) {
     g[c] = two ? starts[c] : 0;
-    if (two && c < a.n_chunks) acomp_reset_chunk(&chunks[c]);
+    if (two && c < a.n_chunks) reset_chunk_enc(&chunks[c]);
   }
 }
 
@@ -257,7 +236,7 @@ inline PcoB200Error acomp_check_plan(const PcoB200AsyncCompressPlan* p, AcompGeo
     return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_compress_async_plan");
   *g = acomp_geom(p->n, p->max_page_n);
   *lay = acomp_layout(*g, nt_bits(p->dtype) / 8, p->n_vars);
-  if (p->workspace_bytes != lay->total || p->index_bytes != acomp_index_bytes(*g, p->n_vars))
+  if (p->workspace_bytes != lay->total || p->index_bytes != equal_pages(p->n, p->max_page_n).index_bytes(p->n_vars))
     return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_compress_async_plan");
   return PCO_B200_OK;
 }
@@ -306,26 +285,14 @@ AcompRegions<L> acomp_regions(const AcompArgs& a) {
 }
 
 // The EncParams of the encode stage: the spec fields of the plan (P: a compress_async or compress_files_async plan), the chunks of g,
-// the starts and row bases the init kernel wrote, and the caller's n_total and unoptimized_bins_log per var.
+// the starts and row bases the init kernel wrote, and the caller's n_total and unoptimized_bins_log (or level, for CHUNK_BINS).
 template <typename P>
-EncParams acomp_enc_params(const P& p, const AcompGeom& g, const AcompArgs& a, const void* nums, uint64_t n_total, uint32_t bins_log0,
-                           uint32_t bins_log1) {
-  EncParams ep;
-  std::memset(&ep, 0, sizeof(ep));
-  ep.dtype = p.dtype;
-  ep.uniform_type = p.uniform_type_header ? p.dtype : 0;
-  ep.mode = p.mode;
-  ep.mode_base = p.mode_base;
-  ep.base_bits = p.base_bits;
-  ep.inv_base_bits = p.inv_base_bits;
-  ep.mode_k = p.mode_k;
-  ep.order = p.order;
-  ep.n_vars = p.n_vars;
+EncParams acomp_enc_params(const P& p, const AcompGeom& g, const AcompArgs& a, const void* nums, uint64_t n_total, uint32_t bins_log) {
+  EncParams ep = enc_params(p.dtype, p.uniform_type_header ? p.dtype : 0, ModeSel{p.mode, p.mode_base, p.base_bits, p.inv_base_bits, p.mode_k}, p.order,
+                            bins_log);
   ep.n_total = n_total;
   ep.n_chunks = uint32_t(g.n_chunks);
   ep.max_chunk_n = uint32_t(g.max_n);
-  ep.bins_log[0] = bins_log0;
-  ep.bins_log[1] = bins_log1;
   ep.nums = nums;
   ep.chunk_starts = reinterpret_cast<const uint64_t*>(a.ws + a.lay.starts);
   ep.row_base = reinterpret_cast<const uint64_t*>(a.ws + a.lay.rows);
@@ -433,8 +400,7 @@ void acomp_launch(const PcoB200AsyncCompressPlan& p, const AcompGeom& g, const A
   acomp_init_kernel<<<init_ctas, ACOMP_THREADS, 0, stream>>>(a, g.bpc);
   ln.end();
   if (p.n > 0) {
-    // the secondary var takes at most LIMITED_UNOPTIMIZED_BINS_LOG (chunk_compressor.rs:238-248)
-    const EncParams ep = acomp_enc_params(p, g, a, nums, p.n, p.bins_log, std::min<uint32_t>(p.bins_log, 6));
+    const EncParams ep = acomp_enc_params(p, g, a, nums, p.n, p.bins_log);
     const AcompRegions<L> r = acomp_regions<L>(a);
     enqueue_encode_kernels<L, false>(g, a, ep, ln);
     chunk_offsets_kernel<<<1, 1024, 0, stream>>>(r.chunks, nc, a.header_bytes, 1u, &r.head->total);

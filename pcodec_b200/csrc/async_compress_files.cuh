@@ -34,31 +34,6 @@ constexpr int ACF_SCAN_THREADS = 1024;  // the one-CTA launches
 constexpr int ACF_INDEX_THREADS = 128;
 enum { ACF_NUMS = 0, ACF_CHUNKS, ACF_ROWS, ACF_FRAME, ACF_IDX, ACF_SUMS };
 
-// standalone_header_into's length for a size hint of n
-__host__ __device__ inline uint32_t standalone_header_len(uint64_t n) {
-  uint32_t power = 1;
-  while (power < 64 && (n >> power) != 0) power++;
-  return 8 + (6 + power + 7) / 8;
-}
-
-// One file's chunks (n_per_page's EqualPagesUpTo in closed form) and the sizes that depend on its count only
-struct AcfGeom {
-  uint64_t k, low, rem, rows, idx;
-};
-__host__ __device__ inline AcfGeom acf_geom(uint64_t n, uint64_t mp, uint32_t n_vars) {
-  AcfGeom g = {};
-  if (n == 0) {
-    g.idx = sizeof(IndexHeader);
-    return g;
-  }
-  g.k = (n + mp - 1) / mp;
-  g.low = n / g.k;
-  g.rem = n % g.k;
-  g.rows = g.rem * acomp_rows_of(g.low + 1) + (g.k - g.rem) * acomp_rows_of(g.low);
-  g.idx = sizeof(IndexHeader) + g.k * sizeof(IndexChunk) + g.rem * acomp_entries_bytes(n_vars, g.low + 1) + (g.k - g.rem) * acomp_entries_bytes(n_vars, g.low);
-  return g;
-}
-
 struct AcfPart {  // per CTA of acf_files_kernel: the CTA's sums, then (acf_scan_kernel) the sums of the CTAs before it
   ArSum s[ACF_SUMS];
 };
@@ -130,12 +105,12 @@ __device__ __forceinline__ AcfPart* acf_parts(const AcfArgs& g) { return reinter
 __device__ __forceinline__ void acf_file_sums(const AcfArgs& g, uint64_t f, uint64_t nf, ArSum* s, uint64_t* n_out) {
   const uint64_t n = f < nf ? g.file_ns[f] : 0;
   const uint64_t nn = min(n, g.max_file_n);
-  const AcfGeom fg = acf_geom(nn, g.max_page_n, g.a.n_vars);
+  const EqualPages fp = equal_pages(nn, g.max_page_n);
   s[ACF_NUMS] = ar_sum(n);
-  s[ACF_CHUNKS] = ar_sum(fg.k);
-  s[ACF_ROWS] = ar_sum(fg.rows);
+  s[ACF_CHUNKS] = ar_sum(fp.n_chunks);
+  s[ACF_ROWS] = ar_sum(fp.row_start(fp.n_chunks));
   s[ACF_FRAME] = ar_sum(f < nf && g.framed ? standalone_header_len(nn) + 1 : 0);
-  s[ACF_IDX] = ar_sum(f < nf ? fg.idx : 0);
+  s[ACF_IDX] = ar_sum(f < nf ? fp.index_bytes(g.a.n_vars) : 0);
   *n_out = n;
 }
 __device__ __forceinline__ uint64_t acf_n_files(const AcfArgs& g) {
@@ -239,17 +214,17 @@ __global__ void __launch_bounds__(ACF_THREADS) acf_init_kernel(AcfArgs g) {
           else hi = m;
         }
         const AcfFile& f = fl[lo];
-        const AcfGeom fg = acf_geom(f.n, g.max_page_n, g.a.n_vars);
-        const uint64_t j = t - f.first[ACF_CHUNKS], q = j < fg.rem ? j : fg.rem;
-        s = f.first[ACF_NUMS] + j * fg.low + q;
-        r = f.first[ACF_ROWS] + q * acomp_rows_of(fg.low + 1) + (j - q) * acomp_rows_of(fg.low);
+        const EqualPages fp = equal_pages(f.n, g.max_page_n);
+        const uint64_t j = t - f.first[ACF_CHUNKS];
+        s = f.first[ACF_NUMS] + fp.start(j);
+        r = f.first[ACF_ROWS] + fp.row_start(j);
         file = uint32_t(lo);
       }
       starts[t] = s;
       rows[t] = r;
       if (t < nc) {
         cfile[t] = file;
-        acomp_reset_chunk(&chunks[t]);
+        reset_chunk_enc(&chunks[t]);
       }
     }
     if (t < n_sums) ob_sum[t] = 0;
@@ -327,10 +302,11 @@ __global__ void __launch_bounds__(ACF_THREADS) acf_frame_kernel(AcfArgs g) {
   if (f >= st->n_files) return;
   const AcfFile r = acf_files(g)[f];
   const uint64_t* pre = reinterpret_cast<const uint64_t*>(g.a.ws + g.l.pre);
-  const uint64_t c0 = r.first[ACF_CHUNKS], k = acf_geom(r.n, g.max_page_n, g.a.n_vars).k;
+  const EqualPages fp = equal_pages(r.n, g.max_page_n);
+  const uint64_t c0 = r.first[ACF_CHUNKS], k = fp.n_chunks;
   const uint64_t off = pre[c0] + r.first[ACF_FRAME];
   const uint64_t len = r.hdr_len + (pre[c0 + k] - pre[c0]) + 1;
-  const uint64_t ilen = acf_geom(r.n, g.max_page_n, g.a.n_vars).idx;
+  const uint64_t ilen = fp.index_bytes(g.a.n_vars);
   PcoB200FileRef ref;
   ref.offset = off;
   ref.len = len;
@@ -366,13 +342,11 @@ __global__ void __launch_bounds__(ACF_INDEX_THREADS) acf_index_kernel(AcfArgs g)
   if (c >= st->live_chunks || !st->fits) return;
   const ChunkEnc* chunks = reinterpret_cast<const ChunkEnc*>(g.a.ws + g.a.lay.chunks);
   const AcfFile& f = acf_files(g)[reinterpret_cast<const uint32_t*>(g.a.ws + g.l.cfile)[c]];
-  const AcfGeom fg = acf_geom(f.n, g.max_page_n, g.a.n_vars);
-  const uint64_t j = c - f.first[ACF_CHUNKS], q = j < fg.rem ? j : fg.rem;
+  const uint64_t j = c - f.first[ACF_CHUNKS];
   const uint64_t cs = acomp_starts(g.a)[c], n = acomp_starts(g.a)[c + 1] - cs;
   const uint32_t nb = n_batches_of(uint32_t(n));
   const uint32_t n_vars = chunks[c].fallback ? 1 : g.a.n_vars;
-  const uint64_t eoff = sizeof(IndexHeader) + fg.k * sizeof(IndexChunk) + q * acomp_entries_bytes(g.a.n_vars, fg.low + 1) +
-                        (j - q) * acomp_entries_bytes(g.a.n_vars, fg.low);
+  const uint64_t eoff = equal_pages(f.n, g.max_page_n).entries_offset(g.a.n_vars, j);
   uint8_t* ix = g.a.index + f.first[ACF_IDX];
   if (threadIdx.x == 0) {
     IndexChunk ic;
@@ -384,7 +358,7 @@ __global__ void __launch_bounds__(ACF_INDEX_THREADS) acf_index_kernel(AcfArgs g)
     reinterpret_cast<IndexChunk*>(ix + sizeof(IndexHeader))[j] = ic;
   }
   const BatchEntry* entries = reinterpret_cast<const BatchEntry*>(g.a.ws + g.a.lay.entries);
-  const uint64_t words = acomp_entries_bytes(g.a.n_vars, n) / 4, used = uint64_t(n_vars) * nb * 3;
+  const uint64_t words = entries_bytes(g.a.n_vars, n) / 4, used = uint64_t(n_vars) * nb * 3;
   uint32_t* dst = reinterpret_cast<uint32_t*>(ix + eoff);
   for (uint64_t w = threadIdx.x; w < words; w += ACF_INDEX_THREADS) {
     uint32_t x = 0;
@@ -431,8 +405,7 @@ struct AcfPlanGeom {
   AcfLayout l;
 };
 inline uint64_t acf_chunk_n(uint64_t max_page_n, uint64_t max_file_n, uint64_t nums_cap) {
-  const uint64_t mp = max_page_n == 0 ? (uint64_t(1) << 18) : max_page_n;
-  return std::max<uint64_t>(1, std::min({mp, max_file_n, nums_cap}));
+  return std::max<uint64_t>(1, std::min({page_cap(max_page_n), max_file_n, nums_cap}));
 }
 inline AcfPlanGeom acf_plan_geom(const PcoB200AsyncCompressFilesPlan& p) {
   AcfPlanGeom pg;
@@ -469,7 +442,7 @@ void acf_launch_encode(const PcoB200AsyncCompressFilesPlan& p, const AcompGeom& 
   acf_init_kernel<<<init_ctas, ACF_THREADS, 0, stream>>>(fa);
   ln.end();
   // the CHUNK_BINS kernels compute each chunk's unoptimized_bins_log from the level and its n
-  const EncParams ep = acomp_enc_params(p, g, fa.a, nums, p.nums_cap, p.level, 0);
+  const EncParams ep = acomp_enc_params(p, g, fa.a, nums, p.nums_cap, p.level);
   enqueue_encode_kernels<L, true>(g, fa.a, ep, ln);
   // ---- placement: every chunk's final place in dst, behind its file's header
   ln.begin("acf_bytes_kernel");

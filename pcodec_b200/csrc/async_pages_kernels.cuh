@@ -65,7 +65,7 @@ struct ApLayout : AsyncDecodeTail {
   uint64_t state, tab, index, index_len, frames, pad_frame, pstat, wst, ends, parts, table, fast_page, cold_list;
 };
 __host__ __device__ inline uint64_t ap_ctas(uint64_t n) { return (n + AP_THREADS - 1) / AP_THREADS; }
-// Batch entries of an accepted batch: each page's entries_room (16-byte aligned room for MAX_VARS x ceil(n / 256) entries of 12 bytes)
+// Batch entries of an accepted batch: each page's entries_bytes(MAX_VARS, n) (16-byte aligned room for MAX_VARS x ceil(n / 256) entries of 12 bytes)
 // is at most 24 floor(n / 256) + 32 bytes, and the pages hold at most dst_cap numbers.
 __host__ __device__ inline uint64_t ap_entries_bound(uint64_t max_pages, uint64_t dst_cap) { return 24 * (dst_cap / BATCH_N) + 32 * max_pages; }
 __host__ __device__ inline ApLayout ap_layout(uint64_t max_pages, uint64_t dst_cap, uint64_t frame_cap) {
@@ -94,9 +94,6 @@ __device__ __forceinline__ uint64_t ap_n_pages(const ApArgs& g) {
 }
 // a page's framed chunk: [dtype][page_n - 1, 24 bits][meta][page], 16-byte aligned (decompress_pages_impl)
 __device__ __forceinline__ uint64_t ap_frame_bytes(const PcoB200PageRef& r) { return (4 + r.meta_len + r.page_len + 15) & ~uint64_t(15); }
-__device__ __forceinline__ uint64_t ap_entries_room(uint64_t n) {
-  return (uint64_t(MAX_VARS) * n_batches_of(uint32_t(n)) * sizeof(BatchEntry) + 15) & ~uint64_t(15);
-}
 
 // ceil(max_pages / AP_THREADS) CTAs, one page slot per thread: the argument checks decompress_pages_impl makes for each page, in its order
 // (meta range, page range, page_n), and the sizes the placement scans.
@@ -118,7 +115,7 @@ __global__ void __launch_bounds__(AP_THREADS) ap_pages_kernel(ApArgs g, AsyncChe
       atomicMin(&s_bad, (i << 32) | ref);
     } else {
       frame = ap_frame_bytes(r);
-      room = ap_entries_room(r.page_n);
+      room = entries_bytes(MAX_VARS, r.page_n);
       nums = r.page_n;
     }
   }
@@ -202,7 +199,7 @@ __global__ void __launch_bounds__(AP_THREADS) ap_place_kernel(ApArgs g, const Ap
   const bool in = (pre == ST_OK || pre == PCO_B200_ASYNC_PAGES_DST || pre == PCO_B200_ASYNC_FRAMES) && i < n;
   PcoB200PageRef r{0, 0, 0, 0, 0};
   if (in) r = g.refs[i];
-  const uint64_t frame = in ? ap_frame_bytes(r) : 0, room = in ? ap_entries_room(r.page_n) : 0, nums = in ? r.page_n : 0;
+  const uint64_t frame = in ? ap_frame_bytes(r) : 0, room = in ? entries_bytes(MAX_VARS, r.page_n) : 0, nums = in ? r.page_n : 0;
   ArSum tot;
   const ArSum f_ex = ar_add(parts[blockIdx.x].frames, ar_block_scan<AP_THREADS>(ar_sum(frame), &tot));
   const ArSum e_ex = ar_add(parts[blockIdx.x].entries, ar_block_scan<AP_THREADS>(ar_sum(room), &tot));

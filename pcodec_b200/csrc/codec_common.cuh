@@ -70,6 +70,56 @@ __host__ __device__ inline bool index_header_ok(const IndexHeader& ih, uint64_t 
          ih.n_chunks <= (index_len - ih.chunks_offset) / sizeof(IndexChunk);
 }
 
+__host__ __device__ inline uint32_t n_batches_of(uint32_t n) { return (n + BATCH_N - 1) / BATCH_N; }
+// latent slots of a chunk of `size` numbers in the encoder's per-number arrays: whole batches
+__host__ __device__ inline uint64_t rows_of(uint64_t size) { return (size + BATCH_N - 1) / BATCH_N * BATCH_N; }
+// A chunk's region of batch entries in a side index: n_vars x batches records of a chunk of n numbers, rounded up to 16 bytes.
+__host__ __device__ inline uint64_t entries_bytes(uint32_t n_vars, uint64_t n) {
+  return (uint64_t(n_vars) * n_batches_of(uint32_t(n)) * sizeof(BatchEntry) + 15) & ~uint64_t(15);
+}
+
+// PagingSpec::EqualPagesUpTo(max_page_n) over n numbers (pco/src/chunk_config.rs:134-183): n_chunks chunks, the first `rem` of
+// low + 1 numbers, the others of low.  max_page_n 0 is the default, 2^18.
+__host__ __device__ inline uint64_t page_cap(uint64_t max_page_n) { return max_page_n == 0 ? (uint64_t(1) << 18) : max_page_n; }
+struct EqualPages {
+  uint64_t n_chunks, low, rem;
+  __host__ __device__ uint64_t start(uint64_t c) const { return c * low + (c < rem ? c : rem); }
+  __host__ __device__ uint64_t size(uint64_t c) const { return low + (c < rem ? 1 : 0); }
+  __host__ __device__ uint64_t row_start(uint64_t c) const {
+    const uint64_t q = c < rem ? c : rem;
+    return q * rows_of(low + 1) + (c - q) * rows_of(low);
+  }
+  // the side index compress_typed writes for these chunks: header, chunk records, then each chunk's entries of n_vars vars
+  __host__ __device__ uint64_t entries_offset(uint32_t n_vars, uint64_t c) const {
+    const uint64_t q = c < rem ? c : rem;
+    return ((sizeof(IndexHeader) + n_chunks * sizeof(IndexChunk) + 15) & ~uint64_t(15)) + q * entries_bytes(n_vars, low + 1) +
+           (c - q) * entries_bytes(n_vars, low);
+  }
+  __host__ __device__ uint64_t index_bytes(uint32_t n_vars) const { return entries_offset(n_vars, n_chunks); }
+};
+__host__ __device__ inline EqualPages equal_pages(uint64_t n, uint64_t max_page_n) {
+  EqualPages p = {0, 0, 0};
+  if (n == 0) return p;
+  const uint64_t mp = page_cap(max_page_n);
+  p.n_chunks = (n + mp - 1) / mp;
+  p.low = n / p.n_chunks;
+  p.rem = n % p.n_chunks;
+  return p;
+}
+
+// unoptimized_bins_log of var v of a chunk of n >= 1 numbers at compression level `level` (pco/src/wrapped/chunk_compressor.rs:362-371;
+// the secondary var takes at most 6, LIMITED_UNOPTIMIZED_BINS_LOG, :238-248).
+__host__ __device__ __forceinline__ uint32_t unoptimized_bins_log(uint32_t level, uint64_t n, int v) {
+#ifdef __CUDA_ARCH__
+  const uint32_t log_n = 63u - uint32_t(__clzll((long long)n));
+#else
+  const uint32_t log_n = 63u - uint32_t(__builtin_clzll(n));
+#endif
+  const uint32_t fast = log_n >= 4 ? log_n - 4 : 0;
+  const uint32_t b = level <= fast ? level : fast + (level - fast) / 2;
+  return v == 0 ? b : (b < 6u ? b : 6u);
+}
+
 // ---------------------------------------------------------------------------
 // Bit stream view: a byte range addressed through 8-byte aligned words.
 // ---------------------------------------------------------------------------

@@ -1,8 +1,6 @@
 // Host orchestration of the compress path: validates the ChunkConfig like the reference, lays out the
 // chunks, runs the encode kernels on one stream and returns the .pco bytes (+ optional side index).
 #pragma once
-#include <cstdlib>
-
 #include <atomic>
 #include <cmath>
 #include <map>
@@ -13,10 +11,6 @@
 #include "host_common.hpp"
 #include "mode_search.hpp"
 
-#ifndef PCOB_ONE_PASS_DEFAULT
-#define PCOB_ONE_PASS_DEFAULT true  // PCOB200_ONE_PASS_FRONT_END=0 selects the two-kernel front end (A/B runs)
-#endif
-
 namespace pcob200 {
 
 // internal flag of compress_typed (not in the public enum): the call's chunks are the PAGES of one wrapped chunk and share
@@ -26,9 +20,8 @@ constexpr uint32_t PCO_B200_INTERNAL_SHARED_BINS = 1u << 16;
 
 struct CompressScratch {
   DevBuf lat0, lat1, keys_a, keys_b, sym0, sym1, ans0, ans1, ob_sum, ans_sum, entries, plans, chunks, starts, seg, out, small, index, probes, sample, sample_starts, key16_0, key16_1, idx_out, lb_vals, lb_resid, lb_scratch;
-  // kernel attributes are per instantiation: one flag per latent width (index log2(sizeof(L)))
-  bool plan_attr_set[4] = {false, false, false, false}, union_attr_set[4] = {false, false, false, false}, sort_attr_set[4] = {false, false, false, false};
-  bool wide_attr_set[4] = {false, false, false, false};  // the wide (more than 256 bins) instantiations
+  // set_encode_attrs has run for [WIDE][log2(sizeof(L))]
+  bool encode_attrs_set[2][4] = {};
   bool src_in_place = false;  // this call reads its numbers from the caller's page-locked host buffer (host_common.hpp, zero copy)
   // ans_encode_kernel's round counters of the last call, kept only while profiling is on (pco_b200_profile_ans_paths)
   DevBuf ans_paths;
@@ -41,26 +34,14 @@ struct CompressScratch {
   }
 };
 
-// pco/src/wrapped/chunk_compressor.rs:362-371
-inline uint32_t choose_unoptimized_bins_log(uint32_t level, size_t n) {
-  uint32_t log_n = uint32_t(std::floor(std::log2(double(n))));
-  uint32_t fast = log_n >= 4 ? log_n - 4 : 0;
-  if (level <= fast) return level;
-  return fast + (level - fast) / 2;
-}
-
 // pco/src/chunk_config.rs:134-183
 inline PcoB200Error n_per_page(const PcoB200ChunkConfig& cfg, size_t n, std::vector<uint64_t>* out) {
   out->clear();
   if (cfg.paging_spec == PCO_B200_PAGING_EXACT) {
     out->assign(cfg.exact_page_ns, cfg.exact_page_ns + cfg.n_exact_pages);
   } else {
-    if (n == 0) return PCO_B200_OK;
-    size_t max_page_n = cfg.max_page_n == 0 ? (size_t(1) << 18) : size_t(cfg.max_page_n);
-    size_t n_pages = (n + max_page_n - 1) / max_page_n;
-    size_t low = n / n_pages, r = n % n_pages;
-    out->assign(n_pages, low);
-    for (size_t i = 0; i < r; i++) (*out)[i] = low + 1;
+    const EqualPages ep = equal_pages(n, cfg.max_page_n);
+    for (uint64_t c = 0; c < ep.n_chunks; c++) out->push_back(ep.size(c));
   }
   uint64_t summed = 0;
   for (uint64_t p : *out) summed += p;
@@ -71,19 +52,34 @@ inline PcoB200Error n_per_page(const PcoB200ChunkConfig& cfg, size_t n, std::vec
   return PCO_B200_OK;
 }
 
+// Scratch of one CHUNKS_ONLY pass of compress_typed over n numbers in chunks of the given sizes: the chunks' bytes (64, and each chunk's
+// size guarantee plus 8 bytes of slack) and the side index.
+struct ChunksScratch {
+  size_t bytes, index;
+};
+inline ChunksScratch chunks_only_scratch(uint32_t lbits, uint64_t n, const std::vector<uint64_t>& chunk_ns) {
+  ChunksScratch s{64, pco_b200_index_size_bound(size_t(n), chunk_ns.size()) + 64 * chunk_ns.size()};
+  for (uint64_t p : chunk_ns) s.bytes += standalone_chunk_size_guarantee(lbits, size_t(p)) + 8;
+  return s;
+}
+
 // standalone header bytes (pco/src/standalone/compressor.rs:12-16,85-105) into out[0 .. STANDALONE_HEADER_MAX); returns their count.
 // The size hint is a varint: 6 bits (power - 1), then the `power` bits of n_hint.
 constexpr uint32_t STANDALONE_HEADER_MAX = 17;
+__host__ __device__ inline uint32_t size_hint_power(uint64_t n_hint) {
+  uint32_t power = 1;
+  while (power < 64 && (n_hint >> power) != 0) power++;
+  return power;
+}
+__host__ __device__ inline uint32_t standalone_header_len(uint64_t n_hint) { return 8 + (6 + size_hint_power(n_hint) + 7) / 8; }
 __host__ __device__ inline uint32_t standalone_header_into(uint64_t n_hint, uint8_t uniform_type, uint8_t* out) {
   const uint8_t magic[6] = {112, 99, 111, 33, 3, uniform_type};
   for (int i = 0; i < 6; i++) out[i] = magic[i];
-  uint32_t power = 1;
-  while (power < 64 && (n_hint >> power) != 0) power++;
-  const uint32_t nbytes = (6 + power + 7) / 8;
-  for (uint32_t i = 0; i < nbytes; i++) out[6 + i] = uint8_t(i == 0 ? ((power - 1) | (n_hint << 6)) : (n_hint >> (8 * i - 6)));
-  out[6 + nbytes] = 4;
-  out[7 + nbytes] = 1;
-  return 8 + nbytes;
+  const uint32_t power = size_hint_power(n_hint), len = standalone_header_len(n_hint);
+  for (uint32_t i = 0; i < len - 8; i++) out[6 + i] = uint8_t(i == 0 ? ((power - 1) | (n_hint << 6)) : (n_hint >> (8 * i - 6)));
+  out[len - 2] = 4;
+  out[len - 1] = 1;
+  return len;
 }
 inline std::vector<uint8_t> make_standalone_header(uint64_t n_hint, uint8_t uniform_type) {
   uint8_t h[STANDALONE_HEADER_MAX];
@@ -170,6 +166,55 @@ inline void set_float_mult(ModeSel* ms, uint32_t lbits, double base_d, double in
     ms->inv_base_bits = ib;
     ms->mode_base = (bb >> 31) ? uint32_t(~bb) : (bb ^ 0x80000000u);
   }
+}
+
+// The EncParams of a pass: the number type, the header flavour (uniform_type: the dtype or 0), the mode, the delta order and the primary
+// var's unoptimized_bins_log (the CHUNK_BINS kernels read the level there).  The caller fills the chunk fields.
+inline EncParams enc_params(uint32_t dtype, uint32_t uniform_type, const ModeSel& ms, uint32_t order, uint32_t bins_log) {
+  EncParams ep;
+  std::memset(&ep, 0, sizeof(ep));
+  ep.dtype = dtype;
+  ep.uniform_type = uniform_type;
+  ep.mode = ms.mode;
+  ep.mode_base = ms.mode_base;
+  ep.base_bits = ms.base_bits;
+  ep.inv_base_bits = ms.inv_base_bits;
+  ep.mode_k = ms.mode_k;
+  ep.order = order;
+  ep.n_vars = ms.mode == MODE_CLASSIC ? 1 : 2;
+  ep.bins_log[0] = bins_log;
+  ep.bins_log[1] = std::min<uint32_t>(bins_log, 6);  // LIMITED_UNOPTIMIZED_BINS_LOG (chunk_compressor.rs:238-248)
+  return ep;
+}
+
+// The shared-memory size and carveout attributes of the encode kernels of latent type L: the narrow instantiations (the planner's in
+// their CHUNK_BINS form when CHUNK_BINS), or the wide ones when WIDE.
+template <typename L, bool WIDE, bool CHUNK_BINS = false>
+inline cudaError_t set_encode_attrs() {
+  const int count_smem = int(((size_t(1) << PLAN_MAX_COUNT_BITS) + 1) * 4 + 16), max_shared = int(cudaSharedmemCarveoutMaxShared);
+  cudaError_t err = cudaSuccess;
+  auto set = [&](const void* f, cudaFuncAttribute attr, int value) {
+    if (err == cudaSuccess) err = cudaFuncSetAttribute(f, attr, value);
+  };
+  if constexpr (WIDE) {
+    set((const void*)plan_probe_kernel<L, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, count_smem);
+    set((const void*)plan_solve_wide_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(sizeof(WideSolveSmem)));
+    set((const void*)pack_kernel<L, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(sizeof(PackSmemT<true>)));
+    set((const void*)plan_probe_kernel<L, true, true>, cudaFuncAttributePreferredSharedMemoryCarveout, max_shared);
+    set((const void*)plan_solve_wide_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, max_shared);
+    set((const void*)pack_kernel<L, true>, cudaFuncAttributePreferredSharedMemoryCarveout, max_shared);
+  } else {
+    set((const void*)plan_probe_kernel<L, true, false, CHUNK_BINS>, cudaFuncAttributeMaxDynamicSharedMemorySize, count_smem);
+    set((const void*)split_count_kernel<L, CHUNK_BINS>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(size_t(SC_N) * 4));
+    set((const void*)union_probe_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(size_t(SC_N) * 4));
+    set((const void*)pack_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(sizeof(PackSmem)));
+    set((const void*)radix_sort_segments_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(size_t(RS_WARPS) * RS_BINS * sizeof(uint32_t)));
+    // several counting CTAs per SM: ask for the largest shared-memory carveout
+    set((const void*)plan_probe_kernel<L, true, false, CHUNK_BINS>, cudaFuncAttributePreferredSharedMemoryCarveout, max_shared);
+    set((const void*)pack_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, max_shared);
+    set((const void*)bin_lut_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, max_shared);
+  }
+  return err;
 }
 
 // the numbers of every chunk at the positions choose_mode_sample visits (sampling.rs:73-95): positions depend on the chunk's n only
@@ -381,11 +426,6 @@ static PcoB200Error plan_front(CompressScratch& S, cudaStream_t stream, EncParam
     }
     profiler().end(stream);
   };
-  auto ensure_sort_attr = [&]() -> cudaError_t {
-    if (S.sort_attr_set[LW]) return cudaSuccess;
-    S.sort_attr_set[LW] = true;
-    return cudaFuncSetAttribute(radix_sort_segments_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RS_SMEM);
-  };
 
     const uint32_t n_chunks = e.n_chunks;
     PCOB_CUDA_TRY(S.lat0.reserve(slots * sizeof(L) + 64));
@@ -393,31 +433,13 @@ static PcoB200Error plan_front(CompressScratch& S, cudaStream_t stream, EncParam
     d_lat[0] = S.lat0.as<L>();
     d_lat[1] = S.lat1.as<L>();
     init_chunks_kernel<<<(n_chunks + 255) / 256, 256, 0, stream>>>(d_chunks, n_chunks);
-    if (!S.plan_attr_set[LW]) {
-      S.plan_attr_set[LW] = true;
-      PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)(((size_t(1) << PLAN_MAX_COUNT_BITS) + 1) * 4 + 16)));
-      PCOB_CUDA_TRY(cudaFuncSetAttribute(split_count_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(size_t(SC_N) * 4)));
-      PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PackSmem)));
-      // several counting CTAs per SM: ask for the largest shared-memory carveout
-      PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-      PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-      PCOB_CUDA_TRY(cudaFuncSetAttribute(bin_lut_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    for (const bool wide : {false, WIDE}) {
+      if (S.encode_attrs_set[wide][LW]) continue;
+      S.encode_attrs_set[wide][LW] = true;
+      PCOB_CUDA_TRY((wide ? set_encode_attrs<L, true>() : set_encode_attrs<L, false>()));
     }
-    if (WIDE && !S.wide_attr_set[LW]) {
-      S.wide_attr_set[LW] = true;
-      PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)(((size_t(1) << PLAN_MAX_COUNT_BITS) + 1) * 4 + 16)));
-      PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_solve_wide_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WideSolveSmem)));
-      PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PackSmemT<true>)));
-      PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-      PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_solve_wide_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-      PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L, true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    }
-#ifndef PCOB_NO_SPLIT_COUNT
     if constexpr (!WIDE) {  // (wide sets: the two-kernel path below)
-    static const bool one_pass = [] { const char* v = std::getenv("PCOB200_ONE_PASS_FRONT_END"); return v ? v[0] != '0' : PCOB_ONE_PASS_DEFAULT; }();
-    if (one_pass && e.mode == MODE_CLASSIC && e.n_vars == 1) {
+    if (e.mode == MODE_CLASSIC && e.n_vars == 1) {
       // one-pass front end: split + delta + counting histogram + 16-bit keys, no 64-bit latents (split_count_kernel).
       // It assumes every chunk's stored latents span < 2^15; a chunk that does not raises flags[1] and the call is redone
       // on the two-kernel path below (the speculation costs one read of the input).
@@ -432,10 +454,6 @@ static PcoB200Error plan_front(CompressScratch& S, cudaStream_t stream, EncParam
       call_trace().mark("c.flags");
       if (fl[1] == 0 && shared) {
         // pages of one chunk: one histogram over all of them, one plan, copied to every page's slot
-        if (!S.union_attr_set[LW]) {
-          S.union_attr_set[LW] = true;
-          PCOB_CUDA_TRY(cudaFuncSetAttribute(union_probe_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(size_t(SC_N) * 4)));
-        }
         PCOB_CUDA_TRY(cudaMemsetAsync(d_small, 0, 8, stream));
         profiler().begin("union_probe_kernel", stream);
         union_probe_kernel<L><<<1, SC_THREADS, size_t(SC_N) * 4, stream>>>(e, n_chunks, d_chunks, d_probes, S.key16_0.as<uint16_t>(), d_small);
@@ -471,7 +489,6 @@ static PcoB200Error plan_front(CompressScratch& S, cudaStream_t stream, EncParam
       }
     }
     }
-#endif
     profiler().begin("split_delta_kernel", stream);
     switch (e.mode) {
       case MODE_CLASSIC: split_delta_kernel<L, MODE_CLASSIC><<<n_chunks * tiles, SPLIT_THREADS, 0, stream>>>(e, tiles, d_lat[0], d_lat[1], d_chunks); break;
@@ -510,7 +527,6 @@ static PcoB200Error plan_front(CompressScratch& S, cudaStream_t stream, EncParam
       const L* sorted = S.keys_a.as<L>();
       if (stored_total > 1) {
         const uint32_t sort_bits = std::max<uint32_t>(range_bits, 1);
-        PCOB_CUDA_TRY(ensure_sort_attr());
         profiler().begin("union_radix_sort_kernel", stream);
         radix_sort_segments_kernel<L><<<1, RS_THREADS, RS_SMEM, stream>>>(S.keys_a.as<L>(), S.keys_b.as<L>(), d_seg, d_seg + 1, sort_bits);
         profiler().end(stream);
@@ -554,7 +570,6 @@ static PcoB200Error plan_front(CompressScratch& S, cudaStream_t stream, EncParam
       const L* sorted = S.keys_a.as<L>();
       {
         const uint32_t sort_bits = std::max<uint32_t>(range_bits, 1);
-        PCOB_CUDA_TRY(ensure_sort_attr());
         profiler().begin("radix_sort_segments_kernel", stream);
         radix_sort_segments_kernel<L><<<n_chunks, RS_THREADS, RS_SMEM, stream>>>(S.keys_a.as<L>(), S.keys_b.as<L>(), seg_begin, seg_end, sort_bits);
         profiler().end(stream);
@@ -679,12 +694,12 @@ static PcoB200Error compress_typed(CompressScratch& S, const void* nums, size_t 
   // that disagree (small chunks on either side of a power of two) go through the pipeline in separate runs below.  The Auto searches plan
   // all chunks' samples in one launch: they still need one value.
   const bool shared_bins = (flags & PCO_B200_INTERNAL_SHARED_BINS) && pages.size() > 1;
-  const uint32_t bins_log = choose_unoptimized_bins_log(cfg.compression_level, shared_bins ? n : size_t(pages[0]));
+  const uint32_t bins_log = unoptimized_bins_log(cfg.compression_level, shared_bins ? n : pages[0], 0);
   std::vector<uint32_t> chunk_bins_log(pages.size(), bins_log);
   bool bins_log_uniform = true;
   if (!shared_bins)
     for (size_t i = 0; i < pages.size(); i++) {
-      chunk_bins_log[i] = choose_unoptimized_bins_log(cfg.compression_level, size_t(pages[i]));
+      chunk_bins_log[i] = unoptimized_bins_log(cfg.compression_level, pages[i], 0);
       if (chunk_bins_log[i] != bins_log) bins_log_uniform = false;
     }
   if (!bins_log_uniform && (auto_mode || auto_delta))
@@ -715,9 +730,6 @@ static PcoB200Error compress_typed(CompressScratch& S, const void* nums, size_t 
     call_trace().mark("c.h2d_submitted");
   }
   // scratch sized for the whole call; every run below (and the Auto searches) indexes it from 0
-  std::vector<uint64_t> rows_all(pages.size() + 1, 0);
-  for (size_t i = 0; i < pages.size(); i++) rows_all[i + 1] = rows_all[i] + ((pages[i] + BATCH_N - 1) / BATCH_N) * BATCH_N;
-  const uint32_t bpc_all = n_batches_of(uint32_t(max_chunk_n));
   PCOB_CUDA_TRY(S.plans.reserve(size_t(n_chunks_all) * MAX_VARS * (any_wide ? sizeof(VarPlanT<true>) : sizeof(VarPlan))));
   PCOB_CUDA_TRY(S.chunks.reserve(size_t(n_chunks_all) * sizeof(ChunkEnc)));
   PCOB_CUDA_TRY(S.starts.reserve((starts.size() + 1) * 32));
@@ -851,19 +863,14 @@ static PcoB200Error compress_typed(CompressScratch& S, const void* nums, size_t 
       PCOB_CUDA_TRY(cudaMemcpyAsync(d_ustarts, ustarts.data(), ustarts.size() * 8, cudaMemcpyHostToDevice, stream));
       PCOB_CUDA_TRY(cudaMemcpyAsync(d_modes, hm.data(), hm.size() * sizeof(ModeSelDev), cudaMemcpyHostToDevice, stream));
       gather_primary_sample_kernel<L><<<uint32_t(n_units), 256, 0, stream>>>(static_cast<const L*>(d_nums), d_ustarts, d_ss, d_modes, dtype, S.sample.as<L>());
-      EncParams es;
-      std::memset(&es, 0, sizeof(es));
-      es.dtype = lbits == 8 ? NT_U8 : lbits == 16 ? NT_U16 : lbits == 32 ? NT_U32 : NT_U64;  // the sample holds latents: unsigned numbers of the same width
-      es.mode = MODE_CLASSIC;
-      es.n_vars = 1;
+      // the sample holds latents: unsigned numbers of the same width
+      EncParams es = enc_params(lbits == 8 ? NT_U8 : lbits == 16 ? NT_U16 : lbits == 32 ? NT_U32 : NT_U64, 0, ModeSel{}, 0, bins_log);
       es.nums = S.sample.p;
       es.chunk_starts = d_ss;
       es.row_base = d_srows;
       es.n_total = s_starts.back();
       es.n_chunks = uint32_t(n_units);
       es.max_chunk_n = uint32_t(max_ns);
-      es.bins_log[0] = bins_log;
-      es.bins_log[1] = std::min<uint32_t>(bins_log, 6);
       const uint32_t s_tiles = uint32_t((max_ns + SPLIT_TILE - 1) / SPLIT_TILE);
       std::vector<Summary> h_sum(n_units);
       std::vector<float> best_cost(n_units, 0.f);
@@ -981,7 +988,7 @@ static PcoB200Error compress_typed(CompressScratch& S, const void* nums, size_t 
     for (const Run& r : runs)
       for (size_t c = r.c0; c < r.c1; c++) {
         eoff[c] = off;
-        off += (uint64_t(r.ms.mode == MODE_CLASSIC ? 1 : 2) * n_batches_of(uint32_t(pages[c])) * sizeof(BatchEntry) + 15) & ~uint64_t(15);
+        off += entries_bytes(r.ms.mode == MODE_CLASSIC ? 1 : 2, pages[c]);
       }
     if (off > index_cap) return fail(PCO_B200_IO, "index buffer too small (need " + std::to_string(off) + " bytes)");
     index_total = off;
@@ -1012,22 +1019,10 @@ static PcoB200Error compress_typed(CompressScratch& S, const void* nums, size_t 
       rrows[i + 1] = rrows[i] + ((rpages[i] + BATCH_N - 1) / BATCH_N) * BATCH_N;
       run_max_n = std::max(run_max_n, rpages[i]);
     }
-    EncParams ep;
-    std::memset(&ep, 0, sizeof(ep));
-    ep.dtype = dtype;
-    ep.uniform_type = uniform_type ? dtype : 0;
-    ep.mode = run.ms.mode;
-    ep.mode_base = run.ms.mode_base;
-    ep.base_bits = run.ms.base_bits;
-    ep.inv_base_bits = run.ms.inv_base_bits;
-    ep.mode_k = run.ms.mode_k;
-    ep.order = run.order;
-    ep.n_vars = ep.mode == MODE_CLASSIC ? 1 : 2;
+    EncParams ep = enc_params(dtype, uniform_type ? dtype : 0, run.ms, run.order, run.bins_log);
     ep.n_total = rstarts.back();
     ep.n_chunks = n_chunks;
     ep.max_chunk_n = uint32_t(run_max_n);
-    ep.bins_log[0] = run.bins_log;
-    ep.bins_log[1] = std::min<uint32_t>(run.bins_log, 6);  // LIMITED_UNOPTIMIZED_BINS_LOG (chunk_compressor.rs:238-248)
     ep.nums = static_cast<const L*>(d_nums) + starts[run.c0];
     const uint32_t bpc = n_batches_of(uint32_t(run_max_n));
     const uint32_t tiles_per_chunk = uint32_t((run_max_n + SPLIT_TILE - 1) / SPLIT_TILE);

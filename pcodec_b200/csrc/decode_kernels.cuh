@@ -268,8 +268,6 @@ struct WalkResult {     // written by the serial walker
   uint64_t n_total;     // numbers in the indexed chunks
 };
 
-__host__ __device__ inline uint32_t n_batches_of(uint32_t n) { return (n + BATCH_N - 1) / BATCH_N; }
-
 // Walk one chunk whose header is already parsed and tables built (WALKER nodes: the field byte is the bin's offset_bits), by ONE
 // thread: the chunk's bit cursor is a single serial chain (batch boundaries are not in the stream: a batch's offsets section is as long
 // as the sum of the offset bits of the symbols just walked, page_latent_decompressor.rs:106-134).  What the chain costs per group of 4

@@ -67,16 +67,8 @@ struct EncParams {
   uint32_t uniform_type;   // header flavour
 };
 
-// unoptimized_bins_log of var v of a chunk of n >= 1 numbers at compression level `level` (choose_unoptimized_bins_log,
-// chunk_compressor.rs:362-371; the secondary var takes at most 6, LIMITED_UNOPTIMIZED_BINS_LOG, chunk_compressor.rs:238-248).  The
-// CHUNK_BINS instantiations of the planner kernels take the level in ep.bins_log[0] and compute each chunk's value with this, so one
-// launch serves chunks whose sizes imply different values.
-__device__ __forceinline__ uint32_t chunk_bins_log(uint32_t level, uint64_t n, int v) {
-  const uint32_t log_n = 63u - uint32_t(__clzll((long long)n));
-  const uint32_t fast = log_n >= 4 ? log_n - 4 : 0;
-  const uint32_t b = level <= fast ? level : fast + (level - fast) / 2;
-  return v == 0 ? b : min(b, 6u);
-}
+// The CHUNK_BINS instantiations of the planner kernels take the level in ep.bins_log[0] and compute each chunk's value with
+// unoptimized_bins_log (codec_common.cuh), so one launch serves chunks whose sizes imply different values.
 
 template <bool WIDE>
 struct VarPlanT {
@@ -348,13 +340,17 @@ __global__ void __launch_bounds__(SPLIT_THREADS) split_delta_kernel(EncParams ep
   }
 }
 
-__global__ void init_chunks_kernel(ChunkEnc* chunks, uint32_t n_chunks) {
-  uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= n_chunks) return;
+// a chunk's record before the front end: zero, and an empty latent range
+__device__ inline void reset_chunk_enc(ChunkEnc* ch) {
   ChunkEnc z;
   memset(&z, 0, sizeof(z));
   z.vmin[0] = z.vmin[1] = ~uint64_t(0);
-  chunks[c] = z;
+  *ch = z;
+}
+__global__ void init_chunks_kernel(ChunkEnc* chunks, uint32_t n_chunks) {
+  uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n_chunks) return;
+  reset_chunk_enc(&chunks[c]);
 }
 
 // Stored range of var v in chunk [cs, ce): [cs + order_v, ce)
@@ -652,7 +648,7 @@ __global__ void __launch_bounds__(PLAN_THREADS) plan_probe_kernel(EncParams ep, 
     return lo;
   };
   PlanProbesT<WIDE>& pr = probes[c];
-  const uint32_t n_bins_log = CHUNK_BINS ? chunk_bins_log(ep.bins_log[0], ce - cs, v) : ep.bins_log[v];
+  const uint32_t n_bins_log = CHUNK_BINS ? unoptimized_bins_log(ep.bins_log[0], ce - cs, v) : ep.bins_log[v];
   const uint32_t nbk = 1u << n_bins_log;
   auto c_count_of = [&](uint32_t b) -> uint32_t { return uint32_t((uint64_t(b + 1) * n + nbk - 1) >> n_bins_log); };
   if (tid == 0) pr.first = s_at(0);
@@ -883,7 +879,7 @@ __global__ void __launch_bounds__(SC_THREADS, 1) split_count_kernel(EncParams ep
     return lo;
   };
   PlanProbes& pr = probes[c];
-  const uint32_t n_bins_log = CHUNK_BINS ? chunk_bins_log(ep.bins_log[0], n, 0) : ep.bins_log[0];
+  const uint32_t n_bins_log = CHUNK_BINS ? unoptimized_bins_log(ep.bins_log[0], n, 0) : ep.bins_log[0];
   const uint32_t nbk = 1u << n_bins_log;
   auto c_count_of = [&](uint32_t b) -> uint32_t { return uint32_t((uint64_t(b + 1) * stored + nbk - 1) >> n_bins_log); };
   if (tid == 0) pr.first = s_at(0);
@@ -1030,7 +1026,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS) plan_solve_kernel(EncParams ep,
     return;
   }
   ENC_TICK_INIT();
-  const uint32_t n_bins_log = CHUNK_BINS ? chunk_bins_log(ep.bins_log[0], ce - cs, v) : ep.bins_log[v];
+  const uint32_t n_bins_log = CHUNK_BINS ? unoptimized_bins_log(ep.bins_log[0], ce - cs, v) : ep.bins_log[v];
   const uint32_t nbk = 1u << n_bins_log;
   const bool small_n = n <= (1u << 20);  // (cc << n_bins_log) fits 32 bits (n_bins_log <= 8)
   // (cc << n_bins_log) / n, cc <= n: the quotient is at most 2^n_bins_log <= 256, so a float estimate is within 1 of it and one

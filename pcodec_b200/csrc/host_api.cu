@@ -274,14 +274,11 @@ static PcoB200Error out_buffer(Context& c, void* dst, bool dst_dev, uint64_t byt
   return PCO_B200_OK;
 }
 
-// Room for MAX_VARS vars of batch entries for a chunk of `n` numbers, 16-byte aligned.
-static uint64_t entries_room(uint32_t n) { return (uint64_t(MAX_VARS) * n_batches_of(n) * sizeof(BatchEntry) + 15) & ~uint64_t(15); }
-
-// Placeholder records for a walk: from `begin` on, each record gets entries_room of its `n` numbers.  Returns where the entries end.
+// Placeholder records for a walk: from `begin` on, each record gets the entries of MAX_VARS vars of its `n` numbers.  Returns where the entries end.
 static uint64_t lay_out_entries(IndexChunk* recs, size_t n_recs, uint64_t begin) {
   for (size_t k = 0; k < n_recs; k++) {
     recs[k].entries_offset = begin;
-    begin += entries_room(recs[k].n);
+    begin += entries_bytes(MAX_VARS, recs[k].n);
   }
   return begin;
 }
@@ -477,7 +474,7 @@ static PcoB200Error speculative_walk_rounds(Context& c, const uint8_t* src, bool
       std::sort(cs.begin(), cs.end());
       if (cs.empty() || cs.size() > FILE_CAND_CAP || cs[0] != f.pos) { tail[i] = 1; continue; }
       const uint32_t n0 = ((scans[s].pattern >> 8) & 0xffffffu) + 1;
-      const uint64_t stride = entries_room(n0);
+      const uint64_t stride = entries_bytes(MAX_VARS, n0);
       const uint64_t fit = std::min((f.cap - f.count) / n0, FILE_CAND_CAP);  // chunks of this size the cap still takes (>= 1)
       // a few more candidates than fit: coincidences may lie in front of the last chunk that does
       uint64_t m = std::min<uint64_t>({cs.size(), std::max<uint64_t>(1, INDEX_BUDGET / (stride + sizeof(IndexChunk))), fit + 8});
@@ -542,7 +539,7 @@ static PcoB200Error speculative_walk_rounds(Context& c, const uint8_t* src, bool
         ic.out_offset = f.count;
         f.count += n0;
         f.recs.push_back(ic);
-        kept_end = std::max(kept_end, ic.entries_offset + entries_room(n0));
+        kept_end = std::max(kept_end, ic.entries_offset + entries_bytes(MAX_VARS, n0));
       }
       f.pos = p;
       progress = true;
@@ -802,7 +799,7 @@ static void fill_explicit_spec(P* plan, const ConfigCheck& ck) {
 }
 
 // The one-time device set-up of an asynchronous compress plan, here and not in a call (which may be inside a capture): the device, the
-// attributes compress_typed sets on first use, and loaded: the encode stage's kernels for dtype (split_count_kernel and the planner
+// attributes plan_front sets on first use (set_encode_attrs), and loaded: the encode stage's kernels for dtype (split_count_kernel and the planner
 // kernels in their CHUNK_BINS instantiations when CHUNK_BINS) and the call's `extra` kernels.
 template <bool CHUNK_BINS>
 static PcoB200Error async_encode_setup(unsigned char dtype, std::initializer_list<const void*> extra) {
@@ -814,15 +811,7 @@ static PcoB200Error async_encode_setup(unsigned char dtype, std::initializer_lis
                                      (const void*)layout_kernel<false>})) return e;
   return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
     using L = decltype(tag);
-    constexpr size_t RS_SMEM = size_t(RS_WARPS) * RS_BINS * sizeof(uint32_t);
-    const int count_smem = int(((size_t(1) << PLAN_MAX_COUNT_BITS) + 1) * 4 + 16);
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true, false, CHUNK_BINS>, cudaFuncAttributeMaxDynamicSharedMemorySize, count_smem));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(split_count_kernel<L, CHUNK_BINS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(size_t(SC_N) * 4)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PackSmem)));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(radix_sort_segments_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RS_SMEM));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(plan_probe_kernel<L, true, false, CHUNK_BINS>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(pack_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    PCOB_CUDA_TRY(cudaFuncSetAttribute(bin_lut_kernel<L>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    PCOB_CUDA_TRY((set_encode_attrs<L, false, CHUNK_BINS>()));
     return load_kernels({(const void*)split_count_kernel<L, CHUNK_BINS>, (const void*)split_delta_kernel<L, MODE_CLASSIC>, (const void*)split_delta_kernel<L, MODE_INT_MULT>,
                          (const void*)split_delta_kernel<L, MODE_FLOAT_QUANT>, (const void*)split_delta_kernel<L, MODE_FLOAT_MULT>,
                          (const void*)plan_probe_kernel<L, false, false, CHUNK_BINS>, (const void*)sort_keys_kernel<L>, (const void*)plan_solve_kernel<L, CHUNK_BINS>,
@@ -912,13 +901,9 @@ int pco_b200_device_available(void) {
 size_t pco_standalone_guarantee_file_size(size_t n, unsigned char dtype) {
   if (!nt_valid(dtype)) return 0;
   // PagingSpec::default() = EqualPagesUpTo(2^18) (pco/src/chunk_config.rs:127-132, :134-183)
-  const size_t max_page_n = size_t(1) << 18;
+  const EqualPages ep = equal_pages(n, 0);
   size_t res = standalone_header_size();
-  if (n > 0) {
-    size_t n_pages = (n + max_page_n - 1) / max_page_n;
-    size_t low = n / n_pages, r = n % n_pages;
-    res += r * standalone_chunk_size_guarantee(nt_bits(dtype), low + 1) + (n_pages - r) * standalone_chunk_size_guarantee(nt_bits(dtype), low);
-  }
+  if (n > 0) res += ep.rem * standalone_chunk_size_guarantee(nt_bits(dtype), ep.low + 1) + (ep.n_chunks - ep.rem) * standalone_chunk_size_guarantee(nt_bits(dtype), ep.low);
   return res + 1;
 }
 
@@ -1026,45 +1011,6 @@ struct PcoB200ChunkCompressor {
   std::vector<size_t> page_off, page_n;  // byte offset of each emission (+ one past the last), numbers per page
 };
 
-namespace {
-// Byte length of a chunk meta (metadata/chunk.rs:127-189, delta_encoding.rs, chunk_latent_var.rs:55-71) read from host bytes.
-// Only what the GPU path writes/reads is accepted: Classic / IntMult / FloatMult / FloatQuant, delta None / Consecutive.
-PcoB200Error host_chunk_meta_len(const uint8_t* b, size_t len, uint32_t dtype, size_t* out) {
-  const uint32_t lbits = nt_bits(dtype);
-  uint64_t pos = 0;
-  bool short_read = false;
-  auto rd = [&](uint32_t nb) -> uint64_t {
-    uint64_t v = 0;
-    for (uint32_t i = 0; i < nb; i++) {
-      const uint64_t bit = pos + i;
-      if ((bit >> 3) >= len) { short_read = true; break; }
-      v |= uint64_t((b[bit >> 3] >> (bit & 7)) & 1) << i;
-    }
-    pos += nb;
-    return v;
-  };
-  const uint32_t mode = uint32_t(rd(4));
-  uint32_t n_vars = 2;
-  switch (mode) {
-    case MODE_CLASSIC: n_vars = 1; break;
-    case MODE_INT_MULT: case MODE_FLOAT_MULT: pos += lbits; break;
-    case MODE_FLOAT_QUANT: pos += 8; break;
-    default: return fail(PCO_B200_UNSUPPORTED, "wrapped chunk meta: mode outside the GPU hot path");
-  }
-  const uint32_t delta = uint32_t(rd(4));
-  if (delta == 1) pos += 4;  // order (3 bits) + secondary_uses_delta (1 bit)
-  else if (delta != 0) return fail(PCO_B200_UNSUPPORTED, "wrapped chunk meta: delta encoding outside the GPU hot path");
-  for (uint32_t v = 0; v < n_vars; v++) {
-    const uint32_t size_log = uint32_t(rd(4));
-    const uint32_t n_bins = uint32_t(rd(15));
-    pos += uint64_t(n_bins) * (size_log + lbits + offset_bits_bits(lbits));
-  }
-  if (short_read || (pos + 7) / 8 > len) return fail(PCO_B200_INSUFFICIENT_DATA, "chunk meta is cut short");
-  *out = size_t((pos + 7) / 8);
-  return PCO_B200_OK;
-}
-}  // namespace
-
 PcoB200Error pco_b200_file_compressor_write_header(void* dst, size_t dst_cap, size_t* n_written) {
   if (dst_cap < 2) return fail(PCO_B200_IO, "failed to write whole buffer");
   static_cast<uint8_t*>(dst)[0] = 4;  // FormatVersion { major: 4, minor: 1 } (metadata/format_version.rs:30-34,87-91)
@@ -1099,12 +1045,10 @@ PcoB200Error pco_b200_chunk_compressor_new(const void* nums, size_t n, unsigned 
   if (PcoB200Error e = n_per_page(cfg, n, &pages)) return e;
   auto cc = std::make_unique<PcoB200ChunkCompressor>();
   cc->n = n;
-  const uint32_t lbits = nt_bits(dtype);
-  size_t cap = 64;
-  for (uint64_t pn : pages) cap += standalone_chunk_size_guarantee(lbits, size_t(pn)) + 8;
-  cc->bytes.resize(cap);
+  const ChunksScratch cs = chunks_only_scratch(nt_bits(dtype), n, pages);
+  cc->bytes.resize(cs.bytes);
   size_t written = 0, ilen = 0;
-  std::vector<uint8_t> index(pco_b200_index_size_bound(n, pages.size()) + 64 * pages.size());
+  std::vector<uint8_t> index(cs.index);
   // several pages: the pipeline runs them as the call's chunks with ONE set of bins trained on all of them
   const uint32_t flags = PCO_B200_CHUNKS_ONLY | (pages.size() > 1 ? PCO_B200_INTERNAL_SHARED_BINS : 0u);
   if (PcoB200Error e = compress_dispatch(nums, n, dtype, &cfg, false, cc->bytes.data(), cc->bytes.size(), &written, index.data(), index.size(), &ilen, flags,
@@ -1122,7 +1066,7 @@ PcoB200Error pco_b200_chunk_compressor_new(const void* nums, size_t n, unsigned 
     cc->page_n.push_back(size_t(pages[p]));
   }
   cc->page_off.push_back(written);
-  if (PcoB200Error e = host_chunk_meta_len(cc->bytes.data() + 4, cc->page_off[1] - 4, dtype, &cc->meta_len)) return e;
+  if (PcoB200Error e = pco_b200_chunk_meta_size(cc->bytes.data() + 4, cc->page_off[1] - 4, dtype, &cc->meta_len)) return e;
   for (size_t p = 1; p < pages.size(); p++)  // shared bins: every page's emission repeats the chunk meta
     if (cc->page_off[p + 1] - cc->page_off[p] < 4 + cc->meta_len ||
         std::memcmp(cc->bytes.data() + 4, cc->bytes.data() + cc->page_off[p] + 4, cc->meta_len) != 0)
@@ -1157,11 +1101,17 @@ PcoB200Error pco_b200_chunk_compressor_write_page(const PcoB200ChunkCompressor* 
   return PCO_B200_OK;
 }
 
+// Only what the GPU path writes and reads is accepted: Classic / IntMult / FloatMult / FloatQuant, delta None / Consecutive.
 PcoB200Error pco_b200_chunk_meta_size(const void* src, size_t src_len, unsigned char dtype, size_t* meta_len) {
   if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
-  size_t len = 0;
-  if (PcoB200Error e = host_chunk_meta_len(static_cast<const uint8_t*>(src), src_len, dtype, &len)) return e;
-  if (meta_len) *meta_len = len;
+  uint64_t len = 0;
+  bool cold = false;
+  uint32_t mode = 0, variant = 0;
+  wrapped_meta_len(static_cast<const uint8_t*>(src), src_len, dtype, &len, &cold, &mode, &variant);
+  if (mode > MODE_FLOAT_QUANT) return fail(PCO_B200_UNSUPPORTED, "wrapped chunk meta: mode outside the GPU hot path");
+  if (variant > DELTA_CONSECUTIVE) return fail(PCO_B200_UNSUPPORTED, "wrapped chunk meta: delta encoding outside the GPU hot path");
+  if (len > src_len) return fail(PCO_B200_INSUFFICIENT_DATA, "chunk meta is cut short");
+  if (meta_len) *meta_len = size_t(len);
   return PCO_B200_OK;
 }
 
@@ -1578,10 +1528,8 @@ static PcoB200Error compress_wrapped_impl(const void* nums, size_t n, uint32_t d
   // the chunks simple_compress would write; a paging spec that does not fit is reported by the pipeline, with its other checks
   std::vector<uint64_t> chunk_ns;
   if (n_per_page(cfg, n, &chunk_ns) != PCO_B200_OK) chunk_ns.clear();
-  const uint32_t lbits = nt_bits(dtype);
-  size_t cap = 64;
-  for (uint64_t p : chunk_ns) cap += standalone_chunk_size_guarantee(lbits, size_t(p));
-  const size_t icap = pco_b200_index_size_bound(n, chunk_ns.size()) + 64 * chunk_ns.size();
+  const ChunksScratch cs = chunks_only_scratch(nt_bits(dtype), n, chunk_ns);
+  const size_t cap = cs.bytes, icap = cs.index;
   PCOB_CUDA_TRY(c.wrap_file.reserve(cap + 32));
   PCOB_CUDA_TRY(c.wrap_index.reserve(icap));
   uint8_t* d_file = c.wrap_file.as<uint8_t>();
@@ -1681,8 +1629,8 @@ static PcoB200Error compress_files_find_refusal(Context& c, const void* nums, co
     const size_t n = size_t(file_ns[i]);
     std::vector<uint64_t> pages;
     n_per_page(cfg, n, &pages);
-    size_t cap = 64, icap = pco_b200_index_size_bound(n, pages.size()) + 64 * pages.size();
-    for (uint64_t p : pages) cap += standalone_chunk_size_guarantee(nt_bits(dtype), size_t(p));
+    const ChunksScratch cs = chunks_only_scratch(nt_bits(dtype), n, pages);
+    const size_t cap = cs.bytes, icap = cs.index;
     PCOB_CUDA_TRY(c.wrap_file.reserve(cap + 32));
     PCOB_CUDA_TRY(c.wrap_index.reserve(icap));
     CompressResult cr;
@@ -1719,9 +1667,9 @@ static PcoB200Error compress_files_impl(const void* nums, const uint64_t* file_n
     ConfigCheck ck;
     PcoB200Error e = check_config(cfg, dtype, size_t(file_ns[i]), &ck);
     if (e == PCO_B200_OK && !ck.pages.empty()) {
-      bins[i] = choose_unoptimized_bins_log(cfg.compression_level, size_t(ck.pages[0]));
+      bins[i] = unoptimized_bins_log(cfg.compression_level, ck.pages[0], 0);
       bool uniform_bins = true;
-      for (uint64_t p : ck.pages) uniform_bins = uniform_bins && choose_unoptimized_bins_log(cfg.compression_level, size_t(p)) == bins[i];
+      for (uint64_t p : ck.pages) uniform_bins = uniform_bins && unoptimized_bins_log(cfg.compression_level, p, 0) == bins[i];
       if (!uniform_bins && (ck.auto_mode || ck.auto_delta))  // compress_typed's refusal for one array
         e = fail(PCO_B200_UNSUPPORTED, "ModeSpec::Auto / DeltaSpec::Auto over chunks whose sizes imply different unoptimized_bins_log in one call");
     }
@@ -1750,25 +1698,25 @@ static PcoB200Error compress_files_impl(const void* nums, const uint64_t* file_n
   std::map<uint32_t, std::vector<uint32_t>> groups;
   for (size_t i = 0; i < first_bad; i++)
     if (file_ns[i] > 0) groups[bins[i]].push_back(uint32_t(i));
-  struct Group { uint64_t out_at, out_cap, idx_at, idx_cap, total, index_bytes; std::vector<IndexChunk> recs; };
+  struct Group { uint64_t out_at, out_cap, idx_at, idx_cap, total, index_bytes; std::vector<IndexChunk> recs; std::vector<uint64_t> exact; };
   std::vector<Group> gs;
   std::vector<uint32_t> file_group(first_bad, 0), file_c0(first_bad, 0);
   uint64_t out_scratch = 0, idx_scratch = 0;
   for (auto& kv : groups) {
     Group g{};
-    uint64_t cap = 64, nc = 0, n = 0;
+    uint64_t n = 0;
     for (uint32_t f : kv.second) {
       file_group[f] = uint32_t(gs.size());
-      file_c0[f] = uint32_t(nc);
-      for (uint64_t p : pages[f]) cap += standalone_chunk_size_guarantee(lbits, size_t(p));
-      nc += pages[f].size();
+      file_c0[f] = uint32_t(g.exact.size());
+      g.exact.insert(g.exact.end(), pages[f].begin(), pages[f].end());
       n += file_ns[f];
     }
+    const ChunksScratch cs = chunks_only_scratch(lbits, n, g.exact);
     g.out_at = out_scratch;
-    g.out_cap = cap;
+    g.out_cap = cs.bytes;
     g.idx_at = idx_scratch;
-    g.idx_cap = pco_b200_index_size_bound(size_t(n), size_t(nc)) + 64 * nc;
-    out_scratch += (cap + 15) & ~uint64_t(15);
+    g.idx_cap = cs.index;
+    out_scratch += (g.out_cap + 15) & ~uint64_t(15);
     idx_scratch += (g.idx_cap + 15) & ~uint64_t(15);
     gs.push_back(std::move(g));
   }
@@ -1780,8 +1728,7 @@ static PcoB200Error compress_files_impl(const void* nums, const uint64_t* file_n
   for (auto& kv : groups) {
     Group& g = gs[gi++];
     const std::vector<uint32_t>& fl = kv.second;
-    std::vector<uint64_t> exact;
-    for (uint32_t f : fl) exact.insert(exact.end(), pages[f].begin(), pages[f].end());
+    const std::vector<uint64_t>& exact = g.exact;
     PcoB200ChunkConfig cg = cfg;
     cg.paging_spec = PCO_B200_PAGING_EXACT;
     cg.exact_page_ns = exact.data();
@@ -3075,10 +3022,10 @@ PcoB200Error pco_b200_compress_async_plan(size_t n, unsigned char dtype, const P
   const AcompGeom g = acomp_geom(n, cfg.max_page_n);
   uint32_t bins_log = 0;
   if (n > 0) {
-    bins_log = choose_unoptimized_bins_log(cfg.compression_level, size_t(g.max_n));
+    bins_log = unoptimized_bins_log(cfg.compression_level, g.max_n, 0);
     if (bins_log > ENC_NARROW_BINS_LOG)
       return fail(PCO_B200_UNSUPPORTED, "more than 256 unoptimized bins (levels 9-12): the asynchronous compress runs the narrow kernels only");
-    if (g.rem != 0 && g.low > 0 && choose_unoptimized_bins_log(cfg.compression_level, size_t(g.low)) != bins_log)
+    if (g.rem != 0 && g.low > 0 && unoptimized_bins_log(cfg.compression_level, g.low, 0) != bins_log)
       return fail(PCO_B200_UNSUPPORTED, "the chunk sizes imply different unoptimized_bins_log (compress_ex encodes them in several runs)");
   }
   std::memset(plan, 0, sizeof(*plan));
@@ -3090,7 +3037,7 @@ PcoB200Error pco_b200_compress_async_plan(size_t n, unsigned char dtype, const P
   plan->max_page_n = cfg.max_page_n;
   plan->dst_cap = dst_cap;
   plan->index_cap = index_cap;
-  plan->index_bytes = acomp_index_bytes(g, plan->n_vars);
+  plan->index_bytes = equal_pages(n, cfg.max_page_n).index_bytes(plan->n_vars);
   plan->workspace_bytes = acomp_layout(g, nt_bits(dtype) / 8, plan->n_vars).total;
   if (index_cap != 0 && index_cap < plan->index_bytes)
     return fail(PCO_B200_IO, "index buffer too small (need " + std::to_string(plan->index_bytes) + " bytes)");
@@ -3164,7 +3111,7 @@ static PcoB200Error acf_plan_checks(unsigned char dtype, const PcoB200ChunkConfi
   if (PcoB200Error e = check_config(cfg, dtype, size_t(chunk_n), &ck)) return e;
   if (ck.auto_mode || ck.auto_delta)
     return fail(PCO_B200_UNSUPPORTED, "ModeSpec::Auto and DeltaSpec::Auto search on host threads: the asynchronous compress takes explicit specs only");
-  if (choose_unoptimized_bins_log(cfg.compression_level, size_t(chunk_n)) > ENC_NARROW_BINS_LOG)
+  if (unoptimized_bins_log(cfg.compression_level, chunk_n, 0) > ENC_NARROW_BINS_LOG)
     return fail(PCO_B200_UNSUPPORTED, "more than 256 unoptimized bins (levels 9-12): the asynchronous compress runs the narrow kernels only");
   const uint64_t max_chunks = uint64_t(nums_cap) / chunk_n + max_items;
   const uint64_t tiles = (chunk_n + SPLIT_TILE - 1) / SPLIT_TILE, bpc = n_batches_of(uint32_t(chunk_n));
@@ -3228,7 +3175,7 @@ static AcfArgs acf_args(const PcoB200AsyncCompressFilesPlan& p, const AcfPlanGeo
   fa.max_files = p.max_files;
   fa.max_file_n = p.max_file_n;
   fa.nums_cap = p.nums_cap;
-  fa.max_page_n = p.max_page_n == 0 ? (uint64_t(1) << 18) : p.max_page_n;
+  fa.max_page_n = p.max_page_n;
   fa.index_cap = index ? p.index_cap : 0;
   fa.uniform_type = p.uniform_type_header ? p.dtype : 0;
   fa.bpc = pg.g.bpc;
@@ -3258,8 +3205,7 @@ PcoB200Error pco_b200_compress_files_async(const PcoB200AsyncCompressFilesPlan* 
 }
 
 size_t pco_b200_debug_standalone_header(uint64_t n_hint, unsigned char uniform_type, unsigned char* out) {
-  const uint32_t len = standalone_header_into(n_hint, uniform_type, out);
-  return len == standalone_header_len(n_hint) ? len : 0;
+  return standalone_header_into(n_hint, uniform_type, out);
 }
 
 PcoB200Error pco_b200_compress_files_async_result(const PcoB200AsyncCompressFilesStatus* s, size_t* dst_len, size_t* index_len) {

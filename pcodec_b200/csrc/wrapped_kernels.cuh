@@ -34,7 +34,7 @@ struct MetaBits {
   const uint8_t* p;
   uint64_t avail;
   uint64_t pos;
-  __device__ uint64_t read(uint32_t nb) {
+  __host__ __device__ uint64_t read(uint32_t nb) {
     uint64_t v = 0;
     for (uint32_t i = 0; i < nb; i++) {
       const uint64_t bit = pos + i;
@@ -49,13 +49,17 @@ struct MetaBits {
 // chunk_latent_var.rs:102-143; format 4.x), for every mode and delta encoding: the same fields cold_decode_kernel reads, skipped
 // by their sizes.  *cold: the fast kernels decline the chunk (Dict, Lookback, Conv1, secondary_uses_delta, tables above 2^10 states
 // or 256 bins, FloatMult below 32 bits).  Only an unknown mode or delta variant makes the length undefined (ST_CORRUPTION); every
-// other defect is reported by the kernels that decode the chunk.
-__device__ inline uint32_t wrapped_meta_len(const uint8_t* p, uint64_t avail, uint32_t dtype, uint64_t* len, bool* cold) {
+// other defect is reported by the kernels that decode the chunk.  *mode and *variant, when asked for, are set as soon as they are read.
+// Bytes past avail read as 0, so a meta cut short parses to a length past avail.
+__host__ __device__ inline uint32_t wrapped_meta_len(const uint8_t* p, uint64_t avail, uint32_t dtype, uint64_t* len, bool* cold,
+                                                     uint32_t* mode = nullptr, uint32_t* variant = nullptr) {
   const uint32_t nb = nt_bits(dtype);
   MetaBits r{p, avail, 0};
   bool c = false;
   uint32_t n_vars = 1, prim_bits = nb;
-  switch (uint32_t(r.read(4))) {
+  const uint32_t m = uint32_t(r.read(4));
+  if (mode) *mode = m;
+  switch (m) {
     case MODE_CLASSIC: break;
     case MODE_INT_MULT: r.pos += nb; n_vars = 2; break;
     case MODE_FLOAT_MULT: r.pos += nb; n_vars = 2; c |= nb < 32; break;
@@ -70,22 +74,23 @@ __device__ inline uint32_t wrapped_meta_len(const uint8_t* p, uint64_t avail, ui
     }
     default: return ST_CORRUPTION;
   }
-  const uint32_t variant = uint32_t(r.read(4));
+  const uint32_t dv = uint32_t(r.read(4));
+  if (variant) *variant = dv;
   uint32_t lookback = 0;
-  if (variant == 1) {
+  if (dv == 1) {
     r.pos += 3;                               // order
     c |= r.read(1) != 0 && n_vars > 1;        // secondary_uses_delta
-  } else if (variant == 2) {
+  } else if (dv == 2) {
     r.pos += 5 + 4;                           // window_n_log - 1, state_n_log
     r.pos += 1;                               // secondary_uses_delta
     lookback = 1;
     c = true;
-  } else if (variant == 3) {
+  } else if (dv == 3) {
     r.pos += 5 + 64;                          // quantization, bias
     const uint32_t order = 1 + uint32_t(r.read(5));
     r.pos += 32ull * order;                   // weights
     c = true;
-  } else if (variant != 0) {
+  } else if (dv != 0) {
     return ST_CORRUPTION;
   }
   // latent vars: [lookback (32-bit latents)], primary, [secondary]
