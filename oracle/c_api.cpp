@@ -390,6 +390,7 @@ size_t pco_oracle_file_size_guarantee(size_t n, uint8_t dtype) {
 int pco_oracle_chunk_compressor_new(const void* nums, size_t n, uint8_t dtype, const pco_oracle_config* config, void** handle) {
   return guarded([&] {
     ChunkConfig cfg = to_config(config);
+    fallback_margins().clear();
     auto* h = new OracleChunkCompressor();
     h->bits = number_type_valid(dtype) ? number_type_bits(dtype) : 0;
     try {
@@ -562,6 +563,18 @@ int pco_oracle_kat_histogram_u64(const uint64_t* latents, size_t n, uint32_t n_b
 }
 // histograms.rs:250-258: heapsort fallbacks taken by every histogram built in this process so far
 uint64_t pco_oracle_heapsort_fallbacks(void) { return heapsort_fallbacks().load(std::memory_order_relaxed); }
+
+// chunk_compressor.rs:502-541: worst_case_size and baseline (bytes) of each chunk of this thread's last compress (a standalone
+// file from pco_oracle_simple_compress, or one wrapped chunk from pco_oracle_chunk_compressor_new), in chunk order; the chunk
+// fell back where worst > baseline.  Returns the chunk count, writes up to `cap`.
+size_t pco_oracle_last_fallback_margins(uint64_t* worst, uint64_t* baseline, size_t cap) {
+  const auto& m = fallback_margins();
+  for (size_t i = 0; i < m.size() && i < cap; i++) {
+    worst[i] = m[i].first;
+    baseline[i] = m[i].second;
+  }
+  return m.size();
+}
 // histograms.rs apply_sorted over several pre-sorted slices (tests :375-386)
 int pco_oracle_kat_histogram_sorted_u32(const uint32_t* latents, const size_t* slice_lens, size_t n_slices, size_t n, uint32_t n_bins_log,
                                         uint64_t* out, size_t* n_out, uint64_t* incomplete_out, int* has_incomplete) {

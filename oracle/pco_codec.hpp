@@ -934,6 +934,16 @@ struct PageInfoVar {
   size_t start = 0, end = 0;  // stored range in the var's latent array
 };
 
+// (worst_case_size, baseline) in bytes of each should_fallback decision of this thread's last compress, one per chunk in chunk
+// order.  Every compress clears it first: simple_compress (the standalone file of every caller, dictionary chunks included, and
+// each chunk of pco_oracle_bench_roundtrip) and pco_oracle_chunk_compressor_new (one wrapped chunk), so it never holds more than
+// one call's chunks.  Test infrastructure: the tests build chunks a byte either side of the size guarantee and check how far off
+// they are.
+inline std::vector<std::pair<uint64_t, uint64_t>>& fallback_margins() {
+  static thread_local std::vector<std::pair<uint64_t, uint64_t>> margins;
+  return margins;
+}
+
 template <typename L>  // L = number's latent type
 struct ChunkCompressor {
   ChunkMeta meta;
@@ -949,7 +959,6 @@ struct ChunkCompressor {
 
   // chunk_compressor.rs:502-541
   bool should_fallback(size_t n) const {
-    if (meta.delta.kind == DeltaKind::NoOp && meta.mode.kind == ModeKind::Classic) return false;
     size_t worst_case_body_bit_size = 7 * n_pages();
     auto add = [&](const LatentVarMeta& vm, const std::vector<Weight>& counts) {
       for (size_t i = 0; i < vm.bins.size() && i < counts.size(); i++) {
@@ -969,6 +978,8 @@ struct ChunkCompressor {
     base.primary.ans_size_log = 0;
     base.primary.bins = {Bin{1, 0, meta.number_bits}};
     size_t baseline = base.max_size() + (n * size_t(meta.number_bits) + 7) / 8;
+    fallback_margins().emplace_back(uint64_t(worst_case_size), uint64_t(baseline));
+    if (meta.delta.kind == DeltaKind::NoOp && meta.mode.kind == ModeKind::Classic) return false;  // already the fallback's layout
     return worst_case_size > baseline;
   }
 
@@ -1975,6 +1986,7 @@ inline void write_standalone_dict_chunk(const L* nums, size_t n, uint8_t number_
 template <typename L>
 inline void simple_compress(const L* nums, size_t n, uint8_t number_type, const ChunkConfig& config, bool uniform_type,
                             std::vector<uint8_t>& dst) {
+  fallback_margins().clear();
   write_standalone_header(dst, n, uniform_type ? number_type : 0);
   std::vector<size_t> chunks = n_per_page(config, n);
   size_t start = 0;

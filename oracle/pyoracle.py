@@ -172,6 +172,18 @@ def file_size_guarantee(n, dtype):
     return lib().pco_oracle_file_size_guarantee(n, NP_TO_BYTE[np.dtype(dtype)])
 
 
+def last_fallback_margins():
+    """[(worst_case_size, baseline)] in bytes for each chunk of this thread's last simple_compress or ChunkCompressor, in chunk
+    order (chunk_compressor.rs:502-541): the chunk fell back to Classic / NoOp where worst_case_size > baseline."""
+    f = lib().pco_oracle_last_fallback_margins
+    f.restype = C.c_size_t
+    f.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+    n = f(None, None, 0)
+    worst, base = np.zeros(n, dtype=np.uint64), np.zeros(n, dtype=np.uint64)
+    f(worst.ctypes.data_as(C.c_void_p), base.ctypes.data_as(C.c_void_p), n)
+    return [(int(w), int(b)) for w, b in zip(worst, base)]
+
+
 def inspect(data, dtype):
     dt = NP_TO_BYTE[np.dtype(dtype)]
     out = C.c_void_p()

@@ -152,16 +152,20 @@ __device__ __forceinline__ uint32_t int_float_to_latent_bits(uint32_t fbits) {
   return (fbits & MID) ? (MID - 1 - abs_int) : (MID + abs_int);
 }
 
-// float_mult split of one number (pco/src/mode/float_mult.rs:38-60).  NaN operands follow the CPU rule
-// (operand NaN propagates quieted), see float_mult_unadjusted in decode_kernels.cuh.
+// float_mult split of one number (pco/src/mode/float_mult.rs:38-60).  NaNs follow the x86 rules the reference runs under,
+// see float_mult_unadjusted in decode_kernels.cuh: an operand NaN propagates quieted, and a NaN the multiply produces is
+// x86's default NaN (sign set, quiet, zero payload).  Only ±0 * inv_base produces one, when a subnormal base (at most
+// 2^-1024 for f64, 2^-128 for f32) makes inv_base +inf.  The f32 multiply on the GPU returns the canonical NaN 0x7FFFFFFF
+// there (sign clear), which moved every zero's primary latent and adjustment; the f64 one gave x86's bits on an H100, and
+// the rule is stated for both so neither depends on it.
 __device__ __forceinline__ void float_mult_split(uint64_t xbits, uint64_t base_bits, uint64_t inv_bits, uint64_t& primary, uint64_t& secondary) {
-  const uint64_t MID = uint64_t(1) << 63, QUIET = 0x0008000000000000ull;
+  const uint64_t MID = uint64_t(1) << 63, QUIET = 0x0008000000000000ull, X86_DEFAULT_NAN = 0xFFF8000000000000ull;
   double x = __longlong_as_double((long long)xbits);
   uint64_t mult_bits;
   if (x != x) mult_bits = xbits | QUIET;
   else {
     double q = __dmul_rn(x, __longlong_as_double((long long)inv_bits));
-    mult_bits = (uint64_t)__double_as_longlong(round(q));  // round half away from zero
+    mult_bits = q != q ? X86_DEFAULT_NAN : (uint64_t)__double_as_longlong(round(q));  // round half away from zero
   }
   primary = int_float_to_latent_bits(mult_bits);
   double mult = __longlong_as_double((long long)mult_bits);
@@ -171,13 +175,13 @@ __device__ __forceinline__ void float_mult_split(uint64_t xbits, uint64_t base_b
   secondary = (a - b) + MID;
 }
 __device__ __forceinline__ void float_mult_split(uint32_t xbits, uint32_t base_bits, uint32_t inv_bits, uint32_t& primary, uint32_t& secondary) {
-  const uint32_t MID = 1u << 31, QUIET = 0x00400000u;
+  const uint32_t MID = 1u << 31, QUIET = 0x00400000u, X86_DEFAULT_NAN = 0xFFC00000u;
   float x = __uint_as_float(xbits);
   uint32_t mult_bits;
   if (x != x) mult_bits = xbits | QUIET;
   else {
     float q = __fmul_rn(x, __uint_as_float(inv_bits));
-    mult_bits = __float_as_uint(roundf(q));
+    mult_bits = q != q ? X86_DEFAULT_NAN : __float_as_uint(roundf(q));  // see the f64 overload
   }
   primary = int_float_to_latent_bits(mult_bits);
   float mult = __uint_as_float(mult_bits);
