@@ -405,6 +405,63 @@ PcoB200Error pco_b200_decompress_async(const PcoB200AsyncPlan *plan, const void 
  * sets the last-error message ("chunk 17: ...") and, when the kind is OK, fills *progress (may be NULL). */
 PcoB200Error pco_b200_decompress_async_result(const PcoB200AsyncStatus *host_status, PcoB200Progress *progress);
 
+/* ---- asynchronous side index of a standalone file (no reference counterpart): pco_b200_build_index on the caller's stream, for files
+ * without an index - those pco itself writes - so that "build the index, then pco_b200_decompress_async" can be queued behind other GPU
+ * work or captured in one CUDA graph.  The call only enqueues kernels and returns at once; it makes no synchronising, allocating or
+ * host-to-device copy call and refers to no memory of the library's per-thread scratch.  The file length is read from device memory,
+ * so one plan (and one captured graph) indexes a different file of the same number type and header flavour on each call.  Chunks are
+ * found as the index-free decompress finds them (DESIGN.md): every position that carries the chunk pattern at the cursor is walked at
+ * once, the chain of real chunks is followed on the device, in two such rounds (a file pco pages with EqualPagesUpTo has chunks of at
+ * most two sizes), and one serial walk indexes what the rounds leave. */
+typedef struct PcoB200AsyncIndexPlan {  /* filled by pco_b200_build_index_async_plan; treat as opaque */
+  uint32_t dtype, uniform_type, format_major, reserved;
+  uint64_t src_cap, index_cap, max_chunks;
+  uint64_t workspace_bytes;             /* device workspace one in-flight call needs */
+} PcoB200AsyncIndexPlan;
+
+typedef struct PcoB200AsyncIndexStatus {  /* written on the device by every call */
+  uint32_t kind;                          /* PcoB200Error */
+  uint32_t device_status;                 /* the device word behind it: a chunk's PcoB200Error kind, or PCO_B200_ASYNC_* */
+  uint64_t chunk;                         /* failing chunk (UINT64_MAX if none) */
+  uint64_t n_chunks, n_total;             /* chunks indexed and their numbers (on TOO_MANY_CHUNKS: max_chunks + 1) */
+  uint64_t index_bytes;                   /* bytes written to index (0 unless OK) */
+  uint64_t serial_chunks;                 /* chunks the serial walker indexed; the rest came from the speculative rounds */
+} PcoB200AsyncIndexStatus;
+
+/* Makes a plan.  `head` holds the first bytes of a standalone file in host memory (as pco_b200_decompress_async_plan); src_cap and
+ * index_cap are the byte sizes of the file and index buffers every call will pass, max_chunks bounds the chunks of any file indexed with
+ * the plan.  Checked before the device is touched, with the kinds of pco_b200_decompress_async_plan: dtype, the header, the uniform type;
+ * then max_chunks in 1 .. 2^31 - 9 and src_cap at most (2^31 - 1) x 4096 bytes, so that every grid of a call (one CTA per candidate chunk,
+ * one per 4096 bytes of src_cap) is one the runtime launches (PCO_B200_INVALID_ARGUMENT).  Then *plan is filled and the one-time device
+ * set-up runs on the current device, which the calls must use; without a device that is PCO_B200_CUDA.  workspace_bytes is, with each
+ * term rounded up to a multiple of 256,
+ *   256 + 8 * ceil(src_cap / 4096) + 52 * (max_chunks + 8) (4 terms) + 40 * (max_chunks + 1) (2 terms) + 2 * index_cap + index_cap
+ * (the call's state, find counts, candidates, chunk records, the arena the speculative walks write entries into, and the region of the
+ * serial walker's entries). */
+PcoB200Error pco_b200_build_index_async_plan(const void *head, size_t head_len, unsigned char dtype, size_t src_cap,
+                                             size_t index_cap, size_t max_chunks, PcoB200AsyncIndexPlan *plan);
+/* Enqueues the indexing of the file of *src_len bytes (a device word, at most src_cap) in `src` into `index` on `cuda_stream`, and the
+ * outcome into *status; returns without waiting.  src, src_len, index (16-byte aligned), workspace (plan->workspace_bytes, 256-byte
+ * aligned) and status are device pointers; one workspace serves one call in flight.  The index is the one pco_b200_compress_ex writes for
+ * the same chunks: header (file_len = *src_len, end_byte the byte behind the terminator), exactly n_chunks records, then each chunk's
+ * entries at the next 16-byte boundary with the padding zeroed; index_bytes of it are written, and nothing unless the kind is OK.  Reads
+ * stay inside *src_len bytes of src.  Outcomes, as pco_b200_build_index reports them where it has one:
+ *   - a header that does not parse or differs from the plan's flavour: PCO_B200_ASYNC_HEADER_* (as pco_b200_decompress_async);
+ *   - *src_len above src_cap: PCO_B200_ASYNC_FILE_OUTSIDE (PCO_B200_INVALID_ARGUMENT);
+ *   - more than max_chunks chunks: PCO_B200_ASYNC_TOO_MANY_CHUNKS (PCO_B200_INVALID_ARGUMENT);
+ *   - an index larger than index_cap: PCO_B200_ASYNC_FILES_INDEX_FULL (PCO_B200_IO); of these two, the one the walk meets first in file
+ *     order is reported;
+ *   - a chunk that is corrupt, truncated or that the walker declines (Lookback, Dict, Conv1, tables above 2^12 states): its kind and
+ *     `chunk`, as pco_b200_build_index.
+ * The return value covers the host side only: null pointers, an unaligned workspace or index, or a plan that was not filled
+ * (PCO_B200_INVALID_ARGUMENT), a launch the runtime refuses (PCO_B200_CUDA).  With pco_b200_profile_enable(1), a call outside a stream
+ * capture records its kernel spans for pco_b200_profile_last; a call inside a capture records none. */
+PcoB200Error pco_b200_build_index_async(const PcoB200AsyncIndexPlan *plan, const void *src, const uint64_t *src_len, void *index,
+                                        void *workspace, PcoB200AsyncIndexStatus *status, void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory at a point of the caller's choosing.  Returns the kind,
+ * sets the last-error message ("chunk 17: ...") and, when the kind is OK, sets *index_len (may be NULL) to the index's bytes. */
+PcoB200Error pco_b200_build_index_async_result(const PcoB200AsyncIndexStatus *host_status, size_t *index_len);
+
 /* ---- asynchronous compress (no reference counterpart): the other half of pco_b200_decompress_async.  The call only enqueues kernels on
  * the caller's stream and returns at once; it makes no synchronising, allocating or host-to-device copy call and refers to no memory of
  * the library's per-thread scratch, so it can be queued behind other GPU work and captured in a CUDA graph, and a captured call may be

@@ -93,8 +93,9 @@ __device__ __forceinline__ uint64_t async_ld_u64(const uint8_t* p) {  // any ali
 }
 
 // parse_standalone_header (host_common.hpp) on the device, over the first bytes of a file of `file_len` bytes: ST_OK, or the refusal
-// that gives the kind the host parse gives.
-__device__ inline uint32_t async_parse_header(const uint8_t* b, uint64_t file_len, uint32_t* uniform_type, uint32_t* format_major) {
+// that gives the kind the host parse gives.  On ST_OK, *first_chunk_byte (when given) is where the first chunk starts.
+__device__ inline uint32_t async_parse_header(const uint8_t* b, uint64_t file_len, uint32_t* uniform_type, uint32_t* format_major,
+                                              uint64_t* first_chunk_byte = nullptr) {
   auto byte_at = [&](uint64_t i) -> uint32_t { return i < file_len ? b[i] : 0u; };
   if (file_len < 4) return PCO_B200_ASYNC_HEADER_SHORT;
   if (b[0] != 112 || b[1] != 99 || b[2] != 111 || b[3] != 33) return PCO_B200_ASYNC_HEADER_CORRUPT;  // "pco!"
@@ -128,6 +129,7 @@ __device__ inline uint32_t async_parse_header(const uint8_t* b, uint64_t file_le
   if (pos > file_len) return PCO_B200_ASYNC_HEADER_SHORT;
   *uniform_type = uniform;
   *format_major = major;
+  if (first_chunk_byte) *first_chunk_byte = pos;
   return ST_OK;
 }
 

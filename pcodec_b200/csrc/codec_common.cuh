@@ -107,6 +107,43 @@ __host__ __device__ inline EqualPages equal_pages(uint64_t n, uint64_t max_page_
   return p;
 }
 
+// The chain of real chunks among the candidates of a speculative walk of one index-free file: the host's rounds (follow_chunk_chain,
+// host_common.hpp) and the device's (ai_chain_kernel, async_index_kernels.cuh).  `cand` (sorted, m entries) are the positions that look
+// like a chunk start of `n0` numbers, `st` / `ends` what walking each of them as a chunk gave (status, first byte behind it).  Starting
+// from `pos` - a real chunk start - the chunk at p is real, and the next real chunk starts where it ends: follow that for as long as the
+// end is on the list, the walk succeeded, made progress and stayed inside the file (which ends at `src_len`), and the cap (`dst_len`
+// units, `out_off` of them taken, `n0` per chunk) has room for another chunk.  take(k) gets the index (into cand) of each verified chunk
+// in file order; returns their count and leaves the position behind the last one in *next_pos.  A candidate that no verified chunk ends
+// on is a coincidence and is never reached.
+#pragma nv_exec_check_disable
+template <typename Take>
+__host__ __device__ inline uint64_t chunk_chain(const uint64_t* cand, const uint32_t* st, const uint64_t* ends, uint32_t m, uint64_t pos, uint64_t n0,
+                                                uint64_t out_off, uint64_t dst_len, uint64_t src_len, uint64_t* next_pos, Take take) {
+  uint64_t p = pos, taken = 0;
+  uint32_t lo = 0;  // the chain only moves forward: the lower bound of p is searched behind the last chunk taken, galloping
+  for (;;) {
+    uint32_t hi = lo, step = 1;
+    while (hi < m && cand[hi] < p) {
+      lo = hi + 1;
+      hi = m - lo > step ? lo + step : m;
+      step <<= 1;
+    }
+    while (lo < hi) {
+      const uint32_t mid = lo + (hi - lo) / 2;
+      if (cand[mid] < p) lo = mid + 1; else hi = mid;
+    }
+    if (lo == m || cand[lo] != p) break;
+    if (st[lo] != ST_OK || ends[lo] <= p || ends[lo] > src_len) break;  // the serial walker reports what is wrong with this chunk
+    if (out_off + (taken + 1) * n0 > dst_len) break;
+    take(lo);
+    taken++;
+    p = ends[lo];
+    lo++;
+  }
+  *next_pos = p;
+  return taken;
+}
+
 // unoptimized_bins_log of var v of a chunk of n >= 1 numbers at compression level `level` (pco/src/wrapped/chunk_compressor.rs:362-371;
 // the secondary var takes at most 6, LIMITED_UNOPTIMIZED_BINS_LOG, :238-248).
 __host__ __device__ __forceinline__ uint32_t unoptimized_bins_log(uint32_t level, uint64_t n, int v) {

@@ -8,6 +8,7 @@
 #include "async_compress_files.cuh"
 #include "async_compress_wrapped.cuh"
 #include "async_files_kernels.cuh"
+#include "async_index_kernels.cuh"
 #include "async_kernels.cuh"
 #include "async_pages_kernels.cuh"
 #include "async_ranges_kernels.cuh"
@@ -3367,6 +3368,134 @@ PcoB200Error pco_b200_build_index(const void* compressed, size_t compressed_len,
   }
   if (index_len) *index_len = used;
   return PCO_B200_OK;
+}
+
+// ---- asynchronous side index of a standalone file (pco_b200_build_index_async; kernels in async_index_kernels.cuh)
+// The plan fixes what the launches take by value and every grid size (from src_cap and max_chunks); the file's length comes from the
+// device.  A call is a fixed sequence of launches: head, two rounds of seven, serial, place, copy, finish.
+
+// Every grid of a call stays within 2^31 - 1 CTAs: the candidate walks launch max_chunks + AI_SPARE_CANDS, the find grid one CTA per
+// AI_FIND_SPAN bytes of src_cap.
+constexpr uint64_t AI_MAX_CHUNKS = 0x7fffffffull - AI_SPARE_CANDS;
+constexpr uint64_t AI_MAX_SRC_CAP = 0x7fffffffull * AI_FIND_SPAN;
+
+static bool ai_plan_ok(const PcoB200AsyncIndexPlan* p) {
+  return nt_valid(p->dtype) && p->max_chunks >= 1 && p->max_chunks <= AI_MAX_CHUNKS && p->src_cap <= AI_MAX_SRC_CAP &&
+         p->workspace_bytes == ai_layout(p->src_cap, p->index_cap, p->max_chunks).total;
+}
+
+PcoB200Error pco_b200_build_index_async_plan(const void* head, size_t head_len, unsigned char dtype, size_t src_cap, size_t index_cap, size_t max_chunks,
+                                             PcoB200AsyncIndexPlan* plan) {
+  StandaloneHeader hdr;
+  if (PcoB200Error e = check_async_head(head, head_len, dtype, plan, &hdr)) return e;
+  if (max_chunks == 0 || uint64_t(max_chunks) > AI_MAX_CHUNKS) return fail(PCO_B200_INVALID_ARGUMENT, "max_chunks must be 1 .. 2^31 - 9");
+  if (uint64_t(src_cap) > AI_MAX_SRC_CAP) return fail(PCO_B200_INVALID_ARGUMENT, "src_cap above (2^31 - 1) x 4096 bytes");
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->uniform_type = hdr.uniform_type;
+  plan->format_major = hdr.format_major;
+  plan->src_cap = src_cap;
+  plan->index_cap = index_cap;
+  plan->max_chunks = max_chunks;
+  plan->workspace_bytes = ai_layout(src_cap, index_cap, max_chunks).total;
+  Context& c = ctx();
+  if (PcoB200Error e = ensure_device(c)) return e;
+  PCOB_CUDA_TRY(cudaFuncSetAttribute(ai_walk_kernel<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WalkSmem<12>)));
+  PCOB_CUDA_TRY(cudaFuncSetAttribute(ai_serial_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WalkSmem<12>)));
+  return load_kernels({(const void*)ai_head_kernel, (const void*)ai_round_kernel, (const void*)ai_count_kernel, (const void*)ai_scan_kernel,
+                       (const void*)ai_scatter_kernel, (const void*)ai_walk_kernel<SMALL_MAX_SIZE_LOG>, (const void*)ai_walk_kernel<12>,
+                       (const void*)ai_chain_kernel, (const void*)ai_serial_kernel, (const void*)ai_place_kernel, (const void*)ai_copy_kernel,
+                       (const void*)ai_finish_kernel});
+}
+
+PcoB200Error pco_b200_build_index_async(const PcoB200AsyncIndexPlan* plan, const void* src, const uint64_t* src_len, void* index, void* workspace,
+                                        PcoB200AsyncIndexStatus* status, void* cuda_stream) {
+  if (!plan || !src || !src_len || !index || !workspace || !status) return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (!ai_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_build_index_async_plan");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  if (reinterpret_cast<uintptr_t>(index) & 15) return fail(PCO_B200_INVALID_ARGUMENT, "the index is not 16-byte aligned");
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+  const cudaStream_t stream = ln.stream;
+
+  const AiLayout lay = ai_layout(plan->src_cap, plan->index_cap, plan->max_chunks);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  AiState* state = reinterpret_cast<AiState*>(ws);
+  uint64_t* parts = reinterpret_cast<uint64_t*>(ws + lay.parts);
+  AiArgs g;
+  g.src = static_cast<const uint8_t*>(src);
+  g.src_len = src_len;
+  g.index = static_cast<uint8_t*>(index);
+  g.ws = ws;
+  g.src_cap = plan->src_cap;
+  g.index_cap = plan->index_cap;
+  g.max_chunks = plan->max_chunks;
+  g.dtype = plan->dtype;
+  g.uniform_type = plan->uniform_type;
+  g.format_major = plan->format_major;
+  const uint32_t find = uint32_t(ai_find_ctas(plan->src_cap));
+  const uint32_t cands = uint32_t(plan->max_chunks + AI_SPARE_CANDS), chunks = uint32_t(plan->max_chunks + 1);
+
+  ln.begin("ai_head_kernel");
+  ai_head_kernel<<<1, 1, 0, stream>>>(g, state);
+  ln.end();
+  for (int round = 0; round < AI_ROUNDS; round++) {
+    ln.begin("ai_round_kernel");
+    ai_round_kernel<<<1, 1, 0, stream>>>(g, state);
+    ln.end();
+    ln.begin("ai_count_kernel");
+    ai_count_kernel<<<find, AI_THREADS, 0, stream>>>(g, state, parts);
+    ln.end();
+    ln.begin("ai_scan_kernel");
+    ai_scan_kernel<<<1, AI_SCAN_THREADS, 0, stream>>>(g, state, parts);
+    ln.end();
+    ln.begin("ai_scatter_kernel");
+    ai_scatter_kernel<<<find, AI_THREADS, 0, stream>>>(g, state, parts, reinterpret_cast<uint64_t*>(ws + lay.cand), reinterpret_cast<IndexChunk*>(ws + lay.crec));
+    ln.end();
+    ln.begin("ai_walk_kernel<10>");
+    ai_walk_kernel<SMALL_MAX_SIZE_LOG><<<cands, WALK_THREADS, sizeof(WalkSmem<SMALL_MAX_SIZE_LOG>), stream>>>(
+        g, state, reinterpret_cast<uint32_t*>(ws + lay.cst), reinterpret_cast<uint64_t*>(ws + lay.cend));
+    ln.end();
+    ln.begin("ai_walk_kernel<12>");
+    ai_walk_kernel<12><<<cands, WALK_THREADS, sizeof(WalkSmem<12>), stream>>>(g, state, reinterpret_cast<uint32_t*>(ws + lay.cst),
+                                                                              reinterpret_cast<uint64_t*>(ws + lay.cend));
+    ln.end();
+    ln.begin("ai_chain_kernel");
+    ai_chain_kernel<<<1, AI_THREADS, 0, stream>>>(g, state);
+    ln.end();
+  }
+  ln.begin("ai_serial_kernel");
+  ai_serial_kernel<<<1, WALK_THREADS, sizeof(WalkSmem<12>), stream>>>(g, state);
+  ln.end();
+  ln.begin("ai_place_kernel");
+  ai_place_kernel<<<1, AI_SCAN_THREADS, 0, stream>>>(g, state);
+  ln.end();
+  ln.begin("ai_copy_kernel");
+  ai_copy_kernel<<<chunks, AI_THREADS, 0, stream>>>(g, state);
+  ln.end();
+  ln.begin("ai_finish_kernel");
+  ai_finish_kernel<<<1, 1, 0, stream>>>(g, state, status);
+  ln.end();
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
+}
+
+PcoB200Error pco_b200_build_index_async_result(const PcoB200AsyncIndexStatus* s, size_t* index_len) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200Error kind = async_result_kind(s->kind);
+  if (kind == PCO_B200_OK) {
+    if (index_len) *index_len = size_t(s->index_bytes);
+    return PCO_B200_OK;
+  }
+  if (const char* h = async_header_refusal(s->device_status)) return fail(kind, h);
+  switch (s->device_status) {
+    case PCO_B200_ASYNC_FILE_OUTSIDE: return fail(kind, "the file length *src_len exceeds the plan's src_cap");
+    case PCO_B200_ASYNC_TOO_MANY_CHUNKS: return fail(kind, "the file has more chunks than the plan's max_chunks");
+    case PCO_B200_ASYNC_FILES_INDEX_FULL: return fail(kind, "index buffer too small: the side index needs more than the plan's index_cap bytes");
+    default:
+      status_to_error(s->device_status, "this chunk");
+      return fail(kind, "chunk " + std::to_string(s->chunk) + ": " + last_error_ref());
+  }
 }
 
 // ---------------------------------------------------------------------------

@@ -285,30 +285,11 @@ inline void* mapped_host_ptr(const void* host) {
 }
 
 // ---- the chain of real chunks among the candidates of a speculative walk (host_api.cu speculative_walk_rounds) ---------------------
-// One index-free file, of a one-file call or of a batch.  `cand` (sorted, m entries) are the positions that look like a chunk start of
-// `n0` numbers, `st` / `ends` what walking each of them as a chunk gave (status, first byte behind it).  Starting from `pos` - a real
-// chunk start - the chunk at p is real, and the next real chunk starts where it ends: follow that for as long as the end is on the list,
-// the walk succeeded, made progress and stayed inside the file (which ends at `src_len`), and the file's cap (`dst_len` numbers, the
-// destination of a one-file call, ~0 in a batch; `out_off` of them taken) has room for another `n0`.  Returns the indices (into cand)
-// of the verified chunks in file order and leaves the position behind the last one in *next_pos.  A candidate that no verified chunk
-// ends on is a coincidence and is never reached.
+// chunk_chain (codec_common.cuh) with the verified chunks' indices collected in file order.
 inline std::vector<uint32_t> follow_chunk_chain(const uint64_t* cand, const uint32_t* st, const uint64_t* ends, uint32_t m, uint64_t pos, uint64_t n0,
                                                 uint64_t out_off, uint64_t dst_len, uint64_t src_len, uint64_t* next_pos) {
   std::vector<uint32_t> real;
-  uint64_t p = pos;
-  for (;;) {
-    uint32_t lo = 0, hi = m;  // lower bound of p in cand
-    while (lo < hi) {
-      const uint32_t mid = lo + (hi - lo) / 2;
-      if (cand[mid] < p) lo = mid + 1; else hi = mid;
-    }
-    if (lo == m || cand[lo] != p) break;
-    if (st[lo] != ST_OK || ends[lo] <= p || ends[lo] > src_len) break;  // the serial walker reports what is wrong with this chunk
-    if (out_off + (uint64_t(real.size()) + 1) * n0 > dst_len) break;
-    real.push_back(lo);
-    p = ends[lo];
-  }
-  *next_pos = p;
+  chunk_chain(cand, st, ends, m, pos, n0, out_off, dst_len, src_len, next_pos, [&](uint32_t k) { real.push_back(k); });
   return real;
 }
 

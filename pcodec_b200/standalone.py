@@ -448,6 +448,68 @@ class AsyncDecompressor(_lib._AsyncCall):
         return Progress(prog.n_processed, bool(prog.finished))
 
 
+class _CAsyncIndexPlan(C.Structure):  # PcoB200AsyncIndexPlan (include/pco_b200.h)
+    _fields_ = [("dtype", C.c_uint32), ("uniform_type", C.c_uint32), ("format_major", C.c_uint32), ("reserved", C.c_uint32),
+                ("src_cap", C.c_uint64), ("index_cap", C.c_uint64), ("max_chunks", C.c_uint64), ("workspace_bytes", C.c_uint64)]
+
+
+class _CAsyncIndexStatus(C.Structure):  # PcoB200AsyncIndexStatus (include/pco_b200.h)
+    _fields_ = [("kind", C.c_uint32), ("device_status", C.c_uint32), ("chunk", C.c_uint64), ("n_chunks", C.c_uint64), ("n_total", C.c_uint64),
+                ("index_bytes", C.c_uint64), ("serial_chunks", C.c_uint64)]
+
+
+def _lib_async_index():
+    return _lib.bind("_async_index_ready",
+                     pco_b200_build_index_async_plan=[C.c_void_p, C.c_size_t, C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p],
+                     pco_b200_build_index_async=[C.c_void_p] * 7,
+                     pco_b200_build_index_async_result=[C.c_void_p, C.POINTER(C.c_size_t)])
+
+
+class AsyncIndexBuilder(_lib._AsyncCall):
+    """Builds the side index of a standalone file without one (as pco writes them) on the current CUDA stream without waiting for the
+    device (pco_b200_build_index_async): a file loaded into device memory can be indexed behind other GPU work, and "build the index, then
+    AsyncDecompressor" can be captured in one torch.cuda.CUDAGraph.
+
+    The plan comes from `head`, the first bytes of a file (as AsyncDecompressor).  src_cap and index_cap (bytes) are the sizes of the
+    buffers every call passes, max_chunks the most chunks a file may have.  The file length is read from a device tensor, so one captured
+    call indexes a different file on each replay.  The builder owns a device workspace and a status; it serves one call in flight."""
+
+    _Plan, _Status = _CAsyncIndexPlan, _CAsyncIndexStatus
+
+    def __init__(self, head, dtype, src_cap, index_cap, max_chunks, device=None):
+        self.dtype = np.dtype(dtype)
+        h = self._head(head)
+        self._make_plan(device, lambda plan: _lib_async_index().pco_b200_build_index_async_plan(
+            h.ctypes.data_as(C.c_void_p), C.c_size_t(h.size), C.c_ubyte(_lib.dtype_byte(self.dtype)), C.c_size_t(src_cap), C.c_size_t(index_cap),
+            C.c_size_t(max_chunks), plan))
+        self._alloc()
+
+    def __call__(self, src, src_len, index):
+        """Enqueues the indexing of the file of src_len[0] bytes in `src` (uint8 CUDA tensor of at least src_cap bytes) into `index` (a
+        16-byte aligned uint8 CUDA tensor of at least index_cap bytes) on torch.cuda.current_stream(); `src_len` is a 1-element int64 CUDA
+        tensor.  Returns nothing and does not wait; result() reports the outcome."""
+        import torch
+
+        p = self._plan
+        self._check_tensors(src=src, src_len=src_len, index=index)
+        if src.numel() * src.element_size() < p.src_cap or index.numel() * index.element_size() < p.index_cap:
+            raise ValueError(f"src holds fewer than src_cap = {p.src_cap} bytes, or index fewer than index_cap = {p.index_cap}")
+        if src_len.dtype != torch.int64 or src_len.numel() != 1:
+            raise ValueError("src_len must be a 1-element int64 tensor")
+        rc = _lib_async_index().pco_b200_build_index_async(C.byref(p), C.c_void_p(src.data_ptr()), C.c_void_p(src_len.data_ptr()),
+                                                           C.c_void_p(index.data_ptr()), C.c_void_p(self.workspace.data_ptr()),
+                                                           C.c_void_p(self.status.data_ptr()), self._stream())
+        _lib.check(rc)
+
+    def result(self):
+        """Copies the status of the last call back (waiting for it on the current stream) and returns the index length in bytes, or raises
+        PcoError with the kind build_index gives ("chunk 17: ...")."""
+        s = self.status_record()
+        n = C.c_size_t()
+        _lib.check(_lib_async_index().pco_b200_build_index_async_result(C.byref(s), C.byref(n)))
+        return int(n.value)
+
+
 class _CAsyncRangesPlan(C.Structure):  # PcoB200AsyncRangesPlan (include/pco_b200.h)
     _fields_ = [("dtype", C.c_uint32), ("uniform_type", C.c_uint32), ("format_major", C.c_uint32), ("reserved", C.c_uint32),
                 ("src_cap", C.c_uint64), ("index_cap", C.c_uint64), ("max_chunks", C.c_uint64), ("max_ranges", C.c_uint64),
