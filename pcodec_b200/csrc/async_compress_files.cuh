@@ -25,7 +25,8 @@
 // writes nothing but the status; a batch that does not fit writes `files` and the status only, as pco_b200_compress_files does.
 #pragma once
 #include "async_compress.cuh"
-#include "async_ranges_kernels.cuh"  // ArSum and its block scan
+#include "async_kernels.cuh"  // async_kind_of
+#include "cta_scan.cuh"
 
 namespace pcob200 {
 
@@ -35,7 +36,7 @@ constexpr int ACF_INDEX_THREADS = 128;
 enum { ACF_NUMS = 0, ACF_CHUNKS, ACF_ROWS, ACF_FRAME, ACF_IDX, ACF_SUMS };
 
 struct AcfPart {  // per CTA of acf_files_kernel: the CTA's sums, then (acf_scan_kernel) the sums of the CTAs before it
-  ArSum s[ACF_SUMS];
+  CarrySum s[ACF_SUMS];
 };
 struct AcfFile {  // per file, by acf_place_kernel: where its numbers, chunks, rows, frame bytes and index start
   uint64_t n, first[ACF_SUMS], hdr_len;
@@ -45,10 +46,10 @@ struct AcfState {
   uint32_t fits;        // acf_bytes_scan_kernel: the batch fits dst_cap and index_cap
   uint64_t n_read;      // *n_files as read
   uint64_t n_files;     // the files the call runs over (0 when *n_files is above max_files)
-  unsigned long long bad;  // (file << 32) | status: the lowest file refusal (AR_NONE64: none)
+  unsigned long long bad;  // (file << 32) | status: the lowest file refusal (NONE64: none)
   uint64_t live_chunks; // chunks of the batch, 0 when refused
   uint64_t dst_bytes, index_bytes;  // what the batch needs (index_bytes 0 without an index)
-  ArSum total[ACF_SUMS];
+  CarrySum total[ACF_SUMS];
 };
 
 static_assert(sizeof(AcfState) == 136 && sizeof(AcfFile) == 56 && sizeof(AcfPart) == 80, "the workspace formula in pco_b200.h");
@@ -59,7 +60,6 @@ struct AcfLayout {
   AcompLayout enc;
   uint64_t state, files, parts, cfile, cparts, pre, total;
 };
-__host__ __device__ inline uint64_t acf_ctas(uint64_t n) { return (n + ACF_THREADS - 1) / ACF_THREADS; }
 inline AcompGeom acf_enc_geom(uint64_t max_chunks, uint64_t chunk_n, uint64_t nums_cap) {
   AcompGeom g = {};
   g.n_chunks = max_chunks;
@@ -76,9 +76,9 @@ inline AcfLayout acf_layout(const AcompGeom& g, uint32_t lbytes, uint32_t n_vars
   auto take = [&](uint64_t bytes) { const uint64_t o = at; at += acomp_align(bytes); return o; };
   l.state = take(sizeof(AcfState));
   l.files = take(max_files * sizeof(AcfFile));
-  l.parts = take(acf_ctas(max_files) * sizeof(AcfPart));
+  l.parts = take(ctas_of<ACF_THREADS>(max_files) * sizeof(AcfPart));
   l.cfile = take(g.n_chunks * 4);
-  l.cparts = take(acf_ctas(g.n_chunks + 1) * 8);
+  l.cparts = take(ctas_of<ACF_THREADS>(g.n_chunks + 1) * 8);
   l.pre = take((g.n_chunks + 1) * 8);
   l.total = at;
   return l;
@@ -102,15 +102,15 @@ __device__ __forceinline__ AcfPart* acf_parts(const AcfArgs& g) { return reinter
 
 // The sizes of file slot f (zeros past the batch): its count for the nums_cap check, and the rest from its count clamped to max_file_n
 // (a file above it refuses the batch, so its other sums only have to stay finite).
-__device__ __forceinline__ void acf_file_sums(const AcfArgs& g, uint64_t f, uint64_t nf, ArSum* s, uint64_t* n_out) {
+__device__ __forceinline__ void acf_file_sums(const AcfArgs& g, uint64_t f, uint64_t nf, CarrySum* s, uint64_t* n_out) {
   const uint64_t n = f < nf ? g.file_ns[f] : 0;
   const uint64_t nn = min(n, g.max_file_n);
   const EqualPages fp = equal_pages(nn, g.max_page_n);
-  s[ACF_NUMS] = ar_sum(n);
-  s[ACF_CHUNKS] = ar_sum(fp.n_chunks);
-  s[ACF_ROWS] = ar_sum(fp.row_start(fp.n_chunks));
-  s[ACF_FRAME] = ar_sum(f < nf && g.framed ? standalone_header_len(nn) + 1 : 0);
-  s[ACF_IDX] = ar_sum(f < nf ? fp.index_bytes(g.a.n_vars) : 0);
+  s[ACF_NUMS] = carry_sum(n);
+  s[ACF_CHUNKS] = carry_sum(fp.n_chunks);
+  s[ACF_ROWS] = carry_sum(fp.row_start(fp.n_chunks));
+  s[ACF_FRAME] = carry_sum(f < nf && g.framed ? standalone_header_len(nn) + 1 : 0);
+  s[ACF_IDX] = carry_sum(f < nf ? fp.index_bytes(g.a.n_vars) : 0);
   *n_out = n;
 }
 __device__ __forceinline__ uint64_t acf_n_files(const AcfArgs& g) {
@@ -121,41 +121,29 @@ __device__ __forceinline__ uint64_t acf_n_files(const AcfArgs& g) {
 // ceil(max_files / ACF_THREADS) CTAs, one file slot per thread: the CTA's sums.
 __global__ void __launch_bounds__(ACF_THREADS) acf_files_kernel(AcfArgs g) {
   const uint64_t nf = acf_n_files(g);
-  ArSum s[ACF_SUMS], tot[ACF_SUMS];
+  CarrySum s[ACF_SUMS], tot[ACF_SUMS];
   uint64_t n;
   acf_file_sums(g, uint64_t(blockIdx.x) * ACF_THREADS + threadIdx.x, nf, s, &n);
-  for (int k = 0; k < ACF_SUMS; k++) ar_block_scan<ACF_THREADS>(s[k], &tot[k]);
+  for (int k = 0; k < ACF_SUMS; k++) block_exscan<ACF_THREADS>(s[k], &tot[k]);
   if (threadIdx.x == 0)
     for (int k = 0; k < ACF_SUMS; k++) acf_parts(g)[blockIdx.x].s[k] = tot[k];
 }
 
 // One CTA: *n_files against max_files, and the CTA sums scanned into CTA offsets (in place).  Writes the AcfState the next kernels read.
 __global__ void __launch_bounds__(ACF_SCAN_THREADS) acf_scan_kernel(AcfArgs g) {
-  __shared__ ArSum s_carry[ACF_SUMS];
-  const uint32_t tid = threadIdx.x;
-  if (tid < ACF_SUMS) s_carry[tid] = ar_sum(0);
-  __syncthreads();
   AcfPart* parts = acf_parts(g);
-  const uint64_t n_parts = acf_ctas(g.max_files);
-  for (uint64_t base = 0; base < n_parts; base += ACF_SCAN_THREADS) {
-    const uint64_t c = base + tid;
-    for (int k = 0; k < ACF_SUMS; k++) {
-      ArSum tot;
-      const ArSum ex = ar_block_scan<ACF_SCAN_THREADS>(c < n_parts ? parts[c].s[k] : ar_sum(0), &tot);
-      if (c < n_parts) parts[c].s[k] = ar_add(s_carry[k], ex);
-      __syncthreads();
-      if (tid == 0) s_carry[k] = ar_add(s_carry[k], tot);
-      __syncthreads();
-    }
-  }
-  if (tid != 0) return;
+  CarrySum total[ACF_SUMS] = {};
+  cta_scan_inplace<ACF_SCAN_THREADS, 1>(
+      ctas_of<ACF_THREADS>(g.max_files), [&](uint64_t c, int k) { return parts[c].s[k]; }, [&](uint64_t c, int k, CarrySum v) { parts[c].s[k] = v; },
+      total);
+  if (threadIdx.x != 0) return;
   AcfState s;
   memset(&s, 0, sizeof(s));
   s.n_read = *g.n_files;
   s.n_files = acf_n_files(g);
   s.status = s.n_read > g.max_files ? uint32_t(PCO_B200_ASYNC_TOO_MANY_FILES) : uint32_t(ST_OK);
-  s.bad = AR_NONE64;
-  for (int k = 0; k < ACF_SUMS; k++) s.total[k] = s_carry[k];
+  s.bad = NONE64;
+  for (int k = 0; k < ACF_SUMS; k++) s.total[k] = total[k];
   *acf_state(g) = s;
 }
 
@@ -165,12 +153,12 @@ __global__ void __launch_bounds__(ACF_THREADS) acf_place_kernel(AcfArgs g) {
   AcfState* st = acf_state(g);
   const uint64_t nf = st->n_files;
   const uint64_t f = uint64_t(blockIdx.x) * ACF_THREADS + threadIdx.x;
-  ArSum s[ACF_SUMS], ex[ACF_SUMS];
+  CarrySum s[ACF_SUMS], ex[ACF_SUMS];
   uint64_t n;
   acf_file_sums(g, f, nf, s, &n);
   for (int k = 0; k < ACF_SUMS; k++) {
-    ArSum tot;
-    ex[k] = ar_add(acf_parts(g)[blockIdx.x].s[k], ar_block_scan<ACF_THREADS>(s[k], &tot));
+    CarrySum tot;
+    ex[k] = carry_add(acf_parts(g)[blockIdx.x].s[k], block_exscan<ACF_THREADS>(s[k], &tot));
   }
   if (f >= nf) return;
   AcfFile r;
@@ -178,7 +166,7 @@ __global__ void __launch_bounds__(ACF_THREADS) acf_place_kernel(AcfArgs g) {
   for (int k = 0; k < ACF_SUMS; k++) r.first[k] = ex[k].s;
   r.hdr_len = g.framed ? standalone_header_len(n) : 0;
   acf_files(g)[f] = r;
-  const ArSum end = ar_add(ex[ACF_NUMS], s[ACF_NUMS]);
+  const CarrySum end = carry_add(ex[ACF_NUMS], s[ACF_NUMS]);
   uint32_t code = ST_OK;
   if (n > g.max_file_n) code = PCO_B200_ASYNC_FILE_TOO_LARGE;
   else if (end.ovf || end.s > g.nums_cap) code = PCO_B200_ASYNC_NUMS_CAP;
@@ -189,7 +177,7 @@ __global__ void __launch_bounds__(ACF_THREADS) acf_place_kernel(AcfArgs g) {
 // every slot of a refused batch: 0 numbers at the end of the batch's numbers), its ChunkEnc record reset, the sums zeroed.
 __global__ void __launch_bounds__(ACF_THREADS) acf_init_kernel(AcfArgs g) {
   AcfState* st = acf_state(g);
-  const bool ok = st->status == ST_OK && st->bad == AR_NONE64;
+  const bool ok = st->status == ST_OK && st->bad == NONE64;
   const uint64_t nf = ok ? st->n_files : 0, live = ok ? st->total[ACF_CHUNKS].s : 0;
   const uint64_t end_num = ok ? st->total[ACF_NUMS].s : 0, end_row = ok ? st->total[ACF_ROWS].s : 0;
   const uint64_t nc = g.a.n_chunks;
@@ -242,31 +230,20 @@ __global__ void __launch_bounds__(ACF_THREADS) acf_bytes_kernel(AcfArgs g) {
   const uint64_t live = acf_state(g)->live_chunks;
   const ChunkEnc* chunks = reinterpret_cast<const ChunkEnc*>(g.a.ws + g.a.lay.chunks);
   const uint64_t c = uint64_t(blockIdx.x) * ACF_THREADS + threadIdx.x;
-  ArSum tot;
-  ar_block_scan<ACF_THREADS>(ar_sum(c < live ? chunks[c].chunk_bytes : 0), &tot);
-  if (threadIdx.x == 0) reinterpret_cast<uint64_t*>(g.a.ws + g.l.cparts)[blockIdx.x] = tot.s;
+  uint64_t tot;
+  block_exscan<ACF_THREADS>(c < live ? chunks[c].chunk_bytes : 0, &tot);
+  if (threadIdx.x == 0) reinterpret_cast<uint64_t*>(g.a.ws + g.l.cparts)[blockIdx.x] = tot;
 }
 
 // One CTA: the chunk CTA sums scanned into CTA offsets (in place), the bytes the batch needs, and whether it fits.
 __global__ void __launch_bounds__(ACF_SCAN_THREADS) acf_bytes_scan_kernel(AcfArgs g) {
-  __shared__ uint64_t s_carry;
-  const uint32_t tid = threadIdx.x;
-  if (tid == 0) s_carry = 0;
-  __syncthreads();
   uint64_t* parts = reinterpret_cast<uint64_t*>(g.a.ws + g.l.cparts);
-  const uint64_t n_parts = acf_ctas(g.a.n_chunks + 1);
-  for (uint64_t base = 0; base < n_parts; base += ACF_SCAN_THREADS) {
-    const uint64_t c = base + tid;
-    ArSum tot;
-    const ArSum ex = ar_block_scan<ACF_SCAN_THREADS>(ar_sum(c < n_parts ? parts[c] : 0), &tot);
-    if (c < n_parts) parts[c] = s_carry + ex.s;
-    __syncthreads();
-    if (tid == 0) s_carry += tot.s;
-    __syncthreads();
-  }
-  if (tid != 0) return;
+  uint64_t total[1] = {};
+  cta_scan_inplace<ACF_SCAN_THREADS, 1>(
+      ctas_of<ACF_THREADS>(g.a.n_chunks + 1), [&](uint64_t c, int) { return parts[c]; }, [&](uint64_t c, int, uint64_t v) { parts[c] = v; }, total);
+  if (threadIdx.x != 0) return;
   AcfState* st = acf_state(g);
-  st->dst_bytes = s_carry + st->total[ACF_FRAME].s;
+  st->dst_bytes = total[0] + st->total[ACF_FRAME].s;
   st->index_bytes = g.a.index ? st->total[ACF_IDX].s : 0;
   st->fits = st->dst_bytes <= g.a.dst_cap && st->index_bytes <= g.index_cap ? 1u : 0u;
 }
@@ -280,8 +257,8 @@ __global__ void __launch_bounds__(ACF_THREADS) acf_offsets_kernel(AcfArgs g) {
   ChunkEnc* chunks = reinterpret_cast<ChunkEnc*>(g.a.ws + g.a.lay.chunks);
   const uint64_t c = uint64_t(blockIdx.x) * ACF_THREADS + threadIdx.x;
   const uint64_t bytes = c < live ? chunks[c].chunk_bytes : 0;
-  ArSum tot;
-  const uint64_t pre = reinterpret_cast<const uint64_t*>(g.a.ws + g.l.cparts)[blockIdx.x] + ar_block_scan<ACF_THREADS>(ar_sum(bytes), &tot).s;
+  uint64_t tot;
+  const uint64_t pre = reinterpret_cast<const uint64_t*>(g.a.ws + g.l.cparts)[blockIdx.x] + block_exscan<ACF_THREADS>(bytes, &tot);
   if (c > g.a.n_chunks) return;
   reinterpret_cast<uint64_t*>(g.a.ws + g.l.pre)[c] = pre;
   if (c == g.a.n_chunks) return;
@@ -297,7 +274,7 @@ __global__ void __launch_bounds__(ACF_THREADS) acf_offsets_kernel(AcfArgs g) {
 // header, its terminator and its side index header (as frame_files_kernel writes them).
 __global__ void __launch_bounds__(ACF_THREADS) acf_frame_kernel(AcfArgs g) {
   const AcfState* st = acf_state(g);
-  if (st->status != ST_OK || st->bad != AR_NONE64) return;
+  if (st->status != ST_OK || st->bad != NONE64) return;
   const uint64_t f = uint64_t(blockIdx.x) * ACF_THREADS + threadIdx.x;
   if (f >= st->n_files) return;
   const AcfFile r = acf_files(g)[f];
@@ -380,7 +357,7 @@ __global__ void acf_finish_kernel(AcfArgs g, PcoB200AsyncCompressFilesStatus* __
   s.n_files = st->n_read;
   if (st->status != ST_OK) {
     s.device_status = st->status;
-  } else if (st->bad != AR_NONE64) {
+  } else if (st->bad != NONE64) {
     s.device_status = uint32_t(st->bad & 0xffffffffu);
     s.file = st->bad >> 32;
   } else {
@@ -427,7 +404,7 @@ inline PcoB200Error acf_check_plan(const PcoB200AsyncCompressFilesPlan* p, AcfPl
 template <typename L>
 void acf_launch_encode(const PcoB200AsyncCompressFilesPlan& p, const AcompGeom& g, const AcfArgs& fa, const void* nums, const AsyncLaunch& ln) {
   const cudaStream_t stream = ln.stream;
-  const uint32_t file_ctas = uint32_t(acf_ctas(p.max_files)), chunk_ctas = uint32_t(acf_ctas(g.n_chunks + 1));
+  const uint32_t file_ctas = uint32_t(ctas_of<ACF_THREADS>(p.max_files)), chunk_ctas = uint32_t(ctas_of<ACF_THREADS>(g.n_chunks + 1));
   ln.begin("acf_files_kernel");
   acf_files_kernel<<<file_ctas, ACF_THREADS, 0, stream>>>(fa);
   ln.end();
@@ -462,7 +439,7 @@ void acf_launch(const PcoB200AsyncCompressFilesPlan& p, const AcompGeom& g, cons
                 const AsyncLaunch& ln) {
   acf_launch_encode<L>(p, g, fa, nums, ln);
   const cudaStream_t stream = ln.stream;
-  const uint32_t nc = uint32_t(g.n_chunks), file_ctas = uint32_t(acf_ctas(p.max_files));
+  const uint32_t nc = uint32_t(g.n_chunks), file_ctas = uint32_t(ctas_of<ACF_THREADS>(p.max_files));
   // ---- framing
   ln.begin("acf_frame_kernel");
   acf_frame_kernel<<<file_ctas, ACF_THREADS, 0, stream>>>(fa);

@@ -16,6 +16,7 @@
 // writes nothing but the status; a batch that does not fit writes refs, first_chunk and the status only.
 #pragma once
 #include "async_compress_files.cuh"
+#include "cta_scan.cuh"
 #include "wrapped_kernels.cuh"  // wrapped_meta_len, WRAP_THREADS, cta_copy_bytes
 
 namespace pcob200 {
@@ -23,7 +24,7 @@ namespace pcob200 {
 enum { ACW_META = 0, ACW_PAGE, ACW_BAD, ACW_SUMS };
 struct AcwPart {  // per CTA of acw_lens_kernel: the sums of its chunks' meta lengths, page lengths and meta parse failures (the chunks are
                   // this library's own: none fails), then (acw_scan_kernel) the sums of the CTAs before it
-  ArSum s[ACW_SUMS];
+  CarrySum s[ACW_SUMS];
 };
 struct AcwState {  // written by acw_scan_kernel
   uint32_t fits;       // the metas fit metas_cap and the pages pages_cap
@@ -46,7 +47,7 @@ inline AcwLayout acw_layout(const AcfLayout& f, uint64_t stage_bytes, uint64_t m
   l.stage = take(stage_bytes);
   l.state = take(sizeof(AcwState));
   l.lens = take(max_chunks * 4);
-  l.parts = take(acf_ctas(max_chunks + 1) * sizeof(AcwPart));
+  l.parts = take(ctas_of<ACF_THREADS>(max_chunks + 1) * sizeof(AcwPart));
   l.total = at;
   return l;
 }
@@ -63,7 +64,7 @@ struct AcwArgs {
 };
 __device__ __forceinline__ AcwState* acw_state(const AcwArgs& w) { return reinterpret_cast<AcwState*>(w.f.a.ws + w.l.state); }
 __device__ __forceinline__ AcwPart* acw_parts(const AcwArgs& w) { return reinterpret_cast<AcwPart*>(w.f.a.ws + w.l.parts); }
-__device__ __forceinline__ bool acw_placed(const AcfState* st) { return st->status == ST_OK && st->bad == AR_NONE64; }
+__device__ __forceinline__ bool acw_placed(const AcfState* st) { return st->status == ST_OK && st->bad == NONE64; }
 // The chunks staged: those of a placed batch (the staging region holds any batch within the capacities, so acf_bytes_scan_kernel finds
 // that it fits; a staging that did not fit would have placed no chunk, and acw_scan_kernel reports it as chunks that do not split)
 __device__ __forceinline__ uint64_t acw_live(const AcfState* st) { return acw_placed(st) && st->fits ? st->live_chunks : 0; }
@@ -99,36 +100,24 @@ __global__ void __launch_bounds__(ACF_THREADS) acw_lens_kernel(AcwArgs w) {
     }
     reinterpret_cast<uint32_t*>(w.f.a.ws + w.l.lens)[c] = uint32_t(ml);
   }
-  ArSum tot[ACW_SUMS];
-  for (int k = 0; k < ACW_SUMS; k++) ar_block_scan<ACF_THREADS>(ar_sum(v[k]), &tot[k]);
+  CarrySum tot[ACW_SUMS];
+  for (int k = 0; k < ACW_SUMS; k++) block_exscan<ACF_THREADS>(carry_sum(v[k]), &tot[k]);
   if (threadIdx.x == 0)
     for (int k = 0; k < ACW_SUMS; k++) acw_parts(w)[blockIdx.x].s[k] = tot[k];
 }
 
 // One CTA: the CTA sums scanned into CTA offsets (in place), the totals, and whether they fit the caps.
 __global__ void __launch_bounds__(ACF_SCAN_THREADS) acw_scan_kernel(AcwArgs w) {
-  __shared__ ArSum s_carry[ACW_SUMS];
-  const uint32_t tid = threadIdx.x;
-  if (tid < ACW_SUMS) s_carry[tid] = ar_sum(0);
-  __syncthreads();
   AcwPart* parts = acw_parts(w);
-  const uint64_t n_parts = acf_ctas(w.f.a.n_chunks + 1);
-  for (uint64_t base = 0; base < n_parts; base += ACF_SCAN_THREADS) {
-    const uint64_t c = base + tid;
-    for (int k = 0; k < ACW_SUMS; k++) {
-      ArSum tot;
-      const ArSum ex = ar_block_scan<ACF_SCAN_THREADS>(c < n_parts ? parts[c].s[k] : ar_sum(0), &tot);
-      if (c < n_parts) parts[c].s[k] = ar_add(s_carry[k], ex);
-      __syncthreads();
-      if (tid == 0) s_carry[k] = ar_add(s_carry[k], tot);
-      __syncthreads();
-    }
-  }
-  if (tid != 0) return;
+  CarrySum total[ACW_SUMS] = {};
+  cta_scan_inplace<ACF_SCAN_THREADS, 1>(
+      ctas_of<ACF_THREADS>(w.f.a.n_chunks + 1), [&](uint64_t c, int k) { return parts[c].s[k]; },
+      [&](uint64_t c, int k, CarrySum v) { parts[c].s[k] = v; }, total);
+  if (threadIdx.x != 0) return;
   AcwState s;
-  s.metas_bytes = s_carry[ACW_META].s;
-  s.pages_bytes = s_carry[ACW_PAGE].s;
-  s.split_err = s_carry[ACW_BAD].s != 0 || !acf_state(w.f)->fits ? 1u : 0u;
+  s.metas_bytes = total[ACW_META].s;
+  s.pages_bytes = total[ACW_PAGE].s;
+  s.split_err = total[ACW_BAD].s != 0 || !acf_state(w.f)->fits ? 1u : 0u;
   s.fits = s.split_err == 0 && s.metas_bytes <= w.metas_cap && s.pages_bytes <= w.pages_cap ? 1u : 0u;
   s.reserved = 0;
   *acw_state(w) = s;
@@ -143,9 +132,9 @@ __global__ void __launch_bounds__(ACF_THREADS) acw_refs_kernel(AcwArgs w) {
   const uint64_t c = uint64_t(blockIdx.x) * ACF_THREADS + threadIdx.x;
   uint64_t ml, pl;
   acw_chunk_lens(w, c, live, &ml, &pl);
-  ArSum tot;
-  const ArSum mex = ar_block_scan<ACF_THREADS>(ar_sum(ml), &tot);
-  const ArSum pex = ar_block_scan<ACF_THREADS>(ar_sum(pl), &tot);
+  CarrySum tot;
+  const CarrySum mex = block_exscan<ACF_THREADS>(carry_sum(ml), &tot);
+  const CarrySum pex = block_exscan<ACF_THREADS>(carry_sum(pl), &tot);
   if (c < live) {
     const AcwPart& part = acw_parts(w)[blockIdx.x];
     const uint64_t* starts = acomp_starts(w.f.a);
@@ -185,7 +174,7 @@ __global__ void acw_finish_kernel(AcwArgs w, PcoB200AsyncCompressWrappedStatus* 
   s.n_arrays = st->n_read;
   if (st->status != ST_OK) {
     s.device_status = st->status;
-  } else if (st->bad != AR_NONE64) {
+  } else if (st->bad != NONE64) {
     s.device_status = uint32_t(st->bad & 0xffffffffu);
     s.array = st->bad >> 32;
   } else {
@@ -263,7 +252,7 @@ void acw_launch(const PcoB200AsyncCompressWrappedPlan& p, const AcwPlanGeom& pg,
   const cudaStream_t stream = ln.stream;
   acf_launch_encode<L>(acw_files_plan(p), pg.f.g, w.f, nums, ln);
   const uint64_t nc = pg.f.g.n_chunks;
-  const uint32_t chunk_ctas = uint32_t(acf_ctas(nc + 1)), ref_ctas = uint32_t(std::max(acf_ctas(nc + 1), acf_ctas(p.max_arrays + 1)));
+  const uint32_t chunk_ctas = uint32_t(ctas_of<ACF_THREADS>(nc + 1)), ref_ctas = uint32_t(std::max(ctas_of<ACF_THREADS>(nc + 1), ctas_of<ACF_THREADS>(p.max_arrays + 1)));
   ln.begin("acw_lens_kernel");
   acw_lens_kernel<<<chunk_ctas, ACF_THREADS, 0, stream>>>(w);
   ln.end();

@@ -18,7 +18,7 @@
 // j's place in dst; a call refused before the files (too many, a ref outside the buffers) leaves a table of pads only.
 #pragma once
 #include "async_kernels.cuh"
-#include "async_ranges_kernels.cuh"  // ArSum and its scans
+#include "cta_scan.cuh"
 #include "files_kernels.cuh"
 
 namespace pcob200 {
@@ -28,8 +28,8 @@ constexpr int AF_SCAN_THREADS = 1024;  // the one-CTA launches
 
 // per CTA of af_files_kernel (af_scan_kernel turns the sums into CTA offsets, in place)
 struct AfPart {
-  ArSum count, chunks;
-  uint64_t bad_ref;     // lowest ref refusal of the CTA as (file << 32) | status (AR_NONE64: none)
+  CarrySum count, chunks;
+  uint64_t bad_ref;     // lowest ref refusal of the CTA as (file << 32) | status (NONE64: none)
   uint64_t reserved;
 };
 
@@ -40,7 +40,7 @@ struct AfState {
   uint64_t n_read;      // *n_files as read
   uint64_t n_files;     // the files the call runs over (0 when *n_files is above max_files)
   uint64_t bad;         // (file << 32) | status: the lowest refusal (a ref refusal here, or af_place_kernel's by atomicMin)
-  ArSum total, chunks;  // the sums of the counts and of the chunk counts over the files
+  CarrySum total, chunks;  // the sums of the counts and of the chunk counts over the files
 };
 
 // everything the launches take by value; fp.src_len is src_cap
@@ -60,7 +60,6 @@ struct AfArgs {
 struct AfLayout : AsyncDecodeTail {
   uint64_t state, fst, fchk, verdict, merges, parts, table;
 };
-__host__ __device__ inline uint64_t af_ctas(uint64_t n) { return (n + AF_THREADS - 1) / AF_THREADS; }
 __host__ __device__ inline AfLayout af_layout(uint64_t max_files, uint64_t max_chunks, uint64_t dst_cap) {
   AfLayout l;
   l.state = async_align(sizeof(AsyncCheck));
@@ -69,7 +68,7 @@ __host__ __device__ inline AfLayout af_layout(uint64_t max_files, uint64_t max_c
   l.verdict = l.fchk + async_align(max_files * sizeof(FileCheck));
   l.merges = l.verdict + async_align(max_files * sizeof(uint32_t));
   l.parts = l.merges + async_align(max_files * sizeof(FileMerge));
-  l.table = l.parts + async_align(af_ctas(max_files) * sizeof(AfPart));
+  l.table = l.parts + async_align(ctas_of<AF_THREADS>(max_files) * sizeof(AfPart));
   static_cast<AsyncDecodeTail&>(l) =
       async_decode_tail(l.table + async_align(max_chunks * sizeof(IndexChunk)), max_chunks, scratch_rows_total(dst_cap, uint32_t(max_chunks)), 0);
   return l;
@@ -89,7 +88,7 @@ __global__ void __launch_bounds__(AF_THREADS) af_files_kernel(AfArgs g, AsyncChe
                                                               FileCheck* __restrict__ fchk, FileMerge* __restrict__ merges, AfPart* __restrict__ parts) {
   __shared__ unsigned long long s_bad;
   const uint32_t tid = threadIdx.x;
-  if (tid == 0) s_bad = AR_NONE64;
+  if (tid == 0) s_bad = NONE64;
   if (blockIdx.x == 0 && tid == 32) PCOB_ASYNC_FILL_BINOMS(chk->binoms);
   __syncthreads();
   const uint64_t n = af_n_files(g);
@@ -140,9 +139,9 @@ __global__ void __launch_bounds__(AF_THREADS) af_files_kernel(AfArgs g, AsyncChe
     fchk[i] = fc;
     merges[i] = fm;
   }
-  ArSum c_tot, k_tot;
-  ar_block_scan<AF_THREADS>(ar_sum(count), &c_tot);
-  ar_block_scan<AF_THREADS>(ar_sum(n_chunks), &k_tot);
+  CarrySum c_tot, k_tot;
+  block_exscan<AF_THREADS>(carry_sum(count), &c_tot);
+  block_exscan<AF_THREADS>(carry_sum(n_chunks), &k_tot);
   if (tid == 0) parts[blockIdx.x] = AfPart{c_tot, k_tot, s_bad, 0};
 }
 
@@ -150,43 +149,28 @@ __global__ void __launch_bounds__(AF_THREADS) af_files_kernel(AfArgs g, AsyncChe
 // decompress_files_impl does), and the CTA sums scanned into CTA offsets (in place).  Writes the AfState the next kernels read.
 __global__ void __launch_bounds__(AF_SCAN_THREADS) af_scan_kernel(AfArgs g, AfPart* __restrict__ parts, AfState* __restrict__ state) {
   __shared__ unsigned long long s_bad;
-  __shared__ ArSum s_carry[2];
   const uint32_t tid = threadIdx.x;
-  if (tid == 0) {
-    s_bad = AR_NONE64;
-    s_carry[0] = s_carry[1] = ar_sum(0);
-  }
+  if (tid == 0) s_bad = NONE64;
   __syncthreads();
-  const uint64_t n_parts = af_ctas(g.max_files);
-  for (uint64_t base = 0; base < n_parts; base += AF_SCAN_THREADS) {
-    const uint64_t c = base + tid;
-    const AfPart p = c < n_parts ? parts[c] : AfPart{ar_sum(0), ar_sum(0), AR_NONE64, 0};
-    if (p.bad_ref != AR_NONE64) atomicMin(&s_bad, p.bad_ref);
-    ArSum c_tot, k_tot;
-    const ArSum c_ex = ar_block_scan<AF_SCAN_THREADS>(p.count, &c_tot);
-    const ArSum k_ex = ar_block_scan<AF_SCAN_THREADS>(p.chunks, &k_tot);
-    if (c < n_parts) {
-      parts[c].count = ar_add(s_carry[0], c_ex);
-      parts[c].chunks = ar_add(s_carry[1], k_ex);
-    }
-    __syncthreads();
-    if (tid == 0) {
-      s_carry[0] = ar_add(s_carry[0], c_tot);
-      s_carry[1] = ar_add(s_carry[1], k_tot);
-    }
-    __syncthreads();
-  }
+  const uint64_t n_parts = ctas_of<AF_THREADS>(g.max_files);
+  for (uint64_t c = tid; c < n_parts; c += AF_SCAN_THREADS)
+    if (parts[c].bad_ref != NONE64) atomicMin(&s_bad, parts[c].bad_ref);
+  auto sum = [&](uint64_t c, int k) -> CarrySum& { return k ? parts[c].chunks : parts[c].count; };
+  CarrySum total[2] = {};
+  cta_scan_inplace<AF_SCAN_THREADS, 1>(
+      n_parts, [&](uint64_t c, int k) { return sum(c, k); }, [&](uint64_t c, int k, CarrySum v) { sum(c, k) = v; }, total);
+  __syncthreads();
   if (tid != 0) return;
   AfState s;
   s.status = ST_OK;
   s.reserved = 0;
   s.n_read = *g.n_files;
   s.n_files = af_n_files(g);
-  s.bad = AR_NONE64;
-  s.total = s_carry[0];
-  s.chunks = s_carry[1];
+  s.bad = NONE64;
+  s.total = total[0];
+  s.chunks = total[1];
   if (s.n_read > g.max_files) s.status = PCO_B200_ASYNC_TOO_MANY_FILES;
-  else if (s_bad != AR_NONE64) {
+  else if (s_bad != NONE64) {
     s.status = uint32_t(s_bad);
     s.bad = s_bad;
   }
@@ -206,13 +190,13 @@ __global__ void __launch_bounds__(AF_THREADS) af_place_kernel(AfArgs g, const ui
   const uint64_t i = uint64_t(blockIdx.x) * AF_THREADS + tid;
   const bool in = i < n;
   const uint64_t count = in ? fchk[i].n_total : 0, n_chunks = in ? fchk[i].n_chunks : 0;
-  ArSum tot;
-  const ArSum c_ex = ar_add(parts[blockIdx.x].count, ar_block_scan<AF_THREADS>(ar_sum(count), &tot));
-  const ArSum k_ex = ar_add(parts[blockIdx.x].chunks, ar_block_scan<AF_THREADS>(ar_sum(n_chunks), &tot));
+  CarrySum tot;
+  const CarrySum c_ex = carry_add(parts[blockIdx.x].count, block_exscan<AF_THREADS>(carry_sum(count), &tot));
+  const CarrySum k_ex = carry_add(parts[blockIdx.x].chunks, block_exscan<AF_THREADS>(carry_sum(n_chunks), &tot));
   if (!in) return;
   merges[i].list_at = k_ex.s;
   merges[i].out_add = c_ex.s;
-  const ArSum c_inc = ar_add(c_ex, ar_sum(count)), k_inc = ar_add(k_ex, ar_sum(n_chunks));
+  const CarrySum c_inc = carry_add(c_ex, carry_sum(count)), k_inc = carry_add(k_ex, carry_sum(n_chunks));
   uint32_t st = fst[i];
   if (st == ST_OK && n_chunks > 0) {
     const uint32_t v = verdict[i];
@@ -236,13 +220,13 @@ __global__ void __launch_bounds__(AF_THREADS) af_table_kernel(AfArgs g, const Af
   const uint32_t pre = state->status;
   // the files decoded: [0, limit), and their chunks: [0, accepted), at most max_chunks (a file before `limit` that took the running
   // count past max_chunks would have been refused itself)
-  const uint64_t limit = pre != ST_OK ? 0 : bad != AR_NONE64 ? bad >> 32 : n;
+  const uint64_t limit = pre != ST_OK ? 0 : bad != NONE64 ? bad >> 32 : n;
   const uint64_t accepted = limit == 0 ? 0 : limit < n ? merges[limit].list_at : state->chunks.s;
   const uint64_t k = uint64_t(blockIdx.x) * AF_THREADS + threadIdx.x;
   if (k < g.max_files && k >= limit) merges[k].n_chunks = 0;
   if (k < g.max_chunks && k >= accepted) table[k] = IndexChunk{g.fp.src_len, 0u, 0u, 0, 0};
   if (k == 0) {
-    chk->status = pre != ST_OK ? pre : bad != AR_NONE64 ? uint32_t(bad) : uint32_t(ST_OK);
+    chk->status = pre != ST_OK ? pre : bad != NONE64 ? uint32_t(bad) : uint32_t(ST_OK);
     chk->n_chunks = uint32_t(accepted);
   }
 }
@@ -273,8 +257,8 @@ __global__ void __launch_bounds__(AF_SCAN_THREADS) af_finish_kernel(const AfStat
   PcoB200AsyncFilesStatus r;
   r.kind = PCO_B200_OK;
   r.device_status = ST_OK;
-  r.file = AR_NONE64;
-  r.chunk = AR_NONE64;
+  r.file = NONE64;
+  r.chunk = NONE64;
   r.n_written = pending == ST_OK ? state->total.s : 0;
   r.n_files = state->n_read;
   if (s_min != 0xffffffffu) {

@@ -22,6 +22,7 @@
 // The walks write records and entries into the workspace; the index is written only by the last three kernels, and only on success.
 #pragma once
 #include "async_kernels.cuh"
+#include "cta_scan.cuh"
 #include "decode_kernels.cuh"
 
 namespace pcob200 {
@@ -99,56 +100,6 @@ __device__ __forceinline__ FileParams ai_file(const AiArgs& g, const AiState& s)
   return FileParams{g.src, s.src_len, g.dtype, g.uniform_type, g.format_major};
 }
 
-// Exclusive scan of one value per thread over a CTA of T threads (T a multiple of 32, at most 1024); *total gets the sum.
-template <int T, typename V>
-__device__ __forceinline__ V ai_block_exscan(V v, V* total) {
-  __shared__ V s_warp[32];
-  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  V inc = v;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const V o = __shfl_up_sync(0xffffffffu, inc, d);
-    if (lane >= uint32_t(d)) inc += o;
-  }
-  if (lane == 31) s_warp[warp] = inc;
-  __syncthreads();
-  if (warp == 0) {
-    V w = lane < uint32_t(T / 32) ? s_warp[lane] : V(0);
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const V o = __shfl_up_sync(0xffffffffu, w, d);
-      if (lane >= uint32_t(d)) w += o;
-    }
-    s_warp[lane] = w;  // inclusive sums of the warps
-  }
-  __syncthreads();
-  const V before = warp ? s_warp[warp - 1] : V(0);
-  *total = s_warp[T / 32 - 1];
-  __syncthreads();  // s_warp is reused by the next call
-  return before + inc - v;
-}
-
-// One CTA of AI_SCAN_THREADS: v[0, n) replaced by its exclusive prefix sums plus `base`; returns base plus the sum.
-__device__ inline uint64_t ai_scan_inplace(uint64_t* v, uint64_t n, uint64_t base) {
-  constexpr uint64_t TILE = uint64_t(AI_SCAN_THREADS) * AI_SCAN_PER_THREAD;
-  for (uint64_t t0 = 0; t0 < n; t0 += TILE) {
-    const uint64_t i0 = t0 + uint64_t(threadIdx.x) * AI_SCAN_PER_THREAD;
-    uint64_t sum = 0;
-    for (int q = 0; q < AI_SCAN_PER_THREAD; q++)
-      if (i0 + q < n) sum += v[i0 + q];
-    uint64_t tile_total;
-    uint64_t run = base + ai_block_exscan<AI_SCAN_THREADS>(sum, &tile_total);
-    for (int q = 0; q < AI_SCAN_PER_THREAD; q++)
-      if (i0 + q < n) {
-        const uint64_t x = v[i0 + q];
-        v[i0 + q] = run;
-        run += x;
-      }
-    base += tile_total;
-  }
-  return base;
-}
-
 // One thread.  The file length against src_cap, the header against the plan's flavour; the cursor on the first chunk.
 __global__ void ai_head_kernel(AiArgs g, AiState* __restrict__ state) {
   AiState s;
@@ -207,7 +158,7 @@ __global__ void __launch_bounds__(AI_THREADS) ai_count_kernel(AiArgs g, const Ai
   const AiState& s = *state;
   if (!s.active || blockIdx.x < s.find_lo || blockIdx.x >= s.find_hi) return;
   uint64_t total;
-  ai_block_exscan<AI_THREADS>(uint64_t(__popc(ai_matches(g, s))), &total);
+  block_exscan<AI_THREADS>(uint64_t(__popc(ai_matches(g, s))), &total);
   if (threadIdx.x == 0) parts[blockIdx.x] = total;
 }
 
@@ -215,12 +166,15 @@ __global__ void __launch_bounds__(AI_THREADS) ai_count_kernel(AiArgs g, const Ai
 __global__ void __launch_bounds__(AI_SCAN_THREADS) ai_scan_kernel(AiArgs g, AiState* __restrict__ state, uint64_t* __restrict__ parts) {
   AiState& s = *state;
   if (!s.active) return;
-  const uint64_t found = ai_scan_inplace(parts + s.find_lo, s.find_hi - s.find_lo, 0);
+  uint64_t* v = parts + s.find_lo;
+  uint64_t found[1] = {};
+  cta_scan_inplace<AI_SCAN_THREADS, AI_SCAN_PER_THREAD>(
+      s.find_hi - s.find_lo, [&](uint64_t i, int) { return v[i]; }, [&](uint64_t i, int, uint64_t x) { v[i] = x; }, found);
   if (threadIdx.x != 0) return;
   const AiLayout l = ai_layout(g.src_cap, g.index_cap, g.max_chunks);
   const uint64_t at = (s.arena_end + 15) & ~uint64_t(15);
   const uint64_t room = at < l.arena_end ? l.arena_end - at : 0;
-  s.m = min(min(found, g.max_chunks - s.n_chunks + AI_SPARE_CANDS), room / s.stride);
+  s.m = min(min(found[0], g.max_chunks - s.n_chunks + AI_SPARE_CANDS), room / s.stride);
   s.cand_at = at;
 }
 
@@ -231,7 +185,7 @@ __global__ void __launch_bounds__(AI_THREADS) ai_scatter_kernel(AiArgs g, const 
   if (!s.active || blockIdx.x < s.find_lo || blockIdx.x >= s.find_hi || parts[blockIdx.x] >= s.m) return;
   const uint32_t mask = ai_matches(g, s);
   uint64_t total;
-  uint64_t rank = parts[blockIdx.x] + ai_block_exscan<AI_THREADS>(uint64_t(__popc(mask)), &total);
+  uint64_t rank = parts[blockIdx.x] + block_exscan<AI_THREADS>(uint64_t(__popc(mask)), &total);
   const uint64_t p0 = uint64_t(blockIdx.x) * AI_FIND_SPAN + uint64_t(threadIdx.x) * AI_FIND_PER_THREAD;
   for (uint32_t b = mask; b && rank < s.m; b &= b - 1, rank++) {
     const uint64_t p = p0 + __ffs(b) - 1;
@@ -336,10 +290,12 @@ __global__ void __launch_bounds__(AI_SCAN_THREADS) ai_place_kernel(AiArgs g, AiS
   uint64_t* offs = reinterpret_cast<uint64_t*>(g.ws + l.offs);
   for (uint64_t c = threadIdx.x; c < n; c += AI_SCAN_THREADS) offs[c] = entries_bytes(recs[c].n_vars, recs[c].n);
   __syncthreads();
-  const uint64_t end = ai_scan_inplace(offs, n, sizeof(IndexHeader) + n * sizeof(IndexChunk));
+  uint64_t end[1] = {sizeof(IndexHeader) + n * sizeof(IndexChunk)};
+  cta_scan_inplace<AI_SCAN_THREADS, AI_SCAN_PER_THREAD>(
+      n, [&](uint64_t i, int) { return offs[i]; }, [&](uint64_t i, int, uint64_t x) { offs[i] = x; }, end);
   if (threadIdx.x != 0) return;
-  if (end > g.index_cap) s.status = PCO_B200_ASYNC_FILES_INDEX_FULL;
-  else s.index_bytes = end;
+  if (end[0] > g.index_cap) s.status = PCO_B200_ASYNC_FILES_INDEX_FULL;
+  else s.index_bytes = end[0];
 }
 
 // max_chunks + 1 CTAs, one per chunk: its entries (the walked bytes, then zeros up to the 16-byte boundary) and its record into the index.

@@ -18,7 +18,7 @@
 // A refused batch, or one whose lowest failing page is j, decodes nothing at or behind j's slot of dst.
 #pragma once
 #include "async_kernels.cuh"
-#include "async_ranges_kernels.cuh"  // ArSum and its scans
+#include "cta_scan.cuh"
 #include "wrapped_kernels.cuh"
 
 namespace pcob200 {
@@ -28,8 +28,8 @@ constexpr int AP_SCAN_THREADS = 1024;  // the one-CTA launches
 
 // per CTA of ap_pages_kernel (ap_scan_kernel turns the sums into CTA offsets, in place)
 struct ApPart {
-  ArSum frames, entries, nums;
-  uint64_t bad_ref;  // lowest ref refusal of the CTA as (page << 32) | status (AR_NONE64: none)
+  CarrySum frames, entries, nums;
+  uint64_t bad_ref;  // lowest ref refusal of the CTA as (page << 32) | status (NONE64: none)
 };
 
 // decided by the kernels, in launch order
@@ -39,11 +39,11 @@ struct ApState {
   uint64_t n_read;          // *n_pages as read
   uint64_t n_pages;         // the pages the call runs over (0 when *n_pages is above max_pages)
   uint64_t bad;             // (page << 32) | status of a ref refusal, or the page that takes the numbers past dst_cap
-  ArSum frames, nums;       // the totals
-  uint64_t fail_page;       // ap_route_kernel: the lowest page failing its meta or walk (AR_NONE64: none)
+  CarrySum frames, nums;    // the totals
+  uint64_t fail_page;       // ap_route_kernel: the lowest page failing its meta or walk (NONE64: none)
   uint32_t fail_st, rewalk_st;
   uint64_t n_fast, n_cold;  // the decode table's records and the cold list's pages, all in front of fail_page
-  uint64_t decode_fail;     // ap_cold_kernel: (page << 32) | status of the lowest failing decode (AR_NONE64: none)
+  uint64_t decode_fail;     // ap_cold_kernel: (page << 32) | status of the lowest failing decode (NONE64: none)
   WalkResult walk;          // walk_kernel's serial result, not written in per-chunk mode
 };
 static_assert(sizeof(ApPart) == 56 && sizeof(ApState) == 136 && sizeof(WalkSmem<SMALL_MAX_SIZE_LOG>) <= 48 * 1024, "workspace layout");
@@ -64,7 +64,6 @@ struct ApArgs {
 struct ApLayout : AsyncDecodeTail {
   uint64_t state, tab, index, index_len, frames, pad_frame, pstat, wst, ends, parts, table, fast_page, cold_list;
 };
-__host__ __device__ inline uint64_t ap_ctas(uint64_t n) { return (n + AP_THREADS - 1) / AP_THREADS; }
 // Batch entries of an accepted batch: each page's entries_bytes(MAX_VARS, n) (16-byte aligned room for MAX_VARS x ceil(n / 256) entries of 12 bytes)
 // is at most 24 floor(n / 256) + 32 bytes, and the pages hold at most dst_cap numbers.
 __host__ __device__ inline uint64_t ap_entries_bound(uint64_t max_pages, uint64_t dst_cap) { return 24 * (dst_cap / BATCH_N) + 32 * max_pages; }
@@ -80,7 +79,7 @@ __host__ __device__ inline ApLayout ap_layout(uint64_t max_pages, uint64_t dst_c
   l.wst = l.pstat + async_align(max_pages * sizeof(uint32_t));
   l.ends = l.wst + async_align(max_pages * sizeof(uint32_t));
   l.parts = l.ends + async_align(max_pages * sizeof(uint64_t));
-  l.table = l.parts + async_align(ap_ctas(max_pages) * sizeof(ApPart));
+  l.table = l.parts + async_align(ctas_of<AP_THREADS>(max_pages) * sizeof(ApPart));
   l.fast_page = l.table + async_align(max_pages * sizeof(IndexChunk));
   l.cold_list = l.fast_page + async_align(max_pages * sizeof(uint32_t));
   static_cast<AsyncDecodeTail&>(l) =
@@ -100,7 +99,7 @@ __device__ __forceinline__ uint64_t ap_frame_bytes(const PcoB200PageRef& r) { re
 __global__ void __launch_bounds__(AP_THREADS) ap_pages_kernel(ApArgs g, AsyncCheck* __restrict__ chk, ApPart* __restrict__ parts) {
   __shared__ unsigned long long s_bad;
   const uint32_t tid = threadIdx.x;
-  if (tid == 0) s_bad = AR_NONE64;
+  if (tid == 0) s_bad = NONE64;
   if (blockIdx.x == 0 && tid == 32) PCOB_ASYNC_FILL_BINOMS(chk->binoms);
   __syncthreads();
   const uint64_t i = uint64_t(blockIdx.x) * AP_THREADS + tid;
@@ -119,10 +118,10 @@ __global__ void __launch_bounds__(AP_THREADS) ap_pages_kernel(ApArgs g, AsyncChe
       nums = r.page_n;
     }
   }
-  ArSum f_tot, e_tot, n_tot;
-  ar_block_scan<AP_THREADS>(ar_sum(frame), &f_tot);
-  ar_block_scan<AP_THREADS>(ar_sum(room), &e_tot);
-  ar_block_scan<AP_THREADS>(ar_sum(nums), &n_tot);
+  CarrySum f_tot, e_tot, n_tot;
+  block_exscan<AP_THREADS>(carry_sum(frame), &f_tot);
+  block_exscan<AP_THREADS>(carry_sum(room), &e_tot);
+  block_exscan<AP_THREADS>(carry_sum(nums), &n_tot);
   if (tid == 0) parts[blockIdx.x] = ApPart{f_tot, e_tot, n_tot, s_bad};
 }
 
@@ -130,53 +129,35 @@ __global__ void __launch_bounds__(AP_THREADS) ap_pages_kernel(ApArgs g, AsyncChe
 // totals: more numbers than dst_cap (the page that passes it is found by ap_place_kernel), then more frame bytes than frame_cap.
 __global__ void __launch_bounds__(AP_SCAN_THREADS) ap_scan_kernel(ApArgs g, ApPart* __restrict__ parts, ApState* __restrict__ state) {
   __shared__ unsigned long long s_bad;
-  __shared__ ArSum s_carry[3];
   const uint32_t tid = threadIdx.x;
-  if (tid == 0) {
-    s_bad = AR_NONE64;
-    s_carry[0] = s_carry[1] = s_carry[2] = ar_sum(0);
-  }
+  if (tid == 0) s_bad = NONE64;
   __syncthreads();
-  const uint64_t n_parts = ap_ctas(g.max_pages);
-  for (uint64_t base = 0; base < n_parts; base += AP_SCAN_THREADS) {
-    const uint64_t c = base + tid;
-    const ApPart p = c < n_parts ? parts[c] : ApPart{ar_sum(0), ar_sum(0), ar_sum(0), AR_NONE64};
-    if (p.bad_ref != AR_NONE64) atomicMin(&s_bad, p.bad_ref);
-    ArSum f_tot, e_tot, n_tot;
-    const ArSum f_ex = ar_block_scan<AP_SCAN_THREADS>(p.frames, &f_tot);
-    const ArSum e_ex = ar_block_scan<AP_SCAN_THREADS>(p.entries, &e_tot);
-    const ArSum n_ex = ar_block_scan<AP_SCAN_THREADS>(p.nums, &n_tot);
-    if (c < n_parts) {
-      parts[c].frames = ar_add(s_carry[0], f_ex);
-      parts[c].entries = ar_add(s_carry[1], e_ex);
-      parts[c].nums = ar_add(s_carry[2], n_ex);
-    }
-    __syncthreads();
-    if (tid == 0) {
-      s_carry[0] = ar_add(s_carry[0], f_tot);
-      s_carry[1] = ar_add(s_carry[1], e_tot);
-      s_carry[2] = ar_add(s_carry[2], n_tot);
-    }
-    __syncthreads();
-  }
+  const uint64_t n_parts = ctas_of<AP_THREADS>(g.max_pages);
+  for (uint64_t c = tid; c < n_parts; c += AP_SCAN_THREADS)
+    if (parts[c].bad_ref != NONE64) atomicMin(&s_bad, parts[c].bad_ref);
+  auto sum = [&](uint64_t c, int k) -> CarrySum& { return k == 0 ? parts[c].frames : k == 1 ? parts[c].entries : parts[c].nums; };
+  CarrySum total[3] = {};
+  cta_scan_inplace<AP_SCAN_THREADS, 1>(
+      n_parts, [&](uint64_t c, int k) { return sum(c, k); }, [&](uint64_t c, int k, CarrySum v) { sum(c, k) = v; }, total);
+  __syncthreads();
   if (tid != 0) return;
   ApState s;
   s.status = ST_OK;
   s.rewalk = 0;
   s.n_read = *g.n_pages;
   s.n_pages = ap_n_pages(g);
-  s.bad = AR_NONE64;
-  s.frames = s_carry[0];
-  s.nums = s_carry[2];
-  s.fail_page = AR_NONE64;
+  s.bad = NONE64;
+  s.frames = total[0];
+  s.nums = total[2];
+  s.fail_page = NONE64;
   s.fail_st = ST_OK;
   s.rewalk_st = ST_OK;
   s.n_fast = 0;
   s.n_cold = 0;
-  s.decode_fail = AR_NONE64;
+  s.decode_fail = NONE64;
   s.walk = WalkResult{0, 0, 0, 0, 0};
   if (s.n_read > g.max_pages) s.status = PCO_B200_ASYNC_TOO_MANY_PAGES;
-  else if (s_bad != AR_NONE64) {
+  else if (s_bad != NONE64) {
     s.status = uint32_t(s_bad);
     s.bad = s_bad;
   } else if (s.nums.s > g.dst_cap) s.status = PCO_B200_ASYNC_PAGES_DST;  // the page: ap_place_kernel
@@ -200,10 +181,10 @@ __global__ void __launch_bounds__(AP_THREADS) ap_place_kernel(ApArgs g, const Ap
   PcoB200PageRef r{0, 0, 0, 0, 0};
   if (in) r = g.refs[i];
   const uint64_t frame = in ? ap_frame_bytes(r) : 0, room = in ? entries_bytes(MAX_VARS, r.page_n) : 0, nums = in ? r.page_n : 0;
-  ArSum tot;
-  const ArSum f_ex = ar_add(parts[blockIdx.x].frames, ar_block_scan<AP_THREADS>(ar_sum(frame), &tot));
-  const ArSum e_ex = ar_add(parts[blockIdx.x].entries, ar_block_scan<AP_THREADS>(ar_sum(room), &tot));
-  const ArSum n_ex = ar_add(parts[blockIdx.x].nums, ar_block_scan<AP_THREADS>(ar_sum(nums), &tot));
+  CarrySum tot;
+  const CarrySum f_ex = carry_add(parts[blockIdx.x].frames, block_exscan<AP_THREADS>(carry_sum(frame), &tot));
+  const CarrySum e_ex = carry_add(parts[blockIdx.x].entries, block_exscan<AP_THREADS>(carry_sum(room), &tot));
+  const CarrySum n_ex = carry_add(parts[blockIdx.x].nums, block_exscan<AP_THREADS>(carry_sum(nums), &tot));
   if (i >= g.max_pages) return;
   if (in && pre == PCO_B200_ASYNC_PAGES_DST && n_ex.s <= g.dst_cap && n_ex.s + nums > g.dst_cap) state->bad = (i << 32) | pre;
   if (in && pre == ST_OK) {
@@ -231,7 +212,7 @@ __global__ void __launch_bounds__(AP_SCAN_THREADS) ap_route_kernel(ApArgs g, ApS
   __shared__ uint64_t s_carry[2];
   const uint32_t tid = threadIdx.x;
   if (tid == 0) {
-    s_fail = AR_NONE64;
+    s_fail = NONE64;
     s_carry[0] = s_carry[1] = 0;
   }
   __syncthreads();
@@ -260,7 +241,7 @@ __global__ void __launch_bounds__(AP_SCAN_THREADS) ap_route_kernel(ApArgs g, ApS
   }
   __syncthreads();
   const unsigned long long fail = s_fail;
-  const uint64_t limit = fail != AR_NONE64 ? (fail >> 32) : n;
+  const uint64_t limit = fail != NONE64 ? (fail >> 32) : n;
   const uint32_t lane = tid & 31, warp = tid >> 5;
   __shared__ uint32_t s_warp[2][AP_SCAN_THREADS / 32];
   for (uint64_t base = 0; base < limit; base += AP_SCAN_THREADS) {
@@ -304,7 +285,7 @@ __global__ void __launch_bounds__(AP_SCAN_THREADS) ap_route_kernel(ApArgs g, ApS
   if (tid != 0) return;
   state->n_fast = n_fast;
   state->n_cold = s_carry[1];
-  if (fail != AR_NONE64) {
+  if (fail != NONE64) {
     const uint64_t p = fail >> 32;
     state->fail_page = p;
     state->fail_st = uint32_t(fail) & 0x7fffffffu;
@@ -347,7 +328,7 @@ __global__ void __launch_bounds__(ASYNC_THREADS) ap_cold_kernel(ApArgs g, ApStat
     }
   __syncthreads();
   if (tid != 0) return;
-  uint64_t fail = AR_NONE64;
+  uint64_t fail = NONE64;
   if (s_min != 0xffffffffu) fail = (uint64_t(fast_page[s_min]) << 32) | statuses[s_min];
   const uint64_t limit = min(state->fail_page, fail >> 32);
   const uint64_t n_cold = state->n_cold;
@@ -374,17 +355,17 @@ __global__ void __launch_bounds__(32) ap_finish_kernel(const ApState* __restrict
   PcoB200AsyncPagesStatus r;
   r.kind = PCO_B200_OK;
   r.device_status = ST_OK;
-  r.page = AR_NONE64;
+  r.page = NONE64;
   const bool refs_ok = s.status == ST_OK || s.status == PCO_B200_ASYNC_FRAMES;
   r.n_written = refs_ok ? s.nums.s : 0;
   r.n_pages = s.n_read;
-  r.frames_needed = refs_ok || s.status == PCO_B200_ASYNC_PAGES_DST ? (s.frames.ovf ? AR_NONE64 : s.frames.s) : 0;
+  r.frames_needed = refs_ok || s.status == PCO_B200_ASYNC_PAGES_DST ? (s.frames.ovf ? NONE64 : s.frames.s) : 0;
   if (s.status != ST_OK) {
     r.kind = async_kind_of(s.status);
     r.device_status = s.status;
     r.n_written = 0;
     if (s.status != PCO_B200_ASYNC_TOO_MANY_PAGES && s.status != PCO_B200_ASYNC_FRAMES) r.page = s.bad >> 32;
-  } else if (s.fail_page != AR_NONE64 || s.decode_fail != AR_NONE64) {
+  } else if (s.fail_page != NONE64 || s.decode_fail != NONE64) {
     uint32_t st;
     if (s.fail_page <= (s.decode_fail >> 32)) {
       r.page = s.fail_page;

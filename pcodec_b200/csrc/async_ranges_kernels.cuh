@@ -22,6 +22,7 @@
 // general pair needs (vars) x (batches from the first decoded one to ceil(hi / 256)) <= 2 W / 256).
 #pragma once
 #include "async_kernels.cuh"
+#include "cta_scan.cuh"
 #include "decode_kernels.cuh"
 #include "ranges_kernels.cuh"
 
@@ -42,18 +43,14 @@ struct ArMark {
   uint32_t task, reserved;
   uint64_t lone_dst;      // min destination offset of its pieces: the place of a lone piece
 };
-struct ArSum {            // a sum with a flag for a carry out of 64 bits anywhere in it
-  uint64_t s;
-  uint32_t ovf, reserved;
-};
 struct ArChunkPart {      // per CTA of ar_chunks_kernel / ar_window_kernel (ar_gate_kernel turns the last two into offsets)
   uint32_t tile_bad;      // lowest chunk that breaks the tiling (n_chunks: the sum differs from n_total; AR_NONE: none)
   uint32_t reserved;
   uint64_t n_touched, window;
 };
 struct ArRangePart {      // per CTA of ar_count_kernel (ar_scan_kernel turns sum into an offset)
-  ArSum sum;
-  uint64_t bad;           // lowest range past the file, as 2 i (AR_NONE64: none)
+  CarrySum sum;
+  uint64_t bad;           // lowest range past the file, as 2 i (NONE64: none)
   uint64_t reserved;
 };
 struct ArTask {
@@ -61,7 +58,6 @@ struct ArTask {
   uint32_t route, reserved;
   uint64_t slot;          // first number of its slot in the staging area
 };
-constexpr uint64_t AR_NONE64 = ~uint64_t(0);
 
 // decided by ar_scan_kernel, ar_mark_kernel and ar_gate_kernel
 struct ArState {
@@ -69,7 +65,7 @@ struct ArState {
   uint32_t n_ranges;      // ranges the call runs over (0 once refused before the ranges)
   uint32_t n_tasks;       // touched chunks (0 when refused)
   uint32_t reserved;
-  uint64_t bad;           // lowest failing range as 2 i (past the file) or 2 i + 1 (the counts overflow there); AR_NONE64: none
+  uint64_t bad;           // lowest failing range as 2 i (past the file) or 2 i + 1 (the counts overflow there); NONE64: none
   uint64_t bad_chunk;     // the chunk a tiling refusal names
   uint64_t total;         // the sum of the counts
   uint64_t window_needed;
@@ -90,7 +86,6 @@ struct ArArgs {
 struct ArLayout : AsyncDecodeTail {
   uint64_t state, table, marks, cparts, rparts, roff, rspan, tasks, wins, tinfo;
 };
-__host__ __device__ inline uint64_t ar_ctas(uint64_t n) { return (n + AR_THREADS - 1) / AR_THREADS; }
 __host__ __device__ inline uint64_t ar_rows(uint64_t window_cap) { return 2 * (window_cap / BATCH_N); }
 __host__ __device__ inline ArLayout ar_layout(uint64_t max_chunks, uint64_t max_ranges, uint64_t window_cap, uint32_t elem) {
   ArLayout l;
@@ -98,8 +93,8 @@ __host__ __device__ inline ArLayout ar_layout(uint64_t max_chunks, uint64_t max_
   l.table = l.state + async_align(sizeof(ArState));
   l.marks = l.table + async_align(max_chunks * sizeof(IndexChunk));
   l.cparts = l.marks + async_align(max_chunks * sizeof(ArMark));
-  l.rparts = l.cparts + async_align(ar_ctas(max_chunks) * sizeof(ArChunkPart));
-  l.roff = l.rparts + async_align(ar_ctas(max_ranges) * sizeof(ArRangePart));
+  l.rparts = l.cparts + async_align(ctas_of<AR_THREADS>(max_chunks) * sizeof(ArChunkPart));
+  l.roff = l.rparts + async_align(ctas_of<AR_THREADS>(max_ranges) * sizeof(ArRangePart));
   l.rspan = l.roff + async_align(max_ranges * sizeof(uint64_t));
   l.tasks = l.rspan + async_align(max_ranges * sizeof(uint2));
   l.wins = l.tasks + async_align(max_chunks * sizeof(IndexChunk));
@@ -107,49 +102,6 @@ __host__ __device__ inline ArLayout ar_layout(uint64_t max_chunks, uint64_t max_
   static_cast<AsyncDecodeTail&>(l) =
       async_decode_tail(l.tinfo + async_align(max_chunks * sizeof(ArTask)), max_chunks, ar_rows(window_cap), window_cap * elem);
   return l;
-}
-
-__device__ __forceinline__ ArSum ar_add(ArSum a, ArSum b) {
-  ArSum r;
-  r.s = a.s + b.s;
-  r.ovf = a.ovf | b.ovf | (r.s < a.s ? 1u : 0u);
-  r.reserved = 0;
-  return r;
-}
-__device__ __forceinline__ ArSum ar_sum(uint64_t s) { return ArSum{s, 0u, 0u}; }
-__device__ __forceinline__ ArSum ar_shfl_up(ArSum v, int d) {
-  return ArSum{__shfl_up_sync(0xffffffffu, v.s, d), __shfl_up_sync(0xffffffffu, v.ovf, d), 0u};
-}
-
-// Exclusive scan of one ArSum per thread over a CTA of NT threads; *total = the CTA's sum.  Every thread calls it.
-template <int NT>
-__device__ ArSum ar_block_scan(ArSum v, ArSum* total) {
-  __shared__ ArSum s_warp[NT / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  ArSum inc = v;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const ArSum o = ar_shfl_up(inc, d);
-    if (lane >= d) inc = ar_add(o, inc);
-  }
-  ArSum ex = ar_shfl_up(inc, 1);
-  if (lane == 0) ex = ar_sum(0);
-  if (lane == 31) s_warp[warp] = inc;
-  __syncthreads();
-  if (warp == 0) {
-    ArSum w = lane < NT / 32 ? s_warp[lane] : ar_sum(0);
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const ArSum o = ar_shfl_up(w, d);
-      if (lane >= d) w = ar_add(o, w);
-    }
-    if (lane < NT / 32) s_warp[lane] = w;
-  }
-  __syncthreads();
-  const ArSum r = warp ? ar_add(s_warp[warp - 1], ex) : ex;
-  *total = s_warp[NT / 32 - 1];
-  __syncthreads();  // s_warp may be reused by the next call
-  return r;
 }
 
 // ceil(max_chunks / AR_THREADS) CTAs.  Chunk k breaks the tiling when n[k] = 0 or out_offset[k] differs from out_offset[k - 1] + n[k - 1]
@@ -168,7 +120,7 @@ __global__ void __launch_bounds__(AR_THREADS) ar_chunks_kernel(const AsyncCheck*
     const uint64_t expect = k == 0 ? 0 : table[k - 1].out_offset + table[k - 1].n;
     if (r.n == 0 || r.out_offset != expect) atomicMin(&s_bad, uint32_t(k));
     else if (k + 1 == n_chunks && r.out_offset + r.n != chk->n_total) atomicMin(&s_bad, n_chunks);
-    marks[k] = ArMark{AR_NONE, 0u, 0u, AR_NONE, 0u, 0u, AR_NONE64};
+    marks[k] = ArMark{AR_NONE, 0u, 0u, AR_NONE, 0u, 0u, NONE64};
   }
   if (k == 0 && n_chunks == 0 && chk->status == ST_OK && chk->n_total != 0) s_bad = 0;  // no chunks: n_total must be 0
   __syncthreads();
@@ -185,7 +137,7 @@ __device__ __forceinline__ uint64_t ar_n_ranges(const ArArgs& g, const AsyncChec
 __global__ void __launch_bounds__(AR_THREADS) ar_count_kernel(ArArgs g, const AsyncCheck* __restrict__ chk, ArRangePart* __restrict__ rparts) {
   __shared__ unsigned long long s_bad;
   const uint32_t tid = threadIdx.x;
-  if (tid == 0) s_bad = AR_NONE64;
+  if (tid == 0) s_bad = NONE64;
   __syncthreads();
   const uint64_t n = ar_n_ranges(g, chk), n_total = chk->n_total;
   const uint64_t i = uint64_t(blockIdx.x) * AR_THREADS + tid;
@@ -195,8 +147,8 @@ __global__ void __launch_bounds__(AR_THREADS) ar_count_kernel(ArArgs g, const As
     cnt = r.count;
     if (r.count > n_total || r.start > n_total - r.count) atomicMin(&s_bad, 2ull * i);
   }
-  ArSum tot;
-  ar_block_scan<AR_THREADS>(ar_sum(cnt), &tot);
+  CarrySum tot;
+  block_exscan<AR_THREADS>(carry_sum(cnt), &tot);
   if (tid == 0) rparts[blockIdx.x] = ArRangePart{tot, s_bad, 0};
 }
 
@@ -206,37 +158,30 @@ __global__ void __launch_bounds__(AR_SCAN_THREADS) ar_scan_kernel(ArArgs g, cons
                                                                   ArRangePart* __restrict__ rparts, ArState* __restrict__ state) {
   __shared__ uint32_t s_tile;
   __shared__ unsigned long long s_bad;
-  __shared__ ArSum s_carry;
   const uint32_t tid = threadIdx.x;
   if (tid == 0) {
     s_tile = AR_NONE;
-    s_bad = AR_NONE64;
-    s_carry = ar_sum(0);
+    s_bad = NONE64;
   }
   __syncthreads();
-  const uint64_t n_cparts = ar_ctas(g.a.max_chunks), n_rparts = ar_ctas(g.max_ranges);
+  const uint64_t n_cparts = ctas_of<AR_THREADS>(g.a.max_chunks), n_rparts = ctas_of<AR_THREADS>(g.max_ranges);
   for (uint64_t c = tid; c < n_cparts; c += AR_SCAN_THREADS)
     if (cparts[c].tile_bad != AR_NONE) atomicMin(&s_tile, cparts[c].tile_bad);
-  for (uint64_t base = 0; base < n_rparts; base += AR_SCAN_THREADS) {
-    const uint64_t c = base + tid;
-    ArRangePart p = c < n_rparts ? rparts[c] : ArRangePart{ar_sum(0), AR_NONE64, 0};
-    if (p.bad != AR_NONE64) atomicMin(&s_bad, p.bad);
-    ArSum tot;
-    const ArSum ex = ar_block_scan<AR_SCAN_THREADS>(p.sum, &tot);
-    if (c < n_rparts) rparts[c].sum = ar_add(s_carry, ex);
-    __syncthreads();
-    if (tid == 0) s_carry = ar_add(s_carry, tot);
-    __syncthreads();
-  }
+  for (uint64_t c = tid; c < n_rparts; c += AR_SCAN_THREADS)
+    if (rparts[c].bad != NONE64) atomicMin(&s_bad, rparts[c].bad);
+  CarrySum total[1] = {};
+  cta_scan_inplace<AR_SCAN_THREADS, 1>(
+      n_rparts, [&](uint64_t c, int) { return rparts[c].sum; }, [&](uint64_t c, int, CarrySum v) { rparts[c].sum = v; }, total);
+  __syncthreads();
   if (tid != 0) return;
   ArState s;
   s.status = ST_OK;
-  s.bad = AR_NONE64;
-  s.bad_chunk = AR_NONE64;
+  s.bad = NONE64;
+  s.bad_chunk = NONE64;
   s.n_tasks = 0;
   s.reserved = 0;
   s.window_needed = 0;
-  s.total = s_carry.s;
+  s.total = total[0].s;
   if (*g.n_ranges > g.max_ranges) s.status = PCO_B200_ASYNC_TOO_MANY_RANGES;
   else if (chk->status != ST_OK) s.status = chk->status;
   else if (s_tile != AR_NONE) {
@@ -271,9 +216,9 @@ __global__ void __launch_bounds__(AR_THREADS) ar_mark_kernel(ArArgs g, const Asy
   const uint64_t i = uint64_t(blockIdx.x) * AR_THREADS + tid;
   PcoB200Range r{0, 0};
   if (i < n) r = g.ranges[i];
-  ArSum tot;
-  const ArSum ex = ar_add(rparts[blockIdx.x].sum, ar_block_scan<AR_THREADS>(ar_sum(r.count), &tot));
-  const ArSum inc = ar_add(ex, ar_sum(r.count));
+  CarrySum tot;
+  const CarrySum ex = carry_add(rparts[blockIdx.x].sum, block_exscan<AR_THREADS>(carry_sum(r.count), &tot));
+  const CarrySum inc = carry_add(ex, carry_sum(r.count));
   const bool valid = i < n && r.count <= n_total && r.start <= n_total - r.count;
   if (i < n && !ex.ovf && inc.ovf) atomicMin(reinterpret_cast<unsigned long long*>(&state->bad), 2ull * i + 1);
   uint32_t c0 = 0, c1 = 0;
@@ -317,48 +262,30 @@ __global__ void __launch_bounds__(AR_THREADS) ar_window_kernel(const AsyncCheck*
     touched = 1;
     w = (uint64_t(marks[k].hi) + BATCH_N - 1) / BATCH_N * BATCH_N;
   }
-  ArSum t_tot, w_tot;
-  ar_block_scan<AR_THREADS>(ar_sum(touched), &t_tot);
-  ar_block_scan<AR_THREADS>(ar_sum(w), &w_tot);
+  uint64_t t_tot, w_tot;
+  block_exscan<AR_THREADS>(touched, &t_tot);
+  block_exscan<AR_THREADS>(w, &w_tot);
   if (threadIdx.x == 0) {
-    cparts[blockIdx.x].n_touched = t_tot.s;
-    cparts[blockIdx.x].window = w_tot.s;
+    cparts[blockIdx.x].n_touched = t_tot;
+    cparts[blockIdx.x].window = w_tot;
   }
 }
 
 // One CTA: the touched chunks and windows of the CTAs scanned into offsets (in place), and every remaining refusal in the order of
 // pco_b200_decompress_ranges: a range past the file or where the counts overflow, then a total above dst_cap; then the window.
 __global__ void __launch_bounds__(AR_SCAN_THREADS) ar_gate_kernel(ArArgs g, ArChunkPart* __restrict__ cparts, ArState* __restrict__ state) {
-  __shared__ ArSum s_carry[2];
-  const uint32_t tid = threadIdx.x;
   if (state->status != ST_OK) return;
-  if (tid == 0) s_carry[0] = s_carry[1] = ar_sum(0);
-  __syncthreads();
-  const uint64_t n_cparts = ar_ctas(g.a.max_chunks);
-  for (uint64_t base = 0; base < n_cparts; base += AR_SCAN_THREADS) {
-    const uint64_t c = base + tid;
-    const ArChunkPart p = c < n_cparts ? cparts[c] : ArChunkPart{0, 0, 0, 0};
-    ArSum t_tot, w_tot;
-    const ArSum t_ex = ar_block_scan<AR_SCAN_THREADS>(ar_sum(p.n_touched), &t_tot);
-    const ArSum w_ex = ar_block_scan<AR_SCAN_THREADS>(ar_sum(p.window), &w_tot);
-    if (c < n_cparts) {
-      cparts[c].n_touched = s_carry[0].s + t_ex.s;
-      cparts[c].window = s_carry[1].s + w_ex.s;
-    }
-    __syncthreads();
-    if (tid == 0) {
-      s_carry[0] = ar_add(s_carry[0], t_tot);
-      s_carry[1] = ar_add(s_carry[1], w_tot);
-    }
-    __syncthreads();
-  }
-  if (tid != 0) return;
+  auto sum = [&](uint64_t c, int k) -> uint64_t& { return k ? cparts[c].window : cparts[c].n_touched; };
+  uint64_t total[2] = {};
+  cta_scan_inplace<AR_SCAN_THREADS, 1>(
+      ctas_of<AR_THREADS>(g.a.max_chunks), [&](uint64_t c, int k) { return sum(c, k); }, [&](uint64_t c, int k, uint64_t v) { sum(c, k) = v; }, total);
+  if (threadIdx.x != 0) return;
   ArState s = *state;
-  if (s.bad != AR_NONE64) s.status = (s.bad & 1) ? PCO_B200_ASYNC_RANGE_OVERFLOW : PCO_B200_ASYNC_RANGE_PAST;
+  if (s.bad != NONE64) s.status = (s.bad & 1) ? PCO_B200_ASYNC_RANGE_OVERFLOW : PCO_B200_ASYNC_RANGE_PAST;
   else if (s.total > g.a.dst_cap) s.status = PCO_B200_ASYNC_DST_SHORT;
-  if (s.status == ST_OK || s.status == PCO_B200_ASYNC_DST_SHORT) s.window_needed = s_carry[1].s;  // the windows are known once the ranges are
+  if (s.status == ST_OK || s.status == PCO_B200_ASYNC_DST_SHORT) s.window_needed = total[1];  // the windows are known once the ranges are
   if (s.status == ST_OK && s.window_needed > g.window_cap) s.status = PCO_B200_ASYNC_WINDOW;
-  s.n_tasks = s.status == ST_OK ? uint32_t(s_carry[0].s) : 0u;
+  s.n_tasks = s.status == ST_OK ? uint32_t(total[0]) : 0u;
   *state = s;
 }
 
@@ -372,13 +299,13 @@ __global__ void __launch_bounds__(AR_THREADS) ar_tasks_kernel(ArArgs g, const As
                                                               uint8_t* __restrict__ stage) {
   const uint64_t k = uint64_t(blockIdx.x) * AR_THREADS + threadIdx.x;
   const uint32_t n_tasks = state->n_tasks;
-  ArMark m{AR_NONE, 0u, 0u, AR_NONE, 0u, 0u, AR_NONE64};
+  ArMark m{AR_NONE, 0u, 0u, AR_NONE, 0u, 0u, NONE64};
   if (n_tasks && k < chk->n_chunks) m = marks[k];
   const uint64_t touched = m.n_pieces > 0 ? 1 : 0;
   const uint64_t w = touched ? (uint64_t(m.hi) + BATCH_N - 1) / BATCH_N * BATCH_N : 0;
-  ArSum tot;
-  const uint64_t t = cparts[blockIdx.x].n_touched + ar_block_scan<AR_THREADS>(ar_sum(touched), &tot).s;
-  const uint64_t w0 = cparts[blockIdx.x].window + ar_block_scan<AR_THREADS>(ar_sum(w), &tot).s;
+  uint64_t tot;
+  const uint64_t t = cparts[blockIdx.x].n_touched + block_exscan<AR_THREADS>(touched, &tot);
+  const uint64_t w0 = cparts[blockIdx.x].window + block_exscan<AR_THREADS>(w, &tot);
   if (touched) {
     const bool lone = m.n_pieces == 1;
     const uint8_t* at = lone ? dst + m.lone_dst * g.elem : stage + w0 * g.elem;
@@ -465,7 +392,7 @@ __global__ void __launch_bounds__(AR_SCAN_THREADS) ar_finish_kernel(const ArStat
                                                                     const uint32_t* __restrict__ statuses, PcoB200AsyncRangesStatus* __restrict__ out) {
   __shared__ unsigned long long s_min;
   const uint32_t tid = threadIdx.x;
-  if (tid == 0) s_min = AR_NONE64;
+  if (tid == 0) s_min = NONE64;
   __syncthreads();
   const ArState s = *state;
   for (uint32_t t = tid; t < s.n_tasks; t += AR_SCAN_THREADS)
@@ -475,8 +402,8 @@ __global__ void __launch_bounds__(AR_SCAN_THREADS) ar_finish_kernel(const ArStat
   PcoB200AsyncRangesStatus r;
   r.kind = PCO_B200_OK;
   r.device_status = ST_OK;
-  r.range = AR_NONE64;
-  r.chunk = AR_NONE64;
+  r.range = NONE64;
+  r.chunk = NONE64;
   r.window_needed = s.window_needed;
   r.n_written = 0;
   const bool known = s.status == ST_OK || s.status == PCO_B200_ASYNC_DST_SHORT || s.status == PCO_B200_ASYNC_WINDOW;
@@ -486,7 +413,7 @@ __global__ void __launch_bounds__(AR_SCAN_THREADS) ar_finish_kernel(const ArStat
     r.device_status = s.status;
     if (s.status == PCO_B200_ASYNC_RANGE_PAST || s.status == PCO_B200_ASYNC_RANGE_OVERFLOW) r.range = s.bad >> 1;
     if (s.status == PCO_B200_ASYNC_INDEX_TILING) r.chunk = s.bad_chunk;
-  } else if (s_min != AR_NONE64) {
+  } else if (s_min != NONE64) {
     const uint32_t t = uint32_t(s_min);
     const uint32_t st = statuses[t];
     r.kind = async_kind_of(st);

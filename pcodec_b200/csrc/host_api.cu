@@ -2669,7 +2669,7 @@ PcoB200Error pco_b200_decompress_ranges_async(const PcoB200AsyncRangesPlan* plan
   g.window_cap = plan->window_cap;
   g.max_ranges = mr;
   g.elem = elem;
-  const uint32_t cb = uint32_t(ar_ctas(mc)), rb = uint32_t(ar_ctas(mr));
+  const uint32_t cb = uint32_t(ctas_of<AR_THREADS>(mc)), rb = uint32_t(ctas_of<AR_THREADS>(mr));
 
   ln.begin("async_check_kernel");
   async_check_kernel<<<(mc + ASYNC_CHECK_RECS - 1) / ASYNC_CHECK_RECS, ASYNC_THREADS, 0, stream>>>(g.a, chk, table);
@@ -2807,7 +2807,7 @@ PcoB200Error pco_b200_decompress_files_async(const PcoB200AsyncFilesPlan* plan, 
   g.n_files = n_files;
   g.max_files = mf;
   g.max_chunks = mc;
-  const uint32_t fb = uint32_t(af_ctas(mf)), tb = uint32_t(std::max(af_ctas(mf), af_ctas(mc)));
+  const uint32_t fb = uint32_t(ctas_of<AF_THREADS>(mf)), tb = uint32_t(std::max(ctas_of<AF_THREADS>(mf), ctas_of<AF_THREADS>(mc)));
 
   ln.begin("af_files_kernel");
   af_files_kernel<<<fb, AF_THREADS, 0, stream>>>(g, chk, fst, fchk, merges, parts);
@@ -2942,7 +2942,7 @@ PcoB200Error pco_b200_decompress_pages_async(const PcoB200AsyncPagesPlan* plan, 
   g.max_pages = mp;
   // the frames as one file: every page's frame below frame_cap, the pad frame behind them
   const FileParams fp{d_frames, lay.pad_frame + 64, plan->dtype, 0, 4};
-  const uint32_t pb = uint32_t(ap_ctas(mp));
+  const uint32_t pb = uint32_t(ctas_of<AP_THREADS>(mp));
 
   ln.begin("ap_pages_kernel");
   ap_pages_kernel<<<pb, AP_THREADS, 0, stream>>>(g, chk, parts);

@@ -12,6 +12,7 @@
 // Byte copies go through cta_copy_bytes (gather_kernels.cuh): aligned 16-byte stores assembled from unaligned sources.
 #pragma once
 #include "../../include/pco_b200.h"
+#include "cta_scan.cuh"
 #include "decode_kernels.cuh"
 #include "gather_kernels.cuh"
 
@@ -136,54 +137,21 @@ __global__ void __launch_bounds__(WRAP_THREADS) frame_pages_kernel(const uint8_t
 __global__ void __launch_bounds__(1024) chunk_refs_kernel(const uint8_t* __restrict__ file, const IndexChunk* __restrict__ chunks, const uint64_t* __restrict__ sizes,
                                                           uint32_t n_chunks, uint32_t dtype, PcoB200PageRef* __restrict__ refs, uint64_t* __restrict__ tot,
                                                           uint32_t* __restrict__ err) {
-  __shared__ uint64_t warp_tot[2][32];
-  __shared__ uint64_t carry[2];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid == 0) { carry[0] = 0; carry[1] = 0; }
-  __syncthreads();
-  for (uint32_t base = 0; base < n_chunks; base += 1024) {
-    const uint32_t i = base + tid;
+  for (uint32_t i = threadIdx.x; i < n_chunks; i += 1024) {
+    const uint64_t sz = sizes[i];
     uint64_t ml = 0, pl = 0;
-    if (i < n_chunks) {
-      const uint64_t sz = sizes[i];
-      bool cold = false;
-      const uint32_t st = sz >= 4 ? wrapped_meta_len(file + chunks[i].chunk_offset + 4, sz - 4, dtype, &ml, &cold) : ST_CORRUPTION;
-      if (st != ST_OK || ml > sz - 4) { *err = ST_CORRUPTION; ml = 0; }
-      else pl = sz - 4 - ml;
-    }
-    uint64_t a = ml, b = pl;  // inclusive scans over the tile
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const uint64_t oa = __shfl_up_sync(0xffffffffu, a, d), ob = __shfl_up_sync(0xffffffffu, b, d);
-      if (lane >= d) { a += oa; b += ob; }
-    }
-    if (lane == 31) { warp_tot[0][warp] = a; warp_tot[1][warp] = b; }
-    __syncthreads();
-    if (warp == 0) {
-      uint64_t ta = warp_tot[0][lane], tb = warp_tot[1][lane];
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) {
-        const uint64_t oa = __shfl_up_sync(0xffffffffu, ta, d), ob = __shfl_up_sync(0xffffffffu, tb, d);
-        if (lane >= d) { ta += oa; tb += ob; }
-      }
-      warp_tot[0][lane] = ta;
-      warp_tot[1][lane] = tb;
-    }
-    __syncthreads();
-    if (i < n_chunks) {
-      PcoB200PageRef r;
-      r.meta_offset = carry[0] + (warp ? warp_tot[0][warp - 1] : 0) + a - ml;
-      r.meta_len = ml;
-      r.page_offset = carry[1] + (warp ? warp_tot[1][warp - 1] : 0) + b - pl;
-      r.page_len = pl;
-      r.page_n = chunks[i].n;
-      refs[i] = r;
-    }
-    __syncthreads();
-    if (tid == 0) { carry[0] += warp_tot[0][31]; carry[1] += warp_tot[1][31]; }
-    __syncthreads();
+    bool cold = false;
+    const uint32_t st = sz >= 4 ? wrapped_meta_len(file + chunks[i].chunk_offset + 4, sz - 4, dtype, &ml, &cold) : ST_CORRUPTION;
+    if (st != ST_OK || ml > sz - 4) { *err = ST_CORRUPTION; ml = 0; }
+    else pl = sz - 4 - ml;
+    refs[i] = PcoB200PageRef{0, ml, 0, pl, chunks[i].n};
   }
-  if (tid == 0) { tot[0] = carry[0]; tot[1] = carry[1]; }
+  __syncthreads();
+  uint64_t total[2] = {};
+  cta_scan_inplace<1024, 1>(
+      n_chunks, [&](uint64_t i, int k) { return k ? refs[i].page_len : refs[i].meta_len; },
+      [&](uint64_t i, int k, uint64_t v) { (k ? refs[i].page_offset : refs[i].meta_offset) = v; }, total);
+  if (threadIdx.x == 0) { tot[0] = total[0]; tot[1] = total[1]; }
 }
 
 // One CTA per chunk: its meta to metas + meta_offset, its page to pages + page_offset - unless the totals chunk_refs_kernel found do
