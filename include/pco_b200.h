@@ -832,6 +832,74 @@ PcoB200Error pco_b200_decompress_pages_async(const PcoB200AsyncPagesPlan *plan, 
  * NULL) to the sum of page_n. */
 PcoB200Error pco_b200_decompress_pages_async_result(const PcoB200AsyncPagesStatus *host_status, size_t *n_written);
 
+/* ---- asynchronous filter of wrapped-format pages (no reference counterpart): pco_b200_decompress_pages_async with a predicate pushed
+ * into the decoder.  A GPU columnar reader that pruned pages by their statistics still has to find the rows of each surviving page that
+ * pass `lo <= x <= hi`; this call decodes the pages and writes only those numbers, in row order, with their positions, so the decoded
+ * pages never reach HBM whole.  It only enqueues kernels on the caller's stream and returns at once; it makes no synchronising, allocating
+ * or host-to-device copy call and refers to no memory of the library's per-thread scratch, so it can be captured in a CUDA graph, and a
+ * captured call may be replayed after pco_b200_thread_release or after any other call.  A plan made once outside any capture fixes the
+ * grids from its capacities; the refs, their count and the interval are read on the device, so one captured graph serves different refs,
+ * a different count, different bytes and different bounds on each replay. */
+typedef struct PcoB200Interval {  /* the closed interval [lo, hi], in device memory */
+  uint64_t lo_bits;               /* lo as the bit pattern of a number of the plan's dtype, zero-extended (higher bits are ignored) */
+  uint64_t hi_bits;               /* hi, likewise */
+} PcoB200Interval;
+
+typedef struct PcoB200AsyncFilterPlan {  /* filled by pco_b200_filter_pages_async_plan; treat as opaque */
+  uint32_t dtype, reserved;
+  uint64_t metas_cap, pages_cap, max_pages, rows_cap, frame_cap, out_cap;
+  uint64_t workspace_bytes;              /* device workspace one in-flight call needs */
+} PcoB200AsyncFilterPlan;
+
+typedef struct PcoB200AsyncFilterStatus {  /* written on the device by every call */
+  uint32_t kind;                           /* PcoB200Error */
+  uint32_t device_status;                  /* the device word behind it: as PcoB200AsyncPagesStatus, or PCO_B200_FILTER_OUT_FULL */
+  uint64_t page;                           /* the page the outcome names (UINT64_MAX if none) */
+  uint64_t n_written;                      /* the sum of page_n (the rows filtered), once every page passed its checks (0 on a failure) */
+  uint64_t n_pages;                        /* *n_pages as the call read it */
+  uint64_t frames_needed;                  /* bytes of framed pages the batch needs, also when above frame_cap (0 when refused earlier) */
+  uint64_t n_matches;                      /* matches written to out_values / out_positions (0 on a failure) */
+  uint64_t matches_needed;                 /* matches in all, also when above out_cap (0 on a failure) */
+} PcoB200AsyncFilterStatus;
+
+/* device_status of a filter whose matches do not fit */
+enum {
+  PCO_B200_FILTER_OUT_FULL = 0x201  /* more than out_cap matches, matches_needed (PCO_B200_IO); the first out_cap are written */
+};
+
+/* Makes a plan for filters of up to max_pages pages of dtype, whose refs point into metas_cap bytes of metas and pages_cap bytes of pages,
+ * holding at most rows_cap numbers in all (the role dst_cap plays in pco_b200_decompress_pages_async), of which at most out_cap are
+ * written; frame_cap bounds the framed pages as in that call.  Checked before the device is touched: dtype (PCO_B200_INVALID_TYPE),
+ * max_pages in 1 .. 2^31 - 1, rows_cap, frame_cap and out_cap at most 2^56 (PCO_B200_INVALID_ARGUMENT).  Then *plan is filled and the
+ * one-time device set-up runs on the current device, which the calls must use (kernel attributes, and every kernel the call launches
+ * loaded); without a device that is PCO_B200_CUDA.
+ * workspace_bytes is pco_b200_decompress_pages_async_plan's formula with dst_cap = rows_cap, plus these regions, each rounded up to 256
+ * bytes, with m = max_pages, S = floor(rows_cap / 256) + m batch slots and E the bytes of a number of dtype: 40 (the pages status), 16
+ * (state), 4 S (slot counts), 8 S (slot rows), 8 ceil(S / 256) (CTA sums), E rows_cap (staged values) and rows_cap (staged offsets). */
+PcoB200Error pco_b200_filter_pages_async_plan(unsigned char dtype, size_t metas_cap, size_t pages_cap, size_t max_pages, size_t rows_cap,
+                                              size_t frame_cap, size_t out_cap, PcoB200AsyncFilterPlan *plan);
+/* Enqueues the filter of the pages refs[0 : *n_pages) names on `cuda_stream`, and the outcome into *status; returns without waiting.
+ * metas (metas_cap bytes), pages (pages_cap bytes; may be the same buffer as metas), refs (PcoB200PageRef[max_pages]), n_pages (one
+ * uint64_t), interval (one PcoB200Interval), out_values (out_cap numbers), out_positions (uint64_t[out_cap]), n_matches (one uint64_t),
+ * workspace (plan->workspace_bytes, 256-byte aligned) and status are device pointers; one workspace serves one call in flight.
+ * The selection is every number x of the concatenation pco_b200_decompress_pages_async writes for the same arguments (with dst_cap =
+ * rows_cap) with lo <= x <= hi.  Integers compare in their signed or unsigned order; floats (f16, f32, f64) as IEEE values: a NaN never
+ * matches, a NaN bound selects nothing, and -0.0 equals +0.0.  lo > hi selects nothing.  The matches are written in row order:
+ * out_values[k] is the k-th match (its bit pattern) and out_positions[k] its index in the concatenation; *n_matches gets their count.
+ * Refusals and failures are pco_b200_decompress_pages_async's, in its order, with its kinds and naming the same page; they write 0 to
+ * *n_matches and nothing to out_values or out_positions.  When the pages decode and there are more than out_cap matches, the kind is
+ * PCO_B200_IO (PCO_B200_FILTER_OUT_FULL) with matches_needed reported: the first out_cap matches in row order are written, and nothing
+ * beyond out_cap.  The return value covers the host side only: null pointers, an unaligned workspace or a plan that was not filled
+ * (PCO_B200_INVALID_ARGUMENT), a launch the runtime refuses (PCO_B200_CUDA).  With pco_b200_profile_enable(1), a call outside a stream
+ * capture records its kernel spans for pco_b200_profile_last; a call inside a capture records none. */
+PcoB200Error pco_b200_filter_pages_async(const PcoB200AsyncFilterPlan *plan, const void *metas, const void *pages, const PcoB200PageRef *refs,
+                                         const uint64_t *n_pages, const PcoB200Interval *interval, void *out_values, uint64_t *out_positions,
+                                         uint64_t *n_matches, void *workspace, PcoB200AsyncFilterStatus *status, void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory at a point of the caller's choosing.  Returns the kind,
+ * sets the last-error message as pco_b200_decompress_pages_async_result words it ("page 17: ...") and, when the kind is OK, sets
+ * *n_matches (may be NULL) to the number of matches. */
+PcoB200Error pco_b200_filter_pages_async_result(const PcoB200AsyncFilterStatus *host_status, size_t *n_matches);
+
 /* ---- asynchronous batch compress into wrapped-format chunks (no reference counterpart): pco_b200_compress_wrapped over a batch of
  * arrays, with the array sizes, their count and every buffer in device memory.  A GPU writer of a container that embeds pco (a columnar
  * file whose column chunks a kernel sized, a page store) compresses every column chunk behind the step that produced it, with no copy to

@@ -859,6 +859,79 @@ __device__ __forceinline__ void win_store8(const WinTask& w, uint32_t b, int lan
       if (j0 + e >= w.lo && j0 + e < w.hi) out[j0 + e - w.lo] = r[e];
   }
 }
+
+// ---------------------------------------------------------------------------
+// Filter mode (the FILT instantiations, pco_b200_filter_pages_async): a batch stores only its numbers inside a closed interval, compactly,
+// in its own staging slot.  Numbers are staged in the row domain: the batch whose first number is number `row` of the pages'
+// concatenation keeps its matches at stage[row ..] (values, `out`) and offs[row ..] (their offsets in the batch, one byte each), so the
+// slot can never overflow into another batch's.  Its count goes to counts[slot] and, when it has matches, its row to rows[slot]; the
+// slot of batch b of page p (the page's numbers start at row O) is O / 256 + p + b, distinct for every batch of a batch of pages.
+// ---------------------------------------------------------------------------
+struct FiltStage {
+  const uint64_t* interval;   // PcoB200Interval: lo_bits, hi_bits (zero-extended bit patterns of the plan's number type)
+  const uint32_t* fast_page;  // decode-table record -> its page
+  uint32_t* counts;           // per slot: the batch's matches
+  uint64_t* rows;             // per slot with matches: the batch's first row
+  uint8_t* offs;              // per row: a staged match's offset in its batch
+};
+// The interval as keys of the order-preserving map below: a number x matches when any && key(x) - lo <= span (mod 2^bits).
+struct FiltKey {
+  uint64_t lo, span;
+  uint32_t any, kind;  // kind: 0 unsigned, 1 signed, 2 float
+};
+// The unsigned key whose order is the number's: signed integers flip the sign bit; floats flip every bit when negative, else the sign
+// bit (-0.0 then sits right below +0.0, NaNs above +inf or below -inf).
+template <typename L>
+__device__ __forceinline__ L filt_key(L x, uint32_t kind) {
+  constexpr L TOP = L(L(1) << (LT<L>::BITS - 1));
+  if (kind == 1) return L(x ^ TOP);
+  if (kind == 2) return (x & TOP) ? L(~x) : L(x | TOP);
+  return x;
+}
+template <typename L>
+__device__ __forceinline__ FiltKey filt_bounds(const uint64_t* __restrict__ interval, uint32_t dtype) {
+  constexpr L TOP = L(L(1) << (LT<L>::BITS - 1));
+  constexpr L EXP = LT<L>::BITS == 16 ? L(0x7c00u) : LT<L>::BITS == 32 ? L(0x7f800000u) : L(0x7ff0000000000000ull);
+  const uint32_t kind = nt_is_float(dtype) ? 2u : nt_is_signed(dtype) ? 1u : 0u;
+  L lo = L(interval[0]), hi = L(interval[1]);
+  bool any = true;
+  if (kind == 2) {
+    if (L(lo & L(~TOP)) > EXP || L(hi & L(~TOP)) > EXP) any = false;  // a NaN bound selects nothing
+    if (L(lo & L(~TOP)) == 0) lo = TOP;                                 // -0.0 == +0.0: lo takes -0.0, hi +0.0
+    if (L(hi & L(~TOP)) == 0) hi = 0;
+  }
+  const L klo = filt_key<L>(lo, kind), khi = filt_key<L>(hi, kind);
+  if (klo > khi) any = false;
+  return FiltKey{uint64_t(klo), uint64_t(L(khi - klo)), any ? 1u : 0u, kind};
+}
+// The lane's 8 numbers of a batch of `cnt` numbers (row `row`, slot `slot`) tested against the interval; the warp's ballots rank the
+// matches in row order and each lane writes its own behind the matches of the lanes below it.  All 32 lanes call it.
+template <typename L>
+__device__ __forceinline__ void filt_store8(const FiltStage& f, const FiltKey& k, L* __restrict__ stage, uint64_t row, uint64_t slot, uint32_t cnt,
+                                            int lane, const L (&r)[8]) {
+  uint32_t m = 0, below = 0;
+  const uint32_t lt = (1u << lane) - 1;
+#pragma unroll
+  for (int e = 0; e < 8; e++) {
+    const bool hit = k.any && uint32_t(lane * 8 + e) < cnt && L(filt_key<L>(r[e], k.kind) - L(k.lo)) <= L(k.span);
+    const uint32_t bal = __ballot_sync(0xffffffffu, hit);
+    below += __popc(bal & lt);
+    m |= uint32_t(hit) << e;
+  }
+  const uint32_t total = __shfl_sync(0xffffffffu, below + __popc(m), 31);
+  uint64_t at = row + below;
+#pragma unroll
+  for (int e = 0; e < 8; e++)
+    if ((m >> e) & 1u) {
+      stage[at] = r[e];
+      f.offs[at] = uint8_t(lane * 8 + e);
+      at++;
+    }
+  if (lane == 0) {
+    f.counts[slot] = total;
+    if (total) f.rows[slot] = row;
+  }
+}
 template <typename L>
 __device__ __forceinline__ void load8(const L* __restrict__ src, L (&r)[8]) {
   if (sizeof(L) == 8) {
@@ -1132,11 +1205,13 @@ __global__ void __launch_bounds__(SW_THREADS) symwalk_kernel(FileParams fp, cons
 // host launches both and a CTA leaves at once when its chunk belongs to the other (symwalk_kernel recorded each
 // chunk's var count) - one-var chunks then run with the registers of one var and a third CTA per SM.
 // WIN: window mode (symwalk_kernel<true> made the rows; wins[t] says which numbers of task t to store and where; out and out_len are unused).
-template <typename L, int NV, bool WIN = false>
+// FILT: filter mode (filt_store8: only the numbers inside *filt.interval are staged, in row order, with out as the value staging).
+template <typename L, int NV, bool WIN = false, bool FILT = false>
 __global__ void __launch_bounds__(DEC_THREADS, NV == 1 ? PCOB_DEC_NV1_BLOCKS : 2)
 decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __restrict__ statuses, const uint8_t* __restrict__ index_base, uint64_t index_len,
               L* __restrict__ out, uint64_t out_len, const Binoms* __restrict__ binoms, const uint8_t* __restrict__ d_syms,
-              const uint32_t* __restrict__ d_offs, const uint8_t* __restrict__ d_nvars, const WinTask* __restrict__ wins = nullptr) {
+              const uint32_t* __restrict__ d_offs, const uint8_t* __restrict__ d_nvars, const WinTask* __restrict__ wins = nullptr,
+              FiltStage filt = {}) {
   if (d_nvars[blockIdx.x] != NV) return;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   DecodeSmem& sm = *reinterpret_cast<DecodeSmem*>(smem_raw);
@@ -1246,6 +1321,12 @@ decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __
   const int kind = is_float ? 2 : (is_signed ? 1 : 0);
   const uint32_t mode = sm.hdr.mode;
   uint32_t end_err = 0;
+  FiltKey fkey{};
+  uint64_t fslot0 = 0;
+  if constexpr (FILT) {
+    fkey = filt_bounds<L>(filt.interval, fp.dtype);
+    fslot0 = task.out_offset / BATCH_N + filt.fast_page[blockIdx.x];
+  }
   const uint64_t row0 = WIN ? wins[blockIdx.x].row0 : scratch_row0(task.out_offset, blockIdx.x);
   // chunk-relative bit position of batch b's offsets section for var v
   auto off_of = [&](uint32_t v, uint32_t b) -> uint32_t {
@@ -1506,7 +1587,9 @@ decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __
             res[e] = from_latent_kind<L>(L(L(pq << k) + lowest), 2);
           }
         }
-        if constexpr (WIN) {
+        if constexpr (FILT) {
+          filt_store8<L>(filt, fkey, out, task.out_offset + uint64_t(b) * BATCH_N, fslot0 + b, out_cnt, lane, res);
+        } else if constexpr (WIN) {
           win_store8<L>(wins[blockIdx.x], b, lane, res);
         } else if (out_cnt == BATCH_N && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
           store8<L>(dst, res, lane);  // 16-byte stores; a chunk that starts at an odd element offset takes the element-wise path

@@ -7,6 +7,7 @@
 #include "async_compress.cuh"
 #include "async_compress_files.cuh"
 #include "async_compress_wrapped.cuh"
+#include "async_filter_kernels.cuh"
 #include "async_files_kernels.cuh"
 #include "async_index_kernels.cuh"
 #include "async_kernels.cuh"
@@ -40,7 +41,7 @@ namespace pcob200 {
 // The context follows the thread's current device: a cudaSetDevice between calls drops the scratch of the previous device.
 struct Context {
   int device = -1;
-  bool attrs_set[2] = {false, false};  // set_decode_attrs<WIN> has run
+  bool attrs_set[3] = {false, false, false};  // set_decode_attrs<WIN, FILT> has run (index WIN + 2 FILT)
   bool initialized = false;
   bool device_ok = false;
   std::string device_err;
@@ -79,7 +80,7 @@ static void reset_context(Context& c) {
   c.d_binoms = nullptr;
   c.initialized = false;
   c.device_ok = false;
-  c.attrs_set[0] = c.attrs_set[1] = false;
+  c.attrs_set[0] = c.attrs_set[1] = c.attrs_set[2] = false;
 }
 
 static PcoB200Error ensure_device(Context& c) {
@@ -147,20 +148,22 @@ struct DecodeOutcome {
   bool terminated = false;
 };
 
-// Shared-memory attributes of the decode kernels (the window-mode instantiations when WIN), set once per context before their first launch.
-template <bool WIN>
+// Shared-memory attributes of the decode kernels (the window-mode instantiations when WIN, the filter-mode ones when FILT), set once per
+// context before their first launch.
+template <bool WIN, bool FILT = false>
 static PcoB200Error set_decode_attrs(Context& c) {
-  if (c.attrs_set[WIN]) return PCO_B200_OK;
-  c.attrs_set[WIN] = true;
+  static_assert(!(WIN && FILT), "no instantiation is both");
+  if (c.attrs_set[WIN + 2 * FILT]) return PCO_B200_OK;
+  c.attrs_set[WIN + 2 * FILT] = true;
   auto max_shared = [](auto* kernel, size_t smem) {
     const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
     return e != cudaSuccess ? e : cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, int(cudaSharedmemCarveoutMaxShared));
   };
   PCOB_CUDA_TRY(max_shared(symwalk_kernel<WIN>, sizeof(SymWalkSmem)));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint64_t, WIN>, sizeof(FusedSmem)));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint32_t, WIN>, sizeof(FusedSmem)));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint16_t, WIN>, sizeof(FusedSmem)));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint8_t, WIN>, sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint64_t, WIN, FILT>, sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint32_t, WIN, FILT>, sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint16_t, WIN, FILT>, sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint8_t, WIN, FILT>, sizeof(FusedSmem)));
   return PCO_B200_OK;
 }
 
@@ -772,18 +775,19 @@ static PcoB200Error load_kernels(std::initializer_list<const void*> kernels) {
 // The PcoB200Error of an asynchronous call's status kind, as its *_result function returns it (a kind no call writes reads as Corruption)
 static PcoB200Error async_result_kind(uint32_t kind) { return kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(kind) : PCO_B200_CORRUPTION; }
 
-// The set-up of an asynchronous decompress plan: the device, the decode kernels' attributes (the window-mode instantiations when WIN),
-// and loaded: the decode stage's kernels for dtype, the call's catch-all kernel (cold(tag) for a latent type tag) and the call's `kernels`.
-template <bool WIN, typename Cold>
+// The set-up of an asynchronous decompress plan: the device, the decode kernels' attributes (the window-mode instantiations when WIN, the
+// filter-mode ones when FILT), and loaded: the decode stage's kernels for dtype, the call's catch-all kernel (cold(tag) for a latent type
+// tag) and the call's `kernels`.
+template <bool WIN, bool FILT = false, typename Cold>
 static PcoB200Error async_decode_setup(unsigned char dtype, Cold cold, std::initializer_list<const void*> kernels) {
   Context& c = ctx();
   if (PcoB200Error e = ensure_device(c)) return e;
-  if (PcoB200Error e = set_decode_attrs<WIN>(c)) return e;
+  if (PcoB200Error e = set_decode_attrs<WIN, FILT>(c)) return e;
   if (PcoB200Error e = load_kernels(kernels)) return e;
   return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
     using L = decltype(tag);
-    return load_kernels({(const void*)fused_narrow_kernel<L, WIN>, (const void*)symwalk_kernel<WIN>, (const void*)decode_kernel<L, 1, WIN>,
-                         (const void*)decode_kernel<L, 2, WIN>, cold(tag)});
+    return load_kernels({(const void*)fused_narrow_kernel<L, WIN, FILT>, (const void*)symwalk_kernel<WIN>, (const void*)decode_kernel<L, 1, WIN, FILT>,
+                         (const void*)decode_kernel<L, 2, WIN, FILT>, cold(tag)});
   });
 }
 
@@ -847,15 +851,16 @@ struct DecodeStage {
   void* dst;
   uint64_t dst_cap;
   const WinTask* wins;
+  FiltStage filt;  // FILT: dst is the value staging (decode_kernels.cuh, filt_store8)
 };
-template <bool WIN>
+template <bool WIN, bool FILT = false>
 static void enqueue_decode_stage(const AsyncLaunch& ln, const DecodeStage& d) {
   const cudaStream_t stream = ln.stream;
   ln.begin("fused_narrow_kernel");
   dispatch_latent(d.fp.dtype, [&](auto tag) {
     using L = decltype(tag);
-    fused_narrow_kernel<L, WIN><<<d.slots, FZ_THREADS, sizeof(FusedSmem), stream>>>(d.fp, d.table, d.index, d.index_len, d.st, d.cls, static_cast<L*>(d.dst),
-                                                                                   d.dst_cap, d.wins);
+    fused_narrow_kernel<L, WIN, FILT><<<d.slots, FZ_THREADS, sizeof(FusedSmem), stream>>>(d.fp, d.table, d.index, d.index_len, d.st, d.cls,
+                                                                                         static_cast<L*>(d.dst), d.dst_cap, d.wins, d.filt);
     return 0;
   });
   ln.end();
@@ -865,10 +870,10 @@ static void enqueue_decode_stage(const AsyncLaunch& ln, const DecodeStage& d) {
   ln.begin("decode_kernel");
   dispatch_latent(d.fp.dtype, [&](auto tag) {
     using L = decltype(tag);
-    decode_kernel<L, 1, WIN><<<d.slots, DEC_THREADS, sizeof(DecodeSmem), stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst), d.dst_cap,
-                                                                                  d.binoms, d.syms, d.offs, d.cls, d.wins);
-    decode_kernel<L, 2, WIN><<<d.slots, DEC_THREADS, sizeof(DecodeSmem), stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst), d.dst_cap,
-                                                                                  d.binoms, d.syms, d.offs, d.cls, d.wins);
+    decode_kernel<L, 1, WIN, FILT><<<d.slots, DEC_THREADS, sizeof(DecodeSmem), stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst),
+                                                                                        d.dst_cap, d.binoms, d.syms, d.offs, d.cls, d.wins, d.filt);
+    decode_kernel<L, 2, WIN, FILT><<<d.slots, DEC_THREADS, sizeof(DecodeSmem), stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst),
+                                                                                        d.dst_cap, d.binoms, d.syms, d.offs, d.cls, d.wins, d.filt);
     return 0;
   });
   ln.end();
@@ -2902,19 +2907,12 @@ PcoB200Error pco_b200_decompress_pages_async_plan(unsigned char dtype, size_t me
                                     (const void*)ap_finish_kernel});
 }
 
-PcoB200Error pco_b200_decompress_pages_async(const PcoB200AsyncPagesPlan* plan, const void* metas, const void* pages, const PcoB200PageRef* refs,
-                                             const uint64_t* n_pages, void* dst, void* workspace, PcoB200AsyncPagesStatus* status, void* cuda_stream) {
-  if (!plan || !metas || !pages || !refs || !n_pages || !workspace || !status || (!dst && plan->dst_cap))
-    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
-  if (!ap_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_decompress_pages_async_plan");
-  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
-  AsyncLaunch ln;
-  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+// The launches of pco_b200_decompress_pages_async over the workspace `ws` laid out by `lay`: the front end, the decode stage, the
+// catch-all decoder into dst and ap_finish_kernel into *status.  With `filt` the decode stage runs its filter-mode instantiations and dst
+// is their value staging (pco_b200_filter_pages_async).
+static void enqueue_pages(const AsyncLaunch& ln, const ApArgs& g, const ApLayout& lay, uint8_t* ws, void* dst, const FiltStage* filt,
+                          PcoB200AsyncPagesStatus* status) {
   const cudaStream_t stream = ln.stream;
-
-  const uint32_t mp = uint32_t(plan->max_pages);
-  const ApLayout lay = ap_layout(mp, plan->dst_cap, plan->frame_cap);
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
   AsyncCheck* chk = reinterpret_cast<AsyncCheck*>(ws);
   ApState* state = reinterpret_cast<ApState*>(ws + lay.state);
   WrappedPage* tab = reinterpret_cast<WrappedPage*>(ws + lay.tab);
@@ -2929,20 +2927,9 @@ PcoB200Error pco_b200_decompress_pages_async(const PcoB200AsyncPagesPlan* plan, 
   uint32_t* fast_page = reinterpret_cast<uint32_t*>(ws + lay.fast_page);
   uint32_t* cold_list = reinterpret_cast<uint32_t*>(ws + lay.cold_list);
   uint32_t* d_st = reinterpret_cast<uint32_t*>(ws + lay.st);
-  ApArgs g;
-  g.metas = static_cast<const uint8_t*>(metas);
-  g.pages = static_cast<const uint8_t*>(pages);
-  g.refs = refs;
-  g.n_pages = n_pages;
-  g.metas_cap = plan->metas_cap;
-  g.pages_cap = plan->pages_cap;
-  g.dst_cap = plan->dst_cap;
-  g.frame_cap = plan->frame_cap;
-  g.dtype = plan->dtype;
-  g.max_pages = mp;
   // the frames as one file: every page's frame below frame_cap, the pad frame behind them
-  const FileParams fp{d_frames, lay.pad_frame + 64, plan->dtype, 0, 4};
-  const uint32_t pb = uint32_t(ctas_of<AP_THREADS>(mp));
+  const FileParams fp{d_frames, lay.pad_frame + 64, g.dtype, 0, 4};
+  const uint32_t mp = g.max_pages, pb = uint32_t(ctas_of<AP_THREADS>(mp));
 
   ln.begin("ap_pages_kernel");
   ap_pages_kernel<<<pb, AP_THREADS, 0, stream>>>(g, chk, parts);
@@ -2966,10 +2953,12 @@ PcoB200Error pco_b200_decompress_pages_async(const PcoB200AsyncPagesPlan* plan, 
   ln.begin("ap_rewalk_kernel");
   ap_rewalk_kernel<<<1, WALK_THREADS, sizeof(WalkSmem<SMALL_MAX_SIZE_LOG>), stream>>>(g, state, tab, d_frames, d_idx, lay.index_len);
   ln.end();
-  enqueue_decode_stage<false>(ln, DecodeStage{fp, table, d_idx, lay.index_len, mp, d_st, ws + lay.cls, ws + lay.syms,
-                                              reinterpret_cast<uint32_t*>(ws + lay.offs), &chk->binoms, dst, g.dst_cap, nullptr});
+  const DecodeStage d{fp, table, d_idx, lay.index_len, mp, d_st, ws + lay.cls, ws + lay.syms, reinterpret_cast<uint32_t*>(ws + lay.offs),
+                      &chk->binoms, dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{}};
+  if (filt) enqueue_decode_stage<false, true>(ln, d);
+  else enqueue_decode_stage<false>(ln, d);
   ln.begin("ap_cold_kernel");
-  dispatch_latent(plan->dtype, [&](auto tag) {
+  dispatch_latent(g.dtype, [&](auto tag) {
     using L = decltype(tag);
     ap_cold_kernel<L><<<1, ASYNC_THREADS, 0, stream>>>(g, state, tab, recs, d_st, fast_page, cold_list, d_frames, static_cast<L*>(dst), ws + lay.cold);
     return 0;
@@ -2978,6 +2967,23 @@ PcoB200Error pco_b200_decompress_pages_async(const PcoB200AsyncPagesPlan* plan, 
   ln.begin("ap_finish_kernel");
   ap_finish_kernel<<<1, 32, 0, stream>>>(state, status);
   ln.end();
+}
+
+PcoB200Error pco_b200_decompress_pages_async(const PcoB200AsyncPagesPlan* plan, const void* metas, const void* pages, const PcoB200PageRef* refs,
+                                             const uint64_t* n_pages, void* dst, void* workspace, PcoB200AsyncPagesStatus* status, void* cuda_stream) {
+  if (!plan || !metas || !pages || !refs || !n_pages || !workspace || !status || (!dst && plan->dst_cap))
+    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (!ap_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_decompress_pages_async_plan");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+
+  const uint32_t mp = uint32_t(plan->max_pages);
+  const ApLayout lay = ap_layout(mp, plan->dst_cap, plan->frame_cap);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  const ApArgs g{static_cast<const uint8_t*>(metas), static_cast<const uint8_t*>(pages), refs, n_pages, plan->metas_cap, plan->pages_cap, plan->dst_cap,
+                 plan->frame_cap, plan->dtype, mp};
+  enqueue_pages(ln, g, lay, ws, dst, nullptr, status);
   PCOB_CUDA_TRY(cudaGetLastError());
   return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
 }
@@ -3001,6 +3007,112 @@ PcoB200Error pco_b200_decompress_pages_async_result(const PcoB200AsyncPagesStatu
     default:
       status_to_error(s->device_status, "the page");
       return page_fail(kind, p, last_error_ref());
+  }
+}
+
+// ---- asynchronous filter of wrapped pages (pco_b200_filter_pages_async; kernels in async_filter_kernels.cuh).  The pages call's launches
+// (enqueue_pages, with the decode stage's filter-mode instantiations and rows_cap as dst_cap) behind a memset of the slot counts, then
+// fl_cold, fl_count, fl_finish and fl_gather.
+
+static bool fl_plan_ok(const PcoB200AsyncFilterPlan* p) {
+  return nt_valid(p->dtype) && p->max_pages >= 1 && p->max_pages <= 0x7fffffffull && p->rows_cap <= (uint64_t(1) << 56) &&
+         p->frame_cap <= (uint64_t(1) << 56) && p->out_cap <= (uint64_t(1) << 56) &&
+         p->workspace_bytes == fl_layout(p->max_pages, p->rows_cap, p->frame_cap, nt_bits(p->dtype) / 8).fl_total;
+}
+
+PcoB200Error pco_b200_filter_pages_async_plan(unsigned char dtype, size_t metas_cap, size_t pages_cap, size_t max_pages, size_t rows_cap,
+                                              size_t frame_cap, size_t out_cap, PcoB200AsyncFilterPlan* plan) {
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (!plan) return fail(PCO_B200_INVALID_ARGUMENT, "null plan");
+  if (max_pages == 0 || uint64_t(max_pages) > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_pages must be 1 .. 2^31 - 1");
+  if (uint64_t(rows_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "rows_cap above 2^56 numbers");
+  if (uint64_t(frame_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "frame_cap above 2^56 bytes");
+  if (uint64_t(out_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "out_cap above 2^56 numbers");
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->metas_cap = metas_cap;
+  plan->pages_cap = pages_cap;
+  plan->max_pages = max_pages;
+  plan->rows_cap = rows_cap;
+  plan->frame_cap = frame_cap;
+  plan->out_cap = out_cap;
+  plan->workspace_bytes = fl_layout(max_pages, rows_cap, frame_cap, nt_bits(dtype) / 8).fl_total;
+  if (PcoB200Error e = async_decode_setup<false, true>(dtype, [](auto tag) { return (const void*)ap_cold_kernel<decltype(tag)>; },
+                                                       {(const void*)ap_pages_kernel, (const void*)ap_scan_kernel, (const void*)ap_place_kernel,
+                                                        (const void*)frame_pages_kernel, (const void*)walk_kernel<SMALL_MAX_SIZE_LOG>,
+                                                        (const void*)ap_route_kernel, (const void*)ap_rewalk_kernel, (const void*)ap_finish_kernel,
+                                                        (const void*)fl_count_kernel, (const void*)fl_finish_kernel}))
+    return e;
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
+    using L = decltype(tag);
+    return load_kernels({(const void*)fl_cold_kernel<L>, (const void*)fl_gather_kernel<L>});
+  });
+}
+
+PcoB200Error pco_b200_filter_pages_async(const PcoB200AsyncFilterPlan* plan, const void* metas, const void* pages, const PcoB200PageRef* refs,
+                                         const uint64_t* n_pages, const PcoB200Interval* interval, void* out_values, uint64_t* out_positions,
+                                         uint64_t* n_matches, void* workspace, PcoB200AsyncFilterStatus* status, void* cuda_stream) {
+  if (!plan || !metas || !pages || !refs || !n_pages || !interval || !n_matches || !workspace || !status ||
+      ((!out_values || !out_positions) && plan->out_cap))
+    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (!fl_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_filter_pages_async_plan");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+  const cudaStream_t stream = ln.stream;
+
+  const uint32_t mp = uint32_t(plan->max_pages);
+  const FlLayout lay = fl_layout(mp, plan->rows_cap, plan->frame_cap, nt_bits(plan->dtype) / 8);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  const uint64_t slots = fl_slots(mp, plan->rows_cap), n_parts = ctas_of<FL_THREADS>(slots);
+  const ApArgs g{static_cast<const uint8_t*>(metas), static_cast<const uint8_t*>(pages), refs, n_pages, plan->metas_cap, plan->pages_cap, plan->rows_cap,
+                 plan->frame_cap, plan->dtype, mp};
+  const FiltStage filt{reinterpret_cast<const uint64_t*>(interval), reinterpret_cast<const uint32_t*>(ws + lay.fast_page),
+                       reinterpret_cast<uint32_t*>(ws + lay.counts), reinterpret_cast<uint64_t*>(ws + lay.rows), ws + lay.soffs};
+  auto* pstatus = reinterpret_cast<PcoB200AsyncPagesStatus*>(ws + lay.pstatus);
+  auto* fstate = reinterpret_cast<FlState*>(ws + lay.fstate);
+  auto* cparts = reinterpret_cast<uint64_t*>(ws + lay.cparts);
+
+  PCOB_CUDA_TRY(cudaMemsetAsync(filt.counts, 0, slots * sizeof(uint32_t), stream));
+  enqueue_pages(ln, g, lay, ws, ws + lay.stage, &filt, pstatus);
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    ln.begin("fl_cold_kernel");
+    fl_cold_kernel<L><<<mp, FL_THREADS, 0, stream>>>(reinterpret_cast<const ApState*>(ws + lay.state), reinterpret_cast<const IndexChunk*>(ws + lay.index),
+                                                    reinterpret_cast<const uint32_t*>(ws + lay.cold_list), filt, plan->dtype,
+                                                    reinterpret_cast<L*>(ws + lay.stage));
+    ln.end();
+    ln.begin("fl_count_kernel");
+    fl_count_kernel<<<uint32_t(n_parts), FL_THREADS, 0, stream>>>(filt.counts, slots, cparts);
+    ln.end();
+    ln.begin("fl_finish_kernel");
+    fl_finish_kernel<<<1, FL_SCAN_THREADS, 0, stream>>>(pstatus, cparts, n_parts, plan->out_cap, fstate, n_matches, status);
+    ln.end();
+    ln.begin("fl_gather_kernel");
+    fl_gather_kernel<L><<<uint32_t(n_parts), FL_THREADS, 0, stream>>>(fstate, filt.counts, filt.rows, cparts, slots, reinterpret_cast<const L*>(ws + lay.stage),
+                                                                     ws + lay.soffs, plan->out_cap, static_cast<L*>(out_values), out_positions);
+    ln.end();
+    return 0;
+  });
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
+}
+
+PcoB200Error pco_b200_filter_pages_async_result(const PcoB200AsyncFilterStatus* s, size_t* n_matches) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200Error kind = async_result_kind(s->kind);
+  if (kind == PCO_B200_OK) {
+    if (n_matches) *n_matches = size_t(s->n_matches);
+    return PCO_B200_OK;
+  }
+  switch (s->device_status) {
+    case PCO_B200_FILTER_OUT_FULL:
+      return fail(kind, "the pages hold " + std::to_string(s->matches_needed) + " matches, more than the plan's out_cap");
+    case PCO_B200_ASYNC_PAGES_DST: return page_fail(kind, size_t(s->page), "the pages up to this one hold more numbers than rows_cap");
+    default: {  // the pages call's outcome, in its words
+      const PcoB200AsyncPagesStatus p{s->kind, s->device_status, s->page, s->n_written, s->n_pages, s->frames_needed};
+      return pco_b200_decompress_pages_async_result(&p, nullptr);
+    }
   }
 }
 

@@ -8,7 +8,7 @@ Batched forms for containers that keep chunk metas and pages themselves: `compre
 chunks of one page each, `decompress_pages` decodes any number of pages in one call.  Both take host buffers (bytes / numpy)
 or torch CUDA tensors; with CUDA tensors the work runs on torch.cuda.current_stream() and the outputs are CUDA tensors.
 `AsyncChunksCompressor` and `AsyncPagesDecompressor` are their forms with the sizes or refs in device memory, which do not wait for the
-device and can be captured in a CUDA graph."""
+device and can be captured in a CUDA graph; `AsyncPagesFilter` decodes such pages and keeps only the numbers inside an interval."""
 import ctypes as C
 
 import numpy as np
@@ -413,3 +413,101 @@ class AsyncChunksCompressor(_lib._AsyncCall):
         ml, pl, nc = C.c_size_t(), C.c_size_t(), C.c_size_t()
         _lib.check(_lib_async_compress_wrapped().pco_b200_compress_wrapped_async_result(C.byref(s), C.byref(ml), C.byref(pl), C.byref(nc)))
         return int(ml.value), int(pl.value), int(nc.value)
+
+
+class _CAsyncFilterPlan(C.Structure):  # PcoB200AsyncFilterPlan (include/pco_b200.h)
+    _fields_ = [("dtype", C.c_uint32), ("reserved", C.c_uint32), ("metas_cap", C.c_uint64), ("pages_cap", C.c_uint64), ("max_pages", C.c_uint64),
+                ("rows_cap", C.c_uint64), ("frame_cap", C.c_uint64), ("out_cap", C.c_uint64), ("workspace_bytes", C.c_uint64)]
+
+
+class _CAsyncFilterStatus(C.Structure):  # PcoB200AsyncFilterStatus (include/pco_b200.h)
+    _fields_ = [("kind", C.c_uint32), ("device_status", C.c_uint32), ("page", C.c_uint64), ("n_written", C.c_uint64), ("n_pages", C.c_uint64),
+                ("frames_needed", C.c_uint64), ("n_matches", C.c_uint64), ("matches_needed", C.c_uint64)]
+
+
+def _lib_async_filter():
+    return _lib.bind("_async_filter_ready",
+                     pco_b200_filter_pages_async_plan=[C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p],
+                     pco_b200_filter_pages_async=[C.c_void_p] * 12,
+                     pco_b200_filter_pages_async_result=[C.c_void_p, C.POINTER(C.c_size_t)])
+
+
+def pack_interval(lo, hi, dtype):
+    """The PcoB200Interval of [lo, hi] for numbers of `dtype`: a 2-element int64 array holding each bound's bit pattern, zero-extended
+    (copy it to a CUDA tensor for AsyncPagesFilter).  The bounds are Python or numpy numbers, converted to `dtype` (NaN and infinities
+    included for floats); a bound outside an integer dtype's range raises OverflowError."""
+    dt = np.dtype(dtype)
+    _lib.dtype_byte(dt)
+    ut = np.dtype(f"u{dt.itemsize}")
+    bits = []
+    for x in (lo, hi):
+        if dt.kind in "iu":
+            info = np.iinfo(dt)
+            if isinstance(x, (float, np.floating)) and not float(x).is_integer():
+                raise TypeError(f"bound {x!r} is not an integer of {dt}")
+            if not info.min <= int(x) <= info.max:
+                raise OverflowError(f"bound {x!r} lies outside {dt}")
+            v = np.array([int(x)], dtype=dt)
+        else:
+            v = np.array([x], dtype=dt)
+        bits.append(int(v.view(ut)[0]))
+    return np.array(bits, dtype=np.uint64).view(np.int64)
+
+
+class AsyncPagesFilter(_lib._AsyncCall):
+    """Decodes a batch of wrapped-format pages on the current CUDA stream and writes only the numbers inside a closed interval, in row order,
+    with their positions in the pages' concatenation (pco_b200_filter_pages_async): the predicate runs inside the decoder, so the decoded
+    pages never reach HBM whole.  Refs, their count and the interval are read from device tensors, so one captured call serves new pages
+    and new bounds on each replay.
+
+    The capacities are AsyncPagesDecompressor's, with rows_cap (the most numbers of a call's pages) in place of dst_cap, and out_cap the
+    most matches a call writes; frame_cap defaults to metas_cap + pages_cap + 20 * max_pages as there.  The filter owns a device workspace
+    (about rows_cap * (itemsize + 1) bytes beyond the decompressor's) and a status; it serves one call in flight."""
+
+    _Plan, _Status = _CAsyncFilterPlan, _CAsyncFilterStatus
+
+    def __init__(self, dtype, metas_cap, pages_cap, max_pages, rows_cap, out_cap, frame_cap=None, device=None):
+        self.dtype = np.dtype(dtype)
+        if frame_cap is None:
+            frame_cap = metas_cap + pages_cap + 20 * max_pages
+        self._make_plan(device, lambda plan: _lib_async_filter().pco_b200_filter_pages_async_plan(
+            C.c_ubyte(_lib.dtype_byte(self.dtype)), C.c_size_t(metas_cap), C.c_size_t(pages_cap), C.c_size_t(max_pages), C.c_size_t(rows_cap),
+            C.c_size_t(frame_cap), C.c_size_t(out_cap), plan))
+        self._alloc()
+
+    def __call__(self, metas, pages, refs, n_pages, interval, values, positions, n_matches):
+        """Enqueues the filter of the pages refs[: n_pages[0]] names on torch.cuda.current_stream().  `metas`, `pages`, `refs` and `n_pages`
+        are as AsyncPagesDecompressor takes them; `interval` is a 2-element int64 CUDA tensor (pack_interval's bit patterns of lo and hi),
+        `values` a CUDA tensor of the plan's dtype and `positions` an int64 CUDA tensor, each of at least out_cap elements, and `n_matches` a
+        1-element int64 CUDA tensor that receives the count.  Returns nothing and does not wait; result() reports the outcome."""
+        import torch
+
+        p = self._plan
+        self._check_tensors(metas=metas, pages=pages, refs=refs, n_pages=n_pages, interval=interval, values=values, positions=positions,
+                            n_matches=n_matches)
+        if metas.numel() * metas.element_size() < p.metas_cap or pages.numel() * pages.element_size() < p.pages_cap:
+            raise ValueError(f"metas holds fewer than metas_cap = {p.metas_cap} bytes, or pages fewer than pages_cap = {p.pages_cap}")
+        if refs.dtype != torch.int64 or refs.dim() != 2 or refs.shape[1] != 5 or refs.shape[0] < p.max_pages:
+            raise ValueError(f"refs must be an int64 tensor of shape ({p.max_pages}, 5)")
+        for name, t in (("n_pages", n_pages), ("n_matches", n_matches)):
+            if t.dtype != torch.int64 or t.numel() != 1:
+                raise ValueError(f"{name} must be a 1-element int64 tensor")
+        if interval.dtype != torch.int64 or interval.numel() != 2:
+            raise ValueError("interval must be a 2-element int64 tensor")
+        if values.dtype != _torch_dtypes()[self.dtype] or values.numel() < p.out_cap:
+            raise ValueError(f"values must hold at least out_cap = {p.out_cap} numbers of {self.dtype}")
+        if positions.dtype != torch.int64 or positions.numel() < p.out_cap:
+            raise ValueError(f"positions must be an int64 tensor of at least out_cap = {p.out_cap} elements")
+        rc = _lib_async_filter().pco_b200_filter_pages_async(
+            C.byref(p), C.c_void_p(metas.data_ptr()), C.c_void_p(pages.data_ptr()), C.c_void_p(refs.data_ptr()), C.c_void_p(n_pages.data_ptr()),
+            C.c_void_p(interval.data_ptr()), C.c_void_p(values.data_ptr()), C.c_void_p(positions.data_ptr()), C.c_void_p(n_matches.data_ptr()),
+            C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()), self._stream())
+        _lib.check(rc)
+
+    def result(self):
+        """Copies the status of the last call back (waiting for it on the current stream) and returns the number of matches, or raises
+        PcoError with the kind decompress_pages gives ("page 17: ..."), or Io when the matches outnumber out_cap."""
+        s = self.status_record()
+        nm = C.c_size_t()
+        _lib.check(_lib_async_filter().pco_b200_filter_pages_async_result(C.byref(s), C.byref(nm)))
+        return int(nm.value)
