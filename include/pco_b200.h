@@ -900,6 +900,71 @@ PcoB200Error pco_b200_filter_pages_async(const PcoB200AsyncFilterPlan *plan, con
  * *n_matches (may be NULL) to the number of matches. */
 PcoB200Error pco_b200_filter_pages_async_result(const PcoB200AsyncFilterStatus *host_status, size_t *n_matches);
 
+/* ---- asynchronous filter of a batch of indexed standalone files (no reference counterpart): pco_b200_decompress_files_async with the
+ * closed-interval predicate of pco_b200_filter_pages_async pushed into the decoder.  A reader of indexed files that needs only the rows
+ * with lo <= x <= hi gets those numbers, in row order, with their positions, and the decoded files never reach HBM whole.  It only
+ * enqueues kernels on the caller's stream and returns at once; it makes no synchronising, allocating or host-to-device copy call and
+ * refers to no memory of the library's per-thread scratch, so it can be captured in a CUDA graph, and a captured call may be replayed
+ * after pco_b200_thread_release or after any other call.  A plan made once outside any capture fixes the grids from its capacities; the
+ * refs, their count and the interval are read on the device, so one captured graph serves different files, a different count and
+ * different bounds on each replay. */
+typedef struct PcoB200AsyncFilesFilterPlan {  /* filled by pco_b200_filter_files_async_plan; treat as opaque */
+  uint32_t dtype, uniform_type, format_major, reserved;
+  uint64_t src_cap, index_cap, max_files, max_chunks, rows_cap, out_cap;
+  uint64_t workspace_bytes;                   /* device workspace one in-flight call needs */
+} PcoB200AsyncFilesFilterPlan;
+
+typedef struct PcoB200AsyncFilesFilterStatus {  /* written on the device by every call */
+  uint32_t kind;                                /* PcoB200Error */
+  uint32_t device_status;                       /* the device word behind it: as PcoB200AsyncFilesStatus, or PCO_B200_FILTER_OUT_FULL */
+  uint64_t file;                                /* the file the outcome names (UINT64_MAX if none) */
+  uint64_t chunk;                               /* the failing chunk, counted from that file's first chunk (UINT64_MAX if none) */
+  uint64_t n_written;                           /* the sum of the files' counts (the rows filtered), once every file passed its checks and
+                                                   placement (0 before) */
+  uint64_t n_files;                             /* *n_files as the call read it */
+  uint64_t n_matches;                           /* matches written to out_values / out_positions (0 on a failure) */
+  uint64_t matches_needed;                      /* matches in all, also when above out_cap (0 on a failure) */
+} PcoB200AsyncFilesFilterStatus;
+
+/* Makes a plan for filters of up to max_files indexed files of dtype holding at most max_chunks chunks and rows_cap numbers in all (the
+ * role dst_cap plays in pco_b200_decompress_files_async), of which at most out_cap are written.  `head`, src_cap and index_cap are those of
+ * pco_b200_decompress_files_async_plan.  Checked before the device is touched, with that plan's kinds: dtype, the header, the uniform type,
+ * max_files in 1 .. 2^31 - 1, max_chunks in 1 .. 2^32 - 1, rows_cap and out_cap at most 2^56 (PCO_B200_INVALID_ARGUMENT).  Then *plan is
+ * filled and the one-time device set-up runs on the current device, which the calls must use (kernel attributes, and every kernel the
+ * call launches loaded); without a device that is PCO_B200_CUDA.
+ * workspace_bytes is pco_b200_decompress_files_async_plan's formula with dst_cap = rows_cap, plus these regions, each rounded up to 256
+ * bytes, with S = floor(rows_cap / 256) + max_chunks batch slots and E the bytes of a number of dtype: 48 (the files status), 16 (state),
+ * 4 S (slot counts), 8 S (slot rows), 8 ceil(S / 256) (CTA sums), E rows_cap (staged values), rows_cap (staged offsets), 4 max_chunks
+ * (slot map) and 4 (max_chunks + 1) (cold list). */
+PcoB200Error pco_b200_filter_files_async_plan(const void *head, size_t head_len, unsigned char dtype, size_t src_cap, size_t index_cap,
+                                              size_t max_files, size_t max_chunks, size_t rows_cap, size_t out_cap,
+                                              PcoB200AsyncFilesFilterPlan *plan);
+/* Enqueues the filter of files[0 : *n_files) on `cuda_stream`, and the outcome into *status; returns without waiting.  src (src_cap
+ * bytes), index (index_cap bytes), files (PcoB200FileRef[max_files]), n_files (one uint64_t), interval (one PcoB200Interval), out_values
+ * (out_cap numbers), out_positions (uint64_t[out_cap]), n_matches (one uint64_t), file_ns (uint64_t[max_files]; may be NULL), workspace
+ * (plan->workspace_bytes, 256-byte aligned) and status are device pointers; one workspace serves one call in flight.
+ * The selection is every number x of the concatenation pco_b200_decompress_files_async writes for the same arguments (with dst_cap =
+ * rows_cap) with lo <= x <= hi, compared as pco_b200_filter_pages_async compares: integers in their signed or unsigned order, floats as
+ * IEEE values (a NaN never matches, a NaN bound selects nothing, -0.0 equals +0.0), and lo > hi selects nothing.  The matches are written
+ * in row order: out_values[k] is the k-th match (its bit pattern) and out_positions[k] its index in the concatenation; *n_matches gets
+ * their count and file_ns[i] file i's count, as in pco_b200_decompress_files_async, so positions map to files through a search over the
+ * counts' running sum.
+ * Refusals and failures are pco_b200_decompress_files_async's, in its order, with its kinds and naming the same file and chunk
+ * (PCO_B200_ASYNC_FILES_DST against rows_cap); they write 0 to *n_matches and nothing to out_values, out_positions or file_ns.  When the
+ * files decode and there are more than out_cap matches, the kind is PCO_B200_IO (PCO_B200_FILTER_OUT_FULL) with matches_needed reported:
+ * the first out_cap matches in row order are written, nothing beyond out_cap, and file_ns as on success.  The return value covers the host
+ * side only: null pointers, an unaligned workspace or a plan that was not filled (PCO_B200_INVALID_ARGUMENT), a launch the runtime refuses
+ * (PCO_B200_CUDA).  With pco_b200_profile_enable(1), a call outside a stream capture records its kernel spans for pco_b200_profile_last; a
+ * call inside a capture records none. */
+PcoB200Error pco_b200_filter_files_async(const PcoB200AsyncFilesFilterPlan *plan, const void *src, const void *index, const PcoB200FileRef *files,
+                                         const uint64_t *n_files, const PcoB200Interval *interval, void *out_values, uint64_t *out_positions,
+                                         uint64_t *n_matches, uint64_t *file_ns, void *workspace, PcoB200AsyncFilesFilterStatus *status,
+                                         void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory at a point of the caller's choosing.  Returns the kind,
+ * sets the last-error message as pco_b200_decompress_files_async_result words it ("file 3: chunk 2: ...") and, when the kind is OK, sets
+ * *n_matches (may be NULL) to the number of matches. */
+PcoB200Error pco_b200_filter_files_async_result(const PcoB200AsyncFilesFilterStatus *host_status, size_t *n_matches);
+
 /* ---- asynchronous batch compress into wrapped-format chunks (no reference counterpart): pco_b200_compress_wrapped over a batch of
  * arrays, with the array sizes, their count and every buffer in device memory.  A GPU writer of a container that embeds pco (a columnar
  * file whose column chunks a kernel sized, a page store) compresses every column chunk behind the step that produced it, with no copy to

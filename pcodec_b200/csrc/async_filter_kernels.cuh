@@ -52,18 +52,11 @@ __host__ __device__ inline FlLayout fl_layout(uint64_t max_pages, uint64_t rows_
   return l;
 }
 
-// One CTA per cold-list entry k: the cold page's batches, decoded into the value staging by ap_cold_kernel, filtered in place - a warp
-// reads its batch into registers before filt_store8 writes the matches back at the batch's start.  Cold pages at or behind a failure were
-// not decoded; their staging is left alone (a failed call gathers nothing).
+// The batches of record `p` (its numbers at rows rec.out_offset .., decoded into the value staging by a catch-all decoder) filtered in
+// place by the CTA's warps: a warp reads its batch into registers before filt_store8 writes the matches back at the batch's start, into
+// slot rec.out_offset / 256 + p + b.
 template <typename L>
-__global__ void __launch_bounds__(FL_THREADS) fl_cold_kernel(const ApState* __restrict__ state, const IndexChunk* __restrict__ recs,
-                                                             const uint32_t* __restrict__ cold_list, FiltStage f, uint32_t dtype, L* __restrict__ stage) {
-  const uint64_t k = blockIdx.x;
-  if (k >= state->n_cold) return;
-  const uint32_t p = cold_list[k];
-  if (p >= state->fail_page || p >= (state->decode_fail >> 32)) return;
-  const IndexChunk rec = recs[p];
-  const FiltKey key = filt_bounds<L>(f.interval, dtype);
+__device__ __forceinline__ void fl_filter_in_place(const FiltStage& f, const FiltKey& key, const IndexChunk& rec, uint64_t p, L* __restrict__ stage) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const uint32_t nb = n_batches_of(rec.n);
   for (uint32_t b = warp; b < nb; b += FL_THREADS / 32) {
@@ -77,6 +70,20 @@ __global__ void __launch_bounds__(FL_THREADS) fl_cold_kernel(const ApState* __re
   }
 }
 
+// One CTA per cold-list entry k: the cold page, decoded into the value staging by ap_cold_kernel, filtered in place.  Cold pages at or
+// behind a failure were not decoded; their staging is left alone (a failed call gathers nothing).
+template <typename L>
+__global__ void __launch_bounds__(FL_THREADS) fl_cold_kernel(const ApState* __restrict__ state, const IndexChunk* __restrict__ recs,
+                                                             const uint32_t* __restrict__ cold_list, FiltStage f, uint32_t dtype, L* __restrict__ stage) {
+  const uint64_t k = blockIdx.x;
+  if (k >= state->n_cold) return;
+  const uint32_t p = cold_list[k];
+  if (p >= state->fail_page || p >= (state->decode_fail >> 32)) return;
+  const IndexChunk rec = recs[p];
+  const FiltKey key = filt_bounds<L>(f.interval, dtype);
+  fl_filter_in_place<L>(f, key, rec, p, stage);
+}
+
 // ceil(slots / FL_THREADS) CTAs: the sum of each CTA's counts.
 __global__ void __launch_bounds__(FL_THREADS) fl_count_kernel(const uint32_t* __restrict__ counts, uint64_t slots, uint64_t* __restrict__ parts) {
   const uint64_t i = uint64_t(blockIdx.x) * FL_THREADS + threadIdx.x;
@@ -85,14 +92,39 @@ __global__ void __launch_bounds__(FL_THREADS) fl_count_kernel(const uint32_t* __
   if (threadIdx.x == 0) parts[blockIdx.x] = tot;
 }
 
+// The step both finish kernels share, on one CTA of FL_SCAN_THREADS: the CTA sums scanned into CTA offsets (in place); returns the total.
+__device__ __forceinline__ uint64_t fl_scan_parts(uint64_t* __restrict__ parts, uint64_t n_parts) {
+  uint64_t total[1] = {0};
+  cta_scan_inplace<FL_SCAN_THREADS, 1>(
+      n_parts, [&](uint64_t c, int) { return parts[c]; }, [&](uint64_t c, int, uint64_t v) { parts[c] = v; }, total);
+  return total[0];
+}
+
+// Thread 0 of a finish kernel, with the upstream call's outcome already in r (kind and device_status): no matches when that call failed
+// (ok false), else `total` matches of which out_cap at most are written, PCO_B200_IO (PCO_B200_FILTER_OUT_FULL) when there are more.
+// Writes the FlState fl_gather_kernel reads and *n_matches.
+template <typename S>
+__device__ __forceinline__ void fl_decide(bool ok, uint64_t total, uint64_t out_cap, S& r, FlState* __restrict__ fs, uint64_t* __restrict__ n_matches) {
+  r.n_matches = 0;
+  r.matches_needed = 0;
+  if (ok) {
+    r.matches_needed = total;
+    r.n_matches = min(total, out_cap);
+    if (total > out_cap) {
+      r.kind = PCO_B200_IO;
+      r.device_status = PCO_B200_FILTER_OUT_FULL;
+    }
+  }
+  *fs = FlState{ok ? 1u : 0u, 0u, r.n_matches};
+  *n_matches = r.n_matches;
+}
+
 // One CTA: the CTA sums scanned into CTA offsets (in place) and the total; then, from the pages call's outcome, the status: a refusal or
 // failure as that call reports it (no matches), else success, or PCO_B200_IO when the matches outnumber out_cap (out_cap of them written).
 __global__ void __launch_bounds__(FL_SCAN_THREADS) fl_finish_kernel(const PcoB200AsyncPagesStatus* __restrict__ ps, uint64_t* __restrict__ parts,
                                                                     uint64_t n_parts, uint64_t out_cap, FlState* __restrict__ fs,
                                                                     uint64_t* __restrict__ n_matches, PcoB200AsyncFilterStatus* __restrict__ out) {
-  uint64_t total[1] = {0};
-  cta_scan_inplace<FL_SCAN_THREADS, 1>(
-      n_parts, [&](uint64_t c, int) { return parts[c]; }, [&](uint64_t c, int, uint64_t v) { parts[c] = v; }, total);
+  const uint64_t total = fl_scan_parts(parts, n_parts);
   if (threadIdx.x != 0) return;
   const PcoB200AsyncPagesStatus p = *ps;
   PcoB200AsyncFilterStatus r;
@@ -102,19 +134,7 @@ __global__ void __launch_bounds__(FL_SCAN_THREADS) fl_finish_kernel(const PcoB20
   r.n_written = p.n_written;
   r.n_pages = p.n_pages;
   r.frames_needed = p.frames_needed;
-  r.n_matches = 0;
-  r.matches_needed = 0;
-  const bool ok = p.kind == PCO_B200_OK;
-  if (ok) {
-    r.matches_needed = total[0];
-    r.n_matches = min(total[0], out_cap);
-    if (total[0] > out_cap) {
-      r.kind = PCO_B200_IO;
-      r.device_status = PCO_B200_FILTER_OUT_FULL;
-    }
-  }
-  *fs = FlState{ok ? 1u : 0u, 0u, r.n_matches};
-  *n_matches = r.n_matches;
+  fl_decide(p.kind == PCO_B200_OK, total, out_cap, r, fs, n_matches);
   *out = r;
 }
 

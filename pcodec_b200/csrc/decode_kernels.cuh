@@ -861,7 +861,7 @@ __device__ __forceinline__ void win_store8(const WinTask& w, uint32_t b, int lan
 }
 
 // ---------------------------------------------------------------------------
-// Filter mode (the FILT instantiations, pco_b200_filter_pages_async): a batch stores only its numbers inside a closed interval, compactly,
+// Filter mode (the FILT instantiations, both filter calls): a batch stores only its numbers inside a closed interval, compactly,
 // in its own staging slot.  Numbers are staged in the row domain: the batch whose first number is number `row` of the pages'
 // concatenation keeps its matches at stage[row ..] (values, `out`) and offs[row ..] (their offsets in the batch, one byte each), so the
 // slot can never overflow into another batch's.  Its count goes to counts[slot] and, when it has matches, its row to rows[slot]; the
@@ -869,7 +869,7 @@ __device__ __forceinline__ void win_store8(const WinTask& w, uint32_t b, int lan
 // ---------------------------------------------------------------------------
 struct FiltStage {
   const uint64_t* interval;   // PcoB200Interval: lo_bits, hi_bits (zero-extended bit patterns of the plan's number type)
-  const uint32_t* fast_page;  // decode-table record -> its page
+  const uint32_t* fast_page;  // decode-table record -> its page (the files filter: the record itself)
   uint32_t* counts;           // per slot: the batch's matches
   uint64_t* rows;             // per slot with matches: the batch's first row
   uint8_t* offs;              // per row: a staged match's offset in its batch

@@ -7,6 +7,7 @@
 #include "async_compress.cuh"
 #include "async_compress_files.cuh"
 #include "async_compress_wrapped.cuh"
+#include "async_filter_files_kernels.cuh"
 #include "async_filter_kernels.cuh"
 #include "async_files_kernels.cuh"
 #include "async_index_kernels.cuh"
@@ -2779,20 +2780,14 @@ PcoB200Error pco_b200_decompress_files_async_plan(const void* head, size_t head_
                                     (const void*)af_table_kernel, (const void*)merge_index_kernel, (const void*)af_finish_kernel});
 }
 
-PcoB200Error pco_b200_decompress_files_async(const PcoB200AsyncFilesPlan* plan, const void* src, const void* index, const PcoB200FileRef* files,
-                                             const uint64_t* n_files, void* dst, uint64_t* file_ns, void* workspace, PcoB200AsyncFilesStatus* status,
-                                             void* cuda_stream) {
-  if (!plan || !src || !index || !files || !n_files || !workspace || !status || (!dst && plan->dst_cap))
-    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
-  if (!af_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_decompress_files_async_plan");
-  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
-  AsyncLaunch ln;
-  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+// The launches of pco_b200_decompress_files_async over the workspace `ws` laid out by `lay`: the front end, the decode stage, the
+// catch-all decoder into dst and af_finish_kernel into *status (and file_ns).  With `filt` the decode stage runs its filter-mode
+// instantiations, dst is their value staging, and ff_cold_list_kernel records the cold records in the cold list `cold_list` before the
+// catch-all decoder runs (pco_b200_filter_files_async).
+static void enqueue_files(const AsyncLaunch& ln, const AfArgs& g, const AfLayout& lay, uint8_t* ws, void* dst, const FiltStage* filt,
+                          uint32_t* cold_list, uint64_t* file_ns, PcoB200AsyncFilesStatus* status) {
   const cudaStream_t stream = ln.stream;
-
-  const uint32_t mf = uint32_t(plan->max_files), mc = uint32_t(plan->max_chunks);
-  const AfLayout lay = af_layout(mf, mc, plan->dst_cap);
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  const uint32_t mf = g.max_files, mc = g.max_chunks;
   AsyncCheck* chk = reinterpret_cast<AsyncCheck*>(ws);
   AfState* state = reinterpret_cast<AfState*>(ws + lay.state);
   uint32_t* fst = reinterpret_cast<uint32_t*>(ws + lay.fst);
@@ -2802,23 +2797,14 @@ PcoB200Error pco_b200_decompress_files_async(const PcoB200AsyncFilesPlan* plan, 
   AfPart* parts = reinterpret_cast<AfPart*>(ws + lay.parts);
   IndexChunk* table = reinterpret_cast<IndexChunk*>(ws + lay.table);
   uint32_t* d_st = reinterpret_cast<uint32_t*>(ws + lay.st);
-  const uint8_t* d_idx = static_cast<const uint8_t*>(index);
-  AfArgs g;
-  g.fp = FileParams{src, plan->src_cap, plan->dtype, plan->uniform_type, plan->format_major};
-  g.index = d_idx;
-  g.index_cap = plan->index_cap;
-  g.dst_cap = plan->dst_cap;
-  g.files = files;
-  g.n_files = n_files;
-  g.max_files = mf;
-  g.max_chunks = mc;
+  const uint8_t* d_idx = g.index;
   const uint32_t fb = uint32_t(ctas_of<AF_THREADS>(mf)), tb = uint32_t(std::max(ctas_of<AF_THREADS>(mf), ctas_of<AF_THREADS>(mc)));
 
   ln.begin("af_files_kernel");
   af_files_kernel<<<fb, AF_THREADS, 0, stream>>>(g, chk, fst, fchk, merges, parts);
   ln.end();
   ln.begin("check_index_kernel");
-  check_index_kernel<<<mf, 256, 0, stream>>>(static_cast<const uint8_t*>(src), d_idx, plan->dtype, fchk, verdict);
+  check_index_kernel<<<mf, 256, 0, stream>>>(static_cast<const uint8_t*>(g.fp.src), d_idx, g.fp.dtype, fchk, verdict);
   ln.end();
   ln.begin("af_scan_kernel");
   af_scan_kernel<<<1, AF_SCAN_THREADS, 0, stream>>>(g, parts, state);
@@ -2832,10 +2818,18 @@ PcoB200Error pco_b200_decompress_files_async(const PcoB200AsyncFilesPlan* plan, 
   ln.begin("merge_index_kernel");
   merge_index_kernel<<<mf, 256, 0, stream>>>(d_idx, merges, table);
   ln.end();
-  enqueue_decode_stage<false>(ln, DecodeStage{g.fp, table, d_idx, g.index_cap, mc, d_st, ws + lay.cls, ws + lay.syms,
-                                              reinterpret_cast<uint32_t*>(ws + lay.offs), &chk->binoms, dst, g.dst_cap, nullptr});
+  const DecodeStage d{g.fp, table, d_idx, g.index_cap, mc, d_st, ws + lay.cls, ws + lay.syms, reinterpret_cast<uint32_t*>(ws + lay.offs),
+                      &chk->binoms, dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{}};
+  if (filt) {
+    enqueue_decode_stage<false, true>(ln, d);
+    ln.begin("ff_cold_list_kernel");
+    ff_cold_list_kernel<<<uint32_t(ctas_of<FF_THREADS>(mc)), FF_THREADS, 0, stream>>>(chk, d_st, cold_list);
+    ln.end();
+  } else {
+    enqueue_decode_stage<false>(ln, d);
+  }
   ln.begin("cold_chunks_kernel");
-  dispatch_latent(plan->dtype, [&](auto tag) {
+  dispatch_latent(g.fp.dtype, [&](auto tag) {
     using L = decltype(tag);
     cold_chunks_kernel<L><<<1, ASYNC_THREADS, 0, stream>>>(g.fp, table, chk, d_st, static_cast<L*>(dst), g.dst_cap, ws + lay.cold);
     return 0;
@@ -2844,6 +2838,22 @@ PcoB200Error pco_b200_decompress_files_async(const PcoB200AsyncFilesPlan* plan, 
   ln.begin("af_finish_kernel");
   af_finish_kernel<<<1, AF_SCAN_THREADS, 0, stream>>>(state, chk, merges, fchk, d_st, file_ns, status);
   ln.end();
+}
+
+PcoB200Error pco_b200_decompress_files_async(const PcoB200AsyncFilesPlan* plan, const void* src, const void* index, const PcoB200FileRef* files,
+                                             const uint64_t* n_files, void* dst, uint64_t* file_ns, void* workspace, PcoB200AsyncFilesStatus* status,
+                                             void* cuda_stream) {
+  if (!plan || !src || !index || !files || !n_files || !workspace || !status || (!dst && plan->dst_cap))
+    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (!af_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_decompress_files_async_plan");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+
+  const uint32_t mf = uint32_t(plan->max_files), mc = uint32_t(plan->max_chunks);
+  const AfArgs g{FileParams{src, plan->src_cap, plan->dtype, plan->uniform_type, plan->format_major}, static_cast<const uint8_t*>(index),
+                 plan->index_cap, plan->dst_cap, files, n_files, mf, mc};
+  enqueue_files(ln, g, af_layout(mf, mc, plan->dst_cap), static_cast<uint8_t*>(workspace), dst, nullptr, nullptr, file_ns, status);
   PCOB_CUDA_TRY(cudaGetLastError());
   return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
 }
@@ -2873,6 +2883,118 @@ PcoB200Error pco_b200_decompress_files_async_result(const PcoB200AsyncFilesStatu
     default:
       status_to_error(s->device_status, ("chunk " + std::to_string(s->chunk)).c_str());
       return file_fail(kind, f, last_error_ref());
+  }
+}
+
+// ---- asynchronous filter of indexed standalone files (pco_b200_filter_files_async; kernels in async_filter_files_kernels.cuh).  A memset
+// of the slot counts and ff_map_kernel, then the files call's launches (enqueue_files, with the decode stage's filter-mode instantiations,
+// ff_cold_list_kernel and rows_cap as dst_cap), then ff_cold, fl_count, ff_finish and fl_gather.
+
+static bool ff_plan_ok(const PcoB200AsyncFilesFilterPlan* p) {
+  return nt_valid(p->dtype) && p->max_files >= 1 && p->max_files <= 0x7fffffffull && p->max_chunks >= 1 && p->max_chunks <= 0xffffffffull &&
+         p->rows_cap <= (uint64_t(1) << 56) && p->out_cap <= (uint64_t(1) << 56) &&
+         p->workspace_bytes == ff_layout(p->max_files, p->max_chunks, p->rows_cap, nt_bits(p->dtype) / 8).ff_total;
+}
+
+PcoB200Error pco_b200_filter_files_async_plan(const void* head, size_t head_len, unsigned char dtype, size_t src_cap, size_t index_cap,
+                                              size_t max_files, size_t max_chunks, size_t rows_cap, size_t out_cap, PcoB200AsyncFilesFilterPlan* plan) {
+  StandaloneHeader hdr;
+  if (PcoB200Error e = check_async_head(head, head_len, dtype, plan, &hdr)) return e;
+  if (max_files == 0 || uint64_t(max_files) > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_files must be 1 .. 2^31 - 1");
+  if (max_chunks == 0 || uint64_t(max_chunks) > 0xffffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_chunks must be 1 .. 2^32 - 1");
+  if (uint64_t(rows_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "rows_cap above 2^56 numbers");
+  if (uint64_t(out_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "out_cap above 2^56 numbers");
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->uniform_type = hdr.uniform_type;
+  plan->format_major = hdr.format_major;
+  plan->src_cap = src_cap;
+  plan->index_cap = index_cap;
+  plan->max_files = max_files;
+  plan->max_chunks = max_chunks;
+  plan->rows_cap = rows_cap;
+  plan->out_cap = out_cap;
+  plan->workspace_bytes = ff_layout(max_files, max_chunks, rows_cap, nt_bits(dtype) / 8).ff_total;
+  if (PcoB200Error e = async_decode_setup<false, true>(dtype, [](auto tag) { return (const void*)cold_chunks_kernel<decltype(tag)>; },
+                                                       {(const void*)af_files_kernel, (const void*)check_index_kernel, (const void*)af_scan_kernel,
+                                                        (const void*)af_place_kernel, (const void*)af_table_kernel, (const void*)merge_index_kernel,
+                                                        (const void*)af_finish_kernel, (const void*)ff_map_kernel, (const void*)ff_cold_list_kernel,
+                                                        (const void*)fl_count_kernel, (const void*)ff_finish_kernel}))
+    return e;
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
+    using L = decltype(tag);
+    return load_kernels({(const void*)ff_cold_kernel<L>, (const void*)fl_gather_kernel<L>});
+  });
+}
+
+PcoB200Error pco_b200_filter_files_async(const PcoB200AsyncFilesFilterPlan* plan, const void* src, const void* index, const PcoB200FileRef* files,
+                                         const uint64_t* n_files, const PcoB200Interval* interval, void* out_values, uint64_t* out_positions,
+                                         uint64_t* n_matches, uint64_t* file_ns, void* workspace, PcoB200AsyncFilesFilterStatus* status,
+                                         void* cuda_stream) {
+  if (!plan || !src || !index || !files || !n_files || !interval || !n_matches || !workspace || !status ||
+      ((!out_values || !out_positions) && plan->out_cap))
+    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (!ff_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_filter_files_async_plan");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+  const cudaStream_t stream = ln.stream;
+
+  const uint32_t mf = uint32_t(plan->max_files), mc = uint32_t(plan->max_chunks);
+  const FfLayout lay = ff_layout(mf, mc, plan->rows_cap, nt_bits(plan->dtype) / 8);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  const uint64_t slots = fl_slots(mc, plan->rows_cap), n_parts = ctas_of<FL_THREADS>(slots);
+  const AfArgs g{FileParams{src, plan->src_cap, plan->dtype, plan->uniform_type, plan->format_major}, static_cast<const uint8_t*>(index),
+                 plan->index_cap, plan->rows_cap, files, n_files, mf, mc};
+  const FiltStage filt{reinterpret_cast<const uint64_t*>(interval), reinterpret_cast<const uint32_t*>(ws + lay.slot_map),
+                       reinterpret_cast<uint32_t*>(ws + lay.counts), reinterpret_cast<uint64_t*>(ws + lay.rows), ws + lay.soffs};
+  auto* fstatus = reinterpret_cast<PcoB200AsyncFilesStatus*>(ws + lay.fstatus);
+  auto* fstate = reinterpret_cast<FlState*>(ws + lay.fstate);
+  auto* cparts = reinterpret_cast<uint64_t*>(ws + lay.cparts);
+  auto* cold_list = reinterpret_cast<uint32_t*>(ws + lay.cold_list);
+
+  PCOB_CUDA_TRY(cudaMemsetAsync(filt.counts, 0, slots * sizeof(uint32_t), stream));
+  ln.begin("ff_map_kernel");
+  ff_map_kernel<<<uint32_t(ctas_of<FF_THREADS>(mc)), FF_THREADS, 0, stream>>>(mc, reinterpret_cast<uint32_t*>(ws + lay.slot_map), cold_list);
+  ln.end();
+  enqueue_files(ln, g, lay, ws, ws + lay.stage, &filt, cold_list, file_ns, fstatus);
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    ln.begin("ff_cold_kernel");
+    ff_cold_kernel<L><<<std::min(mc, uint32_t(FF_COLD_CTAS)), FL_THREADS, 0, stream>>>(cold_list, reinterpret_cast<const IndexChunk*>(ws + lay.table), filt,
+                                                                                       plan->dtype, reinterpret_cast<L*>(ws + lay.stage));
+    ln.end();
+    ln.begin("fl_count_kernel");
+    fl_count_kernel<<<uint32_t(n_parts), FL_THREADS, 0, stream>>>(filt.counts, slots, cparts);
+    ln.end();
+    ln.begin("ff_finish_kernel");
+    ff_finish_kernel<<<1, FL_SCAN_THREADS, 0, stream>>>(fstatus, cparts, n_parts, plan->out_cap, fstate, n_matches, status);
+    ln.end();
+    ln.begin("fl_gather_kernel");
+    fl_gather_kernel<L><<<uint32_t(n_parts), FL_THREADS, 0, stream>>>(fstate, filt.counts, filt.rows, cparts, slots, reinterpret_cast<const L*>(ws + lay.stage),
+                                                                     ws + lay.soffs, plan->out_cap, static_cast<L*>(out_values), out_positions);
+    ln.end();
+    return 0;
+  });
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
+}
+
+PcoB200Error pco_b200_filter_files_async_result(const PcoB200AsyncFilesFilterStatus* s, size_t* n_matches) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200Error kind = async_result_kind(s->kind);
+  if (kind == PCO_B200_OK) {
+    if (n_matches) *n_matches = size_t(s->n_matches);
+    return PCO_B200_OK;
+  }
+  switch (s->device_status) {
+    case PCO_B200_FILTER_OUT_FULL:
+      return fail(kind, "the files hold " + std::to_string(s->matches_needed) + " matches, more than the plan's out_cap");
+    case PCO_B200_ASYNC_FILES_DST: return file_fail(kind, size_t(s->file), "the files up to this one hold more numbers than rows_cap");
+    default: {  // the files call's outcome, in its words
+      const PcoB200AsyncFilesStatus f{s->kind, s->device_status, s->file, s->chunk, s->n_written, s->n_files};
+      return pco_b200_decompress_files_async_result(&f, nullptr);
+    }
   }
 }
 
