@@ -965,6 +965,127 @@ PcoB200Error pco_b200_filter_files_async(const PcoB200AsyncFilesFilterPlan *plan
  * *n_matches (may be NULL) to the number of matches. */
 PcoB200Error pco_b200_filter_files_async_result(const PcoB200AsyncFilesFilterStatus *host_status, size_t *n_matches);
 
+/* ---- asynchronous aggregates of wrapped-format pages and of indexed standalone files (no reference counterpart): the pages or files
+ * pco_b200_decompress_pages_async / pco_b200_decompress_files_async decode, reduced to count, min, max and sum of the numbers x with
+ * lo <= x <= hi, per page or file and in all.  A scan that wants `count / min / max / sum of x where lo <= x <= hi` gets them without the
+ * decoded numbers or the matches ever reaching HBM: each 256-number batch is reduced in the decoder's registers.  Each call only enqueues
+ * kernels on the caller's stream and returns at once; it makes no synchronising, allocating or host-to-device copy call and refers to no
+ * memory of the library's per-thread scratch, so it can be captured in a CUDA graph, and a captured call may be replayed after
+ * pco_b200_thread_release or after any other call.  A plan made once outside any capture fixes the grids from its capacities; the refs,
+ * their count and the interval are read on the device, so one captured graph serves different pages or files and different bounds on each
+ * replay.
+ * The interval is compared as pco_b200_filter_pages_async compares it: integers in their signed or unsigned order; floats (f16, f32, f64)
+ * as IEEE values: a NaN never matches, a NaN bound selects nothing, and -0.0 equals +0.0; lo > hi selects nothing.
+ * Groups: aggs[i] is ref i's page (pages call) or file i (files call), for i < *n_pages / *n_files; *total covers all of them.  Records
+ * past the count are not written.
+ * min / max: picked in the order of the key that orders the numbers (floats: IEEE order with -0.0 below +0.0, so the bits are fully
+ * determined).
+ * Integer sums: exact; the numbers are sign- or zero-extended to 128 bits (at most 2^56 rows of 2^64: the sum never wraps).
+ * Float sums: f16, f32 and f64 are all added in f64 (the conversions are exact), in an order that depends on neither grids nor timing:
+ *   1. lane partial: each run of 8 numbers at offsets 8 l .. 8 l + 7 of a 256-number batch (l = 0 .. 31), its matches added left to
+ *      right from +0.0;
+ *   2. batch sum: the 32 lane partials as a pairwise tree: (0, 1), (2, 3), ..., then pairs of pairs;
+ *   3. group sum: the group's batches in row order (batches restart at each page, and at each chunk of a file), batch j to lane j mod
+ *      32, each lane adding its batches in order from +0.0, then the tree of step 2;
+ *   4. total: the groups' sums by the rule of step 3, with group g in place of batch j.
+ *   Since every accumulation starts from +0.0 a sum is never -0.0, and empty batches or groups add nothing.  A sum that reaches NaN
+ *   (+inf plus -inf) is a NaN of unspecified payload. */
+typedef struct PcoB200Aggregate {  /* in device memory; one per page / file, and one total */
+  uint64_t n_rows;                 /* numbers the group holds (page_n; the file's count; the total: their sum) */
+  uint64_t count;                  /* numbers x with lo <= x <= hi */
+  uint64_t min_bits;               /* bit pattern of the least match, zero-extended (0 when count == 0) */
+  uint64_t max_bits;               /* of the greatest match (0 when count == 0) */
+  uint64_t sum_lo;                 /* integers: low 64 bits of the exact 128-bit two's-complement sum; floats: the f64 sum's bit pattern */
+  uint64_t sum_hi;                 /* integers: high 64 bits; floats: 0 */
+} PcoB200Aggregate;
+
+typedef struct PcoB200AsyncAggregatePlan {  /* filled by pco_b200_aggregate_pages_async_plan; treat as opaque */
+  uint32_t dtype, reserved;
+  uint64_t metas_cap, pages_cap, max_pages, rows_cap, frame_cap;
+  uint64_t workspace_bytes;                 /* device workspace one in-flight call needs */
+} PcoB200AsyncAggregatePlan;
+
+typedef struct PcoB200AsyncAggregateStatus {  /* written on the device by every call */
+  uint32_t kind;                              /* PcoB200Error */
+  uint32_t device_status;                     /* the device word behind it: as PcoB200AsyncPagesStatus */
+  uint64_t page;                              /* the page the outcome names (UINT64_MAX if none) */
+  uint64_t n_written;                         /* the sum of page_n (the rows reduced), once every page passed its checks (0 on a failure) */
+  uint64_t n_pages;                           /* *n_pages as the call read it */
+  uint64_t frames_needed;                     /* bytes of framed pages the batch needs, also when above frame_cap (0 when refused earlier) */
+  uint64_t n_matches;                         /* total->count (0 on a failure) */
+} PcoB200AsyncAggregateStatus;
+
+/* Makes a plan for aggregates of up to max_pages pages of dtype, whose refs point into metas_cap bytes of metas and pages_cap bytes of
+ * pages, holding at most rows_cap numbers in all (the role dst_cap plays in pco_b200_decompress_pages_async); frame_cap bounds the framed
+ * pages as in that call.  Checked before the device is touched: dtype (PCO_B200_INVALID_TYPE), max_pages in 1 .. 2^31 - 1, rows_cap and
+ * frame_cap at most 2^56 (PCO_B200_INVALID_ARGUMENT).  Then *plan is filled and the one-time device set-up runs on the current device,
+ * which the calls must use (kernel attributes, and every kernel the call launches loaded); without a device that is PCO_B200_CUDA.
+ * workspace_bytes is pco_b200_decompress_pages_async_plan's formula with dst_cap = rows_cap, plus these regions, each rounded up to 256
+ * bytes, with S = floor(rows_cap / 256) + max_pages batch slots and E the bytes of a number of dtype: 40 (the pages status), 4 S (slot
+ * counts), 32 S (slot records), E rows_cap (the cold pages' values) and 48 max_pages (the pages' accumulators). */
+PcoB200Error pco_b200_aggregate_pages_async_plan(unsigned char dtype, size_t metas_cap, size_t pages_cap, size_t max_pages, size_t rows_cap,
+                                                 size_t frame_cap, PcoB200AsyncAggregatePlan *plan);
+/* Enqueues the aggregates of the pages refs[0 : *n_pages) names on `cuda_stream`, and the outcome into *status; returns without waiting.
+ * metas (metas_cap bytes), pages (pages_cap bytes; may be the same buffer as metas), refs (PcoB200PageRef[max_pages]), n_pages (one
+ * uint64_t), interval (one PcoB200Interval), aggs (PcoB200Aggregate[max_pages]), total (one PcoB200Aggregate), workspace
+ * (plan->workspace_bytes, 256-byte aligned) and status are device pointers; one workspace serves one call in flight.
+ * The numbers reduced are the concatenation pco_b200_decompress_pages_async writes for the same arguments (with dst_cap = rows_cap).
+ * Refusals and failures are that call's, in its order, with its kinds and naming the same page; then *total is written as all zeros and
+ * aggs is not written.  The return value covers the host side only: null pointers, an unaligned workspace or a plan that was not filled
+ * (PCO_B200_INVALID_ARGUMENT), a launch the runtime refuses (PCO_B200_CUDA).  With pco_b200_profile_enable(1), a call outside a stream
+ * capture records its kernel spans for pco_b200_profile_last; a call inside a capture records none. */
+PcoB200Error pco_b200_aggregate_pages_async(const PcoB200AsyncAggregatePlan *plan, const void *metas, const void *pages, const PcoB200PageRef *refs,
+                                            const uint64_t *n_pages, const PcoB200Interval *interval, PcoB200Aggregate *aggs, PcoB200Aggregate *total,
+                                            void *workspace, PcoB200AsyncAggregateStatus *status, void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory at a point of the caller's choosing.  Returns the kind,
+ * sets the last-error message as pco_b200_decompress_pages_async_result words it ("page 17: ...") and, when the kind is OK, sets
+ * *n_matches (may be NULL) to the total match count. */
+PcoB200Error pco_b200_aggregate_pages_async_result(const PcoB200AsyncAggregateStatus *host_status, size_t *n_matches);
+
+typedef struct PcoB200AsyncFilesAggregatePlan {  /* filled by pco_b200_aggregate_files_async_plan; treat as opaque */
+  uint32_t dtype, uniform_type, format_major, reserved;
+  uint64_t src_cap, index_cap, max_files, max_chunks, rows_cap;
+  uint64_t workspace_bytes;                      /* device workspace one in-flight call needs */
+} PcoB200AsyncFilesAggregatePlan;
+
+typedef struct PcoB200AsyncFilesAggregateStatus {  /* written on the device by every call */
+  uint32_t kind;                                   /* PcoB200Error */
+  uint32_t device_status;                          /* the device word behind it: as PcoB200AsyncFilesStatus */
+  uint64_t file;                                   /* the file the outcome names (UINT64_MAX if none) */
+  uint64_t chunk;                                  /* the failing chunk, counted from that file's first chunk (UINT64_MAX if none) */
+  uint64_t n_written;                              /* the sum of the files' counts (the rows reduced), once every file passed its checks
+                                                      and placement (0 before) */
+  uint64_t n_files;                                /* *n_files as the call read it */
+  uint64_t n_matches;                              /* total->count (0 on a failure) */
+} PcoB200AsyncFilesAggregateStatus;
+
+/* Makes a plan for aggregates of up to max_files indexed files of dtype holding at most max_chunks chunks and rows_cap numbers in all (the
+ * role dst_cap plays in pco_b200_decompress_files_async).  `head`, src_cap and index_cap are those of pco_b200_decompress_files_async_plan.
+ * Checked before the device is touched, with that plan's kinds: dtype, the header, the uniform type, max_files in 1 .. 2^31 - 1,
+ * max_chunks in 1 .. 2^32 - 1, rows_cap at most 2^56 (PCO_B200_INVALID_ARGUMENT).  Then *plan is filled and the one-time device set-up
+ * runs on the current device, which the calls must use; without a device that is PCO_B200_CUDA.
+ * workspace_bytes is pco_b200_decompress_files_async_plan's formula with dst_cap = rows_cap, plus these regions, each rounded up to 256
+ * bytes, with S = floor(rows_cap / 256) + max_chunks batch slots and E the bytes of a number of dtype: 48 (the files status), 4 S (slot
+ * counts), 32 S (slot records), E rows_cap (the cold chunks' values), 4 max_chunks (slot map), 4 (max_chunks + 1) (cold list) and
+ * 48 max_files (the files' accumulators). */
+PcoB200Error pco_b200_aggregate_files_async_plan(const void *head, size_t head_len, unsigned char dtype, size_t src_cap, size_t index_cap,
+                                                 size_t max_files, size_t max_chunks, size_t rows_cap, PcoB200AsyncFilesAggregatePlan *plan);
+/* Enqueues the aggregates of files[0 : *n_files) on `cuda_stream`, and the outcome into *status; returns without waiting.  src (src_cap
+ * bytes), index (index_cap bytes), files (PcoB200FileRef[max_files]), n_files (one uint64_t), interval (one PcoB200Interval), aggs
+ * (PcoB200Aggregate[max_files]), total (one PcoB200Aggregate), workspace (plan->workspace_bytes, 256-byte aligned) and status are device
+ * pointers; one workspace serves one call in flight.
+ * The numbers reduced are the concatenation pco_b200_decompress_files_async writes for the same arguments (with dst_cap = rows_cap).
+ * Refusals and failures are that call's, in its order, with its kinds and naming the same file and chunk (PCO_B200_ASYNC_FILES_DST
+ * against rows_cap); then *total is written as all zeros and aggs is not written.  The return value covers the host side only, as for
+ * pco_b200_aggregate_pages_async. */
+PcoB200Error pco_b200_aggregate_files_async(const PcoB200AsyncFilesAggregatePlan *plan, const void *src, const void *index, const PcoB200FileRef *files,
+                                            const uint64_t *n_files, const PcoB200Interval *interval, PcoB200Aggregate *aggs, PcoB200Aggregate *total,
+                                            void *workspace, PcoB200AsyncFilesAggregateStatus *status, void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory.  Returns the kind, sets the last-error message as
+ * pco_b200_decompress_files_async_result words it ("file 3: chunk 2: ...") and, when the kind is OK, sets *n_matches (may be NULL) to the
+ * total match count. */
+PcoB200Error pco_b200_aggregate_files_async_result(const PcoB200AsyncFilesAggregateStatus *host_status, size_t *n_matches);
+
 /* ---- asynchronous batch compress into wrapped-format chunks (no reference counterpart): pco_b200_compress_wrapped over a batch of
  * arrays, with the array sizes, their count and every buffer in device memory.  A GPU writer of a container that embeds pco (a columnar
  * file whose column chunks a kernel sized, a page store) compresses every column chunk behind the step that produced it, with no copy to

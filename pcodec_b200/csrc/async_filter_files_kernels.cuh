@@ -60,8 +60,9 @@ __global__ void __launch_bounds__(FF_THREADS) ff_cold_list_kernel(const AsyncChe
 }
 
 // min(max_chunks, FF_COLD_CTAS) CTAs striding over the cold list: each record, decoded into the value staging by cold_chunks_kernel,
-// filtered in place.  A record whose decode failed is filtered too; the call then fails and gathers nothing.
-template <typename L>
+// filtered in place.  A record whose decode failed is filtered too; the call then fails and gathers nothing.  AGG: reduced into the
+// slots instead.
+template <typename L, bool AGG = false>
 __global__ void __launch_bounds__(FL_THREADS) ff_cold_kernel(const uint32_t* __restrict__ cold_list, const IndexChunk* __restrict__ table, FiltStage f,
                                                              uint32_t dtype, L* __restrict__ stage) {
   const uint32_t n_cold = cold_list[0];
@@ -70,7 +71,7 @@ __global__ void __launch_bounds__(FL_THREADS) ff_cold_kernel(const uint32_t* __r
   for (uint32_t k = blockIdx.x; k < n_cold; k += gridDim.x) {
     const uint32_t r = cold_list[1 + k];
     const IndexChunk rec = table[r];
-    fl_filter_in_place<L>(f, key, rec, r, stage);
+    fl_filter_in_place<L, AGG>(f, key, rec, r, stage);
   }
 }
 

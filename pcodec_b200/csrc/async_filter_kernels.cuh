@@ -54,8 +54,8 @@ __host__ __device__ inline FlLayout fl_layout(uint64_t max_pages, uint64_t rows_
 
 // The batches of record `p` (its numbers at rows rec.out_offset .., decoded into the value staging by a catch-all decoder) filtered in
 // place by the CTA's warps: a warp reads its batch into registers before filt_store8 writes the matches back at the batch's start, into
-// slot rec.out_offset / 256 + p + b.
-template <typename L>
+// slot rec.out_offset / 256 + p + b.  AGG: agg_store8 reduces the batch into the slot instead (the aggregate calls).
+template <typename L, bool AGG = false>
 __device__ __forceinline__ void fl_filter_in_place(const FiltStage& f, const FiltKey& key, const IndexChunk& rec, uint64_t p, L* __restrict__ stage) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const uint32_t nb = n_batches_of(rec.n);
@@ -65,14 +65,18 @@ __device__ __forceinline__ void fl_filter_in_place(const FiltStage& f, const Fil
     L r[8];
 #pragma unroll
     for (int e = 0; e < 8; e++) r[e] = uint32_t(lane * 8 + e) < cnt ? stage[row + lane * 8 + e] : L(0);
-    __syncwarp();
-    filt_store8<L>(f, key, stage, row, rec.out_offset / BATCH_N + p + b, cnt, lane, r);
+    if constexpr (AGG) {
+      agg_store8<L>(f, key, rec.out_offset / BATCH_N + p + b, cnt, lane, r);
+    } else {
+      __syncwarp();
+      filt_store8<L>(f, key, stage, row, rec.out_offset / BATCH_N + p + b, cnt, lane, r);
+    }
   }
 }
 
 // One CTA per cold-list entry k: the cold page, decoded into the value staging by ap_cold_kernel, filtered in place.  Cold pages at or
-// behind a failure were not decoded; their staging is left alone (a failed call gathers nothing).
-template <typename L>
+// behind a failure were not decoded; their staging is left alone (a failed call gathers nothing).  AGG: reduced into the slots instead.
+template <typename L, bool AGG = false>
 __global__ void __launch_bounds__(FL_THREADS) fl_cold_kernel(const ApState* __restrict__ state, const IndexChunk* __restrict__ recs,
                                                              const uint32_t* __restrict__ cold_list, FiltStage f, uint32_t dtype, L* __restrict__ stage) {
   const uint64_t k = blockIdx.x;
@@ -81,7 +85,7 @@ __global__ void __launch_bounds__(FL_THREADS) fl_cold_kernel(const ApState* __re
   if (p >= state->fail_page || p >= (state->decode_fail >> 32)) return;
   const IndexChunk rec = recs[p];
   const FiltKey key = filt_bounds<L>(f.interval, dtype);
-  fl_filter_in_place<L>(f, key, rec, p, stage);
+  fl_filter_in_place<L, AGG>(f, key, rec, p, stage);
 }
 
 // ceil(slots / FL_THREADS) CTAs: the sum of each CTA's counts.

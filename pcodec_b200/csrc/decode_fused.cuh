@@ -314,8 +314,8 @@ __device__ __forceinline__ void fused_undelta(L (&x)[8], FusedSmem& sm, uint32_t
 }
 
 // A decoder warp: batches first + d, first + d + FZ_DECODERS, ... of the chunk (K = consecutive delta order; first = 0 unless WIN and K = 0).
-// FILT: the batches go through filt_store8 (fkey: the interval's keys; fslot0: the chunk's first batch slot).
-template <typename L, int K, bool WIN, bool FILT = false>
+// FILT: the batches go through filt_store8 (fkey: the interval's keys; fslot0: the chunk's first batch slot); AGG: through agg_store8.
+template <typename L, int K, bool WIN, bool FILT = false, bool AGG = false>
 __device__ __forceinline__ void fused_decoder(FusedSmem& sm, const FileParams& fp, const BitSrc& src, const IndexChunk& task, uint64_t chunk_bit0, L* __restrict__ out,
                                               uint32_t n, uint32_t n_out, uint32_t first, const WinTask& win, int d, int lane,
                                               const FiltStage& filt = {}, const FiltKey& fkey = {}, uint64_t fslot0 = 0) {
@@ -470,7 +470,9 @@ __device__ __forceinline__ void fused_decoder(FusedSmem& sm, const FileParams& f
 #pragma unroll
       for (int e = 0; e < 8; e++) res[e] = from_latent_kind<L>(res[e], kind);
     }
-    if constexpr (FILT) {
+    if constexpr (AGG) {
+      agg_store8<L>(filt, fkey, fslot0 + b, min(uint32_t(BATCH_N), n_out - b * BATCH_N), lane, res);
+    } else if constexpr (FILT) {
       filt_store8<L>(filt, fkey, out, task.out_offset + uint64_t(b) * BATCH_N, fslot0 + b, min(uint32_t(BATCH_N), n_out - b * BATCH_N), lane, res);
     } else if constexpr (WIN) {
       win_store8<L>(win, b, lane, res);
@@ -508,7 +510,8 @@ __device__ __forceinline__ void fused_decoder(FusedSmem& sm, const FileParams& f
 // WIN: window mode (decode_kernels.cuh, WinTask): task t stores only the numbers wins[t] names (out and out_len are unused), and the
 // status word of a chunk handed to the general pair holds its first batch, which sizes that task's scratch rows.
 // FILT: filter mode (decode_kernels.cuh, filt_store8): only the numbers inside *filt.interval are staged, with out as the value staging.
-template <typename L, bool WIN = false, bool FILT = false>
+// AGG (with FILT): aggregate mode (agg_store8): the matches reduced per batch; out is not written.
+template <typename L, bool WIN = false, bool FILT = false, bool AGG = false>
 __global__ void __launch_bounds__(FZ_THREADS, PCOB_FZ_MIN_BLOCKS)
 fused_narrow_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, const uint8_t* __restrict__ index_base, uint64_t index_len,
                     uint32_t* __restrict__ statuses, uint8_t* __restrict__ d_cls, L* __restrict__ out, uint64_t out_len,
@@ -674,14 +677,14 @@ fused_narrow_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, const 
       fslot0 = task.out_offset / BATCH_N + filt.fast_page[blockIdx.x];
     }
     switch (K) {
-      case 0: fused_decoder<L, 0, WIN, FILT>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
-      case 1: fused_decoder<L, 1, WIN, FILT>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
-      case 2: fused_decoder<L, 2, WIN, FILT>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
-      case 3: fused_decoder<L, 3, WIN, FILT>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
-      case 4: fused_decoder<L, 4, WIN, FILT>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
-      case 5: fused_decoder<L, 5, WIN, FILT>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
-      case 6: fused_decoder<L, 6, WIN, FILT>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
-      default: fused_decoder<L, 7, WIN, FILT>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
+      case 0: fused_decoder<L, 0, WIN, FILT, AGG>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
+      case 1: fused_decoder<L, 1, WIN, FILT, AGG>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
+      case 2: fused_decoder<L, 2, WIN, FILT, AGG>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
+      case 3: fused_decoder<L, 3, WIN, FILT, AGG>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
+      case 4: fused_decoder<L, 4, WIN, FILT, AGG>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
+      case 5: fused_decoder<L, 5, WIN, FILT, AGG>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
+      case 6: fused_decoder<L, 6, WIN, FILT, AGG>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
+      default: fused_decoder<L, 7, WIN, FILT, AGG>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
     }
   }
   __syncthreads();

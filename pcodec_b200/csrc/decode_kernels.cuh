@@ -867,13 +867,21 @@ __device__ __forceinline__ void win_store8(const WinTask& w, uint32_t b, int lan
 // slot can never overflow into another batch's.  Its count goes to counts[slot] and, when it has matches, its row to rows[slot]; the
 // slot of batch b of page p (the page's numbers start at row O) is O / 256 + p + b, distinct for every batch of a batch of pages.
 // ---------------------------------------------------------------------------
+// Aggregate mode (the AGG instantiations, both aggregate calls): the same slots, but a batch's matches are reduced in registers
+// (agg_store8) and only counts[slot] and, when it has matches, its AggSlot are written.  FiltStage is the filter's, unchanged: in aggregate
+// mode its `rows` pointer carries the AggSlot array (agg_slots) and offs is unused.
+struct AggSlot {
+  uint64_t kmin, kmax;  // the least and greatest match as filt_key keys
+  uint64_t lo, hi;      // integers: the 128-bit sum; floats: lo is the f64 sum's bit pattern, hi 0
+};
 struct FiltStage {
   const uint64_t* interval;   // PcoB200Interval: lo_bits, hi_bits (zero-extended bit patterns of the plan's number type)
   const uint32_t* fast_page;  // decode-table record -> its page (the files filter: the record itself)
   uint32_t* counts;           // per slot: the batch's matches
-  uint64_t* rows;             // per slot with matches: the batch's first row
+  uint64_t* rows;             // per slot with matches: the batch's first row (aggregate mode: the AggSlot array)
   uint8_t* offs;              // per row: a staged match's offset in its batch
 };
+__host__ __device__ inline AggSlot* agg_slots(const FiltStage& f) { return reinterpret_cast<AggSlot*>(f.rows); }
 // The interval as keys of the order-preserving map below: a number x matches when any && key(x) - lo <= span (mod 2^bits).
 struct FiltKey {
   uint64_t lo, span;
@@ -930,6 +938,74 @@ __device__ __forceinline__ void filt_store8(const FiltStage& f, const FiltKey& k
   if (lane == 0) {
     f.counts[slot] = total;
     if (total) f.rows[slot] = row;
+  }
+}
+// A number as f64 (f16, f32, f64: exact), and as 64 bits zero-extended (kind 0, 2) or sign-extended (kind 1).
+template <typename L>
+__device__ __forceinline__ double agg_f64(L x) {
+  if constexpr (LT<L>::BITS == 16) {  // f16 bits to f64 bits: sign, exponent rebased from 15 to 1023, mantissa shifted up 42
+    const uint64_t b = uint64_t(x), e = (b >> 10) & 31u, m = b & 1023u, sign = (b >> 15) << 63;
+    if (e == 0) return __longlong_as_double((long long)sign) + (sign ? -1.0 : 1.0) * double(m) * 5.9604644775390625e-08;  // m 2^-24
+    return __longlong_as_double((long long)(sign | ((e == 31 ? uint64_t(2047) : e + 1008) << 52) | (m << 42)));
+  }
+  else if constexpr (LT<L>::BITS == 32) return double(__uint_as_float(uint32_t(x)));
+  else if constexpr (LT<L>::BITS == 64) return __longlong_as_double((long long)(x));
+  else return 0.0;  // no 8-bit float type
+}
+template <typename L>
+__device__ __forceinline__ uint64_t agg_ext(L x, uint32_t kind) {
+  constexpr int SH = 64 - LT<L>::BITS;
+  return kind == 1 ? uint64_t(int64_t(uint64_t(x) << SH) >> SH) : uint64_t(x);
+}
+// (lo, hi) += (blo, bhi), 128-bit two's complement
+__device__ __forceinline__ void agg_add128(uint64_t& lo, uint64_t& hi, uint64_t blo, uint64_t bhi) {
+  lo += blo;
+  hi += bhi + (lo < blo ? 1u : 0u);
+}
+// The warp's reductions by an xor butterfly at distances 1, 2, 4, 8, 16 (every lane ends with them): the least and greatest key, and the
+// 128-bit sum (integers) or the f64 sum (floats: lanes (0, 1), (2, 3), ... then pairs of pairs).
+__device__ __forceinline__ void agg_warp(uint64_t& kmin, uint64_t& kmax, uint64_t& lo, uint64_t& hi, double& fs, bool is_float) {
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    kmin = min(kmin, __shfl_xor_sync(0xffffffffu, kmin, d));
+    kmax = max(kmax, __shfl_xor_sync(0xffffffffu, kmax, d));
+    if (is_float) {
+      fs = fs + __shfl_xor_sync(0xffffffffu, fs, d);
+    } else {
+      const uint64_t ol = __shfl_xor_sync(0xffffffffu, lo, d), oh = __shfl_xor_sync(0xffffffffu, hi, d);
+      agg_add128(lo, hi, ol, oh);
+    }
+  }
+}
+// Aggregate mode's store: the lane's 8 numbers of a batch of `cnt` numbers (slot `slot`) tested against the interval; the matches'
+// count (ballots), least and greatest key, and sum (the lane's matches left to right from +0.0, then agg_warp) reduced in the warp, and
+// written by lane 0 when there is a match.  All 32 lanes call it.
+template <typename L>
+__device__ __forceinline__ void agg_store8(const FiltStage& f, const FiltKey& k, uint64_t slot, uint32_t cnt, int lane, const L (&r)[8]) {
+  uint32_t total = 0;
+  uint64_t kmin = ~uint64_t(0), kmax = 0, lo = 0, hi = 0;
+  double fs = 0.0;
+#pragma unroll
+  for (int e = 0; e < 8; e++) {
+    const L key = filt_key<L>(r[e], k.kind);
+    const bool hit = k.any && uint32_t(lane * 8 + e) < cnt && L(key - L(k.lo)) <= L(k.span);
+    total += __popc(__ballot_sync(0xffffffffu, hit));
+    if (hit) {
+      kmin = min(kmin, uint64_t(key));
+      kmax = max(kmax, uint64_t(key));
+      if (k.kind == 2) {
+        fs = fs + agg_f64<L>(r[e]);
+      } else {
+        const uint64_t v = agg_ext<L>(r[e], k.kind);
+        agg_add128(lo, hi, v, k.kind == 1 && int64_t(v) < 0 ? ~uint64_t(0) : 0);
+      }
+    }
+  }
+  if (total == 0) return;  // the slot stays empty: its count is cleared before the decode
+  agg_warp(kmin, kmax, lo, hi, fs, k.kind == 2);
+  if (lane == 0) {
+    f.counts[slot] = total;
+    agg_slots(f)[slot] = AggSlot{kmin, kmax, k.kind == 2 ? uint64_t(__double_as_longlong(fs)) : lo, hi};
   }
 }
 template <typename L>
@@ -1206,7 +1282,8 @@ __global__ void __launch_bounds__(SW_THREADS) symwalk_kernel(FileParams fp, cons
 // chunk's var count) - one-var chunks then run with the registers of one var and a third CTA per SM.
 // WIN: window mode (symwalk_kernel<true> made the rows; wins[t] says which numbers of task t to store and where; out and out_len are unused).
 // FILT: filter mode (filt_store8: only the numbers inside *filt.interval are staged, in row order, with out as the value staging).
-template <typename L, int NV, bool WIN = false, bool FILT = false>
+// AGG (with FILT): aggregate mode (agg_store8: the matches reduced per batch into filt.counts and filt.agg; out is not written).
+template <typename L, int NV, bool WIN = false, bool FILT = false, bool AGG = false>
 __global__ void __launch_bounds__(DEC_THREADS, NV == 1 ? PCOB_DEC_NV1_BLOCKS : 2)
 decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __restrict__ statuses, const uint8_t* __restrict__ index_base, uint64_t index_len,
               L* __restrict__ out, uint64_t out_len, const Binoms* __restrict__ binoms, const uint8_t* __restrict__ d_syms,
@@ -1587,7 +1664,9 @@ decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __
             res[e] = from_latent_kind<L>(L(L(pq << k) + lowest), 2);
           }
         }
-        if constexpr (FILT) {
+        if constexpr (AGG) {
+          agg_store8<L>(filt, fkey, fslot0 + b, out_cnt, lane, res);
+        } else if constexpr (FILT) {
           filt_store8<L>(filt, fkey, out, task.out_offset + uint64_t(b) * BATCH_N, fslot0 + b, out_cnt, lane, res);
         } else if constexpr (WIN) {
           win_store8<L>(wins[blockIdx.x], b, lane, res);

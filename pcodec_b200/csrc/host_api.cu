@@ -7,6 +7,7 @@
 #include "async_compress.cuh"
 #include "async_compress_files.cuh"
 #include "async_compress_wrapped.cuh"
+#include "async_aggregate_kernels.cuh"
 #include "async_filter_files_kernels.cuh"
 #include "async_filter_kernels.cuh"
 #include "async_files_kernels.cuh"
@@ -42,7 +43,7 @@ namespace pcob200 {
 // The context follows the thread's current device: a cudaSetDevice between calls drops the scratch of the previous device.
 struct Context {
   int device = -1;
-  bool attrs_set[3] = {false, false, false};  // set_decode_attrs<WIN, FILT> has run (index WIN + 2 FILT)
+  bool attrs_set[4] = {false, false, false, false};  // set_decode_attrs<WIN, FILT, AGG> has run (index WIN + 2 FILT + AGG)
   bool initialized = false;
   bool device_ok = false;
   std::string device_err;
@@ -149,22 +150,22 @@ struct DecodeOutcome {
   bool terminated = false;
 };
 
-// Shared-memory attributes of the decode kernels (the window-mode instantiations when WIN, the filter-mode ones when FILT), set once per
-// context before their first launch.
-template <bool WIN, bool FILT = false>
+// Shared-memory attributes of the decode kernels (the window-mode instantiations when WIN, the filter-mode ones when FILT, the
+// aggregate-mode ones when AGG too), set once per context before their first launch.
+template <bool WIN, bool FILT = false, bool AGG = false>
 static PcoB200Error set_decode_attrs(Context& c) {
-  static_assert(!(WIN && FILT), "no instantiation is both");
-  if (c.attrs_set[WIN + 2 * FILT]) return PCO_B200_OK;
-  c.attrs_set[WIN + 2 * FILT] = true;
+  static_assert(!(WIN && FILT) && (FILT || !AGG), "no instantiation is both window and filter mode; aggregate mode is a filter mode");
+  if (c.attrs_set[WIN + 2 * FILT + AGG]) return PCO_B200_OK;
+  c.attrs_set[WIN + 2 * FILT + AGG] = true;
   auto max_shared = [](auto* kernel, size_t smem) {
     const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
     return e != cudaSuccess ? e : cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, int(cudaSharedmemCarveoutMaxShared));
   };
   PCOB_CUDA_TRY(max_shared(symwalk_kernel<WIN>, sizeof(SymWalkSmem)));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint64_t, WIN, FILT>, sizeof(FusedSmem)));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint32_t, WIN, FILT>, sizeof(FusedSmem)));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint16_t, WIN, FILT>, sizeof(FusedSmem)));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint8_t, WIN, FILT>, sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint64_t, WIN, FILT, AGG>, sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint32_t, WIN, FILT, AGG>, sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint16_t, WIN, FILT, AGG>, sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint8_t, WIN, FILT, AGG>, sizeof(FusedSmem)));
   return PCO_B200_OK;
 }
 
@@ -777,18 +778,18 @@ static PcoB200Error load_kernels(std::initializer_list<const void*> kernels) {
 static PcoB200Error async_result_kind(uint32_t kind) { return kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(kind) : PCO_B200_CORRUPTION; }
 
 // The set-up of an asynchronous decompress plan: the device, the decode kernels' attributes (the window-mode instantiations when WIN, the
-// filter-mode ones when FILT), and loaded: the decode stage's kernels for dtype, the call's catch-all kernel (cold(tag) for a latent type
-// tag) and the call's `kernels`.
-template <bool WIN, bool FILT = false, typename Cold>
+// filter-mode ones when FILT, the aggregate-mode ones when AGG too), and loaded: the decode stage's kernels for dtype, the call's catch-all
+// kernel (cold(tag) for a latent type tag) and the call's `kernels`.
+template <bool WIN, bool FILT = false, bool AGG = false, typename Cold>
 static PcoB200Error async_decode_setup(unsigned char dtype, Cold cold, std::initializer_list<const void*> kernels) {
   Context& c = ctx();
   if (PcoB200Error e = ensure_device(c)) return e;
-  if (PcoB200Error e = set_decode_attrs<WIN, FILT>(c)) return e;
+  if (PcoB200Error e = set_decode_attrs<WIN, FILT, AGG>(c)) return e;
   if (PcoB200Error e = load_kernels(kernels)) return e;
   return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
     using L = decltype(tag);
-    return load_kernels({(const void*)fused_narrow_kernel<L, WIN, FILT>, (const void*)symwalk_kernel<WIN>, (const void*)decode_kernel<L, 1, WIN, FILT>,
-                         (const void*)decode_kernel<L, 2, WIN, FILT>, cold(tag)});
+    return load_kernels({(const void*)fused_narrow_kernel<L, WIN, FILT, AGG>, (const void*)symwalk_kernel<WIN>, (const void*)decode_kernel<L, 1, WIN, FILT, AGG>,
+                         (const void*)decode_kernel<L, 2, WIN, FILT, AGG>, cold(tag)});
   });
 }
 
@@ -852,15 +853,15 @@ struct DecodeStage {
   void* dst;
   uint64_t dst_cap;
   const WinTask* wins;
-  FiltStage filt;  // FILT: dst is the value staging (decode_kernels.cuh, filt_store8)
+  FiltStage filt;  // FILT: dst is the value staging (decode_kernels.cuh, filt_store8); AGG: dst is null (agg_store8)
 };
-template <bool WIN, bool FILT = false>
+template <bool WIN, bool FILT = false, bool AGG = false>
 static void enqueue_decode_stage(const AsyncLaunch& ln, const DecodeStage& d) {
   const cudaStream_t stream = ln.stream;
   ln.begin("fused_narrow_kernel");
   dispatch_latent(d.fp.dtype, [&](auto tag) {
     using L = decltype(tag);
-    fused_narrow_kernel<L, WIN, FILT><<<d.slots, FZ_THREADS, sizeof(FusedSmem), stream>>>(d.fp, d.table, d.index, d.index_len, d.st, d.cls,
+    fused_narrow_kernel<L, WIN, FILT, AGG><<<d.slots, FZ_THREADS, sizeof(FusedSmem), stream>>>(d.fp, d.table, d.index, d.index_len, d.st, d.cls,
                                                                                          static_cast<L*>(d.dst), d.dst_cap, d.wins, d.filt);
     return 0;
   });
@@ -871,9 +872,9 @@ static void enqueue_decode_stage(const AsyncLaunch& ln, const DecodeStage& d) {
   ln.begin("decode_kernel");
   dispatch_latent(d.fp.dtype, [&](auto tag) {
     using L = decltype(tag);
-    decode_kernel<L, 1, WIN, FILT><<<d.slots, DEC_THREADS, sizeof(DecodeSmem), stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst),
+    decode_kernel<L, 1, WIN, FILT, AGG><<<d.slots, DEC_THREADS, sizeof(DecodeSmem), stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst),
                                                                                         d.dst_cap, d.binoms, d.syms, d.offs, d.cls, d.wins, d.filt);
-    decode_kernel<L, 2, WIN, FILT><<<d.slots, DEC_THREADS, sizeof(DecodeSmem), stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst),
+    decode_kernel<L, 2, WIN, FILT, AGG><<<d.slots, DEC_THREADS, sizeof(DecodeSmem), stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst),
                                                                                         d.dst_cap, d.binoms, d.syms, d.offs, d.cls, d.wins, d.filt);
     return 0;
   });
@@ -2783,9 +2784,10 @@ PcoB200Error pco_b200_decompress_files_async_plan(const void* head, size_t head_
 // The launches of pco_b200_decompress_files_async over the workspace `ws` laid out by `lay`: the front end, the decode stage, the
 // catch-all decoder into dst and af_finish_kernel into *status (and file_ns).  With `filt` the decode stage runs its filter-mode
 // instantiations, dst is their value staging, and ff_cold_list_kernel records the cold records in the cold list `cold_list` before the
-// catch-all decoder runs (pco_b200_filter_files_async).
+// catch-all decoder runs (pco_b200_filter_files_async).  With `agg` too, the aggregate-mode instantiations, which store nothing to dst;
+// dst is the catch-all decoder's value staging only (pco_b200_aggregate_files_async).
 static void enqueue_files(const AsyncLaunch& ln, const AfArgs& g, const AfLayout& lay, uint8_t* ws, void* dst, const FiltStage* filt,
-                          uint32_t* cold_list, uint64_t* file_ns, PcoB200AsyncFilesStatus* status) {
+                          uint32_t* cold_list, uint64_t* file_ns, PcoB200AsyncFilesStatus* status, bool agg = false) {
   const cudaStream_t stream = ln.stream;
   const uint32_t mf = g.max_files, mc = g.max_chunks;
   AsyncCheck* chk = reinterpret_cast<AsyncCheck*>(ws);
@@ -2819,9 +2821,10 @@ static void enqueue_files(const AsyncLaunch& ln, const AfArgs& g, const AfLayout
   merge_index_kernel<<<mf, 256, 0, stream>>>(d_idx, merges, table);
   ln.end();
   const DecodeStage d{g.fp, table, d_idx, g.index_cap, mc, d_st, ws + lay.cls, ws + lay.syms, reinterpret_cast<uint32_t*>(ws + lay.offs),
-                      &chk->binoms, dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{}};
+                      &chk->binoms, agg ? nullptr : dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{}};
   if (filt) {
-    enqueue_decode_stage<false, true>(ln, d);
+    if (agg) enqueue_decode_stage<false, true, true>(ln, d);
+    else enqueue_decode_stage<false, true>(ln, d);
     ln.begin("ff_cold_list_kernel");
     ff_cold_list_kernel<<<uint32_t(ctas_of<FF_THREADS>(mc)), FF_THREADS, 0, stream>>>(chk, d_st, cold_list);
     ln.end();
@@ -3031,9 +3034,10 @@ PcoB200Error pco_b200_decompress_pages_async_plan(unsigned char dtype, size_t me
 
 // The launches of pco_b200_decompress_pages_async over the workspace `ws` laid out by `lay`: the front end, the decode stage, the
 // catch-all decoder into dst and ap_finish_kernel into *status.  With `filt` the decode stage runs its filter-mode instantiations and dst
-// is their value staging (pco_b200_filter_pages_async).
+// is their value staging (pco_b200_filter_pages_async).  With `agg` too, the aggregate-mode instantiations, which store nothing to dst;
+// dst is the catch-all decoder's value staging only (pco_b200_aggregate_pages_async).
 static void enqueue_pages(const AsyncLaunch& ln, const ApArgs& g, const ApLayout& lay, uint8_t* ws, void* dst, const FiltStage* filt,
-                          PcoB200AsyncPagesStatus* status) {
+                          PcoB200AsyncPagesStatus* status, bool agg = false) {
   const cudaStream_t stream = ln.stream;
   AsyncCheck* chk = reinterpret_cast<AsyncCheck*>(ws);
   ApState* state = reinterpret_cast<ApState*>(ws + lay.state);
@@ -3076,8 +3080,9 @@ static void enqueue_pages(const AsyncLaunch& ln, const ApArgs& g, const ApLayout
   ap_rewalk_kernel<<<1, WALK_THREADS, sizeof(WalkSmem<SMALL_MAX_SIZE_LOG>), stream>>>(g, state, tab, d_frames, d_idx, lay.index_len);
   ln.end();
   const DecodeStage d{fp, table, d_idx, lay.index_len, mp, d_st, ws + lay.cls, ws + lay.syms, reinterpret_cast<uint32_t*>(ws + lay.offs),
-                      &chk->binoms, dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{}};
-  if (filt) enqueue_decode_stage<false, true>(ln, d);
+                      &chk->binoms, agg ? nullptr : dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{}};
+  if (agg) enqueue_decode_stage<false, true, true>(ln, d);
+  else if (filt) enqueue_decode_stage<false, true>(ln, d);
   else enqueue_decode_stage<false>(ln, d);
   ln.begin("ap_cold_kernel");
   dispatch_latent(g.dtype, [&](auto tag) {
@@ -3236,6 +3241,185 @@ PcoB200Error pco_b200_filter_pages_async_result(const PcoB200AsyncFilterStatus* 
       return pco_b200_decompress_pages_async_result(&p, nullptr);
     }
   }
+}
+
+// ---- asynchronous aggregates of wrapped pages and of indexed files (pco_b200_aggregate_pages_async, pco_b200_aggregate_files_async;
+// kernels in async_aggregate_kernels.cuh).  A memset of the slot counts (and, for files, ff_map_kernel), then the decompress call's
+// launches (enqueue_pages / enqueue_files with the decode stage's aggregate-mode instantiations and rows_cap as dst_cap), then the cold
+// pass (fl_cold / ff_cold in aggregate mode), the group kernel over (groups, ag_split) CTAs, and the finish.  A second memset clears the
+// groups' accumulators.
+
+static bool ag_plan_ok(const PcoB200AsyncAggregatePlan* p) {
+  return nt_valid(p->dtype) && p->max_pages >= 1 && p->max_pages <= 0x7fffffffull && p->rows_cap <= (uint64_t(1) << 56) &&
+         p->frame_cap <= (uint64_t(1) << 56) && p->workspace_bytes == ag_layout(p->max_pages, p->rows_cap, p->frame_cap, nt_bits(p->dtype) / 8).ag_total;
+}
+
+PcoB200Error pco_b200_aggregate_pages_async_plan(unsigned char dtype, size_t metas_cap, size_t pages_cap, size_t max_pages, size_t rows_cap,
+                                                 size_t frame_cap, PcoB200AsyncAggregatePlan* plan) {
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (!plan) return fail(PCO_B200_INVALID_ARGUMENT, "null plan");
+  if (max_pages == 0 || uint64_t(max_pages) > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_pages must be 1 .. 2^31 - 1");
+  if (uint64_t(rows_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "rows_cap above 2^56 numbers");
+  if (uint64_t(frame_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "frame_cap above 2^56 bytes");
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->metas_cap = metas_cap;
+  plan->pages_cap = pages_cap;
+  plan->max_pages = max_pages;
+  plan->rows_cap = rows_cap;
+  plan->frame_cap = frame_cap;
+  plan->workspace_bytes = ag_layout(max_pages, rows_cap, frame_cap, nt_bits(dtype) / 8).ag_total;
+  if (PcoB200Error e = async_decode_setup<false, true, true>(dtype, [](auto tag) { return (const void*)ap_cold_kernel<decltype(tag)>; },
+                                                             {(const void*)ap_pages_kernel, (const void*)ap_scan_kernel, (const void*)ap_place_kernel,
+                                                              (const void*)frame_pages_kernel, (const void*)walk_kernel<SMALL_MAX_SIZE_LOG>,
+                                                              (const void*)ap_route_kernel, (const void*)ap_rewalk_kernel, (const void*)ap_finish_kernel}))
+    return e;
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
+    using L = decltype(tag);
+    return load_kernels({(const void*)fl_cold_kernel<L, true>, (const void*)ag_pages_kernel, (const void*)ag_finish_kernel<L>});
+  });
+}
+
+PcoB200Error pco_b200_aggregate_pages_async(const PcoB200AsyncAggregatePlan* plan, const void* metas, const void* pages, const PcoB200PageRef* refs,
+                                            const uint64_t* n_pages, const PcoB200Interval* interval, PcoB200Aggregate* aggs, PcoB200Aggregate* total,
+                                            void* workspace, PcoB200AsyncAggregateStatus* status, void* cuda_stream) {
+  if (!plan || !metas || !pages || !refs || !n_pages || !interval || !aggs || !total || !workspace || !status)
+    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (!ag_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_aggregate_pages_async_plan");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+  const cudaStream_t stream = ln.stream;
+
+  const uint32_t mp = uint32_t(plan->max_pages);
+  const AgLayout lay = ag_layout(mp, plan->rows_cap, plan->frame_cap, nt_bits(plan->dtype) / 8);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  const uint64_t slots = fl_slots(mp, plan->rows_cap);
+  const ApArgs g{static_cast<const uint8_t*>(metas), static_cast<const uint8_t*>(pages), refs, n_pages, plan->metas_cap, plan->pages_cap, plan->rows_cap,
+                 plan->frame_cap, plan->dtype, mp};
+  // aggregate mode: the AggSlot array travels in FiltStage's rows pointer (agg_slots)
+  const FiltStage filt{reinterpret_cast<const uint64_t*>(interval), reinterpret_cast<const uint32_t*>(ws + lay.fast_page),
+                       reinterpret_cast<uint32_t*>(ws + lay.counts), reinterpret_cast<uint64_t*>(ws + lay.aslots), nullptr};
+  auto* groups = reinterpret_cast<AgGroup*>(ws + lay.groups);
+  auto* pstatus = reinterpret_cast<PcoB200AsyncPagesStatus*>(ws + lay.pstatus);
+
+  PCOB_CUDA_TRY(cudaMemsetAsync(filt.counts, 0, slots * sizeof(uint32_t), stream));
+  PCOB_CUDA_TRY(cudaMemsetAsync(groups, 0, uint64_t(mp) * sizeof(AgGroup), stream));
+  enqueue_pages(ln, g, lay, ws, ws + lay.stage, &filt, pstatus, true);
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    ln.begin("fl_cold_kernel");
+    fl_cold_kernel<L, true><<<mp, FL_THREADS, 0, stream>>>(reinterpret_cast<const ApState*>(ws + lay.state), reinterpret_cast<const IndexChunk*>(ws + lay.index),
+                                                          reinterpret_cast<const uint32_t*>(ws + lay.cold_list), filt, plan->dtype,
+                                                          reinterpret_cast<L*>(ws + lay.stage));
+    ln.end();
+    ln.begin("ag_pages_kernel");
+    ag_pages_kernel<<<dim3(mp, ag_split(slots, mp)), AG_THREADS, 0, stream>>>(pstatus, reinterpret_cast<const IndexChunk*>(ws + lay.index), filt.counts,
+                                                                            agg_slots(filt), plan->dtype, groups);
+    ln.end();
+    ln.begin("ag_finish_kernel");
+    ag_finish_kernel<L><<<1, AG_THREADS, 0, stream>>>(pstatus, groups, reinterpret_cast<const IndexChunk*>(ws + lay.index), plan->dtype, aggs, total, status);
+    ln.end();
+    return 0;
+  });
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
+}
+
+PcoB200Error pco_b200_aggregate_pages_async_result(const PcoB200AsyncAggregateStatus* s, size_t* n_matches) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200AsyncFilterStatus f{s->kind, s->device_status, s->page, s->n_written, s->n_pages, s->frames_needed, s->n_matches, s->n_matches};
+  return pco_b200_filter_pages_async_result(&f, n_matches);  // the pages filter's words: rows_cap in the role of dst_cap
+}
+
+static bool agf_plan_ok(const PcoB200AsyncFilesAggregatePlan* p) {
+  return nt_valid(p->dtype) && p->max_files >= 1 && p->max_files <= 0x7fffffffull && p->max_chunks >= 1 && p->max_chunks <= 0xffffffffull &&
+         p->rows_cap <= (uint64_t(1) << 56) &&
+         p->workspace_bytes == agf_layout(p->max_files, p->max_chunks, p->rows_cap, nt_bits(p->dtype) / 8).agf_total;
+}
+
+PcoB200Error pco_b200_aggregate_files_async_plan(const void* head, size_t head_len, unsigned char dtype, size_t src_cap, size_t index_cap,
+                                                 size_t max_files, size_t max_chunks, size_t rows_cap, PcoB200AsyncFilesAggregatePlan* plan) {
+  StandaloneHeader hdr;
+  if (PcoB200Error e = check_async_head(head, head_len, dtype, plan, &hdr)) return e;
+  if (max_files == 0 || uint64_t(max_files) > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_files must be 1 .. 2^31 - 1");
+  if (max_chunks == 0 || uint64_t(max_chunks) > 0xffffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_chunks must be 1 .. 2^32 - 1");
+  if (uint64_t(rows_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "rows_cap above 2^56 numbers");
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->uniform_type = hdr.uniform_type;
+  plan->format_major = hdr.format_major;
+  plan->src_cap = src_cap;
+  plan->index_cap = index_cap;
+  plan->max_files = max_files;
+  plan->max_chunks = max_chunks;
+  plan->rows_cap = rows_cap;
+  plan->workspace_bytes = agf_layout(max_files, max_chunks, rows_cap, nt_bits(dtype) / 8).agf_total;
+  if (PcoB200Error e = async_decode_setup<false, true, true>(dtype, [](auto tag) { return (const void*)cold_chunks_kernel<decltype(tag)>; },
+                                                             {(const void*)af_files_kernel, (const void*)check_index_kernel, (const void*)af_scan_kernel,
+                                                              (const void*)af_place_kernel, (const void*)af_table_kernel, (const void*)merge_index_kernel,
+                                                              (const void*)af_finish_kernel, (const void*)ff_map_kernel, (const void*)ff_cold_list_kernel}))
+    return e;
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
+    using L = decltype(tag);
+    return load_kernels({(const void*)ff_cold_kernel<L, true>, (const void*)ag_files_kernel, (const void*)agf_finish_kernel<L>});
+  });
+}
+
+PcoB200Error pco_b200_aggregate_files_async(const PcoB200AsyncFilesAggregatePlan* plan, const void* src, const void* index, const PcoB200FileRef* files,
+                                            const uint64_t* n_files, const PcoB200Interval* interval, PcoB200Aggregate* aggs, PcoB200Aggregate* total,
+                                            void* workspace, PcoB200AsyncFilesAggregateStatus* status, void* cuda_stream) {
+  if (!plan || !src || !index || !files || !n_files || !interval || !aggs || !total || !workspace || !status)
+    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (!agf_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_aggregate_files_async_plan");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+  const cudaStream_t stream = ln.stream;
+
+  const uint32_t mf = uint32_t(plan->max_files), mc = uint32_t(plan->max_chunks);
+  const AgfLayout lay = agf_layout(mf, mc, plan->rows_cap, nt_bits(plan->dtype) / 8);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  const uint64_t slots = fl_slots(mc, plan->rows_cap);
+  const AfArgs g{FileParams{src, plan->src_cap, plan->dtype, plan->uniform_type, plan->format_major}, static_cast<const uint8_t*>(index),
+                 plan->index_cap, plan->rows_cap, files, n_files, mf, mc};
+  // aggregate mode: the AggSlot array travels in FiltStage's rows pointer (agg_slots)
+  const FiltStage filt{reinterpret_cast<const uint64_t*>(interval), reinterpret_cast<const uint32_t*>(ws + lay.slot_map),
+                       reinterpret_cast<uint32_t*>(ws + lay.counts), reinterpret_cast<uint64_t*>(ws + lay.aslots), nullptr};
+  auto* groups = reinterpret_cast<AgGroup*>(ws + lay.groups);
+  auto* fstatus = reinterpret_cast<PcoB200AsyncFilesStatus*>(ws + lay.fstatus);
+  auto* cold_list = reinterpret_cast<uint32_t*>(ws + lay.cold_list);
+
+  PCOB_CUDA_TRY(cudaMemsetAsync(filt.counts, 0, slots * sizeof(uint32_t), stream));
+  PCOB_CUDA_TRY(cudaMemsetAsync(groups, 0, uint64_t(mf) * sizeof(AgGroup), stream));
+  ln.begin("ff_map_kernel");
+  ff_map_kernel<<<uint32_t(ctas_of<FF_THREADS>(mc)), FF_THREADS, 0, stream>>>(mc, reinterpret_cast<uint32_t*>(ws + lay.slot_map), cold_list);
+  ln.end();
+  enqueue_files(ln, g, lay, ws, ws + lay.stage, &filt, cold_list, nullptr, fstatus, true);
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    ln.begin("ff_cold_kernel");
+    ff_cold_kernel<L, true><<<std::min(mc, uint32_t(FF_COLD_CTAS)), FL_THREADS, 0, stream>>>(cold_list, reinterpret_cast<const IndexChunk*>(ws + lay.table),
+                                                                                             filt, plan->dtype, reinterpret_cast<L*>(ws + lay.stage));
+    ln.end();
+    ln.begin("ag_files_kernel");
+    ag_files_kernel<<<dim3(mf, ag_split(slots, mf)), AG_THREADS, 0, stream>>>(fstatus, reinterpret_cast<const FileMerge*>(ws + lay.merges),
+                                                                            reinterpret_cast<const IndexChunk*>(ws + lay.table), filt.counts,
+                                                                            agg_slots(filt), plan->dtype, groups);
+    ln.end();
+    ln.begin("agf_finish_kernel");
+    agf_finish_kernel<L><<<1, AG_THREADS, 0, stream>>>(fstatus, groups, reinterpret_cast<const FileCheck*>(ws + lay.fchk), plan->dtype, aggs, total, status);
+    ln.end();
+    return 0;
+  });
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
+}
+
+PcoB200Error pco_b200_aggregate_files_async_result(const PcoB200AsyncFilesAggregateStatus* s, size_t* n_matches) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200AsyncFilesFilterStatus f{s->kind, s->device_status, s->file, s->chunk, s->n_written, s->n_files, s->n_matches, s->n_matches};
+  return pco_b200_filter_files_async_result(&f, n_matches);  // the files filter's words: rows_cap in the role of dst_cap
 }
 
 // ---- asynchronous compress (pco_b200_compress_async; gate kernels in async_compress.cuh).  The plan fixes the layout and the config;

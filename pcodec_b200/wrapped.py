@@ -454,6 +454,108 @@ def pack_interval(lo, hi, dtype):
     return np.array(bits, dtype=np.uint64).view(np.int64)
 
 
+def unpack_aggregates(records, dtype):
+    """The PcoB200Aggregate records `records` (an int64 array of shape (n, 6) or (6,), on the host) of numbers of `dtype` as a list of
+    (n_rows, count, min, max, sum) tuples: min and max as numpy scalars of `dtype` (0 when count is 0), the sum as a Python int (the exact
+    128-bit sum, signed for signed dtypes) or, for floats, a float (the f64 sum)."""
+    dt = np.dtype(dtype)
+    _lib.dtype_byte(dt)
+    ut = np.dtype(f"u{dt.itemsize}")
+    recs = np.asarray(records).reshape(-1, 6).view(np.uint64)
+    out = []
+    for n_rows, count, mn, mx, lo, hi in recs.tolist():
+        as_dt = lambda bits: np.array([bits], dtype=np.uint64).astype(ut).view(dt)[0]  # noqa: E731
+        if dt.kind == "f":
+            total = float(np.array([lo], dtype=np.uint64).view(np.float64)[0])
+        else:
+            total = (hi << 64) | lo
+            if dt.kind == "i" and hi >> 63:
+                total -= 1 << 128
+        out.append((int(n_rows), int(count), as_dt(mn), as_dt(mx), total))
+    return out
+
+
+class _CAsyncAggregatePlan(C.Structure):  # PcoB200AsyncAggregatePlan (include/pco_b200.h)
+    _fields_ = [("dtype", C.c_uint32), ("reserved", C.c_uint32), ("metas_cap", C.c_uint64), ("pages_cap", C.c_uint64), ("max_pages", C.c_uint64),
+                ("rows_cap", C.c_uint64), ("frame_cap", C.c_uint64), ("workspace_bytes", C.c_uint64)]
+
+
+class _CAsyncAggregateStatus(C.Structure):  # PcoB200AsyncAggregateStatus (include/pco_b200.h)
+    _fields_ = [("kind", C.c_uint32), ("device_status", C.c_uint32), ("page", C.c_uint64), ("n_written", C.c_uint64), ("n_pages", C.c_uint64),
+                ("frames_needed", C.c_uint64), ("n_matches", C.c_uint64)]
+
+
+def _lib_async_aggregate():
+    return _lib.bind("_async_aggregate_ready",
+                     pco_b200_aggregate_pages_async_plan=[C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p],
+                     pco_b200_aggregate_pages_async=[C.c_void_p] * 11,
+                     pco_b200_aggregate_pages_async_result=[C.c_void_p, C.POINTER(C.c_size_t)])
+
+
+def _check_aggregate_outputs(aggs, total, max_groups):
+    import torch
+
+    if aggs.dtype != torch.int64 or aggs.dim() != 2 or aggs.shape[1] != 6 or aggs.shape[0] < max_groups or not aggs.is_contiguous():
+        raise ValueError(f"aggs must be a contiguous int64 tensor of shape ({max_groups}, 6)")
+    if total.dtype != torch.int64 or total.numel() != 6 or not total.is_contiguous():
+        raise ValueError("total must be a contiguous 6-element int64 tensor")
+
+
+class AsyncPagesAggregate(_lib._AsyncCall):
+    """Decodes a batch of wrapped-format pages on the current CUDA stream and reduces the numbers inside a closed interval to count, min,
+    max and sum, per page and in all (pco_b200_aggregate_pages_async): each 256-number batch is reduced in the decoder's registers, so
+    neither the decoded pages nor the matches reach HBM.  Refs, their count and the interval are read from device tensors, so one captured
+    call serves new pages and new bounds on each replay.
+
+    The capacities are AsyncPagesDecompressor's, with rows_cap (the most numbers of a call's pages) in place of dst_cap; frame_cap defaults
+    to metas_cap + pages_cap + 20 * max_pages as there.  The call owns a device workspace (about rows_cap * (itemsize + 0.15) bytes beyond
+    the decompressor's) and a status; it serves one call in flight."""
+
+    _Plan, _Status = _CAsyncAggregatePlan, _CAsyncAggregateStatus
+
+    def __init__(self, dtype, metas_cap, pages_cap, max_pages, rows_cap, frame_cap=None, device=None):
+        self.dtype = np.dtype(dtype)
+        if frame_cap is None:
+            frame_cap = metas_cap + pages_cap + 20 * max_pages
+        self._make_plan(device, lambda plan: _lib_async_aggregate().pco_b200_aggregate_pages_async_plan(
+            C.c_ubyte(_lib.dtype_byte(self.dtype)), C.c_size_t(metas_cap), C.c_size_t(pages_cap), C.c_size_t(max_pages), C.c_size_t(rows_cap),
+            C.c_size_t(frame_cap), plan))
+        self._alloc()
+
+    def __call__(self, metas, pages, refs, n_pages, interval, aggs, total):
+        """Enqueues the aggregates of the pages refs[: n_pages[0]] names on torch.cuda.current_stream().  `metas`, `pages`, `refs` and
+        `n_pages` are as AsyncPagesDecompressor takes them; `interval` is a 2-element int64 CUDA tensor (pack_interval's bit patterns of lo
+        and hi), `aggs` an int64 CUDA tensor of shape (max_pages, 6) whose row i receives page i's PcoB200Aggregate, and `total` a 6-element
+        int64 CUDA tensor that receives the total (unpack_aggregates reads them).  Returns nothing and does not wait; result() reports the
+        outcome."""
+        import torch
+
+        p = self._plan
+        self._check_tensors(metas=metas, pages=pages, refs=refs, n_pages=n_pages, interval=interval, aggs=aggs, total=total)
+        if metas.numel() * metas.element_size() < p.metas_cap or pages.numel() * pages.element_size() < p.pages_cap:
+            raise ValueError(f"metas holds fewer than metas_cap = {p.metas_cap} bytes, or pages fewer than pages_cap = {p.pages_cap}")
+        if refs.dtype != torch.int64 or refs.dim() != 2 or refs.shape[1] != 5 or refs.shape[0] < p.max_pages:
+            raise ValueError(f"refs must be an int64 tensor of shape ({p.max_pages}, 5)")
+        if n_pages.dtype != torch.int64 or n_pages.numel() != 1:
+            raise ValueError("n_pages must be a 1-element int64 tensor")
+        if interval.dtype != torch.int64 or interval.numel() != 2:
+            raise ValueError("interval must be a 2-element int64 tensor")
+        _check_aggregate_outputs(aggs, total, p.max_pages)
+        rc = _lib_async_aggregate().pco_b200_aggregate_pages_async(
+            C.byref(p), C.c_void_p(metas.data_ptr()), C.c_void_p(pages.data_ptr()), C.c_void_p(refs.data_ptr()), C.c_void_p(n_pages.data_ptr()),
+            C.c_void_p(interval.data_ptr()), C.c_void_p(aggs.data_ptr()), C.c_void_p(total.data_ptr()), C.c_void_p(self.workspace.data_ptr()),
+            C.c_void_p(self.status.data_ptr()), self._stream())
+        _lib.check(rc)
+
+    def result(self):
+        """Copies the status of the last call back (waiting for it on the current stream) and returns the total match count, or raises
+        PcoError with the kind decompress_pages gives ("page 17: ...")."""
+        s = self.status_record()
+        nm = C.c_size_t()
+        _lib.check(_lib_async_aggregate().pco_b200_aggregate_pages_async_result(C.byref(s), C.byref(nm)))
+        return int(nm.value)
+
+
 class AsyncPagesFilter(_lib._AsyncCall):
     """Decodes a batch of wrapped-format pages on the current CUDA stream and writes only the numbers inside a closed interval, in row order,
     with their positions in the pages' concatenation (pco_b200_filter_pages_async): the predicate runs inside the decoder, so the decoded
