@@ -1086,6 +1086,129 @@ PcoB200Error pco_b200_aggregate_files_async(const PcoB200AsyncFilesAggregatePlan
  * total match count. */
 PcoB200Error pco_b200_aggregate_files_async_result(const PcoB200AsyncFilesAggregateStatus *host_status, size_t *n_matches);
 
+/* ---- asynchronous take from wrapped-format pages and from indexed standalone files (no reference counterpart): the numbers at given
+ * positions of the concatenation pco_b200_decompress_pages_async / pco_b200_decompress_files_async write, decoding only the pages or
+ * chunks the positions touch.  A reader that filtered column A (pco_b200_filter_pages_async / pco_b200_filter_files_async write the
+ * positions of the matches) gets column B at those rows, and a sampler or a join probe gets the rows it holds the ids of, without
+ * decompressing B whole: a page or chunk no position touches is not decoded, and each decoded batch writes its selected numbers straight to
+ * their final index.  Each call only enqueues kernels on the caller's stream and returns at once; it makes no synchronising, allocating or
+ * host-to-device copy call and refers to no memory of the library's per-thread scratch, so it can be captured in a CUDA graph, and a
+ * captured call may be replayed after pco_b200_thread_release or after any other call.  A plan made once outside any capture fixes the
+ * grids from its capacities; the refs, their count, the positions and their count are read on the device, so one captured graph serves
+ * new pages or files, new positions and new counts on each replay.
+ * positions (uint64_t[max_positions]), n_positions (one uint64_t) and out_values (max_positions numbers) are device memory, of the types a
+ * filter call writes its out_positions and n_matches in, so a filter's output is a take's input in the same graph.  A position indexes the
+ * concatenation; positions must be strictly ascending.  out_values[j] gets the bit pattern of the number at positions[j] (NaN payloads,
+ * signed zeros and infinities come through unchanged) for j < *n_positions, and nothing is written past them; *n_positions = 0 writes
+ * nothing.
+ * Refusals, in this order, each decided before any page or chunk is decoded; a refused call writes nothing to out_values:
+ *   1. the decompress call's refusals before its decode stage, in its order, with its kinds and naming the same page, or file and chunk:
+ *      for pages every check up to and including the walk of every page (meta and walk failures of any page), for files every check up
+ *      to and including placement (PCO_B200_ASYNC_PAGES_DST / PCO_B200_ASYNC_FILES_DST against rows_cap);
+ *   2. *n_positions above max_positions (PCO_B200_TAKE_TOO_MANY);
+ *   3. the lowest j with positions[j] <= positions[j - 1] (PCO_B200_TAKE_ORDER, position j);
+ *   4. the lowest j with positions[j] at or past the rows of the concatenation (PCO_B200_TAKE_PAST, position j).
+ * Then only the pages or chunks some position touches are decoded, so a decode failure is reported only for a touched one, as the
+ * decompress call names it; a corrupt page or chunk no position touches does not fail the call.  out_values then follows the rule the
+ * decompress call follows for dst: a position whose row that call would leave unwritten is left unwritten. */
+enum {
+  PCO_B200_TAKE_TOO_MANY = 0x301,  /* *n_positions (n_positions) is above the plan's max_positions (PCO_B200_INVALID_ARGUMENT) */
+  PCO_B200_TAKE_ORDER = 0x302,     /* positions[position] is not above the position before it (PCO_B200_INVALID_ARGUMENT) */
+  PCO_B200_TAKE_PAST = 0x303       /* positions[position] lies at or past the n_written rows of the concatenation (PCO_B200_INVALID_ARGUMENT) */
+};
+
+typedef struct PcoB200AsyncTakePlan {  /* filled by pco_b200_take_pages_async_plan; treat as opaque */
+  uint32_t dtype, reserved;
+  uint64_t metas_cap, pages_cap, max_pages, rows_cap, frame_cap, max_positions;
+  uint64_t workspace_bytes;            /* device workspace one in-flight call needs */
+} PcoB200AsyncTakePlan;
+
+typedef struct PcoB200AsyncTakeStatus {  /* written on the device by every call */
+  uint32_t kind;                         /* PcoB200Error */
+  uint32_t device_status;                /* the device word behind it: as PcoB200AsyncPagesStatus, or PCO_B200_TAKE_* */
+  uint64_t page;                         /* the page the outcome names (UINT64_MAX if none) */
+  uint64_t n_written;                    /* the rows of the concatenation (the sum of page_n), once every page passed its checks (0 on a
+                                            failure of the pages call) */
+  uint64_t n_pages;                      /* *n_pages as the call read it */
+  uint64_t frames_needed;                /* bytes of framed pages the batch needs, also when above frame_cap (0 when refused earlier) */
+  uint64_t n_positions;                  /* *n_positions as the call read it */
+  uint64_t position;                     /* the position index a PCO_B200_TAKE_ORDER / _PAST refusal names (UINT64_MAX if none) */
+  uint64_t records_decoded;              /* the pages decoded: those some position touches (0 unless the kind is OK) */
+} PcoB200AsyncTakeStatus;
+
+/* Makes a plan for takes of up to max_positions numbers from up to max_pages pages of dtype, whose refs point into metas_cap bytes of
+ * metas and pages_cap bytes of pages, holding at most rows_cap numbers in all (the role dst_cap plays in pco_b200_decompress_pages_async);
+ * frame_cap bounds the framed pages as in that call.  Checked before the device is touched: dtype (PCO_B200_INVALID_TYPE), max_pages in
+ * 1 .. 2^31 - 1, max_positions in 1 .. 2^56, rows_cap and frame_cap at most 2^56 (PCO_B200_INVALID_ARGUMENT).  Then *plan is filled and
+ * the one-time device set-up runs on the current device, which the calls must use (kernel attributes, and every kernel the call launches
+ * loaded); without a device that is PCO_B200_CUDA.
+ * workspace_bytes is pco_b200_decompress_pages_async_plan's formula with dst_cap = rows_cap, plus these regions, each rounded up to 256
+ * bytes, with S = floor(rows_cap / 256) + max_pages batch slots and E the bytes of a number of dtype: 40 (the pages status), 56 (the
+ * take's state), 16 S (each slot's run of positions), 4 max_pages (touched flags) and E rows_cap (the cold pages' values). */
+PcoB200Error pco_b200_take_pages_async_plan(unsigned char dtype, size_t metas_cap, size_t pages_cap, size_t max_pages, size_t rows_cap,
+                                            size_t frame_cap, size_t max_positions, PcoB200AsyncTakePlan *plan);
+/* Enqueues the take of positions[0 : *n_positions) from the pages refs[0 : *n_pages) names on `cuda_stream`, and the outcome into
+ * *status; returns without waiting.  metas (metas_cap bytes), pages (pages_cap bytes; may be the same buffer as metas), refs
+ * (PcoB200PageRef[max_pages]), n_pages (one uint64_t), positions, n_positions, out_values, workspace (plan->workspace_bytes, 256-byte
+ * aligned) and status are device pointers; one workspace serves one call in flight.  The positions index the concatenation
+ * pco_b200_decompress_pages_async writes for the same arguments with dst_cap = rows_cap.  The return value covers the host side only:
+ * null pointers, an unaligned workspace or a plan that was not filled (PCO_B200_INVALID_ARGUMENT), a launch the runtime refuses
+ * (PCO_B200_CUDA).  With pco_b200_profile_enable(1), a call outside a stream capture records its kernel spans for pco_b200_profile_last; a
+ * call inside a capture records none. */
+PcoB200Error pco_b200_take_pages_async(const PcoB200AsyncTakePlan *plan, const void *metas, const void *pages, const PcoB200PageRef *refs,
+                                       const uint64_t *n_pages, const uint64_t *positions, const uint64_t *n_positions, void *out_values,
+                                       void *workspace, PcoB200AsyncTakeStatus *status, void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory at a point of the caller's choosing.  Returns the kind,
+ * sets the last-error message as pco_b200_filter_pages_async_result words it ("page 17: ...") or, for the take's own refusals, naming the
+ * position index ("position 17: ..."), and, when the kind is OK, sets *n_written (may be NULL) to the numbers written (*n_positions). */
+PcoB200Error pco_b200_take_pages_async_result(const PcoB200AsyncTakeStatus *host_status, size_t *n_written);
+
+typedef struct PcoB200AsyncFilesTakePlan {  /* filled by pco_b200_take_files_async_plan; treat as opaque */
+  uint32_t dtype, uniform_type, format_major, reserved;
+  uint64_t src_cap, index_cap, max_files, max_chunks, rows_cap, max_positions;
+  uint64_t workspace_bytes;                 /* device workspace one in-flight call needs */
+} PcoB200AsyncFilesTakePlan;
+
+typedef struct PcoB200AsyncFilesTakeStatus {  /* written on the device by every call */
+  uint32_t kind;                              /* PcoB200Error */
+  uint32_t device_status;                     /* the device word behind it: as PcoB200AsyncFilesStatus, or PCO_B200_TAKE_* */
+  uint64_t file;                              /* the file the outcome names (UINT64_MAX if none) */
+  uint64_t chunk;                             /* the failing chunk, counted from that file's first chunk (UINT64_MAX if none) */
+  uint64_t n_written;                         /* the rows of the concatenation (the sum of the files' counts), once every file passed its
+                                                 checks and placement (0 before) */
+  uint64_t n_files;                           /* *n_files as the call read it */
+  uint64_t n_positions;                       /* *n_positions as the call read it */
+  uint64_t position;                          /* the position index a PCO_B200_TAKE_ORDER / _PAST refusal names (UINT64_MAX if none) */
+  uint64_t records_decoded;                   /* the chunks decoded: those some position touches (0 unless the kind is OK) */
+} PcoB200AsyncFilesTakeStatus;
+
+/* Makes a plan for takes of up to max_positions numbers from up to max_files indexed files of dtype holding at most max_chunks chunks and
+ * rows_cap numbers in all (the role dst_cap plays in pco_b200_decompress_files_async).  `head`, src_cap and index_cap are those of
+ * pco_b200_decompress_files_async_plan.  Checked before the device is touched, with that plan's kinds: dtype, the header, the uniform
+ * type, max_files in 1 .. 2^31 - 1, max_chunks in 1 .. 2^32 - 1, rows_cap at most 2^56, max_positions in 1 .. 2^56
+ * (PCO_B200_INVALID_ARGUMENT).  Then *plan is filled and the one-time device set-up runs on the current device, which the calls must use;
+ * without a device that is PCO_B200_CUDA.
+ * workspace_bytes is pco_b200_decompress_files_async_plan's formula with dst_cap = rows_cap, plus these regions, each rounded up to 256
+ * bytes, with S = floor(rows_cap / 256) + max_chunks batch slots and E the bytes of a number of dtype: 40 (the files status), 56 (the
+ * take's state), 16 S (each slot's run of positions), 4 max_chunks (touched flags), E rows_cap (the cold chunks' values), 4 max_chunks
+ * (slot map) and 4 (max_chunks + 1) (cold list). */
+PcoB200Error pco_b200_take_files_async_plan(const void *head, size_t head_len, unsigned char dtype, size_t src_cap, size_t index_cap,
+                                            size_t max_files, size_t max_chunks, size_t rows_cap, size_t max_positions,
+                                            PcoB200AsyncFilesTakePlan *plan);
+/* Enqueues the take of positions[0 : *n_positions) from files[0 : *n_files) on `cuda_stream`, and the outcome into *status; returns
+ * without waiting.  src (src_cap bytes), index (index_cap bytes), files (PcoB200FileRef[max_files]), n_files (one uint64_t), positions,
+ * n_positions, out_values, file_ns (uint64_t[max_files]; may be NULL), workspace (plan->workspace_bytes, 256-byte aligned) and status are
+ * device pointers; one workspace serves one call in flight.  The positions index the concatenation pco_b200_decompress_files_async writes
+ * for the same arguments with dst_cap = rows_cap; on success file_ns[i] gets file i's count, as that call writes it, and a failed or
+ * refused call writes no file_ns.  The return value covers the host side only, as for pco_b200_take_pages_async. */
+PcoB200Error pco_b200_take_files_async(const PcoB200AsyncFilesTakePlan *plan, const void *src, const void *index, const PcoB200FileRef *files,
+                                       const uint64_t *n_files, const uint64_t *positions, const uint64_t *n_positions, void *out_values,
+                                       uint64_t *file_ns, void *workspace, PcoB200AsyncFilesTakeStatus *status, void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory.  Returns the kind, sets the last-error message as
+ * pco_b200_filter_files_async_result words it ("file 3: chunk 2: ...") or, for the take's own refusals, naming the position index
+ * ("position 17: ..."), and, when the kind is OK, sets *n_written (may be NULL) to the numbers written (*n_positions). */
+PcoB200Error pco_b200_take_files_async_result(const PcoB200AsyncFilesTakeStatus *host_status, size_t *n_written);
+
 /* ---- asynchronous batch compress into wrapped-format chunks (no reference counterpart): pco_b200_compress_wrapped over a batch of
  * arrays, with the array sizes, their count and every buffer in device memory.  A GPU writer of a container that embeds pco (a columnar
  * file whose column chunks a kernel sized, a page store) compresses every column chunk behind the step that produced it, with no copy to

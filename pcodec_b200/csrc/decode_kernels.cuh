@@ -1008,6 +1008,70 @@ __device__ __forceinline__ void agg_store8(const FiltStage& f, const FiltKey& k,
     agg_slots(f)[slot] = AggSlot{kmin, kmax, k.kind == 2 ? uint64_t(__double_as_longlong(fs)) : lo, hi};
   }
 }
+// ---------------------------------------------------------------------------
+// Take mode (the TAKE instantiations, both take calls; with FILT): the same slots, but a batch stores the numbers at the caller's
+// positions straight to their final index.  The take's plan (async_take_kernels.cuh) gives slot s the run [first, end) of position
+// indices that fall in its batch; a strictly ascending position array makes each run contiguous.  FiltStage is unchanged: `interval`
+// carries the positions, `counts` one touched flag per record (a record no position touches leaves the fused kernel at once), `rows` the
+// TakeRun array (take_runs) and `offs` out_values.
+// ---------------------------------------------------------------------------
+struct TakeRun {
+  uint64_t first, end;  // the positions of the batch: positions[first .. end)
+};
+__host__ __device__ inline TakeRun* take_runs(const FiltStage& f) { return reinterpret_cast<TakeRun*>(f.rows); }
+// The run of a slot, and the lane's first position of it (0 for a lane past the run): what take_store8 reads first.  The fused decoder
+// loads them a batch ahead, so their latency overlaps the decode.
+__device__ __forceinline__ TakeRun take_run(const FiltStage& f, uint64_t slot) { return take_runs(f)[slot]; }
+__device__ __forceinline__ uint64_t take_pos0(const FiltStage& f, const TakeRun& run, int lane) {
+  return uint64_t(lane) < run.end - run.first ? f.interval[run.first + lane] : 0;
+}
+// Take mode's store: the lane's 8 numbers of a batch of `cnt` numbers (first row `row`) whose slot has the run `run` (pos0: take_pos0);
+// out_values[first + rank] gets the number at row + offset for every position in the run, rank counting the run's positions below it.
+// The lanes hold the run's positions and build the batch's 256-bit membership mask (8 words, each OR-reduced over the warp); a lane's 8
+// numbers are byte `lane` of it.  A run that holds the whole batch is stored as the batch (store8 when whole and aligned).  All 32 lanes
+// call it.
+template <typename L>
+__device__ __forceinline__ void take_store8(const FiltStage& f, const TakeRun& run, uint64_t pos0, uint64_t row, uint32_t cnt, int lane,
+                                            const L (&r)[8]) {
+  const uint32_t m = uint32_t(run.end - run.first);
+  if (m == 0) return;
+  L* __restrict__ out = reinterpret_cast<L*>(f.offs) + run.first;
+  if (m == cnt) {
+    if (cnt == BATCH_N && (reinterpret_cast<uintptr_t>(out + lane * 8) & 15) == 0) {
+      store8<L>(out + lane * 8, r, lane);
+    } else {
+#pragma unroll
+      for (int e = 0; e < 8; e++)
+        if (uint32_t(lane * 8 + e) < cnt) out[lane * 8 + e] = r[e];
+    }
+    return;
+  }
+  uint32_t w[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  for (uint32_t i = lane; i < m; i += 32) {
+    const uint32_t o = uint32_t((i == uint32_t(lane) ? pos0 : f.interval[run.first + i]) - row);
+#pragma unroll
+    for (int k = 0; k < 8; k++) w[k] |= (o >> 5) == uint32_t(k) ? 1u << (o & 31) : 0u;
+  }
+  uint32_t mine = 0, base = 0;
+#pragma unroll
+  for (int k = 0; k < 8; k++) {
+    const uint32_t v = __reduce_or_sync(0xffffffffu, w[k]);
+    if (k < (lane >> 2)) base += __popc(v);
+    if (k == (lane >> 2)) mine = v;
+  }
+  const uint32_t sh = uint32_t(lane & 3) * 8;
+  base += __popc(mine & ((1u << sh) - 1));
+  const uint32_t bits = (mine >> sh) & 0xffu;
+#pragma unroll
+  for (int e = 0; e < 8; e++)
+    if ((bits >> e) & 1u) out[base + __popc(bits & ((1u << e) - 1))] = r[e];
+}
+// take_store8 of the batch in slot `slot`, its run and first positions read here.
+template <typename L>
+__device__ __forceinline__ void take_store8(const FiltStage& f, uint64_t row, uint64_t slot, uint32_t cnt, int lane, const L (&r)[8]) {
+  const TakeRun run = take_run(f, slot);
+  take_store8<L>(f, run, take_pos0(f, run, lane), row, cnt, lane, r);
+}
 template <typename L>
 __device__ __forceinline__ void load8(const L* __restrict__ src, L (&r)[8]) {
   if (sizeof(L) == 8) {
@@ -1283,7 +1347,8 @@ __global__ void __launch_bounds__(SW_THREADS) symwalk_kernel(FileParams fp, cons
 // WIN: window mode (symwalk_kernel<true> made the rows; wins[t] says which numbers of task t to store and where; out and out_len are unused).
 // FILT: filter mode (filt_store8: only the numbers inside *filt.interval are staged, in row order, with out as the value staging).
 // AGG (with FILT): aggregate mode (agg_store8: the matches reduced per batch into filt.counts and filt.agg; out is not written).
-template <typename L, int NV, bool WIN = false, bool FILT = false, bool AGG = false>
+// TAKE (with FILT): take mode (take_store8: the numbers at the run's positions to out_values; out is not written).
+template <typename L, int NV, bool WIN = false, bool FILT = false, bool AGG = false, bool TAKE = false>
 __global__ void __launch_bounds__(DEC_THREADS, NV == 1 ? PCOB_DEC_NV1_BLOCKS : 2)
 decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __restrict__ statuses, const uint8_t* __restrict__ index_base, uint64_t index_len,
               L* __restrict__ out, uint64_t out_len, const Binoms* __restrict__ binoms, const uint8_t* __restrict__ d_syms,
@@ -1401,7 +1466,7 @@ decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __
   FiltKey fkey{};
   uint64_t fslot0 = 0;
   if constexpr (FILT) {
-    fkey = filt_bounds<L>(filt.interval, fp.dtype);
+    if constexpr (!TAKE) fkey = filt_bounds<L>(filt.interval, fp.dtype);
     fslot0 = task.out_offset / BATCH_N + filt.fast_page[blockIdx.x];
   }
   const uint64_t row0 = WIN ? wins[blockIdx.x].row0 : scratch_row0(task.out_offset, blockIdx.x);
@@ -1664,7 +1729,9 @@ decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __
             res[e] = from_latent_kind<L>(L(L(pq << k) + lowest), 2);
           }
         }
-        if constexpr (AGG) {
+        if constexpr (TAKE) {
+          take_store8<L>(filt, task.out_offset + uint64_t(b) * BATCH_N, fslot0 + b, out_cnt, lane, res);
+        } else if constexpr (AGG) {
           agg_store8<L>(filt, fkey, fslot0 + b, out_cnt, lane, res);
         } else if constexpr (FILT) {
           filt_store8<L>(filt, fkey, out, task.out_offset + uint64_t(b) * BATCH_N, fslot0 + b, out_cnt, lane, res);

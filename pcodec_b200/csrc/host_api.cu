@@ -2,6 +2,7 @@
 // There is no CPU implementation of the hot path in this library: without a CUDA device every
 // compute entry point fails with PCO_B200_CUDA.
 #include <algorithm>
+#include <functional>
 #include <initializer_list>
 
 #include "async_compress.cuh"
@@ -15,6 +16,7 @@
 #include "async_kernels.cuh"
 #include "async_pages_kernels.cuh"
 #include "async_ranges_kernels.cuh"
+#include "async_take_kernels.cuh"
 #include "compress_host.cuh"
 #include "decode_kernels.cuh"
 #include "decode_fused.cuh"
@@ -43,7 +45,7 @@ namespace pcob200 {
 // The context follows the thread's current device: a cudaSetDevice between calls drops the scratch of the previous device.
 struct Context {
   int device = -1;
-  bool attrs_set[4] = {false, false, false, false};  // set_decode_attrs<WIN, FILT, AGG> has run (index WIN + 2 FILT + AGG)
+  bool attrs_set[5] = {false, false, false, false, false};  // set_decode_attrs<WIN, FILT, AGG, TAKE> has run (index WIN + 2 FILT + AGG + 2 TAKE)
   bool initialized = false;
   bool device_ok = false;
   std::string device_err;
@@ -82,7 +84,7 @@ static void reset_context(Context& c) {
   c.d_binoms = nullptr;
   c.initialized = false;
   c.device_ok = false;
-  c.attrs_set[0] = c.attrs_set[1] = c.attrs_set[2] = false;
+  for (bool& a : c.attrs_set) a = false;
 }
 
 static PcoB200Error ensure_device(Context& c) {
@@ -151,21 +153,22 @@ struct DecodeOutcome {
 };
 
 // Shared-memory attributes of the decode kernels (the window-mode instantiations when WIN, the filter-mode ones when FILT, the
-// aggregate-mode ones when AGG too), set once per context before their first launch.
-template <bool WIN, bool FILT = false, bool AGG = false>
+// aggregate-mode ones when AGG too, the take-mode ones when TAKE too), set once per context before their first launch.
+template <bool WIN, bool FILT = false, bool AGG = false, bool TAKE = false>
 static PcoB200Error set_decode_attrs(Context& c) {
-  static_assert(!(WIN && FILT) && (FILT || !AGG), "no instantiation is both window and filter mode; aggregate mode is a filter mode");
-  if (c.attrs_set[WIN + 2 * FILT + AGG]) return PCO_B200_OK;
-  c.attrs_set[WIN + 2 * FILT + AGG] = true;
+  static_assert(!(WIN && FILT) && (FILT || !AGG) && (FILT || !TAKE) && !(AGG && TAKE),
+                "no instantiation is both window and filter mode; aggregate and take mode are filter modes, and exclusive");
+  if (c.attrs_set[WIN + 2 * FILT + AGG + 2 * TAKE]) return PCO_B200_OK;
+  c.attrs_set[WIN + 2 * FILT + AGG + 2 * TAKE] = true;
   auto max_shared = [](auto* kernel, size_t smem) {
     const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
     return e != cudaSuccess ? e : cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, int(cudaSharedmemCarveoutMaxShared));
   };
   PCOB_CUDA_TRY(max_shared(symwalk_kernel<WIN>, sizeof(SymWalkSmem)));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint64_t, WIN, FILT, AGG>, sizeof(FusedSmem)));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint32_t, WIN, FILT, AGG>, sizeof(FusedSmem)));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint16_t, WIN, FILT, AGG>, sizeof(FusedSmem)));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint8_t, WIN, FILT, AGG>, sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint64_t, WIN, FILT, AGG, TAKE>, sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint32_t, WIN, FILT, AGG, TAKE>, sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint16_t, WIN, FILT, AGG, TAKE>, sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint8_t, WIN, FILT, AGG, TAKE>, sizeof(FusedSmem)));
   return PCO_B200_OK;
 }
 
@@ -778,18 +781,18 @@ static PcoB200Error load_kernels(std::initializer_list<const void*> kernels) {
 static PcoB200Error async_result_kind(uint32_t kind) { return kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(kind) : PCO_B200_CORRUPTION; }
 
 // The set-up of an asynchronous decompress plan: the device, the decode kernels' attributes (the window-mode instantiations when WIN, the
-// filter-mode ones when FILT, the aggregate-mode ones when AGG too), and loaded: the decode stage's kernels for dtype, the call's catch-all
-// kernel (cold(tag) for a latent type tag) and the call's `kernels`.
-template <bool WIN, bool FILT = false, bool AGG = false, typename Cold>
+// filter-mode ones when FILT, the aggregate-mode ones when AGG too, the take-mode ones when TAKE too), and loaded: the decode stage's
+// kernels for dtype, the call's catch-all kernel (cold(tag) for a latent type tag) and the call's `kernels`.
+template <bool WIN, bool FILT = false, bool AGG = false, bool TAKE = false, typename Cold>
 static PcoB200Error async_decode_setup(unsigned char dtype, Cold cold, std::initializer_list<const void*> kernels) {
   Context& c = ctx();
   if (PcoB200Error e = ensure_device(c)) return e;
-  if (PcoB200Error e = set_decode_attrs<WIN, FILT, AGG>(c)) return e;
+  if (PcoB200Error e = set_decode_attrs<WIN, FILT, AGG, TAKE>(c)) return e;
   if (PcoB200Error e = load_kernels(kernels)) return e;
   return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
     using L = decltype(tag);
-    return load_kernels({(const void*)fused_narrow_kernel<L, WIN, FILT, AGG>, (const void*)symwalk_kernel<WIN>, (const void*)decode_kernel<L, 1, WIN, FILT, AGG>,
-                         (const void*)decode_kernel<L, 2, WIN, FILT, AGG>, cold(tag)});
+    return load_kernels({(const void*)fused_narrow_kernel<L, WIN, FILT, AGG, TAKE>, (const void*)symwalk_kernel<WIN>,
+                         (const void*)decode_kernel<L, 1, WIN, FILT, AGG, TAKE>, (const void*)decode_kernel<L, 2, WIN, FILT, AGG, TAKE>, cold(tag)});
   });
 }
 
@@ -853,15 +856,15 @@ struct DecodeStage {
   void* dst;
   uint64_t dst_cap;
   const WinTask* wins;
-  FiltStage filt;  // FILT: dst is the value staging (decode_kernels.cuh, filt_store8); AGG: dst is null (agg_store8)
+  FiltStage filt;  // FILT: dst is the value staging (decode_kernels.cuh, filt_store8); AGG: dst is null (agg_store8); TAKE: likewise (take_store8)
 };
-template <bool WIN, bool FILT = false, bool AGG = false>
+template <bool WIN, bool FILT = false, bool AGG = false, bool TAKE = false>
 static void enqueue_decode_stage(const AsyncLaunch& ln, const DecodeStage& d) {
   const cudaStream_t stream = ln.stream;
   ln.begin("fused_narrow_kernel");
   dispatch_latent(d.fp.dtype, [&](auto tag) {
     using L = decltype(tag);
-    fused_narrow_kernel<L, WIN, FILT, AGG><<<d.slots, FZ_THREADS, sizeof(FusedSmem), stream>>>(d.fp, d.table, d.index, d.index_len, d.st, d.cls,
+    fused_narrow_kernel<L, WIN, FILT, AGG, TAKE><<<d.slots, FZ_THREADS, sizeof(FusedSmem), stream>>>(d.fp, d.table, d.index, d.index_len, d.st, d.cls,
                                                                                          static_cast<L*>(d.dst), d.dst_cap, d.wins, d.filt);
     return 0;
   });
@@ -872,9 +875,9 @@ static void enqueue_decode_stage(const AsyncLaunch& ln, const DecodeStage& d) {
   ln.begin("decode_kernel");
   dispatch_latent(d.fp.dtype, [&](auto tag) {
     using L = decltype(tag);
-    decode_kernel<L, 1, WIN, FILT, AGG><<<d.slots, DEC_THREADS, sizeof(DecodeSmem), stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst),
+    decode_kernel<L, 1, WIN, FILT, AGG, TAKE><<<d.slots, DEC_THREADS, sizeof(DecodeSmem), stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst),
                                                                                         d.dst_cap, d.binoms, d.syms, d.offs, d.cls, d.wins, d.filt);
-    decode_kernel<L, 2, WIN, FILT, AGG><<<d.slots, DEC_THREADS, sizeof(DecodeSmem), stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst),
+    decode_kernel<L, 2, WIN, FILT, AGG, TAKE><<<d.slots, DEC_THREADS, sizeof(DecodeSmem), stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst),
                                                                                         d.dst_cap, d.binoms, d.syms, d.offs, d.cls, d.wins, d.filt);
     return 0;
   });
@@ -2785,9 +2788,12 @@ PcoB200Error pco_b200_decompress_files_async_plan(const void* head, size_t head_
 // catch-all decoder into dst and af_finish_kernel into *status (and file_ns).  With `filt` the decode stage runs its filter-mode
 // instantiations, dst is their value staging, and ff_cold_list_kernel records the cold records in the cold list `cold_list` before the
 // catch-all decoder runs (pco_b200_filter_files_async).  With `agg` too, the aggregate-mode instantiations, which store nothing to dst;
-// dst is the catch-all decoder's value staging only (pco_b200_aggregate_files_async).
+// dst is the catch-all decoder's value staging only (pco_b200_aggregate_files_async).  With `take` instead of `agg`, the take-mode
+// instantiations, likewise (pco_b200_take_files_async).  `between`, when given, enqueues its launches behind the front end
+// (merge_index_kernel) and before the decode stage.
 static void enqueue_files(const AsyncLaunch& ln, const AfArgs& g, const AfLayout& lay, uint8_t* ws, void* dst, const FiltStage* filt,
-                          uint32_t* cold_list, uint64_t* file_ns, PcoB200AsyncFilesStatus* status, bool agg = false) {
+                          uint32_t* cold_list, uint64_t* file_ns, PcoB200AsyncFilesStatus* status, bool agg = false, bool take = false,
+                          const std::function<void()>& between = {}) {
   const cudaStream_t stream = ln.stream;
   const uint32_t mf = g.max_files, mc = g.max_chunks;
   AsyncCheck* chk = reinterpret_cast<AsyncCheck*>(ws);
@@ -2820,10 +2826,12 @@ static void enqueue_files(const AsyncLaunch& ln, const AfArgs& g, const AfLayout
   ln.begin("merge_index_kernel");
   merge_index_kernel<<<mf, 256, 0, stream>>>(d_idx, merges, table);
   ln.end();
+  if (between) between();
   const DecodeStage d{g.fp, table, d_idx, g.index_cap, mc, d_st, ws + lay.cls, ws + lay.syms, reinterpret_cast<uint32_t*>(ws + lay.offs),
-                      &chk->binoms, agg ? nullptr : dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{}};
+                      &chk->binoms, agg || take ? nullptr : dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{}};
   if (filt) {
     if (agg) enqueue_decode_stage<false, true, true>(ln, d);
+    else if (take) enqueue_decode_stage<false, true, false, true>(ln, d);
     else enqueue_decode_stage<false, true>(ln, d);
     ln.begin("ff_cold_list_kernel");
     ff_cold_list_kernel<<<uint32_t(ctas_of<FF_THREADS>(mc)), FF_THREADS, 0, stream>>>(chk, d_st, cold_list);
@@ -3035,9 +3043,11 @@ PcoB200Error pco_b200_decompress_pages_async_plan(unsigned char dtype, size_t me
 // The launches of pco_b200_decompress_pages_async over the workspace `ws` laid out by `lay`: the front end, the decode stage, the
 // catch-all decoder into dst and ap_finish_kernel into *status.  With `filt` the decode stage runs its filter-mode instantiations and dst
 // is their value staging (pco_b200_filter_pages_async).  With `agg` too, the aggregate-mode instantiations, which store nothing to dst;
-// dst is the catch-all decoder's value staging only (pco_b200_aggregate_pages_async).
+// dst is the catch-all decoder's value staging only (pco_b200_aggregate_pages_async).  With `take` instead of `agg`, the take-mode
+// instantiations, likewise (pco_b200_take_pages_async).  `between`, when given, enqueues its launches behind the front end
+// (ap_rewalk_kernel) and before the decode stage.
 static void enqueue_pages(const AsyncLaunch& ln, const ApArgs& g, const ApLayout& lay, uint8_t* ws, void* dst, const FiltStage* filt,
-                          PcoB200AsyncPagesStatus* status, bool agg = false) {
+                          PcoB200AsyncPagesStatus* status, bool agg = false, bool take = false, const std::function<void()>& between = {}) {
   const cudaStream_t stream = ln.stream;
   AsyncCheck* chk = reinterpret_cast<AsyncCheck*>(ws);
   ApState* state = reinterpret_cast<ApState*>(ws + lay.state);
@@ -3079,9 +3089,11 @@ static void enqueue_pages(const AsyncLaunch& ln, const ApArgs& g, const ApLayout
   ln.begin("ap_rewalk_kernel");
   ap_rewalk_kernel<<<1, WALK_THREADS, sizeof(WalkSmem<SMALL_MAX_SIZE_LOG>), stream>>>(g, state, tab, d_frames, d_idx, lay.index_len);
   ln.end();
+  if (between) between();
   const DecodeStage d{fp, table, d_idx, lay.index_len, mp, d_st, ws + lay.cls, ws + lay.syms, reinterpret_cast<uint32_t*>(ws + lay.offs),
-                      &chk->binoms, agg ? nullptr : dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{}};
+                      &chk->binoms, agg || take ? nullptr : dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{}};
   if (agg) enqueue_decode_stage<false, true, true>(ln, d);
+  else if (take) enqueue_decode_stage<false, true, false, true>(ln, d);
   else if (filt) enqueue_decode_stage<false, true>(ln, d);
   else enqueue_decode_stage<false>(ln, d);
   ln.begin("ap_cold_kernel");
@@ -3420,6 +3432,237 @@ PcoB200Error pco_b200_aggregate_files_async_result(const PcoB200AsyncFilesAggreg
   if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
   const PcoB200AsyncFilesFilterStatus f{s->kind, s->device_status, s->file, s->chunk, s->n_written, s->n_files, s->n_matches, s->n_matches};
   return pco_b200_filter_files_async_result(&f, n_matches);  // the files filter's words: rows_cap in the role of dst_cap
+}
+
+// ---- asynchronous take from wrapped pages and from indexed files (pco_b200_take_pages_async, pco_b200_take_files_async; kernels in
+// async_take_kernels.cuh).  The decompress call's launches (enqueue_pages / enqueue_files with the decode stage's take-mode instantiations
+// and rows_cap as dst_cap; for files behind ff_map_kernel) with the take's plan between the front end and the decode stage: the front
+// kernel, the position checks, the marks (and, for pages, the cold list kept to the touched pages); then the cold take and the finish.
+
+// The take's plan, enqueued between the front end and the decode stage; `front` writes the TkState.
+static void enqueue_take_plan(const AsyncLaunch& ln, const std::function<void()>& front, const uint64_t* positions, uint64_t max_positions,
+                              const IndexChunk* recs, uint64_t max_records, TkState* ts, uint32_t* touched, TakeRun* runs) {
+  const cudaStream_t stream = ln.stream;
+  front();
+  ln.begin("tk_check_kernel");
+  tk_check_kernel<<<uint32_t(std::min(ctas_of<TK_THREADS>(max_positions), TK_MAX_CTAS)), TK_THREADS, 0, stream>>>(positions, max_positions, ts);
+  ln.end();
+  ln.begin("tk_mark_kernel");
+  tk_mark_kernel<<<uint32_t(std::min(max_records, TK_MAX_CTAS)), TK_THREADS, 0, stream>>>(positions, max_positions, recs, ts, touched, runs);
+  ln.end();
+}
+
+static bool tk_plan_ok(const PcoB200AsyncTakePlan* p) {
+  return nt_valid(p->dtype) && p->max_pages >= 1 && p->max_pages <= 0x7fffffffull && p->rows_cap <= (uint64_t(1) << 56) &&
+         p->frame_cap <= (uint64_t(1) << 56) && p->max_positions >= 1 && p->max_positions <= (uint64_t(1) << 56) &&
+         p->workspace_bytes == tk_layout(p->max_pages, p->rows_cap, p->frame_cap, nt_bits(p->dtype) / 8).tk_total;
+}
+
+PcoB200Error pco_b200_take_pages_async_plan(unsigned char dtype, size_t metas_cap, size_t pages_cap, size_t max_pages, size_t rows_cap,
+                                            size_t frame_cap, size_t max_positions, PcoB200AsyncTakePlan* plan) {
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (!plan) return fail(PCO_B200_INVALID_ARGUMENT, "null plan");
+  if (max_pages == 0 || uint64_t(max_pages) > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_pages must be 1 .. 2^31 - 1");
+  if (uint64_t(rows_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "rows_cap above 2^56 numbers");
+  if (uint64_t(frame_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "frame_cap above 2^56 bytes");
+  if (max_positions == 0 || uint64_t(max_positions) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "max_positions must be 1 .. 2^56");
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->metas_cap = metas_cap;
+  plan->pages_cap = pages_cap;
+  plan->max_pages = max_pages;
+  plan->rows_cap = rows_cap;
+  plan->frame_cap = frame_cap;
+  plan->max_positions = max_positions;
+  plan->workspace_bytes = tk_layout(max_pages, rows_cap, frame_cap, nt_bits(dtype) / 8).tk_total;
+  if (PcoB200Error e = async_decode_setup<false, true, false, true>(
+          dtype, [](auto tag) { return (const void*)ap_cold_kernel<decltype(tag)>; },
+          {(const void*)ap_pages_kernel, (const void*)ap_scan_kernel, (const void*)ap_place_kernel, (const void*)frame_pages_kernel,
+           (const void*)walk_kernel<SMALL_MAX_SIZE_LOG>, (const void*)ap_route_kernel, (const void*)ap_rewalk_kernel, (const void*)ap_finish_kernel,
+           (const void*)tk_front_pages_kernel, (const void*)tk_check_kernel, (const void*)tk_mark_kernel, (const void*)tk_cold_list_kernel,
+           (const void*)tk_finish_pages_kernel}))
+    return e;
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error { return load_kernels({(const void*)tk_cold_pages_kernel<decltype(tag)>}); });
+}
+
+PcoB200Error pco_b200_take_pages_async(const PcoB200AsyncTakePlan* plan, const void* metas, const void* pages, const PcoB200PageRef* refs,
+                                       const uint64_t* n_pages, const uint64_t* positions, const uint64_t* n_positions, void* out_values,
+                                       void* workspace, PcoB200AsyncTakeStatus* status, void* cuda_stream) {
+  if (!plan || !metas || !pages || !refs || !n_pages || !positions || !n_positions || !out_values || !workspace || !status)
+    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (!tk_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_take_pages_async_plan");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+  const cudaStream_t stream = ln.stream;
+
+  const uint32_t mp = uint32_t(plan->max_pages);
+  const TkLayout lay = tk_layout(mp, plan->rows_cap, plan->frame_cap, nt_bits(plan->dtype) / 8);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  const ApArgs g{static_cast<const uint8_t*>(metas), static_cast<const uint8_t*>(pages), refs, n_pages, plan->metas_cap, plan->pages_cap, plan->rows_cap,
+                 plan->frame_cap, plan->dtype, mp};
+  // take mode: the positions travel in FiltStage's interval pointer, the touched flags in counts, the runs in rows, out_values in offs
+  const FiltStage filt{positions, reinterpret_cast<const uint32_t*>(ws + lay.fast_page), reinterpret_cast<uint32_t*>(ws + lay.touched),
+                       reinterpret_cast<uint64_t*>(ws + lay.runs), static_cast<uint8_t*>(out_values)};
+  auto* state = reinterpret_cast<ApState*>(ws + lay.state);
+  auto* recs = reinterpret_cast<const IndexChunk*>(ws + lay.index);
+  auto* cold_list = reinterpret_cast<uint32_t*>(ws + lay.cold_list);
+  auto* pstatus = reinterpret_cast<PcoB200AsyncPagesStatus*>(ws + lay.pstatus);
+  auto* ts = reinterpret_cast<TkState*>(ws + lay.tstate);
+
+  enqueue_pages(ln, g, lay, ws, ws + lay.stage, &filt, pstatus, false, true, [&] {
+    auto front = [&] {
+      ln.begin("tk_front_pages_kernel");
+      tk_front_pages_kernel<<<1, 32, 0, stream>>>(state, n_positions, ts);
+      ln.end();
+    };
+    enqueue_take_plan(ln, front, positions, plan->max_positions, recs, mp, ts, filt.counts, take_runs(filt));
+    ln.begin("tk_cold_list_kernel");
+    tk_cold_list_kernel<<<1, TK_SCAN_THREADS, 0, stream>>>(state, cold_list, filt.counts);
+    ln.end();
+  });
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    ln.begin("tk_cold_pages_kernel");
+    tk_cold_pages_kernel<L><<<mp, TK_THREADS, 0, stream>>>(state, recs, cold_list, filt, reinterpret_cast<const L*>(ws + lay.stage));
+    ln.end();
+    return 0;
+  });
+  ln.begin("tk_finish_pages_kernel");
+  tk_finish_pages_kernel<<<1, 32, 0, stream>>>(pstatus, ts, plan->max_positions, status);
+  ln.end();
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
+}
+
+// The words of the take's own refusals of a position, or nullptr for any other status.
+static const char* tk_refusal(uint32_t device_status) {
+  switch (device_status) {
+    case PCO_B200_TAKE_ORDER: return "not above the position before it (positions must be strictly ascending)";
+    case PCO_B200_TAKE_PAST: return "lies at or past the rows of the concatenation";
+    default: return nullptr;
+  }
+}
+static PcoB200Error tk_result(PcoB200Error kind, uint32_t device_status, uint64_t n_positions, uint64_t position, uint64_t rows) {
+  if (device_status == PCO_B200_TAKE_TOO_MANY)
+    return fail(kind, "*n_positions is " + std::to_string(n_positions) + ", above the plan's max_positions");
+  std::string what = "position " + std::to_string(position) + ": " + tk_refusal(device_status);
+  if (device_status == PCO_B200_TAKE_PAST) what += " (" + std::to_string(rows) + " rows)";
+  return fail(kind, what);
+}
+
+PcoB200Error pco_b200_take_pages_async_result(const PcoB200AsyncTakeStatus* s, size_t* n_written) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200Error kind = async_result_kind(s->kind);
+  if (kind == PCO_B200_OK) {
+    if (n_written) *n_written = size_t(s->n_positions);
+    return PCO_B200_OK;
+  }
+  if (s->device_status == PCO_B200_TAKE_TOO_MANY || tk_refusal(s->device_status))
+    return tk_result(kind, s->device_status, s->n_positions, s->position, s->n_written);
+  const PcoB200AsyncFilterStatus f{s->kind, s->device_status, s->page, s->n_written, s->n_pages, s->frames_needed, 0, 0};
+  return pco_b200_filter_pages_async_result(&f, nullptr);  // the pages filter's words: rows_cap in the role of dst_cap
+}
+
+static bool tkf_plan_ok(const PcoB200AsyncFilesTakePlan* p) {
+  return nt_valid(p->dtype) && p->max_files >= 1 && p->max_files <= 0x7fffffffull && p->max_chunks >= 1 && p->max_chunks <= 0xffffffffull &&
+         p->rows_cap <= (uint64_t(1) << 56) && p->max_positions >= 1 && p->max_positions <= (uint64_t(1) << 56) &&
+         p->workspace_bytes == tkf_layout(p->max_files, p->max_chunks, p->rows_cap, nt_bits(p->dtype) / 8).tkf_total;
+}
+
+PcoB200Error pco_b200_take_files_async_plan(const void* head, size_t head_len, unsigned char dtype, size_t src_cap, size_t index_cap,
+                                            size_t max_files, size_t max_chunks, size_t rows_cap, size_t max_positions, PcoB200AsyncFilesTakePlan* plan) {
+  StandaloneHeader hdr;
+  if (PcoB200Error e = check_async_head(head, head_len, dtype, plan, &hdr)) return e;
+  if (max_files == 0 || uint64_t(max_files) > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_files must be 1 .. 2^31 - 1");
+  if (max_chunks == 0 || uint64_t(max_chunks) > 0xffffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_chunks must be 1 .. 2^32 - 1");
+  if (uint64_t(rows_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "rows_cap above 2^56 numbers");
+  if (max_positions == 0 || uint64_t(max_positions) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "max_positions must be 1 .. 2^56");
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->uniform_type = hdr.uniform_type;
+  plan->format_major = hdr.format_major;
+  plan->src_cap = src_cap;
+  plan->index_cap = index_cap;
+  plan->max_files = max_files;
+  plan->max_chunks = max_chunks;
+  plan->rows_cap = rows_cap;
+  plan->max_positions = max_positions;
+  plan->workspace_bytes = tkf_layout(max_files, max_chunks, rows_cap, nt_bits(dtype) / 8).tkf_total;
+  if (PcoB200Error e = async_decode_setup<false, true, false, true>(
+          dtype, [](auto tag) { return (const void*)cold_chunks_kernel<decltype(tag)>; },
+          {(const void*)af_files_kernel, (const void*)check_index_kernel, (const void*)af_scan_kernel, (const void*)af_place_kernel,
+           (const void*)af_table_kernel, (const void*)merge_index_kernel, (const void*)af_finish_kernel, (const void*)ff_map_kernel,
+           (const void*)ff_cold_list_kernel, (const void*)tk_front_files_kernel, (const void*)tk_check_kernel, (const void*)tk_mark_kernel,
+           (const void*)tk_finish_files_kernel}))
+    return e;
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error { return load_kernels({(const void*)tk_cold_files_kernel<decltype(tag)>}); });
+}
+
+PcoB200Error pco_b200_take_files_async(const PcoB200AsyncFilesTakePlan* plan, const void* src, const void* index, const PcoB200FileRef* files,
+                                       const uint64_t* n_files, const uint64_t* positions, const uint64_t* n_positions, void* out_values,
+                                       uint64_t* file_ns, void* workspace, PcoB200AsyncFilesTakeStatus* status, void* cuda_stream) {
+  if (!plan || !src || !index || !files || !n_files || !positions || !n_positions || !out_values || !workspace || !status)
+    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (!tkf_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_take_files_async_plan");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+  const cudaStream_t stream = ln.stream;
+
+  const uint32_t mf = uint32_t(plan->max_files), mc = uint32_t(plan->max_chunks);
+  const TkfLayout lay = tkf_layout(mf, mc, plan->rows_cap, nt_bits(plan->dtype) / 8);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  const AfArgs g{FileParams{src, plan->src_cap, plan->dtype, plan->uniform_type, plan->format_major}, static_cast<const uint8_t*>(index),
+                 plan->index_cap, plan->rows_cap, files, n_files, mf, mc};
+  // take mode: the positions travel in FiltStage's interval pointer, the touched flags in counts, the runs in rows, out_values in offs
+  const FiltStage filt{positions, reinterpret_cast<const uint32_t*>(ws + lay.slot_map), reinterpret_cast<uint32_t*>(ws + lay.touched),
+                       reinterpret_cast<uint64_t*>(ws + lay.runs), static_cast<uint8_t*>(out_values)};
+  auto* fstatus = reinterpret_cast<PcoB200AsyncFilesStatus*>(ws + lay.fstatus);
+  auto* ts = reinterpret_cast<TkState*>(ws + lay.tstate);
+  auto* cold_list = reinterpret_cast<uint32_t*>(ws + lay.cold_list);
+  auto* table = reinterpret_cast<const IndexChunk*>(ws + lay.table);
+  auto* afstate = reinterpret_cast<const AfState*>(ws + lay.state);
+
+  ln.begin("ff_map_kernel");
+  ff_map_kernel<<<uint32_t(ctas_of<FF_THREADS>(mc)), FF_THREADS, 0, stream>>>(mc, reinterpret_cast<uint32_t*>(ws + lay.slot_map), cold_list);
+  ln.end();
+  // file_ns: tk_finish_files_kernel writes it, only when the take succeeds
+  enqueue_files(ln, g, lay, ws, ws + lay.stage, &filt, cold_list, nullptr, fstatus, false, true, [&] {
+    auto front = [&] {
+      ln.begin("tk_front_files_kernel");
+      tk_front_files_kernel<<<1, 32, 0, stream>>>(afstate, reinterpret_cast<const AsyncCheck*>(ws), n_positions, ts);
+      ln.end();
+    };
+    enqueue_take_plan(ln, front, positions, plan->max_positions, table, mc, ts, filt.counts, take_runs(filt));
+  });
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    ln.begin("tk_cold_files_kernel");
+    tk_cold_files_kernel<L><<<std::min(mc, uint32_t(FF_COLD_CTAS)), TK_THREADS, 0, stream>>>(cold_list, table, reinterpret_cast<const uint32_t*>(ws + lay.st),
+                                                                                             filt, reinterpret_cast<const L*>(ws + lay.stage));
+    ln.end();
+    return 0;
+  });
+  ln.begin("tk_finish_files_kernel");
+  tk_finish_files_kernel<<<1, TK_SCAN_THREADS, 0, stream>>>(fstatus, ts, afstate, reinterpret_cast<const FileCheck*>(ws + lay.fchk), plan->max_positions,
+                                                            file_ns, status);
+  ln.end();
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
+}
+
+PcoB200Error pco_b200_take_files_async_result(const PcoB200AsyncFilesTakeStatus* s, size_t* n_written) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200Error kind = async_result_kind(s->kind);
+  if (kind == PCO_B200_OK) {
+    if (n_written) *n_written = size_t(s->n_positions);
+    return PCO_B200_OK;
+  }
+  if (s->device_status == PCO_B200_TAKE_TOO_MANY || tk_refusal(s->device_status))
+    return tk_result(kind, s->device_status, s->n_positions, s->position, s->n_written);
+  const PcoB200AsyncFilesFilterStatus f{s->kind, s->device_status, s->file, s->chunk, s->n_written, s->n_files, 0, 0};
+  return pco_b200_filter_files_async_result(&f, nullptr);  // the files filter's words: rows_cap in the role of dst_cap
 }
 
 // ---- asynchronous compress (pco_b200_compress_async; gate kernels in async_compress.cuh).  The plan fixes the layout and the config;

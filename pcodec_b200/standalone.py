@@ -906,6 +906,85 @@ class AsyncFilesAggregate(_lib._AsyncCall):
         return int(nm.value)
 
 
+class _CAsyncFilesTakePlan(C.Structure):  # PcoB200AsyncFilesTakePlan (include/pco_b200.h)
+    _fields_ = [("dtype", C.c_uint32), ("uniform_type", C.c_uint32), ("format_major", C.c_uint32), ("reserved", C.c_uint32),
+                ("src_cap", C.c_uint64), ("index_cap", C.c_uint64), ("max_files", C.c_uint64), ("max_chunks", C.c_uint64),
+                ("rows_cap", C.c_uint64), ("max_positions", C.c_uint64), ("workspace_bytes", C.c_uint64)]
+
+
+class _CAsyncFilesTakeStatus(C.Structure):  # PcoB200AsyncFilesTakeStatus (include/pco_b200.h)
+    _fields_ = [("kind", C.c_uint32), ("device_status", C.c_uint32), ("file", C.c_uint64), ("chunk", C.c_uint64), ("n_written", C.c_uint64),
+                ("n_files", C.c_uint64), ("n_positions", C.c_uint64), ("position", C.c_uint64), ("records_decoded", C.c_uint64)]
+
+
+def _lib_async_take_files():
+    return _lib.bind("_async_take_files_ready",
+                     pco_b200_take_files_async_plan=[C.c_void_p, C.c_size_t, C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                                     C.c_size_t, C.c_size_t, C.c_void_p],
+                     pco_b200_take_files_async=[C.c_void_p] * 12,
+                     pco_b200_take_files_async_result=[C.c_void_p, C.POINTER(C.c_size_t)])
+
+
+class AsyncFilesTake(_lib._AsyncCall):
+    """Takes the numbers at strictly ascending positions of a batch of indexed standalone files' concatenation on the current CUDA stream
+    (pco_b200_take_files_async), decoding only the chunks the positions touch: each decoded batch writes its selected numbers straight to
+    their final index.  Refs, their count, the positions and their count are read from device tensors, so one captured call serves new
+    files and new positions on each replay, and AsyncFilesFilter's positions and count can be passed straight in.
+
+    The plan and capacities are AsyncFilesDecompressor's, with rows_cap (the most numbers of a call's files) in place of dst_cap, and
+    max_positions the most positions a call takes.  The call owns a device workspace (about rows_cap * (itemsize + 0.07) bytes beyond the
+    decompressor's) and a status; it serves one call in flight."""
+
+    _Plan, _Status = _CAsyncFilesTakePlan, _CAsyncFilesTakeStatus
+
+    def __init__(self, head, dtype, src_cap, index_cap, max_files, max_chunks, rows_cap, max_positions, device=None):
+        self.dtype = np.dtype(dtype)
+        h = self._head(head)
+        self._make_plan(device, lambda plan: _lib_async_take_files().pco_b200_take_files_async_plan(
+            h.ctypes.data_as(C.c_void_p), C.c_size_t(h.size), C.c_ubyte(_lib.dtype_byte(self.dtype)), C.c_size_t(src_cap), C.c_size_t(index_cap),
+            C.c_size_t(max_files), C.c_size_t(max_chunks), C.c_size_t(rows_cap), C.c_size_t(max_positions), plan))
+        self._alloc()
+
+    def __call__(self, src, index, files, n_files, positions, n_positions, values, file_ns=None):
+        """Enqueues the take of positions[: n_positions[0]] from files[: n_files[0]] on torch.cuda.current_stream().  `src`, `index`,
+        `files` and `n_files` are as AsyncFilesDecompressor takes them; `positions` is an int64 CUDA tensor of at least max_positions
+        elements (strictly ascending indices into the files' concatenation), `n_positions` a 1-element int64 CUDA tensor, `values` a CUDA
+        tensor of the plan's dtype of at least max_positions elements that receives the numbers, and `file_ns` (optional) an int64 CUDA
+        tensor of at least max_files elements that receives each file's count.  Returns nothing and does not wait; result() reports the
+        outcome."""
+        import torch
+
+        from .wrapped import _check_take_tensors
+
+        p = self._plan
+        self._check_tensors(src=src, index=index, files=files, n_files=n_files, positions=positions, n_positions=n_positions, values=values,
+                            **({} if file_ns is None else {"file_ns": file_ns}))
+        if src.numel() * src.element_size() < p.src_cap or index.numel() * index.element_size() < p.index_cap:
+            raise ValueError(f"src holds fewer than src_cap = {p.src_cap} bytes, or index fewer than index_cap = {p.index_cap}")
+        if files.dtype != torch.int64 or files.dim() != 2 or files.shape[1] != 4 or files.shape[0] < p.max_files:
+            raise ValueError(f"files must be an int64 tensor of shape ({p.max_files}, 4)")
+        if n_files.dtype != torch.int64 or n_files.numel() != 1:
+            raise ValueError("n_files must be a 1-element int64 tensor")
+        _check_take_tensors(positions, n_positions, values, self.dtype, p.max_positions)
+        if file_ns is not None and (file_ns.dtype != torch.int64 or file_ns.numel() < p.max_files):
+            raise ValueError(f"file_ns must be an int64 tensor of at least max_files = {p.max_files} elements")
+        rc = _lib_async_take_files().pco_b200_take_files_async(
+            C.byref(p), C.c_void_p(src.data_ptr()), C.c_void_p(index.data_ptr()), C.c_void_p(files.data_ptr()), C.c_void_p(n_files.data_ptr()),
+            C.c_void_p(positions.data_ptr()), C.c_void_p(n_positions.data_ptr()), C.c_void_p(values.data_ptr()),
+            C.c_void_p(None if file_ns is None else file_ns.data_ptr()), C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()),
+            self._stream())
+        _lib.check(rc)
+
+    def result(self):
+        """Copies the status of the last call back (waiting for it on the current stream) and returns the number of values written, or
+        raises PcoError with the kind pco_b200_decompress_files gives ("file 3: chunk 2: ...") or, for the positions, InvalidArgument
+        ("position 17: ...")."""
+        s = self.status_record()
+        nw = C.c_size_t()
+        _lib.check(_lib_async_take_files().pco_b200_take_files_async_result(C.byref(s), C.byref(nw)))
+        return int(nw.value)
+
+
 class _CAsyncCompressFilesPlan(C.Structure):  # PcoB200AsyncCompressFilesPlan (include/pco_b200.h)
     _fields_ = [("dtype", C.c_uint32), ("uniform_type_header", C.c_uint32), ("mode", C.c_uint32), ("order", C.c_uint32),
                 ("n_vars", C.c_uint32), ("level", C.c_uint32), ("mode_k", C.c_uint32), ("reserved", C.c_uint32),

@@ -556,6 +556,87 @@ class AsyncPagesAggregate(_lib._AsyncCall):
         return int(nm.value)
 
 
+class _CAsyncTakePlan(C.Structure):  # PcoB200AsyncTakePlan (include/pco_b200.h)
+    _fields_ = [("dtype", C.c_uint32), ("reserved", C.c_uint32), ("metas_cap", C.c_uint64), ("pages_cap", C.c_uint64), ("max_pages", C.c_uint64),
+                ("rows_cap", C.c_uint64), ("frame_cap", C.c_uint64), ("max_positions", C.c_uint64), ("workspace_bytes", C.c_uint64)]
+
+
+class _CAsyncTakeStatus(C.Structure):  # PcoB200AsyncTakeStatus (include/pco_b200.h)
+    _fields_ = [("kind", C.c_uint32), ("device_status", C.c_uint32), ("page", C.c_uint64), ("n_written", C.c_uint64), ("n_pages", C.c_uint64),
+                ("frames_needed", C.c_uint64), ("n_positions", C.c_uint64), ("position", C.c_uint64), ("records_decoded", C.c_uint64)]
+
+
+def _lib_async_take():
+    return _lib.bind("_async_take_ready",
+                     pco_b200_take_pages_async_plan=[C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p],
+                     pco_b200_take_pages_async=[C.c_void_p] * 11,
+                     pco_b200_take_pages_async_result=[C.c_void_p, C.POINTER(C.c_size_t)])
+
+
+def _check_take_tensors(positions, n_positions, values, dtype, max_positions):
+    import torch
+
+    if positions.dtype != torch.int64 or positions.numel() < max_positions:
+        raise ValueError(f"positions must be an int64 tensor of at least max_positions = {max_positions} elements")
+    if n_positions.dtype != torch.int64 or n_positions.numel() != 1:
+        raise ValueError("n_positions must be a 1-element int64 tensor")
+    if values.dtype != _torch_dtypes()[dtype] or values.numel() < max_positions:
+        raise ValueError(f"values must hold at least max_positions = {max_positions} numbers of {dtype}")
+
+
+class AsyncPagesTake(_lib._AsyncCall):
+    """Takes the numbers at strictly ascending positions of a batch of wrapped-format pages' concatenation on the current CUDA stream
+    (pco_b200_take_pages_async), decoding only the pages the positions touch: each decoded batch writes its selected numbers straight to
+    their final index.  Refs, their count, the positions and their count are read from device tensors, so one captured call serves new
+    pages and new positions on each replay, and AsyncPagesFilter's positions and count can be passed straight in.
+
+    The capacities are AsyncPagesDecompressor's, with rows_cap (the most numbers of a call's pages) in place of dst_cap, and max_positions
+    the most positions a call takes; frame_cap defaults to metas_cap + pages_cap + 20 * max_pages as there.  The call owns a device
+    workspace (about rows_cap * (itemsize + 0.07) bytes beyond the decompressor's) and a status; it serves one call in flight."""
+
+    _Plan, _Status = _CAsyncTakePlan, _CAsyncTakeStatus
+
+    def __init__(self, dtype, metas_cap, pages_cap, max_pages, rows_cap, max_positions, frame_cap=None, device=None):
+        self.dtype = np.dtype(dtype)
+        if frame_cap is None:
+            frame_cap = metas_cap + pages_cap + 20 * max_pages
+        self._make_plan(device, lambda plan: _lib_async_take().pco_b200_take_pages_async_plan(
+            C.c_ubyte(_lib.dtype_byte(self.dtype)), C.c_size_t(metas_cap), C.c_size_t(pages_cap), C.c_size_t(max_pages), C.c_size_t(rows_cap),
+            C.c_size_t(frame_cap), C.c_size_t(max_positions), plan))
+        self._alloc()
+
+    def __call__(self, metas, pages, refs, n_pages, positions, n_positions, values):
+        """Enqueues the take of positions[: n_positions[0]] from the pages refs[: n_pages[0]] names on torch.cuda.current_stream().
+        `metas`, `pages`, `refs` and `n_pages` are as AsyncPagesDecompressor takes them; `positions` is an int64 CUDA tensor of at least
+        max_positions elements (strictly ascending indices into the pages' concatenation), `n_positions` a 1-element int64 CUDA tensor, and
+        `values` a CUDA tensor of the plan's dtype of at least max_positions elements that receives the numbers.  Returns nothing and does
+        not wait; result() reports the outcome."""
+        import torch
+
+        p = self._plan
+        self._check_tensors(metas=metas, pages=pages, refs=refs, n_pages=n_pages, positions=positions, n_positions=n_positions, values=values)
+        if metas.numel() * metas.element_size() < p.metas_cap or pages.numel() * pages.element_size() < p.pages_cap:
+            raise ValueError(f"metas holds fewer than metas_cap = {p.metas_cap} bytes, or pages fewer than pages_cap = {p.pages_cap}")
+        if refs.dtype != torch.int64 or refs.dim() != 2 or refs.shape[1] != 5 or refs.shape[0] < p.max_pages:
+            raise ValueError(f"refs must be an int64 tensor of shape ({p.max_pages}, 5)")
+        if n_pages.dtype != torch.int64 or n_pages.numel() != 1:
+            raise ValueError("n_pages must be a 1-element int64 tensor")
+        _check_take_tensors(positions, n_positions, values, self.dtype, p.max_positions)
+        rc = _lib_async_take().pco_b200_take_pages_async(
+            C.byref(p), C.c_void_p(metas.data_ptr()), C.c_void_p(pages.data_ptr()), C.c_void_p(refs.data_ptr()), C.c_void_p(n_pages.data_ptr()),
+            C.c_void_p(positions.data_ptr()), C.c_void_p(n_positions.data_ptr()), C.c_void_p(values.data_ptr()),
+            C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()), self._stream())
+        _lib.check(rc)
+
+    def result(self):
+        """Copies the status of the last call back (waiting for it on the current stream) and returns the number of values written, or
+        raises PcoError with the kind decompress_pages gives ("page 17: ...") or, for the positions, InvalidArgument ("position 17: ...")."""
+        s = self.status_record()
+        nw = C.c_size_t()
+        _lib.check(_lib_async_take().pco_b200_take_pages_async_result(C.byref(s), C.byref(nw)))
+        return int(nw.value)
+
+
 class AsyncPagesFilter(_lib._AsyncCall):
     """Decodes a batch of wrapped-format pages on the current CUDA stream and writes only the numbers inside a closed interval, in row order,
     with their positions in the pages' concatenation (pco_b200_filter_pages_async): the predicate runs inside the decoder, so the decoded
