@@ -1295,6 +1295,83 @@ PcoB200Error pco_b200_compress_wrapped_async(const PcoB200AsyncCompressWrappedPl
 PcoB200Error pco_b200_compress_wrapped_async_result(const PcoB200AsyncCompressWrappedStatus *host_status, size_t *metas_len, size_t *pages_len,
                                                     size_t *n_chunks);
 
+/* ---- asynchronous transcode of wrapped-format pages into one indexed standalone file (no reference counterpart).  Every pages call
+ * first walks each page serially to find its batch boundaries; a files call reads them from the side index instead.  A reader that keeps
+ * pco pages in HBM and scans them more than once (a page cache of column chunks, a row group filtered on one column and taken on another)
+ * pays that walk once with this call: page i becomes chunk i of a standalone file, its bytes pco's own and not re-encoded (so f16
+ * FloatMult pages and metas shared by several pages carry over), and the file's side index is written beside it.  Every files call
+ * (pco_b200_decompress_files_async, pco_b200_filter_files_async, pco_b200_aggregate_files_async, pco_b200_take_files_async, and
+ * pco_b200_decompress_async / pco_b200_decompress_ranges_async) then serves the pages with no walk, with the same row positions.  The call
+ * has the contract of the other asynchronous calls: it only enqueues kernels, it can be captured in a CUDA graph, refs and their count are
+ * read on the device, and a plan fixes the grids. */
+typedef struct PcoB200AsyncPagesToFilePlan {  /* filled by pco_b200_pages_to_file_async_plan; treat as opaque, but for uniform_type */
+  uint32_t dtype;
+  uint32_t uniform_type;                      /* the file header's uniform type byte: 0, or dtype (uniform_type_header) */
+  uint64_t metas_cap, pages_cap, max_pages, frame_cap, dst_cap, index_cap;
+  uint64_t workspace_bytes;                   /* device workspace one in-flight call needs */
+} PcoB200AsyncPagesToFilePlan;
+
+typedef struct PcoB200AsyncPagesToFileStatus {  /* written on the device by every call */
+  uint32_t kind;                                /* PcoB200Error */
+  uint32_t device_status;                       /* the device word behind it: a page's PcoB200Error kind, or PCO_B200_ASYNC_* */
+  uint64_t page;                                /* the page the outcome names (UINT64_MAX if none) */
+  uint64_t n_pages;                             /* *n_pages as the call read it */
+  uint64_t n_total;                             /* the sum of page_n, once every ref passed its checks (0 before) */
+  uint64_t file_len;                            /* bytes written to dst (0 unless OK) */
+  uint64_t index_len;                           /* bytes written to index (0 unless OK) */
+  uint64_t frames_needed;                       /* bytes of framed pages the batch needs, as PcoB200AsyncPagesStatus */
+  uint64_t file_needed;                         /* bytes the file needs, also when above dst_cap (0 until every page passed) */
+  uint64_t index_needed;                        /* bytes the index needs, also when above index_cap (0 until every page passed) */
+} PcoB200AsyncPagesToFileStatus;
+
+/* Makes a plan for batches of up to max_pages pages of dtype, whose refs point into metas_cap bytes of metas and pages_cap bytes of pages,
+ * written as a file of up to dst_cap bytes with the header flavour uniform_type_header selects (as pco_b200_compress_ex) and a side index
+ * of up to index_cap bytes.  frame_cap bounds the pages framed in the workspace, as in pco_b200_decompress_pages_async_plan.  Checked before
+ * the device is touched: dtype (PCO_B200_INVALID_TYPE), max_pages in 1 .. 2^31 - 1, and frame_cap, dst_cap and index_cap at most 2^56
+ * (PCO_B200_INVALID_ARGUMENT).  Then *plan is filled and the one-time device set-up runs on the current device, which the calls must use;
+ * without a device that is PCO_B200_CUDA.  plan->uniform_type is the output's header flavour, so a files plan for the output can be made
+ * before any call runs (the flavour is all of the header those plans read).
+ * workspace_bytes is the sum of these regions, each rounded up to 256 bytes, with m = max_pages and E = 24 floor(index_cap / 12): 1880
+ * (the binomial table), 136 (state), 48 m (page table), 32 (m + 1) + E + 32 m (walked records and batch entries), ceil(frame_cap / 16) * 16
+ * + 64 (frames and a pad frame), 4 m, 4 m and 8 m (meta statuses, walk statuses, walk ends), 56 ceil(m / 256) (CTA sums), 32 m (decode
+ * table), 4 m (its pages), 4 m (cold list), 32 (transcode state), 4 m and 8 m (wide walk statuses and ends), 8 m and 8 m (chunk and
+ * entries offsets).  E is room for the batch entries of every batch whose index fits index_cap, at two latent vars per page. */
+PcoB200Error pco_b200_pages_to_file_async_plan(unsigned char dtype, int uniform_type_header, size_t metas_cap, size_t pages_cap, size_t max_pages,
+                                               size_t frame_cap, size_t dst_cap, size_t index_cap, PcoB200AsyncPagesToFilePlan *plan);
+/* Enqueues the transcode of the pages refs[0 : *n_pages) names on `cuda_stream`, and the outcome into *status; returns without waiting.
+ * metas (metas_cap bytes), pages (pages_cap bytes; may be the same buffer as metas), refs (PcoB200PageRef[max_pages]), n_pages (one
+ * uint64_t), dst (dst_cap bytes), index (index_cap bytes, 16-byte aligned), file_ref (one PcoB200FileRef), workspace
+ * (plan->workspace_bytes, 256-byte aligned) and status are device pointers; one workspace serves one call in flight.  Pages may repeat,
+ * come in any order and share a meta, as in pco_b200_decompress_pages_async.
+ * On success dst[0 : file_len) is, byte for byte, what pco_b200_compress_ex writes when its chunks are these pages: the standalone header
+ * of the plan's flavour with n_hint the sum of page_n, for each ref in refs order the chunk's preamble [dtype][page_n - 1], its meta and
+ * the page's bytes up to where its walk ends (not up to page_len), then the terminator.  index[0 : index_len) is the side index
+ * pco_b200_build_index_async builds for that file (and pco_b200_compress_ex writes), with exactly *n_pages chunk records.  *file_ref is
+ * {0, file_len, 0, index_len}, so a files call captured behind this call can read the output with no readback; on any failure it is
+ * zeroed, so such a call refuses the file instead of reading stale bytes.  An empty batch gives header + terminator and an index of 0
+ * chunks.
+ * Refusals, in this order, with the kinds of pco_b200_decompress_pages_async and naming the same page:
+ *   - that call's refusals before the device touches a page (PCO_B200_ASYNC_TOO_MANY_PAGES, _META_OUTSIDE, _PAGE_OUTSIDE, _PAGE_N,
+ *     _FRAMES; there is no number destination, so PCO_B200_ASYNC_PAGES_DST does not arise);
+ *   - the lowest page that fails its meta length (INVALID_ARGUMENT), its meta layout (CORRUPTION) or its walk (the kind its walk gives);
+ *   - the lowest page that neither the 2^10- nor the 2^12-state walker takes - Dict, Lookback and Conv1 pages, tables above 2^12 states -
+ *     as PCO_B200_UNSUPPORTED: a side index holds no entries for them;
+ *   - a file above dst_cap (PCO_B200_ASYNC_FILES_DST_FULL), then an index above index_cap (PCO_B200_ASYNC_FILES_INDEX_FULL), both
+ *     PCO_B200_IO with file_needed and index_needed reported.  When the pages' batch entries do not even fit the walks' room (an index of
+ *     more than about twice index_cap), the walk stops early and index_needed is 0.
+ * The call validates what the walk validates and no more: a page that walks but fails to decode is written out, and fails later in the
+ * files call, which names chunk i for page i.  A refused call writes nothing to dst or index.  The return value covers the host side only:
+ * null pointers, an unaligned workspace or index or a plan that was not filled (PCO_B200_INVALID_ARGUMENT), a launch the runtime refuses
+ * (PCO_B200_CUDA).  With pco_b200_profile_enable(1), a call outside a stream capture records its kernel spans for pco_b200_profile_last;
+ * a call inside a capture records none. */
+PcoB200Error pco_b200_pages_to_file_async(const PcoB200AsyncPagesToFilePlan *plan, const void *metas, const void *pages, const PcoB200PageRef *refs,
+                                          const uint64_t *n_pages, void *dst, void *index, PcoB200FileRef *file_ref, void *workspace,
+                                          PcoB200AsyncPagesToFileStatus *status, void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory at a point of the caller's choosing.  Returns the kind,
+ * sets the last-error message as pco_b200_decompress_pages words it ("page 17: ...") and, when the kind is OK, sets *file_len and
+ * *index_len (either may be NULL) to the bytes written. */
+PcoB200Error pco_b200_pages_to_file_async_result(const PcoB200AsyncPagesToFileStatus *host_status, size_t *file_len, size_t *index_len);
+
 #if defined(__cplusplus)
 }
 #endif

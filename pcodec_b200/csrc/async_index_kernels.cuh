@@ -65,6 +65,33 @@ struct AiArgs {
   uint32_t dtype, uniform_type, format_major;
 };
 
+// Chunk c's record `r` (chunk_offset as the index states it) and its walked entries at `from` (n_vars x batches of them, then anything)
+// into the index: the entries at byte `at`, zeros up to the next 16-byte boundary, and the record with entries_offset = at.  Every
+// thread of a CTA of AI_THREADS calls it.
+__device__ __forceinline__ void index_copy_chunk(IndexChunk r, const uint32_t* from, uint8_t* index, uint64_t at, uint64_t c) {
+  uint32_t* to = reinterpret_cast<uint32_t*>(index + at);
+  const uint64_t words = uint64_t(r.n_vars) * n_batches_of(r.n) * (sizeof(BatchEntry) / 4), room = entries_bytes(r.n_vars, r.n) / 4;
+  for (uint64_t w = threadIdx.x; w < room; w += AI_THREADS) to[w] = w < words ? from[w] : 0u;
+  if (threadIdx.x == 0) {
+    r.entries_offset = at;
+    reinterpret_cast<IndexChunk*>(index + sizeof(IndexHeader))[c] = r;
+  }
+}
+
+// The header of a side index of n_chunks records right behind it, for a file of file_len bytes whose terminator ends at end_byte.
+__device__ __forceinline__ void write_index_header(uint8_t* index, uint64_t n_chunks, uint64_t n_total, uint64_t file_len, uint64_t end_byte) {
+  IndexHeader h;
+  memset(&h, 0, sizeof(h));
+  h.magic = INDEX_MAGIC;
+  h.version = 1;
+  h.n_chunks = n_chunks;
+  h.n_total = n_total;
+  h.file_len = file_len;
+  h.chunks_offset = sizeof(IndexHeader);
+  h.end_byte = end_byte;
+  *reinterpret_cast<IndexHeader*>(index) = h;
+}
+
 // Workspace of one in-flight call, byte offsets, each region 256-byte aligned: AiState | find CTA counts (8 bytes per AI_FIND_SPAN bytes
 // of src_cap) | per candidate (max_chunks + AI_SPARE_CANDS): position, record, status, end | per chunk (max_chunks + 1, the one that
 // tells a file of too many chunks): record, final entries offset | the round arena, the candidates' entries (2 x index_cap: a
@@ -306,14 +333,7 @@ __global__ void __launch_bounds__(AI_THREADS) ai_copy_kernel(AiArgs g, const AiS
   const AiLayout l = ai_layout(g.src_cap, g.index_cap, g.max_chunks);
   IndexChunk r = reinterpret_cast<const IndexChunk*>(g.ws + l.recs)[c];
   const uint64_t at = reinterpret_cast<const uint64_t*>(g.ws + l.offs)[c];
-  const uint32_t* from = reinterpret_cast<const uint32_t*>(g.ws + r.entries_offset);
-  uint32_t* to = reinterpret_cast<uint32_t*>(g.index + at);
-  const uint64_t words = uint64_t(r.n_vars) * n_batches_of(r.n) * (sizeof(BatchEntry) / 4), room = entries_bytes(r.n_vars, r.n) / 4;
-  for (uint64_t w = threadIdx.x; w < room; w += AI_THREADS) to[w] = w < words ? from[w] : 0u;
-  if (threadIdx.x == 0) {
-    r.entries_offset = at;
-    reinterpret_cast<IndexChunk*>(g.index + sizeof(IndexHeader))[c] = r;
-  }
+  index_copy_chunk(r, reinterpret_cast<const uint32_t*>(g.ws + r.entries_offset), g.index, at, c);
 }
 
 // One thread: the index header (on success) and the status.
@@ -327,18 +347,7 @@ __global__ void ai_finish_kernel(AiArgs g, const AiState* __restrict__ state, Pc
   r.n_total = s.n_total;
   r.index_bytes = s.status == ST_OK ? s.index_bytes : 0;
   r.serial_chunks = s.serial_chunks;
-  if (s.status == ST_OK) {
-    IndexHeader h;
-    memset(&h, 0, sizeof(h));
-    h.magic = INDEX_MAGIC;
-    h.version = 1;
-    h.n_chunks = s.n_chunks;
-    h.n_total = s.n_total;
-    h.file_len = s.src_len;
-    h.chunks_offset = sizeof(IndexHeader);
-    h.end_byte = s.end_byte;
-    *reinterpret_cast<IndexHeader*>(g.index) = h;
-  }
+  if (s.status == ST_OK) write_index_header(g.index, s.n_chunks, s.n_total, s.src_len, s.end_byte);
   *out = r;
 }
 

@@ -15,6 +15,7 @@
 #include "async_index_kernels.cuh"
 #include "async_kernels.cuh"
 #include "async_pages_kernels.cuh"
+#include "async_pages_to_file_kernels.cuh"
 #include "async_ranges_kernels.cuh"
 #include "async_take_kernels.cuh"
 #include "compress_host.cuh"
@@ -3040,14 +3041,10 @@ PcoB200Error pco_b200_decompress_pages_async_plan(unsigned char dtype, size_t me
                                     (const void*)ap_finish_kernel});
 }
 
-// The launches of pco_b200_decompress_pages_async over the workspace `ws` laid out by `lay`: the front end, the decode stage, the
-// catch-all decoder into dst and ap_finish_kernel into *status.  With `filt` the decode stage runs its filter-mode instantiations and dst
-// is their value staging (pco_b200_filter_pages_async).  With `agg` too, the aggregate-mode instantiations, which store nothing to dst;
-// dst is the catch-all decoder's value staging only (pco_b200_aggregate_pages_async).  With `take` instead of `agg`, the take-mode
-// instantiations, likewise (pco_b200_take_pages_async).  `between`, when given, enqueues its launches behind the front end
-// (ap_rewalk_kernel) and before the decode stage.
-static void enqueue_pages(const AsyncLaunch& ln, const ApArgs& g, const ApLayout& lay, uint8_t* ws, void* dst, const FiltStage* filt,
-                          PcoB200AsyncPagesStatus* status, bool agg = false, bool take = false, const std::function<void()>& between = {}) {
+// The pages front end of pco_b200_decompress_pages_async over the workspace `ws` laid out by `lay`: every page checked, placed, framed
+// and walked, and routed, up to the re-walk of the lowest failing page (ap_pages ... ap_rewalk).  enqueue_pages runs it in front of the
+// decode stage, pco_b200_pages_to_file_async in front of its writers.
+static void enqueue_pages_front(const AsyncLaunch& ln, const ApArgs& g, const ApLayout& lay, uint8_t* ws) {
   const cudaStream_t stream = ln.stream;
   AsyncCheck* chk = reinterpret_cast<AsyncCheck*>(ws);
   ApState* state = reinterpret_cast<ApState*>(ws + lay.state);
@@ -3062,7 +3059,6 @@ static void enqueue_pages(const AsyncLaunch& ln, const ApArgs& g, const ApLayout
   IndexChunk* table = reinterpret_cast<IndexChunk*>(ws + lay.table);
   uint32_t* fast_page = reinterpret_cast<uint32_t*>(ws + lay.fast_page);
   uint32_t* cold_list = reinterpret_cast<uint32_t*>(ws + lay.cold_list);
-  uint32_t* d_st = reinterpret_cast<uint32_t*>(ws + lay.st);
   // the frames as one file: every page's frame below frame_cap, the pad frame behind them
   const FileParams fp{d_frames, lay.pad_frame + 64, g.dtype, 0, 4};
   const uint32_t mp = g.max_pages, pb = uint32_t(ctas_of<AP_THREADS>(mp));
@@ -3089,6 +3085,31 @@ static void enqueue_pages(const AsyncLaunch& ln, const ApArgs& g, const ApLayout
   ln.begin("ap_rewalk_kernel");
   ap_rewalk_kernel<<<1, WALK_THREADS, sizeof(WalkSmem<SMALL_MAX_SIZE_LOG>), stream>>>(g, state, tab, d_frames, d_idx, lay.index_len);
   ln.end();
+}
+
+// The launches of pco_b200_decompress_pages_async over the workspace `ws` laid out by `lay`: the front end, the decode stage, the
+// catch-all decoder into dst and ap_finish_kernel into *status.  With `filt` the decode stage runs its filter-mode instantiations and dst
+// is their value staging (pco_b200_filter_pages_async).  With `agg` too, the aggregate-mode instantiations, which store nothing to dst;
+// dst is the catch-all decoder's value staging only (pco_b200_aggregate_pages_async).  With `take` instead of `agg`, the take-mode
+// instantiations, likewise (pco_b200_take_pages_async).  `between`, when given, enqueues its launches behind the front end
+// (ap_rewalk_kernel) and before the decode stage.
+static void enqueue_pages(const AsyncLaunch& ln, const ApArgs& g, const ApLayout& lay, uint8_t* ws, void* dst, const FiltStage* filt,
+                          PcoB200AsyncPagesStatus* status, bool agg = false, bool take = false, const std::function<void()>& between = {}) {
+  const cudaStream_t stream = ln.stream;
+  AsyncCheck* chk = reinterpret_cast<AsyncCheck*>(ws);
+  ApState* state = reinterpret_cast<ApState*>(ws + lay.state);
+  WrappedPage* tab = reinterpret_cast<WrappedPage*>(ws + lay.tab);
+  uint8_t* d_idx = ws + lay.index;
+  IndexChunk* recs = reinterpret_cast<IndexChunk*>(d_idx);
+  uint8_t* d_frames = ws + lay.frames;
+  IndexChunk* table = reinterpret_cast<IndexChunk*>(ws + lay.table);
+  uint32_t* fast_page = reinterpret_cast<uint32_t*>(ws + lay.fast_page);
+  uint32_t* cold_list = reinterpret_cast<uint32_t*>(ws + lay.cold_list);
+  uint32_t* d_st = reinterpret_cast<uint32_t*>(ws + lay.st);
+  const FileParams fp{d_frames, lay.pad_frame + 64, g.dtype, 0, 4};
+  const uint32_t mp = g.max_pages;
+
+  enqueue_pages_front(ln, g, lay, ws);
   if (between) between();
   const DecodeStage d{fp, table, d_idx, lay.index_len, mp, d_st, ws + lay.cls, ws + lay.syms, reinterpret_cast<uint32_t*>(ws + lay.offs),
                       &chk->binoms, agg || take ? nullptr : dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{}};
@@ -4156,6 +4177,108 @@ PcoB200Error pco_b200_build_index_async_result(const PcoB200AsyncIndexStatus* s,
     default:
       status_to_error(s->device_status, "this chunk");
       return fail(kind, "chunk " + std::to_string(s->chunk) + ": " + last_error_ref());
+  }
+}
+
+// ---- asynchronous transcode of wrapped pages into an indexed standalone file (pco_b200_pages_to_file_async; kernels in
+// async_pages_to_file_kernels.cuh).  A call is a fixed sequence of launches: the pages front end (enqueue_pages_front), the wide walk, the
+// gate, the file writer, the index writer, the finish.
+
+static bool pf_plan_ok(const PcoB200AsyncPagesToFilePlan* p) {
+  constexpr uint64_t cap = uint64_t(1) << 56;
+  return nt_valid(p->dtype) && (p->uniform_type == 0 || p->uniform_type == p->dtype) && p->max_pages >= 1 && p->max_pages <= 0x7fffffffull &&
+         p->frame_cap <= cap && p->dst_cap <= cap && p->index_cap <= cap && p->workspace_bytes == pf_layout(p->max_pages, p->frame_cap, p->index_cap).total;
+}
+
+PcoB200Error pco_b200_pages_to_file_async_plan(unsigned char dtype, int uniform_type_header, size_t metas_cap, size_t pages_cap, size_t max_pages,
+                                               size_t frame_cap, size_t dst_cap, size_t index_cap, PcoB200AsyncPagesToFilePlan* plan) {
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (!plan) return fail(PCO_B200_INVALID_ARGUMENT, "null plan");
+  if (max_pages == 0 || uint64_t(max_pages) > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_pages must be 1 .. 2^31 - 1");
+  if (uint64_t(frame_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "frame_cap above 2^56 bytes");
+  if (uint64_t(dst_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "dst_cap above 2^56 bytes");
+  if (uint64_t(index_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "index_cap above 2^56 bytes");
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->uniform_type = uniform_type_header ? dtype : 0;
+  plan->metas_cap = metas_cap;
+  plan->pages_cap = pages_cap;
+  plan->max_pages = max_pages;
+  plan->frame_cap = frame_cap;
+  plan->dst_cap = dst_cap;
+  plan->index_cap = index_cap;
+  plan->workspace_bytes = pf_layout(max_pages, frame_cap, index_cap).total;
+  Context& c = ctx();
+  if (PcoB200Error e = ensure_device(c)) return e;
+  PCOB_CUDA_TRY(cudaFuncSetAttribute(pf_walk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WalkSmem<12>)));
+  return load_kernels({(const void*)ap_pages_kernel, (const void*)ap_scan_kernel, (const void*)ap_place_kernel, (const void*)frame_pages_kernel,
+                       (const void*)walk_kernel<SMALL_MAX_SIZE_LOG>, (const void*)ap_route_kernel, (const void*)ap_rewalk_kernel,
+                       (const void*)pf_walk_kernel, (const void*)pf_gate_kernel, (const void*)pf_file_kernel, (const void*)pf_index_kernel,
+                       (const void*)pf_finish_kernel});
+}
+
+PcoB200Error pco_b200_pages_to_file_async(const PcoB200AsyncPagesToFilePlan* plan, const void* metas, const void* pages, const PcoB200PageRef* refs,
+                                          const uint64_t* n_pages, void* dst, void* index, PcoB200FileRef* file_ref, void* workspace,
+                                          PcoB200AsyncPagesToFileStatus* status, void* cuda_stream) {
+  if (!plan || !metas || !pages || !refs || !n_pages || !dst || !index || !file_ref || !workspace || !status)
+    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (!pf_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_pages_to_file_async_plan");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  if (reinterpret_cast<uintptr_t>(index) & 15) return fail(PCO_B200_INVALID_ARGUMENT, "the index is not 16-byte aligned");
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+  const cudaStream_t stream = ln.stream;
+
+  const uint32_t mp = uint32_t(plan->max_pages);
+  const PfLayout lay = pf_layout(mp, plan->frame_cap, plan->index_cap);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  // no numbers are written: a number capacity that no batch of max_pages pages of at most 2^24 numbers reaches
+  const ApArgs ag{static_cast<const uint8_t*>(metas), static_cast<const uint8_t*>(pages), refs, n_pages, plan->metas_cap, plan->pages_cap, NONE64,
+                  plan->frame_cap, plan->dtype, mp};
+  const PfArgs g{ws, static_cast<uint8_t*>(dst), static_cast<uint8_t*>(index), file_ref, plan->max_pages, plan->frame_cap, plan->dst_cap,
+                 plan->index_cap, plan->dtype, plan->uniform_type};
+  enqueue_pages_front(ln, ag, lay.ap, ws);
+  ln.begin("pf_walk_kernel");
+  pf_walk_kernel<<<mp, WALK_THREADS, sizeof(WalkSmem<12>), stream>>>(g);
+  ln.end();
+  ln.begin("pf_gate_kernel");
+  pf_gate_kernel<<<1, AP_SCAN_THREADS, 0, stream>>>(g);
+  ln.end();
+  ln.begin("pf_file_kernel");
+  pf_file_kernel<<<pf_file_ctas(plan->dst_cap), GATHER_THREADS, 0, stream>>>(g);
+  ln.end();
+  ln.begin("pf_index_kernel");
+  pf_index_kernel<<<mp, AI_THREADS, 0, stream>>>(g);
+  ln.end();
+  ln.begin("pf_finish_kernel");
+  pf_finish_kernel<<<1, 1, 0, stream>>>(g, status);
+  ln.end();
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
+}
+
+PcoB200Error pco_b200_pages_to_file_async_result(const PcoB200AsyncPagesToFileStatus* s, size_t* file_len, size_t* index_len) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200Error kind = async_result_kind(s->kind);
+  if (kind == PCO_B200_OK) {
+    if (file_len) *file_len = size_t(s->file_len);
+    if (index_len) *index_len = size_t(s->index_len);
+    return PCO_B200_OK;
+  }
+  switch (s->device_status) {
+    case PCO_B200_ASYNC_FILES_DST_FULL:
+      return fail(kind, "the file needs " + std::to_string(s->file_needed) + " bytes, more than the plan's dst_cap");
+    case PCO_B200_ASYNC_FILES_INDEX_FULL:
+      if (s->index_needed == 0) return fail(kind, "the side index needs more than the walks' room, about twice the plan's index_cap bytes");
+      return fail(kind, "the side index needs " + std::to_string(s->index_needed) + " bytes, more than the plan's index_cap");
+    case ST_UNSUPPORTED:
+      if (s->page != NONE64)
+        return page_fail(kind, size_t(s->page), "neither walker takes this page (Dict, Lookback, Conv1, or tables above 2^12 states), so no side index can hold it");
+      [[fallthrough]];
+    default: {  // the pages call's words
+      const PcoB200AsyncPagesStatus p{s->kind, s->device_status, s->page, 0, s->n_pages, s->frames_needed};
+      return pco_b200_decompress_pages_async_result(&p, nullptr);
+    }
   }
 }
 

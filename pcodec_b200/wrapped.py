@@ -8,7 +8,8 @@ Batched forms for containers that keep chunk metas and pages themselves: `compre
 chunks of one page each, `decompress_pages` decodes any number of pages in one call.  Both take host buffers (bytes / numpy)
 or torch CUDA tensors; with CUDA tensors the work runs on torch.cuda.current_stream() and the outputs are CUDA tensors.
 `AsyncChunksCompressor` and `AsyncPagesDecompressor` are their forms with the sizes or refs in device memory, which do not wait for the
-device and can be captured in a CUDA graph; `AsyncPagesFilter` decodes such pages and keeps only the numbers inside an interval."""
+device and can be captured in a CUDA graph; `AsyncPagesFilter` decodes such pages and keeps only the numbers inside an interval, and
+`AsyncPagesToFile` writes them out as one indexed standalone file that the files calls of `standalone` scan without a walk."""
 import ctypes as C
 
 import numpy as np
@@ -694,3 +695,97 @@ class AsyncPagesFilter(_lib._AsyncCall):
         nm = C.c_size_t()
         _lib.check(_lib_async_filter().pco_b200_filter_pages_async_result(C.byref(s), C.byref(nm)))
         return int(nm.value)
+
+
+class _CAsyncPagesToFilePlan(C.Structure):  # PcoB200AsyncPagesToFilePlan (include/pco_b200.h)
+    _fields_ = [("dtype", C.c_uint32), ("uniform_type", C.c_uint32), ("metas_cap", C.c_uint64), ("pages_cap", C.c_uint64), ("max_pages", C.c_uint64),
+                ("frame_cap", C.c_uint64), ("dst_cap", C.c_uint64), ("index_cap", C.c_uint64), ("workspace_bytes", C.c_uint64)]
+
+
+class _CAsyncPagesToFileStatus(C.Structure):  # PcoB200AsyncPagesToFileStatus (include/pco_b200.h)
+    _fields_ = [("kind", C.c_uint32), ("device_status", C.c_uint32), ("page", C.c_uint64), ("n_pages", C.c_uint64), ("n_total", C.c_uint64),
+                ("file_len", C.c_uint64), ("index_len", C.c_uint64), ("frames_needed", C.c_uint64), ("file_needed", C.c_uint64),
+                ("index_needed", C.c_uint64)]
+
+
+def _lib_async_pages_to_file():
+    return _lib.bind("_async_pages_to_file_ready",
+                     pco_b200_pages_to_file_async_plan=[C.c_ubyte, C.c_int, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                                        C.c_void_p],
+                     pco_b200_pages_to_file_async=[C.c_void_p] * 11,
+                     pco_b200_pages_to_file_async_result=[C.c_void_p, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)])
+
+
+class AsyncPagesToFile(_lib._AsyncCall):
+    """Writes a batch of wrapped-format pages out as one indexed standalone file on the current CUDA stream, without waiting for the device
+    (pco_b200_pages_to_file_async): page i becomes chunk i, its bytes copied and not re-encoded, and the file's side index is written beside
+    it.  Every pages call walks each page serially before it decodes; the files calls of `standalone` read the walk's result from the side
+    index, so a reader that scans the same pages more than once pays the walk once.  Refs and their count are read from device tensors, so
+    one captured call serves different pages on each replay.
+
+    metas_cap, pages_cap, max_pages and frame_cap are AsyncPagesDecompressor's (frame_cap has the same default); dst_cap and index_cap are
+    the bytes of the file and of its index (index_cap: at least 64 + 32 max_pages + 12 per 256 numbers and latent var, rounded up to 16
+    bytes per page).  uniform_type_header picks the header flavour, as simple_compress_into.  The call owns the output tensors `file`,
+    `index` and `file_ref` (an int64 (1, 4) FILE_REF row, zeroed when the call fails), plus a workspace and a status; it serves one call in
+    flight.  files_args() gives the first arguments of standalone.AsyncFilesDecompressor, AsyncFilesFilter, AsyncFilesAggregate and
+    AsyncFilesTake for the output, so their plans need no readback, and file_ref with n_files (a 1-element int64 tensor holding 1) is
+    their `files` and `n_files`."""
+
+    _Plan, _Status = _CAsyncPagesToFilePlan, _CAsyncPagesToFileStatus
+
+    def __init__(self, dtype, metas_cap, pages_cap, max_pages, dst_cap, index_cap, frame_cap=None, uniform_type_header=False, device=None):
+        import torch
+
+        self.dtype = np.dtype(dtype)
+        if frame_cap is None:
+            frame_cap = metas_cap + pages_cap + 20 * max_pages
+        self._make_plan(device, lambda plan: _lib_async_pages_to_file().pco_b200_pages_to_file_async_plan(
+            C.c_ubyte(_lib.dtype_byte(self.dtype)), C.c_int(1 if uniform_type_header else 0), C.c_size_t(metas_cap), C.c_size_t(pages_cap),
+            C.c_size_t(max_pages), C.c_size_t(frame_cap), C.c_size_t(dst_cap), C.c_size_t(index_cap), plan))
+        self._alloc()
+        p = self._plan
+        self.file = torch.empty(max(p.dst_cap, 1), dtype=torch.uint8, device=self.device)
+        self.index = torch.empty(max(p.index_cap, 1), dtype=torch.uint8, device=self.device)
+        self.file_ref = torch.zeros((1, 4), dtype=torch.int64, device=self.device)
+        self.n_files = torch.ones(1, dtype=torch.int64, device=self.device)
+
+    @property
+    def head(self):
+        """A whole empty standalone file of the output's header flavour (header with a size hint of 0, then the terminator): what the files
+        plans read of a header, so it stands for any output of this call."""
+        return bytes([112, 99, 111, 33, 3, self._plan.uniform_type, 0, 4, 1, 0])
+
+    def files_args(self):
+        """The arguments (head, dtype, src_cap, index_cap, max_files, max_chunks) of a standalone files call's plan for this call's output."""
+        p = self._plan
+        return dict(head=self.head, dtype=self.dtype, src_cap=int(p.dst_cap), index_cap=int(p.index_cap), max_files=1, max_chunks=int(p.max_pages))
+
+    def __call__(self, metas, pages, refs, n_pages):
+        """Enqueues the transcode of the pages refs[: n_pages[0]] names on torch.cuda.current_stream() into `file`, `index` and `file_ref`,
+        and returns those three tensors.  `metas`, `pages`, `refs` and `n_pages` are as AsyncPagesDecompressor takes them.  Does not wait;
+        result() reports the outcome."""
+        import torch
+
+        p = self._plan
+        self._check_tensors(metas=metas, pages=pages, refs=refs, n_pages=n_pages)
+        if metas.numel() * metas.element_size() < p.metas_cap or pages.numel() * pages.element_size() < p.pages_cap:
+            raise ValueError(f"metas holds fewer than metas_cap = {p.metas_cap} bytes, or pages fewer than pages_cap = {p.pages_cap}")
+        if refs.dtype != torch.int64 or refs.dim() != 2 or refs.shape[1] != 5 or refs.shape[0] < p.max_pages:
+            raise ValueError(f"refs must be an int64 tensor of shape ({p.max_pages}, 5)")
+        if n_pages.dtype != torch.int64 or n_pages.numel() != 1:
+            raise ValueError("n_pages must be a 1-element int64 tensor")
+        rc = _lib_async_pages_to_file().pco_b200_pages_to_file_async(
+            C.byref(p), C.c_void_p(metas.data_ptr()), C.c_void_p(pages.data_ptr()), C.c_void_p(refs.data_ptr()), C.c_void_p(n_pages.data_ptr()),
+            C.c_void_p(self.file.data_ptr()), C.c_void_p(self.index.data_ptr()), C.c_void_p(self.file_ref.data_ptr()),
+            C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()), self._stream())
+        _lib.check(rc)
+        return self.file, self.index, self.file_ref
+
+    def result(self):
+        """Copies the status of the last call back (waiting for it on the current stream) and returns (file_len, index_len), or raises
+        PcoError with the kind decompress_pages gives ("page 17: ..."), Unsupported for a page no walker takes, or Io when the file or the
+        index does not fit."""
+        s = self.status_record()
+        fl, il = C.c_size_t(), C.c_size_t()
+        _lib.check(_lib_async_pages_to_file().pco_b200_pages_to_file_async_result(C.byref(s), C.byref(fl), C.byref(il)))
+        return int(fl.value), int(il.value)
