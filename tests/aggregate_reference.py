@@ -35,7 +35,7 @@ def matches(x, lo, hi):
 
 def tree(v):
     """Pairwise tree over the last axis (a power of two): (0, 1), (2, 3), ..., then pairs of pairs."""
-    with np.errstate(invalid="ignore"):  # +inf + -inf is NaN, as on the device
+    with np.errstate(invalid="ignore", over="ignore"):  # +inf + -inf is NaN, a finite sum may overflow to +-inf, as on the device
         while v.shape[-1] > 1:
             v = v[..., 0::2] + v[..., 1::2]
     return v[..., 0]
@@ -46,7 +46,7 @@ def strided_sum(sums):
     s = np.asarray(sums, dtype=np.float64)
     s = np.concatenate([s, np.zeros((-len(s)) % 32)]).reshape(-1, 32)
     acc = np.zeros(32)
-    with np.errstate(invalid="ignore"):
+    with np.errstate(invalid="ignore", over="ignore"):
         for row in s:
             acc = acc + row
     return float(tree(acc))
@@ -57,7 +57,7 @@ def batch_sums(v, m):
     x = np.where(m, v, 0.0)  # non-matches add +0.0, which changes no sum that starts from +0.0
     x = np.concatenate([x, np.zeros((-len(x)) % 256)]).reshape(-1, 32, 8)
     acc = np.zeros(x.shape[:2])
-    with np.errstate(invalid="ignore"):
+    with np.errstate(invalid="ignore", over="ignore"):
         for e in range(8):
             acc = acc + x[:, :, e]
     return tree(acc)

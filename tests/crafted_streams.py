@@ -420,6 +420,73 @@ def is_cold(f):
     return any(c["route"] == "cold" for c in f["chunks"])
 
 
+# ---- what the scan calls are asked: intervals over a batch's numbers, positions over its chunks ----------------------------------------
+def intervals(want, dtype):
+    """Named closed intervals (lo, hi) over the numbers `want` of `dtype`, for the filter and aggregate calls: everything (the type's
+    min..max; -inf..+inf for floats, every number but NaN), nothing (lo > hi), NaN bounds, point intervals at the most frequent value, at
+    the type's min and max and at the numbers of latents MID - 1 and MID (where they occur), the two halves split at the median value with
+    every bound a value that occurs, and for floats the finite range and the signed zeros and infinities alone."""
+    dt = np.dtype(dtype)
+    x = np.asarray(want, dtype=dt)
+    floats = dt.kind == "f"
+    vals = x[~np.isnan(x)] if floats else x
+    u, counts = np.unique(vals, return_counts=True)  # by value: -0.0 and +0.0 are one
+    lim = np.finfo(dt) if floats else np.iinfo(dt)
+    out = {"all": (-np.inf, np.inf) if floats else (dt.type(lim.min), dt.type(lim.max))}
+    out["nothing"] = (u[-1], u[0]) if u.size > 1 else (dt.type(lim.max), dt.type(lim.min))
+    if floats:
+        out["nan_lo"] = (np.nan, np.inf)
+        out["nan_hi"] = (-np.inf, np.nan)
+        out["finite"] = (dt.type(lim.min), dt.type(lim.max))
+    if u.size:
+        m = u[np.argmax(counts)]
+        out["most_frequent"] = (m, m)
+    mid = 1 << (nbits(dt) - 1)
+    for name, v in (("type_min", lim.min), ("type_max", lim.max)):
+        v = dt.type(v)
+        if (x == v).any():
+            out[name] = (v, v)
+    for name, lat in (("mid_minus_1", mid - 1), ("mid", mid)) if not floats else ():  # floats: -0.0 and +0.0, below
+        v = from_latents(np.array([lat], dtype=np.uint64), dt)[0]
+        if (x == v).any():
+            out[name] = (v, v)
+    if u.size > 1:
+        k = u.size // 2 - 1
+        out["lower_half"] = (u[0], u[k])
+        out["upper_half"] = (u[k + 1], u[-1])
+    if floats:
+        out.update({"neg_zero": (-0.0, -0.0), "pos_zero": (0.0, 0.0), "neg_inf": (-np.inf, -np.inf), "pos_inf": (np.inf, np.inf)})
+    return out
+
+
+def positions(chunk_ns, seed):
+    """Named, strictly ascending int64 positions into the concatenation of chunks of `chunk_ns` numbers, for the take calls: none and
+    every row; every row of the largest chunk; each chunk's first and last row; rows 255, 256 and 257 of each chunk; random 1 % and 50 %;
+    every partial last batch whole (a take of a batch's every row that is shorter than 256); and a whole batch behind one earlier row, so
+    that its numbers start at an odd output index."""
+    ns = np.asarray(chunk_ns, dtype=np.int64)
+    starts = np.concatenate([[0], np.cumsum(ns)[:-1]]).astype(np.int64)
+    total = int(ns.sum())
+    rng = np.random.default_rng(seed)
+    out = {"empty": np.zeros(0, np.int64), "every_row": np.arange(total, dtype=np.int64)}
+    if ns.size:
+        k = int(np.argmax(ns))
+        out["one_chunk"] = np.arange(starts[k], starts[k] + ns[k], dtype=np.int64)
+    out["chunk_ends"] = np.unique(np.concatenate([starts, starts + ns - 1])[np.concatenate([ns, ns]) > 0]).astype(np.int64)
+    near = [s + d for s, n in zip(starts, ns) for d in (255, 256, 257) if d < n]
+    out["rows_255_256_257"] = np.array(near, dtype=np.int64)
+    for name, frac in (("random_1pct", 0.01), ("random_50pct", 0.5)):
+        out[name] = np.sort(rng.choice(total, size=max(int(total * frac), 1), replace=False)).astype(np.int64) if total else np.zeros(0, np.int64)
+    tails = [np.arange(s + n // 256 * 256, s + n, dtype=np.int64) for s, n in zip(starts, ns) if n % 256]
+    if tails:
+        out["partial_last_batches"] = np.concatenate(tails)
+    full = [s + b * 256 for s, n in zip(starts, ns) for b in range(n // 256) if s + b * 256 > 0]
+    if full:
+        b0 = int(full[0])
+        out["odd_start_batch"] = np.concatenate([[b0 - 1], np.arange(b0, b0 + 256)]).astype(np.int64)
+    return out
+
+
 def class_counts(f):
     """Expected pco_b200_profile_chunk_classes counts of a fast family (index k = class k)."""
     counts = [0] * 8

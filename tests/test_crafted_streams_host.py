@@ -143,6 +143,73 @@ def test_families_cover_every_route():
     assert routes == {"fused3", "fused4", "fused5", "general1", "general2", "cold"}
 
 
+# ---- the scan calls' intervals and positions ------------------------------------------------------------------------------------
+BATCH_TYPES = sorted({f["dtype"].name for f in FAMILIES})
+
+
+def _batch(dtype_str):
+    """The expected numbers and chunk sizes of every family of one number type, in family order (one scan batch)."""
+    fams = [f for f in FAMILIES if f["dtype"].name == dtype_str]
+    return np.concatenate([cs.expected(f) for f in fams]), [c["n"] for f in fams for c in f["chunks"]]
+
+
+@pytest.mark.parametrize("dtype_str", BATCH_TYPES)
+def test_intervals_split_every_batch(dtype_str):
+    from tests.aggregate_reference import matches
+
+    want, _ = _batch(dtype_str)
+    iv = cs.intervals(want, want.dtype)
+    lower, upper = (matches(want, *iv[k]) for k in ("lower_half", "upper_half"))
+    n = int((~np.isnan(want)).sum()) if want.dtype.kind == "f" else want.size
+    for half in (lower, upper):
+        assert 0 < half.sum() < n, (dtype_str, int(half.sum()), n)
+    assert (lower | upper).sum() == n and not (lower & upper).any()  # the halves cut at a value: every number in exactly one
+    for k in ("lower_half", "upper_half", "most_frequent", "type_min", "type_max", "mid_minus_1", "mid"):
+        if k in iv:  # each bound is a number of the batch
+            assert all((want == b).any() for b in iv[k]), (k, iv[k])
+    assert matches(want, *iv["all"]).sum() == n and not matches(want, *iv["nothing"]).any()
+
+
+@pytest.mark.parametrize("dtype_str", ["f16", "f32", "f64"])
+def test_float_intervals_are_ieee_comparisons(dtype_str):
+    from tests.aggregate_reference import matches
+
+    dt = np.dtype(cs.DTYPES[dtype_str])
+    x = np.array([np.nan, -np.nan, np.inf, -np.inf, 0.0, -0.0, 1.5, -2.0, np.finfo(dt).max, np.finfo(dt).min], dtype=dt)
+    iv = cs.intervals(x, dt)
+    sel = {k: matches(x, *v) for k, v in iv.items()}
+    nan = np.isnan(x)
+    assert (sel["all"] == ~nan).all(), "-inf..+inf selects every number but NaN"
+    assert not sel["nan_lo"].any() and not sel["nan_hi"].any() and not sel["nothing"].any()
+    zeros = (x == 0) & ~nan
+    assert (sel["neg_zero"] == zeros).all() and (sel["pos_zero"] == zeros).all(), "-0.0 == +0.0"
+    assert (sel["pos_inf"] == (x == np.inf)).all() and (sel["neg_inf"] == (x == -np.inf)).all()
+    assert (sel["finite"] == np.isfinite(x)).all()
+    assert sel["type_min"].sum() == 1 and sel["type_max"].sum() == 1
+    # and on every float batch, the same intervals select what IEEE comparisons do
+    want, _ = _batch(dt.name)
+    for name, (lo, hi) in cs.intervals(want, want.dtype).items():
+        with np.errstate(invalid="ignore"):
+            ieee = (want >= want.dtype.type(lo)) & (want <= want.dtype.type(hi))
+        assert (matches(want, lo, hi) == ieee).all(), name
+
+
+@pytest.mark.parametrize("dtype_str", BATCH_TYPES)
+def test_positions_are_ascending_and_in_range(dtype_str):
+    _, ns = _batch(dtype_str)
+    total = sum(ns)
+    sets = cs.positions(ns, seed=1)
+    assert sets["every_row"].size == total and sets["empty"].size == 0
+    for name, p in sets.items():
+        assert p.dtype == np.int64 and (np.diff(p) > 0).all(), name
+        assert p.size == 0 or (p[0] >= 0 and p[-1] < total), name
+    starts = np.concatenate([[0], np.cumsum(ns)[:-1]])
+    assert sets["partial_last_batches"].size == sum(n % 256 for n in ns) > 0
+    odd = sets["odd_start_batch"]
+    b0 = int(odd[1])
+    assert odd.size == 257 and odd[0] < b0 and any(b0 - s >= 0 and (b0 - s) % 256 == 0 and b0 - s + 256 <= n for s, n in zip(starts, ns))
+
+
 # ---- invalid specs --------------------------------------------------------------------------------------------------------------
 def _one(bins, n=8, bits_ob=None, offsets=None, **kw):
     sym = [i % len(bins) for i in range(n)]
