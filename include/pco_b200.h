@@ -5,8 +5,9 @@
  *
  * Every entry point is plain C: pointers, sizes and POD structs; no torch / CUDA types in
  * signatures (a cudaStream_t travels as void*).  Each declaration cites the reference
- * interface it stands in for.  All functions are thread-safe; the library keeps only a
- * mutex-guarded cache of device scratch memory between calls.
+ * interface it stands in for.  All functions are thread-safe; between calls the library keeps
+ * device scratch memory per calling thread (see pco_b200_thread_release) and a mutex-guarded
+ * host cache of mode-search sample positions.
  */
 #ifndef PCO_B200_H
 #define PCO_B200_H
@@ -143,7 +144,8 @@ int pco_b200_profile_last(char *buf, size_t cap);
  * thread's next call), so calls from different threads - each with its own cudaStream_t - run concurrently, e.g. compress of
  * chunk group g + 1 on one thread while group g decompresses on another (both PCIe directions busy).  A worker thread that is
  * about to exit returns its device scratch with pco_b200_thread_release(); a thread that goes on calling the library afterwards gets
- * fresh scratch on its next call. */
+ * fresh scratch on its next call.  A call that fails with PCO_B200_CUDA (e.g. a refused allocation) leaves its thread usable: the
+ * next call sets up again what it needs. */
 void pco_b200_thread_release(void);
 /* Page-locked host buffers in place ("zero copy"): with bit 0 set, pco_b200_compress_ex (explicit Classic configs) reads a HOST `nums`
  * that is page-locked (cudaHostAlloc / cudaHostRegister, e.g. torch pin_memory) straight over PCIe in its one pass over the input; with

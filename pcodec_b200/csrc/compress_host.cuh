@@ -386,8 +386,10 @@ inline float lookback_sample_cost(const Summary& d, const Summary& p, uint32_t l
   return float((meta_bits + 7) / 8 + (page_bits + 7) / 8 + (body_bits + 7) / 8);
 }
 
-// mode sample positions per chunk size (host, computed once per distinct n; sampling.rs:73-95)
-inline const std::vector<uint32_t>& mode_sample_positions(size_t n) {
+// mode sample positions per chunk size (host, computed once per distinct n; sampling.rs:73-95).  Returned by value, copied under the
+// lock: the cache is process-wide and cleared once it holds more than 64 sizes, so a reference into it would dangle as soon as
+// another thread's Auto compress over new sizes clears it.
+inline std::vector<uint32_t> mode_sample_positions(size_t n) {
   static std::mutex mu;
   static std::map<size_t, std::vector<uint32_t>> cache;
   std::lock_guard<std::mutex> lock(mu);
@@ -435,8 +437,8 @@ static PcoB200Error plan_front(CompressScratch& S, cudaStream_t stream, EncParam
     init_chunks_kernel<<<(n_chunks + 255) / 256, 256, 0, stream>>>(d_chunks, n_chunks);
     for (const bool wide : {false, WIDE}) {
       if (S.encode_attrs_set[wide][LW]) continue;
-      S.encode_attrs_set[wide][LW] = true;
       PCOB_CUDA_TRY((wide ? set_encode_attrs<L, true>() : set_encode_attrs<L, false>()));
+      S.encode_attrs_set[wide][LW] = true;  // after success only: a failed call leaves the attributes to the next
     }
     if constexpr (!WIDE) {  // (wide sets: the two-kernel path below)
     if (e.mode == MODE_CLASSIC && e.n_vars == 1) {
@@ -776,7 +778,7 @@ static PcoB200Error compress_typed(CompressScratch& S, const void* nums, size_t 
     uint64_t* d_ustarts = S.sample_starts.as<uint64_t>();
     PCOB_CUDA_TRY(cudaMemcpyAsync(d_ustarts, ustarts.data(), ustarts.size() * 8, cudaMemcpyHostToDevice, stream));
     for (auto& kv : by_n) {
-      const std::vector<uint32_t>& pos = mode_sample_positions(size_t(kv.first));
+      const std::vector<uint32_t> pos = mode_sample_positions(size_t(kv.first));
       const uint32_t m = uint32_t(pos.size());
       if (m == 0) continue;  // fewer than MIN_SAMPLE numbers: Classic (sampling.rs:14-20)
       const std::vector<uint32_t>& ids = kv.second;

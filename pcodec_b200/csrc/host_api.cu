@@ -97,22 +97,26 @@ static PcoB200Error ensure_device(Context& c) {
       cudaSetDevice(cur);
     }
   }
+  // Only permanent outcomes are cached (set up, no device, not sm_90).  A set-up step that fails - a cudaMalloc refused on a GPU that
+  // is short of memory, or while another thread captures a CUDA graph in global mode - frees what it made and leaves the context
+  // uninitialised, so the thread's next call tries again.
   if (!c.initialized) {
-    c.initialized = true;
     int n = 0;
     cudaError_t e = cudaGetDeviceCount(&n);
     if (e != cudaSuccess || n == 0) {
+      c.initialized = true;
       c.device_err = e != cudaSuccess ? cudaGetErrorString(e) : "no CUDA device";
       cudaGetLastError();
     } else {
       cudaDeviceProp prop;
       int dev = 0;
-      cudaGetDevice(&dev);
+      PCOB_CUDA_TRY(cudaGetDevice(&dev));
+      PCOB_CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
       c.device = dev;
-      e = cudaGetDeviceProperties(&prop, dev);
-      if (e != cudaSuccess) c.device_err = cudaGetErrorString(e);
-      else if (prop.major != 9 || prop.minor != 0) c.device_err = std::string("device ") + prop.name + " is not sm_90 (the kernels are built for sm_90a only)";
-      else {
+      if (prop.major != 9 || prop.minor != 0) {
+        c.initialized = true;
+        c.device_err = std::string("device ") + prop.name + " is not sm_90 (the kernels are built for sm_90a only)";
+      } else {
         c.sm_count = prop.multiProcessorCount;
         // binomials mod 2^64 by Pascal additions
         Binoms hb;
@@ -124,12 +128,17 @@ static PcoB200Error ensure_device(Context& c) {
         for (int l = 0; l < 32; l++)
           for (int j = 0; j < MAX_ORDER; j++) hb.lane8[l][j] = C[8 * l][j];
         for (int j = 0; j < MAX_ORDER; j++) hb.full[j] = C[256][j];
-        e = cudaMalloc(&c.d_binoms, sizeof(Binoms));
+        if (!c.d_binoms) e = cudaMalloc(&c.d_binoms, sizeof(Binoms));
         if (e == cudaSuccess) e = cudaMemcpy(c.d_binoms, &hb, sizeof(Binoms), cudaMemcpyHostToDevice);
         if (e == cudaSuccess) e = cudaFuncSetAttribute(walk_kernel<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WalkSmem<12>));
         if (e == cudaSuccess) e = cudaFuncSetAttribute(walk_kernel<SMALL_MAX_SIZE_LOG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WalkSmem<SMALL_MAX_SIZE_LOG>));
-        if (e != cudaSuccess) c.device_err = cudaGetErrorString(e);
-        else c.device_ok = true;
+        if (e != cudaSuccess) {
+          // a free that is refused as well (the same global capture) keeps the table for the next try; reset_context frees it
+          if (c.d_binoms && cudaFree(c.d_binoms) == cudaSuccess) c.d_binoms = nullptr;
+          return cuda_fail(e, "CUDA device set-up (binomial table, walk kernel attributes)");
+        }
+        c.initialized = true;
+        c.device_ok = true;
       }
     }
   }
@@ -160,7 +169,6 @@ static PcoB200Error set_decode_attrs(Context& c) {
   static_assert(!(WIN && FILT) && (FILT || !AGG) && (FILT || !TAKE) && !(AGG && TAKE),
                 "no instantiation is both window and filter mode; aggregate and take mode are filter modes, and exclusive");
   if (c.attrs_set[WIN + 2 * FILT + AGG + 2 * TAKE]) return PCO_B200_OK;
-  c.attrs_set[WIN + 2 * FILT + AGG + 2 * TAKE] = true;
   auto max_shared = [](auto* kernel, size_t smem) {
     const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
     return e != cudaSuccess ? e : cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, int(cudaSharedmemCarveoutMaxShared));
@@ -170,6 +178,7 @@ static PcoB200Error set_decode_attrs(Context& c) {
   PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint32_t, WIN, FILT, AGG, TAKE>, sizeof(FusedSmem)));
   PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint16_t, WIN, FILT, AGG, TAKE>, sizeof(FusedSmem)));
   PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint8_t, WIN, FILT, AGG, TAKE>, sizeof(FusedSmem)));
+  c.attrs_set[WIN + 2 * FILT + AGG + 2 * TAKE] = true;  // only once every attribute is set: a failed call leaves them to the next
   return PCO_B200_OK;
 }
 
@@ -1212,7 +1221,7 @@ int pco_b200_zero_copy(int mask) { return mask < 0 ? zero_copy_mask().load() : z
 // thread's next call).
 void pco_b200_thread_release(void) {
   Context& c = ctx();
-  if (c.initialized && c.device_ok) reset_context(c);
+  if (c.initialized || c.d_binoms) reset_context(c);  // also a context whose set-up failed (it may hold the binomial table)
   readback_bounce().release();
 }
 // Which decode instantiation served the chunks of the last decode launch: counts[k] = chunks of class k
@@ -4025,6 +4034,9 @@ PcoB200Error pco_b200_build_index(const void* compressed, size_t compressed_len,
   PCOB_CUDA_TRY(c.index.reserve(index_cap));
   PCOB_CUDA_TRY(c.misc.reserve(sizeof(WalkResult)));
   uint8_t* d_index = c.index.as<uint8_t>();
+  // The walk writes only the records and entries of the file's chunks, but the bytes returned also hold the unused record slots and
+  // the padding before the entries: zeroed, so the index is the same on every call instead of carrying what the thread's scratch held.
+  PCOB_CUDA_TRY(cudaMemsetAsync(d_index, 0, index_cap, stream));
   walk_kernel<12><<<1, WALK_THREADS, sizeof(WalkSmem<12>), stream>>>(fp, d_index, chunks_offset, uint32_t(max_chunks), entries_begin, index_cap, hdr.first_chunk_byte,
                                                     0, ~uint64_t(0), nullptr, c.misc.as<WalkResult>(), 1);
   PCOB_CUDA_TRY(cudaGetLastError());

@@ -1,4 +1,4 @@
-// Host-side support for libcpcodec.so: error state, device scratch cache, standalone header
+// Host-side support for libcpcodec.so: error state, grow-only device buffers, standalone header
 // parse/write and size guarantees.  Independent of oracle/ (the product never links it).
 #pragma once
 #include <cuda_runtime.h>
@@ -27,7 +27,10 @@ inline PcoB200Error fail(PcoB200Error e, const std::string& msg) {
   last_error_ref() = msg;
   return e;
 }
+// Also clears the runtime's non-sticky last error of this thread: the calls check cudaGetLastError() after their launches, and an
+// error left over from a refused allocation would otherwise fail the thread's next call, which did nothing wrong.
 inline PcoB200Error cuda_fail(cudaError_t ce, const char* what) {
+  cudaGetLastError();
   return fail(PCO_B200_CUDA, std::string(what) + ": " + cudaGetErrorString(ce) +
                                  " (libcpcodec has no CPU fallback: a CUDA device is required)");
 }
@@ -299,7 +302,10 @@ struct DevBuf {
   size_t cap = 0;
   cudaError_t reserve(size_t n) {
     if (n <= cap) return cudaSuccess;
-    if (p) cudaFree(p);
+    if (p) {
+      cudaError_t e = cudaFree(p);
+      if (e != cudaSuccess) return e;  // (refused, e.g. during another thread's global capture): keep the buffer, not leak it
+    }
     p = nullptr;
     cap = 0;
     size_t want = n + (n >> 3) + 256;
