@@ -1211,6 +1211,148 @@ PcoB200Error pco_b200_take_files_async(const PcoB200AsyncFilesTakePlan *plan, co
  * ("position 17: ..."), and, when the kind is OK, sets *n_written (may be NULL) to the numbers written (*n_positions). */
 PcoB200Error pco_b200_take_files_async_result(const PcoB200AsyncFilesTakeStatus *host_status, size_t *n_written);
 
+/* ---- asynchronous segment aggregates of wrapped-format pages and of indexed standalone files (no reference counterpart): count, min,
+ * max and sum of the numbers x with lo <= x <= hi per caller-given row segment of the concatenation pco_b200_decompress_pages_async /
+ * pco_b200_decompress_files_async write, decoding only the pages or chunks the segments cover.  Time buckets over a column sorted by time
+ * (a chart's points, a downsampled series), one range per sensor or session of sorted logs, or the rows of a window are reduced without
+ * the decoded numbers ever reaching HBM: each 256-number batch is reduced per segment in the decoder's registers.  Each call only enqueues
+ * kernels on the caller's stream and returns at once; it makes no synchronising, allocating or host-to-device copy call and refers to no
+ * memory of the library's per-thread scratch, so it can be captured in a CUDA graph, and a captured call may be replayed after
+ * pco_b200_thread_release or after any other call.  A plan made once outside any capture fixes the grids from its capacities; the refs,
+ * their count, the bounds, their count and the interval are read on the device, so one captured graph serves new pages or files, new
+ * segments and new bounds on each replay.
+ * bounds (uint64_t[max_segments + 1]) and n_segments (one uint64_t) are device memory, of the types a filter call writes its positions
+ * and count in (and torch.searchsorted writes), so they can be computed in the same graph.  With M = *n_segments, segment g < M is the
+ * rows [bounds[g], bounds[g + 1]) of the concatenation.  bounds must be non-decreasing; equal bounds make an empty segment.  Rows before
+ * bounds[0] or at or after bounds[M] belong to no segment.  M = 0 reads no bound, decodes nothing, writes no aggs and a total of zeros.
+ * aggs[g] (PcoB200Aggregate[max_segments]) gets n_rows = bounds[g + 1] - bounds[g] and the count, min, max and sum of the segment's numbers
+ * inside the interval, compared, ordered and summed as pco_b200_aggregate_pages_async does; *total covers the union of the segments
+ * (n_rows = bounds[M] - bounds[0]).  Records past M are not written.
+ * Float sums, in an order that depends on neither grids nor timing:
+ *   1. batch partial of segment g in one 256-number batch of a page or chunk: steps 1 - 2 of the aggregate's rule, with the batch's rows
+ *      outside the segment counted as non-matches (they add +0.0);
+ *   2. segment sum: the batches that hold rows of the segment, in row order, batch j (counted from 0 and running on across pages and
+ *      chunks) to lane j mod 32, each lane adding its partials in order from +0.0, then the pairwise tree;
+ *   3. total: the segments' sums by the rule of step 2, with segment g in place of batch j.
+ *   So segments equal to the pages (or files) give pco_b200_aggregate_pages_async's (_files_async's) aggs and total bit for bit, and one
+ *   segment over every row of one page (or file) gives its total.
+ * Refusals, in this order, each decided before any page or chunk is decoded; a refused call writes no aggs and a total of zeros:
+ *   1. the decompress call's refusals before its decode stage, in its order, with its kinds and naming the same page, or file and chunk:
+ *      for pages every check up to and including the walk of every page, for files every check up to and including placement
+ *      (PCO_B200_ASYNC_PAGES_DST / PCO_B200_ASYNC_FILES_DST against rows_cap);
+ *   2. *n_segments above max_segments (PCO_B200_SEGMENTS_TOO_MANY);
+ *   3. the lowest j with bounds[j] < bounds[j - 1] (PCO_B200_SEGMENTS_ORDER, segment j);
+ *   4. the lowest j with bounds[j] past the rows of the concatenation (PCO_B200_SEGMENTS_PAST, segment j).
+ * Then only the pages or chunks whose rows meet [bounds[0], bounds[M]) are decoded, so a decode failure is reported only for one of
+ * them, as the decompress call names it; a corrupt page or chunk outside that range does not fail the call (pages are still walked). */
+enum {
+  PCO_B200_SEGMENTS_TOO_MANY = 0x401,  /* *n_segments (n_segments) is above the plan's max_segments (PCO_B200_INVALID_ARGUMENT) */
+  PCO_B200_SEGMENTS_ORDER = 0x402,     /* bounds[segment] is below the bound before it (PCO_B200_INVALID_ARGUMENT) */
+  PCO_B200_SEGMENTS_PAST = 0x403       /* bounds[segment] lies past the n_written rows of the concatenation (PCO_B200_INVALID_ARGUMENT) */
+};
+
+typedef struct PcoB200AsyncSegmentAggregatePlan {  /* filled by pco_b200_segment_aggregate_pages_async_plan; treat as opaque */
+  uint32_t dtype, reserved;
+  uint64_t metas_cap, pages_cap, max_pages, rows_cap, frame_cap, max_segments;
+  uint64_t workspace_bytes;                        /* device workspace one in-flight call needs */
+} PcoB200AsyncSegmentAggregatePlan;
+
+typedef struct PcoB200AsyncSegmentAggregateStatus {  /* written on the device by every call */
+  uint32_t kind;                                     /* PcoB200Error */
+  uint32_t device_status;                            /* the device word behind it: as PcoB200AsyncPagesStatus, or PCO_B200_SEGMENTS_* */
+  uint64_t page;                                     /* the page the outcome names (UINT64_MAX if none) */
+  uint64_t n_written;                                /* the rows of the concatenation (the sum of page_n), once every page passed its
+                                                        checks (0 on a failure of the pages call) */
+  uint64_t n_pages;                                  /* *n_pages as the call read it */
+  uint64_t frames_needed;                            /* bytes of framed pages the batch needs, also when above frame_cap (0 when refused
+                                                        earlier) */
+  uint64_t n_segments;                               /* *n_segments as the call read it */
+  uint64_t segment;                                  /* the bound index a PCO_B200_SEGMENTS_ORDER / _PAST refusal names (UINT64_MAX if none) */
+  uint64_t records_decoded;                          /* the pages decoded: those the segments touch (0 unless the kind is OK) */
+  uint64_t n_matches;                                /* total->count (0 unless the kind is OK) */
+} PcoB200AsyncSegmentAggregateStatus;
+
+/* Makes a plan for segment aggregates over up to max_segments segments of up to max_pages pages of dtype, whose refs point into
+ * metas_cap bytes of metas and pages_cap bytes of pages, holding at most rows_cap numbers in all (the role dst_cap plays in
+ * pco_b200_decompress_pages_async); frame_cap bounds the framed pages as in that call.  Checked before the device is touched: dtype
+ * (PCO_B200_INVALID_TYPE), max_pages in 1 .. 2^31 - 1, rows_cap and frame_cap at most 2^56, max_segments in 1 .. 2^31 - 1
+ * (PCO_B200_INVALID_ARGUMENT).  Then *plan is filled and the one-time device set-up runs on the current device, which the calls must use
+ * (kernel attributes, and every kernel the call launches loaded); without a device that is PCO_B200_CUDA.
+ * workspace_bytes is pco_b200_decompress_pages_async_plan's formula with dst_cap = rows_cap, plus these regions, each rounded up to 256
+ * bytes, with S = floor(rows_cap / 256) + max_pages batch slots, R = S + max_segments records and E the bytes of a number of dtype: 40 (the
+ * pages status), 56 (the plan's state), 8 S (each slot's run of segments), 4 max_pages (touched flags), 8 (max_segments + 3) (the
+ * interval and bounds), 40 R (the batch-segment records), E rows_cap (the cold pages' values), 48 max_segments (the segments'
+ * accumulators) and 24 (rows_cap / 262144 + 2) (the long segments). */
+PcoB200Error pco_b200_segment_aggregate_pages_async_plan(unsigned char dtype, size_t metas_cap, size_t pages_cap, size_t max_pages, size_t rows_cap,
+                                                         size_t frame_cap, size_t max_segments, PcoB200AsyncSegmentAggregatePlan *plan);
+/* Enqueues the segment aggregates of the pages refs[0 : *n_pages) names on `cuda_stream`, and the outcome into *status; returns without
+ * waiting.  metas (metas_cap bytes), pages (pages_cap bytes; may be the same buffer as metas), refs (PcoB200PageRef[max_pages]), n_pages
+ * (one uint64_t), bounds, n_segments, interval (one PcoB200Interval), aggs, total (one PcoB200Aggregate), workspace
+ * (plan->workspace_bytes, 256-byte aligned) and status are device pointers; one workspace serves one call in flight.  The bounds index the
+ * concatenation pco_b200_decompress_pages_async writes for the same arguments with dst_cap = rows_cap.  The return value covers the host
+ * side only: null pointers, an unaligned workspace or a plan that was not filled (PCO_B200_INVALID_ARGUMENT), a launch the runtime refuses
+ * (PCO_B200_CUDA).  With pco_b200_profile_enable(1), a call outside a stream capture records its kernel spans for pco_b200_profile_last;
+ * a call inside a capture records none. */
+PcoB200Error pco_b200_segment_aggregate_pages_async(const PcoB200AsyncSegmentAggregatePlan *plan, const void *metas, const void *pages,
+                                                    const PcoB200PageRef *refs, const uint64_t *n_pages, const uint64_t *bounds,
+                                                    const uint64_t *n_segments, const PcoB200Interval *interval, PcoB200Aggregate *aggs,
+                                                    PcoB200Aggregate *total, void *workspace, PcoB200AsyncSegmentAggregateStatus *status,
+                                                    void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory at a point of the caller's choosing.  Returns the kind,
+ * sets the last-error message as pco_b200_aggregate_pages_async_result words it ("page 17: ...") or, for the call's own refusals, naming
+ * the bound index ("segment 17: ..."), and, when the kind is OK, sets *n_matches (may be NULL) to the total match count. */
+PcoB200Error pco_b200_segment_aggregate_pages_async_result(const PcoB200AsyncSegmentAggregateStatus *host_status, size_t *n_matches);
+
+typedef struct PcoB200AsyncFilesSegmentAggregatePlan {  /* filled by pco_b200_segment_aggregate_files_async_plan; treat as opaque */
+  uint32_t dtype, uniform_type, format_major, reserved;
+  uint64_t src_cap, index_cap, max_files, max_chunks, rows_cap, max_segments;
+  uint64_t workspace_bytes;                             /* device workspace one in-flight call needs */
+} PcoB200AsyncFilesSegmentAggregatePlan;
+
+typedef struct PcoB200AsyncFilesSegmentAggregateStatus {  /* written on the device by every call */
+  uint32_t kind;                                          /* PcoB200Error */
+  uint32_t device_status;                                 /* the device word behind it: as PcoB200AsyncFilesStatus, or PCO_B200_SEGMENTS_* */
+  uint64_t file;                                          /* the file the outcome names (UINT64_MAX if none) */
+  uint64_t chunk;                                         /* the failing chunk, counted from that file's first chunk (UINT64_MAX if none) */
+  uint64_t n_written;                                     /* the rows of the concatenation (the sum of the files' counts), once every file
+                                                             passed its checks and placement (0 before) */
+  uint64_t n_files;                                       /* *n_files as the call read it */
+  uint64_t n_segments;                                    /* *n_segments as the call read it */
+  uint64_t segment;                                       /* the bound index a PCO_B200_SEGMENTS_ORDER / _PAST refusal names (UINT64_MAX
+                                                             if none) */
+  uint64_t records_decoded;                               /* the chunks decoded: those the segments touch (0 unless the kind is OK) */
+  uint64_t n_matches;                                     /* total->count (0 unless the kind is OK) */
+} PcoB200AsyncFilesSegmentAggregateStatus;
+
+/* Makes a plan for segment aggregates over up to max_segments segments of up to max_files indexed files of dtype holding at most
+ * max_chunks chunks and rows_cap numbers in all (the role dst_cap plays in pco_b200_decompress_files_async).  `head`, src_cap and
+ * index_cap are those of pco_b200_decompress_files_async_plan.  Checked before the device is touched, with that plan's kinds: dtype, the
+ * header, the uniform type, max_files in 1 .. 2^31 - 1, max_chunks in 1 .. 2^32 - 1, rows_cap at most 2^56, max_segments in
+ * 1 .. 2^31 - 1 (PCO_B200_INVALID_ARGUMENT).  Then *plan is filled and the one-time device set-up runs on the current device, which the
+ * calls must use; without a device that is PCO_B200_CUDA.
+ * workspace_bytes is pco_b200_decompress_files_async_plan's formula with dst_cap = rows_cap, plus these regions, each rounded up to 256
+ * bytes, with S = floor(rows_cap / 256) + max_chunks batch slots, R = S + max_segments records and E the bytes of a number of dtype: 40
+ * (the files status), 56 (the plan's state), 8 S (each slot's run of segments), 4 max_chunks (touched flags), 8 (max_segments + 3) (the
+ * interval and bounds), 40 R (the batch-segment records), E rows_cap (the cold chunks' values), 4 max_chunks (slot map),
+ * 4 (max_chunks + 1) (cold list), 48 max_segments (the segments' accumulators) and 24 (rows_cap / 262144 + 2) (the long segments). */
+PcoB200Error pco_b200_segment_aggregate_files_async_plan(const void *head, size_t head_len, unsigned char dtype, size_t src_cap, size_t index_cap,
+                                                         size_t max_files, size_t max_chunks, size_t rows_cap, size_t max_segments,
+                                                         PcoB200AsyncFilesSegmentAggregatePlan *plan);
+/* Enqueues the segment aggregates of files[0 : *n_files) on `cuda_stream`, and the outcome into *status; returns without waiting.  src
+ * (src_cap bytes), index (index_cap bytes), files (PcoB200FileRef[max_files]), n_files (one uint64_t), bounds, n_segments, interval, aggs,
+ * total, workspace (plan->workspace_bytes, 256-byte aligned) and status are device pointers; one workspace serves one call in flight.
+ * The bounds index the concatenation pco_b200_decompress_files_async writes for the same arguments with dst_cap = rows_cap.  The return
+ * value covers the host side only, as for pco_b200_segment_aggregate_pages_async. */
+PcoB200Error pco_b200_segment_aggregate_files_async(const PcoB200AsyncFilesSegmentAggregatePlan *plan, const void *src, const void *index,
+                                                    const PcoB200FileRef *files, const uint64_t *n_files, const uint64_t *bounds,
+                                                    const uint64_t *n_segments, const PcoB200Interval *interval, PcoB200Aggregate *aggs,
+                                                    PcoB200Aggregate *total, void *workspace, PcoB200AsyncFilesSegmentAggregateStatus *status,
+                                                    void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory.  Returns the kind, sets the last-error message as
+ * pco_b200_aggregate_files_async_result words it ("file 3: chunk 2: ...") or, for the call's own refusals, naming the bound index
+ * ("segment 17: ..."), and, when the kind is OK, sets *n_matches (may be NULL) to the total match count. */
+PcoB200Error pco_b200_segment_aggregate_files_async_result(const PcoB200AsyncFilesSegmentAggregateStatus *host_status, size_t *n_matches);
+
 /* ---- asynchronous batch compress into wrapped-format chunks (no reference counterpart): pco_b200_compress_wrapped over a batch of
  * arrays, with the array sizes, their count and every buffer in device memory.  A GPU writer of a container that embeds pco (a columnar
  * file whose column chunks a kernel sized, a page store) compresses every column chunk behind the step that produced it, with no copy to

@@ -1072,6 +1072,64 @@ __device__ __forceinline__ void take_store8(const FiltStage& f, uint64_t row, ui
   const TakeRun run = take_run(f, slot);
   take_store8<L>(f, run, take_pos0(f, run, lane), row, cnt, lane, r);
 }
+// ---------------------------------------------------------------------------
+// Segment mode (the SEG instantiations, both segment-aggregate calls; with FILT): the same slots, but a batch is reduced once per
+// caller segment its rows meet, as agg_store8 reduces it with the rows outside the segment counted as non-matches.  The plan
+// (async_segment_aggregate_kernels.cuh) gives slot s the run {g0, g1} of segments its rows meet (g0 > g1: none), and segment g's partial
+// of slot s goes to record s + g; a slot's segments are above every earlier slot's, so no two (slot, segment) pairs share a record.
+// FiltStage: `interval` carries the interval's two words followed by the bounds (seg_bounds), `counts` one touched flag per record,
+// `rows` the SegRec array (seg_recs) and `offs` the SegRun array (seg_runs).
+// ---------------------------------------------------------------------------
+struct SegRun {
+  uint32_t g0, g1;  // the segments the batch's rows meet, inclusive
+};
+struct SegRec {
+  uint64_t count, kmin, kmax, lo, hi;  // agg_store8's fields with the count; written for every (batch, segment) pair, matches or not
+};
+__host__ __device__ inline const uint64_t* seg_bounds(const FiltStage& f) { return f.interval + 2; }
+__host__ __device__ inline SegRec* seg_recs(const FiltStage& f) { return reinterpret_cast<SegRec*>(f.rows); }
+__host__ __device__ inline SegRun* seg_runs(const FiltStage& f) { return reinterpret_cast<SegRun*>(f.offs); }
+// Segment mode's store: the lane's 8 numbers of a batch of `cnt` numbers (first row `row`, slot `slot`), reduced for each segment of
+// the slot's run that holds some of its rows.  All 32 lanes call it; the loop is uniform over the warp.
+template <typename L>
+__device__ __forceinline__ void seg_store8(const FiltStage& f, const FiltKey& k, uint64_t row, uint64_t slot, uint32_t cnt, int lane,
+                                           const L (&r)[8]) {
+  const SegRun run = seg_runs(f)[slot];
+  if (run.g0 > run.g1) return;  // no segment meets the batch (segments are below 2^31, so g1 + 1 never wraps)
+  const uint64_t* __restrict__ bounds = seg_bounds(f);
+  uint32_t hitm = 0;
+  uint64_t key[8];
+#pragma unroll
+  for (int e = 0; e < 8; e++) {
+    key[e] = uint64_t(filt_key<L>(r[e], k.kind));
+    hitm |= uint32_t(k.any && uint32_t(lane * 8 + e) < cnt && L(L(key[e]) - L(k.lo)) <= L(k.span)) << e;
+  }
+  for (uint32_t g = run.g0; g <= run.g1; g++) {
+    const uint64_t a = max(bounds[g], row), b = min(bounds[g + 1], row + cnt);
+    if (a >= b) continue;  // an empty segment between two bounds of this batch
+    uint32_t total = 0;
+    uint64_t kmin = ~uint64_t(0), kmax = 0, lo = 0, hi = 0;
+    double fs = 0.0;
+#pragma unroll
+    for (int e = 0; e < 8; e++) {
+      const uint64_t x = row + uint64_t(lane * 8 + e);
+      const bool hit = ((hitm >> e) & 1u) && x >= a && x < b;
+      total += __popc(__ballot_sync(0xffffffffu, hit));
+      if (hit) {
+        kmin = min(kmin, key[e]);
+        kmax = max(kmax, key[e]);
+        if (k.kind == 2) {
+          fs = fs + agg_f64<L>(r[e]);
+        } else {
+          const uint64_t v = agg_ext<L>(r[e], k.kind);
+          agg_add128(lo, hi, v, k.kind == 1 && int64_t(v) < 0 ? ~uint64_t(0) : 0);
+        }
+      }
+    }
+    agg_warp(kmin, kmax, lo, hi, fs, k.kind == 2);
+    if (lane == 0) seg_recs(f)[slot + g] = SegRec{total, kmin, kmax, k.kind == 2 ? uint64_t(__double_as_longlong(fs)) : lo, hi};
+  }
+}
 template <typename L>
 __device__ __forceinline__ void load8(const L* __restrict__ src, L (&r)[8]) {
   if (sizeof(L) == 8) {
@@ -1348,7 +1406,8 @@ __global__ void __launch_bounds__(SW_THREADS) symwalk_kernel(FileParams fp, cons
 // FILT: filter mode (filt_store8: only the numbers inside *filt.interval are staged, in row order, with out as the value staging).
 // AGG (with FILT): aggregate mode (agg_store8: the matches reduced per batch into filt.counts and filt.agg; out is not written).
 // TAKE (with FILT): take mode (take_store8: the numbers at the run's positions to out_values; out is not written).
-template <typename L, int NV, bool WIN = false, bool FILT = false, bool AGG = false, bool TAKE = false>
+// SEG (with FILT): segment mode (seg_store8: the matches reduced per batch and segment into the SegRec records; out is not written).
+template <typename L, int NV, bool WIN = false, bool FILT = false, bool AGG = false, bool TAKE = false, bool SEG = false>
 __global__ void __launch_bounds__(DEC_THREADS, NV == 1 ? PCOB_DEC_NV1_BLOCKS : 2)
 decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __restrict__ statuses, const uint8_t* __restrict__ index_base, uint64_t index_len,
               L* __restrict__ out, uint64_t out_len, const Binoms* __restrict__ binoms, const uint8_t* __restrict__ d_syms,
@@ -1729,7 +1788,9 @@ decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __
             res[e] = from_latent_kind<L>(L(L(pq << k) + lowest), 2);
           }
         }
-        if constexpr (TAKE) {
+        if constexpr (SEG) {
+          seg_store8<L>(filt, fkey, task.out_offset + uint64_t(b) * BATCH_N, fslot0 + b, out_cnt, lane, res);
+        } else if constexpr (TAKE) {
           take_store8<L>(filt, task.out_offset + uint64_t(b) * BATCH_N, fslot0 + b, out_cnt, lane, res);
         } else if constexpr (AGG) {
           agg_store8<L>(filt, fkey, fslot0 + b, out_cnt, lane, res);

@@ -17,6 +17,7 @@
 #include "async_pages_kernels.cuh"
 #include "async_pages_to_file_kernels.cuh"
 #include "async_ranges_kernels.cuh"
+#include "async_segment_aggregate_kernels.cuh"
 #include "async_take_kernels.cuh"
 #include "compress_host.cuh"
 #include "decode_kernels.cuh"
@@ -46,7 +47,7 @@ namespace pcob200 {
 // The context follows the thread's current device: a cudaSetDevice between calls drops the scratch of the previous device.
 struct Context {
   int device = -1;
-  bool attrs_set[5] = {false, false, false, false, false};  // set_decode_attrs<WIN, FILT, AGG, TAKE> has run (index WIN + 2 FILT + AGG + 2 TAKE)
+  bool attrs_set[6] = {false, false, false, false, false, false};  // set_decode_attrs<WIN, FILT, AGG, TAKE, SEG> has run (index WIN + 2 FILT + AGG + 2 TAKE + 3 SEG)
   bool initialized = false;
   bool device_ok = false;
   std::string device_err;
@@ -163,22 +164,23 @@ struct DecodeOutcome {
 };
 
 // Shared-memory attributes of the decode kernels (the window-mode instantiations when WIN, the filter-mode ones when FILT, the
-// aggregate-mode ones when AGG too, the take-mode ones when TAKE too), set once per context before their first launch.
-template <bool WIN, bool FILT = false, bool AGG = false, bool TAKE = false>
+// aggregate-mode ones when AGG too, the take-mode ones when TAKE too, the segment-mode ones when SEG too), set once per context before
+// their first launch.
+template <bool WIN, bool FILT = false, bool AGG = false, bool TAKE = false, bool SEG = false>
 static PcoB200Error set_decode_attrs(Context& c) {
-  static_assert(!(WIN && FILT) && (FILT || !AGG) && (FILT || !TAKE) && !(AGG && TAKE),
-                "no instantiation is both window and filter mode; aggregate and take mode are filter modes, and exclusive");
-  if (c.attrs_set[WIN + 2 * FILT + AGG + 2 * TAKE]) return PCO_B200_OK;
+  static_assert(!(WIN && FILT) && (FILT || !AGG) && (FILT || !TAKE) && (FILT || !SEG) && int(AGG) + int(TAKE) + int(SEG) <= 1,
+                "no instantiation is both window and filter mode; aggregate, take and segment mode are filter modes, and exclusive");
+  if (c.attrs_set[WIN + 2 * FILT + AGG + 2 * TAKE + 3 * SEG]) return PCO_B200_OK;
   auto max_shared = [](auto* kernel, size_t smem) {
     const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
     return e != cudaSuccess ? e : cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, int(cudaSharedmemCarveoutMaxShared));
   };
   PCOB_CUDA_TRY(max_shared(symwalk_kernel<WIN>, sizeof(SymWalkSmem)));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint64_t, WIN, FILT, AGG, TAKE>, sizeof(FusedSmem)));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint32_t, WIN, FILT, AGG, TAKE>, sizeof(FusedSmem)));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint16_t, WIN, FILT, AGG, TAKE>, sizeof(FusedSmem)));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint8_t, WIN, FILT, AGG, TAKE>, sizeof(FusedSmem)));
-  c.attrs_set[WIN + 2 * FILT + AGG + 2 * TAKE] = true;  // only once every attribute is set: a failed call leaves them to the next
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint64_t, WIN, FILT, AGG, TAKE, SEG>, sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint32_t, WIN, FILT, AGG, TAKE, SEG>, sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint16_t, WIN, FILT, AGG, TAKE, SEG>, sizeof(FusedSmem)));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint8_t, WIN, FILT, AGG, TAKE, SEG>, sizeof(FusedSmem)));
+  c.attrs_set[WIN + 2 * FILT + AGG + 2 * TAKE + 3 * SEG] = true;  // only once every attribute is set: a failed call leaves them to the next
   return PCO_B200_OK;
 }
 
@@ -791,18 +793,18 @@ static PcoB200Error load_kernels(std::initializer_list<const void*> kernels) {
 static PcoB200Error async_result_kind(uint32_t kind) { return kind <= PCO_B200_UNSUPPORTED ? PcoB200Error(kind) : PCO_B200_CORRUPTION; }
 
 // The set-up of an asynchronous decompress plan: the device, the decode kernels' attributes (the window-mode instantiations when WIN, the
-// filter-mode ones when FILT, the aggregate-mode ones when AGG too, the take-mode ones when TAKE too), and loaded: the decode stage's
-// kernels for dtype, the call's catch-all kernel (cold(tag) for a latent type tag) and the call's `kernels`.
-template <bool WIN, bool FILT = false, bool AGG = false, bool TAKE = false, typename Cold>
+// filter-mode ones when FILT, the aggregate-mode ones when AGG too, the take-mode ones when TAKE too, the segment-mode ones when SEG too),
+// and loaded: the decode stage's kernels for dtype, the call's catch-all kernel (cold(tag) for a latent type tag) and the call's `kernels`.
+template <bool WIN, bool FILT = false, bool AGG = false, bool TAKE = false, bool SEG = false, typename Cold>
 static PcoB200Error async_decode_setup(unsigned char dtype, Cold cold, std::initializer_list<const void*> kernels) {
   Context& c = ctx();
   if (PcoB200Error e = ensure_device(c)) return e;
-  if (PcoB200Error e = set_decode_attrs<WIN, FILT, AGG, TAKE>(c)) return e;
+  if (PcoB200Error e = set_decode_attrs<WIN, FILT, AGG, TAKE, SEG>(c)) return e;
   if (PcoB200Error e = load_kernels(kernels)) return e;
   return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
     using L = decltype(tag);
-    return load_kernels({(const void*)fused_narrow_kernel<L, WIN, FILT, AGG, TAKE>, (const void*)symwalk_kernel<WIN>,
-                         (const void*)decode_kernel<L, 1, WIN, FILT, AGG, TAKE>, (const void*)decode_kernel<L, 2, WIN, FILT, AGG, TAKE>, cold(tag)});
+    return load_kernels({(const void*)fused_narrow_kernel<L, WIN, FILT, AGG, TAKE, SEG>, (const void*)symwalk_kernel<WIN>,
+                         (const void*)decode_kernel<L, 1, WIN, FILT, AGG, TAKE, SEG>, (const void*)decode_kernel<L, 2, WIN, FILT, AGG, TAKE, SEG>, cold(tag)});
   });
 }
 
@@ -866,15 +868,15 @@ struct DecodeStage {
   void* dst;
   uint64_t dst_cap;
   const WinTask* wins;
-  FiltStage filt;  // FILT: dst is the value staging (decode_kernels.cuh, filt_store8); AGG: dst is null (agg_store8); TAKE: likewise (take_store8)
+  FiltStage filt;  // FILT: dst is the value staging (decode_kernels.cuh, filt_store8); AGG: dst is null (agg_store8); TAKE, SEG: likewise
 };
-template <bool WIN, bool FILT = false, bool AGG = false, bool TAKE = false>
+template <bool WIN, bool FILT = false, bool AGG = false, bool TAKE = false, bool SEG = false>
 static void enqueue_decode_stage(const AsyncLaunch& ln, const DecodeStage& d) {
   const cudaStream_t stream = ln.stream;
   ln.begin("fused_narrow_kernel");
   dispatch_latent(d.fp.dtype, [&](auto tag) {
     using L = decltype(tag);
-    fused_narrow_kernel<L, WIN, FILT, AGG, TAKE><<<d.slots, FZ_THREADS, sizeof(FusedSmem), stream>>>(d.fp, d.table, d.index, d.index_len, d.st, d.cls,
+    fused_narrow_kernel<L, WIN, FILT, AGG, TAKE, SEG><<<d.slots, FZ_THREADS, sizeof(FusedSmem), stream>>>(d.fp, d.table, d.index, d.index_len, d.st, d.cls,
                                                                                          static_cast<L*>(d.dst), d.dst_cap, d.wins, d.filt);
     return 0;
   });
@@ -885,9 +887,9 @@ static void enqueue_decode_stage(const AsyncLaunch& ln, const DecodeStage& d) {
   ln.begin("decode_kernel");
   dispatch_latent(d.fp.dtype, [&](auto tag) {
     using L = decltype(tag);
-    decode_kernel<L, 1, WIN, FILT, AGG, TAKE><<<d.slots, DEC_THREADS, sizeof(DecodeSmem), stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst),
+    decode_kernel<L, 1, WIN, FILT, AGG, TAKE, SEG><<<d.slots, DEC_THREADS, sizeof(DecodeSmem), stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst),
                                                                                         d.dst_cap, d.binoms, d.syms, d.offs, d.cls, d.wins, d.filt);
-    decode_kernel<L, 2, WIN, FILT, AGG, TAKE><<<d.slots, DEC_THREADS, sizeof(DecodeSmem), stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst),
+    decode_kernel<L, 2, WIN, FILT, AGG, TAKE, SEG><<<d.slots, DEC_THREADS, sizeof(DecodeSmem), stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst),
                                                                                         d.dst_cap, d.binoms, d.syms, d.offs, d.cls, d.wins, d.filt);
     return 0;
   });
@@ -2800,10 +2802,11 @@ PcoB200Error pco_b200_decompress_files_async_plan(const void* head, size_t head_
 // catch-all decoder runs (pco_b200_filter_files_async).  With `agg` too, the aggregate-mode instantiations, which store nothing to dst;
 // dst is the catch-all decoder's value staging only (pco_b200_aggregate_files_async).  With `take` instead of `agg`, the take-mode
 // instantiations, likewise (pco_b200_take_files_async).  `between`, when given, enqueues its launches behind the front end
-// (merge_index_kernel) and before the decode stage.
+// (merge_index_kernel) and before the decode stage.  With `seg` (and neither `agg` nor `take`), the segment-mode instantiations, likewise
+// (pco_b200_segment_aggregate_files_async).
 static void enqueue_files(const AsyncLaunch& ln, const AfArgs& g, const AfLayout& lay, uint8_t* ws, void* dst, const FiltStage* filt,
                           uint32_t* cold_list, uint64_t* file_ns, PcoB200AsyncFilesStatus* status, bool agg = false, bool take = false,
-                          const std::function<void()>& between = {}) {
+                          const std::function<void()>& between = {}, bool seg = false) {
   const cudaStream_t stream = ln.stream;
   const uint32_t mf = g.max_files, mc = g.max_chunks;
   AsyncCheck* chk = reinterpret_cast<AsyncCheck*>(ws);
@@ -2838,9 +2841,10 @@ static void enqueue_files(const AsyncLaunch& ln, const AfArgs& g, const AfLayout
   ln.end();
   if (between) between();
   const DecodeStage d{g.fp, table, d_idx, g.index_cap, mc, d_st, ws + lay.cls, ws + lay.syms, reinterpret_cast<uint32_t*>(ws + lay.offs),
-                      &chk->binoms, agg || take ? nullptr : dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{}};
+                      &chk->binoms, agg || take || seg ? nullptr : dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{}};
   if (filt) {
-    if (agg) enqueue_decode_stage<false, true, true>(ln, d);
+    if (seg) enqueue_decode_stage<false, true, false, false, true>(ln, d);
+    else if (agg) enqueue_decode_stage<false, true, true>(ln, d);
     else if (take) enqueue_decode_stage<false, true, false, true>(ln, d);
     else enqueue_decode_stage<false, true>(ln, d);
     ln.begin("ff_cold_list_kernel");
@@ -3101,9 +3105,11 @@ static void enqueue_pages_front(const AsyncLaunch& ln, const ApArgs& g, const Ap
 // is their value staging (pco_b200_filter_pages_async).  With `agg` too, the aggregate-mode instantiations, which store nothing to dst;
 // dst is the catch-all decoder's value staging only (pco_b200_aggregate_pages_async).  With `take` instead of `agg`, the take-mode
 // instantiations, likewise (pco_b200_take_pages_async).  `between`, when given, enqueues its launches behind the front end
-// (ap_rewalk_kernel) and before the decode stage.
+// (ap_rewalk_kernel) and before the decode stage.  With `seg` (and neither `agg` nor `take`), the segment-mode instantiations, likewise
+// (pco_b200_segment_aggregate_pages_async).
 static void enqueue_pages(const AsyncLaunch& ln, const ApArgs& g, const ApLayout& lay, uint8_t* ws, void* dst, const FiltStage* filt,
-                          PcoB200AsyncPagesStatus* status, bool agg = false, bool take = false, const std::function<void()>& between = {}) {
+                          PcoB200AsyncPagesStatus* status, bool agg = false, bool take = false, const std::function<void()>& between = {},
+                          bool seg = false) {
   const cudaStream_t stream = ln.stream;
   AsyncCheck* chk = reinterpret_cast<AsyncCheck*>(ws);
   ApState* state = reinterpret_cast<ApState*>(ws + lay.state);
@@ -3121,8 +3127,9 @@ static void enqueue_pages(const AsyncLaunch& ln, const ApArgs& g, const ApLayout
   enqueue_pages_front(ln, g, lay, ws);
   if (between) between();
   const DecodeStage d{fp, table, d_idx, lay.index_len, mp, d_st, ws + lay.cls, ws + lay.syms, reinterpret_cast<uint32_t*>(ws + lay.offs),
-                      &chk->binoms, agg || take ? nullptr : dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{}};
-  if (agg) enqueue_decode_stage<false, true, true>(ln, d);
+                      &chk->binoms, agg || take || seg ? nullptr : dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{}};
+  if (seg) enqueue_decode_stage<false, true, false, false, true>(ln, d);
+  else if (agg) enqueue_decode_stage<false, true, true>(ln, d);
   else if (take) enqueue_decode_stage<false, true, false, true>(ln, d);
   else if (filt) enqueue_decode_stage<false, true>(ln, d);
   else enqueue_decode_stage<false>(ln, d);
@@ -3693,6 +3700,271 @@ PcoB200Error pco_b200_take_files_async_result(const PcoB200AsyncFilesTakeStatus*
     return tk_result(kind, s->device_status, s->n_positions, s->position, s->n_written);
   const PcoB200AsyncFilesFilterStatus f{s->kind, s->device_status, s->file, s->chunk, s->n_written, s->n_files, 0, 0};
   return pco_b200_filter_files_async_result(&f, nullptr);  // the files filter's words: rows_cap in the role of dst_cap
+}
+
+// ---- asynchronous segment aggregates of wrapped pages and of indexed files (pco_b200_segment_aggregate_pages_async,
+// pco_b200_segment_aggregate_files_async; kernels in async_segment_aggregate_kernels.cuh).  The decompress call's launches (enqueue_pages /
+// enqueue_files with the decode stage's segment-mode instantiations and rows_cap as dst_cap; for files behind ff_map_kernel) with the
+// plan between the front end and the decode stage: the front kernel, the bound checks and copy, the marks (and, for pages, the cold list
+// kept to the touched pages); then the cold reduction, the group kernels and the finish.  Memsets clear the records and the long list.
+
+// The segment plan, enqueued between the front end and the decode stage; `front` writes the SgState.
+static void enqueue_segment_plan(const AsyncLaunch& ln, const std::function<void()>& front, const uint64_t* bounds, const PcoB200Interval* interval,
+                                 uint64_t max_segments, const IndexChunk* recs, uint64_t max_records, SgState* ss, const FiltStage& filt) {
+  const cudaStream_t stream = ln.stream;
+  uint64_t* copy = const_cast<uint64_t*>(filt.interval);
+  front();
+  ln.begin("sg_check_kernel");
+  sg_check_kernel<<<uint32_t(std::min(ctas_of<SG_THREADS>(max_segments + 1), SG_MAX_CTAS)), SG_THREADS, 0, stream>>>(
+      bounds, reinterpret_cast<const uint64_t*>(interval), max_segments, ss, copy);
+  ln.end();
+  ln.begin("sg_mark_kernel");
+  sg_mark_kernel<<<uint32_t(std::min(max_records, SG_MAX_CTAS)), SG_THREADS, 0, stream>>>(copy, max_segments, recs, ss, filt.counts, seg_runs(filt));
+  ln.end();
+}
+
+// The group stage and the finish's grid: a warp per segment, striding.
+static uint32_t sg_group_ctas(uint64_t max_segments) {
+  return uint32_t(std::min((max_segments + SG_THREADS / 32 - 1) / (SG_THREADS / 32), SG_MAX_CTAS));
+}
+
+// The words of the segment calls' own refusals, or nullptr for any other status.
+static const char* sg_refusal(uint32_t device_status) {
+  switch (device_status) {
+    case PCO_B200_SEGMENTS_ORDER: return "bound below the bound before it (bounds must be non-decreasing)";
+    case PCO_B200_SEGMENTS_PAST: return "bound lies past the rows of the concatenation";
+    default: return nullptr;
+  }
+}
+static PcoB200Error sg_result(PcoB200Error kind, uint32_t device_status, uint64_t n_segments, uint64_t segment, uint64_t rows) {
+  if (device_status == PCO_B200_SEGMENTS_TOO_MANY)
+    return fail(kind, "*n_segments is " + std::to_string(n_segments) + ", above the plan's max_segments");
+  std::string what = "segment " + std::to_string(segment) + ": " + sg_refusal(device_status);
+  if (device_status == PCO_B200_SEGMENTS_PAST) what += " (" + std::to_string(rows) + " rows)";
+  return fail(kind, what);
+}
+
+static bool sg_plan_ok(const PcoB200AsyncSegmentAggregatePlan* p) {
+  return nt_valid(p->dtype) && p->max_pages >= 1 && p->max_pages <= 0x7fffffffull && p->rows_cap <= (uint64_t(1) << 56) &&
+         p->frame_cap <= (uint64_t(1) << 56) && p->max_segments >= 1 && p->max_segments <= 0x7fffffffull &&
+         p->workspace_bytes == sg_layout(p->max_pages, p->rows_cap, p->frame_cap, p->max_segments, nt_bits(p->dtype) / 8).sg_total;
+}
+
+PcoB200Error pco_b200_segment_aggregate_pages_async_plan(unsigned char dtype, size_t metas_cap, size_t pages_cap, size_t max_pages, size_t rows_cap,
+                                                         size_t frame_cap, size_t max_segments, PcoB200AsyncSegmentAggregatePlan* plan) {
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (!plan) return fail(PCO_B200_INVALID_ARGUMENT, "null plan");
+  if (max_pages == 0 || uint64_t(max_pages) > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_pages must be 1 .. 2^31 - 1");
+  if (uint64_t(rows_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "rows_cap above 2^56 numbers");
+  if (uint64_t(frame_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "frame_cap above 2^56 bytes");
+  if (max_segments == 0 || uint64_t(max_segments) > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_segments must be 1 .. 2^31 - 1");
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->metas_cap = metas_cap;
+  plan->pages_cap = pages_cap;
+  plan->max_pages = max_pages;
+  plan->rows_cap = rows_cap;
+  plan->frame_cap = frame_cap;
+  plan->max_segments = max_segments;
+  plan->workspace_bytes = sg_layout(max_pages, rows_cap, frame_cap, max_segments, nt_bits(dtype) / 8).sg_total;
+  if (PcoB200Error e = async_decode_setup<false, true, false, false, true>(
+          dtype, [](auto tag) { return (const void*)ap_cold_kernel<decltype(tag)>; },
+          {(const void*)ap_pages_kernel, (const void*)ap_scan_kernel, (const void*)ap_place_kernel, (const void*)frame_pages_kernel,
+           (const void*)walk_kernel<SMALL_MAX_SIZE_LOG>, (const void*)ap_route_kernel, (const void*)ap_rewalk_kernel, (const void*)ap_finish_kernel,
+           (const void*)sg_front_pages_kernel, (const void*)sg_check_kernel, (const void*)sg_mark_kernel, (const void*)tk_cold_list_kernel,
+           (const void*)sg_group_kernel, (const void*)sg_long_kernel}))
+    return e;
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
+    using L = decltype(tag);
+    return load_kernels({(const void*)sg_cold_pages_kernel<L>, (const void*)sg_finish_pages_kernel<L>});
+  });
+}
+
+PcoB200Error pco_b200_segment_aggregate_pages_async(const PcoB200AsyncSegmentAggregatePlan* plan, const void* metas, const void* pages,
+                                                    const PcoB200PageRef* refs, const uint64_t* n_pages, const uint64_t* bounds,
+                                                    const uint64_t* n_segments, const PcoB200Interval* interval, PcoB200Aggregate* aggs,
+                                                    PcoB200Aggregate* total, void* workspace, PcoB200AsyncSegmentAggregateStatus* status,
+                                                    void* cuda_stream) {
+  if (!plan || !metas || !pages || !refs || !n_pages || !bounds || !n_segments || !interval || !aggs || !total || !workspace || !status)
+    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (!sg_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_segment_aggregate_pages_async_plan");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+  const cudaStream_t stream = ln.stream;
+
+  const uint32_t mp = uint32_t(plan->max_pages);
+  const uint64_t ms = plan->max_segments;
+  const SgLayout lay = sg_layout(mp, plan->rows_cap, plan->frame_cap, ms, nt_bits(plan->dtype) / 8);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  const ApArgs g{static_cast<const uint8_t*>(metas), static_cast<const uint8_t*>(pages), refs, n_pages, plan->metas_cap, plan->pages_cap, plan->rows_cap,
+                 plan->frame_cap, plan->dtype, mp};
+  // segment mode: the interval and bounds copy travels in FiltStage's interval pointer, the touched flags in counts, the records in
+  // rows, the runs in offs
+  const FiltStage filt{reinterpret_cast<const uint64_t*>(ws + lay.bounds), reinterpret_cast<const uint32_t*>(ws + lay.fast_page),
+                       reinterpret_cast<uint32_t*>(ws + lay.touched), reinterpret_cast<uint64_t*>(ws + lay.recs), ws + lay.runs};
+  auto* state = reinterpret_cast<ApState*>(ws + lay.state);
+  auto* recs = reinterpret_cast<const IndexChunk*>(ws + lay.index);
+  auto* cold_list = reinterpret_cast<uint32_t*>(ws + lay.cold_list);
+  auto* pstatus = reinterpret_cast<PcoB200AsyncPagesStatus*>(ws + lay.pstatus);
+  auto* ss = reinterpret_cast<SgState*>(ws + lay.sstate);
+  auto* groups = reinterpret_cast<AgGroup*>(ws + lay.groups);
+  auto* longs = reinterpret_cast<SgLong*>(ws + lay.longs);
+
+  PCOB_CUDA_TRY(cudaMemsetAsync(seg_recs(filt), 0, sg_records(fl_slots(mp, plan->rows_cap), ms) * sizeof(SegRec), stream));
+  PCOB_CUDA_TRY(cudaMemsetAsync(longs, 0, sizeof(SgLong), stream));
+  enqueue_pages(ln, g, lay, ws, ws + lay.stage, &filt, pstatus, false, false, [&] {
+    auto front = [&] {
+      ln.begin("sg_front_pages_kernel");
+      sg_front_pages_kernel<<<1, 32, 0, stream>>>(state, n_segments, ss);
+      ln.end();
+    };
+    enqueue_segment_plan(ln, front, bounds, interval, ms, recs, mp, ss, filt);
+    ln.begin("tk_cold_list_kernel");
+    tk_cold_list_kernel<<<1, TK_SCAN_THREADS, 0, stream>>>(state, cold_list, filt.counts);
+    ln.end();
+  }, true);
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    ln.begin("sg_cold_pages_kernel");
+    sg_cold_pages_kernel<L><<<mp, SG_THREADS, 0, stream>>>(state, recs, cold_list, filt, plan->dtype, reinterpret_cast<const L*>(ws + lay.stage));
+    ln.end();
+    ln.begin("sg_group_kernel");
+    sg_group_kernel<<<sg_group_ctas(ms), SG_THREADS, 0, stream>>>(&pstatus->kind, ss, ms, filt.interval, recs, seg_recs(filt), plan->dtype, groups,
+                                                                  longs);
+    ln.end();
+    ln.begin("sg_long_kernel");
+    sg_long_kernel<<<SG_LONG_CTAS, AG_THREADS, 0, stream>>>(&pstatus->kind, ss, ms, longs, seg_recs(filt), plan->dtype, groups);
+    ln.end();
+    ln.begin("sg_finish_pages_kernel");
+    sg_finish_pages_kernel<L><<<1, AG_THREADS, 0, stream>>>(pstatus, ss, ms, filt.interval, groups, plan->dtype, aggs, total, status);
+    ln.end();
+    return 0;
+  });
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
+}
+
+PcoB200Error pco_b200_segment_aggregate_pages_async_result(const PcoB200AsyncSegmentAggregateStatus* s, size_t* n_matches) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200Error kind = async_result_kind(s->kind);
+  if (kind != PCO_B200_OK && (s->device_status == PCO_B200_SEGMENTS_TOO_MANY || sg_refusal(s->device_status)))
+    return sg_result(kind, s->device_status, s->n_segments, s->segment, s->n_written);
+  const PcoB200AsyncFilterStatus f{s->kind, s->device_status, s->page, s->n_written, s->n_pages, s->frames_needed, s->n_matches, s->n_matches};
+  return pco_b200_filter_pages_async_result(&f, n_matches);  // the pages filter's words: rows_cap in the role of dst_cap
+}
+
+static bool sgf_plan_ok(const PcoB200AsyncFilesSegmentAggregatePlan* p) {
+  return nt_valid(p->dtype) && p->max_files >= 1 && p->max_files <= 0x7fffffffull && p->max_chunks >= 1 && p->max_chunks <= 0xffffffffull &&
+         p->rows_cap <= (uint64_t(1) << 56) && p->max_segments >= 1 && p->max_segments <= 0x7fffffffull &&
+         p->workspace_bytes == sgf_layout(p->max_files, p->max_chunks, p->rows_cap, p->max_segments, nt_bits(p->dtype) / 8).sgf_total;
+}
+
+PcoB200Error pco_b200_segment_aggregate_files_async_plan(const void* head, size_t head_len, unsigned char dtype, size_t src_cap, size_t index_cap,
+                                                         size_t max_files, size_t max_chunks, size_t rows_cap, size_t max_segments,
+                                                         PcoB200AsyncFilesSegmentAggregatePlan* plan) {
+  StandaloneHeader hdr;
+  if (PcoB200Error e = check_async_head(head, head_len, dtype, plan, &hdr)) return e;
+  if (max_files == 0 || uint64_t(max_files) > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_files must be 1 .. 2^31 - 1");
+  if (max_chunks == 0 || uint64_t(max_chunks) > 0xffffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_chunks must be 1 .. 2^32 - 1");
+  if (uint64_t(rows_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "rows_cap above 2^56 numbers");
+  if (max_segments == 0 || uint64_t(max_segments) > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_segments must be 1 .. 2^31 - 1");
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->uniform_type = hdr.uniform_type;
+  plan->format_major = hdr.format_major;
+  plan->src_cap = src_cap;
+  plan->index_cap = index_cap;
+  plan->max_files = max_files;
+  plan->max_chunks = max_chunks;
+  plan->rows_cap = rows_cap;
+  plan->max_segments = max_segments;
+  plan->workspace_bytes = sgf_layout(max_files, max_chunks, rows_cap, max_segments, nt_bits(dtype) / 8).sgf_total;
+  if (PcoB200Error e = async_decode_setup<false, true, false, false, true>(
+          dtype, [](auto tag) { return (const void*)cold_chunks_kernel<decltype(tag)>; },
+          {(const void*)af_files_kernel, (const void*)check_index_kernel, (const void*)af_scan_kernel, (const void*)af_place_kernel,
+           (const void*)af_table_kernel, (const void*)merge_index_kernel, (const void*)af_finish_kernel, (const void*)ff_map_kernel,
+           (const void*)ff_cold_list_kernel, (const void*)sg_front_files_kernel, (const void*)sg_check_kernel, (const void*)sg_mark_kernel,
+           (const void*)sg_group_kernel, (const void*)sg_long_kernel}))
+    return e;
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
+    using L = decltype(tag);
+    return load_kernels({(const void*)sg_cold_files_kernel<L>, (const void*)sg_finish_files_kernel<L>});
+  });
+}
+
+PcoB200Error pco_b200_segment_aggregate_files_async(const PcoB200AsyncFilesSegmentAggregatePlan* plan, const void* src, const void* index,
+                                                    const PcoB200FileRef* files, const uint64_t* n_files, const uint64_t* bounds,
+                                                    const uint64_t* n_segments, const PcoB200Interval* interval, PcoB200Aggregate* aggs,
+                                                    PcoB200Aggregate* total, void* workspace, PcoB200AsyncFilesSegmentAggregateStatus* status,
+                                                    void* cuda_stream) {
+  if (!plan || !src || !index || !files || !n_files || !bounds || !n_segments || !interval || !aggs || !total || !workspace || !status)
+    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (!sgf_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_segment_aggregate_files_async_plan");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+  const cudaStream_t stream = ln.stream;
+
+  const uint32_t mf = uint32_t(plan->max_files), mc = uint32_t(plan->max_chunks);
+  const uint64_t ms = plan->max_segments;
+  const SgfLayout lay = sgf_layout(mf, mc, plan->rows_cap, ms, nt_bits(plan->dtype) / 8);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  const AfArgs g{FileParams{src, plan->src_cap, plan->dtype, plan->uniform_type, plan->format_major}, static_cast<const uint8_t*>(index),
+                 plan->index_cap, plan->rows_cap, files, n_files, mf, mc};
+  // segment mode: as the pages call, with the slot map in place of fast_page
+  const FiltStage filt{reinterpret_cast<const uint64_t*>(ws + lay.bounds), reinterpret_cast<const uint32_t*>(ws + lay.slot_map),
+                       reinterpret_cast<uint32_t*>(ws + lay.touched), reinterpret_cast<uint64_t*>(ws + lay.recs), ws + lay.runs};
+  auto* fstatus = reinterpret_cast<PcoB200AsyncFilesStatus*>(ws + lay.fstatus);
+  auto* ss = reinterpret_cast<SgState*>(ws + lay.sstate);
+  auto* cold_list = reinterpret_cast<uint32_t*>(ws + lay.cold_list);
+  auto* table = reinterpret_cast<const IndexChunk*>(ws + lay.table);
+  auto* afstate = reinterpret_cast<const AfState*>(ws + lay.state);
+  auto* groups = reinterpret_cast<AgGroup*>(ws + lay.groups);
+  auto* longs = reinterpret_cast<SgLong*>(ws + lay.longs);
+
+  PCOB_CUDA_TRY(cudaMemsetAsync(seg_recs(filt), 0, sg_records(fl_slots(mc, plan->rows_cap), ms) * sizeof(SegRec), stream));
+  PCOB_CUDA_TRY(cudaMemsetAsync(longs, 0, sizeof(SgLong), stream));
+  ln.begin("ff_map_kernel");
+  ff_map_kernel<<<uint32_t(ctas_of<FF_THREADS>(mc)), FF_THREADS, 0, stream>>>(mc, reinterpret_cast<uint32_t*>(ws + lay.slot_map), cold_list);
+  ln.end();
+  enqueue_files(ln, g, lay, ws, ws + lay.stage, &filt, cold_list, nullptr, fstatus, false, false, [&] {
+    auto front = [&] {
+      ln.begin("sg_front_files_kernel");
+      sg_front_files_kernel<<<1, 32, 0, stream>>>(afstate, reinterpret_cast<const AsyncCheck*>(ws), n_segments, ss);
+      ln.end();
+    };
+    enqueue_segment_plan(ln, front, bounds, interval, ms, table, mc, ss, filt);
+  }, true);
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    ln.begin("sg_cold_files_kernel");
+    sg_cold_files_kernel<L><<<std::min(mc, uint32_t(FF_COLD_CTAS)), SG_THREADS, 0, stream>>>(cold_list, table, reinterpret_cast<const uint32_t*>(ws + lay.st),
+                                                                                             filt, plan->dtype, reinterpret_cast<const L*>(ws + lay.stage));
+    ln.end();
+    ln.begin("sg_group_kernel");
+    sg_group_kernel<<<sg_group_ctas(ms), SG_THREADS, 0, stream>>>(&fstatus->kind, ss, ms, filt.interval, table, seg_recs(filt), plan->dtype, groups,
+                                                                  longs);
+    ln.end();
+    ln.begin("sg_long_kernel");
+    sg_long_kernel<<<SG_LONG_CTAS, AG_THREADS, 0, stream>>>(&fstatus->kind, ss, ms, longs, seg_recs(filt), plan->dtype, groups);
+    ln.end();
+    ln.begin("sg_finish_files_kernel");
+    sg_finish_files_kernel<L><<<1, AG_THREADS, 0, stream>>>(fstatus, ss, ms, filt.interval, groups, plan->dtype, aggs, total, status);
+    ln.end();
+    return 0;
+  });
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
+}
+
+PcoB200Error pco_b200_segment_aggregate_files_async_result(const PcoB200AsyncFilesSegmentAggregateStatus* s, size_t* n_matches) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200Error kind = async_result_kind(s->kind);
+  if (kind != PCO_B200_OK && (s->device_status == PCO_B200_SEGMENTS_TOO_MANY || sg_refusal(s->device_status)))
+    return sg_result(kind, s->device_status, s->n_segments, s->segment, s->n_written);
+  const PcoB200AsyncFilesFilterStatus f{s->kind, s->device_status, s->file, s->chunk, s->n_written, s->n_files, s->n_matches, s->n_matches};
+  return pco_b200_filter_files_async_result(&f, n_matches);  // the files filter's words: rows_cap in the role of dst_cap
 }
 
 // ---- asynchronous compress (pco_b200_compress_async; gate kernels in async_compress.cuh).  The plan fixes the layout and the config;

@@ -985,6 +985,81 @@ class AsyncFilesTake(_lib._AsyncCall):
         return int(nw.value)
 
 
+class _CAsyncFilesSegmentAggregatePlan(C.Structure):  # PcoB200AsyncFilesSegmentAggregatePlan (include/pco_b200.h)
+    _fields_ = [("dtype", C.c_uint32), ("uniform_type", C.c_uint32), ("format_major", C.c_uint32), ("reserved", C.c_uint32),
+                ("src_cap", C.c_uint64), ("index_cap", C.c_uint64), ("max_files", C.c_uint64), ("max_chunks", C.c_uint64),
+                ("rows_cap", C.c_uint64), ("max_segments", C.c_uint64), ("workspace_bytes", C.c_uint64)]
+
+
+class _CAsyncFilesSegmentAggregateStatus(C.Structure):  # PcoB200AsyncFilesSegmentAggregateStatus (include/pco_b200.h)
+    _fields_ = [("kind", C.c_uint32), ("device_status", C.c_uint32), ("file", C.c_uint64), ("chunk", C.c_uint64), ("n_written", C.c_uint64),
+                ("n_files", C.c_uint64), ("n_segments", C.c_uint64), ("segment", C.c_uint64), ("records_decoded", C.c_uint64),
+                ("n_matches", C.c_uint64)]
+
+
+def _lib_async_segment_aggregate_files():
+    return _lib.bind("_async_segment_aggregate_files_ready",
+                     pco_b200_segment_aggregate_files_async_plan=[C.c_void_p, C.c_size_t, C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t,
+                                                                  C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p],
+                     pco_b200_segment_aggregate_files_async=[C.c_void_p] * 13,
+                     pco_b200_segment_aggregate_files_async_result=[C.c_void_p, C.POINTER(C.c_size_t)])
+
+
+class AsyncFilesSegmentAggregate(_lib._AsyncCall):
+    """Decodes a batch of indexed standalone files on the current CUDA stream and reduces the numbers inside a closed interval to count,
+    min, max and sum per row segment [bounds[g], bounds[g + 1]) of the files' concatenation and in all
+    (pco_b200_segment_aggregate_files_async), decoding only the chunks the segments cover.  Refs, their count, the bounds, their count and
+    the interval are read from device tensors, so one captured call serves new files and new segments on each replay.
+
+    The plan and capacities are AsyncFilesAggregate's, with max_segments the most segments a call reduces.  The call owns a device workspace
+    (about rows_cap * (itemsize + 0.2) + 96 * max_segments bytes beyond the decompressor's) and a status; it serves one call in flight.
+    wrapped.unpack_aggregates reads the records."""
+
+    _Plan, _Status = _CAsyncFilesSegmentAggregatePlan, _CAsyncFilesSegmentAggregateStatus
+
+    def __init__(self, head, dtype, src_cap, index_cap, max_files, max_chunks, rows_cap, max_segments, device=None):
+        self.dtype = np.dtype(dtype)
+        h = self._head(head)
+        self._make_plan(device, lambda plan: _lib_async_segment_aggregate_files().pco_b200_segment_aggregate_files_async_plan(
+            h.ctypes.data_as(C.c_void_p), C.c_size_t(h.size), C.c_ubyte(_lib.dtype_byte(self.dtype)), C.c_size_t(src_cap), C.c_size_t(index_cap),
+            C.c_size_t(max_files), C.c_size_t(max_chunks), C.c_size_t(rows_cap), C.c_size_t(max_segments), plan))
+        self._alloc()
+
+    def __call__(self, src, index, files, n_files, bounds, n_segments, interval, aggs, total):
+        """Enqueues the segment aggregates of files[: n_files[0]] on torch.cuda.current_stream().  `src`, `index`, `files` and `n_files`
+        are as AsyncFilesDecompressor takes them; `bounds`, `n_segments`, `interval`, `aggs` and `total` are as
+        wrapped.AsyncPagesSegmentAggregate takes them, the bounds indexing the files' concatenation.  Returns nothing and does not wait;
+        result() reports the outcome."""
+        import torch
+
+        from .wrapped import _check_segment_tensors
+
+        p = self._plan
+        self._check_tensors(src=src, index=index, files=files, n_files=n_files, bounds=bounds, n_segments=n_segments, interval=interval,
+                            aggs=aggs, total=total)
+        if src.numel() * src.element_size() < p.src_cap or index.numel() * index.element_size() < p.index_cap:
+            raise ValueError(f"src holds fewer than src_cap = {p.src_cap} bytes, or index fewer than index_cap = {p.index_cap}")
+        if files.dtype != torch.int64 or files.dim() != 2 or files.shape[1] != 4 or files.shape[0] < p.max_files:
+            raise ValueError(f"files must be an int64 tensor of shape ({p.max_files}, 4)")
+        if n_files.dtype != torch.int64 or n_files.numel() != 1:
+            raise ValueError("n_files must be a 1-element int64 tensor")
+        _check_segment_tensors(bounds, n_segments, interval, aggs, total, p.max_segments)
+        rc = _lib_async_segment_aggregate_files().pco_b200_segment_aggregate_files_async(
+            C.byref(p), C.c_void_p(src.data_ptr()), C.c_void_p(index.data_ptr()), C.c_void_p(files.data_ptr()), C.c_void_p(n_files.data_ptr()),
+            C.c_void_p(bounds.data_ptr()), C.c_void_p(n_segments.data_ptr()), C.c_void_p(interval.data_ptr()), C.c_void_p(aggs.data_ptr()),
+            C.c_void_p(total.data_ptr()), C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()), self._stream())
+        _lib.check(rc)
+
+    def result(self):
+        """Copies the status of the last call back (waiting for it on the current stream) and returns the total match count, or raises
+        PcoError with the kind pco_b200_decompress_files gives ("file 3: chunk 2: ...") or, for the bounds, InvalidArgument
+        ("segment 17: ...")."""
+        s = self.status_record()
+        nm = C.c_size_t()
+        _lib.check(_lib_async_segment_aggregate_files().pco_b200_segment_aggregate_files_async_result(C.byref(s), C.byref(nm)))
+        return int(nm.value)
+
+
 class _CAsyncCompressFilesPlan(C.Structure):  # PcoB200AsyncCompressFilesPlan (include/pco_b200.h)
     _fields_ = [("dtype", C.c_uint32), ("uniform_type_header", C.c_uint32), ("mode", C.c_uint32), ("order", C.c_uint32),
                 ("n_vars", C.c_uint32), ("level", C.c_uint32), ("mode_k", C.c_uint32), ("reserved", C.c_uint32),

@@ -638,6 +638,93 @@ class AsyncPagesTake(_lib._AsyncCall):
         return int(nw.value)
 
 
+class _CAsyncSegmentAggregatePlan(C.Structure):  # PcoB200AsyncSegmentAggregatePlan (include/pco_b200.h)
+    _fields_ = [("dtype", C.c_uint32), ("reserved", C.c_uint32), ("metas_cap", C.c_uint64), ("pages_cap", C.c_uint64), ("max_pages", C.c_uint64),
+                ("rows_cap", C.c_uint64), ("frame_cap", C.c_uint64), ("max_segments", C.c_uint64), ("workspace_bytes", C.c_uint64)]
+
+
+class _CAsyncSegmentAggregateStatus(C.Structure):  # PcoB200AsyncSegmentAggregateStatus (include/pco_b200.h)
+    _fields_ = [("kind", C.c_uint32), ("device_status", C.c_uint32), ("page", C.c_uint64), ("n_written", C.c_uint64), ("n_pages", C.c_uint64),
+                ("frames_needed", C.c_uint64), ("n_segments", C.c_uint64), ("segment", C.c_uint64), ("records_decoded", C.c_uint64),
+                ("n_matches", C.c_uint64)]
+
+
+def _lib_async_segment_aggregate():
+    return _lib.bind("_async_segment_aggregate_ready",
+                     pco_b200_segment_aggregate_pages_async_plan=[C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                                                  C.c_size_t, C.c_void_p],
+                     pco_b200_segment_aggregate_pages_async=[C.c_void_p] * 13,
+                     pco_b200_segment_aggregate_pages_async_result=[C.c_void_p, C.POINTER(C.c_size_t)])
+
+
+def _check_segment_tensors(bounds, n_segments, interval, aggs, total, max_segments):
+    import torch
+
+    if bounds.dtype != torch.int64 or bounds.numel() < max_segments + 1:
+        raise ValueError(f"bounds must be an int64 tensor of at least max_segments + 1 = {max_segments + 1} elements")
+    if n_segments.dtype != torch.int64 or n_segments.numel() != 1:
+        raise ValueError("n_segments must be a 1-element int64 tensor")
+    if interval.dtype != torch.int64 or interval.numel() != 2:
+        raise ValueError("interval must be a 2-element int64 tensor")
+    _check_aggregate_outputs(aggs, total, max_segments)
+
+
+class AsyncPagesSegmentAggregate(_lib._AsyncCall):
+    """Decodes a batch of wrapped-format pages on the current CUDA stream and reduces the numbers inside a closed interval to count, min,
+    max and sum per row segment [bounds[g], bounds[g + 1]) of the pages' concatenation and in all (pco_b200_segment_aggregate_pages_async):
+    time buckets, per-session ranges or a window's rows, with only the pages the segments cover decoded and each 256-number batch reduced
+    in the decoder's registers.  Refs, their count, the bounds, their count and the interval are read from device tensors, so one captured
+    call serves new pages and new segments on each replay, and torch.searchsorted's output can be passed straight in.
+
+    The capacities are AsyncPagesAggregate's, with max_segments the most segments a call reduces.  The call owns a device workspace (about
+    rows_cap * (itemsize + 0.2) + 96 * max_segments bytes beyond the decompressor's) and a status; it serves one call in flight.
+    unpack_aggregates reads the records."""
+
+    _Plan, _Status = _CAsyncSegmentAggregatePlan, _CAsyncSegmentAggregateStatus
+
+    def __init__(self, dtype, metas_cap, pages_cap, max_pages, rows_cap, max_segments, frame_cap=None, device=None):
+        self.dtype = np.dtype(dtype)
+        if frame_cap is None:
+            frame_cap = metas_cap + pages_cap + 20 * max_pages
+        self._make_plan(device, lambda plan: _lib_async_segment_aggregate().pco_b200_segment_aggregate_pages_async_plan(
+            C.c_ubyte(_lib.dtype_byte(self.dtype)), C.c_size_t(metas_cap), C.c_size_t(pages_cap), C.c_size_t(max_pages), C.c_size_t(rows_cap),
+            C.c_size_t(frame_cap), C.c_size_t(max_segments), plan))
+        self._alloc()
+
+    def __call__(self, metas, pages, refs, n_pages, bounds, n_segments, interval, aggs, total):
+        """Enqueues the segment aggregates of the pages refs[: n_pages[0]] names on torch.cuda.current_stream().  `metas`, `pages`, `refs`
+        and `n_pages` are as AsyncPagesDecompressor takes them; `bounds` is an int64 CUDA tensor of at least max_segments + 1 elements
+        (non-decreasing row indices into the pages' concatenation), `n_segments` a 1-element int64 CUDA tensor, `interval` a 2-element
+        int64 CUDA tensor (pack_interval's bit patterns of lo and hi), `aggs` an int64 CUDA tensor of shape (max_segments, 6) whose row g
+        receives segment g's PcoB200Aggregate, and `total` a 6-element int64 CUDA tensor that receives the total.  Returns nothing and
+        does not wait; result() reports the outcome."""
+        import torch
+
+        p = self._plan
+        self._check_tensors(metas=metas, pages=pages, refs=refs, n_pages=n_pages, bounds=bounds, n_segments=n_segments, interval=interval,
+                            aggs=aggs, total=total)
+        if metas.numel() * metas.element_size() < p.metas_cap or pages.numel() * pages.element_size() < p.pages_cap:
+            raise ValueError(f"metas holds fewer than metas_cap = {p.metas_cap} bytes, or pages fewer than pages_cap = {p.pages_cap}")
+        if refs.dtype != torch.int64 or refs.dim() != 2 or refs.shape[1] != 5 or refs.shape[0] < p.max_pages:
+            raise ValueError(f"refs must be an int64 tensor of shape ({p.max_pages}, 5)")
+        if n_pages.dtype != torch.int64 or n_pages.numel() != 1:
+            raise ValueError("n_pages must be a 1-element int64 tensor")
+        _check_segment_tensors(bounds, n_segments, interval, aggs, total, p.max_segments)
+        rc = _lib_async_segment_aggregate().pco_b200_segment_aggregate_pages_async(
+            C.byref(p), C.c_void_p(metas.data_ptr()), C.c_void_p(pages.data_ptr()), C.c_void_p(refs.data_ptr()), C.c_void_p(n_pages.data_ptr()),
+            C.c_void_p(bounds.data_ptr()), C.c_void_p(n_segments.data_ptr()), C.c_void_p(interval.data_ptr()), C.c_void_p(aggs.data_ptr()),
+            C.c_void_p(total.data_ptr()), C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()), self._stream())
+        _lib.check(rc)
+
+    def result(self):
+        """Copies the status of the last call back (waiting for it on the current stream) and returns the total match count, or raises
+        PcoError with the kind decompress_pages gives ("page 17: ...") or, for the bounds, InvalidArgument ("segment 17: ...")."""
+        s = self.status_record()
+        nm = C.c_size_t()
+        _lib.check(_lib_async_segment_aggregate().pco_b200_segment_aggregate_pages_async_result(C.byref(s), C.byref(nm)))
+        return int(nm.value)
+
+
 class AsyncPagesFilter(_lib._AsyncCall):
     """Decodes a batch of wrapped-format pages on the current CUDA stream and writes only the numbers inside a closed interval, in row order,
     with their positions in the pages' concatenation (pco_b200_filter_pages_async): the predicate runs inside the decoder, so the decoded
