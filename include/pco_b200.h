@@ -1353,6 +1353,125 @@ PcoB200Error pco_b200_segment_aggregate_files_async(const PcoB200AsyncFilesSegme
  * ("segment 17: ..."), and, when the kind is OK, sets *n_matches (may be NULL) to the total match count. */
 PcoB200Error pco_b200_segment_aggregate_files_async_result(const PcoB200AsyncFilesSegmentAggregateStatus *host_status, size_t *n_matches);
 
+/* ---- asynchronous histograms of wrapped-format pages and of indexed standalone files (no reference counterpart): how many numbers of
+ * the concatenation pco_b200_decompress_pages_async / pco_b200_decompress_files_async write fall in each of B value buckets, per page or
+ * file and in all.  Latency percentiles, heat maps, threshold counts and per-page distribution statistics come from one pass over the
+ * compressed column without the decoded numbers ever reaching HBM: each decode CTA counts its numbers in shared memory and adds its counts
+ * to its page's or file's row when it is done.  Each call only enqueues kernels on the caller's stream and returns at once; it makes no
+ * synchronising, allocating or host-to-device copy call and refers to no memory of the library's per-thread scratch, so it can be captured
+ * in a CUDA graph, and a captured call may be replayed after pco_b200_thread_release or after any other call.  A plan made once outside any
+ * capture fixes the grids and B from its capacities; the refs, their count and the edges are read on the device, so one captured graph
+ * serves new pages or files and new edges on each replay.
+ * edges (uint64_t[B + 1]) holds the bucket edges e_0 < e_1 < ... < e_B as zero-extended bit patterns of the plan's number type, the
+ * encoding PcoB200Interval uses.  Each group's row has W = B + 3 uint64_t counts:
+ *   [0]      x < e_0;
+ *   [1 + b]  e_b <= x < e_{b+1}, for b < B - 1, and e_{B-1} <= x <= e_B for the last bucket (numpy's and torch's convention);
+ *   [B + 1]  x > e_B;
+ *   [B + 2]  x is a NaN.
+ * So a row always sums to its group's numbers.  Numbers compare as the filter calls compare them: integers in their signed or unsigned
+ * order, floats as IEEE values (-0.0 equals +0.0; -inf and +inf are ordinary numbers and valid edges; a NaN of any payload or sign goes to
+ * column B + 2 only).  hists[g * W ..] is page g (pages call) or file g (files call) for g below *n_pages / *n_files; rows past it are not
+ * written.  *total (W counts) is the column sum of those rows.
+ * Refusals, in this order, each decided before any page or chunk is decoded; on a refusal or failure *total is written as all zeros and
+ * hists is not written:
+ *   1. the decompress call's refusals before its decode stage, in its order, with its kinds and naming the same page, or file and chunk:
+ *      for pages every check up to and including the walk of every page, for files every check up to and including placement
+ *      (PCO_B200_ASYNC_PAGES_DST / PCO_B200_ASYNC_FILES_DST against rows_cap);
+ *   2. the lowest j whose edge is a NaN, or is not strictly above edge j - 1 (PCO_B200_HIST_EDGES_ORDER, edge j).  Since -0.0 and +0.0 are
+ *      equal, -0.0 followed by +0.0 is refused.
+ * Then every page or chunk is decoded; a decode failure is reported as the decompress call reports it. */
+enum {
+  PCO_B200_HIST_EDGES_ORDER = 0x501  /* edges[edge] is a NaN, or not above edges[edge - 1] (PCO_B200_INVALID_ARGUMENT) */
+};
+
+typedef struct PcoB200AsyncHistogramPlan {  /* filled by pco_b200_histogram_pages_async_plan; treat as opaque */
+  uint32_t dtype, reserved;
+  uint64_t metas_cap, pages_cap, max_pages, rows_cap, frame_cap, n_buckets;
+  uint64_t workspace_bytes;                 /* device workspace one in-flight call needs */
+} PcoB200AsyncHistogramPlan;
+
+typedef struct PcoB200AsyncHistogramStatus {  /* written on the device by every call */
+  uint32_t kind;                              /* PcoB200Error */
+  uint32_t device_status;                     /* the device word behind it: as PcoB200AsyncPagesStatus, or PCO_B200_HIST_EDGES_ORDER */
+  uint64_t page;                              /* the page the outcome names (UINT64_MAX if none) */
+  uint64_t n_written;                         /* the rows of the concatenation (the sum of page_n), once every page passed its checks (0 on
+                                                 a failure of the pages call) */
+  uint64_t n_pages;                           /* *n_pages as the call read it */
+  uint64_t frames_needed;                     /* bytes of framed pages the batch needs, also when above frame_cap (0 when refused earlier) */
+  uint64_t edge;                              /* the edge index a PCO_B200_HIST_EDGES_ORDER refusal names (UINT64_MAX if none) */
+} PcoB200AsyncHistogramStatus;
+
+/* Makes a plan for histograms of n_buckets buckets over up to max_pages pages of dtype, whose refs point into metas_cap bytes of metas and
+ * pages_cap bytes of pages, holding at most rows_cap numbers in all (the role dst_cap plays in pco_b200_decompress_pages_async); frame_cap
+ * bounds the framed pages as in that call.  Checked before the device is touched: dtype (PCO_B200_INVALID_TYPE), max_pages in
+ * 1 .. 2^31 - 1, rows_cap and frame_cap at most 2^56, n_buckets in 1 .. 4096 (PCO_B200_INVALID_ARGUMENT).  Then *plan is filled and the
+ * one-time device set-up runs on the current device, which the calls must use (kernel attributes, and every kernel the call launches
+ * loaded); without a device that is PCO_B200_CUDA.
+ * workspace_bytes is pco_b200_decompress_pages_async_plan's formula with dst_cap = rows_cap, plus these regions, each rounded up to 256
+ * bytes, with W = n_buckets + 3 and E the bytes of a number of dtype: 40 (the pages status), 16 (the plan's state), 4 max_pages (each
+ * page's group), 8 (n_buckets + 2) (the edge table), E rows_cap (the cold pages' values), 8 W max_pages (the pages' rows) and 8 W (the
+ * column sums). */
+PcoB200Error pco_b200_histogram_pages_async_plan(unsigned char dtype, size_t metas_cap, size_t pages_cap, size_t max_pages, size_t rows_cap,
+                                                 size_t frame_cap, size_t n_buckets, PcoB200AsyncHistogramPlan *plan);
+/* Enqueues the histograms of the pages refs[0 : *n_pages) names on `cuda_stream`, and the outcome into *status; returns without waiting.
+ * metas (metas_cap bytes), pages (pages_cap bytes; may be the same buffer as metas), refs (PcoB200PageRef[max_pages]), n_pages (one
+ * uint64_t), edges (uint64_t[n_buckets + 1]), hists (uint64_t[max_pages * W]), total (uint64_t[W]), workspace (plan->workspace_bytes,
+ * 256-byte aligned) and status are device pointers; one workspace serves one call in flight.  The numbers counted are the concatenation
+ * pco_b200_decompress_pages_async writes for the same arguments with dst_cap = rows_cap.  The return value covers the host side only: null
+ * pointers, an unaligned workspace or a plan that was not filled (PCO_B200_INVALID_ARGUMENT), a launch the runtime refuses (PCO_B200_CUDA).
+ * With pco_b200_profile_enable(1), a call outside a stream capture records its kernel spans for pco_b200_profile_last; a call inside a
+ * capture records none. */
+PcoB200Error pco_b200_histogram_pages_async(const PcoB200AsyncHistogramPlan *plan, const void *metas, const void *pages, const PcoB200PageRef *refs,
+                                            const uint64_t *n_pages, const uint64_t *edges, uint64_t *hists, uint64_t *total, void *workspace,
+                                            PcoB200AsyncHistogramStatus *status, void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory at a point of the caller's choosing.  Returns the kind,
+ * sets the last-error message as pco_b200_aggregate_pages_async_result words it ("page 17: ...") or, for the edge refusal, naming the
+ * edge index ("edge 3: ..."), and, when the kind is OK, sets *n_rows (may be NULL) to the numbers counted (the sum of *total). */
+PcoB200Error pco_b200_histogram_pages_async_result(const PcoB200AsyncHistogramStatus *host_status, size_t *n_rows);
+
+typedef struct PcoB200AsyncFilesHistogramPlan {  /* filled by pco_b200_histogram_files_async_plan; treat as opaque */
+  uint32_t dtype, uniform_type, format_major, reserved;
+  uint64_t src_cap, index_cap, max_files, max_chunks, rows_cap, n_buckets;
+  uint64_t workspace_bytes;                      /* device workspace one in-flight call needs */
+} PcoB200AsyncFilesHistogramPlan;
+
+typedef struct PcoB200AsyncFilesHistogramStatus {  /* written on the device by every call */
+  uint32_t kind;                                   /* PcoB200Error */
+  uint32_t device_status;                          /* the device word behind it: as PcoB200AsyncFilesStatus, or PCO_B200_HIST_EDGES_ORDER */
+  uint64_t file;                                   /* the file the outcome names (UINT64_MAX if none) */
+  uint64_t chunk;                                  /* the failing chunk, counted from that file's first chunk (UINT64_MAX if none) */
+  uint64_t n_written;                              /* the rows of the concatenation (the sum of the files' counts), once every file passed
+                                                      its checks and placement (0 before) */
+  uint64_t n_files;                                /* *n_files as the call read it */
+  uint64_t edge;                                   /* the edge index a PCO_B200_HIST_EDGES_ORDER refusal names (UINT64_MAX if none) */
+} PcoB200AsyncFilesHistogramStatus;
+
+/* Makes a plan for histograms of n_buckets buckets over up to max_files indexed files of dtype holding at most max_chunks chunks and
+ * rows_cap numbers in all (the role dst_cap plays in pco_b200_decompress_files_async).  `head`, src_cap and index_cap are those of
+ * pco_b200_decompress_files_async_plan.  Checked before the device is touched, with that plan's kinds: dtype, the header, the uniform
+ * type, max_files in 1 .. 2^31 - 1, max_chunks in 1 .. 2^32 - 1, rows_cap at most 2^56, n_buckets in 1 .. 4096
+ * (PCO_B200_INVALID_ARGUMENT).  Then *plan is filled and the one-time device set-up runs on the current device, which the calls must use;
+ * without a device that is PCO_B200_CUDA.
+ * workspace_bytes is pco_b200_decompress_files_async_plan's formula with dst_cap = rows_cap, plus these regions, each rounded up to 256
+ * bytes, with W = n_buckets + 3 and E the bytes of a number of dtype: 40 (the files status), 16 (the plan's state), 4 max_chunks (each
+ * chunk's group), 8 (n_buckets + 2) (the edge table), E rows_cap (the cold chunks' values), 4 max_chunks (slot map), 4 (max_chunks + 1)
+ * (cold list), 8 W max_files (the files' rows) and 8 W (the column sums). */
+PcoB200Error pco_b200_histogram_files_async_plan(const void *head, size_t head_len, unsigned char dtype, size_t src_cap, size_t index_cap,
+                                                 size_t max_files, size_t max_chunks, size_t rows_cap, size_t n_buckets,
+                                                 PcoB200AsyncFilesHistogramPlan *plan);
+/* Enqueues the histograms of files[0 : *n_files) on `cuda_stream`, and the outcome into *status; returns without waiting.  src (src_cap
+ * bytes), index (index_cap bytes), files (PcoB200FileRef[max_files]), n_files (one uint64_t), edges (uint64_t[n_buckets + 1]), hists
+ * (uint64_t[max_files * W]), total (uint64_t[W]), workspace (plan->workspace_bytes, 256-byte aligned) and status are device pointers; one
+ * workspace serves one call in flight.  The numbers counted are the concatenation pco_b200_decompress_files_async writes for the same
+ * arguments with dst_cap = rows_cap.  The return value covers the host side only, as for pco_b200_histogram_pages_async. */
+PcoB200Error pco_b200_histogram_files_async(const PcoB200AsyncFilesHistogramPlan *plan, const void *src, const void *index, const PcoB200FileRef *files,
+                                            const uint64_t *n_files, const uint64_t *edges, uint64_t *hists, uint64_t *total, void *workspace,
+                                            PcoB200AsyncFilesHistogramStatus *status, void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory.  Returns the kind, sets the last-error message as
+ * pco_b200_aggregate_files_async_result words it ("file 3: chunk 2: ...") or, for the edge refusal, naming the edge index ("edge 3: ..."),
+ * and, when the kind is OK, sets *n_rows (may be NULL) to the numbers counted (the sum of *total). */
+PcoB200Error pco_b200_histogram_files_async_result(const PcoB200AsyncFilesHistogramStatus *host_status, size_t *n_rows);
+
 /* ---- asynchronous batch compress into wrapped-format chunks (no reference counterpart): pco_b200_compress_wrapped over a batch of
  * arrays, with the array sizes, their count and every buffer in device memory.  A GPU writer of a container that embeds pco (a columnar
  * file whose column chunks a kernel sized, a page store) compresses every column chunk behind the step that produced it, with no copy to

@@ -1130,6 +1130,85 @@ __device__ __forceinline__ void seg_store8(const FiltStage& f, const FiltKey& k,
     if (lane == 0) seg_recs(f)[slot + g] = SegRec{total, kmin, kmax, k.kind == 2 ? uint64_t(__double_as_longlong(fs)) : lo, hi};
   }
 }
+// ---------------------------------------------------------------------------
+// Histogram mode (the HIST instantiations, both histogram calls; with FILT): each number goes to one of W = B + 3 columns of a caller-given
+// edge table, counted in CTA-private uint32 counters in dynamic shared memory behind the kernel's own (4 W bytes), which the CTA adds to its
+// group's row in the workspace when its record is done (hist_flush).  Columns: 0 below edge 0, 1 + b for edge b <= x < edge b + 1 (the
+// last bucket closed: edge B - 1 <= x <= edge B), B + 1 above edge B, B + 2 NaN.  The plan (async_histogram_kernels.cuh) stages the edge
+// table and flags the records.  FiltStage: `interval` carries the edge table (word 0: B; words 1 .. B + 1: the edges' keys, hist_key),
+// `counts` per record (by its map entry) its group + 1 (0: not decoded), `rows` the groups' rows of W uint64 counts.
+// ---------------------------------------------------------------------------
+// filt_key with -0.0 mapped to +0.0's key, so the two compare equal, as IEEE values do.
+template <typename L>
+__device__ __forceinline__ L hist_key(L x, uint32_t kind) {
+  constexpr L TOP = L(L(1) << (LT<L>::BITS - 1));
+  return filt_key<L>(kind == 2 && L(x & L(~TOP)) == 0 ? L(0) : x, kind);
+}
+template <typename L>
+__device__ __forceinline__ bool hist_is_nan(L x, uint32_t kind) {
+  constexpr L TOP = L(L(1) << (LT<L>::BITS - 1));
+  constexpr L EXP = LT<L>::BITS == 16 ? L(0x7c00u) : LT<L>::BITS == 32 ? L(0x7f800000u) : L(0x7ff0000000000000ull);
+  return kind == 2 && L(x & L(~TOP)) > EXP;
+}
+__host__ __device__ inline uint32_t hist_width(const FiltStage& f) { return uint32_t(f.interval[0]) + 3; }
+__device__ __forceinline__ FiltKey hist_fkey(uint32_t dtype) { return FiltKey{0, 0, 1u, nt_is_float(dtype) ? 2u : nt_is_signed(dtype) ? 1u : 0u}; }
+// Histogram mode's store: the lane's 8 numbers of a batch of `cnt` numbers counted into the CTA's counters hc.  Each number's column comes
+// from a branch-free lower-bound search over the B + 1 edge keys (the same steps for every lane); the warp then meets equal columns with
+// __match_any_sync, so one lane adds a whole group of equal columns by one shared-memory atomic (and a warp whose every lane holds 8 numbers
+// of one column adds them once).  All 32 lanes call it.
+template <typename L>
+__device__ __forceinline__ void hist_store8(const FiltStage& f, const FiltKey& k, uint32_t* hc, uint32_t cnt, int lane, const L (&r)[8]) {
+  constexpr uint32_t NONE = 0xffffffffu;
+  const uint64_t* __restrict__ ek = f.interval + 1;
+  const uint32_t nb = uint32_t(f.interval[0]);
+  uint64_t key[8];
+  uint32_t at[8];
+#pragma unroll
+  for (int e = 0; e < 8; e++) {
+    key[e] = uint64_t(hist_key<L>(r[e], k.kind));
+    at[e] = 0;
+  }
+  for (uint32_t n = nb + 1; n > 1;) {  // invariant per number: ek[at] <= key, or at = 0; the edges at .. at + n - 1 are left
+    const uint32_t half = n >> 1;
+#pragma unroll
+    for (int e = 0; e < 8; e++) at[e] = __ldg(ek + at[e] + half) <= key[e] ? at[e] + half : at[e];
+    n -= half;
+  }
+  uint32_t col[8];
+#pragma unroll
+  for (int e = 0; e < 8; e++) {
+    const uint64_t ka = __ldg(ek + at[e]);
+    const uint32_t c = at[e] + (ka <= key[e] ? 1u : 0u);  // the edges at or below the number
+    col[e] = uint32_t(lane * 8 + e) >= cnt ? NONE : hist_is_nan<L>(r[e], k.kind) ? nb + 2 : c == nb + 1 && ka == key[e] ? nb : c;
+  }
+  bool one = col[0] != NONE;
+#pragma unroll
+  for (int e = 1; e < 8; e++) one = one && col[e] == col[0];
+  if (__all_sync(0xffffffffu, one)) {
+    const uint32_t peers = __match_any_sync(0xffffffffu, col[0]);
+    if (lane == __ffs(peers) - 1) atomicAdd(&hc[col[0]], 8u * __popc(peers));
+    return;
+  }
+#pragma unroll
+  for (int e = 0; e < 8; e++) {
+    const uint32_t peers = __match_any_sync(0xffffffffu, col[e]);
+    if (col[e] != NONE && lane == __ffs(peers) - 1) atomicAdd(&hc[col[e]], __popc(peers));
+  }
+}
+// The CTA's counters hc added to the row of group g1 - 1, a 64-bit atomic per non-zero counter.  Threads tid .. W by nthreads.
+__device__ __forceinline__ void hist_flush(const FiltStage& f, const uint32_t* hc, uint32_t g1, int tid, int nthreads) {
+  const uint32_t w = hist_width(f);
+  unsigned long long* row = reinterpret_cast<unsigned long long*>(f.rows) + uint64_t(g1 - 1) * w;
+  for (uint32_t i = tid; i < w; i += nthreads) {
+    const uint32_t v = hc[i];
+    if (v) atomicAdd(row + i, (unsigned long long)v);
+  }
+}
+// The counters of a HIST decode kernel, behind its own shared memory, cleared.  Threads tid .. W by nthreads; a __syncthreads must follow.
+__device__ __forceinline__ void hist_clear(const FiltStage& f, uint32_t* hc, int tid, int nthreads) {
+  const uint32_t w = hist_width(f);
+  for (uint32_t i = tid; i < w; i += nthreads) hc[i] = 0;
+}
 template <typename L>
 __device__ __forceinline__ void load8(const L* __restrict__ src, L (&r)[8]) {
   if (sizeof(L) == 8) {
@@ -1407,7 +1486,9 @@ __global__ void __launch_bounds__(SW_THREADS) symwalk_kernel(FileParams fp, cons
 // AGG (with FILT): aggregate mode (agg_store8: the matches reduced per batch into filt.counts and filt.agg; out is not written).
 // TAKE (with FILT): take mode (take_store8: the numbers at the run's positions to out_values; out is not written).
 // SEG (with FILT): segment mode (seg_store8: the matches reduced per batch and segment into the SegRec records; out is not written).
-template <typename L, int NV, bool WIN = false, bool FILT = false, bool AGG = false, bool TAKE = false, bool SEG = false>
+// HIST (with FILT): histogram mode (hist_store8: each batch counted into the CTA's counters behind DecodeSmem, added to the chunk's group
+// row at the end; out is not written).
+template <typename L, int NV, bool WIN = false, bool FILT = false, bool AGG = false, bool TAKE = false, bool SEG = false, bool HIST = false>
 __global__ void __launch_bounds__(DEC_THREADS, NV == 1 ? PCOB_DEC_NV1_BLOCKS : 2)
 decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __restrict__ statuses, const uint8_t* __restrict__ index_base, uint64_t index_len,
               L* __restrict__ out, uint64_t out_len, const Binoms* __restrict__ binoms, const uint8_t* __restrict__ d_syms,
@@ -1445,6 +1526,7 @@ decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __
   for (int i = tid; i < CHAIN_RING; i += DEC_THREADS) sm.m_flag[i] = 0;
   for (int i = tid; i < 32 * MAX_ORDER; i += DEC_THREADS) sm.binom_lane8[i / MAX_ORDER][i % MAX_ORDER] = binoms->lane8[i / MAX_ORDER][i % MAX_ORDER];
   if (tid < MAX_ORDER) sm.binom_full[tid] = binoms->full[tid];
+  if constexpr (HIST) hist_clear(filt, reinterpret_cast<uint32_t*>(&sm + 1), tid, DEC_THREADS);
   __syncthreads();
   if (sm.hdr.status != ST_OK) {
     if (tid == 0) statuses[blockIdx.x] = sm.hdr.status;
@@ -1525,7 +1607,8 @@ decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __
   FiltKey fkey{};
   uint64_t fslot0 = 0;
   if constexpr (FILT) {
-    if constexpr (!TAKE) fkey = filt_bounds<L>(filt.interval, fp.dtype);
+    if constexpr (HIST) fkey = hist_fkey(fp.dtype);
+    else if constexpr (!TAKE) fkey = filt_bounds<L>(filt.interval, fp.dtype);
     fslot0 = task.out_offset / BATCH_N + filt.fast_page[blockIdx.x];
   }
   const uint64_t row0 = WIN ? wins[blockIdx.x].row0 : scratch_row0(task.out_offset, blockIdx.x);
@@ -1788,7 +1871,9 @@ decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __
             res[e] = from_latent_kind<L>(L(L(pq << k) + lowest), 2);
           }
         }
-        if constexpr (SEG) {
+        if constexpr (HIST) {
+          hist_store8<L>(filt, fkey, reinterpret_cast<uint32_t*>(&sm + 1), out_cnt, lane, res);
+        } else if constexpr (SEG) {
           seg_store8<L>(filt, fkey, task.out_offset + uint64_t(b) * BATCH_N, fslot0 + b, out_cnt, lane, res);
         } else if constexpr (TAKE) {
           take_store8<L>(filt, task.out_offset + uint64_t(b) * BATCH_N, fslot0 + b, out_cnt, lane, res);
@@ -1827,6 +1912,7 @@ decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __
 #endif
   if (end_err) atomicMax(&sm.err, end_err);
   __syncthreads();
+  if constexpr (HIST) hist_flush(filt, reinterpret_cast<const uint32_t*>(&sm + 1), filt.counts[filt.fast_page[blockIdx.x]], tid, DEC_THREADS);
   if (tid == 0) statuses[blockIdx.x] = sm.err;
 }
 

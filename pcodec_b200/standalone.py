@@ -906,6 +906,78 @@ class AsyncFilesAggregate(_lib._AsyncCall):
         return int(nm.value)
 
 
+class _CAsyncFilesHistogramPlan(C.Structure):  # PcoB200AsyncFilesHistogramPlan (include/pco_b200.h)
+    _fields_ = [("dtype", C.c_uint32), ("uniform_type", C.c_uint32), ("format_major", C.c_uint32), ("reserved", C.c_uint32),
+                ("src_cap", C.c_uint64), ("index_cap", C.c_uint64), ("max_files", C.c_uint64), ("max_chunks", C.c_uint64),
+                ("rows_cap", C.c_uint64), ("n_buckets", C.c_uint64), ("workspace_bytes", C.c_uint64)]
+
+
+class _CAsyncFilesHistogramStatus(C.Structure):  # PcoB200AsyncFilesHistogramStatus (include/pco_b200.h)
+    _fields_ = [("kind", C.c_uint32), ("device_status", C.c_uint32), ("file", C.c_uint64), ("chunk", C.c_uint64), ("n_written", C.c_uint64),
+                ("n_files", C.c_uint64), ("edge", C.c_uint64)]
+
+
+def _lib_async_histogram_files():
+    return _lib.bind("_async_histogram_files_ready",
+                     pco_b200_histogram_files_async_plan=[C.c_void_p, C.c_size_t, C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                                          C.c_size_t, C.c_size_t, C.c_void_p],
+                     pco_b200_histogram_files_async=[C.c_void_p] * 11,
+                     pco_b200_histogram_files_async_result=[C.c_void_p, C.POINTER(C.c_size_t)])
+
+
+class AsyncFilesHistogram(_lib._AsyncCall):
+    """Decodes a batch of indexed standalone files on the current CUDA stream and counts how many numbers fall in each of n_buckets
+    buckets, per file and in all (pco_b200_histogram_files_async): each decode CTA counts its numbers in shared memory, so the decoded
+    files never reach HBM.  Refs, their count and the edges are read from device tensors, so one captured call serves new files and new
+    edges on each replay.  Rows are wrapped.AsyncPagesHistogram's.
+
+    The plan and capacities are AsyncFilesDecompressor's, with rows_cap (the most numbers of a call's files) in place of dst_cap, and
+    n_buckets (1 .. 4096) fixed by the plan.  The call owns a device workspace (about rows_cap * itemsize + 8 * (n_buckets + 3) *
+    max_files bytes beyond the decompressor's) and a status; it serves one call in flight."""
+
+    _Plan, _Status = _CAsyncFilesHistogramPlan, _CAsyncFilesHistogramStatus
+
+    def __init__(self, head, dtype, src_cap, index_cap, max_files, max_chunks, rows_cap, n_buckets, device=None):
+        self.dtype = np.dtype(dtype)
+        h = self._head(head)
+        self._make_plan(device, lambda plan: _lib_async_histogram_files().pco_b200_histogram_files_async_plan(
+            h.ctypes.data_as(C.c_void_p), C.c_size_t(h.size), C.c_ubyte(_lib.dtype_byte(self.dtype)), C.c_size_t(src_cap), C.c_size_t(index_cap),
+            C.c_size_t(max_files), C.c_size_t(max_chunks), C.c_size_t(rows_cap), C.c_size_t(n_buckets), plan))
+        self._alloc()
+
+    def __call__(self, src, index, files, n_files, edges, hists, total):
+        """Enqueues the histograms of files[: n_files[0]] on torch.cuda.current_stream().  `src`, `index`, `files` and `n_files` are as
+        AsyncFilesDecompressor takes them; `edges`, `hists` (of shape (max_files, n_buckets + 3)) and `total` are as
+        wrapped.AsyncPagesHistogram takes them, row i of hists receiving file i's counts.  Returns nothing and does not wait; result()
+        reports the outcome."""
+        import torch
+
+        from .wrapped import _check_histogram_inputs
+
+        p = self._plan
+        self._check_tensors(src=src, index=index, files=files, n_files=n_files, edges=edges, hists=hists, total=total)
+        if src.numel() * src.element_size() < p.src_cap or index.numel() * index.element_size() < p.index_cap:
+            raise ValueError(f"src holds fewer than src_cap = {p.src_cap} bytes, or index fewer than index_cap = {p.index_cap}")
+        if files.dtype != torch.int64 or files.dim() != 2 or files.shape[1] != 4 or files.shape[0] < p.max_files:
+            raise ValueError(f"files must be an int64 tensor of shape ({p.max_files}, 4)")
+        if n_files.dtype != torch.int64 or n_files.numel() != 1:
+            raise ValueError("n_files must be a 1-element int64 tensor")
+        _check_histogram_inputs(edges, hists, total, p.n_buckets, p.max_files)
+        rc = _lib_async_histogram_files().pco_b200_histogram_files_async(
+            C.byref(p), C.c_void_p(src.data_ptr()), C.c_void_p(index.data_ptr()), C.c_void_p(files.data_ptr()), C.c_void_p(n_files.data_ptr()),
+            C.c_void_p(edges.data_ptr()), C.c_void_p(hists.data_ptr()), C.c_void_p(total.data_ptr()), C.c_void_p(self.workspace.data_ptr()),
+            C.c_void_p(self.status.data_ptr()), self._stream())
+        _lib.check(rc)
+
+    def result(self):
+        """Copies the status of the last call back (waiting for it on the current stream) and returns the numbers counted, or raises
+        PcoError with the kind pco_b200_decompress_files gives ("file 3: chunk 2: ...") or naming the lowest bad edge ("edge 3: ...")."""
+        s = self.status_record()
+        n = C.c_size_t()
+        _lib.check(_lib_async_histogram_files().pco_b200_histogram_files_async_result(C.byref(s), C.byref(n)))
+        return int(n.value)
+
+
 class _CAsyncFilesTakePlan(C.Structure):  # PcoB200AsyncFilesTakePlan (include/pco_b200.h)
     _fields_ = [("dtype", C.c_uint32), ("uniform_type", C.c_uint32), ("format_major", C.c_uint32), ("reserved", C.c_uint32),
                 ("src_cap", C.c_uint64), ("index_cap", C.c_uint64), ("max_files", C.c_uint64), ("max_chunks", C.c_uint64),

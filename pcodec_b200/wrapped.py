@@ -437,22 +437,35 @@ def pack_interval(lo, hi, dtype):
     """The PcoB200Interval of [lo, hi] for numbers of `dtype`: a 2-element int64 array holding each bound's bit pattern, zero-extended
     (copy it to a CUDA tensor for AsyncPagesFilter).  The bounds are Python or numpy numbers, converted to `dtype` (NaN and infinities
     included for floats); a bound outside an integer dtype's range raises OverflowError."""
+    return _pack_values((lo, hi), dtype, "bound")
+
+
+def _pack_values(values, dtype, what):
+    """The zero-extended bit patterns of `values` as numbers of `dtype` (an int64 array): the per-value conversion pack_interval and
+    pack_edges share.  `what` names a value in the errors."""
     dt = np.dtype(dtype)
     _lib.dtype_byte(dt)
     ut = np.dtype(f"u{dt.itemsize}")
     bits = []
-    for x in (lo, hi):
+    for x in values:
         if dt.kind in "iu":
             info = np.iinfo(dt)
             if isinstance(x, (float, np.floating)) and not float(x).is_integer():
-                raise TypeError(f"bound {x!r} is not an integer of {dt}")
+                raise TypeError(f"{what} {x!r} is not an integer of {dt}")
             if not info.min <= int(x) <= info.max:
-                raise OverflowError(f"bound {x!r} lies outside {dt}")
+                raise OverflowError(f"{what} {x!r} lies outside {dt}")
             v = np.array([int(x)], dtype=dt)
         else:
             v = np.array([x], dtype=dt)
         bits.append(int(v.view(ut)[0]))
     return np.array(bits, dtype=np.uint64).view(np.int64)
+
+
+def pack_edges(edges, dtype):
+    """The B + 1 bucket edges `edges` (a sequence or array of Python or numpy numbers) for numbers of `dtype` as the int64 array of their
+    zero-extended bit patterns that AsyncPagesHistogram and standalone.AsyncFilesHistogram read (copy it to a CUDA tensor), converted as
+    pack_interval converts its bounds.  Whether the edges ascend is checked by the call, on the device."""
+    return _pack_values(list(edges), dtype, "edge")
 
 
 def unpack_aggregates(records, dtype):
@@ -555,6 +568,91 @@ class AsyncPagesAggregate(_lib._AsyncCall):
         nm = C.c_size_t()
         _lib.check(_lib_async_aggregate().pco_b200_aggregate_pages_async_result(C.byref(s), C.byref(nm)))
         return int(nm.value)
+
+
+class _CAsyncHistogramPlan(C.Structure):  # PcoB200AsyncHistogramPlan (include/pco_b200.h)
+    _fields_ = [("dtype", C.c_uint32), ("reserved", C.c_uint32), ("metas_cap", C.c_uint64), ("pages_cap", C.c_uint64), ("max_pages", C.c_uint64),
+                ("rows_cap", C.c_uint64), ("frame_cap", C.c_uint64), ("n_buckets", C.c_uint64), ("workspace_bytes", C.c_uint64)]
+
+
+class _CAsyncHistogramStatus(C.Structure):  # PcoB200AsyncHistogramStatus (include/pco_b200.h)
+    _fields_ = [("kind", C.c_uint32), ("device_status", C.c_uint32), ("page", C.c_uint64), ("n_written", C.c_uint64), ("n_pages", C.c_uint64),
+                ("frames_needed", C.c_uint64), ("edge", C.c_uint64)]
+
+
+def _lib_async_histogram():
+    return _lib.bind("_async_histogram_ready",
+                     pco_b200_histogram_pages_async_plan=[C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                                          C.c_void_p],
+                     pco_b200_histogram_pages_async=[C.c_void_p] * 11,
+                     pco_b200_histogram_pages_async_result=[C.c_void_p, C.POINTER(C.c_size_t)])
+
+
+def _check_histogram_inputs(edges, hists, total, n_buckets, max_groups):
+    import torch
+
+    w = n_buckets + 3
+    if edges.dtype != torch.int64 or edges.numel() != n_buckets + 1:
+        raise ValueError(f"edges must be an int64 tensor of {n_buckets + 1} elements (pack_edges' bit patterns)")
+    if hists.dtype != torch.int64 or hists.dim() != 2 or hists.shape[1] != w or hists.shape[0] < max_groups or not hists.is_contiguous():
+        raise ValueError(f"hists must be a contiguous int64 tensor of shape ({max_groups}, {w})")
+    if total.dtype != torch.int64 or total.numel() != w or not total.is_contiguous():
+        raise ValueError(f"total must be a contiguous {w}-element int64 tensor")
+
+
+class AsyncPagesHistogram(_lib._AsyncCall):
+    """Decodes a batch of wrapped-format pages on the current CUDA stream and counts how many numbers fall in each of n_buckets buckets,
+    per page and in all (pco_b200_histogram_pages_async): each decode CTA counts its numbers in shared memory, so the decoded pages never
+    reach HBM.  Refs, their count and the edges are read from device tensors, so one captured call serves new pages and new edges on each
+    replay.  A row holds n_buckets + 3 counts: below edge 0, the buckets (the last one closed, as numpy.histogram's), above the last edge,
+    and NaNs.
+
+    The capacities are AsyncPagesDecompressor's, with rows_cap (the most numbers of a call's pages) in place of dst_cap; frame_cap defaults
+    to metas_cap + pages_cap + 20 * max_pages as there.  n_buckets (1 .. 4096) is fixed by the plan.  The call owns a device workspace
+    (about rows_cap * itemsize + 8 * (n_buckets + 3) * max_pages bytes beyond the decompressor's) and a status; it serves one call in
+    flight."""
+
+    _Plan, _Status = _CAsyncHistogramPlan, _CAsyncHistogramStatus
+
+    def __init__(self, dtype, metas_cap, pages_cap, max_pages, rows_cap, n_buckets, frame_cap=None, device=None):
+        self.dtype = np.dtype(dtype)
+        if frame_cap is None:
+            frame_cap = metas_cap + pages_cap + 20 * max_pages
+        self._make_plan(device, lambda plan: _lib_async_histogram().pco_b200_histogram_pages_async_plan(
+            C.c_ubyte(_lib.dtype_byte(self.dtype)), C.c_size_t(metas_cap), C.c_size_t(pages_cap), C.c_size_t(max_pages), C.c_size_t(rows_cap),
+            C.c_size_t(frame_cap), C.c_size_t(n_buckets), plan))
+        self._alloc()
+
+    def __call__(self, metas, pages, refs, n_pages, edges, hists, total):
+        """Enqueues the histograms of the pages refs[: n_pages[0]] names on torch.cuda.current_stream().  `metas`, `pages`, `refs` and
+        `n_pages` are as AsyncPagesDecompressor takes them; `edges` is an int64 CUDA tensor of n_buckets + 1 elements (pack_edges' bit
+        patterns), `hists` an int64 CUDA tensor of shape (max_pages, n_buckets + 3) whose row i receives page i's counts, and `total` an
+        int64 CUDA tensor of n_buckets + 3 elements that receives their column sums.  Returns nothing and does not wait; result() reports
+        the outcome."""
+        import torch
+
+        p = self._plan
+        self._check_tensors(metas=metas, pages=pages, refs=refs, n_pages=n_pages, edges=edges, hists=hists, total=total)
+        if metas.numel() * metas.element_size() < p.metas_cap or pages.numel() * pages.element_size() < p.pages_cap:
+            raise ValueError(f"metas holds fewer than metas_cap = {p.metas_cap} bytes, or pages fewer than pages_cap = {p.pages_cap}")
+        if refs.dtype != torch.int64 or refs.dim() != 2 or refs.shape[1] != 5 or refs.shape[0] < p.max_pages:
+            raise ValueError(f"refs must be an int64 tensor of shape ({p.max_pages}, 5)")
+        if n_pages.dtype != torch.int64 or n_pages.numel() != 1:
+            raise ValueError("n_pages must be a 1-element int64 tensor")
+        _check_histogram_inputs(edges, hists, total, p.n_buckets, p.max_pages)
+        rc = _lib_async_histogram().pco_b200_histogram_pages_async(
+            C.byref(p), C.c_void_p(metas.data_ptr()), C.c_void_p(pages.data_ptr()), C.c_void_p(refs.data_ptr()), C.c_void_p(n_pages.data_ptr()),
+            C.c_void_p(edges.data_ptr()), C.c_void_p(hists.data_ptr()), C.c_void_p(total.data_ptr()), C.c_void_p(self.workspace.data_ptr()),
+            C.c_void_p(self.status.data_ptr()), self._stream())
+        _lib.check(rc)
+
+    def result(self):
+        """Copies the status of the last call back (waiting for it on the current stream) and returns the numbers counted, or raises
+        PcoError with the kind decompress_pages gives ("page 17: ...") or naming the lowest bad edge ("edge 3: ...")."""
+        s = self.status_record()
+        n = C.c_size_t()
+        _lib.check(_lib_async_histogram().pco_b200_histogram_pages_async_result(C.byref(s), C.byref(n)))
+        return int(n.value)
 
 
 class _CAsyncTakePlan(C.Structure):  # PcoB200AsyncTakePlan (include/pco_b200.h)
