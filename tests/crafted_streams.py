@@ -487,6 +487,108 @@ def positions(chunk_ns, seed):
     return out
 
 
+def bounds(record_ns, seed, cold=None):
+    """Named segment bounds (non-decreasing int64 row indices in [0, rows]) over the concatenation of records of `record_ns` numbers, for
+    the segment aggregate calls: one segment over every row; each record a segment; bounds at each record start, one below and above it and
+    at its rows 255, 256 and 257, with one-row segments and a run of three equal bounds (two empty segments); each 256-number batch a segment
+    (a record's partial last batch shorter); about 40 random bounds strictly inside the rows; windows inside the first record `cold` flags and
+    from a fast record into a cold one; one empty segment; and, when the rows allow, segments of more than 2^18 rows that start and end
+    mid-batch, one of them with an end inside a cold record."""
+    ns = np.asarray(record_ns, dtype=np.int64)
+    starts = np.concatenate([[0], np.cumsum(ns)[:-1]]).astype(np.int64)
+    rows = int(ns.sum())
+    cold = np.zeros(ns.size, bool) if cold is None else np.asarray(cold, bool)
+    rng = np.random.default_rng(seed)
+
+    def arr(v):
+        return np.array(sorted(int(b) for b in v if 0 <= b <= rows), dtype=np.int64)
+
+    out = {"all": np.array([0, rows], np.int64), "records": arr(list(starts) + [rows])}
+    near = {int(s) + d for s in starts for d in (-1, 0, 1, 255, 256, 257)} | {rows}
+    near |= {int(p) + d for p in rng.integers(0, max(rows - 1, 1), size=4) for d in (0, 1)}  # one-row segments at random rows
+    b = sorted(v for v in near if 0 <= v <= rows)
+    k = len(b) // 2
+    out["record_edges"] = np.array(b[:k] + [b[k]] * 2 + b[k:], np.int64)  # b[k] three times: two empty segments
+    out["every_batch"] = np.concatenate([o + np.arange(0, n, 256) for o, n in zip(starts, ns) if n] + [[rows]]).astype(np.int64)
+    if rows > 2:
+        out["inner"] = np.sort(rng.integers(1, rows, size=40)).astype(np.int64)
+    c = np.flatnonzero(cold)
+    if c.size:
+        c0 = int(c[0])
+        s0, n0 = int(starts[c0]), int(ns[c0])
+        w = [s0 + min(3, n0 - 1), s0 + max(n0 - 3, min(3, n0 - 1))]  # inside the first cold record
+        after = [int(i) for i in c if i > 0 and not cold[i - 1]]
+        if after:  # from the middle of a fast record into the cold record behind it
+            i = after[0]
+            w += [int(starts[i - 1]) + int(ns[i - 1]) // 2, int(starts[i]) + (int(ns[i]) + 1) // 2]
+        out["cold_window"] = arr(w)
+    out["empty"] = np.array([rows // 2, rows // 2], np.int64)
+    if rows > 2 * (1 << 18) + 1024 and c.size:
+        def mid_batch(v):  # moved off a batch start of the record holding row v
+            r = int(np.searchsorted(starts, v, side="right")) - 1
+            return v + 77 if (v - int(starts[r])) % 256 == 0 else v
+
+        big = max(c, key=lambda i: ns[i])  # an end inside the largest cold record
+        first = mid_batch(int(starts[big]) + int(ns[big]) // 2)
+        b = [first]
+        while b[0] > (1 << 18) + 512:  # long segments in front of it
+            b.insert(0, mid_batch(b[0] - (1 << 18) - 333))
+        while b[-1] + (1 << 18) + 512 < rows:  # and behind it
+            b.append(mid_batch(b[-1] + (1 << 18) + 333))
+        out["long"] = arr(b)
+    return out
+
+
+def _succ(v, dt):
+    """The next numbers of dt above the numbers v (integers: each below the type's max)."""
+    v = np.asarray(v, dtype=dt)
+    with np.errstate(over="ignore"):  # the largest finite float steps to +inf
+        return v + dt.type(1) if dt.kind in "iu" else np.nextafter(v, dt.type(np.inf))
+
+
+def edges(want, dtype):
+    """Named bucket edges (strictly ascending numbers of `dtype`, no NaN, 2 to 4097 of them) for the histogram calls over the numbers
+    `want`: the type's extremes (floats: -inf and +inf); the numbers one inside them (floats: the largest finite numbers), so that the
+    extremes fall below and above; a top edge that is the largest number present (the closed last bucket takes it); for integers the
+    numbers of latents MID - 2 .. MID + 1, where the signed key flips; for floats edges at and around the signed zeros and the infinities;
+    edges alternating between a number present and one absent (8-bit batches hold every number: none there); and the quantiles of the
+    distinct numbers at 1, 7, 255 and 4096 buckets, or evenly spaced numbers of the type where there are too few of them."""
+    dt = np.dtype(dtype)
+    x = np.asarray(want, dtype=dt)
+    floats = dt.kind == "f"
+    u = np.unique(x[~np.isnan(x)] if floats else x)  # by value: -0.0 and +0.0 are one
+    lim = np.finfo(dt) if floats else np.iinfo(dt)
+    lo, hi = (dt.type(-np.inf), dt.type(np.inf)) if floats else (dt.type(lim.min), dt.type(lim.max))
+    out = {"extremes": np.array([lo, hi], dt)}
+    out["inside_extremes"] = np.array([lim.min, lim.max], dt) if floats else np.array([int(lim.min) + 1, int(lim.max) - 1], dt)
+    if u.size:
+        top = u[-1]
+        below = [v for v in (u[0], u[u.size // 2]) if v < top] or [top - dt.type(1)]
+        out["closed_top"] = np.unique(np.array(below + [top], dt))
+    mid = 1 << (nbits(dt) - 1)
+    if not floats:
+        out["mid"] = from_latents(np.arange(mid - 2, mid + 2, dtype=np.uint64), dt)
+    else:
+        tiny = np.array(lim.smallest_subnormal, dt)
+        out.update({"zeros_first": np.array([0.0, 1.0], dt), "zeros_last": np.array([-1.0, -0.0], dt),
+                    "subnormal_zero": np.array([-tiny, 0.0, tiny], dt), "inf_buckets": np.array([-np.inf, lim.min, lim.max, np.inf], dt)})
+    gaps = np.flatnonzero(_succ(u[:-1], dt) < u[1:])  # u[j] present, the number above it absent
+    if gaps.size:
+        pick = gaps[np.linspace(0, gaps.size - 1, min(gaps.size, 128)).astype(np.int64)]
+        out["occurring_and_between"] = np.stack([u[pick], _succ(u[pick], dt)], axis=1).reshape(-1).astype(dt)
+    for nb in (1, 7, 255, 4096):
+        if u.size >= nb + 1:
+            e = u[np.linspace(0, u.size - 1, nb + 1).astype(np.int64)]
+        elif floats:  # evenly spaced latents of the finite numbers
+            a, z = (float_latent(v, dt) for v in (lim.min, lim.max))
+            e = np.unique(from_latents(np.array([a + (z - a) * i // nb for i in range(nb + 1)], np.uint64), dt))
+        else:
+            a, z = int(lim.min), int(lim.max)
+            e = np.unique(np.array([a + (z - a) * i // nb for i in range(nb + 1)], dtype=object).astype(dt))
+        out[f"q{nb}"] = np.asarray(e, dt)
+    return out
+
+
 def class_counts(f):
     """Expected pco_b200_profile_chunk_classes counts of a fast family (index k = class k)."""
     counts = [0] * 8

@@ -4,6 +4,8 @@ The writer is pinned to the format first: fed the bins the oracle's own compress
 the stored latents, it must write the compressor's file byte for byte, for every number type, Classic and IntMult, and consecutive
 orders 0-7.  Then every crafted family must decode on the oracle to the numpy restatement of the decode, and pcodec_b200.inspect
 must read the crafted bins back.  Specs the format's reader would refuse are refused by the writer."""
+import bisect
+
 import numpy as np
 import pytest
 
@@ -208,6 +210,115 @@ def test_positions_are_ascending_and_in_range(dtype_str):
     odd = sets["odd_start_batch"]
     b0 = int(odd[1])
     assert odd.size == 257 and odd[0] < b0 and any(b0 - s >= 0 and (b0 - s) % 256 == 0 and b0 - s + 256 <= n for s, n in zip(starts, ns))
+
+
+# ---- the segment and histogram calls' bounds and edges -----------------------------------------------------------------------------
+def _colds(dtype_str):
+    return [c["route"] == "cold" for f in FAMILIES if f["dtype"].name == dtype_str for c in f["chunks"]]
+
+
+def _record_of(starts, v):
+    return int(np.searchsorted(starts, v, side="right")) - 1
+
+
+@pytest.mark.parametrize("dtype_str", BATCH_TYPES)
+def test_bounds_are_well_formed(dtype_str):
+    _, ns = _batch(dtype_str)
+    cold = np.array(_colds(dtype_str))
+    rows = sum(ns)
+    starts = np.concatenate([[0], np.cumsum(ns)[:-1]])
+    sets = cs.bounds(ns, seed=1, cold=cold)
+    for name, b in sets.items():
+        assert b.dtype == np.int64 and b.size >= 2 and (np.diff(b) >= 0).all(), name
+        assert b[0] >= 0 and b[-1] <= rows, name
+    assert sets["all"].tolist() == [0, rows] and sets["records"].tolist() == starts.tolist() + [rows]
+    e = sets["record_edges"]
+    assert (np.diff(e) == 0).sum() >= 2 and (np.diff(e) == 1).sum() >= 4, "empty and one-row segments"
+    assert all({s, s + 1} <= set(e.tolist()) for s in starts) and all(s + 257 in e for s, n in zip(starts, ns) if s + 257 <= rows)
+    assert all(s - 1 in e for s in starts[1:])
+    seg = np.diff(sets["every_batch"])
+    assert (seg > 0).all() and (seg <= 256).all() and seg.size == sum((n + 255) // 256 for n in ns)
+    assert sets["inner"][0] > 0 and sets["inner"][-1] < rows and sets["inner"].size == 40
+    # the cold windows: a segment inside the first cold record, and one from a fast record into a cold one
+    c0 = int(np.flatnonzero(cold)[0])
+    w = sets["cold_window"]
+    segs = list(zip(w[:-1].tolist(), w[1:].tolist()))
+    assert any(a < b and _record_of(starts, a) == _record_of(starts, b - 1) == c0 for a, b in segs), (w, c0)
+    assert any(not cold[_record_of(starts, a)] and cold[_record_of(starts, b - 1)] for a, b in segs if a < b), w
+    assert sets["empty"][0] == sets["empty"][1]
+    if dtype_str != "uint32":
+        assert "long" not in sets
+        return
+    long = sets["long"]
+    assert (np.diff(long) > 1 << 18).all() and long.size >= 3
+    assert all((v - starts[_record_of(starts, v)]) % 256 for v in long), "long segments start and end mid-batch"
+    assert any(cold[_record_of(starts, v)] for v in long)
+
+
+@pytest.mark.parametrize("dtype_str", BATCH_TYPES)
+def test_edges_are_well_formed(dtype_str):
+    want, _ = _batch(dtype_str)
+    dt = want.dtype
+    floats = dt.kind == "f"
+    sets = cs.edges(want, dt)
+    assert ("mid" in sets) != floats and ("zeros_first" in sets) == floats
+    for name, e in sets.items():
+        assert e.dtype == dt and 2 <= e.size <= 4097, (name, e.size)
+        assert not np.isnan(e).any() if floats else True, name
+        assert (e[1:] > e[:-1]).all(), f"{name}: not strictly ascending under IEEE comparison"
+    present = set(want[~np.isnan(want)].tolist()) if floats else set(want.tolist())
+    lim = np.finfo(dt) if floats else np.iinfo(dt)
+    top = max(present)
+    assert sets["closed_top"][-1] == top and top == (np.inf if floats else lim.max), "the batch holds the type's top"
+    alt = sets.get("occurring_and_between")
+    if dt.itemsize == 1:
+        assert alt is None and len(present) == 256 and sets["q4096"].size == 256
+    else:
+        assert [v in present for v in alt.tolist()] == [True, False] * (alt.size // 2)
+    for nb in (1, 7, 255, 4096):
+        assert sets[f"q{nb}"].size == min(nb, 255 if dt.itemsize == 1 else nb) + 1, nb
+    if not floats:
+        assert [int(v) for v in cs.to_latents(sets["mid"])] == [(1 << (8 * dt.itemsize - 1)) + d for d in (-2, -1, 0, 1)]
+
+
+def _brute_columns(x, edges):
+    """One number at a time in Python int / float: NaN in the last column, -0.0 as +0.0, below the first edge in column 0, above the last
+    in column B + 1, on the last edge in the closed last bucket B, and otherwise column 1 + i for the last edge i at or below it."""
+    e = edges.tolist()
+    b = len(e) - 1
+    out = []
+    for v in x.tolist():
+        if v != v:
+            out.append(b + 2)
+            continue
+        if isinstance(v, float) and v == 0:
+            v = 0.0  # -0.0 compares as +0.0
+        if v < e[0]:
+            out.append(0)
+        elif v > e[b]:
+            out.append(b + 1)
+        elif v == e[b]:
+            out.append(b)
+        else:
+            out.append(bisect.bisect_right(e, v))  # 1 + the last edge at or below it
+    return np.array(out, np.int64)
+
+
+@pytest.mark.parametrize("dtype_str", BATCH_TYPES)
+def test_histogram_reference_against_one_number_at_a_time(dtype_str):
+    """histogram_reference.columns (np.searchsorted in the numbers' own dtype) equals the rules applied to each number as a Python int or
+    float, on the crafted batch's NaN payloads of both signs, signed zeros, infinities and 64-bit integers."""
+    from tests import histogram_reference as hr
+
+    want, _ = _batch(dtype_str)
+    sets = cs.edges(want, want.dtype)
+    names = ["extremes", "inside_extremes", "closed_top", "mid", "zeros_first", "zeros_last", "subnormal_zero", "inf_buckets", "q7", "q255"]
+    for name in names:
+        if name in sets:
+            np.testing.assert_array_equal(hr.columns(want, sets[name]), _brute_columns(want, sets[name]), err_msg=name)
+    if want.dtype.kind == "f":  # and the batch holds what these sets are for
+        assert np.isnan(want).any() and (want == np.inf).any() and (want == -np.inf).any()
+        assert (np.signbit(want) & (want == 0)).any() and (~np.signbit(want) & (want == 0)).any()
 
 
 # ---- invalid specs --------------------------------------------------------------------------------------------------------------
