@@ -1472,6 +1472,110 @@ PcoB200Error pco_b200_histogram_files_async(const PcoB200AsyncFilesHistogramPlan
  * and, when the kind is OK, sets *n_rows (may be NULL) to the numbers counted (the sum of *total). */
 PcoB200Error pco_b200_histogram_files_async_result(const PcoB200AsyncFilesHistogramStatus *host_status, size_t *n_rows);
 
+/* ---- asynchronous top-k of wrapped-format pages and of indexed standalone files (no reference counterpart): the k smallest or largest
+ * numbers inside a closed interval of the concatenation pco_b200_decompress_pages_async / pco_b200_decompress_files_async write, with
+ * their positions in it (ORDER BY x [DESC] LIMIT k).  The column is decoded once and never reaches HBM: each decode CTA keeps its best
+ * matches in shared memory, and the CTAs' lists are merged on the device.  Each call only enqueues kernels on the caller's stream and
+ * returns at once; it makes no synchronising, allocating or host-to-device copy call and refers to no memory of the library's per-thread
+ * scratch, so it can be captured in a CUDA graph, and a captured call may be replayed after pco_b200_thread_release or after any other
+ * call.  A plan made once outside any capture fixes the grids, k and the direction from its capacities; the refs, their count and the
+ * interval are read on the device, so one captured graph serves new pages or files and a new interval on each replay.
+ * Numbers compare as the filter calls compare them: integers in their signed or unsigned order, floats as IEEE values (-0.0 equals +0.0;
+ * -inf and +inf are ordinary numbers; a NaN of any payload or sign never matches).  Only numbers x with lo <= x <= hi of the interval are
+ * candidates; lo > hi or a NaN bound selects nothing.  A number's rank is the pair (value, position), the lower position winning a tie in
+ * both directions, so the output is a unique function of the numbers.  out_values[0 : *n_out) holds the min(k, matches) best numbers, best
+ * first, each with its own bits (a -0.0 stays -0.0), and out_positions[0 : *n_out) their positions (uint64_t, as the filter calls write
+ * them; sorted ascending they feed the take calls); slots past *n_out are not written.
+ * Refusals and decode failures are the decompress call's, in its order, with its kinds and naming the same page, or file and chunk (rows_cap
+ * in the role of dst_cap).  On any failure *n_out is written as 0 and out_values and out_positions are not written. */
+typedef struct PcoB200AsyncTopkPlan {  /* filled by pco_b200_topk_pages_async_plan; treat as opaque */
+  uint32_t dtype, largest;
+  uint64_t metas_cap, pages_cap, max_pages, rows_cap, frame_cap, k;
+  uint64_t workspace_bytes;            /* device workspace one in-flight call needs */
+} PcoB200AsyncTopkPlan;
+
+typedef struct PcoB200AsyncTopkStatus {  /* written on the device by every call */
+  uint32_t kind;                         /* PcoB200Error */
+  uint32_t device_status;                /* the device word behind it: as PcoB200AsyncPagesStatus */
+  uint64_t page;                         /* the page the outcome names (UINT64_MAX if none) */
+  uint64_t n_written;                    /* the rows of the concatenation (the sum of page_n), once every page passed its checks (0 on a
+                                            failure of the pages call) */
+  uint64_t n_pages;                      /* *n_pages as the call read it */
+  uint64_t frames_needed;                /* bytes of framed pages the batch needs, also when above frame_cap (0 when refused earlier) */
+  uint64_t n_matches;                    /* the numbers inside the interval, in all (0 on a failure) */
+} PcoB200AsyncTopkStatus;
+
+/* Makes a plan for the k best numbers (largest = 0: the k smallest; 1: the k largest) over up to max_pages pages of dtype, whose refs
+ * point into metas_cap bytes of metas and pages_cap bytes of pages, holding at most rows_cap numbers in all (the role dst_cap plays in
+ * pco_b200_decompress_pages_async); frame_cap bounds the framed pages as in that call.  Checked before the device is touched: dtype
+ * (PCO_B200_INVALID_TYPE), max_pages in 1 .. 2^31 - 1, rows_cap and frame_cap at most 2^56, k in 1 .. 1024, largest 0 or 1
+ * (PCO_B200_INVALID_ARGUMENT).  Then *plan is filled and the one-time device set-up runs on the current device, which the calls must use
+ * (kernel attributes, and every kernel the call launches loaded); without a device that is PCO_B200_CUDA.
+ * workspace_bytes is pco_b200_decompress_pages_async_plan's formula with dst_cap = rows_cap, plus these regions, each rounded up to 256
+ * bytes, with E the bytes of a number of dtype: 40 (the pages status), 16 (the plan's state), 4 max_pages (each page's flag), 48 (the top-k
+ * table), E rows_cap (the cold pages' values), 4 max_pages (the pages' list lengths) and 16 k max_pages (the pages' candidate lists). */
+PcoB200Error pco_b200_topk_pages_async_plan(unsigned char dtype, size_t metas_cap, size_t pages_cap, size_t max_pages, size_t rows_cap,
+                                            size_t frame_cap, size_t k, int largest, PcoB200AsyncTopkPlan *plan);
+/* Enqueues the top-k of the pages refs[0 : *n_pages) names on `cuda_stream`, and the outcome into *status; returns without waiting.
+ * metas (metas_cap bytes), pages (pages_cap bytes; may be the same buffer as metas), refs (PcoB200PageRef[max_pages]), n_pages (one
+ * uint64_t), interval, out_values (k numbers of dtype), out_positions (uint64_t[k]), n_out (one uint64_t), workspace
+ * (plan->workspace_bytes, 256-byte aligned) and status are device pointers; one workspace serves one call in flight.  The numbers ranked
+ * are the concatenation pco_b200_decompress_pages_async writes for the same arguments with dst_cap = rows_cap; *n_pages = 0 gives
+ * *n_out = 0.  The return value covers the host side only: null pointers, an unaligned workspace or a plan that was not filled
+ * (PCO_B200_INVALID_ARGUMENT), a launch the runtime refuses (PCO_B200_CUDA).  With pco_b200_profile_enable(1), a call outside a stream
+ * capture records its kernel spans for pco_b200_profile_last; a call inside a capture records none. */
+PcoB200Error pco_b200_topk_pages_async(const PcoB200AsyncTopkPlan *plan, const void *metas, const void *pages, const PcoB200PageRef *refs,
+                                       const uint64_t *n_pages, const PcoB200Interval *interval, void *out_values, uint64_t *out_positions,
+                                       uint64_t *n_out, void *workspace, PcoB200AsyncTopkStatus *status, void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory.  Returns the kind, sets the last-error message as
+ * pco_b200_aggregate_pages_async_result words it ("page 17: ..."), and, when the kind is OK, sets *n_matches (may be NULL) to the numbers
+ * inside the interval. */
+PcoB200Error pco_b200_topk_pages_async_result(const PcoB200AsyncTopkStatus *host_status, size_t *n_matches);
+
+typedef struct PcoB200AsyncFilesTopkPlan {  /* filled by pco_b200_topk_files_async_plan; treat as opaque */
+  uint32_t dtype, uniform_type, format_major, largest;
+  uint64_t src_cap, index_cap, max_files, max_chunks, rows_cap, k;
+  uint64_t workspace_bytes;                 /* device workspace one in-flight call needs */
+} PcoB200AsyncFilesTopkPlan;
+
+typedef struct PcoB200AsyncFilesTopkStatus {  /* written on the device by every call */
+  uint32_t kind;                              /* PcoB200Error */
+  uint32_t device_status;                     /* the device word behind it: as PcoB200AsyncFilesStatus */
+  uint64_t file;                              /* the file the outcome names (UINT64_MAX if none) */
+  uint64_t chunk;                             /* the failing chunk, counted from that file's first chunk (UINT64_MAX if none) */
+  uint64_t n_written;                         /* the rows of the concatenation (the sum of the files' counts), once every file passed its
+                                                 checks and placement (0 before) */
+  uint64_t n_files;                           /* *n_files as the call read it */
+  uint64_t n_matches;                         /* the numbers inside the interval, in all (0 on a failure) */
+} PcoB200AsyncFilesTopkStatus;
+
+/* Makes a plan for the k best numbers (largest = 0: the k smallest; 1: the k largest) over up to max_files indexed files of dtype holding
+ * at most max_chunks chunks and rows_cap numbers in all (the role dst_cap plays in pco_b200_decompress_files_async).  `head`, src_cap and
+ * index_cap are those of pco_b200_decompress_files_async_plan.  Checked before the device is touched, with that plan's kinds: dtype, the
+ * header, the uniform type, max_files in 1 .. 2^31 - 1, max_chunks in 1 .. 2^32 - 1, rows_cap at most 2^56, k in 1 .. 1024, largest 0 or 1
+ * (PCO_B200_INVALID_ARGUMENT).  Then *plan is filled and the one-time device set-up runs on the current device, which the calls must use;
+ * without a device that is PCO_B200_CUDA.
+ * workspace_bytes is pco_b200_decompress_files_async_plan's formula with dst_cap = rows_cap, plus these regions, each rounded up to 256
+ * bytes, with E the bytes of a number of dtype: 40 (the files status), 16 (the plan's state), 4 max_chunks (each chunk's flag), 48 (the
+ * top-k table), E rows_cap (the cold chunks' values), 4 max_chunks (slot map), 4 (max_chunks + 1) (cold list), 4 max_chunks (the chunks'
+ * list lengths) and 16 k max_chunks (the chunks' candidate lists). */
+PcoB200Error pco_b200_topk_files_async_plan(const void *head, size_t head_len, unsigned char dtype, size_t src_cap, size_t index_cap,
+                                            size_t max_files, size_t max_chunks, size_t rows_cap, size_t k, int largest,
+                                            PcoB200AsyncFilesTopkPlan *plan);
+/* Enqueues the top-k of files[0 : *n_files) on `cuda_stream`, and the outcome into *status; returns without waiting.  src (src_cap bytes),
+ * index (index_cap bytes), files (PcoB200FileRef[max_files]), n_files (one uint64_t), interval, out_values (k numbers of dtype),
+ * out_positions (uint64_t[k]), n_out (one uint64_t), workspace (plan->workspace_bytes, 256-byte aligned) and status are device pointers;
+ * one workspace serves one call in flight.  The numbers ranked are the concatenation pco_b200_decompress_files_async writes for the same
+ * arguments with dst_cap = rows_cap; *n_files = 0 gives *n_out = 0.  The return value covers the host side only, as for
+ * pco_b200_topk_pages_async. */
+PcoB200Error pco_b200_topk_files_async(const PcoB200AsyncFilesTopkPlan *plan, const void *src, const void *index, const PcoB200FileRef *files,
+                                       const uint64_t *n_files, const PcoB200Interval *interval, void *out_values, uint64_t *out_positions,
+                                       uint64_t *n_out, void *workspace, PcoB200AsyncFilesTopkStatus *status, void *cuda_stream);
+/* Host only: the outcome of a call, from its status copied back to host memory.  Returns the kind, sets the last-error message as
+ * pco_b200_aggregate_files_async_result words it ("file 3: chunk 2: ..."), and, when the kind is OK, sets *n_matches (may be NULL) to the
+ * numbers inside the interval. */
+PcoB200Error pco_b200_topk_files_async_result(const PcoB200AsyncFilesTopkStatus *host_status, size_t *n_matches);
+
 /* ---- asynchronous batch compress into wrapped-format chunks (no reference counterpart): pco_b200_compress_wrapped over a batch of
  * arrays, with the array sizes, their count and every buffer in device memory.  A GPU writer of a container that embeds pco (a columnar
  * file whose column chunks a kernel sized, a page store) compresses every column chunk behind the step that produced it, with no copy to

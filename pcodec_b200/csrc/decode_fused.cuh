@@ -315,8 +315,10 @@ __device__ __forceinline__ void fused_undelta(L (&x)[8], FusedSmem& sm, uint32_t
 
 // A decoder warp: batches first + d, first + d + FZ_DECODERS, ... of the chunk (K = consecutive delta order; first = 0 unless WIN and K = 0).
 // FILT: the batches go through filt_store8 (fkey: the interval's keys; fslot0: the chunk's first batch slot); AGG: through agg_store8;
-// TAKE: through take_store8; SEG: through seg_store8; HIST: through hist_store8, into the counters behind sm.
-template <typename L, int K, bool WIN, bool FILT = false, bool AGG = false, bool TAKE = false, bool SEG = false, bool HIST = false>
+// TAKE: through take_store8; SEG: through seg_store8; HIST: through hist_store8, into the counters behind sm; TOPK: through topk_store8,
+// into the candidate buffer behind sm.
+template <typename L, int K, bool WIN, bool FILT = false, bool AGG = false, bool TAKE = false, bool SEG = false, bool HIST = false,
+          bool TOPK = false>
 __device__ __forceinline__ void fused_decoder(FusedSmem& sm, const FileParams& fp, const BitSrc& src, const IndexChunk& task, uint64_t chunk_bit0, L* __restrict__ out,
                                               uint32_t n, uint32_t n_out, uint32_t first, const WinTask& win, int d, int lane,
                                               const FiltStage& filt = {}, const FiltKey& fkey = {}, uint64_t fslot0 = 0) {
@@ -482,7 +484,9 @@ __device__ __forceinline__ void fused_decoder(FusedSmem& sm, const FileParams& f
 #pragma unroll
       for (int e = 0; e < 8; e++) res[e] = from_latent_kind<L>(res[e], kind);
     }
-    if constexpr (HIST) {
+    if constexpr (TOPK) {
+      topk_store8<L>(filt, fkey, &sm + 1, task.out_offset + uint64_t(b) * BATCH_N, min(uint32_t(BATCH_N), n_out - b * BATCH_N), lane, res);
+    } else if constexpr (HIST) {
       hist_store8<L>(filt, fkey, reinterpret_cast<uint32_t*>(&sm + 1), min(uint32_t(BATCH_N), n_out - b * BATCH_N), lane, res);
     } else if constexpr (SEG) {
       seg_store8<L>(filt, fkey, task.out_offset + uint64_t(b) * BATCH_N, fslot0 + b, min(uint32_t(BATCH_N), n_out - b * BATCH_N), lane, res);
@@ -536,7 +540,10 @@ __device__ __forceinline__ void fused_decoder(FusedSmem& sm, const FileParams& f
 // is done at once, as in take mode.
 // HIST (with FILT): histogram mode (hist_store8): each batch counted into the CTA's counters (4 W bytes of dynamic shared memory behind
 // FusedSmem), which the CTA adds to its group's row at the end; out is not written.  An unflagged record is done at once, as in take mode.
-template <typename L, bool WIN = false, bool FILT = false, bool AGG = false, bool TAKE = false, bool SEG = false, bool HIST = false>
+// TOPK (with FILT): top-k mode (topk_store8): the matches kept in the CTA's candidate buffer (topk_smem_bytes behind FusedSmem), whose k
+// best go to the record's slot at the end; out is not written.  An unflagged record is done at once, as in take mode.
+template <typename L, bool WIN = false, bool FILT = false, bool AGG = false, bool TAKE = false, bool SEG = false, bool HIST = false,
+          bool TOPK = false>
 __global__ void __launch_bounds__(FZ_THREADS, PCOB_FZ_MIN_BLOCKS)
 fused_narrow_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, const uint8_t* __restrict__ index_base, uint64_t index_len,
                     uint32_t* __restrict__ statuses, uint8_t* __restrict__ d_cls, L* __restrict__ out, uint64_t out_len,
@@ -551,7 +558,7 @@ fused_narrow_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, const 
   const uint64_t max_blk = (src.n_bits == 0 ? 0 : (src.n_bits - 1) >> 6) >> 1;
   const uint64_t a0_blk = chunk_bit0 >> 7;
   const bool in_file = task.chunk_offset < fp.src_len;
-  if constexpr (TAKE || SEG || HIST) {
+  if constexpr (TAKE || SEG || HIST || TOPK) {
     if (in_file && !filt.counts[filt.fast_page[blockIdx.x]]) {  // uniform: every thread leaves
       if (tid == 0) { statuses[blockIdx.x] = ST_OK; d_cls[blockIdx.x] = CLS_DONE; }
       return;
@@ -693,6 +700,7 @@ fused_narrow_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, const 
     if (tid < int(K)) sm.mo.mvec[0][tid] = sm.hdr.moments[0][tid];
   }
   if constexpr (HIST) hist_clear(filt, reinterpret_cast<uint32_t*>(&sm + 1), tid, FZ_THREADS);
+  if constexpr (TOPK) topk_clear(&sm + 1, tid);
   __syncthreads();
   // the walkers' warp slots rotate with the CTA so that the CTAs of an SM do not all put them on the same schedulers
   const int role = (warp + FZ_WARPS - int((blockIdx.x * FZ_WALKERS) & uint32_t(FZ_WARPS - 1))) & (FZ_WARPS - 1);  // 0 .. FZ_WALKERS - 1: walkers, the rest: decoders
@@ -710,18 +718,19 @@ fused_narrow_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, const 
       fslot0 = task.out_offset / BATCH_N + filt.fast_page[blockIdx.x];
     }
     switch (K) {
-      case 0: fused_decoder<L, 0, WIN, FILT, AGG, TAKE, SEG, HIST>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
-      case 1: fused_decoder<L, 1, WIN, FILT, AGG, TAKE, SEG, HIST>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
-      case 2: fused_decoder<L, 2, WIN, FILT, AGG, TAKE, SEG, HIST>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
-      case 3: fused_decoder<L, 3, WIN, FILT, AGG, TAKE, SEG, HIST>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
-      case 4: fused_decoder<L, 4, WIN, FILT, AGG, TAKE, SEG, HIST>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
-      case 5: fused_decoder<L, 5, WIN, FILT, AGG, TAKE, SEG, HIST>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
-      case 6: fused_decoder<L, 6, WIN, FILT, AGG, TAKE, SEG, HIST>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
-      default: fused_decoder<L, 7, WIN, FILT, AGG, TAKE, SEG, HIST>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
+      case 0: fused_decoder<L, 0, WIN, FILT, AGG, TAKE, SEG, HIST, TOPK>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
+      case 1: fused_decoder<L, 1, WIN, FILT, AGG, TAKE, SEG, HIST, TOPK>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
+      case 2: fused_decoder<L, 2, WIN, FILT, AGG, TAKE, SEG, HIST, TOPK>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
+      case 3: fused_decoder<L, 3, WIN, FILT, AGG, TAKE, SEG, HIST, TOPK>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
+      case 4: fused_decoder<L, 4, WIN, FILT, AGG, TAKE, SEG, HIST, TOPK>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
+      case 5: fused_decoder<L, 5, WIN, FILT, AGG, TAKE, SEG, HIST, TOPK>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
+      case 6: fused_decoder<L, 6, WIN, FILT, AGG, TAKE, SEG, HIST, TOPK>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
+      default: fused_decoder<L, 7, WIN, FILT, AGG, TAKE, SEG, HIST, TOPK>(sm, fp, src, task, chunk_bit0, out, n, n_out, first, win, d, lane, filt, fkey, fslot0); break;
     }
   }
   __syncthreads();
   if constexpr (HIST) hist_flush(filt, reinterpret_cast<const uint32_t*>(&sm + 1), filt.counts[filt.fast_page[blockIdx.x]], tid, FZ_THREADS);
+  if constexpr (TOPK) topk_flush(filt, &sm + 1, filt.fast_page[blockIdx.x], tid, FZ_THREADS);
   if (tid == 0) { statuses[blockIdx.x] = sm.err; d_cls[blockIdx.x] = uint8_t(CLS_DONE | (K == 0 ? CLS_NARROW0 : K == 1 ? CLS_NARROW1 : CLS_NARROWK)); }
 }
 

@@ -1209,6 +1209,173 @@ __device__ __forceinline__ void hist_clear(const FiltStage& f, uint32_t* hc, int
   const uint32_t w = hist_width(f);
   for (uint32_t i = tid; i < w; i += nthreads) hc[i] = 0;
 }
+// ---------------------------------------------------------------------------
+// Top-k mode (the TOPK instantiations, both top-k calls; with FILT): each CTA keeps the best of its numbers inside the interval as
+// (key, tag) entries in a candidate buffer in dynamic shared memory behind the kernel's own (topk_smem_bytes), and writes its at most k
+// best, sorted, to its record's slot when the record is done (topk_flush).  The key is hist_key's (-0.0 equals +0.0), complemented for the
+// k largest, so that the best entry has the least key in both directions; the tag is the number's row in the concatenation, with bit 63
+// set for a -0.0, so that the output keeps the number's own bits.  Entries rank by (key, row): the lower row wins a tie.  The plan
+// (async_topk_kernels.cuh) stages the top-k table and flags the records.  FiltStage: `interval` carries the table (TOPK_* words),
+// `counts` per record (by its map entry) a flag (0: not decoded), `rows` the records' slots of k entries, `offs` the slots' entry counts
+// (uint32 each).
+// ---------------------------------------------------------------------------
+enum : uint32_t { TOPK_LO = 0, TOPK_HI = 1, TOPK_K = 2, TOPK_LARGEST = 3, TOPK_GLOBAL = 4, TOPK_MATCHES = 5, TOPK_WORDS = 6 };
+constexpr uint64_t TOPK_ROW_MASK = (uint64_t(1) << 63) - 1;
+// The head of a TOPK kernel's candidate buffer; its entries (ulonglong2: key, tag) follow.  Appends stop at 2k entries; the buffer has
+// room for the next power of two, which the sort pads.
+struct TopkCta {
+  unsigned long long key, row;  // the threshold: an entry must rank before (key, row); all ones until the buffer held k entries
+  uint32_t n, lock;             // the entries; the lock a warp holds while it appends or compacts
+  unsigned long long matches;   // the CTA's numbers inside the interval
+};
+static_assert(sizeof(TopkCta) == 32, "the entries behind it are 16-byte aligned");
+__host__ __device__ constexpr uint32_t topk_cap(uint32_t k) {
+  uint32_t c = 1;
+  while (c < 2 * k) c <<= 1;
+  return c;
+}
+// 16: the slack that aligns the buffer behind a kernel's own shared memory
+__host__ __device__ constexpr size_t topk_smem_bytes(uint32_t k) { return 16 + sizeof(TopkCta) + size_t(topk_cap(k)) * sizeof(ulonglong2); }
+__device__ __forceinline__ TopkCta* topk_cta(void* behind) {
+  return reinterpret_cast<TopkCta*>((reinterpret_cast<uintptr_t>(behind) + 15) & ~uintptr_t(15));
+}
+__device__ __forceinline__ unsigned long long* topk_global(const FiltStage& f) {
+  return reinterpret_cast<unsigned long long*>(const_cast<uint64_t*>(f.interval) + TOPK_GLOBAL);
+}
+__host__ __device__ __forceinline__ bool topk_before(uint64_t ka, uint64_t ta, uint64_t kb, uint64_t tb) {
+  return ka < kb || (ka == kb && (ta & TOPK_ROW_MASK) < (tb & TOPK_ROW_MASK));
+}
+template <typename L>
+__device__ __forceinline__ uint64_t topk_key(L x, uint32_t kind, bool largest) {
+  const uint64_t h = uint64_t(hist_key<L>(x, kind));
+  return largest ? ~h : h;
+}
+// The number an entry holds: its key back through filt_key, and -0.0 from the tag.
+template <typename L>
+__device__ __forceinline__ L topk_value(ulonglong2 e, uint32_t kind, bool largest) {
+  constexpr L TOP = L(L(1) << (LT<L>::BITS - 1));
+  const L k = L(largest ? ~e.x : e.x);
+  const L x = kind == 1 ? L(k ^ TOP) : kind == 2 ? ((k & TOP) ? L(k ^ TOP) : L(~k)) : k;
+  return (e.y >> 63) ? TOP : x;
+}
+// A bitonic sort of e[0 : n) by rank, padded with all-ones entries to the power of two at or above n.  Threads t .. by nt: a warp (CTA
+// false; all 32 lanes) or the whole CTA (CTA true; every thread, behind a __syncthreads).
+template <bool CTA>
+__device__ __forceinline__ void topk_sort(ulonglong2* e, uint32_t n, int t, int nt) {
+  uint32_t p = 1;
+  while (p < n) p <<= 1;
+  for (uint32_t i = n + t; i < p; i += nt) e[i] = make_ulonglong2(~0ull, ~0ull);
+  if constexpr (CTA) __syncthreads(); else __syncwarp();
+  for (uint32_t size = 2; size <= p; size <<= 1)
+    for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
+      for (uint32_t i = t; i < p / 2; i += nt) {
+        const uint32_t a = 2 * i - (i & (stride - 1)), b = a + stride;
+        const ulonglong2 x = e[a], y = e[b];
+        if (topk_before(y.x, y.y, x.x, x.y) == ((a & size) == 0)) {
+          e[a] = y;
+          e[b] = x;
+        }
+      }
+      if constexpr (CTA) __syncthreads(); else __syncwarp();
+    }
+}
+// The lock holder's compaction of a full buffer: sorted, cut to the k best, the threshold raised to the k-th and offered to the global
+// threshold (the least k-th key of any CTA: no entry with a greater key can be among the k best).  All 32 lanes call it.
+__device__ __forceinline__ void topk_compact(TopkCta* c, uint32_t k, unsigned long long* global, int lane) {
+  volatile TopkCta* vc = c;
+  ulonglong2* e = reinterpret_cast<ulonglong2*>(c + 1);
+  topk_sort<false>(e, vc->n, lane, 32);
+  if (lane == 0) {
+    const ulonglong2 kth = e[k - 1];
+    vc->key = kth.x;
+    vc->row = kth.y & TOPK_ROW_MASK;
+    vc->n = k;
+    atomicMin(global, kth.x);
+  }
+  __syncwarp();
+}
+// Top-k mode's store: the lane's 8 numbers of a batch of `cnt` numbers (its first at row `row`) tested against the interval, counted,
+// and those whose key is at or below both thresholds' keys appended to the CTA's buffer by the warp under the buffer's lock, in ballot
+// order, each re-checked against the CTA's whole (key, row) threshold; a full buffer is compacted first.  A warp none of whose numbers
+// pass takes no lock.  All 32 lanes call it.
+template <typename L>
+__device__ __forceinline__ void topk_store8(const FiltStage& f, const FiltKey& k, void* behind, uint64_t row, uint32_t cnt, int lane,
+                                            const L (&r)[8]) {
+  constexpr L TOP = L(L(1) << (LT<L>::BITS - 1));
+  TopkCta* c = topk_cta(behind);
+  volatile TopkCta* vc = c;
+  ulonglong2* e = reinterpret_cast<ulonglong2*>(c + 1);
+  const uint32_t kk = uint32_t(f.interval[TOPK_K]);
+  const bool largest = f.interval[TOPK_LARGEST] != 0;
+  unsigned long long* global = topk_global(f);
+  const uint64_t bound = min(uint64_t(vc->key), uint64_t(*reinterpret_cast<volatile unsigned long long*>(global)));
+  uint64_t key[8];
+  uint32_t m = 0, hits = 0;
+#pragma unroll
+  for (int i = 0; i < 8; i++) {
+    const bool hit = k.any && uint32_t(lane * 8 + i) < cnt && L(filt_key<L>(r[i], k.kind) - L(k.lo)) <= L(k.span);
+    hits += __popc(__ballot_sync(0xffffffffu, hit));
+    key[i] = topk_key<L>(r[i], k.kind, largest);
+    m |= uint32_t(hit && key[i] <= bound) << i;
+  }
+  if (lane == 0 && hits) atomicAdd(&c->matches, (unsigned long long)hits);
+  if (!__any_sync(0xffffffffu, m)) return;
+  if (lane == 0) {
+    while (atomicCAS(&c->lock, 0u, 1u) != 0u) {
+    }
+    __threadfence_block();
+  }
+  __syncwarp();
+  const uint32_t fill = 2 * kk, lt = (1u << lane) - 1;
+#pragma unroll 1
+  for (int i = 0; i < 8; i++) {
+    const uint64_t tag = (row + uint32_t(lane * 8 + i)) | (k.kind == 2 && r[i] == TOP ? uint64_t(1) << 63 : 0);
+    bool want = (m >> i) & 1u;
+    for (;;) {
+      want = want && topk_before(key[i], tag, vc->key, vc->row);
+      const uint32_t bal = __ballot_sync(0xffffffffu, want);
+      if (!bal) break;
+      const uint32_t n = vc->n;
+      if (n == fill) {
+        topk_compact(c, kk, global, lane);
+        continue;
+      }
+      const uint32_t rank = __popc(bal & lt);
+      if (want && rank < fill - n) {
+        e[n + rank] = make_ulonglong2(key[i], tag);
+        want = false;
+      }
+      __syncwarp();
+      if (lane == 0) vc->n = n + min(uint32_t(__popc(bal)), fill - n);
+      __syncwarp();
+    }
+  }
+  if (lane == 0) {
+    __threadfence_block();
+    atomicExch(&c->lock, 0u);
+  }
+}
+// The CTA's buffer, emptied.  Thread 0; a __syncthreads must follow.
+__device__ __forceinline__ void topk_clear(void* behind, int tid) {
+  if (tid != 0) return;
+  TopkCta* c = topk_cta(behind);
+  *c = TopkCta{~0ull, ~0ull, 0u, 0u, 0ull};
+}
+// The CTA's buffer sorted and its at most k best written to `slot` with their count, and its match count added to the table's.  Every
+// thread calls it, behind a __syncthreads.
+__device__ __forceinline__ void topk_flush(const FiltStage& f, void* behind, uint32_t slot, int tid, int nthreads) {
+  TopkCta* c = topk_cta(behind);
+  ulonglong2* e = reinterpret_cast<ulonglong2*>(c + 1);
+  const uint32_t kk = uint32_t(f.interval[TOPK_K]), n = c->n;
+  topk_sort<true>(e, n, tid, nthreads);
+  const uint32_t keep = min(n, kk);
+  ulonglong2* out = reinterpret_cast<ulonglong2*>(f.rows) + uint64_t(slot) * kk;
+  for (uint32_t i = tid; i < keep; i += nthreads) out[i] = e[i];
+  if (tid == 0) {
+    reinterpret_cast<uint32_t*>(f.offs)[slot] = keep;
+    if (c->matches) atomicAdd(reinterpret_cast<unsigned long long*>(const_cast<uint64_t*>(f.interval) + TOPK_MATCHES), c->matches);
+  }
+}
 template <typename L>
 __device__ __forceinline__ void load8(const L* __restrict__ src, L (&r)[8]) {
   if (sizeof(L) == 8) {
@@ -1488,7 +1655,10 @@ __global__ void __launch_bounds__(SW_THREADS) symwalk_kernel(FileParams fp, cons
 // SEG (with FILT): segment mode (seg_store8: the matches reduced per batch and segment into the SegRec records; out is not written).
 // HIST (with FILT): histogram mode (hist_store8: each batch counted into the CTA's counters behind DecodeSmem, added to the chunk's group
 // row at the end; out is not written).
-template <typename L, int NV, bool WIN = false, bool FILT = false, bool AGG = false, bool TAKE = false, bool SEG = false, bool HIST = false>
+// TOPK (with FILT): top-k mode (topk_store8: the matches kept in the CTA's candidate buffer behind DecodeSmem, whose k best go to the
+// chunk's slot at the end; out is not written).
+template <typename L, int NV, bool WIN = false, bool FILT = false, bool AGG = false, bool TAKE = false, bool SEG = false, bool HIST = false,
+          bool TOPK = false>
 __global__ void __launch_bounds__(DEC_THREADS, NV == 1 ? PCOB_DEC_NV1_BLOCKS : 2)
 decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __restrict__ statuses, const uint8_t* __restrict__ index_base, uint64_t index_len,
               L* __restrict__ out, uint64_t out_len, const Binoms* __restrict__ binoms, const uint8_t* __restrict__ d_syms,
@@ -1527,6 +1697,7 @@ decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __
   for (int i = tid; i < 32 * MAX_ORDER; i += DEC_THREADS) sm.binom_lane8[i / MAX_ORDER][i % MAX_ORDER] = binoms->lane8[i / MAX_ORDER][i % MAX_ORDER];
   if (tid < MAX_ORDER) sm.binom_full[tid] = binoms->full[tid];
   if constexpr (HIST) hist_clear(filt, reinterpret_cast<uint32_t*>(&sm + 1), tid, DEC_THREADS);
+  if constexpr (TOPK) topk_clear(&sm + 1, tid);
   __syncthreads();
   if (sm.hdr.status != ST_OK) {
     if (tid == 0) statuses[blockIdx.x] = sm.hdr.status;
@@ -1871,7 +2042,9 @@ decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __
             res[e] = from_latent_kind<L>(L(L(pq << k) + lowest), 2);
           }
         }
-        if constexpr (HIST) {
+        if constexpr (TOPK) {
+          topk_store8<L>(filt, fkey, &sm + 1, task.out_offset + uint64_t(b) * BATCH_N, out_cnt, lane, res);
+        } else if constexpr (HIST) {
           hist_store8<L>(filt, fkey, reinterpret_cast<uint32_t*>(&sm + 1), out_cnt, lane, res);
         } else if constexpr (SEG) {
           seg_store8<L>(filt, fkey, task.out_offset + uint64_t(b) * BATCH_N, fslot0 + b, out_cnt, lane, res);
@@ -1913,6 +2086,7 @@ decode_kernel(FileParams fp, const IndexChunk* __restrict__ chunks, uint32_t* __
   if (end_err) atomicMax(&sm.err, end_err);
   __syncthreads();
   if constexpr (HIST) hist_flush(filt, reinterpret_cast<const uint32_t*>(&sm + 1), filt.counts[filt.fast_page[blockIdx.x]], tid, DEC_THREADS);
+  if constexpr (TOPK) topk_flush(filt, &sm + 1, filt.fast_page[blockIdx.x], tid, DEC_THREADS);
   if (tid == 0) statuses[blockIdx.x] = sm.err;
 }
 

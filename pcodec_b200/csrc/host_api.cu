@@ -12,6 +12,7 @@
 #include "async_filter_files_kernels.cuh"
 #include "async_filter_kernels.cuh"
 #include "async_histogram_kernels.cuh"
+#include "async_topk_kernels.cuh"
 #include "async_files_kernels.cuh"
 #include "async_index_kernels.cuh"
 #include "async_kernels.cuh"
@@ -48,8 +49,8 @@ namespace pcob200 {
 // The context follows the thread's current device: a cudaSetDevice between calls drops the scratch of the previous device.
 struct Context {
   int device = -1;
-  bool attrs_set[7] = {false, false, false, false, false, false, false};  // set_decode_attrs<WIN, FILT, AGG, TAKE, SEG, HIST> has run (index
-                                                                          // WIN + 2 FILT + AGG + 2 TAKE + 3 SEG + 4 HIST)
+  bool attrs_set[8] = {false, false, false, false, false, false, false, false};  // set_decode_attrs<WIN, FILT, AGG, TAKE, SEG, HIST, TOPK> has
+                                                                                 // run (index WIN + 2 FILT + AGG + 2 TAKE + 3 SEG + 4 HIST + 5 TOPK)
   bool initialized = false;
   bool device_ok = false;
   std::string device_err;
@@ -173,17 +174,24 @@ static cudaError_t set_hist_decode_attrs(MaxShared max_shared, size_t smem) {
   const cudaError_t e = max_shared(decode_kernel<L, 1, false, true, false, false, false, true>, smem);
   return e != cudaSuccess ? e : max_shared(decode_kernel<L, 2, false, true, false, false, false, true>, smem);
 }
+// The decode_kernel<L, 1 / 2> TOPK instantiations' shared-memory attributes, likewise.
+template <typename L, typename MaxShared>
+static cudaError_t set_topk_decode_attrs(MaxShared max_shared, size_t smem) {
+  const cudaError_t e = max_shared(decode_kernel<L, 1, false, true, false, false, false, false, true>, smem);
+  return e != cudaSuccess ? e : max_shared(decode_kernel<L, 2, false, true, false, false, false, false, true>, smem);
+}
 
 // Shared-memory attributes of the decode kernels (the window-mode instantiations when WIN, the filter-mode ones when FILT, the
 // aggregate-mode ones when AGG too, the take-mode ones when TAKE too, the segment-mode ones when SEG too, the histogram-mode ones when
-// HIST too, whose kernels may take the counters of HG_MAX_BUCKETS buckets behind their own shared memory), set once per context before
-// their first launch.
-template <bool WIN, bool FILT = false, bool AGG = false, bool TAKE = false, bool SEG = false, bool HIST = false>
+// HIST too, whose kernels may take the counters of HG_MAX_BUCKETS buckets behind their own shared memory, the top-k-mode ones when TOPK
+// too, whose kernels may take the candidate buffer of TOPK_MAX_K behind theirs), set once per context before their first launch.
+template <bool WIN, bool FILT = false, bool AGG = false, bool TAKE = false, bool SEG = false, bool HIST = false, bool TOPK = false>
 static PcoB200Error set_decode_attrs(Context& c) {
-  static_assert(!(WIN && FILT) && (FILT || !AGG) && (FILT || !TAKE) && (FILT || !SEG) && (FILT || !HIST) &&
-                    int(AGG) + int(TAKE) + int(SEG) + int(HIST) <= 1,
-                "no instantiation is both window and filter mode; aggregate, take, segment and histogram mode are filter modes, and exclusive");
-  constexpr int at = WIN + 2 * FILT + AGG + 2 * TAKE + 3 * SEG + 4 * HIST;
+  static_assert(!(WIN && FILT) && (FILT || !AGG) && (FILT || !TAKE) && (FILT || !SEG) && (FILT || !HIST) && (FILT || !TOPK) &&
+                    int(AGG) + int(TAKE) + int(SEG) + int(HIST) + int(TOPK) <= 1,
+                "no instantiation is both window and filter mode; aggregate, take, segment, histogram and top-k mode are filter modes, and "
+                "exclusive");
+  constexpr int at = WIN + 2 * FILT + AGG + 2 * TAKE + 3 * SEG + 4 * HIST + 5 * TOPK;
   if (c.attrs_set[at]) return PCO_B200_OK;
   auto max_shared = [](auto* kernel, size_t smem) {
     const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
@@ -191,15 +199,22 @@ static PcoB200Error set_decode_attrs(Context& c) {
   };
   PCOB_CUDA_TRY(max_shared(symwalk_kernel<WIN>, sizeof(SymWalkSmem)));
   constexpr size_t hist = HIST ? hist_smem_bytes(HG_MAX_BUCKETS) : 0;
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint64_t, WIN, FILT, AGG, TAKE, SEG, HIST>, sizeof(FusedSmem) + hist));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint32_t, WIN, FILT, AGG, TAKE, SEG, HIST>, sizeof(FusedSmem) + hist));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint16_t, WIN, FILT, AGG, TAKE, SEG, HIST>, sizeof(FusedSmem) + hist));
-  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint8_t, WIN, FILT, AGG, TAKE, SEG, HIST>, sizeof(FusedSmem) + hist));
+  constexpr size_t topk = TOPK ? topk_smem_bytes(TOPK_MAX_K) : 0;
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint64_t, WIN, FILT, AGG, TAKE, SEG, HIST, TOPK>, sizeof(FusedSmem) + hist + topk));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint32_t, WIN, FILT, AGG, TAKE, SEG, HIST, TOPK>, sizeof(FusedSmem) + hist + topk));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint16_t, WIN, FILT, AGG, TAKE, SEG, HIST, TOPK>, sizeof(FusedSmem) + hist + topk));
+  PCOB_CUDA_TRY(max_shared(fused_narrow_kernel<uint8_t, WIN, FILT, AGG, TAKE, SEG, HIST, TOPK>, sizeof(FusedSmem) + hist + topk));
   if constexpr (HIST) {  // the other instantiations launch decode_kernel within the default 48 KB
     PCOB_CUDA_TRY(set_hist_decode_attrs<uint64_t>(max_shared, sizeof(DecodeSmem) + hist));
     PCOB_CUDA_TRY(set_hist_decode_attrs<uint32_t>(max_shared, sizeof(DecodeSmem) + hist));
     PCOB_CUDA_TRY(set_hist_decode_attrs<uint16_t>(max_shared, sizeof(DecodeSmem) + hist));
     PCOB_CUDA_TRY(set_hist_decode_attrs<uint8_t>(max_shared, sizeof(DecodeSmem) + hist));
+  }
+  if constexpr (TOPK) {
+    PCOB_CUDA_TRY(set_topk_decode_attrs<uint64_t>(max_shared, sizeof(DecodeSmem) + topk));
+    PCOB_CUDA_TRY(set_topk_decode_attrs<uint32_t>(max_shared, sizeof(DecodeSmem) + topk));
+    PCOB_CUDA_TRY(set_topk_decode_attrs<uint16_t>(max_shared, sizeof(DecodeSmem) + topk));
+    PCOB_CUDA_TRY(set_topk_decode_attrs<uint8_t>(max_shared, sizeof(DecodeSmem) + topk));
   }
   c.attrs_set[at] = true;  // only once every attribute is set: a failed call leaves them to the next
   return PCO_B200_OK;
@@ -815,19 +830,19 @@ static PcoB200Error async_result_kind(uint32_t kind) { return kind <= PCO_B200_U
 
 // The set-up of an asynchronous decompress plan: the device, the decode kernels' attributes (the window-mode instantiations when WIN, the
 // filter-mode ones when FILT, the aggregate-mode ones when AGG too, the take-mode ones when TAKE too, the segment-mode ones when SEG too,
-// the histogram-mode ones when HIST too), and loaded: the decode stage's kernels for dtype, the call's catch-all kernel (cold(tag) for a
-// latent type tag) and the call's `kernels`.
-template <bool WIN, bool FILT = false, bool AGG = false, bool TAKE = false, bool SEG = false, bool HIST = false, typename Cold>
+// the histogram-mode ones when HIST too, the top-k-mode ones when TOPK too), and loaded: the decode stage's kernels for dtype, the call's
+// catch-all kernel (cold(tag) for a latent type tag) and the call's `kernels`.
+template <bool WIN, bool FILT = false, bool AGG = false, bool TAKE = false, bool SEG = false, bool HIST = false, bool TOPK = false, typename Cold>
 static PcoB200Error async_decode_setup(unsigned char dtype, Cold cold, std::initializer_list<const void*> kernels) {
   Context& c = ctx();
   if (PcoB200Error e = ensure_device(c)) return e;
-  if (PcoB200Error e = set_decode_attrs<WIN, FILT, AGG, TAKE, SEG, HIST>(c)) return e;
+  if (PcoB200Error e = set_decode_attrs<WIN, FILT, AGG, TAKE, SEG, HIST, TOPK>(c)) return e;
   if (PcoB200Error e = load_kernels(kernels)) return e;
   return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
     using L = decltype(tag);
-    return load_kernels({(const void*)fused_narrow_kernel<L, WIN, FILT, AGG, TAKE, SEG, HIST>, (const void*)symwalk_kernel<WIN>,
-                         (const void*)decode_kernel<L, 1, WIN, FILT, AGG, TAKE, SEG, HIST>, (const void*)decode_kernel<L, 2, WIN, FILT, AGG, TAKE, SEG, HIST>,
-                         cold(tag)});
+    return load_kernels({(const void*)fused_narrow_kernel<L, WIN, FILT, AGG, TAKE, SEG, HIST, TOPK>, (const void*)symwalk_kernel<WIN>,
+                         (const void*)decode_kernel<L, 1, WIN, FILT, AGG, TAKE, SEG, HIST, TOPK>,
+                         (const void*)decode_kernel<L, 2, WIN, FILT, AGG, TAKE, SEG, HIST, TOPK>, cold(tag)});
   });
 }
 
@@ -891,16 +906,17 @@ struct DecodeStage {
   void* dst;
   uint64_t dst_cap;
   const WinTask* wins;
-  FiltStage filt;  // FILT: dst is the value staging (decode_kernels.cuh, filt_store8); AGG: dst is null (agg_store8); TAKE, SEG, HIST: likewise
+  FiltStage filt;  // FILT: dst is the value staging (decode_kernels.cuh, filt_store8); AGG: dst is null (agg_store8); TAKE, SEG, HIST, TOPK: likewise
   size_t hist_smem = 0;  // HIST: the counters' bytes behind each decode kernel's shared memory (hist_smem_bytes)
+  size_t topk_smem = 0;  // TOPK: the candidate buffer's bytes behind each decode kernel's shared memory (topk_smem_bytes)
 };
-template <bool WIN, bool FILT = false, bool AGG = false, bool TAKE = false, bool SEG = false, bool HIST = false>
+template <bool WIN, bool FILT = false, bool AGG = false, bool TAKE = false, bool SEG = false, bool HIST = false, bool TOPK = false>
 static void enqueue_decode_stage(const AsyncLaunch& ln, const DecodeStage& d) {
   const cudaStream_t stream = ln.stream;
   ln.begin("fused_narrow_kernel");
   dispatch_latent(d.fp.dtype, [&](auto tag) {
     using L = decltype(tag);
-    fused_narrow_kernel<L, WIN, FILT, AGG, TAKE, SEG, HIST><<<d.slots, FZ_THREADS, sizeof(FusedSmem) + d.hist_smem, stream>>>(d.fp, d.table, d.index, d.index_len, d.st, d.cls,
+    fused_narrow_kernel<L, WIN, FILT, AGG, TAKE, SEG, HIST, TOPK><<<d.slots, FZ_THREADS, sizeof(FusedSmem) + d.hist_smem + d.topk_smem, stream>>>(d.fp, d.table, d.index, d.index_len, d.st, d.cls,
                                                                                          static_cast<L*>(d.dst), d.dst_cap, d.wins, d.filt);
     return 0;
   });
@@ -911,9 +927,9 @@ static void enqueue_decode_stage(const AsyncLaunch& ln, const DecodeStage& d) {
   ln.begin("decode_kernel");
   dispatch_latent(d.fp.dtype, [&](auto tag) {
     using L = decltype(tag);
-    decode_kernel<L, 1, WIN, FILT, AGG, TAKE, SEG, HIST><<<d.slots, DEC_THREADS, sizeof(DecodeSmem) + d.hist_smem, stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst),
+    decode_kernel<L, 1, WIN, FILT, AGG, TAKE, SEG, HIST, TOPK><<<d.slots, DEC_THREADS, sizeof(DecodeSmem) + d.hist_smem + d.topk_smem, stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst),
                                                                                         d.dst_cap, d.binoms, d.syms, d.offs, d.cls, d.wins, d.filt);
-    decode_kernel<L, 2, WIN, FILT, AGG, TAKE, SEG, HIST><<<d.slots, DEC_THREADS, sizeof(DecodeSmem) + d.hist_smem, stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst),
+    decode_kernel<L, 2, WIN, FILT, AGG, TAKE, SEG, HIST, TOPK><<<d.slots, DEC_THREADS, sizeof(DecodeSmem) + d.hist_smem + d.topk_smem, stream>>>(d.fp, d.table, d.st, d.index, d.index_len, static_cast<L*>(d.dst),
                                                                                         d.dst_cap, d.binoms, d.syms, d.offs, d.cls, d.wins, d.filt);
     return 0;
   });
@@ -2828,10 +2844,11 @@ PcoB200Error pco_b200_decompress_files_async_plan(const void* head, size_t head_
 // instantiations, likewise (pco_b200_take_files_async).  `between`, when given, enqueues its launches behind the front end
 // (merge_index_kernel) and before the decode stage.  With `seg` (and neither `agg` nor `take`), the segment-mode instantiations, likewise
 // (pco_b200_segment_aggregate_files_async).  With hist_smem (and none of the three), the histogram-mode instantiations with that many
-// bytes of counters, likewise (pco_b200_histogram_files_async).
+// bytes of counters, likewise (pco_b200_histogram_files_async).  With topk_smem (and none of the four), the top-k-mode instantiations with
+// that many bytes of candidate buffer, likewise (pco_b200_topk_files_async).
 static void enqueue_files(const AsyncLaunch& ln, const AfArgs& g, const AfLayout& lay, uint8_t* ws, void* dst, const FiltStage* filt,
                           uint32_t* cold_list, uint64_t* file_ns, PcoB200AsyncFilesStatus* status, bool agg = false, bool take = false,
-                          const std::function<void()>& between = {}, bool seg = false, size_t hist_smem = 0) {
+                          const std::function<void()>& between = {}, bool seg = false, size_t hist_smem = 0, size_t topk_smem = 0) {
   const cudaStream_t stream = ln.stream;
   const uint32_t mf = g.max_files, mc = g.max_chunks;
   AsyncCheck* chk = reinterpret_cast<AsyncCheck*>(ws);
@@ -2866,9 +2883,11 @@ static void enqueue_files(const AsyncLaunch& ln, const AfArgs& g, const AfLayout
   ln.end();
   if (between) between();
   const DecodeStage d{g.fp, table, d_idx, g.index_cap, mc, d_st, ws + lay.cls, ws + lay.syms, reinterpret_cast<uint32_t*>(ws + lay.offs),
-                      &chk->binoms, agg || take || seg || hist_smem ? nullptr : dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{}, hist_smem};
+                      &chk->binoms, agg || take || seg || hist_smem || topk_smem ? nullptr : dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{},
+                      hist_smem, topk_smem};
   if (filt) {
-    if (hist_smem) enqueue_decode_stage<false, true, false, false, false, true>(ln, d);
+    if (topk_smem) enqueue_decode_stage<false, true, false, false, false, false, true>(ln, d);
+    else if (hist_smem) enqueue_decode_stage<false, true, false, false, false, true>(ln, d);
     else if (seg) enqueue_decode_stage<false, true, false, false, true>(ln, d);
     else if (agg) enqueue_decode_stage<false, true, true>(ln, d);
     else if (take) enqueue_decode_stage<false, true, false, true>(ln, d);
@@ -3133,10 +3152,11 @@ static void enqueue_pages_front(const AsyncLaunch& ln, const ApArgs& g, const Ap
 // instantiations, likewise (pco_b200_take_pages_async).  `between`, when given, enqueues its launches behind the front end
 // (ap_rewalk_kernel) and before the decode stage.  With `seg` (and neither `agg` nor `take`), the segment-mode instantiations, likewise
 // (pco_b200_segment_aggregate_pages_async).  With hist_smem (and none of the three), the histogram-mode instantiations with that many
-// bytes of counters, likewise (pco_b200_histogram_pages_async).
+// bytes of counters, likewise (pco_b200_histogram_pages_async).  With topk_smem (and none of the four), the top-k-mode instantiations with
+// that many bytes of candidate buffer, likewise (pco_b200_topk_pages_async).
 static void enqueue_pages(const AsyncLaunch& ln, const ApArgs& g, const ApLayout& lay, uint8_t* ws, void* dst, const FiltStage* filt,
                           PcoB200AsyncPagesStatus* status, bool agg = false, bool take = false, const std::function<void()>& between = {},
-                          bool seg = false, size_t hist_smem = 0) {
+                          bool seg = false, size_t hist_smem = 0, size_t topk_smem = 0) {
   const cudaStream_t stream = ln.stream;
   AsyncCheck* chk = reinterpret_cast<AsyncCheck*>(ws);
   ApState* state = reinterpret_cast<ApState*>(ws + lay.state);
@@ -3154,8 +3174,10 @@ static void enqueue_pages(const AsyncLaunch& ln, const ApArgs& g, const ApLayout
   enqueue_pages_front(ln, g, lay, ws);
   if (between) between();
   const DecodeStage d{fp, table, d_idx, lay.index_len, mp, d_st, ws + lay.cls, ws + lay.syms, reinterpret_cast<uint32_t*>(ws + lay.offs),
-                      &chk->binoms, agg || take || seg || hist_smem ? nullptr : dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{}, hist_smem};
-  if (hist_smem) enqueue_decode_stage<false, true, false, false, false, true>(ln, d);
+                      &chk->binoms, agg || take || seg || hist_smem || topk_smem ? nullptr : dst, g.dst_cap, nullptr, filt ? *filt : FiltStage{},
+                      hist_smem, topk_smem};
+  if (topk_smem) enqueue_decode_stage<false, true, false, false, false, false, true>(ln, d);
+  else if (hist_smem) enqueue_decode_stage<false, true, false, false, false, true>(ln, d);
   else if (seg) enqueue_decode_stage<false, true, false, false, true>(ln, d);
   else if (agg) enqueue_decode_stage<false, true, true>(ln, d);
   else if (take) enqueue_decode_stage<false, true, false, true>(ln, d);
@@ -4235,6 +4257,247 @@ PcoB200Error pco_b200_histogram_files_async_result(const PcoB200AsyncFilesHistog
   if (kind != PCO_B200_OK && s->device_status == PCO_B200_HIST_EDGES_ORDER) return hg_result(kind, s->edge);
   const PcoB200AsyncFilesFilterStatus f{s->kind, s->device_status, s->file, s->chunk, s->n_written, s->n_files, s->n_written, s->n_written};
   return pco_b200_filter_files_async_result(&f, n_rows);  // the files filter's words: rows_cap in the role of dst_cap
+}
+
+// ---- asynchronous top-k of wrapped pages and of indexed files (pco_b200_topk_pages_async, pco_b200_topk_files_async; kernels in
+// async_topk_kernels.cuh).  The top-k table, then the decompress call's launches (enqueue_pages / enqueue_files with the decode stage's
+// top-k-mode instantiations and rows_cap as dst_cap; for files behind ff_map_kernel) with the histogram's gate between the front end and
+// the decode stage: the front kernel, the record flags (and, for pages, the cold list kept to the flagged pages); then the cold
+// selection, the merge rounds and the finish.  A memset clears the slots' entry counts (and, for files, the flags).
+
+static PcoB200Error check_topk(size_t k, int largest) {
+  if (k == 0 || uint64_t(k) > TOPK_MAX_K) return fail(PCO_B200_INVALID_ARGUMENT, "k must be 1 .. 1024");
+  if (largest != 0 && largest != 1) return fail(PCO_B200_INVALID_ARGUMENT, "largest must be 0 (the k smallest) or 1 (the k largest)");
+  return PCO_B200_OK;
+}
+
+// The merge rounds over `slots` slot lists, enqueued behind the cold selection: slot 0 ends with the k best.
+static void enqueue_topk_merge(const AsyncLaunch& ln, ulonglong2* lists, uint32_t* counts, uint64_t slots, uint32_t k) {
+  for (uint64_t stride = 1; stride < slots; stride <<= 1) {
+    ln.begin("topk_merge_kernel");
+    topk_merge_kernel<<<uint32_t((slots + 2 * stride - 1) / (2 * stride)), TOPK_THREADS, 2 * size_t(k) * sizeof(ulonglong2), ln.stream>>>(
+        lists, counts, slots, k, stride);
+    ln.end();
+  }
+}
+
+static bool topk_plan_ok(const PcoB200AsyncTopkPlan* p) {
+  return nt_valid(p->dtype) && p->max_pages >= 1 && p->max_pages <= 0x7fffffffull && p->rows_cap <= (uint64_t(1) << 56) &&
+         p->frame_cap <= (uint64_t(1) << 56) && p->k >= 1 && p->k <= TOPK_MAX_K && p->largest <= 1 &&
+         p->workspace_bytes == topk_layout(p->max_pages, p->rows_cap, p->frame_cap, p->k, nt_bits(p->dtype) / 8).topk_total;
+}
+
+PcoB200Error pco_b200_topk_pages_async_plan(unsigned char dtype, size_t metas_cap, size_t pages_cap, size_t max_pages, size_t rows_cap,
+                                            size_t frame_cap, size_t k, int largest, PcoB200AsyncTopkPlan* plan) {
+  if (!nt_valid(dtype)) return fail(PCO_B200_INVALID_TYPE, "unknown number type byte: " + std::to_string(dtype));
+  if (!plan) return fail(PCO_B200_INVALID_ARGUMENT, "null plan");
+  if (max_pages == 0 || uint64_t(max_pages) > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_pages must be 1 .. 2^31 - 1");
+  if (uint64_t(rows_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "rows_cap above 2^56 numbers");
+  if (uint64_t(frame_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "frame_cap above 2^56 bytes");
+  if (PcoB200Error e = check_topk(k, largest)) return e;
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->largest = uint32_t(largest);
+  plan->metas_cap = metas_cap;
+  plan->pages_cap = pages_cap;
+  plan->max_pages = max_pages;
+  plan->rows_cap = rows_cap;
+  plan->frame_cap = frame_cap;
+  plan->k = k;
+  plan->workspace_bytes = topk_layout(max_pages, rows_cap, frame_cap, k, nt_bits(dtype) / 8).topk_total;
+  if (PcoB200Error e = async_decode_setup<false, true, false, false, false, false, true>(
+          dtype, [](auto tag) { return (const void*)ap_cold_kernel<decltype(tag)>; },
+          {(const void*)ap_pages_kernel, (const void*)ap_scan_kernel, (const void*)ap_place_kernel, (const void*)frame_pages_kernel,
+           (const void*)walk_kernel<SMALL_MAX_SIZE_LOG>, (const void*)ap_route_kernel, (const void*)ap_rewalk_kernel, (const void*)ap_finish_kernel,
+           (const void*)topk_table_kernel, (const void*)hg_front_pages_kernel, (const void*)hg_mark_pages_kernel, (const void*)tk_cold_list_kernel,
+           (const void*)topk_merge_kernel}))
+    return e;
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
+    using L = decltype(tag);
+    return load_kernels({(const void*)topk_cold_pages_kernel<L>, (const void*)topk_finish_pages_kernel<L>});
+  });
+}
+
+PcoB200Error pco_b200_topk_pages_async(const PcoB200AsyncTopkPlan* plan, const void* metas, const void* pages, const PcoB200PageRef* refs,
+                                       const uint64_t* n_pages, const PcoB200Interval* interval, void* out_values, uint64_t* out_positions,
+                                       uint64_t* n_out, void* workspace, PcoB200AsyncTopkStatus* status, void* cuda_stream) {
+  if (!plan || !metas || !pages || !refs || !n_pages || !interval || !out_values || !out_positions || !n_out || !workspace || !status)
+    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (!topk_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_topk_pages_async_plan");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+  const cudaStream_t stream = ln.stream;
+
+  const uint32_t mp = uint32_t(plan->max_pages), k = uint32_t(plan->k);
+  const TopkLayout lay = topk_layout(mp, plan->rows_cap, plan->frame_cap, k, nt_bits(plan->dtype) / 8);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  const ApArgs g{static_cast<const uint8_t*>(metas), static_cast<const uint8_t*>(pages), refs, n_pages, plan->metas_cap, plan->pages_cap, plan->rows_cap,
+                 plan->frame_cap, plan->dtype, mp};
+  // top-k mode: the top-k table travels in FiltStage's interval pointer, the record flags in counts, the slot lists in rows, their
+  // lengths in offs
+  auto* table = reinterpret_cast<uint64_t*>(ws + lay.topk_table);
+  auto* lists = reinterpret_cast<ulonglong2*>(ws + lay.lists);
+  auto* counts = reinterpret_cast<uint32_t*>(ws + lay.counts);
+  const FiltStage filt{table, reinterpret_cast<const uint32_t*>(ws + lay.fast_page), reinterpret_cast<uint32_t*>(ws + lay.flags),
+                       reinterpret_cast<uint64_t*>(lists), reinterpret_cast<uint8_t*>(counts)};
+  auto* state = reinterpret_cast<ApState*>(ws + lay.state);
+  auto* recs = reinterpret_cast<const IndexChunk*>(ws + lay.index);
+  auto* cold_list = reinterpret_cast<uint32_t*>(ws + lay.cold_list);
+  auto* pstatus = reinterpret_cast<PcoB200AsyncPagesStatus*>(ws + lay.pstatus);
+  auto* hs = reinterpret_cast<HgState*>(ws + lay.hstate);
+
+  PCOB_CUDA_TRY(cudaMemsetAsync(counts, 0, uint64_t(mp) * sizeof(uint32_t), stream));
+  ln.begin("topk_table_kernel");
+  topk_table_kernel<<<1, 32, 0, stream>>>(reinterpret_cast<const uint64_t*>(interval), k, plan->largest, table);
+  ln.end();
+  enqueue_pages(ln, g, lay, ws, ws + lay.stage, &filt, pstatus, false, false, [&] {
+    ln.begin("hg_front_pages_kernel");
+    hg_front_pages_kernel<<<1, 32, 0, stream>>>(state, hs);
+    ln.end();
+    ln.begin("hg_mark_pages_kernel");
+    hg_mark_pages_kernel<<<uint32_t(std::min(ctas_of<HG_THREADS>(mp), HG_MAX_CTAS)), HG_THREADS, 0, stream>>>(hs, mp, filt.counts);
+    ln.end();
+    ln.begin("tk_cold_list_kernel");
+    tk_cold_list_kernel<<<1, TK_SCAN_THREADS, 0, stream>>>(state, cold_list, filt.counts);
+    ln.end();
+  }, false, 0, topk_smem_bytes(k));
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    ln.begin("topk_cold_pages_kernel");
+    topk_cold_pages_kernel<L><<<mp, TOPK_THREADS, topk_smem_bytes(k), stream>>>(state, recs, cold_list, filt, plan->dtype,
+                                                                                 reinterpret_cast<const L*>(ws + lay.stage));
+    ln.end();
+    return 0;
+  });
+  enqueue_topk_merge(ln, lists, counts, mp, k);
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    ln.begin("topk_finish_pages_kernel");
+    topk_finish_pages_kernel<L><<<1, TOPK_THREADS, 0, stream>>>(pstatus, table, plan->dtype, lists, counts, static_cast<L*>(out_values), out_positions,
+                                                                n_out, status);
+    ln.end();
+    return 0;
+  });
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
+}
+
+PcoB200Error pco_b200_topk_pages_async_result(const PcoB200AsyncTopkStatus* s, size_t* n_matches) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200AsyncFilterStatus f{s->kind, s->device_status, s->page, s->n_written, s->n_pages, s->frames_needed, s->n_matches, s->n_matches};
+  return pco_b200_filter_pages_async_result(&f, n_matches);  // the pages filter's words: rows_cap in the role of dst_cap
+}
+
+static bool topkf_plan_ok(const PcoB200AsyncFilesTopkPlan* p) {
+  return nt_valid(p->dtype) && p->max_files >= 1 && p->max_files <= 0x7fffffffull && p->max_chunks >= 1 && p->max_chunks <= 0xffffffffull &&
+         p->rows_cap <= (uint64_t(1) << 56) && p->k >= 1 && p->k <= TOPK_MAX_K && p->largest <= 1 &&
+         p->workspace_bytes == topkf_layout(p->max_files, p->max_chunks, p->rows_cap, p->k, nt_bits(p->dtype) / 8).topkf_total;
+}
+
+PcoB200Error pco_b200_topk_files_async_plan(const void* head, size_t head_len, unsigned char dtype, size_t src_cap, size_t index_cap,
+                                            size_t max_files, size_t max_chunks, size_t rows_cap, size_t k, int largest,
+                                            PcoB200AsyncFilesTopkPlan* plan) {
+  StandaloneHeader hdr;
+  if (PcoB200Error e = check_async_head(head, head_len, dtype, plan, &hdr)) return e;
+  if (max_files == 0 || uint64_t(max_files) > 0x7fffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_files must be 1 .. 2^31 - 1");
+  if (max_chunks == 0 || uint64_t(max_chunks) > 0xffffffffull) return fail(PCO_B200_INVALID_ARGUMENT, "max_chunks must be 1 .. 2^32 - 1");
+  if (uint64_t(rows_cap) > (uint64_t(1) << 56)) return fail(PCO_B200_INVALID_ARGUMENT, "rows_cap above 2^56 numbers");
+  if (PcoB200Error e = check_topk(k, largest)) return e;
+  std::memset(plan, 0, sizeof(*plan));
+  plan->dtype = dtype;
+  plan->uniform_type = hdr.uniform_type;
+  plan->format_major = hdr.format_major;
+  plan->largest = uint32_t(largest);
+  plan->src_cap = src_cap;
+  plan->index_cap = index_cap;
+  plan->max_files = max_files;
+  plan->max_chunks = max_chunks;
+  plan->rows_cap = rows_cap;
+  plan->k = k;
+  plan->workspace_bytes = topkf_layout(max_files, max_chunks, rows_cap, k, nt_bits(dtype) / 8).topkf_total;
+  if (PcoB200Error e = async_decode_setup<false, true, false, false, false, false, true>(
+          dtype, [](auto tag) { return (const void*)cold_chunks_kernel<decltype(tag)>; },
+          {(const void*)af_files_kernel, (const void*)check_index_kernel, (const void*)af_scan_kernel, (const void*)af_place_kernel,
+           (const void*)af_table_kernel, (const void*)merge_index_kernel, (const void*)af_finish_kernel, (const void*)ff_map_kernel,
+           (const void*)ff_cold_list_kernel, (const void*)topk_table_kernel, (const void*)hg_front_files_kernel, (const void*)hg_mark_files_kernel,
+           (const void*)topk_merge_kernel}))
+    return e;
+  return dispatch_latent(dtype, [&](auto tag) -> PcoB200Error {
+    using L = decltype(tag);
+    return load_kernels({(const void*)topk_cold_files_kernel<L>, (const void*)topk_finish_files_kernel<L>});
+  });
+}
+
+PcoB200Error pco_b200_topk_files_async(const PcoB200AsyncFilesTopkPlan* plan, const void* src, const void* index, const PcoB200FileRef* files,
+                                       const uint64_t* n_files, const PcoB200Interval* interval, void* out_values, uint64_t* out_positions,
+                                       uint64_t* n_out, void* workspace, PcoB200AsyncFilesTopkStatus* status, void* cuda_stream) {
+  if (!plan || !src || !index || !files || !n_files || !interval || !out_values || !out_positions || !n_out || !workspace || !status)
+    return fail(PCO_B200_INVALID_ARGUMENT, "null buffer");
+  if (!topkf_plan_ok(plan)) return fail(PCO_B200_INVALID_ARGUMENT, "the plan was not made by pco_b200_topk_files_async_plan");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(PCO_B200_INVALID_ARGUMENT, "the workspace is not 256-byte aligned");
+  AsyncLaunch ln;
+  if (PcoB200Error e = open_async_launch(cuda_stream, &ln)) return e;
+  const cudaStream_t stream = ln.stream;
+
+  const uint32_t mf = uint32_t(plan->max_files), mc = uint32_t(plan->max_chunks), k = uint32_t(plan->k);
+  const TopkfLayout lay = topkf_layout(mf, mc, plan->rows_cap, k, nt_bits(plan->dtype) / 8);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  const AfArgs g{FileParams{src, plan->src_cap, plan->dtype, plan->uniform_type, plan->format_major}, static_cast<const uint8_t*>(index),
+                 plan->index_cap, plan->rows_cap, files, n_files, mf, mc};
+  // top-k mode: as the pages call, with the slot map in place of fast_page
+  auto* table = reinterpret_cast<uint64_t*>(ws + lay.topk_table);
+  auto* lists = reinterpret_cast<ulonglong2*>(ws + lay.lists);
+  auto* counts = reinterpret_cast<uint32_t*>(ws + lay.counts);
+  const FiltStage filt{table, reinterpret_cast<const uint32_t*>(ws + lay.slot_map), reinterpret_cast<uint32_t*>(ws + lay.flags),
+                       reinterpret_cast<uint64_t*>(lists), reinterpret_cast<uint8_t*>(counts)};
+  auto* fstatus = reinterpret_cast<PcoB200AsyncFilesStatus*>(ws + lay.fstatus);
+  auto* hs = reinterpret_cast<HgState*>(ws + lay.hstate);
+  auto* cold_list = reinterpret_cast<uint32_t*>(ws + lay.cold_list);
+  auto* recs = reinterpret_cast<const IndexChunk*>(ws + lay.table);
+
+  PCOB_CUDA_TRY(cudaMemsetAsync(counts, 0, uint64_t(mc) * sizeof(uint32_t), stream));
+  PCOB_CUDA_TRY(cudaMemsetAsync(filt.counts, 0, uint64_t(mc) * sizeof(uint32_t), stream));
+  ln.begin("topk_table_kernel");
+  topk_table_kernel<<<1, 32, 0, stream>>>(reinterpret_cast<const uint64_t*>(interval), k, plan->largest, table);
+  ln.end();
+  ln.begin("ff_map_kernel");
+  ff_map_kernel<<<uint32_t(ctas_of<FF_THREADS>(mc)), FF_THREADS, 0, stream>>>(mc, reinterpret_cast<uint32_t*>(ws + lay.slot_map), cold_list);
+  ln.end();
+  enqueue_files(ln, g, lay, ws, ws + lay.stage, &filt, cold_list, nullptr, fstatus, false, false, [&] {
+    ln.begin("hg_front_files_kernel");
+    hg_front_files_kernel<<<1, 32, 0, stream>>>(reinterpret_cast<const AsyncCheck*>(ws), hs);
+    ln.end();
+    ln.begin("hg_mark_files_kernel");
+    hg_mark_files_kernel<<<uint32_t(std::min(uint64_t(mf), HG_MAX_CTAS)), HG_THREADS, 0, stream>>>(
+        hs, n_files, mf, reinterpret_cast<const FileMerge*>(ws + lay.merges), filt.counts);
+    ln.end();
+  }, false, 0, topk_smem_bytes(k));
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    ln.begin("topk_cold_files_kernel");
+    topk_cold_files_kernel<L><<<std::min(mc, uint32_t(FF_COLD_CTAS)), TOPK_THREADS, topk_smem_bytes(k), stream>>>(
+        cold_list, recs, reinterpret_cast<const uint32_t*>(ws + lay.st), filt, plan->dtype, reinterpret_cast<const L*>(ws + lay.stage));
+    ln.end();
+    return 0;
+  });
+  enqueue_topk_merge(ln, lists, counts, mc, k);
+  dispatch_latent(plan->dtype, [&](auto tag) {
+    using L = decltype(tag);
+    ln.begin("topk_finish_files_kernel");
+    topk_finish_files_kernel<L><<<1, TOPK_THREADS, 0, stream>>>(fstatus, table, plan->dtype, lists, counts, static_cast<L*>(out_values), out_positions,
+                                                                n_out, status);
+    ln.end();
+    return 0;
+  });
+  PCOB_CUDA_TRY(cudaGetLastError());
+  return PCO_B200_OK;  // spans stay pending until pco_b200_profile_last reads them
+}
+
+PcoB200Error pco_b200_topk_files_async_result(const PcoB200AsyncFilesTopkStatus* s, size_t* n_matches) {
+  if (!s) return fail(PCO_B200_INVALID_ARGUMENT, "null status");
+  const PcoB200AsyncFilesFilterStatus f{s->kind, s->device_status, s->file, s->chunk, s->n_written, s->n_files, s->n_matches, s->n_matches};
+  return pco_b200_filter_files_async_result(&f, n_matches);  // the files filter's words: rows_cap in the role of dst_cap
 }
 
 // ---- asynchronous compress (pco_b200_compress_async; gate kernels in async_compress.cuh).  The plan fixes the layout and the config;

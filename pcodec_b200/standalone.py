@@ -978,6 +978,78 @@ class AsyncFilesHistogram(_lib._AsyncCall):
         return int(n.value)
 
 
+class _CAsyncFilesTopkPlan(C.Structure):  # PcoB200AsyncFilesTopkPlan (include/pco_b200.h)
+    _fields_ = [("dtype", C.c_uint32), ("uniform_type", C.c_uint32), ("format_major", C.c_uint32), ("largest", C.c_uint32),
+                ("src_cap", C.c_uint64), ("index_cap", C.c_uint64), ("max_files", C.c_uint64), ("max_chunks", C.c_uint64),
+                ("rows_cap", C.c_uint64), ("k", C.c_uint64), ("workspace_bytes", C.c_uint64)]
+
+
+class _CAsyncFilesTopkStatus(C.Structure):  # PcoB200AsyncFilesTopkStatus (include/pco_b200.h)
+    _fields_ = [("kind", C.c_uint32), ("device_status", C.c_uint32), ("file", C.c_uint64), ("chunk", C.c_uint64), ("n_written", C.c_uint64),
+                ("n_files", C.c_uint64), ("n_matches", C.c_uint64)]
+
+
+def _lib_async_topk_files():
+    return _lib.bind("_async_topk_files_ready",
+                     pco_b200_topk_files_async_plan=[C.c_void_p, C.c_size_t, C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                                     C.c_size_t, C.c_size_t, C.c_int, C.c_void_p],
+                     pco_b200_topk_files_async=[C.c_void_p] * 12,
+                     pco_b200_topk_files_async_result=[C.c_void_p, C.POINTER(C.c_size_t)])
+
+
+class AsyncFilesTopK(_lib._AsyncCall):
+    """Decodes a batch of indexed standalone files on the current CUDA stream and returns the k smallest (largest=False) or k largest
+    (largest=True) numbers inside a closed interval, with their positions in the files' concatenation (pco_b200_topk_files_async), as
+    wrapped.AsyncPagesTopK does for pages.  Refs, their count and the interval are read from device tensors, so one captured call serves
+    new files and a new interval on each replay.
+
+    The plan and capacities are AsyncFilesDecompressor's, with rows_cap (the most numbers of a call's files) in place of dst_cap, and k
+    (1 .. 1024) and the direction fixed by the plan.  The call owns a device workspace (about rows_cap * itemsize + 16 * k * max_chunks
+    bytes beyond the decompressor's) and a status; it serves one call in flight."""
+
+    _Plan, _Status = _CAsyncFilesTopkPlan, _CAsyncFilesTopkStatus
+
+    def __init__(self, head, dtype, src_cap, index_cap, max_files, max_chunks, rows_cap, k, largest=False, device=None):
+        self.dtype = np.dtype(dtype)
+        h = self._head(head)
+        self._make_plan(device, lambda plan: _lib_async_topk_files().pco_b200_topk_files_async_plan(
+            h.ctypes.data_as(C.c_void_p), C.c_size_t(h.size), C.c_ubyte(_lib.dtype_byte(self.dtype)), C.c_size_t(src_cap), C.c_size_t(index_cap),
+            C.c_size_t(max_files), C.c_size_t(max_chunks), C.c_size_t(rows_cap), C.c_size_t(k), C.c_int(int(largest)), plan))
+        self._alloc()
+
+    def __call__(self, src, index, files, n_files, interval, out_values, out_positions, n_out):
+        """Enqueues the top-k of files[: n_files[0]] on torch.cuda.current_stream().  `src`, `index`, `files` and `n_files` are as
+        AsyncFilesDecompressor takes them; `interval`, `out_values`, `out_positions` and `n_out` are as wrapped.AsyncPagesTopK takes them.
+        Returns nothing and does not wait; result() reports the outcome."""
+        import torch
+
+        from .wrapped import _check_topk_inputs
+
+        p = self._plan
+        self._check_tensors(src=src, index=index, files=files, n_files=n_files, interval=interval, out_values=out_values,
+                            out_positions=out_positions, n_out=n_out)
+        if src.numel() * src.element_size() < p.src_cap or index.numel() * index.element_size() < p.index_cap:
+            raise ValueError(f"src holds fewer than src_cap = {p.src_cap} bytes, or index fewer than index_cap = {p.index_cap}")
+        if files.dtype != torch.int64 or files.dim() != 2 or files.shape[1] != 4 or files.shape[0] < p.max_files:
+            raise ValueError(f"files must be an int64 tensor of shape ({p.max_files}, 4)")
+        if n_files.dtype != torch.int64 or n_files.numel() != 1:
+            raise ValueError("n_files must be a 1-element int64 tensor")
+        _check_topk_inputs(interval, out_values, out_positions, n_out, p.k, self.dtype)
+        rc = _lib_async_topk_files().pco_b200_topk_files_async(
+            C.byref(p), C.c_void_p(src.data_ptr()), C.c_void_p(index.data_ptr()), C.c_void_p(files.data_ptr()), C.c_void_p(n_files.data_ptr()),
+            C.c_void_p(interval.data_ptr()), C.c_void_p(out_values.data_ptr()), C.c_void_p(out_positions.data_ptr()), C.c_void_p(n_out.data_ptr()),
+            C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()), self._stream())
+        _lib.check(rc)
+
+    def result(self):
+        """Copies the status of the last call back (waiting for it on the current stream) and returns the numbers inside the interval, or
+        raises PcoError with the kind pco_b200_decompress_files gives ("file 3: chunk 2: ...")."""
+        s = self.status_record()
+        n = C.c_size_t()
+        _lib.check(_lib_async_topk_files().pco_b200_topk_files_async_result(C.byref(s), C.byref(n)))
+        return int(n.value)
+
+
 class _CAsyncFilesTakePlan(C.Structure):  # PcoB200AsyncFilesTakePlan (include/pco_b200.h)
     _fields_ = [("dtype", C.c_uint32), ("uniform_type", C.c_uint32), ("format_major", C.c_uint32), ("reserved", C.c_uint32),
                 ("src_cap", C.c_uint64), ("index_cap", C.c_uint64), ("max_files", C.c_uint64), ("max_chunks", C.c_uint64),

@@ -655,6 +655,94 @@ class AsyncPagesHistogram(_lib._AsyncCall):
         return int(n.value)
 
 
+class _CAsyncTopkPlan(C.Structure):  # PcoB200AsyncTopkPlan (include/pco_b200.h)
+    _fields_ = [("dtype", C.c_uint32), ("largest", C.c_uint32), ("metas_cap", C.c_uint64), ("pages_cap", C.c_uint64), ("max_pages", C.c_uint64),
+                ("rows_cap", C.c_uint64), ("frame_cap", C.c_uint64), ("k", C.c_uint64), ("workspace_bytes", C.c_uint64)]
+
+
+class _CAsyncTopkStatus(C.Structure):  # PcoB200AsyncTopkStatus (include/pco_b200.h)
+    _fields_ = [("kind", C.c_uint32), ("device_status", C.c_uint32), ("page", C.c_uint64), ("n_written", C.c_uint64), ("n_pages", C.c_uint64),
+                ("frames_needed", C.c_uint64), ("n_matches", C.c_uint64)]
+
+
+def _lib_async_topk():
+    return _lib.bind("_async_topk_ready",
+                     pco_b200_topk_pages_async_plan=[C.c_ubyte, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int,
+                                                     C.c_void_p],
+                     pco_b200_topk_pages_async=[C.c_void_p] * 12,
+                     pco_b200_topk_pages_async_result=[C.c_void_p, C.POINTER(C.c_size_t)])
+
+
+def _check_topk_inputs(interval, out_values, out_positions, n_out, k, dtype):
+    import torch
+
+    if interval.dtype != torch.int64 or interval.numel() != 2:
+        raise ValueError("interval must be a 2-element int64 tensor (pack_interval's bit patterns)")
+    if out_values.dtype != _torch_dtypes()[np.dtype(dtype)] or out_values.numel() < k or not out_values.is_contiguous():
+        raise ValueError(f"out_values must be a contiguous tensor of at least k = {k} numbers of {np.dtype(dtype)}")
+    if out_positions.dtype != torch.int64 or out_positions.numel() < k or not out_positions.is_contiguous():
+        raise ValueError(f"out_positions must be a contiguous int64 tensor of at least k = {k} elements")
+    if n_out.dtype != torch.int64 or n_out.numel() != 1:
+        raise ValueError("n_out must be a 1-element int64 tensor")
+
+
+class AsyncPagesTopK(_lib._AsyncCall):
+    """Decodes a batch of wrapped-format pages on the current CUDA stream and returns the k smallest (largest=False) or k largest
+    (largest=True) numbers inside a closed interval, with their positions in the pages' concatenation (pco_b200_topk_pages_async): each
+    decode CTA keeps its best matches in shared memory, so the decoded pages never reach HBM.  Numbers compare as AsyncPagesFilter compares
+    them; ties go to the lower position, so the output is a unique function of the numbers.  Refs, their count and the interval are read
+    from device tensors, so one captured call serves new pages and a new interval on each replay.
+
+    The capacities are AsyncPagesDecompressor's, with rows_cap (the most numbers of a call's pages) in place of dst_cap; frame_cap defaults
+    to metas_cap + pages_cap + 20 * max_pages as there.  k (1 .. 1024) and the direction are fixed by the plan.  The call owns a device
+    workspace (about rows_cap * itemsize + 16 * k * max_pages bytes beyond the decompressor's) and a status; it serves one call in
+    flight."""
+
+    _Plan, _Status = _CAsyncTopkPlan, _CAsyncTopkStatus
+
+    def __init__(self, dtype, metas_cap, pages_cap, max_pages, rows_cap, k, largest=False, frame_cap=None, device=None):
+        self.dtype = np.dtype(dtype)
+        if frame_cap is None:
+            frame_cap = metas_cap + pages_cap + 20 * max_pages
+        self._make_plan(device, lambda plan: _lib_async_topk().pco_b200_topk_pages_async_plan(
+            C.c_ubyte(_lib.dtype_byte(self.dtype)), C.c_size_t(metas_cap), C.c_size_t(pages_cap), C.c_size_t(max_pages), C.c_size_t(rows_cap),
+            C.c_size_t(frame_cap), C.c_size_t(k), C.c_int(int(largest)), plan))
+        self._alloc()
+
+    def __call__(self, metas, pages, refs, n_pages, interval, out_values, out_positions, n_out):
+        """Enqueues the top-k of the pages refs[: n_pages[0]] names on torch.cuda.current_stream().  `metas`, `pages`, `refs` and
+        `n_pages` are as AsyncPagesDecompressor takes them and `interval` as AsyncPagesFilter takes it (pack_interval(lo, hi, dtype) on the
+        device; the full range of the dtype for every number).  The best numbers, best first, go to out_values (a CUDA tensor of at least
+        k numbers of the dtype, each with its own bits), their positions to out_positions (an int64 CUDA tensor of at least k elements) and
+        their count, min(k, matches), to n_out (a 1-element int64 CUDA tensor; 0 on a failure).  Returns nothing and does not wait;
+        result() reports the outcome."""
+        import torch
+
+        p = self._plan
+        self._check_tensors(metas=metas, pages=pages, refs=refs, n_pages=n_pages, interval=interval, out_values=out_values,
+                            out_positions=out_positions, n_out=n_out)
+        if metas.numel() * metas.element_size() < p.metas_cap or pages.numel() * pages.element_size() < p.pages_cap:
+            raise ValueError(f"metas holds fewer than metas_cap = {p.metas_cap} bytes, or pages fewer than pages_cap = {p.pages_cap}")
+        if refs.dtype != torch.int64 or refs.dim() != 2 or refs.shape[1] != 5 or refs.shape[0] < p.max_pages:
+            raise ValueError(f"refs must be an int64 tensor of shape ({p.max_pages}, 5)")
+        if n_pages.dtype != torch.int64 or n_pages.numel() != 1:
+            raise ValueError("n_pages must be a 1-element int64 tensor")
+        _check_topk_inputs(interval, out_values, out_positions, n_out, p.k, self.dtype)
+        rc = _lib_async_topk().pco_b200_topk_pages_async(
+            C.byref(p), C.c_void_p(metas.data_ptr()), C.c_void_p(pages.data_ptr()), C.c_void_p(refs.data_ptr()), C.c_void_p(n_pages.data_ptr()),
+            C.c_void_p(interval.data_ptr()), C.c_void_p(out_values.data_ptr()), C.c_void_p(out_positions.data_ptr()), C.c_void_p(n_out.data_ptr()),
+            C.c_void_p(self.workspace.data_ptr()), C.c_void_p(self.status.data_ptr()), self._stream())
+        _lib.check(rc)
+
+    def result(self):
+        """Copies the status of the last call back (waiting for it on the current stream) and returns the numbers inside the interval, or
+        raises PcoError with the kind decompress_pages gives ("page 17: ...")."""
+        s = self.status_record()
+        n = C.c_size_t()
+        _lib.check(_lib_async_topk().pco_b200_topk_pages_async_result(C.byref(s), C.byref(n)))
+        return int(n.value)
+
+
 class _CAsyncTakePlan(C.Structure):  # PcoB200AsyncTakePlan (include/pco_b200.h)
     _fields_ = [("dtype", C.c_uint32), ("reserved", C.c_uint32), ("metas_cap", C.c_uint64), ("pages_cap", C.c_uint64), ("max_pages", C.c_uint64),
                 ("rows_cap", C.c_uint64), ("frame_cap", C.c_uint64), ("max_positions", C.c_uint64), ("workspace_bytes", C.c_uint64)]
